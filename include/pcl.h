@@ -304,7 +304,9 @@ int pcl_render(pcl_handle* h, const uint8_t* d_backdrop, int64_t backdrop_bstrid
                const uint8_t* d_z_order, uint8_t* d_board, void* stream);
 
 /* Byte-per-cell view of drape `drape_index`'s current curtain (Drape.curtain,
- * things.py:213-217): u8 [B, rows, pitch]. */
+ * things.py:213-217): u8 [B, rows, pitch], the drape's plane of a one-character
+ * pcl_layers call.  PCL_ERR_UNSUPPORTED where pcl_layers is; PCL_ERR_INVALID when
+ * the bound state holds no curtain for that drape. */
 int pcl_export_curtain(pcl_handle* h, int drape_index, uint8_t* d_out, void* stream);
 
 /* Layers of BaseUnoccludedObservationRenderer (rendering.py:187-301, selected by
@@ -313,7 +315,7 @@ int pcl_export_curtain(pcl_handle* h, int drape_index, uint8_t* d_out, void* str
  * occluded or not — the backdrop where it holds that character, a drape's whole
  * curtain, a visible sprite's cell.  `chars` is a HOST array of n_chars <= 32 ASCII
  * codes.  PCL_ERR_UNSUPPORTED for programs whose drape curtain is implicit
- * (warehouse 'X', aperture). */
+ * (warehouse 'X', aperture, hello). */
 int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_out,
                void* stream);
 

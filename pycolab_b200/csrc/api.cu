@@ -337,11 +337,15 @@ int launched(pcl_handle* h, cudaError_t e, const char* what) {
   return PCL_OK;
 }
 
+// The per-env outputs every step writes and every hand-off record carries.
+bool outputs_set(const pcl_outputs& out) {
+  return out.d_reward && out.d_has_reward && out.d_discount && out.d_done;
+}
+
 int check_ready(const pcl_handle* h, const pcl_outputs* out) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  if (!out->d_board || !out->d_reward || !out->d_has_reward || !out->d_discount || !out->d_done)
-    return PCL_ERR_INVALID;
+  if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
   return PCL_OK;
 }
 
@@ -633,37 +637,53 @@ int pcl_render(pcl_handle* h, const uint8_t* d_backdrop, int64_t backdrop_bstrid
   return launched(h, pcl::launch_render(p, (cudaStream_t)stream), "launch_render");
 }
 
+namespace {
+// Where drape d's curtain lives in the bound state: a window of a Scrolly pattern at
+// the drape's corner, or bit rows of the board.  Fills d's fields of `p`.
+int resolve_curtain(const pcl_handle* h, int d, pcl::LayersParams* p) {
+  const pcl_spec& sp = h->spec;
+  if (sp.program == PCL_PROG_SCROLLY_MAZE || (sp.program == PCL_PROG_FIXTURE && sp.drape_kind[d])) {
+    p->scrolly[d] = 1;
+    p->bits[d] = h->st.d_pattern[d]; p->bits_bstride[d] = h->st.pattern_bstride[d];
+    p->row_words[d] = sp.pattern_words;
+    const bool coins = sp.program == PCL_PROG_SCROLLY_MAZE && d == 1;
+    p->stale_slot[d] = coins;
+    p->per_level[d] = !coins && h->st.d_level != nullptr;   // read-only patterns: per level
+  } else if (sp.program == PCL_PROG_MARAUDERS || sp.program == PCL_PROG_BETTER_SCROLLY ||
+             sp.program == PCL_PROG_FIXTURE || sp.program == PCL_PROG_ORDEAL ||
+             sp.program == PCL_PROG_SHOCKWAVE) {
+    p->bits[d] = h->st.d_bits[d]; p->bits_bstride[d] = h->st.bits_bstride[d];
+    p->row_words[d] = sp.bits_words;
+  } else {
+    return PCL_ERR_UNSUPPORTED;    // curtain held implicitly (warehouse 'X', aperture, hello)
+  }
+  return p->bits[d] ? PCL_OK : PCL_ERR_INVALID;
+}
+
+// A layers launch over `n_chars` planes; the caller fills the planes and resolves the
+// drapes they read.
+pcl::LayersParams layers_params(const pcl_handle* h, int n_chars, uint8_t* d_out) {
+  const pcl_spec& sp = h->spec;
+  pcl::LayersParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = h->batch; p.H = sp.rows; p.W = sp.cols; p.pitch = sp.pitch;
+  p.S = sp.n_sprites; p.D = sp.n_drapes; p.n_chars = n_chars;
+  p.backdrop = h->st.d_backdrop; p.backdrop_bstride = h->st.backdrop_bstride;
+  p.level = h->st.d_level; p.sprites = h->st.d_sprites; p.drapes = h->st.d_drapes;
+  p.out = d_out;
+  return p;
+}
+}  // namespace
+
 int pcl_export_curtain(pcl_handle* h, int drape_index, uint8_t* d_out, void* stream) {
   if (!h || !d_out || drape_index < 0 || drape_index >= h->spec.n_drapes) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  pcl::ExportParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
-  p.PWW = h->spec.pattern_words; p.BW = h->spec.bits_words;
-  p.drape = drape_index; p.D = h->spec.n_drapes; p.drapes = h->st.d_drapes;
-  p.out = d_out; p.stale_slot = -1;
-  if (h->spec.program == PCL_PROG_SCROLLY_MAZE) {
-    p.scrolly = 1;
-    p.bits = h->st.d_pattern[drape_index];
-    p.bits_bstride = h->st.pattern_bstride[drape_index];
-    if (drape_index == 1) p.stale_slot = 0;
-    else p.level = h->st.d_level;            // the wall pattern is read-only: per level
-  } else if (h->spec.program == PCL_PROG_MARAUDERS ||
-             h->spec.program == PCL_PROG_BETTER_SCROLLY || h->spec.program == PCL_PROG_ORDEAL ||
-             h->spec.program == PCL_PROG_SHOCKWAVE ||
-             (h->spec.program == PCL_PROG_FIXTURE && !h->spec.drape_kind[drape_index])) {
-    p.scrolly = 0;
-    p.bits = h->st.d_bits[drape_index];
-    p.bits_bstride = h->st.bits_bstride[drape_index];
-  } else if (h->spec.program == PCL_PROG_FIXTURE) {
-    p.scrolly = 1;
-    p.bits = h->st.d_pattern[drape_index];
-    p.bits_bstride = h->st.pattern_bstride[drape_index];
-    p.level = h->st.d_level;                 // fixture patterns are read-only: per level
-  } else {
-    return PCL_ERR_UNSUPPORTED;
-  }
-  return launched(h, pcl::launch_export_curtain(p, (cudaStream_t)stream), "launch_export_curtain");
+  pcl::LayersParams p = layers_params(h, 1, d_out);
+  p.chars[0] = h->spec.drape_char[drape_index];
+  p.sprite_of[0] = -1; p.drape_of[0] = (int8_t)drape_index;
+  const int r = resolve_curtain(h, drape_index, &p);
+  if (r != PCL_OK) return r;
+  return launched(h, pcl::launch_layers(p, (cudaStream_t)stream), "launch_layers");
 }
 
 int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_out,
@@ -673,32 +693,10 @@ int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_
     return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   const pcl_spec& sp = h->spec;
-  pcl::LayersParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.H = sp.rows; p.W = sp.cols; p.pitch = sp.pitch;
-  p.S = sp.n_sprites; p.D = sp.n_drapes; p.n_chars = n_chars;
-  p.backdrop = h->st.d_backdrop; p.backdrop_bstride = h->st.backdrop_bstride;
-  p.level = h->st.d_level; p.sprites = h->st.d_sprites; p.drapes = h->st.d_drapes;
-  p.out = d_out;
+  pcl::LayersParams p = layers_params(h, n_chars, d_out);
   for (int d = 0; d < sp.n_drapes; ++d) {
-    // Where each program keeps a drape's curtain (as pcl_export_curtain).
-    if (sp.program == PCL_PROG_SCROLLY_MAZE ||
-        (sp.program == PCL_PROG_FIXTURE && sp.drape_kind[d])) {
-      p.scrolly[d] = 1;
-      p.bits[d] = h->st.d_pattern[d]; p.bits_bstride[d] = h->st.pattern_bstride[d];
-      p.row_words[d] = sp.pattern_words;
-      const bool coins = sp.program == PCL_PROG_SCROLLY_MAZE && d == 1;
-      p.stale_slot[d] = coins;
-      p.per_level[d] = !coins && h->st.d_level != nullptr;   // read-only patterns: per level
-    } else if (sp.program == PCL_PROG_MARAUDERS || sp.program == PCL_PROG_BETTER_SCROLLY ||
-               sp.program == PCL_PROG_FIXTURE || sp.program == PCL_PROG_ORDEAL ||
-               sp.program == PCL_PROG_SHOCKWAVE) {
-      p.bits[d] = h->st.d_bits[d]; p.bits_bstride[d] = h->st.bits_bstride[d];
-      p.row_words[d] = sp.bits_words;
-    } else {
-      return PCL_ERR_UNSUPPORTED;       // curtain held implicitly (warehouse 'X', aperture)
-    }
-    if (!p.bits[d]) return PCL_ERR_INVALID;
+    const int r = resolve_curtain(h, d, &p);
+    if (r != PCL_OK) return r;
   }
   for (int k = 0; k < n_chars; ++k) {
     p.chars[k] = chars[k];
@@ -710,16 +708,43 @@ int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_
 }
 
 namespace {
-// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts.
+// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts, for every
+// cropper entry point.
 int crop_spec_ok(const pcl_handle* h, const pcl_crop_spec* crop) {
   if (crop->rows <= 0 || crop->cols <= 0) return PCL_ERR_INVALID;
+  // sprite_index names the tracked sprite only when no priority list is given (a
+  // cropper may track a drape in a game without sprites).
   if (crop->track[0] == 0 && crop->sprite_index >= h->spec.n_sprites) return PCL_ERR_INVALID;
   if (crop->sprite_index >= 0 &&
       (2 * crop->margin_rows >= crop->rows || 2 * crop->margin_cols >= crop->cols))
     return PCL_ERR_INVALID;                                  // cropping.py:374-380
   if (crop->pad_char < 0 && (crop->rows > h->spec.rows || crop->cols > h->spec.cols))
     return PCL_ERR_INVALID;                                  // cropping.py:384-391
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
+    if (crop->sprite_index < 0) return PCL_ERR_INVALID;      // a FixedCropper tracks nothing
+    if (crop->track[i] > h->spec.n_sprites || crop->track[i] < -h->spec.n_drapes)
+      return PCL_ERR_INVALID;                                // no such sprite / drape
+  }
   return PCL_OK;
+}
+
+bool tracks_drape(const pcl_crop_spec* crop) {
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i)
+    if (crop->track[i] < 0) return true;
+  return false;
+}
+
+pcl::CropParams crop_params(const pcl_handle* h, const pcl_crop_spec* crop,
+                            const uint8_t* d_board, uint8_t* d_crop, int32_t* d_crop_state) {
+  pcl::CropParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
+  p.S = h->spec.n_sprites; p.crop = *crop;
+  p.sprites = h->st.d_sprites; p.plot = h->st.d_plot; p.board = d_board; p.out = d_crop;
+  p.state = d_crop_state;
+  // floor(2^32 / cols) + 1: __umulhi(i, recip) == i / cols for every i < 65536 (cols >= 1).
+  p.cols_recip = crop->cols > 1 ? (uint32_t)(0x100000000ull / (uint32_t)crop->cols) + 1u : 0u;
+  return p;
 }
 }  // namespace
 
@@ -736,16 +761,8 @@ int pcl_attach_cropper(pcl_handle* h, const pcl_crop_spec* crop, uint8_t* d_crop
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
   if ((int64_t)crop->rows * crop->cols >= 65536) return PCL_ERR_UNSUPPORTED;
-  for (int i = 0; i < PCL_MAX_TRACK; ++i) {
-    if (crop->track[i] < 0) return PCL_ERR_UNSUPPORTED;      // drape medians need scratch memory
-    if (crop->track[i] > h->spec.n_sprites) return PCL_ERR_INVALID;
-  }
-  pcl::CropParams& c = h->base.cropper;
-  memset(&c, 0, sizeof(c));
-  c.B = h->batch; c.H = h->spec.rows; c.W = h->spec.cols; c.pitch = h->spec.pitch;
-  c.S = h->spec.n_sprites; c.crop = *crop;
-  c.sprites = h->st.d_sprites; c.plot = h->st.d_plot; c.out = d_crop; c.state = d_crop_state;
-  c.cols_recip = crop->cols > 1 ? (uint32_t)(0x100000000ull / (uint32_t)crop->cols) + 1u : 0u;
+  if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape medians need scratch memory
+  h->base.cropper = crop_params(h, crop, nullptr, d_crop, d_crop_state);
   h->base.has_cropper = 1;
   return PCL_OK;
 }
@@ -761,32 +778,14 @@ int pcl_crop_tracking(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d
   Range nvtx_range("pcl_crop (ScrollingCropper.crop)");
   if (!h || !crop || !d_board || !d_crop) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  if (crop->rows <= 0 || crop->cols <= 0) return PCL_ERR_INVALID;
-  // sprite_index names the tracked sprite only when no priority list is given (a
-  // cropper may track a drape in a game without sprites).
-  if (crop->track[0] == 0 && crop->sprite_index >= h->spec.n_sprites) return PCL_ERR_INVALID;
-  if (crop->sprite_index >= 0 &&
-      (2 * crop->margin_rows >= crop->rows || 2 * crop->margin_cols >= crop->cols))
-    return PCL_ERR_INVALID;                                  // cropping.py:374-380
-  if (crop->pad_char < 0 && (crop->rows > h->spec.rows || crop->cols > h->spec.cols))
-    return PCL_ERR_INVALID;                                  // cropping.py:384-391
-  pcl::CropParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
-  p.S = h->spec.n_sprites; p.crop = *crop;
-  p.sprites = h->st.d_sprites; p.plot = h->st.d_plot; p.board = d_board; p.out = d_crop;
-  p.state = d_crop_state;
-  for (int i = 0; i < PCL_MAX_TRACK; ++i) {
-    const int code = crop->track[i];
-    if (code == 0) break;
-    if (crop->sprite_index < 0) return PCL_ERR_INVALID;      // a FixedCropper tracks nothing
-    if (code > 0) {
-      if (code - 1 >= h->spec.n_sprites) return PCL_ERR_INVALID;
-    } else {
-      if (-code - 1 >= h->spec.n_drapes || !d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
-      if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
-      p.curtains[i] = d_curtains[i];
-    }
+  const int ok = crop_spec_ok(h, crop);
+  if (ok != PCL_OK) return ok;
+  pcl::CropParams p = crop_params(h, crop, d_board, d_crop, d_crop_state);
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
+    if (crop->track[i] > 0) continue;
+    if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
+    if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
+    p.curtains[i] = d_curtains[i];
   }
   return launched(h, pcl::launch_crop(p, (cudaStream_t)stream), "launch_crop");
 }
@@ -797,29 +796,17 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   Range nvtx_range("pcl_crop_handoff");
   if (!h || !crop || !d_board || !out || !x) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  if (!out->d_reward || !out->d_has_reward || !out->d_discount || !out->d_done)
-    return PCL_ERR_INVALID;
-  if (crop->rows <= 0 || crop->cols <= 0 || crop->sprite_index >= h->spec.n_sprites)
-    return PCL_ERR_INVALID;
-  for (int i = 0; i < PCL_MAX_TRACK; ++i)
-    if (crop->track[i] < 0) return PCL_ERR_UNSUPPORTED;      // drape tracking: pcl_crop_tracking
-  if (crop->sprite_index >= 0 &&
-      (2 * crop->margin_rows >= crop->rows || 2 * crop->margin_cols >= crop->cols))
-    return PCL_ERR_INVALID;
-  if (crop->pad_char < 0 && (crop->rows > h->spec.rows || crop->cols > h->spec.cols))
-    return PCL_ERR_INVALID;
+  if (!outputs_set(*out)) return PCL_ERR_INVALID;
+  const int ok = crop_spec_ok(h, crop);
+  if (ok != PCL_OK) return ok;
+  if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape tracking: pcl_crop_tracking
   const int view = crop->rows * crop->cols;
   if (x->n_peers < 1 || x->n_peers > PCL_MAX_PEERS || x->rank < 0 || x->rank >= x->n_peers)
     return PCL_ERR_INVALID;
   if ((x->record_bytes & 15) || x->record_bytes < PCL_HANDOFF_RECORD_BYTES(view) ||
       x->record_bytes > 256) return PCL_ERR_INVALID;
   if (!x->d_local || x->first_row < 0 || x->first_row + h->batch > x->rows) return PCL_ERR_INVALID;
-  pcl::CropParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
-  p.S = h->spec.n_sprites; p.crop = *crop;
-  p.sprites = h->st.d_sprites; p.plot = h->st.d_plot; p.board = d_board; p.out = nullptr;
-  p.state = d_crop_state;
+  const pcl::CropParams p = crop_params(h, crop, d_board, nullptr, d_crop_state);
   pcl::HandoffParams q;
   memset(&q, 0, sizeof(q));
   q.n_peers = x->n_peers; q.rank = x->rank; q.record_bytes = x->record_bytes;
@@ -842,8 +829,7 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
 int pcl_pack_handoff(pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
                      const pcl_outputs* out, uint8_t* d_packed, void* stream) {
   if (!h || !d_view || !out || !d_packed || view_bytes <= 0) return PCL_ERR_INVALID;
-  if (!out->d_reward || !out->d_has_reward || !out->d_discount || !out->d_done)
-    return PCL_ERR_INVALID;
+  if (!outputs_set(*out)) return PCL_ERR_INVALID;
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;
@@ -858,8 +844,7 @@ int pcl_pack_handoff_peers(pcl_handle* h, const uint8_t* d_view, int32_t view_by
   if (!h || !d_view || !out || !d_peer_bases || view_bytes <= 0 || first_row < 0)
     return PCL_ERR_INVALID;
   if (n_peers < 1 || n_peers > PCL_MAX_PEERS) return PCL_ERR_INVALID;
-  if (!out->d_reward || !out->d_has_reward || !out->d_discount || !out->d_done)
-    return PCL_ERR_INVALID;
+  if (!outputs_set(*out)) return PCL_ERR_INVALID;
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;

@@ -122,8 +122,8 @@ __device__ __forceinline__ void crop_corner(const CropParams& p, int env, int la
 
 // Four consecutive cells i .. i + 3 of the crop window (row-major over rows x cols)
 // as one little-endian word, pad character outside the board (_do_crop :118-227).
-// One division per word (by a runtime width, as a multiply-high with the reciprocal the
-// launcher put in CropParams: exact for i < 65536), then the cell walks along the row.
+// One division per word (by a runtime width, as a multiply-high with the reciprocal in
+// CropParams::cols_recip: exact for i < 65536), then the cell walks along the row.
 __device__ __forceinline__ uint32_t crop_word(const CropParams& p, const uint8_t* board, int wr,
                                               int wc, int i, int cells) {
   const pcl_crop_spec& c = p.crop;

@@ -17,7 +17,7 @@ struct CropParams {
   const uint8_t* board;
   uint8_t* out;
   const uint8_t* curtains[PCL_MAX_TRACK];   // byte curtains of tracked drapes (or NULL)
-  uint32_t cols_recip;           // floor(2^32 / crop.cols) + 1, set by the launcher
+  uint32_t cols_recip;           // floor(2^32 / crop.cols) + 1 (crop_params, api.cu)
 };
 
 // Everything a fused step kernel needs, by value (fits the 4 KB param space).
@@ -103,16 +103,6 @@ struct RenderParams {
 };
 cudaError_t launch_render(const RenderParams& p, cudaStream_t s);
 
-struct ExportParams {
-  int B, H, W, pitch, PWW, BW, drape, scrolly;
-  const uint32_t* bits; int64_t bits_bstride;   // pattern (scrolly) or board bits
-  const int32_t* level;          // level index when `bits` is per-level static data, else NULL
-  const int32_t* drapes; int D;
-  int stale_slot;                // drape aux pair holding a stale cell, or -1
-  uint8_t* out;
-};
-cudaError_t launch_export_curtain(const ExportParams& p, cudaStream_t s);
-
 // Unoccluded layers (rendering.py:187-301): one mask per requested character.
 #define PCL_MAX_LAYER_CHARS 32
 struct LayersParams {
@@ -120,7 +110,7 @@ struct LayersParams {
   uint8_t chars[PCL_MAX_LAYER_CHARS];
   int8_t sprite_of[PCL_MAX_LAYER_CHARS];   // sprite index painting that char, or -1
   int8_t drape_of[PCL_MAX_LAYER_CHARS];    // drape index painting that char, or -1
-  // per drape: where its curtain lives in the packed state (as ExportParams)
+  // per drape: where its curtain lives in the packed state (resolve_curtain, api.cu)
   const uint32_t* bits[PCL_MAX_DRAPES]; int64_t bits_bstride[PCL_MAX_DRAPES];
   int row_words[PCL_MAX_DRAPES];           // uint32 words per bit row
   int scrolly[PCL_MAX_DRAPES];             // 1: window of a pattern at the drape's corner

@@ -1,4 +1,4 @@
-// render.cu — the stand-alone renderer, curtain export and cropper kernels.
+// render.cu — the stand-alone renderer, unoccluded-layers and cropper kernels.
 //
 // render_kernel is Engine._render() + BaseObservationRenderer (engine.py:737-759,
 // rendering.py:98-179) over reference-layout inputs: one byte per cell for the
@@ -117,39 +117,14 @@ render_kernel(const RenderParams p) {
   }
 }
 
-// Drape.curtain as bytes (things.py:213-217) from the packed device state.
-__global__ void export_curtain_kernel(const ExportParams p) {
-  const int env = blockIdx.x;
-  const int segs_per_row = p.pitch >> 4;
-  const int total = p.H * segs_per_row;
-  const int32_t* drec = p.drapes + ((int64_t)env * p.D + p.drape) * PCL_DRAPE_WORDS;
-  const int cr = p.scrolly ? drec[PCL_D_CORNER_R] : 0;
-  const int cc = p.scrolly ? drec[PCL_D_CORNER_C] : 0;
-  const int stale_r = p.stale_slot >= 0 ? drec[PCL_D_AUX0] : -1;
-  const int stale_c = p.stale_slot >= 0 ? drec[PCL_D_AUX1] : -1;
-  const int rw = p.scrolly ? p.PWW : p.BW;
-  // Read-only patterns are stored once per level (pcl_state.d_level).
-  const int64_t src_index = p.level ? p.level[env] : env;
-  const uint32_t* bits = p.bits + src_index * p.bits_bstride;
-  uint8_t* out = p.out + (int64_t)env * p.H * p.pitch;
-  for (int seg = threadIdx.x; seg < total; seg += blockDim.x) {
-    const int r = seg / segs_per_row;
-    const int c0 = (seg - r * segs_per_row) << 4;
-    const int ncols = min(16, p.W - c0);
-    unsigned b = bits16(bits + (int64_t)(cr + r) * rw, cc + c0) & ((1u << ncols) - 1u);
-    if (r == stale_r && (unsigned)(stale_c - c0) < 16u) b |= 1u << (stale_c - c0);
-    uint4 px = make_uint4(0, 0, 0, 0);
-    paint_bits(px, b, 1);
-    *reinterpret_cast<uint4*>(out + (int64_t)r * p.pitch + c0) = px;
-  }
-}
-
 // BaseUnoccludedObservationRenderer's layers (rendering.py:187-301): the mask of
 // character k shows where its OWNER places it, occluded or not — a backdrop
 // character where the backdrop holds it (paint_all_of :222-236), a drape's whole
 // curtain (paint_drape :262-282 overwrites the layer), a visible sprite's cell on
 // top of the backdrop term (paint_sprite :238-260).  One block per env streams
-// n_chars planes of H * pitch bytes (0 / 1), 16 cells per thread per store.
+// n_chars planes of H * pitch bytes (0 / 1), 16 cells per thread per store.  A
+// drape's plane is its Drape.curtain as bytes (things.py:213-217): pcl_export_curtain
+// is a one-plane launch.
 __global__ void __launch_bounds__(256) layers_kernel(const LayersParams p) {
   const int env = blockIdx.x;
   const int segs_per_row = p.pitch >> 4;
@@ -348,27 +323,17 @@ cudaError_t launch_render(const RenderParams& p, cudaStream_t s) {
   else render_kernel<8, 16><<<p.B, kRenderThreads, 0, s>>>(p);
   return cudaGetLastError();
 }
-cudaError_t launch_export_curtain(const ExportParams& p, cudaStream_t s) {
-  export_curtain_kernel<<<p.B, 128, 0, s>>>(p);
-  return cudaGetLastError();
-}
 cudaError_t launch_layers(const LayersParams& p, cudaStream_t s) {
   layers_kernel<<<p.B, 256, 0, s>>>(p);
   return cudaGetLastError();
 }
-// floor(2^32 / cols) + 1: __umulhi(i, recip) == i / cols for every i < 65536 (cols >= 1).
-static CropParams with_recip(const CropParams& p) {
-  CropParams q = p;
-  q.cols_recip = p.crop.cols > 1 ? (uint32_t)(0x100000000ull / (uint32_t)p.crop.cols) + 1u : 0u;
-  return q;
-}
 cudaError_t launch_crop(const CropParams& p, cudaStream_t s) {
   if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols >= 65536) return cudaErrorInvalidValue;
-  return launch_pdl(crop_kernel, (p.B + 3) / 4, 128, 0, s, with_recip(p));
+  return launch_pdl(crop_kernel, (p.B + 3) / 4, 128, 0, s, p);
 }
 cudaError_t launch_crop_handoff(const CropParams& p, const HandoffParams& x, cudaStream_t s) {
   if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols >= 65536) return cudaErrorInvalidValue;
-  cudaError_t e = launch_pdl(crop_handoff_kernel, (p.B + 3) / 4, 128, 0, s, with_recip(p), x);
+  cudaError_t e = launch_pdl(crop_handoff_kernel, (p.B + 3) / 4, 128, 0, s, p, x);
   if (e != cudaSuccess || !x.signal_kernel) return e;
   handoff_signal_kernel<<<1, 32, 0, s>>>(x);          // plain stream order: after the grid above retires
   return cudaGetLastError();

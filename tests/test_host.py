@@ -21,6 +21,7 @@ from pycolab_b200 import things
 from pycolab_b200.errors import DeviceOnlyError, NotLoweredError
 from pycolab_b200.games import extraterrestrial_marauders as g_marauders
 from pycolab_b200.games import scrolly_maze as g_scrolly
+from pycolab_b200.games import shockwave as g_shockwave
 from pycolab_b200.games import warehouse_manager as g_warehouse
 from pycolab_b200.prefab_parts import sprites as prefab_sprites
 
@@ -565,6 +566,10 @@ def _bound_handle(game, batch=4):
   for d in range(2):
     st.d_pattern[d], st.d_pattern_init[d] = fake, fake
     st.pattern_bstride[d], st.pattern_init_bstride[d] = 64, 64
+  # What shockwave requires: drape 0's live bits and every drape's reset bits.
+  st.d_bits[0], st.bits_bstride[0], st.d_rng = fake, 64, fake
+  for d in range(3):
+    st.d_bits_init[d] = fake
   assert lib.pcl_bind_state(handle, C.byref(st)) == _lib.OK
   return lib, handle
 
@@ -603,6 +608,55 @@ def test_attach_cropper_argument_checks_on_cpu():
   crop = batched.scrolling_crop_spec(5, 5, 0, pad_char=' ', scroll_margins=(None, None))
   assert lib.pcl_attach_cropper(h, C.byref(crop), 0x20000, 0x30000) == _lib.ERR_UNSUPPORTED
   lib.pcl_destroy(h)
+
+
+@pytest.mark.parametrize('game, call, arg, want', [
+    ('scrolly', 'attach', [-1, 1], _lib.ERR_UNSUPPORTED),       # drape medians need scratch
+    ('scrolly', 'attach', [9], _lib.ERR_INVALID),
+    ('scrolly', 'attach', [1, 9], _lib.ERR_INVALID),
+    ('scrolly', 'tracking', [9], _lib.ERR_INVALID),
+    ('scrolly', 'tracking', [1, 9], _lib.ERR_INVALID),
+    ('scrolly', 'handoff', [9], _lib.ERR_INVALID),
+    ('scrolly', 'handoff', [1, 9], _lib.ERR_INVALID),           # sprite 8 of a 4-sprite env
+    ('scrolly', 'handoff', [-1, 1], _lib.ERR_UNSUPPORTED),
+    ('scrolly', 'export', 2, _lib.ERR_INVALID),                 # only drapes 0 and 1
+    ('shockwave', 'export', 1, _lib.ERR_INVALID),               # its bits were never bound
+    ('warehouse', 'export', 0, _lib.ERR_UNSUPPORTED),           # 'X' is implicit in the boxes
+    ('warehouse', 'layers', b'X', _lib.ERR_UNSUPPORTED),
+])
+def test_cropper_and_curtain_argument_checks_on_cpu(game, call, arg, want):
+  """Every cropper entry point refuses a tracking list naming no sprite, and those without
+  drape tracking refuse drapes; pcl_export_curtain and pcl_layers refuse a drape that is
+  out of range, implicit, or not in the bound state — all before anything is launched."""
+  import ctypes as C
+  from pycolab_b200 import batched
+  if game == 'scrolly':
+    art = levels.scrolly_maze_level(3, world_shape=(33, 33), board_shape=(16, 16))
+    lib, h = _bound_handle(lowering.lower(g_scrolly.make_game(*art)))
+  elif game == 'shockwave':
+    lib, h = _bound_handle(lowering.lower(g_shockwave.make_game(0)))
+  else:
+    lib, h = _bound_handle(lowering.lower(
+        g_warehouse.make_game(levels.warehouse_level(1, shape=(20, 24)))))
+  if call in ('attach', 'tracking', 'handoff'):
+    crop = batched.scrolling_crop_spec(9, 9, 0, pad_char=' ', scroll_margins=(None, None),
+                                       track=arg)
+  if call == 'attach':
+    got = lib.pcl_attach_cropper(h, C.byref(crop), 0x20000, 0x30000)
+  elif call == 'tracking':
+    got = lib.pcl_crop_tracking(h, C.byref(crop), 0x9000, 0x20000, 0x30000, None, None)
+  elif call == 'handoff':
+    out = _lib.Outputs(0x1000, 0x2000, 0x3000, 0x4000, 0x5000)
+    x = _lib.HandoffState()
+    x.n_peers, x.rank, x.record_bytes, x.rows, x.first_row = 1, 0, 96, 4, 0
+    x.d_peer_base[0], x.d_peer_flags[0], x.d_local = 0x6000, 0x7000, 0x8000
+    got = lib.pcl_crop_handoff(h, C.byref(crop), 0x9000, 0xa000, C.byref(out), C.byref(x), None)
+  elif call == 'export':
+    got = lib.pcl_export_curtain(h, arg, 0x20000, None)
+  else:
+    got = lib.pcl_layers(h, arg, len(arg), 0x20000, None)
+  lib.pcl_destroy(h)
+  assert got == want
 
 
 def test_crop_handoff_mode_checks_on_cpu():
