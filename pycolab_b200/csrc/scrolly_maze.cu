@@ -39,12 +39,16 @@
 // was that the step is bound by the length of ONE warp's dependent chain, not by issue
 // slots, and that halving the lanes doubles every staging / paint loop on that chain.
 //
-// Residency on H100 (64x64 board): 72 registers x 128 threads allow 7 blocks of the
-// 65 536 registers, and 7424 B of dynamic shared memory per warp (29.7 KB per block) +
-// 2 KB of static selector tables + the 1 KB per-block reserve = 32 KB per block allow 7
-// of the SM's 228 KB.  Both limits give 7 blocks = 28 warps (__launch_bounds__(128, 7)),
-// so a 4096-env launch is 1.11 waves on 132 SMs; one wave would need <= 64 registers AND
-// <= 27.5 KB of shared memory per block.  The cost of the tail wave is not measured.
+// Residency on H100 (64x64 board): 64 registers x 128 threads allow 8 blocks of the
+// 65 536 registers, and 6400 B of dynamic shared memory per warp (25 KB per block) + 2 KB
+// of static selector tables + the 1 KB per-block reserve = 28 KB per block allow 8 of the
+// SM's 228 KB (static_assert below).  8 blocks = 32 warps per SM (__launch_bounds__(128,
+// 8)) = 4224 envs per wave on 132 SMs, so a 4096-env launch is one wave.  At 7 blocks (72
+// registers, segment words in a buffer of their own) it was 1.11 waves: 17.0 us per
+// 4096-env step against 15.0 us at 8 (H100 SXM, 700 W; tools/step_sweep.py and
+// DESIGN.md section 5).  Holding 64 registers without spills is why the '@' drape and the
+// coin count are read from the records only in group 2, and the records' global addresses
+// are recomputed where they are used.
 //
 // Sprite order P,a,b,c (indices 0..3); drape order '#','@' (0, 1).
 // Registers: patroller aux0 = moving_east; P aux0/aux1 = scroll permit mask /
@@ -92,13 +96,19 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
 // pattern row; from the even word at or below corner_c >> 5 it spans at most
 // 63 + W bits.  4 words (two 8-byte cp.async, one 16-byte slot) up to W = 64, 6 or 8
 // beyond (drapes.py:293-376 puts no limit on the board width).
-__host__ __device__ __forceinline__ int window_words(int W) { return 2 * ((63 + W + 63) / 64); }
+__host__ __device__ constexpr int window_words(int W) { return 2 * ((63 + W + 63) / 64); }
 
-__host__ __device__ __forceinline__ size_t warp_smem_bytes(int H, int pitch, int nw) {
-  // records, backdrop tile, two nw-word window rows per board row, one word per segment
-  const size_t rows = (((size_t)H * nw * 4) + 15) & ~(size_t)15;
-  return kRecWords * 4 + (size_t)H * pitch + 2 * rows +
-         (((size_t)H * (pitch >> 2) + 15) & ~(size_t)15);      // keep every warp's slice 16-byte aligned
+// The 4-word fast paths of staging and segment building: a board row is at most 4
+// segments (pitch >= W, so W <= 64 too).
+__host__ __device__ constexpr bool narrow_board(int pitch) { return pitch <= 64; }
+
+__host__ __device__ constexpr size_t warp_smem_bytes(int H, int W, int pitch) {
+  // records, backdrop tile, two window rows of window_words(W) per board row, and one
+  // word per 16-cell segment.  On narrow boards the segment words (pitch / 16 <= 4 per
+  // row) take the place of the wall window rows (4 words per row), which are dead by then.
+  return kRecWords * 4 + (size_t)H * pitch +
+         2 * ((((size_t)H * window_words(W) * 4) + 15) & ~(size_t)15) +
+         (narrow_board(pitch) ? 0 : (((size_t)H * (pitch >> 2) + 15) & ~(size_t)15));
 }
 
 // Programmatic dependent launch: let the next kernel of the stream begin its
@@ -127,6 +137,13 @@ constexpr SelTable make_sel_table() {
   return t;
 }
 __device__ __align__(16) const SelTable g_sel = make_sel_table();
+
+// 8 blocks per SM (__launch_bounds__ below) on a 64x64 board: a block's dynamic shared
+// memory, its per-warp selector tables and the 1 KB the SM reserves per block fit 8 times
+// in the H100's 228 KB.
+static_assert(8 * (kWarpsPerBlock * (warp_smem_bytes(64, 64, 64) + sizeof(SelTable)) + 1024) <=
+                  228 * 1024,
+              "a 64x64 scrolly_maze block no longer fits 8 times per SM");
 
 // 3x3 "blocked" mask (bit (dr+1)*3 + dc+1, sprites.py:495-507) around the virtual
 // position (vrow, vcol) of a walker whose 5x5 wall patch `field` is centred on
@@ -199,7 +216,7 @@ __device__ __forceinline__ void scrolly_move_p(Drape& d, const ScrollyCfg& cfg, 
   plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
 }
 
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, 7)
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
 scrolly_maze_step(const StepParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   // Byte-permute selectors for 4 cells at once: index = wall nibble << 4 | coin
@@ -220,7 +237,7 @@ scrolly_maze_step(const StepParams p) {
   const int pitch = p.pitch;
   const int nw = window_words(W);            // staged words per window row (4 for W <= 64)
 
-  uint8_t* my = smem_raw + warp * warp_smem_bytes(H, pitch, nw);
+  uint8_t* my = smem_raw + warp * warp_smem_bytes(H, W, pitch);
   int32_t* rec = reinterpret_cast<int32_t*>(my);
   uint8_t* s_bd = my + kRecWords * 4;
   uint32_t* s_wall = reinterpret_cast<uint32_t*>(s_bd + (size_t)H * pitch);
@@ -238,9 +255,6 @@ scrolly_maze_step(const StepParams p) {
   }
   const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
 
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * kS * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * 2 * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
   const uint32_t* wall_pat = p.st.d_pattern[0] + lvl * p.st.pattern_bstride[0];
   uint32_t* coin_pat = p.st.d_pattern[1] + (int64_t)env * p.st.pattern_bstride[1];
 
@@ -257,8 +271,9 @@ scrolly_maze_step(const StepParams p) {
     for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
   }
   // ---- 1. records -> smem (coalesced) ------------------------------------
-  rec[lane] = g_sprites[lane];
-  rec[32 + lane] = lane < 16 ? g_drapes[lane] : g_plot[lane - 16];
+  rec[lane] = p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane];
+  rec[32 + lane] = lane < 16 ? p.st.d_drapes[(int64_t)env * 2 * PCL_DRAPE_WORDS + lane]
+                             : p.st.d_plot[(int64_t)env * PCL_PLOT_WORDS + lane - 16];
   __syncwarp();
   // The decision of pcl::env_run, written out: through the helper this kernel compiles
   // to a few more instructions here, and its H100 step measured ~0.9% slower.
@@ -310,17 +325,15 @@ scrolly_maze_step(const StepParams p) {
   const int p_vrow = rec[PCL_S_VROW], p_vcol = rec[PCL_S_VCOL];
   const bool p_vis = rec[PCL_S_FLAGS] & 1;
   const int p_permit = rec[PCL_S_AUX0], p_permit_frame = rec[PCL_S_AUX1];
-  Drape walls, coins;
+  // The '@' drape and the plot's coin count stay in the records until group 2: they
+  // are not held in registers through group 1.
+  const int32_t* rec_coins = rec + 32 + PCL_DRAPE_WORDS;
+  Drape walls;
   {
     const int32_t* r = rec + 32;
     walls.corner_r = r[PCL_D_CORNER_R]; walls.corner_c = r[PCL_D_CORNER_C];
     walls.pre_r = r[PCL_D_PRE_R]; walls.pre_c = r[PCL_D_PRE_C];
     walls.last_frame = r[PCL_D_LAST_FRAME];
-    r += PCL_DRAPE_WORDS;
-    coins.corner_r = r[PCL_D_CORNER_R]; coins.corner_c = r[PCL_D_CORNER_C];
-    coins.pre_r = r[PCL_D_PRE_R]; coins.pre_c = r[PCL_D_PRE_C];
-    coins.last_frame = r[PCL_D_LAST_FRAME];
-    coins.aux0 = r[PCL_D_AUX0]; coins.aux1 = r[PCL_D_AUX1];
   }
   Plot plot;
   {
@@ -328,7 +341,6 @@ scrolly_maze_step(const StepParams p) {
     plot.frame = r[PCL_P_FRAME]; plot.error = r[PCL_P_ERROR];
     plot.order_r = r[PCL_P_ORDER_R]; plot.order_c = r[PCL_P_ORDER_C];
     plot.order_frame = r[PCL_P_ORDER_FRAME]; plot.ego_mask = r[PCL_P_EGO_MASK];
-    plot.aux0 = r[PCL_P_AUX0];
   }
 
   const ScrollyCfg wcfg = scrolly_cfg(H, W, p.PH, p.PW, p.margin[0][0], p.margin[0][1]);
@@ -344,12 +356,12 @@ scrolly_maze_step(const StepParams p) {
   const bool ordered = plot.order_frame == plot.frame;
   const int wr = walls.corner_r, wc = walls.corner_c;
   // Where the '@' window will be after it obeys the same order (checked below).
-  const int cr_pred = coins.corner_r + (ordered && motion != PCL_M_NONE ? plot.order_r : 0);
-  const int cc_pred = coins.corner_c + (ordered && motion != PCL_M_NONE ? plot.order_c : 0);
+  const int cr_pred = rec_coins[PCL_D_CORNER_R] + (ordered && motion != PCL_M_NONE ? plot.order_r : 0);
+  const int cc_pred = rec_coins[PCL_D_CORNER_C] + (ordered && motion != PCL_M_NONE ? plot.order_c : 0);
 
   // ---- 3. one batch of loads ---------------------------------------------
   const int we = (wc >> 5) & ~1, ce = (cc_pred >> 5) & ~1;   // first staged word (even)
-  const bool narrow = W <= 64;               // the 4-word fast paths (pitch <= 64)
+  const bool narrow = narrow_board(pitch);   // the 4-word fast paths
   if (narrow) {
     const int nhalf = H * 2;                 // two 8-byte halves per window row
     for (int i = lane; i < nhalf; i += 32) {
@@ -365,7 +377,11 @@ scrolly_maze_step(const StepParams p) {
       cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
     }
   }
-  scrolly_touch_prescroll(coins, plot);      // '@' has not moved yet this frame
+  // '@' has not moved yet this frame: its pre-scroll corner as scrolly_touch_prescroll
+  // will leave it in group 2.
+  const bool c_touch = rec_coins[PCL_D_LAST_FRAME] < plot.frame;
+  const int c_pre_r = rec_coins[c_touch ? PCL_D_CORNER_R : PCL_D_PRE_R];
+  const int c_pre_c = rec_coins[c_touch ? PCL_D_CORNER_C : PCL_D_PRE_C];
   // Look-up bits, one pattern ROW per lane: lanes 0..19 = row k of the 5x5 wall
   // patch of walker w (lane = 5 w + k; covers every cell any _check_motion of this
   // step can consult, wherever the scroll order moves the walker first), lanes
@@ -382,11 +398,11 @@ scrolly_maze_step(const StepParams p) {
       if ((unsigned)pr < (unsigned)p.PH) { row = wall_pat + (int64_t)pr * PWW; limit = PWW; }
     } else if (lane < 23) {
       const int r = p_vrow + (lane - 20) - 1;
-      c_first = coins.pre_c + p_vcol - 1;
-      if ((unsigned)r < (unsigned)H) { row = coin_pat + (int64_t)(coins.pre_r + r) * PWW; limit = PWW; }
+      c_first = c_pre_c + p_vcol - 1;
+      if ((unsigned)r < (unsigned)H) { row = coin_pat + (int64_t)(c_pre_r + r) * PWW; limit = PWW; }
     } else if (lane == 23) {
-      c_first = coins.pre_c;
-      row = coin_pat + (int64_t)coins.pre_r * PWW; limit = PWW;
+      c_first = c_pre_c;
+      row = coin_pat + (int64_t)c_pre_r * PWW; limit = PWW;
     }
     if (row != nullptr) {
       const int wi = c_first >> 5;           // floor, may be -1
@@ -490,6 +506,13 @@ scrolly_maze_step(const StepParams p) {
   pl.aux0 = __shfl_sync(PCL_FULL, mine.aux0, 0); pl.aux1 = __shfl_sync(PCL_FULL, mine.aux1, 0);
 
   // ---- 4b. update group 2: '@' CashDrape (scrolly_maze.py:341-364) -------
+  Drape coins;
+  coins.corner_r = rec_coins[PCL_D_CORNER_R]; coins.corner_c = rec_coins[PCL_D_CORNER_C];
+  coins.pre_r = rec_coins[PCL_D_PRE_R]; coins.pre_c = rec_coins[PCL_D_PRE_C];
+  coins.last_frame = rec_coins[PCL_D_LAST_FRAME];
+  coins.aux0 = rec_coins[PCL_D_AUX0]; coins.aux1 = rec_coins[PCL_D_AUX1];
+  scrolly_touch_prescroll(coins, plot);
+  plot.aux0 = rec[48 + PCL_P_AUX0];
   int picked_r = -1, picked_c = -1;          // pattern cell cleared this frame
   {
     const int dr = pl.row - p_vrow, dc = pl.col - p_vcol;
@@ -553,9 +576,9 @@ scrolly_maze_step(const StepParams p) {
       s_coin[i] = coin_pat[(int64_t)(cr + i / nw) * PWW + ce_final + i % nw];
   }
   __syncwarp();
-  g_sprites[lane] = rec[lane];
-  if (lane < 16) g_drapes[lane] = rec[32 + lane];
-  else g_plot[lane - 16] = rec[32 + lane];
+  p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane] = rec[lane];
+  if (lane < 16) p.st.d_drapes[(int64_t)env * 2 * PCL_DRAPE_WORDS + lane] = rec[32 + lane];
+  else p.st.d_plot[(int64_t)env * PCL_PLOT_WORDS + lane - 16] = rec[32 + lane];
 
   // ---- 5. final render, z-order a b c @ # P (engine.py:737-759) ----------
   // 5a. Window rows -> ONE word per 16-cell board segment (wall16 << 16 | coin16),
@@ -563,12 +586,17 @@ scrolly_maze_step(const StepParams p) {
   // below does no bit addressing at all.  Cells past W and the stale coin
   // (drapes.py:689 has not refreshed the curtain yet) are folded in here.
   const int spr = pitch >> 4;                // 16-byte segments per row
-  uint32_t* s_seg = s_coin + ((H * nw + 3) & ~3);
+  // Narrow boards keep the segment words where the wall window rows were.
+  uint32_t* s_seg = narrow ? s_wall : s_coin + ((H * nw + 3) & ~3);
   const int wsh = wc - (we << 5), csh = cc - (ce_final << 5);     // 0..63 into the staged row
   if (narrow) {
     const uint32_t m_lo = W >= 32 ? 0xffffffffu : (1u << W) - 1u;
     const uint32_t m_hi = W >= 64 ? 0xffffffffu : W > 32 ? (1u << (W - 32)) - 1u : 0u;
-    for (int r = lane; r < H; r += 32) {
+    // Row r's segment words land in the wall slot of row spr * r / 4 <= r, which may be
+    // another lane's row of the same round: every lane reads its rows before any lane
+    // stores.  A round stores nothing past its own rows, so later rounds read intact slots.
+    for (int r0 = 0; r0 < H; r0 += 32) {
+      const int r = min(r0 + lane, H - 1);   // lanes past the last row redo it, store nothing
       const uint4 wv = *reinterpret_cast<const uint4*>(s_wall + r * 4);
       const uint4 cv = *reinterpret_cast<const uint4*>(s_coin + r * 4);
       const uint32_t wa = (wsh & 32) ? wv.y : wv.x, wb = (wsh & 32) ? wv.z : wv.y,
@@ -579,11 +607,14 @@ scrolly_maze_step(const StepParams p) {
       const uint32_t w_hi = __funnelshift_r(wb, wd, wsh & 31) & m_hi;
       const uint32_t c_lo = __funnelshift_r(ca, cb, csh & 31) & m_lo;
       const uint32_t c_hi = __funnelshift_r(cb, cd, csh & 31) & m_hi;
-      uint32_t* out = s_seg + r * spr;
-      out[0] = __byte_perm(c_lo, w_lo, 0x5410);
-      if (spr > 1) out[1] = __byte_perm(c_lo, w_lo, 0x7632);
-      if (spr > 2) out[2] = __byte_perm(c_hi, w_hi, 0x5410);
-      if (spr > 3) out[3] = __byte_perm(c_hi, w_hi, 0x7632);
+      __syncwarp();
+      if (r0 + lane < H) {
+        uint32_t* out = s_seg + r * spr;
+        out[0] = __byte_perm(c_lo, w_lo, 0x5410);
+        if (spr > 1) out[1] = __byte_perm(c_lo, w_lo, 0x7632);
+        if (spr > 2) out[2] = __byte_perm(c_hi, w_hi, 0x5410);
+        if (spr > 3) out[3] = __byte_perm(c_hi, w_hi, 0x7632);
+      }
     }
   } else {                                   // general width: one (row, segment) per lane and round
     for (int i = lane; i < H * spr; i += 32) {
@@ -648,7 +679,7 @@ scrolly_maze_step(const StepParams p) {
 
 cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s) {
   if (p.PWW & 1) return cudaErrorInvalidValue;   // window rows are staged in 8-byte halves
-  const size_t smem = warp_smem_bytes(p.H, p.pitch, window_words(p.W)) * kWarpsPerBlock;
+  const size_t smem = warp_smem_bytes(p.H, p.W, p.pitch) * kWarpsPerBlock;
   if (smem > 227 * 1024) return cudaErrorInvalidValue;         // board too large for one CTA
   // Programmatic dependent launch: this kernel may start (prologue only) before
   // the previous kernel of the stream has drained.
