@@ -17,20 +17,22 @@
 //   2. group 0 ('#' MazeDrape) is pure register arithmetic and fixes BOTH
 //      final window corners (the '@' drape can only obey an order, never issue
 //      one: by the time it runs, the player's permit is already for frame+1);
-//   3. one batch of loads is issued for everything else the step will read:
-//        - cp.async: the backdrop tile (issued before anything else) and the
-//          two windows of the bit-packed patterns (4 words per row, two 8-byte
-//          copies) -> smem, no registers held;
-//        - plain loads: a 5x5 patch of wall bits around each of the 4 walkers
-//          (covers every cell any _check_motion of this step can consult,
-//          wherever the scroll order moves the walker first) and the 3x3 patch
-//          of coin bits around the player, one cell per lane, 4 per lane;
-//   4. groups 1 and 2 run on registers + ballots of those bits;
+//   3. plain loads, one pattern row per lane: a 5x5 patch of wall bits around each of
+//      the 4 walkers (covers every cell any _check_motion of this step can consult,
+//      wherever the scroll order moves the walker first) and the 3x3 patch of coin bits
+//      around the player;
+//   4. once those bits are in, cp.async of the backdrop tile and of the two windows of
+//      the bit-packed patterns (4 words per row, two 8-byte copies) -> smem, no
+//      registers held; groups 1 and 2 run on registers + shuffles of the patch bits
+//      while the copies fly;
 //   5. each lane shifts whole window rows once into one word per 16-cell board
 //      segment (wall16 << 16 | coin16); the paint loop then composes 16-byte
 //      segments from smem (prmt with a 256-entry selector table) and streams them
 //      out with uint4 stores; records go back with two coalesced stores.
-// So a step costs ~two dependent DRAM round trips (records, then everything).
+// So a step costs two dependent round trips (records, then the patch rows) before the
+// bulk copies start.  In a full wave (32 warps per SM) those trips, not a warp's own
+// arithmetic, set the step's length: with the copies issued first, every warp's 6 KB of
+// copies queued in front of them (DESIGN.md section 5, tools/step_phases.py).
 //
 // Tried and rejected in an A/B on the project's earlier target GPU, not re-measured on
 // H100: HALF a warp per env (two envs per warp, every warp primitive on the half's
@@ -38,6 +40,9 @@
 // Bit-exact on the whole GPU suite, but slower per 4096-env step there; the reading then
 // was that the step is bound by the length of ONE warp's dependent chain, not by issue
 // slots, and that halving the lanes doubles every staging / paint loop on that chain.
+// The phase stamps (PCL_STEP_STAMPS) do not support that reading on H100: there a lone
+// warp's step is ~7 500 cycles, but in the full wave the records and patch-row trips
+// alone took ~12 000 (DESIGN.md section 5).
 //
 // Residency on H100 (64x64 board): 64 registers x 128 threads allow 8 blocks of the
 // 65 536 registers, and 6400 B of dynamic shared memory per warp (25 KB per block) + 2 KB
@@ -138,6 +143,40 @@ constexpr SelTable make_sel_table() {
 }
 __device__ __align__(16) const SelTable g_sel = make_sel_table();
 
+// Phase stamps (build with -DPCL_STEP_STAMPS; read by tools/step_phases.py through
+// pcl_step_stamps): lane 0 of each warp stores the low 32 bits of its SM's cycle counter
+// at each phase boundary, and of %globaltimer (ns) at entry and exit, to
+// g_stamps[env].  Differences of these 32-bit stamps, taken modulo 2^32, are exact.
+// Without the switch PCL_STAMP expands to nothing and the kernel is the production one.
+// The stamp build needs 8 bytes of spill at 64 registers; tools/step_phases.py reports
+// its step time beside the production build's.
+#ifdef PCL_STEP_STAMPS
+constexpr int kStampEnvs = 8192;
+enum {
+  kStEntry, kStPrior, kStRecords, kStPatch, kStGroup2, kStWait, kStPatched, kStPaint, kStEnd,
+  kStTimeIn, kStTimeOut, kStampWords
+};
+__device__ uint32_t g_stamps[kStampEnvs][kStampWords];
+__device__ __forceinline__ uint32_t global_ns() {
+  uint32_t t;
+  asm volatile("mov.u32 %0, %%globaltimer_lo;" : "=r"(t));
+  return t;
+}
+// The env index is re-read at every stamp, so no stamp address stays live in between.
+__device__ __forceinline__ void stamp(int k, uint32_t v) {
+  uint32_t tid, cta;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(cta));
+  const uint32_t e = cta * kWarpsPerBlock + (tid >> 5);
+  if ((tid & 31) == 0 && e < (uint32_t)kStampEnvs) g_stamps[e][k] = v;
+}
+#define PCL_STAMP(k) stamp(k, (uint32_t)clock())
+#define PCL_STAMP_TIME(k) stamp(k, global_ns())
+#else
+#define PCL_STAMP(k) do {} while (0)
+#define PCL_STAMP_TIME(k) do {} while (0)
+#endif
+
 // 8 blocks per SM (__launch_bounds__ below) on a 64x64 board: a block's dynamic shared
 // memory, its per-warp selector tables and the 1 KB the SM reserves per block fit 8 times
 // in the H100's 228 KB.
@@ -219,6 +258,8 @@ __device__ __forceinline__ void scrolly_move_p(Drape& d, const ScrollyCfg& cfg, 
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
 scrolly_maze_step(const StepParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
+  PCL_STAMP(kStEntry);
+  PCL_STAMP_TIME(kStTimeIn);
   // Byte-permute selectors for 4 cells at once: index = wall nibble << 4 | coin
   // nibble; selector nibble k picks byte 5 ('#') if wall_k, else byte 4 ('@') if
   // coin_k, else byte k of the backdrop word (z-order ... '@' '#' ...).
@@ -245,6 +286,7 @@ scrolly_maze_step(const StepParams p) {
   // Everything above ran without touching state earlier kernels may have
   // produced (g_sel is a constant); from here on the kernel reads such state.
   pdl_wait_prior_grids();
+  PCL_STAMP(kStPrior);
   // An attached cropper reads its corner state at the very end: start that line's trip
   // from DRAM now (a hint, no register held).
   if (p.has_cropper && p.cropper.state && live && lane == 0)
@@ -262,19 +304,12 @@ scrolly_maze_step(const StepParams p) {
   // beside theirs, instead of one memory round trip later (it is only USED if the env
   // neither restarts nor is frozen).
   int action = env_action(p, env);
-  // ---- 0. the backdrop tile depends on nothing: get it moving first --------
-  {
-    const uint8_t* src = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * 16;
-    uint8_t* dst = s_bd + lane * 16;
-    const int n16 = (H * pitch) >> 4;
-#pragma unroll 4
-    for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
-  }
   // ---- 1. records -> smem (coalesced) ------------------------------------
   rec[lane] = p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane];
   rec[32 + lane] = lane < 16 ? p.st.d_drapes[(int64_t)env * 2 * PCL_DRAPE_WORDS + lane]
                              : p.st.d_plot[(int64_t)env * PCL_PLOT_WORDS + lane - 16];
   __syncwarp();
+  PCL_STAMP(kStRecords);
   // The decision of pcl::env_run, written out: through the helper this kernel compiles
   // to a few more instructions here, and its H100 step measured ~0.9% slower.
   const int was_over = rec[48 + PCL_P_GAME_OVER];
@@ -362,21 +397,6 @@ scrolly_maze_step(const StepParams p) {
   // ---- 3. one batch of loads ---------------------------------------------
   const int we = (wc >> 5) & ~1, ce = (cc_pred >> 5) & ~1;   // first staged word (even)
   const bool narrow = narrow_board(pitch);   // the 4-word fast paths
-  if (narrow) {
-    const int nhalf = H * 2;                 // two 8-byte halves per window row
-    for (int i = lane; i < nhalf; i += 32) {
-      const int r = i >> 1, k = (i & 1) * 2;
-      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
-      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
-    }
-  } else {                                   // boards wider than 64 columns
-    const int hw = nw >> 1, nhalf = H * hw;
-    for (int i = lane; i < nhalf; i += 32) {
-      const int r = i / hw, k = (i - r * hw) * 2;
-      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
-      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
-    }
-  }
   // '@' has not moved yet this frame: its pre-scroll corner as scrolly_touch_prescroll
   // will leave it in group 2.
   const bool c_touch = rec_coins[PCL_D_LAST_FRAME] < plot.frame;
@@ -425,6 +445,34 @@ scrolly_maze_step(const StepParams p) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) coin9 |= (__shfl_sync(PCL_FULL, rowbits, 20 + k) & colmask) << (3 * k);
     coin9 |= (__shfl_sync(PCL_FULL, rowbits, 23) & 1u) << 9;
+  }
+  PCL_STAMP(kStPatch);
+  // The bulk copies: the backdrop tile and the two windows -> smem, no registers held.
+  // They are first needed after group 2, so they are issued only now: issued ahead of
+  // the record and patch loads (as before), every warp's 6 KB of copies queued in front of
+  // those two dependent round trips, and in a full wave each trip took 2-4x as long as
+  // in a lone warp (tools/step_phases.py; DESIGN.md section 5).
+  {
+    const uint8_t* src = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * 16;
+    uint8_t* dst = s_bd + lane * 16;
+    const int n16 = (H * pitch) >> 4;
+#pragma unroll 4
+    for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
+  }
+  if (narrow) {
+    const int nhalf = H * 2;                 // two 8-byte halves per window row
+    for (int i = lane; i < nhalf; i += 32) {
+      const int r = i >> 1, k = (i & 1) * 2;
+      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
+      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
+    }
+  } else {                                   // boards wider than 64 columns
+    const int hw = nw >> 1, nhalf = H * hw;
+    for (int i = lane; i < nhalf; i += 32) {
+      const int r = i / hw, k = (i - r * hw) * 2;
+      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
+      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
+    }
   }
 
   // ---- 4a. update group 1: patrollers a, b, c then P, ONE WALKER PER LANE ----
@@ -539,9 +587,11 @@ scrolly_maze_step(const StepParams p) {
   } else if (action == 5) {
     terminate(dir);
   }
+  PCL_STAMP(kStGroup2);
 
   // ---- _apply_and_clear_plot (engine.py:761-847); no z-order changes here.
   cp_async_wait_all();
+  PCL_STAMP(kStWait);
   __syncwarp();
   if (lane == 0) {
     int32_t* r = rec + 32;
@@ -651,6 +701,7 @@ scrolly_maze_step(const StepParams p) {
     s_seg[pl.row * spr + (pl.col >> 4)] &= ~(0x00010001u << (pl.col & 15));
   }
   __syncwarp();                              // (also: this warp's s_sel copy has landed, waited above)
+  PCL_STAMP(kStPatched);
   // 5b. The streaming loop: 16 cells per lane per iteration, segment index ==
   // 16-byte index into both the staged tile and the board (pitch = 16 * spr).
   const int total = H * spr;
@@ -666,6 +717,7 @@ scrolly_maze_step(const StepParams p) {
     px.w = prmt(px.w, drape_chars, s_sel[((bits >> 24) & 0xf0u) | ((bits >> 12) & 0xfu)]);
     dst[seg] = px;
   }
+  PCL_STAMP(kStPaint);
   // ---- 6. an attached cropper (pcl_attach_cropper): the egocentric view of the board
   // this warp has just stored, without a second kernel (ScrollingCropper.crop,
   // cropping.py:393-426).
@@ -673,6 +725,8 @@ scrolly_maze_step(const StepParams p) {
     __syncwarp();
     crop_epilogue(p.cropper, p.out.d_board, env, lane, rec, rec + 48);
   }
+  PCL_STAMP(kStEnd);
+  PCL_STAMP_TIME(kStTimeOut);
 }
 
 }  // namespace
@@ -687,3 +741,13 @@ cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s) {
 }
 
 }  // namespace pcl
+
+#ifdef PCL_STEP_STAMPS
+// Copies the stamps of the last scrolly_maze_step launch for envs [0, n) to host memory
+// (n * 11 u32, in the order of the kSt* slots).  Only the stamp build exports it.
+extern "C" int pcl_step_stamps(uint32_t* host, int n) {
+  if (n < 0 || n > pcl::kStampEnvs) return -1;
+  return cudaMemcpyFromSymbol(host, pcl::g_stamps, sizeof(pcl::g_stamps[0]) * n) == cudaSuccess
+             ? 0 : -3;
+}
+#endif
