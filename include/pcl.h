@@ -156,7 +156,11 @@ typedef struct pcl_spec {
   int32_t n_sprites, n_drapes;
   int32_t auto_reset;            /* 1: an env that is game-over is rebuilt by the next step */
   int32_t pattern_rows, pattern_cols; /* Scrolly whole_pattern shape (drapes.py:338-343) */
-  int32_t pattern_words;         /* uint32 words per bit-packed pattern row: >= ceil(cols/32) + 2 (zero padded) */
+  int32_t pattern_words;         /* uint32 words per bit-packed pattern row, even and zero padded.
+                                    PCL_PROG_SCROLLY_MAZE needs >= ceil(pattern_cols/32) + 1 and
+                                    >= ((pattern_cols - cols) / 32 rounded down to even) + nw, where
+                                    nw = 2 * ceil((63 + cols) / 64) words, at least 4, are staged per
+                                    window row */
   int32_t bits_words;            /* uint32 words per bit-packed board-sized row */
   uint8_t sprite_char[PCL_MAX_SPRITES];
   uint8_t drape_char[PCL_MAX_DRAPES];

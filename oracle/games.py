@@ -55,9 +55,11 @@ def mask_position(mask):
 # scrolly_maze
 # ==========================================================================
 
-def make_scrolly_maze(maze_art, board_art, corner_mark='+', beneath='#'):
+def make_scrolly_maze(maze_art, board_art, corner_mark='+', beneath='#',
+                      margins=((2, 3), (2, 3))):
   """examples/scrolly_maze.py:212-242 with Scrolly.PatternInfo
-  (drapes.py:166-291) inlined."""
+  (drapes.py:166-291) inlined.  margins: scroll margins of '#' and '@' (the example
+  keeps the Scrolly default (2, 3) for both)."""
   world_art = art_to_array(maze_art)
   marks = np.argwhere(world_art == ord(corner_mark))
   assert len(marks) == 1
@@ -72,8 +74,8 @@ def make_scrolly_maze(maze_art, board_art, corner_mark='+', beneath='#'):
 
   backdrop, _ = split_art(board_art, 'Pabc#@', ' ')
   things = {}
-  for ch in '#@':
-    things[ch] = em.Scrolly(ch, board_shape, world_art == ord(ch), corner)
+  for ch, m in zip('#@', margins):
+    things[ch] = em.Scrolly(ch, board_shape, world_art == ord(ch), corner, margins=m)
   for ch in 'abc':
     w = em.Walker(ch, board_shape, (0, 0), impassable='#')
     em.walker_teleport(w, *vpos(ch))

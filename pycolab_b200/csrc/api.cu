@@ -112,14 +112,13 @@ int validate(const pcl_spec& s) {
       if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
       {
         // Window rows are staged from the even word at or below corner_c >> 5:
-        // 2 * ceil((63 + W) / 64) words (4 up to 64 columns) must stay inside the row.
-        const int nw = 2 * ((63 + s.cols + 63) / 64);
+        // scrolly_window_words(W) words (4 up to 64 columns) must stay inside the row.
+        const int nw = pcl::scrolly_window_words(s.cols);
         if ((s.pattern_words & 1) || s.pattern_words < (((s.pattern_cols - s.cols) >> 5) & ~1) + nw ||
             s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-        // one CTA (4 envs) stages tile + windows in shared memory
-        const long per_env = 256L + (long)s.rows * s.pitch + 2L * s.rows * nw * 4 +
-                             (long)s.rows * (s.pitch >> 2) + 64;
-        if (per_env * 4 > 227L * 1024) return PCL_ERR_UNSUPPORTED;
+        // one CTA (4 envs) stages tile + windows in shared memory: the launcher's own size
+        if (pcl::scrolly_maze_block_smem(s.rows, s.cols, s.pitch) > pcl::kScrollyMazeMaxSmem)
+          return PCL_ERR_UNSUPPORTED;
       }
       for (int d = 0; d < 2; ++d) {
         const int mr = s.margins[d][0], mc = s.margins[d][1];

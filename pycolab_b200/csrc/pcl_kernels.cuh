@@ -80,6 +80,16 @@ inline cudaError_t launch_step(void (*kern)(StepParams), const StepParams& p, in
 }
 
 cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s);
+// scrolly_maze_step: uint32 words staged per window row of a W-column board (at least 4:
+// the narrow path stages and reads 4 words per row whatever W is), its dynamic shared
+// memory per block, and the most a block may ask for on the H100 (227 KB per block less
+// the kernel's 2 KB of static selector tables).  pcl_create accepts a spec only if its
+// block fits, so an accepted spec always launches.
+__host__ __device__ constexpr int scrolly_window_words(int W) {
+  return W < 2 ? 4 : 2 * ((63 + W + 63) / 64);
+}
+size_t scrolly_maze_block_smem(int H, int W, int pitch);
+constexpr size_t kScrollyMazeMaxSmem = 227 * 1024 - 2048;
 cudaError_t launch_warehouse(const StepParams& p, cudaStream_t s);
 cudaError_t launch_marauders(const StepParams& p, cudaStream_t s);
 cudaError_t launch_fixture(const StepParams& p, cudaStream_t s);

@@ -100,8 +100,10 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
 // Words staged per window row: a W-cell window row starts at bit corner_c of its
 // pattern row; from the even word at or below corner_c >> 5 it spans at most
 // 63 + W bits.  4 words (two 8-byte cp.async, one 16-byte slot) up to W = 64, 6 or 8
-// beyond (drapes.py:293-376 puts no limit on the board width).
-__host__ __device__ constexpr int window_words(int W) { return 2 * ((63 + W + 63) / 64); }
+// beyond (drapes.py:293-376 puts no limit on the board width).  The narrow path always
+// stages and reads 4 words per row, so a one-column board is floored at 4 too (at
+// W = 1, 63 + W bits fit in 2 words).  pcl_create checks pattern_words by the same rule.
+__host__ __device__ constexpr int window_words(int W) { return scrolly_window_words(W); }
 
 // The 4-word fast paths of staging and segment building: a board row is at most 4
 // segments (pitch >= W, so W <= 64 too).
@@ -183,6 +185,8 @@ __device__ __forceinline__ void stamp(int k, uint32_t v) {
 static_assert(8 * (kWarpsPerBlock * (warp_smem_bytes(64, 64, 64) + sizeof(SelTable)) + 1024) <=
                   228 * 1024,
               "a 64x64 scrolly_maze block no longer fits 8 times per SM");
+static_assert(kScrollyMazeMaxSmem + kWarpsPerBlock * sizeof(SelTable) == 227 * 1024,
+              "kScrollyMazeMaxSmem must leave room for the static selector tables");
 
 // 3x3 "blocked" mask (bit (dr+1)*3 + dc+1, sprites.py:495-507) around the virtual
 // position (vrow, vcol) of a walker whose 5x5 wall patch `field` is centred on
@@ -731,10 +735,14 @@ scrolly_maze_step(const StepParams p) {
 
 }  // namespace
 
+size_t scrolly_maze_block_smem(int H, int W, int pitch) {
+  return warp_smem_bytes(H, W, pitch) * kWarpsPerBlock;
+}
+
 cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s) {
   if (p.PWW & 1) return cudaErrorInvalidValue;   // window rows are staged in 8-byte halves
-  const size_t smem = warp_smem_bytes(p.H, p.W, p.pitch) * kWarpsPerBlock;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;         // board too large for one CTA
+  const size_t smem = scrolly_maze_block_smem(p.H, p.W, p.pitch);
+  if (smem > kScrollyMazeMaxSmem) return cudaErrorInvalidValue;   // board too large for one CTA
   // Programmatic dependent launch: this kernel may start (prologue only) before
   // the previous kernel of the stream has drained.
   return launch_step(scrolly_maze_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);

@@ -76,12 +76,13 @@ def warehouse(name, art, wlb, actions, level=None):
        sprites=np.array(sprites, dtype=np.int32), **traj)
 
 
-def marauders(name, seed, actions):
-  art = refdriver.ref_stock_marauders_art()
+def marauders(name, seed, actions, art=None):
+  stock = art is None
+  art = refdriver.ref_stock_marauders_art() if stock else art
   chars = 'Pabcdyz'
   sprites = []
   np.random.seed(seed)            # the reference uses the global NumPy RNG
-  traj = tj.run_trajectory(lambda: refdriver.ref_marauders(), actions,
+  traj = tj.run_trajectory(lambda: refdriver.ref_marauders(None if stock else art), actions,
                            on_frame=sprite_recorder(chars, sprites))
   save(name, art=tj.art_to_u8(art), rng_seed=np.array([seed], dtype=np.int64),
        actions=np.array(actions, dtype=np.int32),
@@ -295,16 +296,17 @@ def apprehends():
         seed, int(traj['game_over'].sum()), int(traj['reward'].sum())))
 
 
-def shockwaves():
+def shockwaves(cases=None, first_seed=0):
   """examples/shockwave.py: the stock level and two generated ones (12x15, 20x40);
   `np.random.seed` fixes the global stream the impact points come from; actions 0-4
   (4 = none of the keys), biased upwards so that some episodes are won."""
   refdriver._import()
   from pycolab.examples import shockwave as ref_shock
   from pycolab_b200 import levels
-  cases = [('stock', ref_shock.LEVELS[0]), ('g12x15', levels.shockwave_level(1, safety_density=0.5)),
-           ('g20x40', levels.shockwave_level(2, 20, 40, 0.6))]
-  for seed, (tag, art) in enumerate(cases):
+  if cases is None:
+    cases = [('stock', ref_shock.LEVELS[0]), ('g12x15', levels.shockwave_level(1, safety_density=0.5)),
+             ('g20x40', levels.shockwave_level(2, 20, 40, 0.6))]
+  for seed, (tag, art) in enumerate(cases, first_seed):
     ref_shock.LEVELS.append(art)
     make = lambda: ref_shock.make_game(len(ref_shock.LEVELS) - 1)
     try:
@@ -558,6 +560,8 @@ def main():
     return apprehends()
   if sys.argv[1:] == ['shockwave']:
     return shockwaves()
+  if sys.argv[1:] == ['shapes']:
+    return shapes()
   # BASELINE.json configs[0]: stock scrolly_maze, 1000 random-action steps.
   for level, T in ((0, 1000), (1, 400), (2, 400)):
     maze, board, beneath = refdriver.ref_stock_scrolly_art(level)
@@ -724,6 +728,21 @@ def classics():
     for which, art in (('stock', None), ('other', levels.classic_level(kind))):
       actions = np.random.RandomState(len(kind) + len(which)).randint(0, n_actions, size=1200)
       classic('classic_%s_%s' % (kind, which), kind, art, actions.tolist())
+
+
+def shapes():
+  """Board shapes the step kernels branch on (tests/scrolly_shapes.py): scrolly_maze at
+  11x33 (3 segments per row), 33x63 (a ragged second round of rows, partial high half)
+  and 65x64 (a third round); marauders and shockwave at the largest board, 32x64."""
+  import scrolly_shapes as ss
+  for name in ('11x33', '33x63', '65x64'):
+    maze, board, beneath = ss.shape_level(name, 0)
+    actions = np.random.RandomState(len(name)).choice([0, 1, 2, 3, 4], size=300,
+                                                      p=[.2, .2, .27, .27, .06])
+    scrolly('scrolly_shape%s' % name, maze, board, beneath, actions.tolist())
+  marauders('marauders_shape32x64', 5, np.random.RandomState(5).randint(0, 4, size=400).tolist(),
+            art=levels.marauders_level(32, 64))
+  shockwaves([('g32x64', levels.shockwave_level(96, 32, 64, 0.5))], first_seed=3)
 
 
 if __name__ == '__main__':

@@ -33,18 +33,33 @@ def _import():
               test_things=test_things)
 
 
-def ref_scrolly_maze(maze_art, board_art, beneath='#', level=None):
+def _with_margins(drape_class, margins):
+  """A subclass of the reference's drape class that passes `scroll_margins` on (the
+  example's make_game never does)."""
+  class WithMargins(drape_class):
+    def __init__(self, *args, **kwargs):
+      kwargs['scroll_margins'] = margins
+      super(WithMargins, self).__init__(*args, **kwargs)
+  return WithMargins
+
+
+def ref_scrolly_maze(maze_art, board_art, beneath='#', level=None, margins=None):
+  """margins: None (the example's drapes) or scroll margins for ('#', '@'), each a pair
+  or None."""
   m = _import()['scrolly_maze']
   if level is not None:
     return m.make_game(level)
-  saved = (m.MAZES_ART, m.MAZES_WHAT_LIES_BENEATH, m.STAR_ART)
+  saved = (m.MAZES_ART, m.MAZES_WHAT_LIES_BENEATH, m.STAR_ART, m.MazeDrape, m.CashDrape)
   try:
     m.MAZES_ART = [maze_art]
     m.MAZES_WHAT_LIES_BENEATH = [beneath]
     m.STAR_ART = board_art
+    if margins is not None:
+      m.MazeDrape = _with_margins(saved[3], margins[0])
+      m.CashDrape = _with_margins(saved[4], margins[1])
     return m.make_game(0)
   finally:
-    m.MAZES_ART, m.MAZES_WHAT_LIES_BENEATH, m.STAR_ART = saved
+    m.MAZES_ART, m.MAZES_WHAT_LIES_BENEATH, m.STAR_ART, m.MazeDrape, m.CashDrape = saved
 
 
 def ref_stock_scrolly_art(level):

@@ -686,3 +686,84 @@ def test_crop_handoff_mode_checks_on_cpu():
   assert call(rows=3) == _lib.ERR_INVALID                              # this rank's rows do not fit
   assert call(rank=1) == _lib.ERR_INVALID
   lib.pcl_destroy(h)
+
+
+# ------------------------------------- scrolly_maze: shapes pcl_create accepts
+
+import scrolly_shapes as ss   # noqa: E402
+
+
+def _scrolly_spec(H, W, pitch=None, PW=None, pattern_words=None):
+  """A scrolly_maze pcl_spec at any board shape (margins None on both drapes)."""
+  game = lowering.lower(g_scrolly.make_game(*levels.scrolly_maze_level(
+      0, world_shape=(33, 33), board_shape=(16, 16))))
+  spec = game.make_spec(auto_reset=True)
+  PW = PW if PW is not None else W + 64
+  spec.rows, spec.cols = H, W
+  spec.pitch = pitch if pitch is not None else ss.ceil16(W)
+  spec.pattern_rows, spec.pattern_cols = H + 16, PW
+  spec.pattern_words = pattern_words if pattern_words is not None else ss.min_pattern_words(W, PW)
+  for d in range(2):
+    spec.margins[d][0] = spec.margins[d][1] = -1
+  return spec
+
+
+def test_create_rejects_a_one_column_scrolly_pattern_too_short_for_four_staged_words():
+  """The narrow path stages and reads 4 words per window row even at W = 1: a corner at
+  column 64 of a 65-column pattern reads words 2..5, so 4 words per row are too few."""
+  assert _create(_scrolly_spec(9, 1, PW=65, pattern_words=4)) == _lib.ERR_INVALID
+  assert _create(_scrolly_spec(9, 1, PW=65, pattern_words=6)) == _lib.OK
+  assert ss.min_pattern_words(1, 65) == 6
+
+
+@pytest.mark.parametrize('W', [1, 2, 16, 31, 32, 33, 48, 63, 64, 65, 96, 127, 128, 129, 130])
+def test_create_enforces_the_window_word_rule(W):
+  """pcl_create accepts pattern_words exactly from the minimum the mirror computes."""
+  for PW in (W, W + 1, W + 31, W + 64, W + 95, 3 * W + 70):
+    want = ss.min_pattern_words(W, PW)
+    assert _create(_scrolly_spec(7, W, PW=PW, pattern_words=want)) == _lib.OK, (W, PW)
+    assert _create(_scrolly_spec(7, W, PW=PW, pattern_words=want - 2)) == _lib.ERR_INVALID, (W, PW)
+
+
+def test_every_staged_word_stays_inside_its_warp_region_and_pattern_row():
+  """The mirror of the kernel's layout: for every board width 1..130 (and pitches one
+  segment wider), every shared-memory access of one warp lies inside the region
+  warp_smem_bytes gives it, the two windows do not overlap, and every pattern word a
+  staged row reads lies inside a row of the minimum pattern_words."""
+  for W in range(1, 131):
+    for pitch in (ss.ceil16(W), ss.ceil16(W) + 16):
+      for H in (1, 5, 32, 33, 65):
+        size = ss.warp_smem_bytes(H, W, pitch)
+        nw = ss.window_words(W)
+        wall = ss.REC_WORDS * 4 + H * pitch
+        coin = wall + 4 * ((H * nw + 3) & ~3)
+        assert coin >= wall + 4 * H * nw and coin + 4 * H * nw <= size, (W, pitch, H)
+        for PW in (W, W + 40, W + 64, 2 * W + 100):
+          for corner_c in {0, 31, 32, 63, 64, 95, 96, PW - W}:
+            if corner_c > PW - W:
+              continue
+            acc, words = ss.warp_accesses(H, W, pitch, corner_c, PW)
+            for off, n in acc:
+              assert 0 <= off and off + n <= size, (W, pitch, H, corner_c, off, n, size)
+            assert max(words) < ss.min_pattern_words(W, PW), (W, PW, corner_c)
+
+
+@pytest.mark.parametrize('W', [16, 48, 64, 65, 128])
+@pytest.mark.parametrize('extra', [0, 16])
+def test_largest_accepted_scrolly_board_is_launchable(W, extra):
+  """pcl_create's shared-memory test and the launcher's agree: at the largest H it
+  accepts, the block (4 warps + the static selector tables) fits the 227 KB a block can
+  opt in to; one row more is refused."""
+  pitch = ss.ceil16(W) + extra
+  lo, hi = 1, 4096
+  assert _create(_scrolly_spec(lo, W, pitch)) == _lib.OK
+  assert _create(_scrolly_spec(hi, W, pitch)) == _lib.ERR_UNSUPPORTED
+  while hi - lo > 1:
+    mid = (lo + hi) // 2
+    if _create(_scrolly_spec(mid, W, pitch)) == _lib.OK:
+      lo = mid
+    else:
+      hi = mid
+  assert ss.accepted_smem(lo, W, pitch) and not ss.accepted_smem(lo + 1, W, pitch), (W, pitch, lo)
+  block = ss.WARPS_PER_BLOCK * (ss.warp_smem_bytes(lo, W, pitch) + ss.SEL_TABLE_BYTES)
+  assert block <= ss.MAX_BLOCK_SMEM

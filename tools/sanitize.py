@@ -62,6 +62,29 @@ def main():
   print('ok crop / layers / export / observe / handoff kernels')
   wide = levels.scrolly_maze_level(9, world_shape=(41, 161), board_shape=(12, 100))
   run('scrolly_maze_step W=100', [scrolly_maze.make_game(*wide)], 5, 5)
+  # Board shapes the kernel's shared-memory layout branches on: 3 segments per row, a
+  # third round of rows, the general path on a narrow board, a one-column board.
+  sys.path.insert(0, os.path.join(ROOT, 'tests'))
+  import scrolly_shapes as ss
+  shapes = [('11x33', None, False), ('65x64', None, False), ('20x20', 80, False),
+            ('9x1_nomargins', None, True)]
+  for name, pitch, min_words in shapes:
+    board, world, margins = ss.SHAPE[name]
+    games = []
+    for i in range(2):
+      g = lowering.lower(ss.facade_game(*ss.open_level(40 + i, board, world), margins=margins))
+      if pitch is not None:
+        bd = np.zeros((g.rows, pitch), dtype=np.uint8)
+        bd[:, :g.cols] = g.backdrop[:, :g.cols]
+        g.backdrop, g.pitch = bd, pitch
+      if min_words:
+        words = ss.min_pattern_words(g.cols, g.pattern_cols)
+        g.patterns = {d: lowering.pack_rows(lowering.unpack_rows(p, g.pattern_cols), words)
+                      for d, p in g.patterns.items()}
+        g.pattern_words = words
+      games.append(g)
+    run('scrolly_maze_step %s%s' % (name, '' if pitch is None else ' pitch %d' % pitch),
+        games, 7, 5, steps=20)
   run('warehouse_step', [warehouse_manager.make_game(
       levels.warehouse_level(3, shape=(14, 21), num_boxes=4, num_goals=5))], 9, 6)
   run('marauders_step', [extraterrestrial_marauders.make_game(levels.marauders_level())], 6, 4,
