@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define PCL_ABI_VERSION 2
+#define PCL_ABI_VERSION 3
 
 #define PCL_MAX_SPRITES 16
 #define PCL_MAX_DRAPES 8
@@ -85,6 +85,19 @@ typedef enum pcl_program {
                                 d_bits[0], record AUX0 = impact cell index, AUX1 = steps since impact), ' '
                                 and '^' (static, d_bits_init[1..2]); program_arg[0] = ring width; d_rng =
                                 NumPy RandomState words (np.random.randint picks the impact cell) */
+  PCL_PROG_T_MAZE = 12,      /* examples/research/lp-rnn/t_maze.py:180-505: sprite 'P', drapes "Q#*ltr" (Q plain,
+                                curtain = the FULL cue in d_bits[0], halved on the device by which goal was
+                                drawn; the other five Scrollys over static patterns, '*' per env in
+                                d_pattern[2]).  Rewards are float64: pcl_outputs.d_reward_f64 is required.
+                                program_arg = level, cue_after_teleport, timeout frames (PCL_T_MAZE_NO_TIMEOUT
+                                = inf), teleport_delay, limbo_time.  Records: every Scrolly's AUX0 = its
+                                np.roll offset (rows << 16 | cols); 't' AUX1 = teleport delay left, AUX2 =
+                                limbo countdown; 'Q' AUX0 = which_goal (0 left, 1 right), AUX1 =
+                                yo_we_have_teleported, AUX2 = the teleporter's in-limbo flag.  Plot AUX0 =
+                                timeout_frames, AUX1 = teleportation_order_frame (-1 = unset), AUX2 / AUX3 =
+                                teleportation_order.  d_rng, when bound, is u32 [B, 2, PCL_MT_WORDS]: slot 0
+                                Python random.Random words (the cue), slot 1 NumPy RandomState words (the
+                                speckle); d_pattern_init[2] then holds the UN-speckled '*' pattern */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */
@@ -95,6 +108,9 @@ typedef enum pcl_program {
  * `next_chapter = None`. */
 enum { PCL_ORDEAL_NEXT_UNSET = -1, PCL_ORDEAL_NEXT_NONE = 0,
        PCL_ORDEAL_CASTLE = 1, PCL_ORDEAL_CAVERN = 2, PCL_ORDEAL_KANSAS = 3 };
+
+/* PCL_PROG_T_MAZE: program_arg[2] for timeout_frames = -1 (never times out). */
+#define PCL_T_MAZE_NO_TIMEOUT 0x7fffffff
 
 /* PCL_PROG_CLASSICS: pcl_spec.program_arg[0] selects the rule set; the games
  * pay float rewards (1.0, -1.0, -100.0, 100.0) which d_reward carries as the
@@ -227,6 +243,10 @@ typedef struct pcl_outputs {
   float*   d_discount;    /* f32 [B]; 1.0 running / 0.0 terminated unless a directive said otherwise
                              (plot.py:104,176-199,247-260) */
   uint8_t* d_done;        /* u8 [B]; Engine.game_over after this step */
+  double*  d_reward_f64;  /* f64 [B]; the summed reward exactly as the reference's float sum produces
+                             it, 0.0 if none.  Written only by programs whose rewards are not integers
+                             (today PCL_PROG_T_MAZE, which then leaves d_reward alone); required by
+                             them (PCL_ERR_INVALID when NULL), ignored by every other program. */
 } pcl_outputs;
 
 typedef struct pcl_handle pcl_handle;
@@ -269,6 +289,11 @@ int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps,
  * CUDA graph on `stream`. */
 int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const* d_actions,
                  const pcl_outputs* const* outs, int steps, void* stream);
+
+/* The host-buffer and hand-off entry points below (pcl_step_host, pcl_step_host_async,
+ * pcl_pack_handoff, pcl_pack_handoff_peers, pcl_crop_handoff) carry an int32 reward in their
+ * host buffers and records: they return PCL_ERR_UNSUPPORTED for a program with float64
+ * rewards (PCL_PROG_T_MAZE).  Step those with pcl_step and read d_reward_f64. */
 
 /* Host-buffer form of pcl_step: copies h_actions to the device, steps, copies
  * the outputs back into the h_* buffers (any may be NULL = skip) and

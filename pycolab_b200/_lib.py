@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # PCL_LIB_PATH: development switch for A/B runs of two builds in one process series.
 LIB_PATH = os.environ.get('PCL_LIB_PATH') or os.path.join(_HERE, 'libpcl.so')
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 MAX_SPRITES = 16
 MAX_DRAPES = 8
 MAX_TRACK = 4                # entities one ScrollingCropper can follow (pcl_crop_spec.track)
@@ -38,7 +38,8 @@ ENV_ERR_BAD_Z = 0x10
 
 PROG_NONE, PROG_SCROLLY_MAZE, PROG_WAREHOUSE, PROG_MARAUDERS, PROG_FIXTURE = 0, 1, 2, 3, 4
 PROG_BETTER_SCROLLY, PROG_CLASSICS, PROG_APERTURE, PROG_ORDEAL, PROG_HELLO = 5, 6, 7, 8, 9
-PROG_APPREHEND, PROG_SHOCKWAVE = 10, 11
+PROG_APPREHEND, PROG_SHOCKWAVE, PROG_T_MAZE = 10, 11, 12
+T_MAZE_NO_TIMEOUT = 0x7fffffff   # program_arg[2] for timeout_frames = inf
 ORDEAL_NEXT_UNSET, ORDEAL_NEXT_NONE, ORDEAL_CASTLE, ORDEAL_CAVERN, ORDEAL_KANSAS = -1, 0, 1, 2, 3
 CLASSIC_FOUR_ROOMS, CLASSIC_CLIFF_WALK, CLASSIC_CHAIN_WALK, CLASSIC_FLUVIAL = 0, 1, 2, 3
 
@@ -114,7 +115,7 @@ class State(C.Structure):
 class Outputs(C.Structure):
   _fields_ = [('d_board', C.c_void_p), ('d_reward', C.c_void_p),
               ('d_has_reward', C.c_void_p), ('d_discount', C.c_void_p),
-              ('d_done', C.c_void_p)]
+              ('d_done', C.c_void_p), ('d_reward_f64', C.c_void_p)]
 
 
 class CropSpec(C.Structure):

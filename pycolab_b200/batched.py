@@ -26,7 +26,8 @@ class StepResult(object):
 
   board: u8 [B, rows, cols] view into the engine-owned output buffer (valid
   until the next step — copy to keep, as upstream rendering.py:55-63).
-  reward: i32 [B] with has_reward u8 [B] == 0 where the reference returns None.
+  reward: i32 [B] (f64 [B] for games whose rewards are not integers, e.g. t_maze) with
+  has_reward u8 [B] == 0 where the reference returns None.
   discount: f32 [B].  done: u8 [B] (Engine.game_over).
   """
   __slots__ = ('board', 'reward', 'has_reward', 'discount', 'done')
@@ -102,10 +103,13 @@ class BatchedEngine(object):
     st.d_backdrop, st.backdrop_bstride = self.backdrop.data_ptr(), bstride(self.backdrop)
     self.patterns, self.bits = {}, {}
     self._keep_bits_init = {}
+    draws = g0.needs_rng and rng_states is not False
     for d in sorted(g0.patterns):
       arrays = [g.patterns[d].view(np.int32) for g in games]
       if g0.pattern_mutable[d]:
-        init = tiled(arrays, np.int32)
+        # a pattern the device redraws at every restart resets from its un-drawn template
+        init = tiled([g.pattern_redraw[d].view(np.int32) for g in games]
+                     if draws and d in g0.pattern_redraw else arrays, np.int32)
         live = per_env(arrays, np.int32)
         st.d_pattern_init[d], st.pattern_init_bstride[d] = init.data_ptr(), bstride(init)
         self._keep.append(init)
@@ -153,9 +157,21 @@ class BatchedEngine(object):
                             2 * _lib.FIXTURE_DIRECTIVES
                             if g0.program == _lib.PROG_FIXTURE else 1)
     self.rng = None
-    if g0.needs_rng and rng_states is not False:
+    if draws:
+      slots = 2 if g0.rng_kind == 't_maze' else 1
       if rng_states is not None:
-        states = np.ascontiguousarray(rng_states, dtype=np.uint32).reshape(B, _lib.MT_WORDS)
+        states = np.ascontiguousarray(rng_states, dtype=np.uint32).reshape(B, slots * _lib.MT_WORDS)
+      elif g0.rng_kind == 't_maze':
+        # t_maze.py:262 and :365: slot 0 = random.Random(seed) words (the cue side), slot 1 =
+        # RandomState(seed) words (the speckle field)
+        import random as _random
+        states = np.empty((B, 2, _lib.MT_WORDS), dtype=np.uint32)
+        for e in range(B):
+          states[e, 0] = _random.Random(rng_seed + env_offset + e).getstate()[1]
+          _, key, pos, _, _ = np.random.RandomState(rng_seed + env_offset + e).get_state()
+          states[e, 1, :624] = key
+          states[e, 1, 624] = pos
+        states = states.reshape(B, 2 * _lib.MT_WORDS)
       elif getattr(g0, 'rng_kind', 'numpy') == 'python':
         # Python's `random` (apprehend.py:103): the 625 words of Random(seed).getstate()
         import random as _random
@@ -181,6 +197,11 @@ class BatchedEngine(object):
     self._out = _lib.Outputs(self._board.data_ptr(), self.reward.data_ptr(),
                              self.has_reward.data_ptr(), self.discount.data_ptr(),
                              self.done.data_ptr())
+    if g0.float_reward:
+      # the kernel writes the float64 sum (pcl_outputs.d_reward_f64) and leaves d_reward alone
+      self._reward_i32 = self.reward
+      self.reward = torch.zeros((B,), dtype=torch.float64, device=dev)
+      self._out.d_reward_f64 = self.reward.data_ptr()
     self._actions = torch.zeros((B * self.actions_per_env,), dtype=torch.int32, device=dev)
     self._host = None           # pinned staging for play_host() / play_host_async(), per slot
     self._slot_shape = {}
@@ -366,6 +387,9 @@ class BatchedEngine(object):
             self.drapes[:, d, _lib.D_AUX1].long()[:, None]) % self.cols
       out.zero_()
       out[:, :, :self.cols] = self._roll_base[lvl[:, None, None], rr[:, :, None], cc[:, None, :]]
+    elif self.game.program == _lib.PROG_T_MAZE and d > 0:
+      out.zero_()
+      out[:, :, :self.cols] = self._t_maze_window(d)
     elif self.game.program == _lib.PROG_APERTURE:
       # ApertureDrape curtain = the (at most two) cells of its `_apertures` list.
       out.zero_()
@@ -378,6 +402,30 @@ class BatchedEngine(object):
                  'pcl_export_curtain', self._h)
     return out
 
+  def _t_maze_window(self, d):
+    """Curtain of t_maze Scrolly `d` as u8 [B, rows, cols]: the board window at the drape's
+    corner onto its pattern rolled by the record's AUX0 (rows << 16 | cols); the teleporter is
+    empty while its delay (AUX1) lasts (t_maze.py:397-428)."""
+    torch = _torch()
+    ph, pw = self.game.pattern_rows, self.game.pattern_cols
+    rec = self.drapes[:, d].long()
+    roll = rec[:, _lib.D_AUX0]
+    rr = (torch.arange(self.rows, device=self.device)[None, :] + rec[:, _lib.D_CORNER_R, None] +
+          (roll >> 16)[:, None]) % ph
+    cc = (torch.arange(self.cols, device=self.device)[None, :] + rec[:, _lib.D_CORNER_C, None] +
+          (roll & 0xffff)[:, None]) % pw
+    pat = self.patterns[d]
+    if pat.shape[0] != self.batch:
+      lvl = (self.level.long() if self.level is not None
+             else torch.zeros(self.batch, dtype=torch.long, device=self.device))
+    else:
+      lvl = torch.arange(self.batch, device=self.device)
+    words = pat[lvl[:, None, None], rr[:, :, None], (cc >> 5)[:, None, :]]
+    bits = ((words >> (cc & 31)[:, None, :].int()) & 1).to(torch.uint8)
+    if self.drape_chars[d] == 't':
+      bits = bits * (rec[:, _lib.D_AUX1] <= 0).to(torch.uint8)[:, None, None]
+    return bits
+
   def unoccluded_layers(self, chars=None):
     """Layers of `BaseUnoccludedObservationRenderer` (rendering.py:187-301) for
     every env: bool [B, len(chars), rows, cols], plane k = everywhere the owner of
@@ -385,6 +433,21 @@ class BatchedEngine(object):
     game, sorted (`self.chars`).  One kernel over the packed device state."""
     torch = _torch()
     chars = self.chars if chars is None else ''.join(chars)
+    if self.game.program == _lib.PROG_T_MAZE:
+      # rolled Scrolly patterns: each layer is the backdrop's cells plus its owner's curtain
+      planes = []
+      for ch in chars:
+        lvl = (self.level.long() if self.level is not None
+               else torch.zeros(self.batch, dtype=torch.long, device=self.device))
+        plane = self.backdrop[lvl, :, :self.cols].eq(ord(ch))
+        if ch in self.drape_chars:
+          plane |= self.curtain(ch)
+        elif ch in self.sprite_chars:
+          rec = self.sprites[:, self.sprite_chars.index(ch)].long()
+          b = torch.nonzero(rec[:, _lib.S_FLAGS] & 1, as_tuple=True)[0]
+          plane[b, rec[b, _lib.S_ROW], rec[b, _lib.S_COL]] = True
+        planes.append(plane)
+      return torch.stack(planes, dim=1)
     out = torch.empty((self.batch, len(chars), self.rows, self.pitch), dtype=torch.uint8,
                       device=self.device)
     _lib.check(self._lib.pcl_layers(self._h, chars.encode('ascii'), len(chars), out.data_ptr(),

@@ -250,6 +250,29 @@ int validate(const pcl_spec& s) {
       if (want_d && s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
       return PCL_OK;
     }
+    case PCL_PROG_T_MAZE: {
+      if (!chars_are(s.sprite_char, s.n_sprites, "P")) return PCL_ERR_UNSUPPORTED;
+      if (!chars_are(s.drape_char, s.n_drapes, "Q#*ltr")) return PCL_ERR_UNSUPPORTED;
+      if (!chars_are(s.z_order, 7, "*#ltrQP")) return PCL_ERR_UNSUPPORTED;
+      const int lens[3] = {3, 1, 3};
+      if (!groups_are(s, "Q#*Pltr", lens, 3)) return PCL_ERR_UNSUPPORTED;
+      if (!set_is(s.impassable[0], "#") || s.sprite_confined[0] || !s.sprite_egocentric[0])
+        return PCL_ERR_UNSUPPORTED;
+      for (int d = 1; d < 6; ++d) if (s.margins[d][0] >= 0) return PCL_ERR_UNSUPPORTED;
+      // one board row per lane; the kernel paints 16-byte rows
+      if (s.rows > 32 || s.pitch != 16) return PCL_ERR_UNSUPPORTED;
+      if (s.pattern_rows < s.rows || s.pattern_cols < s.cols || s.pattern_rows >= 32768 ||
+          s.pattern_cols >= 32768) return PCL_ERR_INVALID;
+      if (s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
+      // the speckle redraw stages the generator and one bit per pattern cell per warp
+      if (s.pattern_rows * s.pattern_cols > 32 * pcl::kTMazeMaxStreamWords) return PCL_ERR_UNSUPPORTED;
+      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
+      const int level = s.program_arg[0];
+      // TeleporterDrape.__init__ (t_maze.py:415-417): the level's hallway lies inside the pattern
+      if (level < 0 || 11 * level + 9 + 5 > s.pattern_rows) return PCL_ERR_INVALID;
+      if (s.program_arg[1] != 0 && s.program_arg[1] != 1) return PCL_ERR_INVALID;
+      return PCL_OK;
+    }
     case PCL_PROG_FIXTURE: {
       // Any MazeWalker / Scrolly / plain-drape mix; entities and z-order must
       // be consistent permutations of each other.
@@ -322,6 +345,7 @@ int launch(pcl_handle* h, const StepParams& p, cudaStream_t stream) {
     case PCL_PROG_HELLO: e = pcl::launch_hello(p, stream); break;
     case PCL_PROG_APPREHEND: e = pcl::launch_apprehend(p, stream); break;
     case PCL_PROG_SHOCKWAVE: e = pcl::launch_shockwave(p, stream); break;
+    case PCL_PROG_T_MAZE: e = pcl::launch_t_maze(p, stream); break;
     default: return PCL_ERR_UNSUPPORTED;
   }
   if (e != cudaSuccess) return cuda_failed(h, e, "step kernel launch");
@@ -341,10 +365,14 @@ bool outputs_set(const pcl_outputs& out) {
   return out.d_reward && out.d_has_reward && out.d_discount && out.d_done;
 }
 
+// Programs whose rewards are not integers write pcl_outputs.d_reward_f64 instead.
+bool float_rewards(const pcl_handle* h) { return h->spec.program == PCL_PROG_T_MAZE; }
+
 int check_ready(const pcl_handle* h, const pcl_outputs* out) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
+  if (float_rewards(h) && !out->d_reward_f64) return PCL_ERR_INVALID;
   return PCL_OK;
 }
 
@@ -440,6 +468,11 @@ int pcl_bind_state(pcl_handle* h, const pcl_state* st) {
   }
   if (h->spec.program == PCL_PROG_BETTER_SCROLLY) {
     if (!st->d_bits[0] || !st->d_bits_init[0] || st->bits_bstride[0] == 0) return PCL_ERR_INVALID;
+  }
+  if (h->spec.program == PCL_PROG_T_MAZE) {
+    if (!st->d_bits[0] || !st->d_bits_init[0] || st->bits_bstride[0] == 0) return PCL_ERR_INVALID;
+    for (int d = 1; d < 6; ++d) if (!st->d_pattern[d]) return PCL_ERR_INVALID;
+    if (!st->d_pattern_init[2] || st->pattern_bstride[2] == 0) return PCL_ERR_INVALID;
   }
   if (h->spec.n_scroll_groups > 1 && (!st->d_groups || !st->d_groups_init)) return PCL_ERR_INVALID;
   if (h->spec.program == PCL_PROG_FIXTURE) {
@@ -559,6 +592,7 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
   Range nvtx_range("pcl_step_host");
   const int r = check_ready(h, out);
   if (r != PCL_OK) return r;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions) return PCL_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t plane = (size_t)h->spec.rows * h->spec.pitch;
@@ -579,6 +613,7 @@ int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_acti
   Range nvtx_range("pcl_step_host_async");
   const int r = check_ready(h, out);
   if (r != PCL_OK) return r;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions || slot < 0 || slot >= PCL_HOST_SLOTS) return PCL_ERR_INVALID;
   if (crop && !d_crop) return PCL_ERR_INVALID;
   int e = host_pipeline_ready(h);
@@ -650,11 +685,12 @@ int resolve_curtain(const pcl_handle* h, int d, pcl::LayersParams* p) {
     p->per_level[d] = !coins && h->st.d_level != nullptr;   // read-only patterns: per level
   } else if (sp.program == PCL_PROG_MARAUDERS || sp.program == PCL_PROG_BETTER_SCROLLY ||
              sp.program == PCL_PROG_FIXTURE || sp.program == PCL_PROG_ORDEAL ||
-             sp.program == PCL_PROG_SHOCKWAVE) {
+             sp.program == PCL_PROG_SHOCKWAVE || (sp.program == PCL_PROG_T_MAZE && d == 0)) {
     p->bits[d] = h->st.d_bits[d]; p->bits_bstride[d] = h->st.bits_bstride[d];
     p->row_words[d] = sp.bits_words;
   } else {
-    return PCL_ERR_UNSUPPORTED;    // curtain held implicitly (warehouse 'X', aperture, hello)
+    return PCL_ERR_UNSUPPORTED;    // curtain held implicitly (warehouse 'X', aperture, hello) or
+                                   // a rolled pattern (t_maze's Scrollys)
   }
   return p->bits[d] ? PCL_OK : PCL_ERR_INVALID;
 }
@@ -796,6 +832,7 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   if (!h || !crop || !d_board || !out || !x) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
   if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape tracking: pcl_crop_tracking
@@ -829,6 +866,7 @@ int pcl_pack_handoff(pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
                      const pcl_outputs* out, uint8_t* d_packed, void* stream) {
   if (!h || !d_view || !out || !d_packed || view_bytes <= 0) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;
@@ -844,6 +882,7 @@ int pcl_pack_handoff_peers(pcl_handle* h, const uint8_t* d_view, int32_t view_by
     return PCL_ERR_INVALID;
   if (n_peers < 1 || n_peers > PCL_MAX_PEERS) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;

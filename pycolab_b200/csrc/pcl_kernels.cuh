@@ -100,6 +100,10 @@ cudaError_t launch_ordeal(const StepParams& p, cudaStream_t s);
 cudaError_t launch_hello(const StepParams& p, cudaStream_t s);
 cudaError_t launch_apprehend(const StepParams& p, cudaStream_t s);
 cudaError_t launch_shockwave(const StepParams& p, cudaStream_t s);
+cudaError_t launch_t_maze(const StepParams& p, cudaStream_t s);
+// t_maze_step redraws the speckle field into a per-warp bit stream of this many words
+// (one bit per pattern cell); pcl_create refuses larger patterns.
+constexpr int kTMazeMaxStreamWords = 480;
 
 struct RenderParams {
   int B, H, W, pitch, S, D;

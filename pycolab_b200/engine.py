@@ -36,6 +36,8 @@ class Engine(object):
     self._board = None
     self._batched = None
     self._backdrop_template = None   # initial curtain of a Backdrop the device animates
+    self._drape_prefills = {}        # char -> the curtain a drape was built with, before its
+                                     # constructor edited it (t_maze.py:263-266 halves the cue)
 
   # ------------------------------------------------------------ set-up API
   def set_backdrop(self, characters, backdrop_class, *args, **kwargs):
@@ -74,6 +76,7 @@ class Engine(object):
                       'Drape')
     curtain = np.zeros((self._rows, self._cols), dtype=np.bool_)
     np.copyto(dst=curtain, src=prefill, casting='equiv')
+    self._drape_prefills[character] = curtain.copy()
     drape = drape_class(curtain, character, *args, **kwargs)
     self._sprites_and_drapes[character] = drape
     self._update_groups[self._current_update_group].append(drape)
@@ -131,7 +134,7 @@ class Engine(object):
                             'terminate_episode, change_default_discount, change_z_order) are '
                             'not carried into the device\'s first frame')
     rng_states = None
-    if lowered.needs_rng and lowered.rng_kind == 'python':
+    if lowered.needs_rng and lowered.rng_kind in ('python', 't_maze'):
       # apprehend.py:103 draws in the sprite's constructor, which has already run
       # (from the global `random`, as upstream): the device takes the drawn value
       # from the template and needs no generator for this one episode.
@@ -186,9 +189,10 @@ class Engine(object):
     torch.cuda.synchronize(self._batched.device)
     board = result.board[0].cpu().numpy().copy()
     # d_reward is int32; games whose reference rewards are Python floats
-    # (examples/classics) get the equal float back.
-    reward = (self._batched.game.reward_type(int(result.reward[0]))
-              if int(result.has_reward[0]) else None)
+    # (examples/classics) get the equal float back; t_maze's are float64 on the device.
+    value = result.reward[0]
+    value = float(value) if self._batched.game.float_reward else int(value)
+    reward = self._batched.game.reward_type(value) if int(result.has_reward[0]) else None
     discount = float(result.discount[0])
     self._game_over = bool(int(result.done[0]))
     self._sync_things()
@@ -256,10 +260,25 @@ class Engine(object):
           from pycolab_b200 import lowering
           packed = b.patterns[i][0].cpu().numpy().view(np.uint32)
           np.copyto(ent.whole_pattern, lowering.unpack_rows(packed, ent.whole_pattern.shape[1]))
+      if b.game.program == _lib.PROG_T_MAZE and i > 0:
+        self._sync_rolled_pattern(ent, i, rec)
       np.copyto(ent.curtain, b.curtain(ch)[0].cpu().numpy())
       if b.game.program == _lib.PROG_APERTURE:       # ApertureDrape._apertures
         cells = [int(rec[_lib.D_AUX0]), int(rec[_lib.D_AUX1])]
         ent._apertures = [None if c < 0 else (c >> 16, c & 0xffff) for c in cells]
+
+  def _sync_rolled_pattern(self, ent, d, rec):
+    """t_maze: whole_pattern = the drape's pattern np.rolled by its record's AUX0 (rows << 16
+    | cols); the teleporter's is empty while its delay lasts (t_maze.py:397-400)."""
+    from pycolab_b200 import lowering
+    b = self._batched
+    shape = ent.whole_pattern.shape
+    base = lowering.unpack_rows(b.patterns[d][0].cpu().numpy().view(np.uint32), shape[1])
+    roll = int(rec[_lib.D_AUX0])
+    base = np.roll(np.roll(base, -(roll >> 16), axis=0), -(roll & 0xffff), axis=1)
+    if b.drape_chars[d] == 't' and int(rec[_lib.D_AUX1]) > 0:
+      base[:] = False
+    np.copyto(ent.whole_pattern, base)
 
   # ------------------------------------------------------------ properties
   @property

@@ -215,3 +215,47 @@ def shockwave_level(seed, height=12, width=15, safety_density=0.15):
   level[-1, int(rs.randint(0, width - 1))] = ord('P')
   level[0] = ord('^')
   return _to_art(level)
+
+
+def t_maze_level(seed=0, shape=(77, 191)):
+  """A research/lp-rnn/t_maze.py world: (maze_art, cue_art).
+
+  The drapes hard-code where things are (t_maze.py:407-415), so the generator keeps those
+  constants and draws the rest: the start room with the teleporter on row 4 and the board
+  corner '+' at (3, 89) (the 7 x 11 board shows the room), the limbo cell (4, 140) walled
+  in on all eight sides, and for every level L a T-maze whose hallway row 13 + 11 L lies
+  dy = 11 L + 9 rows below the teleporter and the limbo cell, centred on column 94 = 140 - 46
+  with goal pads 'l' / 'r' at the ends of two corridors.  The half-width of each level's
+  hallway grows with L and is drawn from RandomState(seed); everything else is dirt '*'.
+  The cue is 'Q' blocks in the bottom rows, on both sides of the board."""
+  rs = np.random.RandomState(seed)
+  rows, cols = shape
+  assert rows >= 11 * 5 + 9 + 5 + 8 and cols >= 191
+  art = np.full((rows, cols), ord('*'), dtype=np.uint8)
+  art[:10] = ord(' ')
+  art[3:8, 92:97] = ord('#')                        # start room, teleporter row 4
+  art[4:7, 93:96] = ord(' ')
+  art[4, 93:96] = ord('t')
+  art[6, 94] = ord('P')
+  art[3, 89] = ord('+')
+  art[3:6, 139:142] = ord('#')                      # limbo cell (4, 140)
+  art[4, 140] = ord(' ')
+  centre = 140 - 46
+  widths = (8, 13, 20, 33, 53, 88)
+  for level, base in enumerate(widths):
+    h = min(base + int(rs.randint(0, 4)), centre - 1, cols - centre - 2)
+    y = 12 + 11 * level
+    west, east = centre - h, centre + h
+    art[y:y + 8, west:east + 1] = ord('#')
+    art[y + 1:y + 3, west + 1:east] = ord(' ')      # the hallway
+    art[y + 3:y + 6, west + 1:west + 4] = ord(' ')  # the corridors
+    art[y + 3:y + 6, east - 3:east] = ord(' ')
+    art[y + 6, west + 1:west + 4] = ord('l')
+    art[y + 6, east - 3:east] = ord('r')
+    art[y + 4:y + 7, west + 5:east - 4] = ord('*')
+  cue = np.full((7, 11), ord(' '), dtype=np.uint8)
+  block = 1 + int(rs.randint(0, 3))                 # 1-3 columns on each side
+  first = 7 - (2 + int(rs.randint(0, 3)))
+  cue[first:, :block] = ord('Q')
+  cue[first:, 11 - block:] = ord('Q')
+  return _to_art(art), _to_art(cue)

@@ -57,6 +57,12 @@ LOWERED_CLASSES = {
     ('shockwave', 'MinimalDrape'): 'shockwave.minimal',
     ('apprehend', 'PlayerSprite'): 'apprehend.player',
     ('apprehend', 'BallSprite'): 'apprehend.ball',
+    ('t_maze', 'PlayerSprite'): 't_maze.player',
+    ('t_maze', 'CueDrape'): 't_maze.cue',
+    ('t_maze', 'MazeDrape'): 't_maze.maze',
+    ('t_maze', 'SpeckleDrape'): 't_maze.speckle',
+    ('t_maze', 'TeleporterDrape'): 't_maze.teleporter',
+    ('t_maze', 'GoalDrape'): 't_maze.goal',
     ('ordeal', 'PlayerSprite'): 'ordeal.player',
     ('ordeal', 'DragonduckSprite'): 'ordeal.dragonduck',
     ('ordeal', 'SwordDrape'): 'ordeal.sword',
@@ -198,6 +204,8 @@ class LoweredGame(object):
     self.backdrop = None        # u8 [H, pitch]
     self.patterns = {}          # drape index -> u32 [PH, PWW]
     self.pattern_mutable = {}   # drape index -> bool
+    self.pattern_redraw = {}    # drape index -> u32 [PH, PWW]: reset template of a pattern the
+                                # device redraws at every restart (when an RNG is bound)
     self.bits = {}              # drape index -> u32 [H, BW]
     self.sprites = None         # i32 [S, 8]
     self.drapes = None          # i32 [D, 8]
@@ -210,6 +218,7 @@ class LoweredGame(object):
     self.dynamic_z = False      # per-env z-order array (Plot.change_z_order)
     self.program_arg = [0] * 8  # pcl_spec.program_arg
     self.reward_type = int      # the reference's reward type (classics pay floats)
+    self.float_reward = False   # rewards are not integers: pcl_outputs.d_reward_f64
     self.backdrop_role = None   # device counterpart of a Backdrop with update() logic
     self.scroll_groups = ['']   # names of the scrolling groups, index = device group id
     self.sprite_group = []      # per sprite: index into scroll_groups
@@ -612,6 +621,100 @@ def _lower_shockwave(engine, roles):
   return game
 
 
+def _lower_t_maze(engine, roles):
+  """examples/research/lp-rnn/t_maze.py:180-505: 'P', the cue 'Q' and five
+  PseudoTeleportingScrollys (drapes 'Q#*ltr' on the device).  What the constructors drew —
+  the cue side, the speckle — is in the templates; with an RNG bound a batched engine redraws
+  both at every restart from the UN-speckled '*' pattern (`pattern_redraw`) and the full cue
+  (`bits[0]`, halved on the device)."""
+  th, plot = engine.things, engine.the_plot
+  want = {'P': 't_maze.player', 'Q': 't_maze.cue', '#': 't_maze.maze', '*': 't_maze.speckle',
+          't': 't_maze.teleporter', 'l': 't_maze.goal', 'r': 't_maze.goal'}
+  if roles != want:
+    raise NotLoweredError('t_maze program needs exactly {} (got {})'.format(want, roles))
+  game = LoweredGame()
+  _common(engine, game, _lib.PROG_T_MAZE)
+  if game.groups != ['Q#*', 'P', 'ltr'] or game.z_order != '*#ltrQP':
+    raise NotLoweredError("t_maze program needs update groups [Q # *] [P] [l t r] and z-order "
+                          "'*#ltrQP'")
+  if engine.rows > 32 or engine.cols > 16:
+    raise NotLoweredError('t_maze program: boards up to 32 x 16')
+  if th['l']._name != 'left' or th['r']._name != 'right':
+    raise NotLoweredError("t_maze program needs the 'left' goal on 'l' and the 'right' on 'r'")
+  player = th['P']
+  _set_sprites(game, [player], [_sprite_record(player, aux0=0, aux1=_lib.NEVER)])
+  scrollys = '#*ltr'
+  shape = th['#'].whole_pattern.shape
+  for ch in scrollys:
+    d = th[ch]
+    if d._scrolling_group != '' or d._scroll_margins is not None:
+      raise NotLoweredError('t_maze Scrollys have margins None in the default scrolling group')
+    if d.whole_pattern.shape != shape or tuple(d._board_shape) != (engine.rows, engine.cols):
+      raise NotLoweredError('t_maze Scrolly patterns of different shapes')
+  tele = th['t']
+  level = (tele._dy - 9) // 11
+  if (11 * level + 9 != tele._dy or (tele._limbo_row, tele._limbo_col, tele._dx) != (4, 140, -46)
+      or tele._in_limbo):
+    raise NotLoweredError('t_maze teleporter with other limbo constants')
+  # TeleporterDrape lands the player in the level's hallway: that cell must exist and be free.
+  hall = (tele._limbo_row + tele._dy, tele._limbo_col + tele._dx)
+  if not (0 <= hall[0] < shape[0] and 0 <= hall[1] < shape[1]) or th['#'].whole_pattern[hall]:
+    raise NotLoweredError('t_maze level {} has no hallway at {}'.format(level, hall))
+  game.drape_chars = 'Q' + scrollys
+  game.margins = [(-1, -1)] * 6
+  game.pattern_rows, game.pattern_cols = shape
+  game.pattern_words = round_up((shape[1] + 31) // 32 + 1, 2)
+  tele_pattern = tele._saved_whole_pattern if tele._teleport_delay > 0 else tele.whole_pattern
+  for d, ch in enumerate(scrollys, 1):
+    game.patterns[d] = pack_rows(tele_pattern if ch == 't' else th[ch].whole_pattern,
+                                 game.pattern_words)
+    game.pattern_mutable[d] = ch == '*'
+  game.pattern_redraw[2] = pack_rows(th['*']._pattern_at_init, game.pattern_words)
+  cue = th['Q']
+  full_cue = engine._drape_prefills['Q']
+  if cue.which_goal not in ('left', 'right'):
+    raise NotLoweredError('t_maze cue names no goal')
+  game.bits = {0: pack_rows(full_cue, game.bits_words)}
+  recs = [[0] * _lib.DRAPE_WORDS]
+  recs[0][_lib.D_LAST_FRAME] = _lib.NEVER
+  recs[0][_lib.D_AUX0] = 0 if cue.which_goal == 'left' else 1
+  recs[0][_lib.D_AUX1] = 1 if plot.get('yo_we_have_teleported') else 0
+  for ch in scrollys:
+    recs.append(_scrolly_record(th[ch]))
+  recs[4][_lib.D_AUX1] = int(tele._teleport_delay)
+  recs[4][_lib.D_AUX2] = int(tele._limbo_countdown)
+  game.drapes = np.array(recs, dtype=np.int32)
+  timeout = plot['timeout_frames']
+  order = plot.get('teleportation_order', (0, 0))
+  game.plot = np.array(_plot_record(
+      aux0=_lib.T_MAZE_NO_TIMEOUT if timeout == float('inf') else int(timeout),
+      aux1=plot.get('teleportation_order_frame', -1), aux2=order[0], aux3=order[1]),
+      dtype=np.int32)
+  game.program_arg[:5] = [level, 1 if cue._cue_after_teleport else 0,
+                          _lib.T_MAZE_NO_TIMEOUT if timeout == float('inf') else int(timeout),
+                          int(tele._teleport_delay), int(tele._limbo_countdown)]
+  game.needs_rng = True
+  game.rng_kind = 't_maze'        # two MT19937 streams per env: Python's random, NumPy's
+  game.reward_type = float
+  game.float_reward = True
+
+  def sync_plot(eng, words):
+    p, b = eng.the_plot, eng.batched
+    p['timeout_frames'] = (float('inf') if int(words[_lib.P_AUX0]) == _lib.T_MAZE_NO_TIMEOUT
+                           else int(words[_lib.P_AUX0]))
+    if int(words[_lib.P_AUX1]) >= 0:
+      p['teleportation_order_frame'] = int(words[_lib.P_AUX1])
+      p['teleportation_order'] = (int(words[_lib.P_AUX2]), int(words[_lib.P_AUX3]))
+    q = b.drapes[0, 0].cpu().numpy()
+    if q[_lib.D_AUX1]:
+      p['yo_we_have_teleported'] = True
+    elif 'yo_we_have_teleported' in p:
+      del p['yo_we_have_teleported']
+    eng.things['Q'].which_goal = 'left' if q[_lib.D_AUX0] == 0 else 'right'
+  game.sync_plot = sync_plot
+  return game
+
+
 def _update_order(engine):
   return [e.character for _, ents in sorted(engine._update_groups.items()) for e in ents]
 
@@ -783,7 +886,7 @@ def lower(engine):
               'classics': _lower_classics, 'better': _lower_better_scrolly,
               'aperture': _lower_aperture, 'ordeal': _lower_ordeal,
               'hello': _lower_hello, 'apprehend': _lower_apprehend,
-              'shockwave': _lower_shockwave}
+              'shockwave': _lower_shockwave, 't_maze': _lower_t_maze}
   if family not in lowerers:
     raise NotLoweredError(family)
   game = lowerers[family](engine, roles)

@@ -75,6 +75,9 @@ class Scrolly(things.Drape):
     self._northwest_corner = things.Sprite.Position(*board_northwest_corner)
     self._scrolling_group = scrolling_group
     self._w_h_o_l_e_p_a_t_t_e_r_n = whole_pattern
+    # The pattern as handed in, before a subclass's constructor edits it (t_maze.py:365
+    # speckles it at random): a device that redraws at every restart starts from this.
+    self._pattern_at_init = np.array(whole_pattern, dtype=bool)
     self._northwest_corner_limit = (whole_pattern.shape[0] - board_shape[0],
                                     whole_pattern.shape[1] - board_shape[1])
     if min(self._northwest_corner_limit) < 0:

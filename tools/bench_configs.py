@@ -45,6 +45,19 @@ def build(name):
                 crop=True,
                 what='scrolly_maze 64x64 + ScrollingCropper 9x9 egocentric, 8192 envs per GPU '
                      '(configs[4] = 65536 over 8 GPUs)')
+  if name == 't_maze':
+    from pycolab_b200.games import t_maze as g
+    games = []
+    for i in range(6):                    # six generated worlds, level 4, 100-frame episodes
+      maze, cue = levels.t_maze_level(i)
+      games.append(lowering.lower(g.make_game(4, False, 100, 5, 10, maze_art=maze,
+                                              cue_art=cue)))
+    return dict(games=games, batch=4096, actions=[1, 2, 3, 4, 5], rotation=3,
+                a_step=7 * 16 + 4 * (8 + 6 * 8 + 16) + 7 * 2 * 4 + 14,
+                kernel='t_maze_step', float_reward=True,
+                what='research/lp-rnn/t_maze level 4, six generated 77x191 worlds, 7x11 board, '
+                     '4096 envs, timeout 100 frames: every env redraws its cue and 191x77 '
+                     'speckle once per 101 steps')
   raise SystemExit('unknown config %r' % name)
 
 
@@ -63,7 +76,10 @@ def run(name, steps=600, warmup=30):
     crop_spec = batched.scrolling_crop_spec(9, 9, 0, pad_char=' ',
                                             scroll_margins=(None, None))
   rs = np.random.RandomState(1)
-  acts_np = rs.randint(0, cfg['n_actions'], size=(warmup + steps, B)).astype(np.int32)
+  if 'actions' in cfg:
+    acts_np = rs.choice(cfg['actions'], size=(warmup + steps, B)).astype(np.int32)
+  else:
+    acts_np = rs.randint(0, cfg['n_actions'], size=(warmup + steps, B)).astype(np.int32)
   acts = torch.from_numpy(acts_np).to(dev)
 
   def step(t, i):
@@ -84,6 +100,23 @@ def run(name, steps=600, warmup=30):
   torch.cuda.synchronize()
   ms = a.elapsed_time(b) / steps
   launches = sum(e.launch_count() for e in engines) - l0
+  if cfg.get('float_reward'):
+    # the host-buffer entry points carry an int32 reward and refuse this program: no e2e
+    # leg; instead the cost of the restart draws, a pcl_reset of every env (cue + speckle)
+    n_reset = 20
+    torch.cuda.synchronize()
+    a.record()
+    for _ in range(n_reset):
+      engines[0].reset()
+    b.record()
+    torch.cuda.synchronize()
+    reset_ms = a.elapsed_time(b) / n_reset
+    print(json.dumps({
+        'config': name, 'workload': cfg['what'], 'batch': B, 'rotation': R,
+        'metric': 'env_steps_per_sec', 'value': B / (ms / 1000.0), 'ms_per_step': ms,
+        'steps': steps, 'gpu_launches': launches, 'reset_all_ms': reset_ms,
+        'env_errors': max(int(e.error_codes().abs().max()) for e in engines)}))
+    return
 
   # End to end: pinned host actions in, (board or crop) + scalars out.
   eng = engines[0]

@@ -24,7 +24,7 @@ def main():
   from pycolab_b200 import batched, dist as pdist, levels, lowering
   from pycolab_b200.games import (aperture, better_scrolly_maze, extraterrestrial_marauders,
                                   apprehend, fixtures, fluvial_natation, hello_world, ordeal,
-                                  shockwave,
+                                  shockwave, t_maze,
                                   scrolly_maze, warehouse_manager)
   from pycolab_b200.games.classics import chain_walk, cliff_walk, four_rooms
   rs = np.random.RandomState(0)
@@ -106,6 +106,8 @@ def main():
   run('apprehend_step (device RNG)', [apprehend.make_game()], 5, 3, steps=30)
   run('shockwave_step', [shockwave.make_game(0), shockwave.make_game(levels.shockwave_level(3, 9, 33))][:1], 5, 5, steps=40)
   run('shockwave_step 9x33', [shockwave.make_game(levels.shockwave_level(3, 9, 33))], 6, 5, steps=40)
+  run('t_maze_step (device RNG)', [t_maze.make_game(1, False, 20, 2, 3, *levels.t_maze_level(s))
+                                   for s in range(2)], 6, 7, steps=45)
   pattern = rs.random_sample((17, 23)) < 0.2
   fx = fixtures.make_game(['           ', '   P       ', '      q    ', '           ',
                            '           ', '           '], ' ',
