@@ -164,11 +164,27 @@ aperture_step(const StepParams p) {
   for (int seg = lane; seg < (tile >> 4); seg += 32) dst[seg] = src[seg];
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (s.n_sprites != 1 || s.n_drapes != 1) return PCL_ERR_UNSUPPORTED;
+  if (s.z_order[0] != s.drape_char[0] || s.z_order[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
+  if (s.n_groups != 2 || s.group_len[0] != 1 || s.group_len[1] != 1 ||
+      s.group_chars[0] != s.sprite_char[0] || s.group_chars[1] != s.drape_char[0])
+    return PCL_ERR_UNSUPPORTED;
+  if (s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
+  if (s.rows >= 32768 || s.cols >= 32768 || s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;
+  return PCL_OK;
+}
 
-cudaError_t launch_aperture(const StepParams& p, cudaStream_t s) {
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch) * kWarpsPerBlock;
   return launch_step(aperture_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+// The drape's curtain is held implicitly (its record's AUX0 / AUX1): nothing to resolve.
+const Program kAperture = {check_spec, nullptr, nullptr, launch, nullptr,
+                           /*float_reward=*/false, /*crop_epilogue=*/false,
+                           /*scroll_groups=*/false};
 
 }  // namespace pcl

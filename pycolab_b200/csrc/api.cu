@@ -13,6 +13,7 @@
 
 struct pcl_handle {
   pcl_spec spec;
+  const pcl::Program* program;   // the descriptor of spec.program
   int batch;
   int device;
   int bound;
@@ -53,256 +54,58 @@ int cuda_failed(pcl_handle* h, cudaError_t e, const char* what) {
     if (e_ != cudaSuccess) return cuda_failed((h), e_, #call);   \
   } while (0)
 
-bool chars_are(const uint8_t* got, int n, const char* want) {
-  if ((int)strlen(want) != n) return false;
-  for (int i = 0; i < n; ++i) if (got[i] != (uint8_t)want[i]) return false;
-  return true;
-}
+int accept_any(const pcl_spec&) { return PCL_OK; }
 
-// The set `want` as a 128-bit ASCII mask equals `got`?
-bool set_is(const uint32_t (&got)[4], const char* want) {
-  uint32_t m[4] = {0, 0, 0, 0};
-  for (const char* c = want; *c; ++c) m[(*c >> 5) & 3] |= 1u << (*c & 31);
-  return m[0] == got[0] && m[1] == got[1] && m[2] == got[2] && m[3] == got[3];
-}
+// No step program: a handle for pcl_render / pcl_crop only; its steps are refused.
+const pcl::Program kNone = {accept_any, nullptr, nullptr, nullptr, nullptr,
+                            /*float_reward=*/false, /*crop_epilogue=*/false,
+                            /*scroll_groups=*/false};
 
-int groups_are(const pcl_spec& s, const char* flat, const int* lens, int n) {
-  if (s.n_groups != n) return 0;
-  int k = 0;
-  for (int g = 0; g < n; ++g) {
-    if (s.group_len[g] != lens[g]) return 0;
-    for (int i = 0; i < lens[g]; ++i, ++k)
-      if (s.group_chars[k] != (uint8_t)flat[k]) return 0;
-  }
-  return 1;
+const struct {
+  int id;
+  const pcl::Program* program;
+} kPrograms[] = {
+    {PCL_PROG_NONE, &kNone},
+    {PCL_PROG_SCROLLY_MAZE, &pcl::kScrollyMaze},
+    {PCL_PROG_WAREHOUSE, &pcl::kWarehouse},
+    {PCL_PROG_MARAUDERS, &pcl::kMarauders},
+    {PCL_PROG_FIXTURE, &pcl::kFixture},
+    {PCL_PROG_BETTER_SCROLLY, &pcl::kBetterScrolly},
+    {PCL_PROG_CLASSICS, &pcl::kClassics},
+    {PCL_PROG_APERTURE, &pcl::kAperture},
+    {PCL_PROG_ORDEAL, &pcl::kOrdeal},
+    {PCL_PROG_HELLO, &pcl::kHello},
+    {PCL_PROG_APPREHEND, &pcl::kApprehend},
+    {PCL_PROG_SHOCKWAVE, &pcl::kShockwave},
+    {PCL_PROG_T_MAZE, &pcl::kTMaze},
+};
+
+// The descriptor of program `id`, or nullptr for an id this build does not know.
+const pcl::Program* program_of(int id) {
+  for (const auto& row : kPrograms) if (row.id == id) return row.program;
+  return nullptr;
 }
 
 // Each program is lowered for one entity layout; anything else is a valid
 // pycolab game that this build does not accelerate.
 int validate(const pcl_spec& s) {
+  const pcl::Program* prog = program_of(s.program);
   if (s.abi_version != PCL_ABI_VERSION) return PCL_ERR_INVALID;
   if (s.rows <= 0 || s.cols <= 0 || s.pitch < s.cols || (s.pitch & 15)) return PCL_ERR_INVALID;
   if (s.n_sprites < 0 || s.n_sprites > PCL_MAX_SPRITES) return PCL_ERR_INVALID;
   if (s.n_drapes < 0 || s.n_drapes > PCL_MAX_DRAPES) return PCL_ERR_INVALID;
   {
-    // Scrolling groups: every entity names one of the declared groups; only the
-    // general program keeps more than one group's blackboard.
+    // Scrolling groups: every entity names one of the declared groups; only
+    // programs that keep more than one group's blackboard accept several.
     const int ng = s.n_scroll_groups < 1 ? 1 : s.n_scroll_groups;
     if (ng > PCL_MAX_SCROLL_GROUPS) return PCL_ERR_UNSUPPORTED;
-    if (ng > 1 && s.program != PCL_PROG_FIXTURE) return PCL_ERR_UNSUPPORTED;
+    if (ng > 1 && !(prog && prog->scroll_groups)) return PCL_ERR_UNSUPPORTED;
     for (int i = 0; i < s.n_sprites; ++i)
       if (s.sprite_group[i] < 0 || s.sprite_group[i] >= ng) return PCL_ERR_INVALID;
     for (int i = 0; i < s.n_drapes; ++i)
       if (s.drape_group[i] < 0 || s.drape_group[i] >= ng) return PCL_ERR_INVALID;
   }
-  switch (s.program) {
-    case PCL_PROG_NONE:
-      return PCL_OK;
-    case PCL_PROG_SCROLLY_MAZE: {
-      if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.drape_char, s.n_drapes, "#@")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.z_order, 6, "abc@#P")) return PCL_ERR_UNSUPPORTED;
-      const int lens[3] = {1, 4, 1};
-      if (!groups_are(s, "#abcP@", lens, 3)) return PCL_ERR_UNSUPPORTED;
-      for (int i = 0; i < 4; ++i) {
-        if (!set_is(s.impassable[i], "#")) return PCL_ERR_UNSUPPORTED;
-        if (s.sprite_confined[i]) return PCL_ERR_UNSUPPORTED;
-        if (s.sprite_egocentric[i] != (i == 0)) return PCL_ERR_UNSUPPORTED;
-      }
-      if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
-      {
-        // Window rows are staged from the even word at or below corner_c >> 5:
-        // scrolly_window_words(W) words (4 up to 64 columns) must stay inside the row.
-        const int nw = pcl::scrolly_window_words(s.cols);
-        if ((s.pattern_words & 1) || s.pattern_words < (((s.pattern_cols - s.cols) >> 5) & ~1) + nw ||
-            s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-        // one CTA (4 envs) stages tile + windows in shared memory: the launcher's own size
-        if (pcl::scrolly_maze_block_smem(s.rows, s.cols, s.pitch) > pcl::kScrollyMazeMaxSmem)
-          return PCL_ERR_UNSUPPORTED;
-      }
-      for (int d = 0; d < 2; ++d) {
-        const int mr = s.margins[d][0], mc = s.margins[d][1];
-        if (mr >= 0 && (mc - 1 >= s.cols - mc || mr - 1 >= s.rows - mr)) return PCL_ERR_INVALID;
-      }
-      return PCL_OK;
-    }
-    case PCL_PROG_WAREHOUSE: {
-      const int nb = s.n_sprites - 1;
-      if (nb < 1 || nb > 10) return PCL_ERR_UNSUPPORTED;
-      if (s.sprite_char[nb] != 'P') return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.drape_char, s.n_drapes, "X")) return PCL_ERR_UNSUPPORTED;
-      const char* order = "1234567890";
-      int k = 0;
-      for (int i = 0; i < nb; ++i) {
-        while (order[k] && order[k] != (char)s.sprite_char[i]) ++k;
-        if (!order[k]) return PCL_ERR_UNSUPPORTED;
-        ++k;
-        if (s.z_order[i] != s.sprite_char[i]) return PCL_ERR_UNSUPPORTED;
-        if (s.sprite_confined[i] || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-      }
-      if (s.z_order[nb] != 'X' || s.z_order[nb + 1] != 'P') return PCL_ERR_UNSUPPORTED;
-      if (s.n_groups != 3 || s.group_len[0] != nb || s.group_len[1] != 1 || s.group_len[2] != 1)
-        return PCL_ERR_UNSUPPORTED;
-      for (int i = 0; i < nb; ++i)
-        if (s.group_chars[i] != s.sprite_char[i]) return PCL_ERR_UNSUPPORTED;
-      if (s.group_chars[nb] != 'X' || s.group_chars[nb + 1] != 'P') return PCL_ERR_UNSUPPORTED;
-      return PCL_OK;
-    }
-    case PCL_PROG_MARAUDERS: {
-      if (!chars_are(s.sprite_char, s.n_sprites, "Pabcdyz")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.drape_char, s.n_drapes, "BX")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.z_order, 9, "PBXabcdyz")) return PCL_ERR_UNSUPPORTED;
-      const int lens[1] = {9};
-      if (!groups_are(s, "PBXabcdyz", lens, 1)) return PCL_ERR_UNSUPPORTED;
-      if (s.rows > 32 || s.rows < 11 || s.cols > 64 || s.bits_words < 2)
-        return PCL_ERR_UNSUPPORTED;
-      for (int i = 0; i < 7; ++i) {
-        if (!set_is(s.impassable[i], "")) return PCL_ERR_UNSUPPORTED;
-        if (s.sprite_confined[i] != (i == 0) || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-      }
-      return PCL_OK;
-    }
-    case PCL_PROG_BETTER_SCROLLY: {
-      if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.drape_char, s.n_drapes, "@")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.z_order, 5, "abc@P")) return PCL_ERR_UNSUPPORTED;
-      const int lens[1] = {5};
-      if (!groups_are(s, "abcP@", lens, 1)) return PCL_ERR_UNSUPPORTED;
-      for (int i = 0; i < 4; ++i)
-        if (s.sprite_confined[i] || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    case PCL_PROG_CLASSICS: {
-      if (!chars_are(s.sprite_char, s.n_sprites, "P") || s.n_drapes != 0) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.z_order, 1, "P")) return PCL_ERR_UNSUPPORTED;
-      const int lens[1] = {1};
-      if (!groups_are(s, "P", lens, 1)) return PCL_ERR_UNSUPPORTED;
-      if (s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
-      const int rule = s.program_arg[0];
-      if (rule != PCL_CLASSIC_FOUR_ROOMS && rule != PCL_CLASSIC_CLIFF_WALK &&
-          rule != PCL_CLASSIC_CHAIN_WALK && rule != PCL_CLASSIC_FLUVIAL) return PCL_ERR_INVALID;
-      if (rule == PCL_CLASSIC_FLUVIAL) {
-        // The kernel re-stages the flowing rows before the swimmer moves, which is
-        // only equivalent when the swimmer never looks at the board.
-        if (!set_is(s.impassable[0], "")) return PCL_ERR_UNSUPPORTED;
-        if (s.program_arg[1] < 0 || s.program_arg[2] < s.program_arg[1]) return PCL_ERR_INVALID;
-      }
-      if (s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;   // the tile is staged per env in smem
-      return PCL_OK;
-    }
-    case PCL_PROG_APERTURE: {
-      if (s.n_sprites != 1 || s.n_drapes != 1) return PCL_ERR_UNSUPPORTED;
-      if (s.z_order[0] != s.drape_char[0] || s.z_order[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
-      if (s.n_groups != 2 || s.group_len[0] != 1 || s.group_len[1] != 1 ||
-          s.group_chars[0] != s.sprite_char[0] || s.group_chars[1] != s.drape_char[0])
-        return PCL_ERR_UNSUPPORTED;
-      if (s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
-      if (s.rows >= 32768 || s.cols >= 32768 || s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;
-      return PCL_OK;
-    }
-    case PCL_PROG_HELLO: {
-      if (s.n_sprites < 1 || s.n_sprites > 4 || s.n_drapes != 1) return PCL_ERR_UNSUPPORTED;
-      if (s.n_groups != 1 || s.group_len[0] != s.n_sprites + 1) return PCL_ERR_UNSUPPORTED;
-      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      for (int k = 0; k < s.n_sprites + 1; ++k)      // program_arg = the z-order
-        if (s.program_arg[k] != s.z_order[k]) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    case PCL_PROG_APPREHEND: {
-      if (s.n_sprites != 2 || s.n_drapes != 0) return PCL_ERR_UNSUPPORTED;
-      // one update group: the ball, then the catcher; the catcher is drawn on top
-      if (s.n_groups != 1 || s.group_len[0] != 2 || s.group_chars[0] != s.sprite_char[1] ||
-          s.group_chars[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
-      if (s.z_order[0] != s.sprite_char[1] || s.z_order[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
-      if (!s.sprite_confined[0] || s.sprite_confined[1]) return PCL_ERR_UNSUPPORTED;
-      for (int i = 0; i < 2; ++i) {
-        if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-        for (int w = 0; w < 4; ++w) if (s.impassable[i][w]) return PCL_ERR_UNSUPPORTED;
-      }
-      if (s.rows < 2) return PCL_ERR_INVALID;          // the slope divides by rows - 1
-      return PCL_OK;
-    }
-    case PCL_PROG_SHOCKWAVE: {
-      if (s.n_sprites != 1 || s.n_drapes != 3) return PCL_ERR_UNSUPPORTED;
-      // one update group [' ', '^', P, '@'] (the two static drapes may come in either
-      // order), z-order ' ' '^' '@' P
-      if (s.n_groups != 1 || s.group_len[0] != 4 || s.group_chars[2] != s.sprite_char[0] ||
-          s.group_chars[3] != s.drape_char[0]) return PCL_ERR_UNSUPPORTED;
-      if (s.z_order[0] != s.drape_char[1] || s.z_order[1] != s.drape_char[2] ||
-          s.z_order[2] != s.drape_char[0] || s.z_order[3] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
-      if (!s.sprite_confined[0] || s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
-      if (s.rows > 32 || s.cols > 64) return PCL_ERR_UNSUPPORTED;      // a curtain row per lane, 64-bit rows
-      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      if (s.program_arg[0] < 0 || s.program_arg[0] > 1024) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    case PCL_PROG_ORDEAL: {
-      const int chapter = s.program_arg[0];
-      const int want_s = chapter == PCL_ORDEAL_CASTLE ? 2 : 1, want_d = chapter == PCL_ORDEAL_CAVERN ? 1 : 0;
-      if (chapter != PCL_ORDEAL_CASTLE && chapter != PCL_ORDEAL_CAVERN && chapter != PCL_ORDEAL_KANSAS)
-        return PCL_ERR_INVALID;
-      if (s.n_sprites != want_s || s.n_drapes != want_d) return PCL_ERR_UNSUPPORTED;
-      if (s.n_groups != 1 || s.group_len[0] != want_s + want_d) return PCL_ERR_UNSUPPORTED;
-      if (s.group_chars[0] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;     // the player moves first
-      for (int i = 0; i < want_s; ++i) if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-      if (s.rows >= 32768 || s.cols >= 32768 || s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;
-      if (want_d && s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    case PCL_PROG_T_MAZE: {
-      if (!chars_are(s.sprite_char, s.n_sprites, "P")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.drape_char, s.n_drapes, "Q#*ltr")) return PCL_ERR_UNSUPPORTED;
-      if (!chars_are(s.z_order, 7, "*#ltrQP")) return PCL_ERR_UNSUPPORTED;
-      const int lens[3] = {3, 1, 3};
-      if (!groups_are(s, "Q#*Pltr", lens, 3)) return PCL_ERR_UNSUPPORTED;
-      if (!set_is(s.impassable[0], "#") || s.sprite_confined[0] || !s.sprite_egocentric[0])
-        return PCL_ERR_UNSUPPORTED;
-      for (int d = 1; d < 6; ++d) if (s.margins[d][0] >= 0) return PCL_ERR_UNSUPPORTED;
-      // one board row per lane; the kernel paints 16-byte rows
-      if (s.rows > 32 || s.pitch != 16) return PCL_ERR_UNSUPPORTED;
-      if (s.pattern_rows < s.rows || s.pattern_cols < s.cols || s.pattern_rows >= 32768 ||
-          s.pattern_cols >= 32768) return PCL_ERR_INVALID;
-      if (s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      // the speckle redraw stages the generator and one bit per pattern cell per warp
-      if (s.pattern_rows * s.pattern_cols > 32 * pcl::kTMazeMaxStreamWords) return PCL_ERR_UNSUPPORTED;
-      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      const int level = s.program_arg[0];
-      // TeleporterDrape.__init__ (t_maze.py:415-417): the level's hallway lies inside the pattern
-      if (level < 0 || 11 * level + 9 + 5 > s.pattern_rows) return PCL_ERR_INVALID;
-      if (s.program_arg[1] != 0 && s.program_arg[1] != 1) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    case PCL_PROG_FIXTURE: {
-      // Any MazeWalker / Scrolly / plain-drape mix; entities and z-order must
-      // be consistent permutations of each other.
-      const int n = s.n_sprites + s.n_drapes;
-      if (n < 1) return PCL_ERR_INVALID;
-      int total = 0;
-      for (int g = 0; g < s.n_groups; ++g) total += s.group_len[g];
-      if (s.n_groups < 1 || total != n) return PCL_ERR_INVALID;
-      for (int i = 0; i < n; ++i) {
-        int in_z = 0, in_groups = 0;
-        const uint8_t ch = i < s.n_sprites ? s.sprite_char[i] : s.drape_char[i - s.n_sprites];
-        for (int k = 0; k < n; ++k) {
-          in_z += s.z_order[k] == ch;
-          in_groups += s.group_chars[k] == ch;
-        }
-        if (in_z != 1 || in_groups != 1 || ch == 0 || ch > 127) return PCL_ERR_INVALID;
-      }
-      for (int d = 0; d < s.n_drapes; ++d) {
-        if (!s.drape_kind[d]) continue;
-        if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
-        if (s.pattern_words < (s.pattern_cols + 31) / 32 + 2) return PCL_ERR_INVALID;
-        const int mr = s.margins[d][0], mc = s.margins[d][1];
-        if (mr >= 0 && (mc - 1 >= s.cols - mc || mr - 1 >= s.rows - mr)) return PCL_ERR_INVALID;
-      }
-      if (s.bits_words < (s.cols + 31) / 32 + 1) return PCL_ERR_INVALID;
-      return PCL_OK;
-    }
-    default:
-      return PCL_ERR_UNSUPPORTED;
-  }
+  return prog ? prog->check_spec(s) : PCL_ERR_UNSUPPORTED;
 }
 
 void fill_params(const pcl_handle* h, StepParams* p) {
@@ -332,22 +135,8 @@ void fill_params(const pcl_handle* h, StepParams* p) {
 }
 
 int launch(pcl_handle* h, const StepParams& p, cudaStream_t stream) {
-  cudaError_t e;
-  switch (h->spec.program) {
-    case PCL_PROG_SCROLLY_MAZE: e = pcl::launch_scrolly_maze(p, stream); break;
-    case PCL_PROG_WAREHOUSE: e = pcl::launch_warehouse(p, stream); break;
-    case PCL_PROG_MARAUDERS: e = pcl::launch_marauders(p, stream); break;
-    case PCL_PROG_FIXTURE: e = pcl::launch_fixture(p, stream); break;
-    case PCL_PROG_BETTER_SCROLLY: e = pcl::launch_better_scrolly(p, stream); break;
-    case PCL_PROG_CLASSICS: e = pcl::launch_classics(p, stream); break;
-    case PCL_PROG_APERTURE: e = pcl::launch_aperture(p, stream); break;
-    case PCL_PROG_ORDEAL: e = pcl::launch_ordeal(p, stream); break;
-    case PCL_PROG_HELLO: e = pcl::launch_hello(p, stream); break;
-    case PCL_PROG_APPREHEND: e = pcl::launch_apprehend(p, stream); break;
-    case PCL_PROG_SHOCKWAVE: e = pcl::launch_shockwave(p, stream); break;
-    case PCL_PROG_T_MAZE: e = pcl::launch_t_maze(p, stream); break;
-    default: return PCL_ERR_UNSUPPORTED;
-  }
+  if (!h->program->launch) return PCL_ERR_UNSUPPORTED;
+  const cudaError_t e = h->program->launch(p, stream);
   if (e != cudaSuccess) return cuda_failed(h, e, "step kernel launch");
   h->launches += 1;              // only launches that were accepted count
   return PCL_OK;
@@ -365,14 +154,11 @@ bool outputs_set(const pcl_outputs& out) {
   return out.d_reward && out.d_has_reward && out.d_discount && out.d_done;
 }
 
-// Programs whose rewards are not integers write pcl_outputs.d_reward_f64 instead.
-bool float_rewards(const pcl_handle* h) { return h->spec.program == PCL_PROG_T_MAZE; }
-
 int check_ready(const pcl_handle* h, const pcl_outputs* out) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h) && !out->d_reward_f64) return PCL_ERR_INVALID;
+  if (h->program->float_reward && !out->d_reward_f64) return PCL_ERR_INVALID;
   return PCL_OK;
 }
 
@@ -414,10 +200,11 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   pcl_handle* h = new (std::nothrow) pcl_handle();
   if (!h) return PCL_ERR_NOMEM;
   h->spec = *spec;
+  h->program = program_of(spec->program);
   h->batch = batch;
   h->device = device;
   h->bound = 0;
-  h->actions_per_env = spec->program == PCL_PROG_FIXTURE ? spec->n_sprites + spec->n_drapes + 2 * PCL_FIXTURE_DIRECTIVES : 1;
+  h->actions_per_env = h->program->actions_per_env ? h->program->actions_per_env(*spec) : 1;
   h->launches = 0;
   h->last_error[0] = 0;
   h->host_ready = 0;
@@ -446,40 +233,10 @@ int pcl_bind_state(pcl_handle* h, const pcl_state* st) {
   // A game may have no sprites at all (engine_test.py:578-640 renders one drape).
   if (h->spec.n_sprites > 0 && (!st->d_sprites || !st->d_sprites_init)) return PCL_ERR_INVALID;
   if (h->spec.n_drapes > 0 && (!st->d_drapes || !st->d_drapes_init)) return PCL_ERR_INVALID;
-  if (h->spec.program == PCL_PROG_SCROLLY_MAZE) {
-    for (int d = 0; d < 2; ++d) if (!st->d_pattern[d]) return PCL_ERR_INVALID;
-    if (!st->d_pattern_init[1] || st->pattern_bstride[1] == 0) return PCL_ERR_INVALID;
-  }
-  if (h->spec.program == PCL_PROG_MARAUDERS) {
-    for (int d = 0; d < 2; ++d)
-      if (!st->d_bits[d] || !st->d_bits_init[d] || st->bits_bstride[d] == 0) return PCL_ERR_INVALID;
-    if (!st->d_rng) return PCL_ERR_INVALID;
-  }
-  if (h->spec.program == PCL_PROG_HELLO && !st->d_bits_init[0]) return PCL_ERR_INVALID;
-  if (h->spec.program == PCL_PROG_SHOCKWAVE) {
-    if (!st->d_bits[0] || st->bits_bstride[0] == 0 || !st->d_rng) return PCL_ERR_INVALID;
-    for (int d = 0; d < 3; ++d) if (!st->d_bits_init[d]) return PCL_ERR_INVALID;
-  }
-  if (h->spec.program == PCL_PROG_ORDEAL) {
-    if (h->spec.n_drapes && (!st->d_bits[0] || !st->d_bits_init[0] || st->bits_bstride[0] == 0))
-      return PCL_ERR_INVALID;
-    if (h->spec.n_sprites + h->spec.n_drapes == 2 && (!st->d_z_order || !st->d_z_order_init))
-      return PCL_ERR_INVALID;                   // the kernel reads the z-order of two entities
-  }
-  if (h->spec.program == PCL_PROG_BETTER_SCROLLY) {
-    if (!st->d_bits[0] || !st->d_bits_init[0] || st->bits_bstride[0] == 0) return PCL_ERR_INVALID;
-  }
-  if (h->spec.program == PCL_PROG_T_MAZE) {
-    if (!st->d_bits[0] || !st->d_bits_init[0] || st->bits_bstride[0] == 0) return PCL_ERR_INVALID;
-    for (int d = 1; d < 6; ++d) if (!st->d_pattern[d]) return PCL_ERR_INVALID;
-    if (!st->d_pattern_init[2] || st->pattern_bstride[2] == 0) return PCL_ERR_INVALID;
-  }
   if (h->spec.n_scroll_groups > 1 && (!st->d_groups || !st->d_groups_init)) return PCL_ERR_INVALID;
-  if (h->spec.program == PCL_PROG_FIXTURE) {
-    if (!st->d_z_order || !st->d_z_order_init) return PCL_ERR_INVALID;
-    for (int d = 0; d < h->spec.n_drapes; ++d) {
-      if (h->spec.drape_kind[d] ? !st->d_pattern[d] : !st->d_bits[d]) return PCL_ERR_INVALID;
-    }
+  if (h->program->check_state) {
+    const int r = h->program->check_state(h->spec, *st);
+    if (r != PCL_OK) return r;
   }
   h->st = *st;
   fill_params(h, &h->base);      // the per-step calls only patch mode / actions / outputs
@@ -592,7 +349,7 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
   Range nvtx_range("pcl_step_host");
   const int r = check_ready(h, out);
   if (r != PCL_OK) return r;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
+  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions) return PCL_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t plane = (size_t)h->spec.rows * h->spec.pitch;
@@ -613,7 +370,7 @@ int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_acti
   Range nvtx_range("pcl_step_host_async");
   const int r = check_ready(h, out);
   if (r != PCL_OK) return r;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
+  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions || slot < 0 || slot >= PCL_HOST_SLOTS) return PCL_ERR_INVALID;
   if (crop && !d_crop) return PCL_ERR_INVALID;
   int e = host_pipeline_ready(h);
@@ -676,21 +433,19 @@ namespace {
 // the drape's corner, or bit rows of the board.  Fills d's fields of `p`.
 int resolve_curtain(const pcl_handle* h, int d, pcl::LayersParams* p) {
   const pcl_spec& sp = h->spec;
-  if (sp.program == PCL_PROG_SCROLLY_MAZE || (sp.program == PCL_PROG_FIXTURE && sp.drape_kind[d])) {
+  const pcl::CurtainAt at = h->program->curtain ? h->program->curtain(sp, d) : pcl::CurtainAt::kNone;
+  if (at == pcl::CurtainAt::kPatternWindow || at == pcl::CurtainAt::kStaleWindow) {
     p->scrolly[d] = 1;
     p->bits[d] = h->st.d_pattern[d]; p->bits_bstride[d] = h->st.pattern_bstride[d];
     p->row_words[d] = sp.pattern_words;
-    const bool coins = sp.program == PCL_PROG_SCROLLY_MAZE && d == 1;
+    const bool coins = at == pcl::CurtainAt::kStaleWindow;
     p->stale_slot[d] = coins;
     p->per_level[d] = !coins && h->st.d_level != nullptr;   // read-only patterns: per level
-  } else if (sp.program == PCL_PROG_MARAUDERS || sp.program == PCL_PROG_BETTER_SCROLLY ||
-             sp.program == PCL_PROG_FIXTURE || sp.program == PCL_PROG_ORDEAL ||
-             sp.program == PCL_PROG_SHOCKWAVE || (sp.program == PCL_PROG_T_MAZE && d == 0)) {
+  } else if (at == pcl::CurtainAt::kBits) {
     p->bits[d] = h->st.d_bits[d]; p->bits_bstride[d] = h->st.bits_bstride[d];
     p->row_words[d] = sp.bits_words;
   } else {
-    return PCL_ERR_UNSUPPORTED;    // curtain held implicitly (warehouse 'X', aperture, hello) or
-                                   // a rolled pattern (t_maze's Scrollys)
+    return PCL_ERR_UNSUPPORTED;    // a curtain the layers kernel cannot read
   }
   return p->bits[d] ? PCL_OK : PCL_ERR_INVALID;
 }
@@ -792,7 +547,7 @@ int pcl_attach_cropper(pcl_handle* h, const pcl_crop_spec* crop, uint8_t* d_crop
     return PCL_OK;
   }
   if (!d_crop) return PCL_ERR_INVALID;
-  if (h->spec.program != PCL_PROG_SCROLLY_MAZE) return PCL_ERR_UNSUPPORTED;
+  if (!h->program->crop_epilogue) return PCL_ERR_UNSUPPORTED;
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
   if ((int64_t)crop->rows * crop->cols >= 65536) return PCL_ERR_UNSUPPORTED;
@@ -832,7 +587,7 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   if (!h || !crop || !d_board || !out || !x) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
   if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape tracking: pcl_crop_tracking
@@ -866,7 +621,7 @@ int pcl_pack_handoff(pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
                      const pcl_outputs* out, uint8_t* d_packed, void* stream) {
   if (!h || !d_view || !out || !d_packed || view_bytes <= 0) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;
@@ -882,7 +637,7 @@ int pcl_pack_handoff_peers(pcl_handle* h, const uint8_t* d_view, int32_t view_by
     return PCL_ERR_INVALID;
   if (n_peers < 1 || n_peers > PCL_MAX_PEERS) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;

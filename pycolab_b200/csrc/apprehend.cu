@@ -122,10 +122,29 @@ apprehend_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (s.n_sprites != 2 || s.n_drapes != 0) return PCL_ERR_UNSUPPORTED;
+  // one update group: the ball, then the catcher; the catcher is drawn on top
+  if (s.n_groups != 1 || s.group_len[0] != 2 || s.group_chars[0] != s.sprite_char[1] ||
+      s.group_chars[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
+  if (s.z_order[0] != s.sprite_char[1] || s.z_order[1] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
+  if (!s.sprite_confined[0] || s.sprite_confined[1]) return PCL_ERR_UNSUPPORTED;
+  for (int i = 0; i < 2; ++i) {
+    if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+    for (int w = 0; w < 4; ++w) if (s.impassable[i][w]) return PCL_ERR_UNSUPPORTED;
+  }
+  if (s.rows < 2) return PCL_ERR_INVALID;          // the slope divides by rows - 1
+  return PCL_OK;
+}
 
-cudaError_t launch_apprehend(const StepParams& p, cudaStream_t s) {
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(apprehend_step, p, kWarpsPerBlock, 0, s);
 }
+
+}  // namespace
+
+const Program kApprehend = {check_spec, nullptr, nullptr, launch, nullptr,
+                            /*float_reward=*/false, /*crop_epilogue=*/false,
+                            /*scroll_groups=*/false};
 
 }  // namespace pcl

@@ -208,12 +208,33 @@ better_scrolly_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.drape_char, s.n_drapes, "@")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.z_order, 5, "abc@P")) return PCL_ERR_UNSUPPORTED;
+  const int lens[1] = {5};
+  if (!groups_are(s, "abcP@", lens, 1)) return PCL_ERR_UNSUPPORTED;
+  for (int i = 0; i < 4; ++i)
+    if (s.sprite_confined[i] || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_better_scrolly(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec&, const pcl_state& st) {
+  if (!st.d_bits[0] || !st.d_bits_init[0] || st.bits_bstride[0] == 0) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t bits_bytes = (((size_t)p.H * p.BW * 4) + 15) & ~(size_t)15;
   const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch + bits_bytes) * kWarpsPerBlock;
   return launch_step(better_scrolly_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+const Program kBetterScrolly = {check_spec, check_state, curtain_bits, launch, nullptr,
+                                /*float_reward=*/false, /*crop_epilogue=*/false,
+                                /*scroll_groups=*/false};
 
 }  // namespace pcl

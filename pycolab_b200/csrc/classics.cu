@@ -155,11 +155,34 @@ classics_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (!chars_are(s.sprite_char, s.n_sprites, "P") || s.n_drapes != 0) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.z_order, 1, "P")) return PCL_ERR_UNSUPPORTED;
+  const int lens[1] = {1};
+  if (!groups_are(s, "P", lens, 1)) return PCL_ERR_UNSUPPORTED;
+  if (s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
+  const int rule = s.program_arg[0];
+  if (rule != PCL_CLASSIC_FOUR_ROOMS && rule != PCL_CLASSIC_CLIFF_WALK &&
+      rule != PCL_CLASSIC_CHAIN_WALK && rule != PCL_CLASSIC_FLUVIAL) return PCL_ERR_INVALID;
+  if (rule == PCL_CLASSIC_FLUVIAL) {
+    // The kernel re-stages the flowing rows before the swimmer moves, which is
+    // only equivalent when the swimmer never looks at the board.
+    if (!set_is(s.impassable[0], "")) return PCL_ERR_UNSUPPORTED;
+    if (s.program_arg[1] < 0 || s.program_arg[2] < s.program_arg[1]) return PCL_ERR_INVALID;
+  }
+  if (s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;   // the tile is staged per env in smem
+  return PCL_OK;
+}
 
-cudaError_t launch_classics(const StepParams& p, cudaStream_t s) {
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch) * kWarpsPerBlock;
   return launch_step(classics_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+const Program kClassics = {check_spec, nullptr, nullptr, launch, nullptr,
+                           /*float_reward=*/false, /*crop_epilogue=*/false,
+                           /*scroll_groups=*/false};
 
 }  // namespace pcl

@@ -348,12 +348,61 @@ fixture_step(const StepParams p) {
     reinterpret_cast<uint4*>(g_board)[i] = reinterpret_cast<const uint4*>(c.board)[i];
 }
 
-}  // namespace
+// Any MazeWalker / Scrolly / plain-drape mix; entities and z-order must be consistent
+// permutations of each other.
+int check_spec(const pcl_spec& s) {
+  const int n = s.n_sprites + s.n_drapes;
+  if (n < 1) return PCL_ERR_INVALID;
+  if (s.n_groups < 1 || s.n_groups > kMaxEnt) return PCL_ERR_INVALID;
+  int total = 0;
+  for (int g = 0; g < s.n_groups; ++g) total += s.group_len[g];
+  if (total != n) return PCL_ERR_INVALID;
+  for (int i = 0; i < n; ++i) {
+    int in_z = 0, in_groups = 0;
+    const uint8_t ch = i < s.n_sprites ? s.sprite_char[i] : s.drape_char[i - s.n_sprites];
+    for (int k = 0; k < n; ++k) {
+      in_z += s.z_order[k] == ch;
+      in_groups += s.group_chars[k] == ch;
+    }
+    if (in_z != 1 || in_groups != 1 || ch == 0 || ch > 127) return PCL_ERR_INVALID;
+  }
+  for (int d = 0; d < s.n_drapes; ++d) {
+    if (!s.drape_kind[d]) continue;
+    if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
+    if (s.pattern_words < (s.pattern_cols + 31) / 32 + 2) return PCL_ERR_INVALID;
+    if (!margins_fit(s, d)) return PCL_ERR_INVALID;
+  }
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_fixture(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec& s, const pcl_state& st) {
+  if (!st.d_z_order || !st.d_z_order_init) return PCL_ERR_INVALID;
+  for (int d = 0; d < s.n_drapes; ++d) {
+    if (s.drape_kind[d] ? !st.d_pattern[d] : !st.d_bits[d]) return PCL_ERR_INVALID;
+  }
+  return PCL_OK;
+}
+
+CurtainAt curtain(const pcl_spec& s, int d) {
+  return s.drape_kind[d] ? CurtainAt::kPatternWindow : CurtainAt::kBits;
+}
+
+// A motion code per entity, then the Plot directives.
+int actions_per_env(const pcl_spec& s) {
+  return s.n_sprites + s.n_drapes + 2 * PCL_FIXTURE_DIRECTIVES;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t board_bytes = ((size_t)p.H * p.pitch + 15) & ~(size_t)15;
   const size_t smem = (sizeof(WarpState) + board_bytes) * kWarpsPerBlock;
   return launch_step(fixture_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+const Program kFixture = {check_spec, check_state, curtain, launch, actions_per_env,
+                          /*float_reward=*/false, /*crop_epilogue=*/false,
+                          /*scroll_groups=*/true};
 
 }  // namespace pcl

@@ -118,10 +118,28 @@ hello_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (s.n_sprites < 1 || s.n_sprites > 4 || s.n_drapes != 1) return PCL_ERR_UNSUPPORTED;
+  if (s.n_groups != 1 || s.group_len[0] != s.n_sprites + 1) return PCL_ERR_UNSUPPORTED;
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  for (int k = 0; k < s.n_sprites + 1; ++k)      // program_arg = the z-order
+    if (s.program_arg[k] != s.z_order[k]) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_hello(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec&, const pcl_state& st) {
+  return st.d_bits_init[0] ? PCL_OK : PCL_ERR_INVALID;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(hello_step, p, kWarpsPerBlock, 0, s);
 }
+
+}  // namespace
+
+// The drape's curtain is held implicitly (the reset curtain rolled by AUX0 / AUX1).
+const Program kHello = {check_spec, check_state, nullptr, launch, nullptr,
+                        /*float_reward=*/false, /*crop_epilogue=*/false,
+                        /*scroll_groups=*/false};
 
 }  // namespace pcl

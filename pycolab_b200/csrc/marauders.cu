@@ -286,11 +286,37 @@ marauders_step(const StepParams p) {
   for (int seg = lane; seg < total; seg += 32) dst[seg] = tile4[seg];
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (!chars_are(s.sprite_char, s.n_sprites, "Pabcdyz")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.drape_char, s.n_drapes, "BX")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.z_order, 9, "PBXabcdyz")) return PCL_ERR_UNSUPPORTED;
+  const int lens[1] = {9};
+  if (!groups_are(s, "PBXabcdyz", lens, 1)) return PCL_ERR_UNSUPPORTED;
+  if (s.rows > 32 || s.rows < 11 || s.cols > 64 || s.bits_words < 2)
+    return PCL_ERR_UNSUPPORTED;
+  for (int i = 0; i < 7; ++i) {
+    if (!set_is(s.impassable[i], "")) return PCL_ERR_UNSUPPORTED;
+    if (s.sprite_confined[i] != (i == 0) || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+  }
+  return PCL_OK;
+}
 
-cudaError_t launch_marauders(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec&, const pcl_state& st) {
+  for (int d = 0; d < 2; ++d)
+    if (!st.d_bits[d] || !st.d_bits_init[d] || st.bits_bstride[d] == 0) return PCL_ERR_INVALID;
+  if (!st.d_rng) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (size_t)p.H * p.pitch * kWarpsPerBlock;   // one staged tile per warp
   return launch_step(marauders_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);
 }
+
+}  // namespace
+
+const Program kMarauders = {check_spec, check_state, curtain_bits, launch, nullptr,
+                            /*float_reward=*/false, /*crop_epilogue=*/false,
+                            /*scroll_groups=*/false};
 
 }  // namespace pcl

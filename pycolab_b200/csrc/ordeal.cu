@@ -223,11 +223,37 @@ ordeal_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  const int chapter = s.program_arg[0];
+  const int want_s = chapter == PCL_ORDEAL_CASTLE ? 2 : 1, want_d = chapter == PCL_ORDEAL_CAVERN ? 1 : 0;
+  if (chapter != PCL_ORDEAL_CASTLE && chapter != PCL_ORDEAL_CAVERN && chapter != PCL_ORDEAL_KANSAS)
+    return PCL_ERR_INVALID;
+  if (s.n_sprites != want_s || s.n_drapes != want_d) return PCL_ERR_UNSUPPORTED;
+  if (s.n_groups != 1 || s.group_len[0] != want_s + want_d) return PCL_ERR_UNSUPPORTED;
+  if (s.group_chars[0] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;     // the player moves first
+  for (int i = 0; i < want_s; ++i) if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+  if (s.rows >= 32768 || s.cols >= 32768 || s.rows * s.pitch > 8192) return PCL_ERR_UNSUPPORTED;
+  if (want_d && !bit_rows_fit(s)) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_ordeal(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec& s, const pcl_state& st) {
+  if (s.n_drapes && (!st.d_bits[0] || !st.d_bits_init[0] || st.bits_bstride[0] == 0))
+    return PCL_ERR_INVALID;
+  if (s.n_sprites + s.n_drapes == 2 && (!st.d_z_order || !st.d_z_order_init))
+    return PCL_ERR_INVALID;                   // the kernel reads the z-order of two entities
+  return PCL_OK;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch) * kWarpsPerBlock;
   return launch_step(ordeal_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+const Program kOrdeal = {check_spec, check_state, curtain_bits, launch, nullptr,
+                         /*float_reward=*/false, /*crop_epilogue=*/false,
+                         /*scroll_groups=*/false};
 
 }  // namespace pcl

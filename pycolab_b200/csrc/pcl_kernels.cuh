@@ -1,8 +1,9 @@
-// pcl_kernels.cuh — kernel parameter blocks + launch prototypes.
+// pcl_kernels.cuh — kernel parameter blocks, step-program descriptors, launch prototypes.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/pcl.h"
 
@@ -79,31 +80,63 @@ inline cudaError_t launch_step(void (*kern)(StepParams), const StepParams& p, in
   return cudaGetLastError();
 }
 
-cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s);
-// scrolly_maze_step: uint32 words staged per window row of a W-column board (at least 4:
-// the narrow path stages and reads 4 words per row whatever W is), its dynamic shared
-// memory per block, and the most a block may ask for on the H100 (227 KB per block less
-// the kernel's 2 KB of static selector tables).  pcl_create accepts a spec only if its
-// block fits, so an accepted spec always launches.
-__host__ __device__ constexpr int scrolly_window_words(int W) {
-  return W < 2 ? 4 : 2 * ((63 + W + 63) / 64);
+// Where a drape's curtain lives in the bound state (resolve_curtain, api.cu): nowhere the
+// layers kernel can read (held implicitly by the program), bit rows of the board
+// (d_bits), or a window of its Scrolly pattern (d_pattern) at the drape's corner, whose
+// drape record may name one stale cell (kStaleWindow: AUX0 / AUX1).
+enum class CurtainAt { kNone, kBits, kPatternWindow, kStaleWindow };
+
+// Everything the C boundary needs to know about one step program.  Each program's .cu
+// file defines its descriptor beside its kernel; api.cu maps PCL_PROG_* ids to them.
+struct Program {
+  int (*check_spec)(const pcl_spec&);                      // PCL_OK / _INVALID / _UNSUPPORTED
+  int (*check_state)(const pcl_spec&, const pcl_state&);   // nullptr: only the common records
+  CurtainAt (*curtain)(const pcl_spec&, int drape);        // nullptr: every drape kNone
+  cudaError_t (*launch)(const StepParams&, cudaStream_t);  // nullptr: nothing to step
+  int (*actions_per_env)(const pcl_spec&);                 // nullptr: 1
+  bool float_reward;             // rewards go to pcl_outputs.d_reward_f64, not d_reward
+  bool crop_epilogue;            // the step kernel runs an attached cropper (pcl_attach_cropper)
+  bool scroll_groups;            // accepts more than one scrolling group
+};
+extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
+    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze;
+
+// Host-side helpers of the programs' check_spec.
+inline bool chars_are(const uint8_t* got, int n, const char* want) {
+  if ((int)strlen(want) != n) return false;
+  for (int i = 0; i < n; ++i) if (got[i] != (uint8_t)want[i]) return false;
+  return true;
 }
-size_t scrolly_maze_block_smem(int H, int W, int pitch);
-constexpr size_t kScrollyMazeMaxSmem = 227 * 1024 - 2048;
-cudaError_t launch_warehouse(const StepParams& p, cudaStream_t s);
-cudaError_t launch_marauders(const StepParams& p, cudaStream_t s);
-cudaError_t launch_fixture(const StepParams& p, cudaStream_t s);
-cudaError_t launch_better_scrolly(const StepParams& p, cudaStream_t s);
-cudaError_t launch_classics(const StepParams& p, cudaStream_t s);
-cudaError_t launch_aperture(const StepParams& p, cudaStream_t s);
-cudaError_t launch_ordeal(const StepParams& p, cudaStream_t s);
-cudaError_t launch_hello(const StepParams& p, cudaStream_t s);
-cudaError_t launch_apprehend(const StepParams& p, cudaStream_t s);
-cudaError_t launch_shockwave(const StepParams& p, cudaStream_t s);
-cudaError_t launch_t_maze(const StepParams& p, cudaStream_t s);
-// t_maze_step redraws the speckle field into a per-warp bit stream of this many words
-// (one bit per pattern cell); pcl_create refuses larger patterns.
-constexpr int kTMazeMaxStreamWords = 480;
+
+// The set `want` as a 128-bit ASCII mask equals `got`?
+inline bool set_is(const uint32_t (&got)[4], const char* want) {
+  uint32_t m[4] = {0, 0, 0, 0};
+  for (const char* c = want; *c; ++c) m[(*c >> 5) & 3] |= 1u << (*c & 31);
+  return m[0] == got[0] && m[1] == got[1] && m[2] == got[2] && m[3] == got[3];
+}
+
+inline int groups_are(const pcl_spec& s, const char* flat, const int* lens, int n) {
+  if (s.n_groups != n) return 0;
+  int k = 0;
+  for (int g = 0; g < n; ++g) {
+    if (s.group_len[g] != lens[g]) return 0;
+    for (int i = 0; i < lens[g]; ++i, ++k)
+      if (s.group_chars[k] != (uint8_t)flat[k]) return 0;
+  }
+  return 1;
+}
+
+// bits_words holds a bit-packed board row (d_bits) and one word more.
+inline bool bit_rows_fit(const pcl_spec& s) { return s.bits_words >= (s.cols + 31) / 32 + 1; }
+
+// Scrolly d's margins (-1 = None) overlap no more than half of the board (drapes.py:350-364).
+inline bool margins_fit(const pcl_spec& s, int d) {
+  const int mr = s.margins[d][0], mc = s.margins[d][1];
+  return !(mr >= 0 && (mc - 1 >= s.cols - mc || mr - 1 >= s.rows - mr));
+}
+
+// Program::curtain of programs that keep every drape in d_bits.
+inline CurtainAt curtain_bits(const pcl_spec&, int) { return CurtainAt::kBits; }
 
 struct RenderParams {
   int B, H, W, pitch, S, D;
@@ -124,7 +157,8 @@ struct LayersParams {
   uint8_t chars[PCL_MAX_LAYER_CHARS];
   int8_t sprite_of[PCL_MAX_LAYER_CHARS];   // sprite index painting that char, or -1
   int8_t drape_of[PCL_MAX_LAYER_CHARS];    // drape index painting that char, or -1
-  // per drape: where its curtain lives in the packed state (resolve_curtain, api.cu)
+  // per drape: where its curtain lives in the packed state, as the program's
+  // Program::curtain says (resolve_curtain, api.cu)
   const uint32_t* bits[PCL_MAX_DRAPES]; int64_t bits_bstride[PCL_MAX_DRAPES];
   int row_words[PCL_MAX_DRAPES];           // uint32 words per bit row
   int scrolly[PCL_MAX_DRAPES];             // 1: window of a pattern at the drape's corner

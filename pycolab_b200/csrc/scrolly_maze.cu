@@ -102,8 +102,10 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
 // 63 + W bits.  4 words (two 8-byte cp.async, one 16-byte slot) up to W = 64, 6 or 8
 // beyond (drapes.py:293-376 puts no limit on the board width).  The narrow path always
 // stages and reads 4 words per row, so a one-column board is floored at 4 too (at
-// W = 1, 63 + W bits fit in 2 words).  pcl_create checks pattern_words by the same rule.
-__host__ __device__ constexpr int window_words(int W) { return scrolly_window_words(W); }
+// W = 1, 63 + W bits fit in 2 words).  check_spec checks pattern_words by the same rule.
+__host__ __device__ constexpr int window_words(int W) {
+  return W < 2 ? 4 : 2 * ((63 + W + 63) / 64);
+}
 
 // The 4-word fast paths of staging and segment building: a board row is at most 4
 // segments (pitch >= W, so W <= 64 too).
@@ -179,14 +181,19 @@ __device__ __forceinline__ void stamp(int k, uint32_t v) {
 #define PCL_STAMP_TIME(k) do {} while (0)
 #endif
 
+// The most dynamic shared memory a block may ask for on the H100: 227 KB per block less
+// the kernel's 2 KB of static selector tables.  check_spec accepts a spec only if its
+// block fits, so an accepted spec always launches.
+constexpr size_t kMaxBlockSmem = 227 * 1024 - 2048;
+
 // 8 blocks per SM (__launch_bounds__ below) on a 64x64 board: a block's dynamic shared
 // memory, its per-warp selector tables and the 1 KB the SM reserves per block fit 8 times
 // in the H100's 228 KB.
 static_assert(8 * (kWarpsPerBlock * (warp_smem_bytes(64, 64, 64) + sizeof(SelTable)) + 1024) <=
                   228 * 1024,
               "a 64x64 scrolly_maze block no longer fits 8 times per SM");
-static_assert(kScrollyMazeMaxSmem + kWarpsPerBlock * sizeof(SelTable) == 227 * 1024,
-              "kScrollyMazeMaxSmem must leave room for the static selector tables");
+static_assert(kMaxBlockSmem + kWarpsPerBlock * sizeof(SelTable) == 227 * 1024,
+              "kMaxBlockSmem must leave room for the static selector tables");
 
 // 3x3 "blocked" mask (bit (dr+1)*3 + dc+1, sprites.py:495-507) around the virtual
 // position (vrow, vcol) of a walker whose 5x5 wall patch `field` is centred on
@@ -733,20 +740,62 @@ scrolly_maze_step(const StepParams p) {
   PCL_STAMP_TIME(kStTimeOut);
 }
 
-}  // namespace
-
-size_t scrolly_maze_block_smem(int H, int W, int pitch) {
+// Dynamic shared memory of one block (kWarpsPerBlock envs).
+size_t block_smem(int H, int W, int pitch) {
   return warp_smem_bytes(H, W, pitch) * kWarpsPerBlock;
 }
 
-cudaError_t launch_scrolly_maze(const StepParams& p, cudaStream_t s) {
+int check_spec(const pcl_spec& s) {
+  if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.drape_char, s.n_drapes, "#@")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.z_order, 6, "abc@#P")) return PCL_ERR_UNSUPPORTED;
+  const int lens[3] = {1, 4, 1};
+  if (!groups_are(s, "#abcP@", lens, 3)) return PCL_ERR_UNSUPPORTED;
+  for (int i = 0; i < 4; ++i) {
+    if (!set_is(s.impassable[i], "#")) return PCL_ERR_UNSUPPORTED;
+    if (s.sprite_confined[i]) return PCL_ERR_UNSUPPORTED;
+    if (s.sprite_egocentric[i] != (i == 0)) return PCL_ERR_UNSUPPORTED;
+  }
+  if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
+  {
+    // Window rows are staged from the even word at or below corner_c >> 5:
+    // window_words(W) words (4 up to 64 columns) must stay inside the row.
+    const int nw = window_words(s.cols);
+    if ((s.pattern_words & 1) || s.pattern_words < (((s.pattern_cols - s.cols) >> 5) & ~1) + nw ||
+        s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
+    // one CTA (4 envs) stages tile + windows in shared memory: the launcher's own size
+    if (block_smem(s.rows, s.cols, s.pitch) > kMaxBlockSmem) return PCL_ERR_UNSUPPORTED;
+  }
+  for (int d = 0; d < 2; ++d)
+    if (!margins_fit(s, d)) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+int check_state(const pcl_spec&, const pcl_state& st) {
+  for (int d = 0; d < 2; ++d) if (!st.d_pattern[d]) return PCL_ERR_INVALID;
+  if (!st.d_pattern_init[1] || st.pattern_bstride[1] == 0) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+// '#' is a window of its pattern; '@' too, less the coin its record names as stale.
+CurtainAt curtain(const pcl_spec&, int d) {
+  return d == 1 ? CurtainAt::kStaleWindow : CurtainAt::kPatternWindow;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   if (p.PWW & 1) return cudaErrorInvalidValue;   // window rows are staged in 8-byte halves
-  const size_t smem = scrolly_maze_block_smem(p.H, p.W, p.pitch);
-  if (smem > kScrollyMazeMaxSmem) return cudaErrorInvalidValue;   // board too large for one CTA
+  const size_t smem = block_smem(p.H, p.W, p.pitch);
+  if (smem > kMaxBlockSmem) return cudaErrorInvalidValue;   // board too large for one CTA
   // Programmatic dependent launch: this kernel may start (prologue only) before
   // the previous kernel of the stream has drained.
   return launch_step(scrolly_maze_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);
 }
+
+}  // namespace
+
+const Program kScrollyMaze = {check_spec, check_state, curtain, launch, nullptr,
+                              /*float_reward=*/false, /*crop_epilogue=*/true,
+                              /*scroll_groups=*/false};
 
 }  // namespace pcl
 

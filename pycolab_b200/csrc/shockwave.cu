@@ -152,10 +152,35 @@ shockwave_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (s.n_sprites != 1 || s.n_drapes != 3) return PCL_ERR_UNSUPPORTED;
+  // one update group [' ', '^', P, '@'] (the two static drapes may come in either
+  // order), z-order ' ' '^' '@' P
+  if (s.n_groups != 1 || s.group_len[0] != 4 || s.group_chars[2] != s.sprite_char[0] ||
+      s.group_chars[3] != s.drape_char[0]) return PCL_ERR_UNSUPPORTED;
+  if (s.z_order[0] != s.drape_char[1] || s.z_order[1] != s.drape_char[2] ||
+      s.z_order[2] != s.drape_char[0] || s.z_order[3] != s.sprite_char[0]) return PCL_ERR_UNSUPPORTED;
+  if (!s.sprite_confined[0] || s.sprite_egocentric[0]) return PCL_ERR_UNSUPPORTED;
+  if (s.rows > 32 || s.cols > 64) return PCL_ERR_UNSUPPORTED;      // a curtain row per lane, 64-bit rows
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  if (s.program_arg[0] < 0 || s.program_arg[0] > 1024) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_shockwave(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec&, const pcl_state& st) {
+  if (!st.d_bits[0] || st.bits_bstride[0] == 0 || !st.d_rng) return PCL_ERR_INVALID;
+  for (int d = 0; d < 3; ++d) if (!st.d_bits_init[d]) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(shockwave_step, p, kWarpsPerBlock, 0, s);
 }
+
+}  // namespace
+
+const Program kShockwave = {check_spec, check_state, curtain_bits, launch, nullptr,
+                            /*float_reward=*/false, /*crop_epilogue=*/false,
+                            /*scroll_groups=*/false};
 
 }  // namespace pcl

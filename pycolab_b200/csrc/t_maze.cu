@@ -42,10 +42,13 @@ namespace {
 constexpr int kWarpsPerBlock = 4;
 enum { DQ = 0, DWALL = 1, DDIRT = 2, DLEFT = 3, DTELE = 4, DRIGHT = 5, ND = 6 };
 constexpr int kLimboRow = 4, kLimboCol = 140, kLimboDx = -46;   // TeleporterDrape :408-415
+// The speckle redraw writes a per-warp bit stream of this many words (one bit per pattern
+// cell); check_spec refuses larger patterns.
+constexpr int kMaxStreamWords = 480;
 
 struct WarpScratch {
   uint32_t mt[PCL_MT_WORDS + 3];
-  uint32_t stream[kTMazeMaxStreamWords + 2];
+  uint32_t stream[kMaxStreamWords + 2];
 };
 
 __device__ __forceinline__ uint32_t temper(uint32_t y) {
@@ -365,10 +368,51 @@ t_maze_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  if (!chars_are(s.sprite_char, s.n_sprites, "P")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.drape_char, s.n_drapes, "Q#*ltr")) return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.z_order, 7, "*#ltrQP")) return PCL_ERR_UNSUPPORTED;
+  const int lens[3] = {3, 1, 3};
+  if (!groups_are(s, "Q#*Pltr", lens, 3)) return PCL_ERR_UNSUPPORTED;
+  if (!set_is(s.impassable[0], "#") || s.sprite_confined[0] || !s.sprite_egocentric[0])
+    return PCL_ERR_UNSUPPORTED;
+  for (int d = 1; d < 6; ++d) if (s.margins[d][0] >= 0) return PCL_ERR_UNSUPPORTED;
+  // one board row per lane; the kernel paints 16-byte rows
+  if (s.rows > 32 || s.pitch != 16) return PCL_ERR_UNSUPPORTED;
+  if (s.pattern_rows < s.rows || s.pattern_cols < s.cols || s.pattern_rows >= 32768 ||
+      s.pattern_cols >= 32768) return PCL_ERR_INVALID;
+  if (s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
+  // the speckle redraw stages the generator and one bit per pattern cell per warp
+  if (s.pattern_rows * s.pattern_cols > 32 * kMaxStreamWords) return PCL_ERR_UNSUPPORTED;
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  const int level = s.program_arg[0];
+  // TeleporterDrape.__init__ (t_maze.py:415-417): the level's hallway lies inside the pattern
+  if (level < 0 || 11 * level + 9 + 5 > s.pattern_rows) return PCL_ERR_INVALID;
+  if (s.program_arg[1] != 0 && s.program_arg[1] != 1) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
 
-cudaError_t launch_t_maze(const StepParams& p, cudaStream_t s) {
+int check_state(const pcl_spec&, const pcl_state& st) {
+  if (!st.d_bits[0] || !st.d_bits_init[0] || st.bits_bstride[0] == 0) return PCL_ERR_INVALID;
+  for (int d = 1; d < 6; ++d) if (!st.d_pattern[d]) return PCL_ERR_INVALID;
+  if (!st.d_pattern_init[2] || st.pattern_bstride[2] == 0) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+// 'Q' is a plain drape; the Scrollys' patterns are rolled, which the layers kernel does
+// not follow.
+CurtainAt curtain(const pcl_spec&, int d) {
+  return d == DQ ? CurtainAt::kBits : CurtainAt::kNone;
+}
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(t_maze_step, p, kWarpsPerBlock, 0, s);
 }
+
+}  // namespace
+
+const Program kTMaze = {check_spec, check_state, curtain, launch, nullptr,
+                        /*float_reward=*/true, /*crop_epilogue=*/false,
+                        /*scroll_groups=*/false};
 
 }  // namespace pcl

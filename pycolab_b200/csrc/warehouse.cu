@@ -235,11 +235,39 @@ warehouse_step(const StepParams p) {
   }
 }
 
-}  // namespace
+int check_spec(const pcl_spec& s) {
+  const int nb = s.n_sprites - 1;
+  if (nb < 1 || nb > 10) return PCL_ERR_UNSUPPORTED;
+  if (s.sprite_char[nb] != 'P') return PCL_ERR_UNSUPPORTED;
+  if (!chars_are(s.drape_char, s.n_drapes, "X")) return PCL_ERR_UNSUPPORTED;
+  const char* order = "1234567890";
+  int k = 0;
+  for (int i = 0; i < nb; ++i) {
+    while (order[k] && order[k] != (char)s.sprite_char[i]) ++k;
+    if (!order[k]) return PCL_ERR_UNSUPPORTED;
+    ++k;
+    if (s.z_order[i] != s.sprite_char[i]) return PCL_ERR_UNSUPPORTED;
+    if (s.sprite_confined[i] || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+  }
+  if (s.z_order[nb] != 'X' || s.z_order[nb + 1] != 'P') return PCL_ERR_UNSUPPORTED;
+  if (s.n_groups != 3 || s.group_len[0] != nb || s.group_len[1] != 1 || s.group_len[2] != 1)
+    return PCL_ERR_UNSUPPORTED;
+  for (int i = 0; i < nb; ++i)
+    if (s.group_chars[i] != s.sprite_char[i]) return PCL_ERR_UNSUPPORTED;
+  if (s.group_chars[nb] != 'X' || s.group_chars[nb + 1] != 'P') return PCL_ERR_UNSUPPORTED;
+  return PCL_OK;
+}
 
-cudaError_t launch_warehouse(const StepParams& p, cudaStream_t s) {
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch) * kWarpsPerBlock;
   return launch_step(warehouse_step, p, kWarpsPerBlock, smem, s);
 }
+
+}  // namespace
+
+// 'X' is held implicitly by the boxes: no curtain to resolve.
+const Program kWarehouse = {check_spec, nullptr, nullptr, launch, nullptr,
+                            /*float_reward=*/false, /*crop_epilogue=*/false,
+                            /*scroll_groups=*/false};
 
 }  // namespace pcl

@@ -111,7 +111,7 @@ def oracle_world(maze, board, beneath, margins=DEFAULT_MARGINS):
 # ----------------------------------------------- the kernel's shared-memory layout
 
 # Mirrors scrolly_maze.cu (window_words, narrow_board, warp_smem_bytes) and the
-# pattern_words rule of pcl_create (api.cu validate).
+# pattern_words rule of its check_spec, which pcl_create applies.
 REC_WORDS = 64
 WARPS_PER_BLOCK = 4
 SEL_TABLE_BYTES = 512                  # one u16[256] selector table per warp (static)
