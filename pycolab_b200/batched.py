@@ -9,6 +9,7 @@ C ABI (`pcl_step`); there is no CPU path.
 """
 
 import ctypes as C
+import random
 
 import numpy as np
 
@@ -19,6 +20,15 @@ from pycolab_b200 import lowering
 def _torch():
   import torch
   return torch
+
+
+def _mt_state(stream, seed):
+  """u32 [625]: the MT19937 words (624 key words + position) of a generator seeded with
+  `seed`: Python's random.Random ('python') or NumPy's RandomState ('numpy')."""
+  if stream == 'python':
+    return np.array(random.Random(seed).getstate()[1], dtype=np.uint32)
+  _, key, pos, _, _ = np.random.RandomState(seed).get_state()
+  return np.append(key, pos).astype(np.uint32)
 
 
 class StepResult(object):
@@ -153,37 +163,15 @@ class BatchedEngine(object):
       self._groups_init = tiled([g.group_records for g in games], np.int32)
       st.d_groups, st.d_groups_init = self.groups.data_ptr(), self._groups_init.data_ptr()
       st.groups_init_bstride = bstride(self._groups_init)
-    self.actions_per_env = (len(g0.sprite_chars) + len(g0.drape_chars) +
-                            2 * _lib.FIXTURE_DIRECTIVES
-                            if g0.program == _lib.PROG_FIXTURE else 1)
+    self.actions_per_env = g0.actions_per_env
     self.rng = None
     if draws:
-      slots = 2 if g0.rng_kind == 't_maze' else 1
       if rng_states is not None:
-        states = np.ascontiguousarray(rng_states, dtype=np.uint32).reshape(B, slots * _lib.MT_WORDS)
-      elif g0.rng_kind == 't_maze':
-        # t_maze.py:262 and :365: slot 0 = random.Random(seed) words (the cue side), slot 1 =
-        # RandomState(seed) words (the speckle field)
-        import random as _random
-        states = np.empty((B, 2, _lib.MT_WORDS), dtype=np.uint32)
-        for e in range(B):
-          states[e, 0] = _random.Random(rng_seed + env_offset + e).getstate()[1]
-          _, key, pos, _, _ = np.random.RandomState(rng_seed + env_offset + e).get_state()
-          states[e, 1, :624] = key
-          states[e, 1, 624] = pos
-        states = states.reshape(B, 2 * _lib.MT_WORDS)
-      elif getattr(g0, 'rng_kind', 'numpy') == 'python':
-        # Python's `random` (apprehend.py:103): the 625 words of Random(seed).getstate()
-        import random as _random
-        states = np.empty((B, _lib.MT_WORDS), dtype=np.uint32)
-        for e in range(B):
-          states[e] = _random.Random(rng_seed + env_offset + e).getstate()[1]
+        states = np.ascontiguousarray(rng_states, dtype=np.uint32).reshape(
+            B, len(g0.rng_streams) * _lib.MT_WORDS)
       else:
-        states = np.empty((B, _lib.MT_WORDS), dtype=np.uint32)
-        for e in range(B):
-          _, key, pos, _, _ = np.random.RandomState(rng_seed + env_offset + e).get_state()
-          states[e, :624] = key
-          states[e, 624] = pos
+        states = np.stack([np.concatenate([_mt_state(stream, rng_seed + env_offset + e)
+                                           for stream in g0.rng_streams]) for e in range(B)])
       self.rng = torch.from_numpy(states.view(np.int32)).to(dev)
       st.d_rng = self.rng.data_ptr()
     self._state = st
@@ -323,7 +311,7 @@ class BatchedEngine(object):
       shape = (self.batch, self.rows, self.pitch)
     else:
       shape = (self.batch, crop_spec.rows, crop_spec.cols)
-      att = getattr(self, '_attached', None)
+      att = self._attached
       if (att is not None and att[3] and bytes(att[0]) == bytes(crop_spec) and
           (crop_state is None or crop_state.data_ptr() == att[1].data_ptr())):
         # this very cropper runs inside the step kernel: ship its view, launch nothing more
@@ -359,72 +347,33 @@ class BatchedEngine(object):
 
   def _curtain_bytes(self, d):
     """Curtain of drape `d` as u8 [B, rows, pitch] (the pcl_export_curtain layout)."""
-    torch = _torch()
-    out = torch.empty((self.batch, self.rows, self.pitch), dtype=torch.uint8,
-                      device=self.device)
-    if self.game.program == _lib.PROG_WAREHOUSE:
-      # JudgeDrape curtain = cells of boxes currently drawn as 'X'.
-      out.zero_()
-      nb = len(self.sprite_chars) - 1
-      rec = self.sprites[:, :nb]
-      on = rec[:, :, _lib.S_AUX0] != 0
-      b, s = torch.nonzero(on, as_tuple=True)
-      out[b, rec[b, s, _lib.S_ROW].long(), rec[b, s, _lib.S_COL].long()] = 1
-    elif self.game.program == _lib.PROG_HELLO:
-      # RollingDrape: the reset curtain shifted by the record's (AUX0, AUX1) counters.
-      from pycolab_b200 import lowering
-      if getattr(self, '_roll_base', None) is None:
-        init = self._keep_bits_init[d].cpu().numpy().view(np.uint32)
-        base = np.stack([lowering.unpack_rows(lvl, self.cols) for lvl in init])
-        self._roll_base = torch.from_numpy(base.astype(np.uint8)).to(self.device)
-      lvl = (self.level.long() if self.level is not None
-             else torch.zeros(self.batch, dtype=torch.long, device=self.device))
-      if self._roll_base.shape[0] == self.batch and self.level is None and self.batch > 1:
-        lvl = torch.arange(self.batch, device=self.device)
-      rr = (torch.arange(self.rows, device=self.device)[None, :] -
-            self.drapes[:, d, _lib.D_AUX0].long()[:, None]) % self.rows
-      cc = (torch.arange(self.cols, device=self.device)[None, :] -
-            self.drapes[:, d, _lib.D_AUX1].long()[:, None]) % self.cols
-      out.zero_()
-      out[:, :, :self.cols] = self._roll_base[lvl[:, None, None], rr[:, :, None], cc[:, None, :]]
-    elif self.game.program == _lib.PROG_T_MAZE and d > 0:
-      out.zero_()
-      out[:, :, :self.cols] = self._t_maze_window(d)
-    elif self.game.program == _lib.PROG_APERTURE:
-      # ApertureDrape curtain = the (at most two) cells of its `_apertures` list.
-      out.zero_()
-      for word in (_lib.D_AUX0, _lib.D_AUX1):
-        cell = self.drapes[:, d, word]
-        b = torch.nonzero(cell >= 0, as_tuple=True)[0]
-        out[b, (cell[b] >> 16).long(), (cell[b] & 0xffff).long()] = 1
-    else:
-      _lib.check(self._lib.pcl_export_curtain(self._h, d, out.data_ptr(), self._stream()),
-                 'pcl_export_curtain', self._h)
+    if self.game.curtain is not None:
+      out = self.game.curtain(self, d)
+      if out is not None:
+        return out
+    out = _torch().empty((self.batch, self.rows, self.pitch), dtype=_torch().uint8,
+                         device=self.device)
+    _lib.check(self._lib.pcl_export_curtain(self._h, d, out.data_ptr(), self._stream()),
+               'pcl_export_curtain', self._h)
     return out
 
-  def _t_maze_window(self, d):
-    """Curtain of t_maze Scrolly `d` as u8 [B, rows, cols]: the board window at the drape's
-    corner onto its pattern rolled by the record's AUX0 (rows << 16 | cols); the teleporter is
-    empty while its delay (AUX1) lasts (t_maze.py:397-428)."""
+  def level_rows(self, t):
+    """i64 [B]: the row of each env in `t`, whose leading axis has one row for all envs,
+    one per level or one per env."""
     torch = _torch()
-    ph, pw = self.game.pattern_rows, self.game.pattern_cols
-    rec = self.drapes[:, d].long()
-    roll = rec[:, _lib.D_AUX0]
-    rr = (torch.arange(self.rows, device=self.device)[None, :] + rec[:, _lib.D_CORNER_R, None] +
-          (roll >> 16)[:, None]) % ph
-    cc = (torch.arange(self.cols, device=self.device)[None, :] + rec[:, _lib.D_CORNER_C, None] +
-          (roll & 0xffff)[:, None]) % pw
-    pat = self.patterns[d]
-    if pat.shape[0] != self.batch:
-      lvl = (self.level.long() if self.level is not None
-             else torch.zeros(self.batch, dtype=torch.long, device=self.device))
-    else:
-      lvl = torch.arange(self.batch, device=self.device)
-    words = pat[lvl[:, None, None], rr[:, :, None], (cc >> 5)[:, None, :]]
-    bits = ((words >> (cc & 31)[:, None, :].int()) & 1).to(torch.uint8)
-    if self.drape_chars[d] == 't':
-      bits = bits * (rec[:, _lib.D_AUX1] <= 0).to(torch.uint8)[:, None, None]
-    return bits
+    if t.shape[0] == self.batch:
+      return torch.arange(self.batch, device=self.device)
+    if t.shape[0] == 1:
+      return torch.zeros(self.batch, dtype=torch.long, device=self.device)
+    return self.level.long()
+
+  def packed_bits(self, packed, rows, cols):
+    """u8 [B, R, C]: cell (rows[e, i], cols[e, j]) of env e's bit rows in `packed` (i32
+    [1 | n_levels | B, H, words], cell c is bit c&31 of word c>>5 as `lowering.pack_rows`
+    lays it out); rows: i64 [B, R], cols: i64 [B, C]."""
+    words = packed[self.level_rows(packed)[:, None, None], rows[:, :, None],
+                   (cols >> 5)[:, None, :]]
+    return ((words >> (cols & 31)[:, None, :].int()) & 1).to(_torch().uint8)
 
   def unoccluded_layers(self, chars=None):
     """Layers of `BaseUnoccludedObservationRenderer` (rendering.py:187-301) for
@@ -433,21 +382,8 @@ class BatchedEngine(object):
     game, sorted (`self.chars`).  One kernel over the packed device state."""
     torch = _torch()
     chars = self.chars if chars is None else ''.join(chars)
-    if self.game.program == _lib.PROG_T_MAZE:
-      # rolled Scrolly patterns: each layer is the backdrop's cells plus its owner's curtain
-      planes = []
-      for ch in chars:
-        lvl = (self.level.long() if self.level is not None
-               else torch.zeros(self.batch, dtype=torch.long, device=self.device))
-        plane = self.backdrop[lvl, :, :self.cols].eq(ord(ch))
-        if ch in self.drape_chars:
-          plane |= self.curtain(ch)
-        elif ch in self.sprite_chars:
-          rec = self.sprites[:, self.sprite_chars.index(ch)].long()
-          b = torch.nonzero(rec[:, _lib.S_FLAGS] & 1, as_tuple=True)[0]
-          plane[b, rec[b, _lib.S_ROW], rec[b, _lib.S_COL]] = True
-        planes.append(plane)
-      return torch.stack(planes, dim=1)
+    if self.game.layers is not None:
+      return self.game.layers(self, chars)
     out = torch.empty((self.batch, len(chars), self.rows, self.pitch), dtype=torch.uint8,
                       device=self.device)
     _lib.check(self._lib.pcl_layers(self._h, chars.encode('ascii'), len(chars), out.data_ptr(),
@@ -497,7 +433,7 @@ class BatchedEngine(object):
     return out
 
   def _after_step(self):
-    att = getattr(self, '_attached', None)
+    att = self._attached
     if att is not None and not att[3]:
       self.crop(att[0], state=att[1], out=att[2])
 

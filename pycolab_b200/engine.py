@@ -14,6 +14,7 @@ import collections
 import numpy as np
 
 from pycolab_b200 import _lib
+from pycolab_b200 import lowering
 from pycolab_b200 import plot
 from pycolab_b200 import rendering
 from pycolab_b200 import things
@@ -35,7 +36,6 @@ class Engine(object):
     self._current_update_group = ''
     self._board = None
     self._batched = None
-    self._backdrop_template = None   # initial curtain of a Backdrop the device animates
     self._drape_prefills = {}        # char -> the curtain a drape was built with, before its
                                      # constructor edited it (t_maze.py:263-266 halves the cue)
 
@@ -121,7 +121,6 @@ class Engine(object):
     if self._backdrop is None:
       raise RuntimeError('its_showtime() called before a Backdrop was supplied')
     from pycolab_b200 import batched
-    from pycolab_b200 import lowering
     lowered = lowering.lower(self)          # NotLoweredError if not accelerable
     # Upstream folds directives issued BEFORE its_showtime() into frame 0
     # (engine.py:761-847 runs on whatever the Plot holds).  The device's frame 0 starts
@@ -134,7 +133,7 @@ class Engine(object):
                             'terminate_episode, change_default_discount, change_z_order) are '
                             'not carried into the device\'s first frame')
     rng_states = None
-    if lowered.needs_rng and lowered.rng_kind in ('python', 't_maze'):
+    if 'python' in lowered.rng_streams:
       # apprehend.py:103 draws in the sprite's constructor, which has already run
       # (from the global `random`, as upstream): the device takes the drawn value
       # from the template and needs no generator for this one episode.
@@ -161,28 +160,10 @@ class Engine(object):
     if self._game_over:
       raise RuntimeError('play() was called after the episode handled by this Engine '
                          'has terminated.')
-    if self._batched.game.program == _lib.PROG_FIXTURE:
-      return self._wrap(self._batched.play([self._fixture_row(actions)]))
+    if self._batched.game.action_row is not None:
+      return self._wrap(self._batched.play([self._batched.game.action_row(self, actions)]))
     action = _lib.ACTION_NONE if actions is None else int(actions)
     return self._wrap(self._batched.play([action]))
-
-  _MOTION_NAMES = ('n', 'ne', 'e', 'se', 's', 'sw', 'w', 'nw')
-
-  def _fixture_row(self, actions):
-    """General-program action row from the fixture conventions
-    (tests/test_things.py:219-250): a direction string for everybody, or
-    {char: direction}; unknown / missing = stay.  Directive keys '_reward',
-    '_terminate', '_z' — or '_directives', an ordered list of Plot calls such as
-    ('terminate_episode', 0.5) — stand in for post_update code injection."""
-    from pycolab_b200.games import fixtures
-    code = lambda d: self._MOTION_NAMES.index(d) if d in self._MOTION_NAMES else 8
-    order = ''.join(self._batched.game.groups)
-    if isinstance(actions, dict):
-      motions = {ch: code(actions.get(ch)) for ch in order}
-      return fixtures.action_rows(self._batched.game, motions, actions.get('_reward'),
-                                  bool(actions.get('_terminate')), actions.get('_z'),
-                                  directives=actions.get('_directives'))
-    return fixtures.action_rows(self._batched.game, {ch: code(actions) for ch in order})
 
   def _wrap(self, result):
     import torch
@@ -228,14 +209,6 @@ class Engine(object):
     sprites = b.sprites[0].cpu().numpy()
     drapes = b.drapes[0].cpu().numpy()
     self._the_plot._frame = int(b.plot[0, _lib.P_FRAME])
-    if b.game.sync_plot is not None:       # dict entries the game keeps on the device
-      b.game.sync_plot(self, b.plot[0].cpu().numpy())
-    if b.game.backdrop_role == 'river':    # RiverBackdrop.update as a rotation count
-      if self._backdrop_template is None:
-        self._backdrop_template = self._backdrop.curtain.copy()
-      r0, r1 = b.game.program_arg[1], b.game.program_arg[2]
-      self._backdrop.curtain[r0:r1] = np.roll(self._backdrop_template[r0:r1],
-                                              -int(b.plot[0, _lib.P_AUX0]), axis=1)
     if b.z_order is not None:             # Plot.change_z_order happened on the device
       order = [chr(c) for c in b.z_order[0].cpu().numpy()]
       self._sprites_and_drapes = collections.OrderedDict(
@@ -257,28 +230,11 @@ class Engine(object):
         last = int(rec[_lib.D_LAST_FRAME])
         ent._last_maybe_move_frame = -float('inf') if last == _lib.NEVER else last
         if b.game.pattern_mutable.get(i):      # e.g. coins picked up on the device
-          from pycolab_b200 import lowering
           packed = b.patterns[i][0].cpu().numpy().view(np.uint32)
           np.copyto(ent.whole_pattern, lowering.unpack_rows(packed, ent.whole_pattern.shape[1]))
-      if b.game.program == _lib.PROG_T_MAZE and i > 0:
-        self._sync_rolled_pattern(ent, i, rec)
       np.copyto(ent.curtain, b.curtain(ch)[0].cpu().numpy())
-      if b.game.program == _lib.PROG_APERTURE:       # ApertureDrape._apertures
-        cells = [int(rec[_lib.D_AUX0]), int(rec[_lib.D_AUX1])]
-        ent._apertures = [None if c < 0 else (c >> 16, c & 0xffff) for c in cells]
-
-  def _sync_rolled_pattern(self, ent, d, rec):
-    """t_maze: whole_pattern = the drape's pattern np.rolled by its record's AUX0 (rows << 16
-    | cols); the teleporter's is empty while its delay lasts (t_maze.py:397-400)."""
-    from pycolab_b200 import lowering
-    b = self._batched
-    shape = ent.whole_pattern.shape
-    base = lowering.unpack_rows(b.patterns[d][0].cpu().numpy().view(np.uint32), shape[1])
-    roll = int(rec[_lib.D_AUX0])
-    base = np.roll(np.roll(base, -(roll >> 16), axis=0), -(roll & 0xffff), axis=1)
-    if b.drape_chars[d] == 't' and int(rec[_lib.D_AUX1]) > 0:
-      base[:] = False
-    np.copyto(ent.whole_pattern, base)
+    if b.game.sync is not None:            # state only this program keeps on the device
+      b.game.sync(self)
 
   # ------------------------------------------------------------ properties
   @property

@@ -7,7 +7,7 @@ game to game in the Plot.
 Set-up only: per-step logic of the three classes is the fused kernel
 csrc/ordeal.cu (one program, the chapter picks the rules); the plot entries the
 reference keeps in Python dict slots travel in the device plot record and are
-mirrored back after every step (lowering._lower_ordeal).
+mirrored back after every step (programs/ordeal.py).
 """
 
 from pycolab_b200 import ascii_art

@@ -118,7 +118,7 @@ def test_apprehend_lowers_and_validates_on_cpu():
   want_dx = random.Random(5).uniform(-2.499, 2.499) / 9.0
   game = lowering.lower(apprehend.make_game())
   assert game.program == _lib.PROG_APPREHEND and game.sprite_chars == 'Pb'
-  assert game.needs_rng and game.rng_kind == 'python'
+  assert game.needs_rng and game.rng_streams == ('python',)
   words = game.sprites[1, [_lib.S_AUX0, _lib.S_AUX1]].astype('<i4')
   assert words.view('<f8')[0] == want_dx
   import ctypes as C

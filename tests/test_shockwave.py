@@ -114,7 +114,7 @@ def test_shockwave_lowers_and_validates_on_cpu():
   from pycolab_b200.games import shockwave
   game = lowering.lower(shockwave.make_game(0))
   assert game.program == _lib.PROG_SHOCKWAVE and game.drape_chars == '@ ^'
-  assert game.needs_rng and game.rng_kind == 'numpy' and game.program_arg[0] == 2
+  assert game.needs_rng and game.rng_streams == ('numpy',) and game.program_arg[0] == 2
   lib = _lib.load()
   handle = C.c_void_p()
   spec = game.make_spec(True)

@@ -170,7 +170,7 @@ def test_t_maze_lowers_and_validates_on_cpu():
   from pycolab_b200 import _lib
   game = _lower_generated(4, level=3, teleport_delay=5, limbo_time=7)
   assert game.program == _lib.PROG_T_MAZE and game.drape_chars == 'Q#*ltr'
-  assert game.float_reward and game.needs_rng and game.rng_kind == 't_maze'
+  assert game.float_reward and game.needs_rng and game.rng_streams == ('python', 'numpy')
   assert list(game.program_arg[:5]) == [3, 0, _lib.T_MAZE_NO_TIMEOUT, 5, 7]
   lib = _lib.load()
   handle = C.c_void_p()
@@ -317,6 +317,11 @@ def test_facade_t_maze_golden(name):
                      int(p.virtual_position[0]), int(p.virtual_position[1])]])
     goals.append(0 if env.things['Q'].which_goal == 'left' else 1)
     assert out[1] is None or isinstance(out[1], float)
+    for ch in '#*ltr':           # the rolled whole_pattern, windowed as drapes.py:689-695
+      d = env.things[ch]
+      r, c = d._northwest_corner
+      np.testing.assert_array_equal(d.curtain, d.whole_pattern[r:r + env.rows, c:c + env.cols],
+                                    '%s frame %d' % (ch, len(goals)))
   got = []
   traj = tj.run_trajectory(_facade(maze, cue, cfg), g['actions'].tolist(),
                            on_frame=lambda env, out: (on_frame(env, out), got.append(
@@ -402,27 +407,31 @@ def test_batched_t_maze_sampled_at_4096():
 
 @pytest.mark.gpu
 def test_t_maze_curtains_and_layers_follow_the_rolls():
-  """curtain() / unoccluded_layers() against the oracle's drapes while patterns roll."""
+  """curtain() / unoccluded_layers() against the oracle's drapes while patterns roll: one
+  shared level, and two levels with share_levels=False (every level tensor one row per env)."""
   import torch
   from pycolab_b200 import batched, levels
   from pycolab_b200.games import t_maze
-  maze, cue = levels.t_maze_level(2)
   cfg = (1, False, -1, 2, 3)
-  eng = batched.BatchedEngine([t_maze.make_game(*cfg, maze_art=maze, cue_art=cue)], batch=2,
-                              rng_seed=8, auto_reset=False)
-  worlds = [otm.make_t_maze(maze, cue, *cfg, rng=random.Random(8 + e),
-                               np_rng=np.random.RandomState(8 + e)) for e in range(2)]
-  for w in worlds:
-    w.its_showtime()
-  eng.its_showtime()
-  for act in [1, 1, 1] + [5] * 6 + [3] * 12:
-    eng.play(torch.full((2,), act, dtype=torch.int32).cuda())
+  for n_worlds, share_levels in ((1, True), (2, False)):
+    arts = [levels.t_maze_level(2 + i) for i in range(n_worlds)]
+    eng = batched.BatchedEngine([t_maze.make_game(*cfg, maze_art=m, cue_art=c) for m, c in arts],
+                                batch=2, rng_seed=8, auto_reset=False, share_levels=share_levels)
+    worlds = [otm.make_t_maze(*arts[e % n_worlds], *cfg, rng=random.Random(8 + e),
+                              np_rng=np.random.RandomState(8 + e)) for e in range(2)]
     for w in worlds:
-      w.play(act)
-    layers = eng.unoccluded_layers('*#ltrQP ').cpu().numpy()
-    for e, w in enumerate(worlds):
-      for ch in 'Q#*ltr':
-        np.testing.assert_array_equal(eng.curtain(ch)[e].cpu().numpy(), w.things[ch].curtain, ch)
-      want = em.unoccluded_layers_of(w.backdrop, w.things, '*#ltrQP ')
-      for k, ch in enumerate('*#ltrQP '):
-        np.testing.assert_array_equal(layers[e, k], want[ch], ch)
+      w.its_showtime()
+    eng.its_showtime()
+    for act in [1, 1, 1] + [5] * 6 + [3] * 12:
+      eng.play(torch.full((2,), act, dtype=torch.int32).cuda())
+      for w in worlds:
+        w.play(act)
+      layers = eng.unoccluded_layers('*#ltrQP ').cpu().numpy()
+      for e, w in enumerate(worlds):
+        for ch in 'Q#*ltr':
+          np.testing.assert_array_equal(eng.curtain(ch)[e].cpu().numpy(), w.things[ch].curtain,
+                                        '%s env %d levels %d' % (ch, e, n_worlds))
+        want = em.unoccluded_layers_of(w.backdrop, w.things, '*#ltrQP ')
+        for k, ch in enumerate('*#ltrQP '):
+          np.testing.assert_array_equal(layers[e, k], want[ch],
+                                        '%s env %d levels %d' % (ch, e, n_worlds))

@@ -34,7 +34,7 @@ def main():
     eng.its_showtime()
     for _ in range(steps):
       a = rs.randint(0, n_actions, size=B * eng.actions_per_env).astype(np.int32)
-      if eng.game.program == 4:                       # fixture rows: motions + no directives
+      if eng.actions_per_env > 1:                     # fixture rows: motions + no directives
         a = a.reshape(B, eng.actions_per_env)
         a[:, -8:] = 0
         a[:, :-8] %= 9
