@@ -48,7 +48,7 @@ typedef enum pcl_status {
   PCL_ERR_INVALID = -1,      /* bad argument / malformed spec (ValueError)   */
   PCL_ERR_UNSUPPORTED = -2,  /* spec is valid pycolab but not lowered        */
   PCL_ERR_CUDA = -3,         /* a CUDA runtime call failed                   */
-  PCL_ERR_UNBOUND = -4,      /* pcl_bind_state has not been called           */
+  PCL_ERR_UNBOUND = -4,      /* pcl_bind_state (or pcl_bind_code) has not been called */
   PCL_ERR_NOMEM = -5
 } pcl_status;
 
@@ -59,6 +59,7 @@ typedef enum pcl_status {
 #define PCL_ENV_ERR_EMPTY_CHOICE     0x4  /* np.random.choice([]) in marauders :253 */
 #define PCL_ENV_ERR_INDEX            0x8  /* NumPy IndexError (board look-up off the array) */
 #define PCL_ENV_ERR_BAD_Z            0x10 /* change_z_order names a missing entity, engine.py:802-812 */
+#define PCL_ENV_ERR_ARITH            0x20 /* ZeroDivisionError: `//` or `%` by zero in compiled code */
 
 /* Which game program advances the envs.  One fused kernel per program; the
  * host "lowering" recognises the reference's entity classes and picks one. */
@@ -98,6 +99,11 @@ typedef enum pcl_program {
                                 teleportation_order.  d_rng, when bound, is u32 [B, 2, PCL_MT_WORDS]: slot 0
                                 Python random.Random words (the cue), slot 1 NumPy RandomState words (the
                                 speckle); d_pattern_init[2] then holds the UN-speckled '*' pattern */
+  PCL_PROG_COMPILED = 14,    /* any registered MazeWalker / plain Drape classes: their update() bodies
+                                compiled to the bytecode below (pcl_bind_code) and interpreted one warp
+                                per env.  Registers: sprite AUX0-AUX2, all eight words of a drape record,
+                                plot AUX0-AUX3 (the_plot keys).  program_arg[0] = 1: rewards are float64
+                                (pcl_outputs.d_reward_f64 is required), 0: int32 */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */
@@ -130,6 +136,57 @@ enum { PCL_DIR_NONE = 0,
        PCL_DIR_DEFAULT_DISCOUNT = 3,  /* arg = f32 bits (plot.py:247-260; upstream resets the default
                                          to 1.0 after every step, plot.py:345-356) */
        PCL_DIR_Z_ORDER = 4 };         /* arg = move_this | in_front_of << 8, 0 = None (plot.py:136-174) */
+
+/* PCL_PROG_COMPILED bytecode (pcl_bind_code): int32 words.  Word 0 = n, the number of entities
+ * (n_sprites + n_drapes); words 1..n = the first word of each entity's update() (sprites first,
+ * then drapes, in spec order).  Entities of one class share their code.  The entry points split
+ * the words after the header into functions; each ends with PCL_OP_RET, and its jumps go
+ * forward to a word inside it, so every update ends.  The operand stack holds int32 values;
+ * "pop r, c" pops c first.  An entity operand of -1 means the entity being updated.  Cell
+ * indices follow NumPy: a negative index counts from the end once, anything else off the board
+ * latches PCL_ENV_ERR_INDEX and reads 0 / writes nothing.  Integers wrap at 32 bits. */
+#define PCL_MAX_CODE_WORDS 16384
+#define PCL_CODE_STACK 16    /* operand stack slots per update */
+#define PCL_CODE_LOCALS 16   /* local variable slots per update */
+enum {
+  PCL_OP_RET = 0,       /* end of this entity's update                                       */
+  PCL_OP_PUSH,          /* imm: push imm                                                      */
+  PCL_OP_POP,           /* pop                                                                */
+  PCL_OP_DUP,           /* push a copy of the top                                             */
+  PCL_OP_LOAD,          /* slot: push local `slot`                                            */
+  PCL_OP_STORE,         /* slot: pop into local `slot`                                        */
+  PCL_OP_JMP,           /* target: jump (target > this word)                                  */
+  PCL_OP_JZ,            /* target: pop; jump if it is 0                                       */
+  PCL_OP_JNZ,           /* target: pop; jump if it is not 0                                   */
+  PCL_OP_ADD, PCL_OP_SUB, PCL_OP_MUL,
+  PCL_OP_FLOORDIV,      /* Python `//` and `%`: floor semantics; by zero latches PCL_ENV_ERR_ARITH */
+  PCL_OP_MOD,
+  PCL_OP_EQ, PCL_OP_NE, PCL_OP_LT, PCL_OP_LE, PCL_OP_GT, PCL_OP_GE,   /* pop b, a; push a op b */
+  PCL_OP_NEG, PCL_OP_NOT,
+  PCL_OP_EQ2,           /* pop (r2, c2), (r1, c1); push r1 == r2 && c1 == c2                  */
+  PCL_OP_IN,            /* k, v_1 .. v_k: pop x; push whether x is one of the v_i (k <= 64)     */
+  PCL_OP_ACTION,        /* push the env's action (PCL_ACTION_NONE at a (re)start)            */
+  PCL_OP_FRAME,         /* push the_plot.frame                                                */
+  PCL_OP_FIELD,         /* sprite, f: push row, col, virtual row, virtual col, visible (f 0-4) */
+  PCL_OP_GETR,          /* k: push register k of the entity being updated (sprite k < 3)      */
+  PCL_OP_SETR,          /* k: pop into it                                                     */
+  PCL_OP_GETP,          /* k: push plot register k (k < 4)                                    */
+  PCL_OP_SETP,          /* k: pop into it                                                     */
+  PCL_OP_BOARD,         /* pop r, c; push the board of the last render at (r, c)             */
+  PCL_OP_BACKDROP,      /* pop r, c; push the backdrop at (r, c)                              */
+  PCL_OP_CURTAIN,       /* drape: pop r, c; push its curtain at (r, c)                        */
+  PCL_OP_SETCELL,       /* pop r, c, v; the updated drape's curtain at (r, c) = v != 0        */
+  PCL_OP_FILL,          /* pop v; every cell of the updated drape's curtain = v != 0          */
+  PCL_OP_ANY,           /* drape: push whether its curtain has a cell set                     */
+  PCL_OP_MOVE,          /* motion (PCL_M_N .. PCL_M_STAY): move the updated walker; push 1 if
+                           it was blocked, 0 if it moved (upstream: None)                     */
+  PCL_OP_TELEPORT,      /* pop r, c: the updated walker's _teleport((r, c))                   */
+  PCL_OP_REWARD,        /* pop x: the_plot.add_reward(x)                                      */
+  PCL_OP_REWARD_F64,    /* lo, hi: add_reward of the float64 with these bit halves            */
+  PCL_OP_TERMINATE,     /* f32 bits: the_plot.terminate_episode(discount)                     */
+  PCL_OP_DISCOUNT,      /* f32 bits: the_plot.change_default_discount(discount)              */
+  PCL_OP_COUNT
+};
 
 /* Motion codes (prefab_parts/sprites.py:140-150). */
 enum { PCL_M_N = 0, PCL_M_NE, PCL_M_E, PCL_M_SE, PCL_M_S, PCL_M_SW, PCL_M_W,
@@ -258,6 +315,19 @@ int pcl_destroy(pcl_handle* h);
 
 /* Attach the caller's device buffers. */
 int pcl_bind_state(pcl_handle* h, const pcl_state* state);
+
+/* PCL_PROG_COMPILED: the bytecode every env runs, h_code a HOST array of n_words int32 words
+ * (see PCL_OP_*).  It is checked before anything touches a device: known opcodes, entry
+ * points that split the code into functions of the right entity kind, each ending in
+ * PCL_OP_RET, forward jumps inside the function, entity, register, local and stack bounds,
+ * n_words <= PCL_MAX_CODE_WORDS; PCL_ERR_INVALID otherwise.  The handle keeps a copy; the
+ * next pcl_reset / pcl_step / pcl_run / pcl_run_many / pcl_step_host* of the handle uploads
+ * it on its own stream and waits for that copy before it launches (it synchronises that
+ * stream once, so that call must not be captured into a CUDA graph), after which launches on
+ * any stream read the new code.  Binding again while kernels of the handle still run is
+ * safe: the upload first waits for the device.  Other programs: PCL_ERR_UNSUPPORTED.
+ * pcl_reset / pcl_step return PCL_ERR_UNBOUND until code is bound. */
+int pcl_bind_code(pcl_handle* h, const int32_t* h_code, int32_t n_words);
 
 /* Engine.its_showtime() (engine.py:520-581) for every env whose d_env_mask
  * byte is non-zero (NULL = all): restore the reset templates, then run the

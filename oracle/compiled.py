@@ -1,0 +1,179 @@
+"""CPU interpreter of the compiled program's bytecode (include/pcl.h PCL_OP_*).  TEST
+INFRASTRUCTURE ONLY; nothing under `pycolab_b200/` imports it.
+
+`make_world(game)` builds an `engine_model.World` from a lowered game of the compiled
+program (`pycolab_b200.programs.compiled.lower`: its templates, registers and code words)
+and `compiled_program(world, ch, actions)` runs entity `ch`'s update() by interpreting the
+same words the device runs, one instruction at a time, over the oracle's registers.  The
+Python reference semantics it restates: NumPy cell indexing, floor `//` and `%`, rewards
+summed in call order as Python sums them (an int sum stays int), the Plot directives of
+plot.py:176-260 and MazeWalker motion (sprites.py:315-546 via engine_model).
+"""
+
+import struct
+
+import numpy as np
+
+from oracle import engine_model as em
+from pycolab_b200 import _lib, lowering
+
+OP = _lib.OP
+_ERR_INDEX, _ERR_ARITH = 0x8, 0x20
+
+
+def _wrap32(x):
+  return (int(x) + 2 ** 31) % 2 ** 32 - 2 ** 31
+
+
+def _f32(bits):
+  return float(struct.unpack('<f', struct.pack('<i', bits))[0])
+
+
+def _f64(lo, hi):
+  return struct.unpack('<d', struct.pack('<ii', lo, hi))[0]
+
+
+def make_world(game):
+  """A fresh oracle env (the its_showtime() state) of lowered compiled game `game`."""
+  rows, cols = game.rows, game.cols
+  ents = {}
+  for s, ch in enumerate(game.sprite_chars):
+    rec = game.sprites[s]
+    w = em.Walker(ch, (rows, cols), (int(rec[_lib.S_ROW]), int(rec[_lib.S_COL])),
+                  confined=bool(game.confined[s]))
+    w.vrow, w.vcol = int(rec[_lib.S_VROW]), int(rec[_lib.S_VCOL])
+    w.visible = bool(rec[_lib.S_FLAGS] & 1)
+    w.prior_visible = (None, False, True)[(int(rec[_lib.S_FLAGS]) >> 1) & 3]
+    mask = game.impassable[s]
+    w.impassable = frozenset(c for c in range(128) if (mask[c >> 5] >> (c & 31)) & 1)
+    w.regs = [int(x) for x in rec[_lib.S_AUX0:]]
+    ents[ch] = w
+  for d, ch in enumerate(game.drape_chars):
+    drape = em.PlainDrape(ch, lowering.unpack_rows(game.bits[d], cols)[:rows])
+    drape.regs = [int(x) for x in game.drapes[d]]
+    ents[ch] = drape
+  world = em.World(rows, cols, game.backdrop[:, :cols], ents, game.z_order,
+                   [list(g) for g in game.groups], compiled_program)
+  world.code = [int(x) for x in game.code]
+  world.entity_chars = game.sprite_chars + game.drape_chars
+  world.plot.regs = [int(x) for x in game.plot[_lib.P_AUX0:_lib.P_AUX0 + 4]]
+  world.error = 0
+  return world
+
+
+def compiled_program(world, ch, actions):
+  code, plot = world.code, world.plot
+  chars = world.entity_chars
+  me = world.things[ch]
+  action = _lib.ACTION_NONE if actions is None else int(actions)
+  stack, local = [], [0] * _lib.CODE_LOCALS
+  pc = code[1 + chars.index(ch)]
+
+  def ent(k):
+    return me if k < 0 else world.things[chars[k]]
+
+  def cell(r, c):
+    """NumPy's index rule, or None (the device latches PCL_ENV_ERR_INDEX)."""
+    r = r + world.rows if r < 0 else r
+    c = c + world.cols if c < 0 else c
+    if 0 <= r < world.rows and 0 <= c < world.cols:
+      return r, c
+    world.error |= _ERR_INDEX
+    return None
+
+  while True:
+    op = code[pc]
+    name = _lib.OPS[op]
+    a = code[pc + 1] if pc + 1 < len(code) else 0
+    nxt = pc + 1 + _lib.OPERANDS[op]
+    if name == 'RET':
+      return
+    elif name == 'PUSH':
+      stack.append(a)
+    elif name == 'POP':
+      stack.pop()
+    elif name == 'DUP':
+      stack.append(stack[-1])
+    elif name == 'LOAD':
+      stack.append(local[a])
+    elif name == 'STORE':
+      local[a] = stack.pop()
+    elif name == 'JMP':
+      nxt = a
+    elif name in ('JZ', 'JNZ'):
+      if (stack.pop() == 0) == (name == 'JZ'):
+        nxt = a
+    elif name in ('ADD', 'SUB', 'MUL', 'FLOORDIV', 'MOD', 'EQ', 'NE', 'LT', 'LE', 'GT', 'GE'):
+      y, x = stack.pop(), stack.pop()
+      if name in ('FLOORDIV', 'MOD') and y == 0:
+        world.error |= _ERR_ARITH
+        v = 0
+      else:
+        v = {'ADD': lambda: x + y, 'SUB': lambda: x - y, 'MUL': lambda: x * y,
+             'FLOORDIV': lambda: x // y, 'MOD': lambda: x % y, 'EQ': lambda: x == y,
+             'NE': lambda: x != y, 'LT': lambda: x < y, 'LE': lambda: x <= y,
+             'GT': lambda: x > y, 'GE': lambda: x >= y}[name]()
+      stack.append(_wrap32(v))
+    elif name == 'NEG':
+      stack.append(_wrap32(-stack.pop()))
+    elif name == 'NOT':
+      stack.append(int(stack.pop() == 0))
+    elif name == 'EQ2':
+      c2, r2, c1, r1 = stack.pop(), stack.pop(), stack.pop(), stack.pop()
+      stack.append(int(r1 == r2 and c1 == c2))
+    elif name == 'IN':
+      values = code[pc + 2:pc + 2 + a]
+      stack.append(int(stack.pop() in values))
+      nxt += a
+    elif name == 'ACTION':
+      stack.append(action)
+    elif name == 'FRAME':
+      stack.append(plot.frame)
+    elif name == 'FIELD':
+      w = ent(a)
+      f = code[pc + 2]
+      stack.append((w.row, w.col, w.vrow, w.vcol, int(bool(w.visible)))[f])
+    elif name == 'GETR':
+      stack.append(me.regs[a])
+    elif name == 'SETR':
+      me.regs[a] = stack.pop()
+    elif name == 'GETP':
+      stack.append(plot.regs[a])
+    elif name == 'SETP':
+      plot.regs[a] = stack.pop()
+    elif name in ('BOARD', 'BACKDROP', 'CURTAIN'):
+      c, r = stack.pop(), stack.pop()
+      at = cell(r, c)
+      if at is None:
+        stack.append(0)
+      elif name == 'BOARD':
+        stack.append(int(world.board[at]))
+      elif name == 'BACKDROP':
+        stack.append(int(world.backdrop[at]))
+      else:
+        stack.append(int(ent(a).curtain[at]))
+    elif name == 'SETCELL':
+      v, c, r = stack.pop(), stack.pop(), stack.pop()
+      at = cell(r, c)
+      if at is not None:
+        me.curtain[at] = v != 0
+    elif name == 'FILL':
+      me.curtain[:] = stack.pop() != 0
+    elif name == 'ANY':
+      stack.append(int(ent(a).curtain.any()))
+    elif name == 'MOVE':
+      stack.append(0 if em.walker_move(me, world.board, plot, a) is None else 1)
+    elif name == 'TELEPORT':
+      c, r = stack.pop(), stack.pop()
+      em.walker_teleport(me, r, c)
+    elif name == 'REWARD':
+      plot.add_reward(stack.pop())
+    elif name == 'REWARD_F64':
+      plot.add_reward(_f64(a, code[pc + 2]))
+    elif name == 'TERMINATE':
+      plot.terminate_episode(_f32(a))
+    elif name == 'DISCOUNT':
+      plot.discount = _f32(a)
+    else:
+      raise AssertionError('opcode %d' % op)
+    pc = nxt

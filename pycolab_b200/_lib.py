@@ -35,13 +35,31 @@ ENV_ERR_SECOND_ORDER = 0x2
 ENV_ERR_EMPTY_CHOICE = 0x4
 ENV_ERR_INDEX = 0x8
 ENV_ERR_BAD_Z = 0x10
+ENV_ERR_ARITH = 0x20
 
 PROG_NONE, PROG_SCROLLY_MAZE, PROG_WAREHOUSE, PROG_MARAUDERS, PROG_FIXTURE = 0, 1, 2, 3, 4
 PROG_BETTER_SCROLLY, PROG_CLASSICS, PROG_APERTURE, PROG_ORDEAL, PROG_HELLO = 5, 6, 7, 8, 9
 PROG_APPREHEND, PROG_SHOCKWAVE, PROG_T_MAZE = 10, 11, 12
+PROG_COMPILED = 14
 T_MAZE_NO_TIMEOUT = 0x7fffffff   # program_arg[2] for timeout_frames = inf
 ORDEAL_NEXT_UNSET, ORDEAL_NEXT_NONE, ORDEAL_CASTLE, ORDEAL_CAVERN, ORDEAL_KANSAS = -1, 0, 1, 2, 3
 CLASSIC_FOUR_ROOMS, CLASSIC_CLIFF_WALK, CLASSIC_CHAIN_WALK, CLASSIC_FLUVIAL = 0, 1, 2, 3
+
+# PCL_PROG_COMPILED bytecode (pcl.h PCL_OP_*): opcode -> operand words (IN: its count more).
+MAX_CODE_WORDS = 16384
+CODE_STACK = 16
+CODE_LOCALS = 16
+OPS = ('RET', 'PUSH', 'POP', 'DUP', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'ADD', 'SUB', 'MUL',
+       'FLOORDIV', 'MOD', 'EQ', 'NE', 'LT', 'LE', 'GT', 'GE', 'NEG', 'NOT', 'EQ2', 'IN', 'ACTION',
+       'FRAME', 'FIELD', 'GETR', 'SETR', 'GETP', 'SETP', 'BOARD', 'BACKDROP', 'CURTAIN',
+       'SETCELL', 'FILL', 'ANY', 'MOVE', 'TELEPORT', 'REWARD', 'REWARD_F64', 'TERMINATE',
+       'DISCOUNT')
+OP = {name: code for code, name in enumerate(OPS)}
+OPERANDS = {OP[n]: (2 if n in ('FIELD', 'REWARD_F64') else
+                    1 if n in ('PUSH', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'IN', 'GETR', 'SETR',
+                               'GETP', 'SETP', 'CURTAIN', 'ANY', 'MOVE', 'TERMINATE',
+                               'DISCOUNT') else 0) for n in OPS}
+FIELD_ROW, FIELD_COL, FIELD_VROW, FIELD_VCOL, FIELD_VISIBLE = range(5)
 
 # Record word indices (pcl.h enums).
 S_ROW, S_COL, S_VROW, S_VCOL, S_FLAGS, S_AUX0, S_AUX1, S_AUX2 = range(8)
@@ -154,6 +172,7 @@ SYMBOLS = {
     'pcl_create': (C.c_int, [C.POINTER(Spec), C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     'pcl_destroy': (C.c_int, [C.c_void_p]),
     'pcl_bind_state': (C.c_int, [C.c_void_p, C.POINTER(State)]),
+    'pcl_bind_code': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     'pcl_reset': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_step': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_run': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs), C.c_void_p]),

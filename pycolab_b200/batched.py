@@ -203,6 +203,9 @@ class BatchedEngine(object):
                                     C.byref(handle)), 'pcl_create')
     self._h = handle
     _lib.check(self._lib.pcl_bind_state(self._h, C.byref(self._state)), 'pcl_bind_state')
+    if g0.code is not None:       # the compiled program's bytecode, shared by every level
+      code = np.ascontiguousarray(g0.code, dtype=np.int32)
+      _lib.check(self._lib.pcl_bind_code(self._h, code.ctypes.data, len(code)), 'pcl_bind_code')
     self._showtime = False
 
   # ---------------------------------------------------------------- running

@@ -1,0 +1,779 @@
+"""Compile entity classes' own `update()` methods to device bytecode (`PCL_PROG_COMPILED`).
+
+    from pycolab_b200 import compiler
+    compiler.register(my_game.PlayerSprite, my_game.CoinDrape)
+
+`register` opts classes in: their `update()` source (`inspect.getsource` + `ast`) is
+compiled to the stack bytecode of include/pcl.h (`PCL_OP_*`), and from then on
+`lowering.lower` runs games made of registered classes on the compiled step program
+(csrc/compiled.cu) instead of refusing them.  Classes that are not registered behave
+as before.
+
+The subset (everything else raises `NotLoweredError` naming the class, the source line
+and the construct):
+  entities    MazeWalker subclasses (any impassable set, confined or not, default
+              scrolling group, not egocentric) and plain Drape subclasses;
+  statements  if / elif / else, return, pass; `del` and docstrings compile to nothing;
+              local variables holding an int, a bool, a position or a motion result;
+              `self.<attr>` and `the_plot['key']` with =, +=, -=, *=, //=, %=;
+              motion helpers (`self._north(board, the_plot)` ... `self._stay(...)`),
+              `self._teleport(pos)`, `the_plot.add_reward(x)`,
+              `the_plot.terminate_episode([discount])`, `the_plot.change_default_discount(c)`;
+              on drapes `self.curtain[cell] = v` and `self.curtain[:] = v`;
+  values      `actions` (==, !=, in, is None only), int and bool literals (float literals
+              only as a reward or a discount), + - * // % and unary -, comparisons
+              (chained, position against position or tuple), `in` over a literal
+              tuple / list / string, and / or / not, `x if c else y`, `is None` on
+              motion results, int(), ord('c'), chr(cell) against characters, positions
+              (`.position`, `.virtual_position`, `.corner`, `.row`, `.col`, [0], [1]),
+              `.visible`, `the_plot.frame`, `the_plot['key']`, `the_plot.get('key')`,
+              `board[cell]`, `backdrop.curtain[cell]`, `layers['X'][cell]`,
+              `self.curtain[cell]`, `things['X'].position / .visible / .curtain[cell]`,
+              `.curtain.any()`.
+Int and bool attributes of `self` become per-entity registers and `the_plot` keys plot
+registers; their values are read from the live objects when the game is lowered.
+Integers are 32 bits on the device; values outside int32 wrap.  After a facade step a
+register is written back with the type (bool or int) its value had at lowering.
+"""
+
+import ast
+import inspect
+import struct
+import textwrap
+
+import numpy as np
+
+from pycolab_b200 import _lib
+from pycolab_b200 import things
+from pycolab_b200.errors import NotLoweredError
+from pycolab_b200.prefab_parts import drapes as prefab_drapes
+from pycolab_b200.prefab_parts import sprites as prefab_sprites
+
+_REGISTRY = {}                # class -> Compiled
+
+_PARAMS = ('self', 'actions', 'board', 'layers', 'backdrop', 'things', 'the_plot')
+_MOTIONS = {'_north': 0, '_northeast': 1, '_east': 2, '_southeast': 3, '_south': 4,
+            '_southwest': 5, '_west': 6, '_northwest': 7, '_stay': 8}
+_BINOPS = {ast.Add: 'ADD', ast.Sub: 'SUB', ast.Mult: 'MUL', ast.FloorDiv: 'FLOORDIV',
+           ast.Mod: 'MOD'}
+_CMPOPS = {ast.Eq: 'EQ', ast.NotEq: 'NE', ast.Lt: 'LT', ast.LtE: 'LE', ast.Gt: 'GT',
+           ast.GtE: 'GE'}
+_POSITIONS = {'position': (_lib.FIELD_ROW, _lib.FIELD_COL),
+              'virtual_position': (_lib.FIELD_VROW, _lib.FIELD_VCOL)}
+# Registers per entity: sprite record AUX0-AUX2, every word of a plain drape's record.
+MAX_REGISTERS = {'sprite': 3, 'drape': _lib.DRAPE_WORDS}
+MAX_PLOT_KEYS = 4
+_TYPE_NAMES = {'int': 'number', 'pos': 'position', 'motion': 'motion result', 'char': 'character'}
+
+
+def _f32_bits(x):
+  return struct.unpack('<i', struct.pack('<f', float(x)))[0]
+
+
+def _f64_halves(x):
+  lo, hi = struct.unpack('<ii', struct.pack('<d', float(x)))
+  return lo, hi
+
+
+class Compiled(object):
+  """One class's update(), compiled with symbolic operands (`link` resolves them):
+  ('attr', name) a register, ('key', name) a plot key, ('ent', char) an entity,
+  ('label', n) a code address, ('rows',) / ('cols',) the board shape."""
+
+  def __init__(self, klass, kind, ir, attrs, keys, float_reward):
+    self.klass, self.kind, self.ir = klass, kind, ir
+    self.attrs = attrs            # register names, in slot order
+    self.keys = keys              # the_plot keys it reads or writes
+    self.float_reward = float_reward
+
+
+def register(*classes):
+  """Compile each class's update() and make `lowering` run it on the device.
+  Returns its argument (so `@compiler.register` decorates a class)."""
+  for klass in classes:
+    _REGISTRY[klass] = compile_class(klass)
+  return classes[0] if len(classes) == 1 else classes
+
+
+def unregister(*classes):
+  for klass in classes:
+    _REGISTRY.pop(klass, None)
+
+
+def registered(cls):
+  """The `Compiled` of the registered class along `cls`'s MRO whose update() `cls` uses,
+  or None."""
+  for klass in cls.__mro__:
+    if klass in _REGISTRY:
+      return _REGISTRY[klass] if cls.update is klass.update else None
+  return None
+
+
+def compile_class(klass):
+  if not isinstance(klass, type):
+    raise TypeError('register() takes classes, got {!r}'.format(klass))
+  if issubclass(klass, prefab_sprites.MazeWalker):
+    kind = 'sprite'
+  elif issubclass(klass, things.Drape) and not issubclass(klass, prefab_drapes.Scrolly):
+    kind = 'drape'
+  else:
+    raise NotLoweredError('{}: only MazeWalker and plain Drape subclasses are compiled'.format(
+        _name(klass)))
+  if klass.update in (prefab_sprites.MazeWalker.update, things.Drape.update):
+    raise NotLoweredError('{}: has no update() of its own to compile'.format(_name(klass)))
+  return _Compiler(klass, kind).run()
+
+
+def _name(klass):
+  return '{}.{}'.format(klass.__module__, klass.__qualname__)
+
+
+class _Compiler(object):
+
+  def __init__(self, klass, kind):
+    self.klass, self.kind = klass, kind
+    fn = klass.update
+    try:
+      lines, self.first = inspect.getsourcelines(fn)
+    except (OSError, TypeError):
+      raise NotLoweredError('{}: the source of update() is not available'.format(_name(klass)))
+    self.lines = lines
+    tree = ast.parse(textwrap.dedent(''.join(lines)))
+    self.fdef = tree.body[0]
+    args = self.fdef.args
+    if (not isinstance(self.fdef, ast.FunctionDef) or len(args.args) != len(_PARAMS) or
+        args.vararg or args.kwarg or args.kwonlyargs or self.fdef.decorator_list):
+      raise NotLoweredError('{}: update() must take the seven standard arguments'.format(
+          _name(klass)))
+    self.role = {a.arg: role for a, role in zip(args.args, _PARAMS)}
+    self.ir = []
+    self.n_labels = 0
+    self.locals = {}              # name -> (first slot, type)
+    self.n_slots = 0
+    self.attrs, self.keys = [], []
+    self.float_reward = False
+
+  def run(self):
+    self.stmts(self.fdef.body)
+    self.emit('RET')
+    return Compiled(self.klass, self.kind, self.ir, self.attrs, self.keys, self.float_reward)
+
+  # -------------------------------------------------------------- helpers
+  def refuse(self, node, what):
+    line = self.first + getattr(node, 'lineno', 1) - 1
+    text = self.lines[getattr(node, 'lineno', 1) - 1].strip()
+    raise NotLoweredError('{}.update, line {}: {} is not compiled: {}'.format(
+        _name(self.klass), line, what, text))
+
+  def emit(self, *ins):
+    self.ir.append(ins)
+
+  def label(self):
+    self.n_labels += 1
+    return ('label', self.n_labels)
+
+  def place(self, lab):
+    self.ir.append(('LABEL', lab[1]))
+
+  def is_param(self, node, role):
+    return isinstance(node, ast.Name) and self.role.get(node.id) == role
+
+  def is_self(self, node):
+    return self.is_param(node, 'self')
+
+  def thing_char(self, node):
+    """'X' of `things['X']`, else None."""
+    if (isinstance(node, ast.Subscript) and self.is_param(node.value, 'things') and
+        isinstance(node.slice, ast.Constant) and isinstance(node.slice.value, str)):
+      return node.slice.value
+    return None
+
+  def plot_key(self, node):
+    """'k' of `the_plot['k']`, else None."""
+    if isinstance(node, ast.Subscript) and self.is_param(node.value, 'the_plot'):
+      if isinstance(node.slice, ast.Constant) and isinstance(node.slice.value, str):
+        return self.use_key(node.slice.value)
+      self.refuse(node, 'a the_plot key that is not a string literal')
+    return None
+
+  def use_key(self, key):
+    if key not in self.keys:
+      self.keys.append(key)
+    return key
+
+  def use_attr(self, node, name):
+    if name in _RESERVED.get(self.kind, ()) or hasattr(self.klass, name):
+      self.refuse(node, 'attribute self.{} (not an int or bool of this object)'.format(name))
+    if name not in self.attrs:
+      self.attrs.append(name)
+    return ('attr', name)
+
+  def need(self, node, kind, what):
+    if self.kind != kind:
+      self.refuse(node, '{} in a {} class'.format(what, self.kind))
+
+  def number(self, node):
+    """Value of an int / float literal, optionally negated, else None."""
+    sign = 1
+    if isinstance(node, ast.UnaryOp) and isinstance(node.op, ast.USub):
+      sign, node = -1, node.operand
+    if (isinstance(node, ast.Constant) and isinstance(node.value, (int, float)) and
+        not isinstance(node.value, bool)):
+      return sign * node.value
+    return None
+
+  # ----------------------------------------------------------- statements
+  def stmts(self, body):
+    for st in body:
+      self.stmt(st)
+
+  def stmt(self, st):
+    if isinstance(st, ast.Expr):
+      v = st.value
+      if isinstance(v, ast.Constant) and isinstance(v.value, str):
+        return                                    # docstring
+      if isinstance(v, ast.Call):
+        return self.call_stmt(v)
+      self.refuse(st, 'an expression statement')
+    elif isinstance(st, ast.Pass):
+      return
+    elif isinstance(st, ast.Delete):
+      if all(isinstance(t, ast.Name) for t in st.targets):
+        return
+      self.refuse(st, '`del` of anything but names')
+    elif isinstance(st, ast.Return):
+      if st.value is not None and not (isinstance(st.value, ast.Constant) and
+                                       st.value.value is None):
+        self.refuse(st, 'returning a value')
+      self.emit('RET')
+    elif isinstance(st, ast.If):
+      self.truth(st.test)
+      other, end = self.label(), self.label()
+      self.emit('JZ', other)
+      self.stmts(st.body)
+      if st.orelse:
+        self.emit('JMP', end)
+      self.place(other)
+      if st.orelse:
+        self.stmts(st.orelse)
+        self.place(end)
+    elif isinstance(st, ast.Assign):
+      if len(st.targets) != 1:
+        self.refuse(st, 'chained assignment')
+      self.assign(st.targets[0], st.value, st)
+    elif isinstance(st, ast.AugAssign):
+      self.aug_assign(st)
+    else:
+      self.refuse(st, type(st).__name__)
+
+  def assign(self, target, value, st):
+    if isinstance(target, ast.Name):
+      if target.id in self.role:
+        self.refuse(st, 'assigning an update() argument')
+      t = self.expr(value)
+      if t == 'char':
+        self.refuse(st, 'a character in a variable')
+      slot, have = self.locals.get(target.id, (None, None))
+      if have is None:
+        slot = self.n_slots
+        self.n_slots += 2 if t == 'pos' else 1
+        if self.n_slots > _lib.CODE_LOCALS:
+          self.refuse(st, 'more than {} local slots'.format(_lib.CODE_LOCALS))
+        self.locals[target.id] = (slot, t)
+      elif have != t:
+        self.refuse(st, 'variable {} holding a {} and a {}'.format(
+            target.id, _TYPE_NAMES[have], _TYPE_NAMES[t]))
+      if t == 'pos':
+        self.emit('STORE', slot + 1)
+      self.emit('STORE', slot)
+      return
+    if isinstance(target, ast.Attribute) and self.is_self(target.value):
+      reg = self.use_attr(target, target.attr)
+      self.scalar(value)
+      self.emit('SETR', reg)
+      return
+    key = self.plot_key(target)
+    if key is not None:
+      self.scalar(value)
+      self.emit('SETP', ('key', key))
+      return
+    if (isinstance(target, ast.Subscript) and isinstance(target.value, ast.Attribute) and
+        self.is_self(target.value.value) and target.value.attr == 'curtain'):
+      self.need(st, 'drape', 'a curtain write')
+      sl = target.slice
+      if isinstance(sl, ast.Slice):
+        if sl.lower is not None or sl.upper is not None or sl.step is not None:
+          self.refuse(st, 'a curtain slice other than [:]')
+        self.scalar(value)
+        self.emit('FILL')
+      else:
+        self.cell(sl, st)
+        self.scalar(value)
+        self.emit('SETCELL')
+      return
+    self.refuse(st, 'this assignment target')
+
+  def aug_assign(self, st):
+    op = _BINOPS.get(type(st.op))
+    if op is None:
+      self.refuse(st, 'augmented assignment ' + type(st.op).__name__)
+    target = st.target
+    if isinstance(target, ast.Attribute) and self.is_self(target.value):
+      reg = self.use_attr(target, target.attr)
+      load, store = ('GETR', reg), ('SETR', reg)
+    elif self.plot_key(target) is not None:
+      key = ('key', self.plot_key(target))
+      load, store = ('GETP', key), ('SETP', key)
+    elif isinstance(target, ast.Name) and self.locals.get(target.id, (0, None))[1] == 'int':
+      slot = self.locals[target.id][0]
+      load, store = ('LOAD', slot), ('STORE', slot)
+    else:
+      self.refuse(st, 'this augmented assignment target')
+    self.emit(*load)
+    self.scalar(st.value)
+    self.emit(op)
+    self.emit(*store)
+
+  def call_stmt(self, call):
+    f = call.func
+    if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS:
+      self.expr(call)
+      self.emit('POP')
+      return
+    if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr == '_teleport':
+      self.need(call, 'sprite', '_teleport')
+      if len(call.args) != 1 or call.keywords:
+        self.refuse(call, '_teleport with other than one position')
+      self.pos(call.args[0], call)
+      self.emit('TELEPORT')
+      return
+    if isinstance(f, ast.Attribute) and self.is_param(f.value, 'the_plot'):
+      if f.attr == 'add_reward' and len(call.args) == 1 and not call.keywords:
+        arg = call.args[0]
+        value = self.number(arg)
+        if isinstance(value, float):
+          self.float_reward = True
+          self.emit('REWARD_F64', *_f64_halves(value))
+        else:
+          self.scalar(arg)
+          self.emit('REWARD')
+        return
+      if f.attr in ('terminate_episode', 'change_default_discount'):
+        args = list(call.args) + [k.value for k in call.keywords if k.arg == 'discount']
+        if len(args) + len([k for k in call.keywords if k.arg != 'discount']) > 1:
+          self.refuse(call, 'these arguments of ' + f.attr)
+        if not args and f.attr == 'terminate_episode':
+          value = 0.0
+        else:
+          value = self.number(args[0]) if args else None
+        if value is None:
+          self.refuse(call, 'a discount that is not a number literal')
+        self.emit('TERMINATE' if f.attr == 'terminate_episode' else 'DISCOUNT', _f32_bits(value))
+        return
+    self.refuse(call, 'the call {}()'.format(ast.unparse(f)))
+
+  # ----------------------------------------------------------- expressions
+  def scalar(self, node):
+    """An int (or bool) value."""
+    t = self.expr(node)
+    if t != 'int':
+      self.refuse(node, 'a {} where a number is needed'.format(_TYPE_NAMES[t]))
+
+  def truth(self, node):
+    t = self.expr(node)
+    if t not in ('int', 'motion'):
+      self.refuse(node, 'a {} as a truth value'.format(_TYPE_NAMES[t]))
+
+  def pos(self, node, where):
+    parts = self.pos_parts(node)
+    if parts is None:
+      self.refuse(where, 'something that is not a position')
+    for part in parts:
+      part()
+
+  def cell(self, node, where):
+    """Push (row, col) of a cell index: [r, c] or a position."""
+    if isinstance(node, ast.Tuple) and len(node.elts) == 2:
+      self.scalar(node.elts[0])
+      self.scalar(node.elts[1])
+    else:
+      self.pos(node, where)
+
+  def pos_parts(self, node):
+    """Two emitters (row, col) of a position expression, else None."""
+    def field(ent, f):
+      return lambda: self.emit('FIELD', ent, f)
+    if isinstance(node, ast.Attribute):
+      owner = None
+      if self.is_self(node.value):
+        owner = -1
+      elif self.thing_char(node.value) is not None:
+        owner = ('ent', self.thing_char(node.value))
+      if owner is not None:
+        if node.attr in _POSITIONS:
+          if owner == -1:
+            self.need(node, 'sprite', '.' + node.attr)
+          return tuple(field(owner, f) for f in _POSITIONS[node.attr])
+        if node.attr == 'corner':
+          return (lambda: self.emit('PUSH', ('rows',)), lambda: self.emit('PUSH', ('cols',)))
+    if isinstance(node, ast.Name) and self.locals.get(node.id, (0, None))[1] == 'pos':
+      slot = self.locals[node.id][0]
+      return (lambda: self.emit('LOAD', slot), lambda: self.emit('LOAD', slot + 1))
+    if isinstance(node, ast.Tuple) and len(node.elts) == 2:
+      return (lambda: self.scalar(node.elts[0]), lambda: self.scalar(node.elts[1]))
+    return None
+
+  def component(self, node, index, where):
+    parts = self.pos_parts(node)
+    if parts is None or isinstance(node, ast.Tuple):
+      self.refuse(where, 'indexing something that is not a position')
+    parts[index]()
+    return 'int'
+
+  def expr(self, node):
+    """Emit code pushing `node`'s value; returns its type: 'int' (bools too), 'pos'
+    (two words), 'motion' (1 = blocked, 0 = None) or 'char' (chr of a cell)."""
+    if isinstance(node, ast.Constant):
+      if isinstance(node.value, (bool, int)):
+        self.emit('PUSH', int(node.value))
+        return 'int'
+      self.refuse(node, 'the literal {!r} here'.format(node.value))
+    if isinstance(node, ast.Name):
+      if node.id in self.locals:
+        slot, t = self.locals[node.id]
+        self.emit('LOAD', slot)
+        if t == 'pos':
+          self.emit('LOAD', slot + 1)
+        return t
+      if self.role.get(node.id) == 'actions':
+        self.refuse(node, '`actions` outside ==, != , in and `is None`')
+      self.refuse(node, 'the name ' + node.id)
+    if isinstance(node, ast.Attribute):
+      return self.attribute(node)
+    if isinstance(node, ast.Subscript):
+      return self.subscript(node)
+    if isinstance(node, ast.Call):
+      return self.call(node)
+    if isinstance(node, ast.BinOp):
+      op = _BINOPS.get(type(node.op))
+      if op is None:
+        self.refuse(node, 'the operator ' + type(node.op).__name__)
+      self.scalar(node.left)
+      self.scalar(node.right)
+      self.emit(op)
+      return 'int'
+    if isinstance(node, ast.UnaryOp):
+      if isinstance(node.op, ast.USub):
+        self.scalar(node.operand)
+        self.emit('NEG')
+      elif isinstance(node.op, ast.UAdd):
+        self.scalar(node.operand)
+      elif isinstance(node.op, ast.Not):
+        self.truth(node.operand)
+        self.emit('NOT')
+      else:
+        self.refuse(node, 'the operator ' + type(node.op).__name__)
+      return 'int'
+    if isinstance(node, ast.BoolOp):
+      # Python's value semantics: `a or b` is a if a is true, else b.
+      end, kinds = self.label(), set()
+      for i, v in enumerate(node.values):
+        t = self.expr(v)
+        if t not in ('int', 'motion'):
+          self.refuse(v, 'a {} in and / or'.format(_TYPE_NAMES[t]))
+        kinds.add(t)
+        if i < len(node.values) - 1:
+          self.emit('DUP')
+          self.emit('JZ' if isinstance(node.op, ast.And) else 'JNZ', end)
+          self.emit('POP')
+      self.place(end)
+      return 'int' if kinds == {'int'} else 'motion'
+    if isinstance(node, ast.IfExp):
+      other, end = self.label(), self.label()
+      self.truth(node.test)
+      self.emit('JZ', other)
+      t = self.expr(node.body)
+      self.emit('JMP', end)
+      self.place(other)
+      if self.expr(node.orelse) != t or t == 'pos':
+        self.refuse(node, 'a conditional expression over different or position values')
+      self.place(end)
+      return t
+    if isinstance(node, ast.Compare):
+      return self.compare(node)
+    self.refuse(node, type(node).__name__)
+
+  def attribute(self, node):
+    if self.pos_parts(node) is not None and not isinstance(node, ast.Tuple):
+      for part in self.pos_parts(node):
+        part()
+      return 'pos'
+    if node.attr in ('row', 'col'):
+      return self.component(node.value, 0 if node.attr == 'row' else 1, node)
+    if self.is_self(node.value):
+      if node.attr == 'visible':
+        self.need(node, 'sprite', '.visible')
+        self.emit('FIELD', -1, _lib.FIELD_VISIBLE)
+        return 'int'
+      self.emit('GETR', self.use_attr(node, node.attr))
+      return 'int'
+    ch = self.thing_char(node.value)
+    if ch is not None and node.attr == 'visible':
+      self.emit('FIELD', ('ent', ch), _lib.FIELD_VISIBLE)
+      return 'int'
+    if self.is_param(node.value, 'the_plot') and node.attr == 'frame':
+      self.emit('FRAME')
+      return 'int'
+    self.refuse(node, 'the attribute .' + node.attr)
+
+  def curtain_owner(self, node):
+    """-1 for `self.curtain`, ('ent', X) for `things['X'].curtain`, else None."""
+    if isinstance(node, ast.Attribute) and node.attr == 'curtain':
+      if self.is_self(node.value):
+        self.need(node, 'drape', 'self.curtain')
+        return -1
+      ch = self.thing_char(node.value)
+      if ch is not None:
+        return ('ent', ch)
+    return None
+
+  def subscript(self, node):
+    key = self.plot_key(node)
+    if key is not None:
+      self.emit('GETP', ('key', key))
+      return 'int'
+    base, sl = node.value, node.slice
+    if self.is_param(base, 'board'):
+      self.cell(sl, node)
+      self.emit('BOARD')
+      return 'int'
+    if (isinstance(base, ast.Subscript) and self.is_param(base.value, 'layers') and
+        isinstance(base.slice, ast.Constant) and isinstance(base.slice.value, str) and
+        len(base.slice.value) == 1):
+      self.cell(sl, node)
+      self.emit('BOARD')
+      self.emit('PUSH', ord(base.slice.value))
+      self.emit('EQ')
+      return 'int'
+    if (isinstance(base, ast.Attribute) and base.attr == 'curtain' and
+        self.is_param(base.value, 'backdrop')):
+      self.cell(sl, node)
+      self.emit('BACKDROP')
+      return 'int'
+    owner = self.curtain_owner(base)
+    if owner is not None:
+      if isinstance(sl, ast.Slice):
+        self.refuse(node, 'reading a curtain slice')
+      self.cell(sl, node)
+      self.emit('CURTAIN', owner)
+      return 'int'
+    if isinstance(sl, ast.Constant) and sl.value in (0, 1) and not isinstance(sl.value, bool):
+      return self.component(base, sl.value, node)
+    self.refuse(node, 'this subscript')
+
+  def call(self, node):
+    f = node.func
+    if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS:
+      self.need(node, 'sprite', f.attr)
+      if (len(node.args) != 2 or node.keywords or not self.is_param(node.args[0], 'board') or
+          not self.is_param(node.args[1], 'the_plot')):
+        self.refuse(node, 'a motion helper not called as (board, the_plot)')
+      self.emit('MOVE', _MOTIONS[f.attr])
+      return 'motion'
+    if isinstance(f, ast.Name) and len(node.args) == 1 and not node.keywords:
+      arg = node.args[0]
+      if f.id == 'int':
+        self.scalar(arg)
+        return 'int'
+      if f.id == 'ord' and isinstance(arg, ast.Constant) and isinstance(arg.value, str) \
+          and len(arg.value) == 1:
+        self.emit('PUSH', ord(arg.value))
+        return 'int'
+      if f.id == 'chr':
+        self.scalar(arg)
+        return 'char'
+    if (isinstance(f, ast.Attribute) and self.is_param(f.value, 'the_plot') and f.attr == 'get'
+        and len(node.args) == 1 and not node.keywords and isinstance(node.args[0], ast.Constant)
+        and isinstance(node.args[0].value, str)):
+      self.emit('GETP', ('key', self.use_key(node.args[0].value)))
+      return 'int'
+    if isinstance(f, ast.Attribute) and f.attr == 'any' and not node.args and not node.keywords:
+      owner = self.curtain_owner(f.value)
+      if owner is not None:
+        self.emit('ANY', owner)
+        return 'int'
+    self.refuse(node, 'the call {}()'.format(ast.unparse(f)))
+
+  def literal_values(self, node, chars):
+    """Codes of a literal tuple / list / string for `in`; `chars`: the left side is chr()."""
+    if isinstance(node, ast.Constant) and isinstance(node.value, str):
+      if not chars:
+        self.refuse(node, '`in` a string on a number')
+      return [ord(c) for c in node.value]
+    if isinstance(node, (ast.Tuple, ast.List)):
+      out = []
+      for e in node.elts:
+        if chars and isinstance(e, ast.Constant) and isinstance(e.value, str) and len(e.value) == 1:
+          out.append(ord(e.value))
+        elif not chars and self.number(e) is not None and isinstance(self.number(e), int):
+          out.append(int(self.number(e)))
+        elif not chars and isinstance(e, ast.Constant) and isinstance(e.value, bool):
+          out.append(int(e.value))
+        else:
+          self.refuse(e, 'a non-literal or mismatched `in` element')
+      if len(out) > 64:
+        self.refuse(node, '`in` over more than 64 values')
+      return out
+    self.refuse(node, '`in` over something that is not a literal tuple, list or string')
+
+  def compare(self, node):
+    if len(node.ops) == 1:
+      self.compare1(node.left, node.ops[0], node.comparators[0], node)
+      return 'int'
+    end = self.label()
+    left = node.left
+    for i, (op, right) in enumerate(zip(node.ops, node.comparators)):
+      self.compare1(left, op, right, node)
+      if i < len(node.ops) - 1:
+        self.emit('DUP')
+        self.emit('JZ', end)
+        self.emit('POP')
+      left = right
+    self.place(end)
+    return 'int'
+
+  def compare1(self, left, op, right, node):
+    none = isinstance(right, ast.Constant) and right.value is None
+    if isinstance(op, (ast.Is, ast.IsNot)):
+      if not none:
+        self.refuse(node, '`is` against anything but None')
+      if self.is_param(left, 'actions'):
+        self.emit('ACTION')
+        self.emit('PUSH', _lib.ACTION_NONE)
+      else:
+        if self.expr(left) != 'motion':
+          self.refuse(node, '`is None` on anything but `actions` and motion results')
+        self.emit('PUSH', 0)
+      self.emit('EQ' if isinstance(op, ast.Is) else 'NE')
+      return
+    if self.is_param(right, 'actions') and isinstance(op, (ast.Eq, ast.NotEq)):
+      left, right = right, left
+    if self.is_param(left, 'actions'):
+      if isinstance(op, (ast.In, ast.NotIn)):
+        values = self.literal_values(right, False)
+        if any(v < 0 for v in values):
+          self.refuse(node, 'a negative action')
+        self.emit('ACTION')
+        self.emit('IN', len(values), *values)
+        if isinstance(op, ast.NotIn):
+          self.emit('NOT')
+        return
+      if not isinstance(op, (ast.Eq, ast.NotEq)):
+        self.refuse(node, 'an ordering comparison on `actions` (None on the first frame)')
+      value = self.number(right)
+      if value is None and isinstance(right, ast.Constant) and isinstance(right.value, bool):
+        value = int(right.value)
+      if not isinstance(value, int) or value < 0:
+        self.refuse(node, '`actions` against anything but a non-negative int literal')
+      self.emit('ACTION')
+      self.emit('PUSH', value)
+      self.emit('EQ' if isinstance(op, ast.Eq) else 'NE')
+      return
+    if isinstance(op, (ast.In, ast.NotIn)):
+      t = self.expr(left)
+      if t not in ('int', 'char'):
+        self.refuse(node, '`in` on a ' + _TYPE_NAMES[t])
+      values = self.literal_values(right, t == 'char')
+      self.emit('IN', len(values), *values)
+      if isinstance(op, ast.NotIn):
+        self.emit('NOT')
+      return
+    name = _CMPOPS[type(op)]
+    lp, rp = self.pos_parts(left), self.pos_parts(right)
+    if lp is not None and rp is not None and name in ('EQ', 'NE') and not (
+        isinstance(left, ast.Tuple) and isinstance(right, ast.Tuple)):
+      for part in lp + rp:
+        part()
+      self.emit('EQ2')
+      if name == 'NE':
+        self.emit('NOT')
+      return
+    if (isinstance(right, ast.Constant) and isinstance(right.value, str) and
+        len(right.value) == 1 and name in ('EQ', 'NE')):
+      if self.expr(left) != 'char':
+        self.refuse(node, 'a number compared with a string')
+      self.emit('PUSH', ord(right.value))
+      self.emit(name)
+      return
+    self.scalar(left)
+    self.scalar(right)
+    self.emit(name)
+
+
+# Attributes the prefabs keep for themselves (their state lives in the device records).
+_RESERVED = {
+    'sprite': {'_virtual_row', '_virtual_col', '_position', '_visible', '_prior_visible',
+               '_c_h_a_r_a_c_t_e_r', '_c_o_r_n_e_r', '_impassable', '_confined_to_board',
+               '_egocentric_scroller', '_scrolling_group'},
+    'drape': {'_c_u_r_t_a_i_n', '_c_h_a_r_a_c_t_e_r'},
+}
+
+
+# ------------------------------------------------------------------ linking
+
+def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys):
+  """Bytecode words for one game.  compiled: char -> `Compiled`; plot_keys: the key
+  order of the plot registers.  Entities of one class share their code."""
+  chars = list(sprite_chars) + list(drape_chars)
+  S = len(sprite_chars)
+  words = [len(chars)] + [0] * len(chars)
+  entry = {}
+  for i, ch in enumerate(chars):
+    comp = compiled[ch]
+    if comp.klass not in entry:
+      entry[comp.klass] = len(words)
+      words += _encode(comp, len(words), chars, S, rows, cols, plot_keys)
+    words[1 + i] = entry[comp.klass]
+  if len(words) > _lib.MAX_CODE_WORDS:
+    raise NotLoweredError('the compiled game needs {} code words, more than {}'.format(
+        len(words), _lib.MAX_CODE_WORDS))
+  return np.array(words, dtype=np.int32)
+
+
+def _encode(comp, base, chars, S, rows, cols, plot_keys):
+  addr, pc = {}, base
+  for ins in comp.ir:                 # pass 1: label addresses
+    if ins[0] == 'LABEL':
+      addr[ins[1]] = pc
+    else:
+      pc += len(ins)
+
+  def resolve(x, op):
+    if not isinstance(x, tuple):
+      return int(x)
+    if x[0] == 'label':
+      return addr[x[1]]
+    if x[0] == 'attr':
+      return comp.attrs.index(x[1])
+    if x[0] == 'key':
+      return plot_keys.index(x[1])
+    if x[0] == 'rows':
+      return rows
+    if x[0] == 'cols':
+      return cols
+    ch = x[1]                         # ('ent', ch)
+    if ch not in chars:
+      raise NotLoweredError('{}: things[{!r}] names no entity of the game'.format(
+          _name(comp.klass), ch))
+    k = chars.index(ch)
+    if (op == 'FIELD') != (k < S):
+      raise NotLoweredError('{}: things[{!r}] is not a {}'.format(
+          _name(comp.klass), ch, 'sprite' if op == 'FIELD' else 'drape'))
+    return k
+
+  out = []
+  for ins in comp.ir:                 # pass 2: words
+    if ins[0] != 'LABEL':
+      out.append(_lib.OP[ins[0]])
+      out += [resolve(x, ins[0]) for x in ins[1:]]
+  return out

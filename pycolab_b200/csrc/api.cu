@@ -28,6 +28,12 @@ struct pcl_handle {
   cudaEvent_t ev_done[PCL_HOST_SLOTS];   // host buffers of that slot are valid (copy stream)
   int host_ready;
   int pending_slot;              // slot of this handle's last async step whose D2H may still run, or -1
+  // pcl_bind_code: the checked host words, and their device copy made at the next launch
+  int32_t* code_host;
+  int code_words;
+  int32_t* code_dev;
+  int code_dev_words;            // words the device buffer holds room for
+  int code_stale;                // code_host changed since the upload
 };
 
 namespace {
@@ -78,6 +84,7 @@ const struct {
     {PCL_PROG_APPREHEND, &pcl::kApprehend},
     {PCL_PROG_SHOCKWAVE, &pcl::kShockwave},
     {PCL_PROG_T_MAZE, &pcl::kTMaze},
+    {PCL_PROG_COMPILED, &pcl::kCompiled},
 };
 
 // The descriptor of program `id`, or nullptr for an id this build does not know.
@@ -132,6 +139,7 @@ void fill_params(const pcl_handle* h, StepParams* p) {
   memcpy(p->group_len, s.group_len, sizeof(p->group_len));
   memcpy(p->group_chars, s.group_chars, sizeof(p->group_chars));
   p->st = h->st;
+  p->code = h->code_dev;
 }
 
 int launch(pcl_handle* h, const StepParams& p, cudaStream_t stream) {
@@ -154,12 +162,44 @@ bool outputs_set(const pcl_outputs& out) {
   return out.d_reward && out.d_has_reward && out.d_discount && out.d_done;
 }
 
-int check_ready(const pcl_handle* h, const pcl_outputs* out) {
+// Are this handle's rewards float64 (pcl_outputs.d_reward_f64)?
+bool float_rewards(const pcl_handle* h) {
+  return h->program->float_reward || (h->program->float_reward_arg0 && h->spec.program_arg[0]);
+}
+
+// Copy the bound bytecode to the device if it changed since the last launch, in order on
+// `s` (the stream of the launch about to use it), and wait for the copy: once this
+// returns, a launch on any stream reads complete code.  Rebinding first waits for the
+// device, so no kernel still running the old code sees its buffer change.  The copy
+// carries two zero words more, so the kernel may read an operand word past a final RET.
+int upload_code(pcl_handle* h, cudaStream_t s) {
+  if (!h->code_stale) return PCL_OK;
+  if (h->code_dev) PCL_CUDA(h, cudaDeviceSynchronize());
+  if (h->code_dev_words < h->code_words + 2) {
+    if (h->code_dev) PCL_CUDA(h, cudaFree(h->code_dev));
+    h->code_dev = nullptr;
+    h->code_dev_words = 0;
+    h->base.code = nullptr;
+    PCL_CUDA(h, cudaMalloc(&h->code_dev, (h->code_words + 2) * sizeof(int32_t)));
+    h->code_dev_words = h->code_words + 2;
+  }
+  PCL_CUDA(h, cudaMemsetAsync(h->code_dev, 0, h->code_dev_words * sizeof(int32_t), s));
+  PCL_CUDA(h, cudaMemcpyAsync(h->code_dev, h->code_host, h->code_words * sizeof(int32_t),
+                              cudaMemcpyHostToDevice, s));
+  PCL_CUDA(h, cudaStreamSynchronize(s));
+  h->base.code = h->code_dev;
+  h->code_stale = 0;
+  return PCL_OK;
+}
+
+// Everything a step or reset on `s` needs is in place; uploads bound code on the way.
+int check_ready(pcl_handle* h, const pcl_outputs* out, cudaStream_t s) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
+  if (h->program->check_code && !h->code_host) return PCL_ERR_UNBOUND;
   if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
-  if (h->program->float_reward && !out->d_reward_f64) return PCL_ERR_INVALID;
-  return PCL_OK;
+  if (float_rewards(h) && !out->d_reward_f64) return PCL_ERR_INVALID;
+  return h->program->check_code ? upload_code(h, s) : PCL_OK;
 }
 
 __global__ void gather_errors(const int32_t* plot, int32_t* out, int B) {
@@ -186,7 +226,7 @@ const char* pcl_status_string(int status) {
     case PCL_ERR_INVALID: return "invalid argument or malformed spec";
     case PCL_ERR_UNSUPPORTED: return "game not lowered to a device program";
     case PCL_ERR_CUDA: return "CUDA runtime error";
-    case PCL_ERR_UNBOUND: return "pcl_bind_state has not been called";
+    case PCL_ERR_UNBOUND: return "pcl_bind_state (or, for PCL_PROG_COMPILED, pcl_bind_code) has not been called";
     case PCL_ERR_NOMEM: return "out of memory";
     default: return "unknown status";
   }
@@ -209,6 +249,11 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->last_error[0] = 0;
   h->host_ready = 0;
   h->pending_slot = -1;
+  h->code_host = nullptr;
+  h->code_words = 0;
+  h->code_dev = nullptr;
+  h->code_dev_words = 0;
+  h->code_stale = 0;
   *out = h;
   return PCL_OK;
 }
@@ -220,6 +265,10 @@ int pcl_destroy(pcl_handle* h) {
       cudaEventDestroy(h->ev_done[i]);
     }
     cudaStreamDestroy(h->copy_stream);
+  }
+  if (h) {
+    if (h->code_dev) cudaFree(h->code_dev);
+    delete[] h->code_host;
   }
   delete h;
   return PCL_OK;
@@ -244,9 +293,25 @@ int pcl_bind_state(pcl_handle* h, const pcl_state* st) {
   return PCL_OK;
 }
 
+int pcl_bind_code(pcl_handle* h, const int32_t* h_code, int32_t n_words) {
+  if (!h || !h_code) return PCL_ERR_INVALID;
+  if (!h->program->check_code) return PCL_ERR_UNSUPPORTED;
+  if (n_words < 1 || n_words > PCL_MAX_CODE_WORDS) return PCL_ERR_INVALID;
+  const int r = h->program->check_code(h->spec, h_code, n_words);
+  if (r != PCL_OK) return r;
+  int32_t* copy = new (std::nothrow) int32_t[n_words];
+  if (!copy) return PCL_ERR_NOMEM;
+  memcpy(copy, h_code, n_words * sizeof(int32_t));
+  delete[] h->code_host;
+  h->code_host = copy;
+  h->code_words = n_words;
+  h->code_stale = 1;
+  return PCL_OK;
+}
+
 int pcl_reset(pcl_handle* h, const uint8_t* d_env_mask, const pcl_outputs* out, void* stream) {
   Range nvtx_range("pcl_reset (Engine.its_showtime)");
-  const int r = check_ready(h, out);
+  const int r = check_ready(h, out, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
   StepParams p = h->base;
   p.mode = pcl::MODE_RESET;
@@ -257,7 +322,7 @@ int pcl_reset(pcl_handle* h, const uint8_t* d_env_mask, const pcl_outputs* out, 
 
 int pcl_step(pcl_handle* h, const int32_t* d_actions, const pcl_outputs* out, void* stream) {
   Range nvtx_range("pcl_step (Engine.play)");
-  const int r = check_ready(h, out);
+  const int r = check_ready(h, out, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
   if (!d_actions) return PCL_ERR_INVALID;
   StepParams p = h->base;
@@ -270,7 +335,7 @@ int pcl_step(pcl_handle* h, const int32_t* d_actions, const pcl_outputs* out, vo
 int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
             void* stream) {
   Range nvtx_range("pcl_run");
-  const int r = check_ready(h, out);
+  const int r = check_ready(h, out, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
   if (!d_actions || steps < 0) return PCL_ERR_INVALID;
   StepParams p = h->base;
@@ -289,7 +354,7 @@ int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const
   Range nvtx_range("pcl_run_many");
   if (!handles || !d_actions || !outs || n_handles < 1 || steps < 0) return PCL_ERR_INVALID;
   for (int i = 0; i < n_handles; ++i) {
-    const int r = check_ready(handles[i], outs[i]);
+    const int r = check_ready(handles[i], outs[i], (cudaStream_t)stream);
     if (r != PCL_OK) return r;
   }
   for (int t = 0; t < steps; ++t) {
@@ -347,9 +412,9 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
                   const pcl_outputs* out, uint8_t* h_board, int32_t* h_reward,
                   uint8_t* h_has_reward, float* h_discount, uint8_t* h_done, void* stream) {
   Range nvtx_range("pcl_step_host");
-  const int r = check_ready(h, out);
+  const int r = check_ready(h, out, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
-  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions) return PCL_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t plane = (size_t)h->spec.rows * h->spec.pitch;
@@ -368,9 +433,9 @@ int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_acti
                         uint8_t* h_has_reward, float* h_discount, uint8_t* h_done, int slot,
                         void* stream) {
   Range nvtx_range("pcl_step_host_async");
-  const int r = check_ready(h, out);
+  const int r = check_ready(h, out, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
-  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions || slot < 0 || slot >= PCL_HOST_SLOTS) return PCL_ERR_INVALID;
   if (crop && !d_crop) return PCL_ERR_INVALID;
   int e = host_pipeline_ready(h);
@@ -587,7 +652,7 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   if (!h || !crop || !d_board || !out || !x) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
   if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape tracking: pcl_crop_tracking
@@ -621,7 +686,7 @@ int pcl_pack_handoff(pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
                      const pcl_outputs* out, uint8_t* d_packed, void* stream) {
   if (!h || !d_view || !out || !d_packed || view_bytes <= 0) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;
@@ -637,7 +702,7 @@ int pcl_pack_handoff_peers(pcl_handle* h, const uint8_t* d_view, int32_t view_by
     return PCL_ERR_INVALID;
   if (n_peers < 1 || n_peers > PCL_MAX_PEERS) return PCL_ERR_INVALID;
   if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (h->program->float_reward) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
   pcl::PackParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.view_bytes = view_bytes;

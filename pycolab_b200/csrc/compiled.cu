@@ -1,0 +1,533 @@
+// compiled.cu — the compiled step program: MazeWalkers and plain drapes whose update()
+// bodies `pycolab_b200.compiler` translated into the bytecode of include/pcl.h (PCL_OP_*).
+//
+// The kernel is fixture.cu's frame — one warp per env, a real board in shared memory,
+// rendered after every update group (engine.py:725-735) — with an interpreter where the
+// fixture reads precomputed motions: each entity runs its class's code over the records
+// in shared memory.  Interpretation is warp-uniform: every lane runs the same
+// instruction on the same values, and the operand stack and locals live in shared
+// memory.  The lanes split up only for a render, a walker's neighbourhood, a curtain
+// fill and a curtain's any().
+//
+// Semantics restated from upstream:
+//   - update() runs on the its_showtime() frame too, with actions=None (engine.py:581);
+//   - another entity's record is read as it is now; a curtain write shows in reads at
+//     once and on the board at the next render;
+//   - Plot directives apply in call order: rewards sum (plot.py:201-214), the last
+//     discount-setting call wins, terminate_episode() does not stop later updates.
+#include "pcl_board.cuh"
+
+#include <vector>
+
+namespace pcl {
+
+namespace {
+
+constexpr int kWarpsPerBlock = 2;
+using board::Ctx;
+using board::WarpState;
+
+// The operand stack and locals, in shared memory, one per warp.  Every lane keeps its
+// own copy of each slot (slot i of lane l is word i * 32 + l, so the lanes hit 32
+// different banks): a lane only ever reads back what it wrote itself, and nothing
+// depends on the warp staying converged between instructions.
+struct Vm {
+  int32_t stack[PCL_CODE_STACK][32];
+  int32_t local[PCL_CODE_LOCALS][32];
+};
+
+// One lane's view of a column of Vm slots.
+struct LaneSlots {
+  int32_t* base;                     // slot 0 of this lane
+  __device__ __forceinline__ int32_t& operator[](int i) const { return base[i * 32]; }
+};
+
+// Operand words of opcode `op` (PCL_OP_IN has its count more).
+__host__ __device__ __forceinline__ int op_operands(int op) {
+  switch (op) {
+    case PCL_OP_FIELD: case PCL_OP_REWARD_F64: return 2;
+    case PCL_OP_PUSH: case PCL_OP_LOAD: case PCL_OP_STORE: case PCL_OP_JMP: case PCL_OP_JZ:
+    case PCL_OP_JNZ: case PCL_OP_IN: case PCL_OP_GETR: case PCL_OP_SETR: case PCL_OP_GETP:
+    case PCL_OP_SETP: case PCL_OP_CURTAIN: case PCL_OP_ANY: case PCL_OP_MOVE:
+    case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: return 1;
+    default: return 0;
+  }
+}
+
+// Stack effect of each opcode (host side: pcl_bind_code's depth check).
+struct OpInfo { int8_t pops, pushes; };
+constexpr OpInfo kOps[PCL_OP_COUNT] = {
+    {0, 0},  // RET
+    {0, 1},  // PUSH
+    {1, 0},  // POP
+    {1, 2},  // DUP
+    {0, 1},  // LOAD
+    {1, 0},  // STORE
+    {0, 0},  // JMP
+    {1, 0},  // JZ
+    {1, 0},  // JNZ
+    {2, 1}, {2, 1}, {2, 1},            // ADD SUB MUL
+    {2, 1}, {2, 1},                       // FLOORDIV MOD
+    {2, 1}, {2, 1}, {2, 1}, {2, 1}, {2, 1}, {2, 1},   // EQ .. GE
+    {1, 1}, {1, 1},                       // NEG NOT
+    {4, 1},  // EQ2
+    {1, 1},  // IN (+ its values)
+    {0, 1},  // ACTION
+    {0, 1},  // FRAME
+    {0, 1},  // FIELD
+    {0, 1},  // GETR
+    {1, 0},  // SETR
+    {0, 1},  // GETP
+    {1, 0},  // SETP
+    {2, 1},  // BOARD
+    {2, 1},  // BACKDROP
+    {2, 1},  // CURTAIN
+    {3, 0},  // SETCELL
+    {1, 0},  // FILL
+    {0, 1},  // ANY
+    {0, 1},  // MOVE
+    {2, 0},  // TELEPORT
+    {1, 0},  // REWARD
+    {0, 0},  // REWARD_F64
+    {0, 0},  // TERMINATE
+    {0, 0},  // DISCOUNT
+};
+constexpr int kMaxIn = 64;
+
+// Python's // and % (floor semantics) on int32 operands, b != 0.
+__device__ __forceinline__ int floordiv(int a, int b) {
+  const long long q = (long long)a / b, r = (long long)a % b;
+  return (int)((r != 0 && ((r < 0) != (b < 0))) ? q - 1 : q);
+}
+__device__ __forceinline__ int floormod(int a, int b) {
+  const long long r = (long long)a % b;
+  return (int)((r != 0 && ((r < 0) != (b < 0))) ? r + b : r);
+}
+
+// NumPy's rule for one index into an axis of n cells: one negative wrap, else in range.
+__device__ __forceinline__ bool cell_index(int& i, int n) {
+  if (i < 0) i += n;
+  return (unsigned)i < (unsigned)n;
+}
+
+// Valid curtain bits of word w of a bit row of W cells.
+__device__ __forceinline__ uint32_t row_word_mask(int w, int W) {
+  const int first = w * 32;
+  if (first >= W) return 0u;
+  return W - first >= 32 ? 0xffffffffu : (1u << (W - first)) - 1u;
+}
+
+struct Rewards {
+  int has;
+  int sum_i;
+  double sum_f;
+};
+
+// The update() of entity `ent` (sprites first, then drapes).
+__device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot,
+                           Directives& dir, Rewards& rw) {
+  const StepParams& p = *c.p;
+  WarpState* st = c.st;
+  const int S = p.S, H = p.H, W = p.W, lane = c.lane;
+  const int32_t* code = p.code;
+  const bool is_sprite = ent < S;
+  int32_t* regs = is_sprite ? &st->sprites[ent][PCL_S_AUX0] : st->drapes[ent - S];
+  const LaneSlots stk = {&vm->stack[0][lane]};
+  const LaneSlots loc = {&vm->local[0][lane]};
+  int sp = 0;
+  int pc = __ldg(code + 1 + ent);
+  for (int i = 0; i < PCL_CODE_LOCALS; ++i) loc[i] = 0;
+  for (;;) {
+    const int op = __ldg(code + pc);
+    const int a = __ldg(code + pc + 1);      // first operand (the device copy is padded)
+    int next = pc + 1 + op_operands(op);
+    switch (op) {
+      case PCL_OP_RET: return;
+      case PCL_OP_PUSH: stk[sp++] = a; break;
+      case PCL_OP_POP: --sp; break;
+      case PCL_OP_DUP: stk[sp] = stk[sp - 1]; ++sp; break;
+      case PCL_OP_LOAD: stk[sp++] = loc[a]; break;
+      case PCL_OP_STORE: loc[a] = stk[--sp]; break;
+      case PCL_OP_JMP: next = a; break;
+      case PCL_OP_JZ: if (stk[--sp] == 0) next = a; break;
+      case PCL_OP_JNZ: if (stk[--sp] != 0) next = a; break;
+      case PCL_OP_ADD: case PCL_OP_SUB: case PCL_OP_MUL: case PCL_OP_FLOORDIV: case PCL_OP_MOD:
+      case PCL_OP_EQ: case PCL_OP_NE: case PCL_OP_LT: case PCL_OP_LE: case PCL_OP_GT:
+      case PCL_OP_GE: {
+        const int y = stk[--sp], x = stk[sp - 1];
+        const unsigned ux = (unsigned)x, uy = (unsigned)y;   // wrapping arithmetic
+        int v = 0;
+        switch (op) {
+          case PCL_OP_ADD: v = (int)(ux + uy); break;
+          case PCL_OP_SUB: v = (int)(ux - uy); break;
+          case PCL_OP_MUL: v = (int)(ux * uy); break;
+          case PCL_OP_FLOORDIV:
+          case PCL_OP_MOD:
+            if (y == 0) plot.error |= PCL_ENV_ERR_ARITH;
+            else v = op == PCL_OP_MOD ? floormod(x, y) : floordiv(x, y);
+            break;
+          case PCL_OP_EQ: v = x == y; break;
+          case PCL_OP_NE: v = x != y; break;
+          case PCL_OP_LT: v = x < y; break;
+          case PCL_OP_LE: v = x <= y; break;
+          case PCL_OP_GT: v = x > y; break;
+          default: v = x >= y; break;
+        }
+        stk[sp - 1] = v;
+        break;
+      }
+      case PCL_OP_NEG: stk[sp - 1] = (int)(0u - (unsigned)stk[sp - 1]); break;
+      case PCL_OP_NOT: stk[sp - 1] = stk[sp - 1] == 0; break;
+      case PCL_OP_EQ2: {
+        sp -= 3;
+        stk[sp - 1] = stk[sp - 1] == stk[sp + 1] && stk[sp] == stk[sp + 2];
+        break;
+      }
+      case PCL_OP_IN: {
+        const int x = stk[sp - 1];
+        int hit = 0;
+        for (int k = 0; k < a; ++k) hit |= __ldg(code + pc + 2 + k) == x;
+        stk[sp - 1] = hit;
+        next += a;
+        break;
+      }
+      case PCL_OP_ACTION: stk[sp++] = action; break;
+      case PCL_OP_FRAME: stk[sp++] = plot.frame; break;
+      case PCL_OP_FIELD: {
+        const int32_t* rec = st->sprites[a < 0 ? ent : a];
+        const int f = __ldg(code + pc + 2);
+        stk[sp++] = f == 4 ? (rec[PCL_S_FLAGS] & 1) : rec[f];
+        break;
+      }
+      case PCL_OP_GETR: stk[sp++] = regs[a]; break;
+      case PCL_OP_SETR: {
+        const int v = stk[--sp];
+        __syncwarp();
+        if (lane == 0) regs[a] = v;
+        __syncwarp();
+        break;
+      }
+      case PCL_OP_GETP: stk[sp++] = st->plot[PCL_P_AUX0 + a]; break;
+      case PCL_OP_SETP: {
+        const int v = stk[--sp];
+        __syncwarp();
+        if (lane == 0) st->plot[PCL_P_AUX0 + a] = v;
+        __syncwarp();
+        break;
+      }
+      case PCL_OP_BOARD: case PCL_OP_BACKDROP: case PCL_OP_CURTAIN: {
+        int col = stk[--sp], r = stk[sp - 1];
+        int v = 0;
+        if (cell_index(r, H) && cell_index(col, W)) {
+          if (op == PCL_OP_BOARD) v = c.board[r * p.pitch + col];
+          else if (op == PCL_OP_BACKDROP) v = c.backdrop[(int64_t)r * p.pitch + col];
+          else v = bit_at(board::bits_row(c, (a < 0 ? ent : a) - S, r), col);
+        } else {
+          plot.error |= PCL_ENV_ERR_INDEX;
+        }
+        stk[sp - 1] = v;
+        break;
+      }
+      case PCL_OP_SETCELL: {
+        sp -= 3;
+        const int v = stk[sp + 2];
+        int r = stk[sp], col = stk[sp + 1];
+        if (cell_index(r, H) && cell_index(col, W)) {
+          uint32_t* row = board::bits_row(c, ent - S, r);
+          __syncwarp();
+          if (lane == 0) {
+            const uint32_t bit = 1u << (col & 31);
+            row[col >> 5] = v ? (row[col >> 5] | bit) : (row[col >> 5] & ~bit);
+          }
+          __syncwarp();
+        } else {
+          plot.error |= PCL_ENV_ERR_INDEX;
+        }
+        break;
+      }
+      case PCL_OP_FILL: {
+        const int v = stk[--sp];
+        __syncwarp();
+        for (int i = lane; i < H * p.BW; i += 32) {
+          const int r = i / p.BW, w = i - r * p.BW;
+          board::bits_row(c, ent - S, r)[w] = v ? row_word_mask(w, W) : 0u;
+        }
+        __syncwarp();
+        break;
+      }
+      case PCL_OP_ANY: {
+        const int d = (a < 0 ? ent : a) - S;
+        bool any = false;
+        for (int i = lane; i < H * p.BW; i += 32) {
+          const int r = i / p.BW, w = i - r * p.BW;
+          any |= board::bits_row(c, d, r)[w] != 0u;
+        }
+        stk[sp++] = __any_sync(PCL_FULL, any) ? 1 : 0;
+        break;
+      }
+      case PCL_OP_MOVE: {
+        Sprite s = board::load_sprite(st->sprites[ent]);
+        const uint32_t* imp = st->impassable[ent];
+        const uint8_t* bd = c.board;
+        const int pitch = p.pitch;
+        const bool moved = walker_move(s, ent, a, plot, H, W, p.confined[ent] != 0, false, lane,
+                                       [&](int r, int col) { return in_set(imp, bd[r * pitch + col]); });
+        board::store_sprite(st->sprites[ent], s, lane);
+        stk[sp++] = moved ? 0 : 1;
+        break;
+      }
+      case PCL_OP_TELEPORT: {
+        sp -= 2;
+        Sprite s = board::load_sprite(st->sprites[ent]);
+        walker_teleport(s, H, W, stk[sp], stk[sp + 1]);
+        board::store_sprite(st->sprites[ent], s, lane);
+        break;
+      }
+      case PCL_OP_REWARD: case PCL_OP_REWARD_F64: {
+        const int x = op == PCL_OP_REWARD ? stk[--sp] : 0;
+        const double f = op == PCL_OP_REWARD ? (double)x
+                                             : __hiloint2double(__ldg(code + pc + 2), a);
+        rw.sum_f = rw.has ? rw.sum_f + f : f;    // Python's `None`, then `reward + r`
+        rw.sum_i = (int)((unsigned)rw.sum_i + (unsigned)x);
+        rw.has = 1;
+        break;
+      }
+      case PCL_OP_TERMINATE: terminate(dir, __int_as_float(a)); break;
+      default: change_default_discount(dir, __int_as_float(a)); break;   // PCL_OP_DISCOUNT
+    }
+    pc = next;
+  }
+}
+
+__global__ void __launch_bounds__(kWarpsPerBlock * 32)
+compiled_step(const StepParams p) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int env = blockIdx.x * kWarpsPerBlock + warp;
+  if (env >= p.B) return;
+  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
+  const int H = p.H, S = p.S, D = p.D, n = S + D;
+  const size_t board_bytes = board::board_bytes(H, p.pitch);
+  uint8_t* my = smem_raw + warp * (sizeof(WarpState) + sizeof(Vm) + board_bytes);
+  WarpState* st = reinterpret_cast<WarpState*>(my);
+  Vm* vm = reinterpret_cast<Vm*>(my + sizeof(WarpState));
+  Ctx c;
+  c.p = &p; c.st = st; c.board = my + sizeof(WarpState) + sizeof(Vm);
+  c.backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
+  c.env = env; c.lane = lane; c.lvl = lvl;
+
+  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
+  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * D * PCL_DRAPE_WORDS;
+  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
+  uint8_t* g_z = p.st.d_z_order + (int64_t)env * n;
+  uint8_t* g_board = p.out.d_board + (int64_t)env * H * p.pitch;
+
+  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  if (run == ENV_SKIP) return;
+  const bool restart = run == ENV_RESTART;
+  const PlotCarry carry = plot_carry(g_plot, restart);
+  board::stage_records(
+      st, restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprites,
+      restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes,
+      restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot,
+      restart ? p.st.d_z_order_init + lvl * p.st.z_order_init_bstride : g_z, S, D, lane);
+  for (int i = lane; i < S * 4; i += 32) (&st->impassable[0][0])[i] = p.impassable[i >> 2][i & 3];
+  if (restart) {
+    // A restart rebuilds every plain curtain from its template (things.py:146-217).
+    for (int d = 0; d < D; ++d) {
+      const uint32_t* src = p.st.d_bits_init[d] + lvl * p.st.bits_init_bstride[d];
+      uint32_t* dst = p.st.d_bits[d] + (int64_t)env * p.st.bits_bstride[d];
+      for (int i = lane; i < H * p.BW; i += 32) dst[i] = src[i];
+    }
+  }
+  __syncwarp();
+  if (restart) {
+    if (lane == 0) store_carry(st->plot, carry);
+    __syncwarp();
+  }
+  // Zero the board's pitch padding too: the whole H * pitch plane goes out to d_board.
+  for (int i = lane; i < (int)board_bytes; i += 32) c.board[i] = 0;
+  __syncwarp();
+  board::stage_board(c, restart, g_board);
+
+  Plot plot;
+  plot.frame = st->plot[PCL_P_FRAME] + 1;    // engine.py:716
+  plot.error = st->plot[PCL_P_ERROR];
+  plot.order_r = st->plot[PCL_P_ORDER_R]; plot.order_c = st->plot[PCL_P_ORDER_C];
+  plot.order_frame = st->plot[PCL_P_ORDER_FRAME]; plot.ego_mask = st->plot[PCL_P_EGO_MASK];
+  Directives dir = fresh_directives();
+  Rewards rw = {0, 0, 0.0};
+  const int action = restart ? PCL_ACTION_NONE : p.actions[(int64_t)env * p.actions_per_env];
+
+  // ---- update groups (engine.py:725-735)
+  int k = 0;
+  for (int g = 0; g < p.n_groups; ++g) {
+    for (int e = 0; e < p.group_len[g]; ++e, ++k) {
+      const int ch = p.group_chars[k];
+      int ent = 0;
+      for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
+      for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
+      run_update(c, vm, ent, action, plot, dir, rw);
+    }
+    board::render(c);
+  }
+
+  __syncwarp();
+  if (lane == 0) {
+    st->plot[PCL_P_FRAME] = plot.frame; st->plot[PCL_P_GAME_OVER] = dir.game_over;
+    st->plot[PCL_P_ERROR] = plot.error;
+    if (p.program_arg[0]) p.out.d_reward_f64[env] = rw.has ? rw.sum_f : 0.0;
+    else p.out.d_reward[env] = rw.has ? rw.sum_i : 0;
+    p.out.d_has_reward[env] = (uint8_t)rw.has;
+    p.out.d_discount[env] = dir.discount;
+    p.out.d_done[env] = (uint8_t)dir.game_over;
+  }
+  __syncwarp();
+  board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
+}
+
+// MazeWalkers (default scrolling group, not egocentric) and plain drapes; the entities
+// and the z-order are consistent permutations of each other.
+int check_spec(const pcl_spec& s) {
+  const int n = s.n_sprites + s.n_drapes;
+  if (n < 1) return PCL_ERR_INVALID;
+  if (s.n_groups < 1 || s.n_groups > board::kMaxEnt) return PCL_ERR_INVALID;
+  int total = 0;
+  for (int g = 0; g < s.n_groups; ++g) total += s.group_len[g];
+  if (total != n) return PCL_ERR_INVALID;
+  for (int i = 0; i < n; ++i) {
+    int in_z = 0, in_groups = 0;
+    const uint8_t ch = i < s.n_sprites ? s.sprite_char[i] : s.drape_char[i - s.n_sprites];
+    for (int k = 0; k < n; ++k) {
+      in_z += s.z_order[k] == ch;
+      in_groups += s.group_chars[k] == ch;
+    }
+    if (in_z != 1 || in_groups != 1 || ch == 0 || ch > 127) return PCL_ERR_INVALID;
+  }
+  for (int i = 0; i < s.n_sprites; ++i)
+    if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
+  for (int d = 0; d < s.n_drapes; ++d)
+    if (s.drape_kind[d]) return PCL_ERR_UNSUPPORTED;
+  if (s.program_arg[0] != 0 && s.program_arg[0] != 1) return PCL_ERR_INVALID;
+  if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+int check_state(const pcl_spec& s, const pcl_state& st) {
+  if (!st.d_z_order || !st.d_z_order_init) return PCL_ERR_INVALID;
+  for (int d = 0; d < s.n_drapes; ++d)
+    if (!st.d_bits[d] || !st.d_bits_init[d]) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+// The checks pcl_bind_code promises (include/pcl.h): after them the kernel can run any
+// entity's code without a bounds test.
+int check_code(const pcl_spec& s, const int32_t* w, int n) {
+  const int S = s.n_sprites, ents = s.n_sprites + s.n_drapes, body = 1 + ents;
+  if (n <= body || n > PCL_MAX_CODE_WORDS || w[0] != ents) return PCL_ERR_INVALID;
+  enum { kNone = 0, kSprite = 1, kDrape = 2 };
+  std::vector<int8_t> starts(n, kNone);          // kind of the function starting at a word
+  for (int i = 0; i < ents; ++i) {
+    const int e = w[1 + i], kind = i < S ? kSprite : kDrape;
+    if (e < body || e >= n) return PCL_ERR_INVALID;
+    if (starts[e] != kNone && starts[e] != kind) return PCL_ERR_INVALID;
+    starts[e] = (int8_t)kind;
+  }
+  if (starts[body] == kNone) return PCL_ERR_INVALID;
+  std::vector<int> depth(n, -1);                 // stack depth on arrival, -1 = unreachable
+  std::vector<int8_t> boundary(n, 0);
+  std::vector<int> targets;
+  int kind = kNone, end = 0;
+  for (int pc = body; pc < n;) {
+    if (starts[pc] != kNone) {                   // a new function
+      kind = starts[pc];
+      for (end = pc + 1; end < n && starts[end] == kNone; ++end) {}
+      depth[pc] = 0;
+    }
+    boundary[pc] = 1;
+    const int op = w[pc];
+    if (op < 0 || op >= PCL_OP_COUNT) return PCL_ERR_INVALID;
+    int len = 1 + op_operands(op);
+    if (pc + len > end) return PCL_ERR_INVALID;
+    const int a = len > 1 ? w[pc + 1] : 0;
+    const bool sprite = kind == kSprite;
+    switch (op) {
+      case PCL_OP_LOAD: case PCL_OP_STORE:
+        if (a < 0 || a >= PCL_CODE_LOCALS) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_JMP: case PCL_OP_JZ: case PCL_OP_JNZ:
+        if (a <= pc || a >= end) return PCL_ERR_INVALID;
+        targets.push_back(a);
+        break;
+      case PCL_OP_IN:
+        if (a < 0 || a > kMaxIn) return PCL_ERR_INVALID;
+        len += a;
+        if (pc + len > end) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_FIELD:
+        if (a < 0 ? !sprite : a >= S) return PCL_ERR_INVALID;
+        if (w[pc + 2] < 0 || w[pc + 2] > 4) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_GETR: case PCL_OP_SETR:
+        if (a < 0 || a >= (sprite ? 3 : PCL_DRAPE_WORDS)) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_GETP: case PCL_OP_SETP:
+        if (a < 0 || a >= 4) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_CURTAIN: case PCL_OP_ANY:
+        if (a < 0 ? sprite : (a < S || a >= ents)) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_SETCELL: case PCL_OP_FILL:
+        if (sprite) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_MOVE:
+        if (!sprite || a < 0 || a > PCL_M_STAY) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_TELEPORT:
+        if (!sprite) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_REWARD_F64:
+        if (!s.program_arg[0]) return PCL_ERR_INVALID;   // an int32 reward cannot carry it
+        break;
+      default: break;
+    }
+    const int d = depth[pc];
+    if (d >= 0) {
+      if (d < kOps[op].pops) return PCL_ERR_INVALID;
+      const int after = d - kOps[op].pops + kOps[op].pushes;
+      if (after > PCL_CODE_STACK) return PCL_ERR_INVALID;
+      auto arrive = [&](int t) {
+        if (depth[t] >= 0 && depth[t] != after) return false;
+        depth[t] = after;
+        return true;
+      };
+      if ((op == PCL_OP_JMP || op == PCL_OP_JZ || op == PCL_OP_JNZ) && !arrive(a))
+        return PCL_ERR_INVALID;
+      if (op != PCL_OP_RET && op != PCL_OP_JMP) {
+        if (pc + len >= end) return PCL_ERR_INVALID;   // falls off the end of its function
+        if (!arrive(pc + len)) return PCL_ERR_INVALID;
+      }
+    }
+    pc += len;
+  }
+  for (int t : targets)
+    if (!boundary[t]) return PCL_ERR_INVALID;
+  return PCL_OK;
+}
+
+int actions_per_env(const pcl_spec&) { return 1; }
+
+cudaError_t launch(const StepParams& p, cudaStream_t s) {
+  const size_t smem = (sizeof(WarpState) + sizeof(Vm) + board::board_bytes(p.H, p.pitch)) *
+                      kWarpsPerBlock;
+  return launch_step(compiled_step, p, kWarpsPerBlock, smem, s);
+}
+
+}  // namespace
+
+const Program kCompiled = {check_spec, check_state, curtain_bits, launch, actions_per_env,
+                           /*float_reward=*/false, /*crop_epilogue=*/false,
+                           /*scroll_groups=*/false, check_code, /*float_reward_arg0=*/true};
+
+}  // namespace pcl

@@ -22,26 +22,19 @@
 // in order, i.e. in the order the entities issued them (include/pcl.h PCL_DIR_*):
 // add_reward(int), terminate_episode(f32 discount), change_default_discount(f32),
 // change_z_order(move_this | in_front_of << 8).
-#include "pcl_device.cuh"
-#include "pcl_kernels.cuh"
+#include "pcl_board.cuh"
 
 namespace pcl {
 
 namespace {
 
 constexpr int kWarpsPerBlock = 2;
-constexpr int kMaxEnt = PCL_MAX_SPRITES + PCL_MAX_DRAPES;
-
-struct WarpState {                   // lives in shared memory, one per warp
-  int32_t sprites[PCL_MAX_SPRITES][PCL_SPRITE_WORDS];
-  int32_t drapes[PCL_MAX_DRAPES][PCL_DRAPE_WORDS];
-  int32_t plot[PCL_PLOT_WORDS];
-  uint32_t impassable[PCL_MAX_SPRITES][4];
-  // One record per scrolling group (protocols/scrolling.py:198-241): the group an
-  // entity belongs to is swapped into the `Plot` registers around its update.
-  int32_t groups[PCL_MAX_SCROLL_GROUPS][PCL_GROUP_WORDS];
-  uint8_t z[kMaxEnt + 8];
-};
+using board::kMaxEnt;
+using board::WarpState;
+using board::Ctx;
+using board::render;
+using board::load_sprite;
+using board::store_sprite;
 
 // The order / egocentric-set registers of scrolling group g <-> `plot`.
 __device__ __forceinline__ void group_in(Plot& plot, const WarpState* st, int g) {
@@ -55,64 +48,6 @@ __device__ __forceinline__ void group_out(const Plot& plot, WarpState* st, int g
     st->groups[g][PCL_G_ORDER_R] = plot.order_r; st->groups[g][PCL_G_ORDER_C] = plot.order_c;
     st->groups[g][PCL_G_ORDER_FRAME] = plot.order_frame;
     st->groups[g][PCL_G_EGO_MASK] = plot.ego_mask;
-  }
-  __syncwarp();
-}
-
-struct Ctx {
-  const StepParams* p;
-  WarpState* st;
-  uint8_t* board;                    // smem, H * pitch
-  const uint8_t* backdrop;
-  int env, lane;
-  int64_t lvl;                       // index of static level data
-};
-
-__device__ __forceinline__ bool drape_bit(const Ctx& c, int d, int r, int col) {
-  const StepParams& p = *c.p;
-  if (p.drape_kind[d]) {             // Scrolly: window of the pattern (drapes.py:689-695)
-    const uint32_t* pat = p.st.d_pattern[d] + c.lvl * p.st.pattern_bstride[d];
-    const int pr = c.st->drapes[d][PCL_D_CORNER_R] + r, pc = c.st->drapes[d][PCL_D_CORNER_C] + col;
-    return bit_at(pat + (int64_t)pr * p.PWW, pc);
-  }
-  const uint32_t* bits = p.st.d_bits[d] + (int64_t)c.env * p.st.bits_bstride[d];
-  return bit_at(bits + (int64_t)r * p.BW, col);
-}
-
-// engine.py:737-759 + rendering.py:98-160 into the smem board.
-__device__ void render(const Ctx& c) {
-  const StepParams& p = *c.p;
-  const int n = p.S + p.D, cells = p.H * p.W;
-  for (int i = c.lane; i < cells; i += 32) {
-    const int r = i / p.W, col = i - r * p.W;
-    int code = c.backdrop[(int64_t)r * p.pitch + col];
-    for (int k = 0; k < n; ++k) {
-      const int ch = c.st->z[k];
-      for (int s = 0; s < p.S; ++s) {
-        if (p.sprite_char[s] == ch) {
-          const int32_t* rec = c.st->sprites[s];
-          if ((rec[PCL_S_FLAGS] & 1) && rec[PCL_S_ROW] == r && rec[PCL_S_COL] == col) code = ch;
-        }
-      }
-      for (int d = 0; d < p.D; ++d)
-        if (p.drape_char[d] == ch && drape_bit(c, d, r, col)) code = ch;
-    }
-    c.board[(int64_t)r * p.pitch + col] = (uint8_t)code;
-  }
-  __syncwarp();
-}
-
-__device__ __forceinline__ Sprite load_sprite(const int32_t* r) {
-  Sprite s;
-  s.row = r[0]; s.col = r[1]; s.vrow = r[2]; s.vcol = r[3];
-  s.flags = r[4]; s.aux0 = r[5]; s.aux1 = r[6]; s.aux2 = r[7];
-  return s;
-}
-__device__ __forceinline__ void store_sprite(int32_t* r, const Sprite& s, int lane) {
-  __syncwarp();
-  if (lane == 0) {
-    r[0] = s.row; r[1] = s.col; r[2] = s.vrow; r[3] = s.vcol;
-    r[4] = s.flags; r[5] = s.aux0; r[6] = s.aux1; r[7] = s.aux2;
   }
   __syncwarp();
 }
@@ -190,7 +125,7 @@ fixture_step(const StepParams p) {
   if (env >= p.B) return;
   const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
   const int H = p.H, W = p.W, S = p.S, D = p.D, n = S + D;
-  const size_t board_bytes = ((size_t)H * p.pitch + 15) & ~(size_t)15;
+  const size_t board_bytes = board::board_bytes(H, p.pitch);
   uint8_t* my = smem_raw + warp * (sizeof(WarpState) + board_bytes);
   WarpState* st = reinterpret_cast<WarpState*>(my);
   Ctx c;
@@ -216,10 +151,7 @@ fixture_step(const StepParams p) {
   const uint8_t* src_z = restart ? p.st.d_z_order_init + lvl * p.st.z_order_init_bstride
                                  : g_z;
   const PlotCarry carry = plot_carry(g_plot, restart);
-  for (int i = lane; i < S * PCL_SPRITE_WORDS; i += 32) (&st->sprites[0][0])[i] = src_s[i];
-  for (int i = lane; i < D * PCL_DRAPE_WORDS; i += 32) (&st->drapes[0][0])[i] = src_d[i];
-  if (lane < PCL_PLOT_WORDS) st->plot[lane] = src_p[lane];
-  if (lane < n) st->z[lane] = src_z[lane];
+  board::stage_records(st, src_s, src_d, src_p, src_z, S, D, lane);
   for (int i = lane; i < S * 4; i += 32) (&st->impassable[0][0])[i] = p.impassable[i >> 2][i & 3];
   for (int i = lane; i < (int)board_bytes; i += 32) c.board[i] = 0;
   __syncwarp();
@@ -238,14 +170,8 @@ fixture_step(const StepParams p) {
   if (restart) {
     if (lane == 0) store_carry(st->plot, carry);
     __syncwarp();
-    render(c);                               // the pre-initial render, engine.py:572-578
-  } else {
-    // The board every entity of the first group reads = last step's final board.
-    const int n16 = (H * p.pitch) >> 4;
-    for (int i = lane; i < n16; i += 32)
-      reinterpret_cast<uint4*>(c.board)[i] = reinterpret_cast<const uint4*>(g_board)[i];
-    __syncwarp();
   }
+  board::stage_board(c, restart, g_board);
 
   Plot plot;
   plot.frame = st->plot[PCL_P_FRAME] + 1;    // engine.py:716
@@ -337,15 +263,9 @@ fixture_step(const StepParams p) {
     store_outputs(p.out, env, dir);
   }
   __syncwarp();
-  for (int i = lane; i < S * PCL_SPRITE_WORDS; i += 32) g_sprites[i] = (&st->sprites[0][0])[i];
-  for (int i = lane; i < D * PCL_DRAPE_WORDS; i += 32) g_drapes[i] = (&st->drapes[0][0])[i];
-  if (lane < PCL_PLOT_WORDS) g_plot[lane] = st->plot[lane];
+  board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
   if (g_groups && n_sg > 1 && lane >= PCL_GROUP_WORDS && lane < n_sg * PCL_GROUP_WORDS)
     g_groups[lane] = (&st->groups[0][0])[lane];
-  if (lane < n) g_z[lane] = st->z[lane];
-  const int n16 = (H * p.pitch) >> 4;
-  for (int i = lane; i < n16; i += 32)
-    reinterpret_cast<uint4*>(g_board)[i] = reinterpret_cast<const uint4*>(c.board)[i];
 }
 
 // Any MazeWalker / Scrolly / plain-drape mix; entities and z-order must be consistent
@@ -394,7 +314,7 @@ int actions_per_env(const pcl_spec& s) {
 }
 
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
-  const size_t board_bytes = ((size_t)p.H * p.pitch + 15) & ~(size_t)15;
+  const size_t board_bytes = board::board_bytes(p.H, p.pitch);
   const size_t smem = (sizeof(WarpState) + board_bytes) * kWarpsPerBlock;
   return launch_step(fixture_step, p, kWarpsPerBlock, smem, s);
 }

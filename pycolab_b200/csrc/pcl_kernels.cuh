@@ -50,6 +50,7 @@ struct StepParams {
   const uint8_t* env_mask;       // u8 [B] or NULL (MODE_RESET)
   int has_cropper;               // pcl_attach_cropper: crop the new board as the kernel's epilogue
   CropParams cropper;            // (board is taken from `out` at launch time)
+  const int32_t* code;           // device copy of the bytecode bound with pcl_bind_code, or NULL
 };
 
 // Launch with the programmatic-stream-serialisation attribute (the kernel calls
@@ -97,9 +98,13 @@ struct Program {
   bool float_reward;             // rewards go to pcl_outputs.d_reward_f64, not d_reward
   bool crop_epilogue;            // the step kernel runs an attached cropper (pcl_attach_cropper)
   bool scroll_groups;            // accepts more than one scrolling group
+  // Programs that run bytecode (pcl_bind_code): checks the host words against the spec,
+  // PCL_OK / PCL_ERR_INVALID.  nullptr: the program takes no code.
+  int (*check_code)(const pcl_spec&, const int32_t* words, int n_words);
+  bool float_reward_arg0;        // rewards are float64 when spec.program_arg[0] != 0
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
-    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze;
+    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled;
 
 // Host-side helpers of the programs' check_spec.
 inline bool chars_are(const uint8_t* got, int n, const char* want) {

@@ -192,6 +192,8 @@ class Engine(object):
                          'not exist')
     if errors & _lib.ENV_ERR_INDEX:
       raise IndexError('a board look-up fell off the array')
+    if errors & _lib.ENV_ERR_ARITH:
+      raise ZeroDivisionError('integer division or modulo by zero in a compiled update()')
     if self._occlusion_in_layers:
       layers = rendering.LazyLayers(board, self._chars)
     else:

@@ -129,8 +129,13 @@ def _is_known_implementation(klass, key):
 
 
 def role_of(entity):
-  """Device role of `entity`, or raise NotLoweredError."""
+  """Device role of `entity`, or raise NotLoweredError.  A class registered with
+  `compiler.register` (along the MRO, update() not overridden below it) comes first."""
   cls = type(entity)
+  from pycolab_b200 import compiler
+  compiled = compiler.registered(cls)
+  if compiled is not None:
+    return 'compiled.walker' if compiled.kind == 'sprite' else 'compiled.drape'
   for klass in cls.__mro__:
     key = (klass.__module__.rsplit('.', 1)[-1], klass.__name__)
     if key in LOWERED_CLASSES:
@@ -230,6 +235,9 @@ class LoweredGame(object):
     self.sync = None            # (Engine): mirror program-private device state into the
                                 # Python objects after a step
     self.action_row = None      # (Engine, facade actions) -> the env's action words
+    self.code = None            # i32 bytecode words (pcl_bind_code) of the compiled program
+    self.registers = {}         # compiled: char -> [(attribute, is_bool)] in register order
+    self.plot_keys = []         # compiled: [(the_plot key, is_bool)] in plot register order
 
   @property
   def needs_rng(self):
@@ -242,7 +250,7 @@ class LoweredGame(object):
             tuple(self.egocentric), tuple(map(tuple, self.margins)), self.z_order,
             tuple(self.groups), self.pattern_rows, self.pattern_cols,
             tuple(self.program_arg), tuple(self.scroll_groups), tuple(self.sprite_group),
-            tuple(self.drape_group))
+            tuple(self.drape_group), None if self.code is None else self.code.tobytes())
 
   def make_spec(self, auto_reset):
     s = _lib.Spec()

@@ -1,0 +1,123 @@
+"""The compiled program `csrc/compiled.cu`: MazeWalkers and plain drapes of classes
+registered with `pycolab_b200.compiler`, whose update() bodies run as device bytecode."""
+
+import numpy as np
+
+from pycolab_b200 import _lib
+from pycolab_b200 import compiler
+from pycolab_b200 import things
+from pycolab_b200.errors import NotLoweredError
+from pycolab_b200.lowering import (LoweredGame, _common, _plot_record, _set_sprites,
+                                   _sprite_record, pack_rows)
+
+_INT32 = (-2 ** 31, 2 ** 31 - 1)
+
+
+def _register_value(owner, value):
+  """An int / bool register value, or NotLoweredError."""
+  if isinstance(value, (bool, np.bool_)):
+    return int(bool(value)), True
+  if isinstance(value, (int, np.integer)):
+    if not _INT32[0] <= int(value) <= _INT32[1]:
+      raise NotLoweredError('{} = {} does not fit a 32-bit register'.format(owner, value))
+    return int(value), False
+  raise NotLoweredError('{} holds {!r}: only int and bool values are compiled'.format(
+      owner, value))
+
+
+def lower(engine, roles):
+  th = engine.things
+  game = LoweredGame()
+  _common(engine, game, _lib.PROG_COMPILED)
+  order = ''.join(game.groups)
+  sprite_chars = [c for c in order if roles[c] == 'compiled.walker']
+  drape_chars = [c for c in order if roles[c] == 'compiled.drape']
+  if len(sprite_chars) > _lib.MAX_SPRITES or len(drape_chars) > _lib.MAX_DRAPES:
+    raise NotLoweredError('too many entities for the compiled device program')
+  comp = {ch: compiler.registered(type(th[ch])) for ch in order}
+  for ch in sprite_chars:
+    if th[ch]._egocentric_scroller:
+      raise NotLoweredError('egocentric MazeWalker {!r} is not compiled'.format(ch))
+  for ch in drape_chars:
+    if type(th[ch]).curtain is not things.Drape.curtain:
+      raise NotLoweredError('drape {!r} overrides `curtain`'.format(ch))
+
+  # the_plot keys: plot registers AUX0.. in order of first use
+  keys = []
+  for ch in order:
+    for key in comp[ch].keys:
+      if key not in keys:
+        keys.append(key)
+  if len(keys) > compiler.MAX_PLOT_KEYS:
+    raise NotLoweredError('the_plot keys {} need more than {} plot registers'.format(
+        keys, compiler.MAX_PLOT_KEYS))
+  plot_regs, plot_bools = [], []
+  for key in keys:
+    if key not in engine.the_plot:
+      raise NotLoweredError('the_plot[{!r}] is read or written by update() but not set when '
+                            'the game is lowered'.format(key))
+    value, is_bool = _register_value('the_plot[{!r}]'.format(key), engine.the_plot[key])
+    plot_regs.append(value)
+    plot_bools.append(is_bool)
+
+  # per-entity registers from the live objects
+  registers = {}                 # char -> [(attr, is_bool)]
+  values = {}
+  for ch in order:
+    c = comp[ch]
+    if len(c.attrs) > compiler.MAX_REGISTERS[c.kind]:
+      raise NotLoweredError('{} needs {} registers; a {} has {}'.format(
+          compiler._name(c.klass), len(c.attrs), c.kind, compiler.MAX_REGISTERS[c.kind]))
+    regs = []
+    values[ch] = []
+    for name in c.attrs:
+      if not hasattr(th[ch], name):
+        raise NotLoweredError('{!r}.{} is used by update() but not set when the game is '
+                              'lowered'.format(ch, name))
+      value, is_bool = _register_value('{!r}.{}'.format(ch, name), getattr(th[ch], name))
+      regs.append((name, is_bool))
+      values[ch].append(value)
+    registers[ch] = regs
+
+  sprites = [th[c] for c in sprite_chars]
+  _set_sprites(game, sprites, [_sprite_record(s, *(values[s.character] + [0, 0, 0])[:3])
+                               for s in sprites])
+  game.drape_chars = ''.join(drape_chars)
+  game.margins = [(-1, -1)] * len(drape_chars)
+  game.drape_kind = [0] * len(drape_chars)
+  recs = []
+  for d, ch in enumerate(drape_chars):
+    recs.append((values[ch] + [0] * _lib.DRAPE_WORDS)[:_lib.DRAPE_WORDS])
+    game.bits[d] = pack_rows(th[ch].curtain, game.bits_words)
+  game.drapes = np.array(recs, dtype=np.int32).reshape(len(drape_chars), _lib.DRAPE_WORDS)
+  game.plot = np.array(_plot_record(**{'aux%d' % i: v for i, v in enumerate(plot_regs)}),
+                       dtype=np.int32)
+  game.dynamic_z = True                  # the kernel renders from the per-env z-order
+  game.code = compiler.link(comp, sprite_chars, drape_chars, engine.rows, engine.cols, keys)
+  game.float_reward = any(c.float_reward for c in comp.values())
+  game.reward_type = float if game.float_reward else int
+  game.program_arg[0] = 1 if game.float_reward else 0
+  game.registers = registers
+  game.plot_keys = list(zip(keys, plot_bools))
+  game.sync = sync
+  return game
+
+
+def sync(engine):
+  """Registers back into the entities' attributes and the Plot's keys (bool stays bool)."""
+  b = engine.batched
+  game = b.game
+  sprites = b.sprites[0].cpu().numpy()
+  drapes = b.drapes[0].cpu().numpy()
+  plot = b.plot[0].cpu().numpy()
+  th = engine.things
+  for ch, regs in game.registers.items():
+    if ch in b.sprite_chars:
+      words = sprites[b.sprite_chars.index(ch)][_lib.S_AUX0:]
+    else:
+      words = drapes[b.drape_chars.index(ch)]
+    for (name, is_bool), word in zip(regs, words):
+      setattr(th[ch], name, bool(word) if is_bool else int(word))
+  for k, (key, is_bool) in enumerate(game.plot_keys):
+    word = plot[_lib.P_AUX0 + k]
+    engine.the_plot[key] = bool(word) if is_bool else int(word)
