@@ -60,6 +60,7 @@ typedef enum pcl_status {
 #define PCL_ENV_ERR_INDEX            0x8  /* NumPy IndexError (board look-up off the array) */
 #define PCL_ENV_ERR_BAD_Z            0x10 /* change_z_order names a missing entity, engine.py:802-812 */
 #define PCL_ENV_ERR_ARITH            0x20 /* ZeroDivisionError: `//` or `%` by zero in compiled code */
+#define PCL_ENV_ERR_RANGE            0x40 /* ValueError: a compiled draw from an empty range */
 
 /* Which game program advances the envs.  One fused kernel per program; the
  * host "lowering" recognises the reference's entity classes and picks one. */
@@ -103,7 +104,11 @@ typedef enum pcl_program {
                                 compiled to the bytecode below (pcl_bind_code) and interpreted one warp
                                 per env.  Registers: sprite AUX0-AUX2, all eight words of a drape record,
                                 plot AUX0-AUX3 (the_plot keys).  program_arg[0] = 1: rewards are float64
-                                (pcl_outputs.d_reward_f64 is required), 0: int32 */
+                                (pcl_outputs.d_reward_f64 is required), 0: int32.  program_arg[1] =
+                                the number of RNG slots the code draws from (0-2); with slots,
+                                pcl_state.d_rng is required and is u32 [B, program_arg[1],
+                                PCL_MT_WORDS], each slot the words of NumPy's RandomState or of
+                                Python's random.Random, continued across auto-resets */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */
@@ -185,8 +190,27 @@ enum {
   PCL_OP_REWARD_F64,    /* lo, hi: add_reward of the float64 with these bit halves            */
   PCL_OP_TERMINATE,     /* f32 bits: the_plot.terminate_episode(discount)                     */
   PCL_OP_DISCOUNT,      /* f32 bits: the_plot.change_default_discount(discount)              */
+  /* Draws from the env's RNG slot `slot` of pcl_state.d_rng (slot < program_arg[1]). */
+  PCL_OP_RANDINT,       /* slot, rule (PCL_RAND_*): pop low, high; push a draw from the rule's
+                           range.  An empty range latches PCL_ENV_ERR_RANGE, pushes low and
+                           consumes no output                                                  */
+  PCL_OP_RANDCMP,       /* slot, cmp, lo, hi: draw a float (two outputs, 53 bits, as NumPy's
+                           random_sample() and Python's random()) and push `draw cmp x`, x the
+                           float64 with bit halves lo / hi, cmp 0-5 = == != < <= > >=          */
+  PCL_OP_PICK,          /* k, v_1 .. v_k: pop i; push v_(i+1) (1 <= k <= 64); i outside 0 .. k-1
+                           latches PCL_ENV_ERR_INDEX and pushes 0                              */
   PCL_OP_COUNT
 };
+
+/* PCL_OP_RANDINT rules, over int32 operands with widths computed in 64 bits:
+ *   PCL_RAND_NUMPY        RandomState.randint(low, high): [low, high); one 32-bit output per
+ *                         try, masked rejection; no output when the range holds one value;
+ *   PCL_RAND_PYTHON       Random.randrange(low, high): low + _randbelow(high - low), where
+ *                         _randbelow(n) repeats getrandbits(n.bit_length()) until it is < n
+ *                         (getrandbits(k <= 32) = one output >> (32 - k); k == 33 = two
+ *                         outputs lo, hi: lo | (hi >> 31) << 32), so a width of 1 consumes output;
+ *   PCL_RAND_PYTHON_CLOSED Random.randint(low, high): as PCL_RAND_PYTHON over [low, high]. */
+enum { PCL_RAND_NUMPY = 0, PCL_RAND_PYTHON = 1, PCL_RAND_PYTHON_CLOSED = 2 };
 
 /* Motion codes (prefab_parts/sprites.py:140-150). */
 enum { PCL_M_N = 0, PCL_M_NE, PCL_M_E, PCL_M_SE, PCL_M_S, PCL_M_SW, PCL_M_W,
@@ -272,7 +296,9 @@ typedef struct pcl_state {
   int32_t* d_sprites;  const int32_t* d_sprites_init; int64_t sprites_init_bstride; /* [B, S, 8] */
   int32_t* d_drapes;   const int32_t* d_drapes_init;  int64_t drapes_init_bstride;  /* [B, D, 8] */
   int32_t* d_plot;     const int32_t* d_plot_init;    int64_t plot_init_bstride;    /* [B, 16]   */
-  uint32_t* d_rng;     /* MT19937 per env, u32 [B, PCL_MT_WORDS]; NULL if unused */
+  uint32_t* d_rng;     /* MT19937 per env, u32 [B, PCL_MT_WORDS]; NULL if unused.  PCL_PROG_T_MAZE
+                          and PCL_PROG_COMPILED keep several slots per env: u32 [B, slots,
+                          PCL_MT_WORDS] (see their pcl_program entries) */
   /* per-env z-order (chars, back to front) for programs whose entities issue
    * Plot.change_z_order (engine.py:796-835): u8 [B, n_sprites + n_drapes]; NULL = spec z_order */
   uint8_t* d_z_order;  const uint8_t* d_z_order_init; int64_t z_order_init_bstride;

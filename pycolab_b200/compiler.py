@@ -30,6 +30,18 @@ and the construct):
               `board[cell]`, `backdrop.curtain[cell]`, `layers['X'][cell]`,
               `self.curtain[cell]`, `things['X'].position / .visible / .curtain[cell]`,
               `.curtain.any()`.
+  draws       from the global generators, whose functions are found through update()'s
+              module globals and compared by identity (so `import numpy as np`,
+              `from numpy import random as npr` and `from random import randint` all
+              work), with int operands and no keywords:
+                NumPy's RandomState: `np.random.randint(high)`, `randint(low, high)`,
+                `choice(n)`, `choice(<literal tuple / list of ints>)`;
+                Python's Random: `random.randint(a, b)`, `randrange(stop)`,
+                `randrange(start, stop)`, `choice(<literal tuple / list of ints>)`;
+                a float draw, `np.random.rand()` / `random()` / `random_sample()` or
+                `random.random()`, only as one side of a comparison with a number literal.
+              Each draw continues the env's copy of that generator on the device
+              (include/pcl.h PCL_OP_RANDINT) and yields what the generator would.
 Int and bool attributes of `self` become per-entity registers and `the_plot` keys plot
 registers; their values are read from the live objects when the game is lowered.
 Integers are 32 bits on the device; values outside int32 wrap.  After a facade step a
@@ -38,8 +50,10 @@ register is written back with the type (bool or int) its value had at lowering.
 
 import ast
 import inspect
+import random
 import struct
 import textwrap
+import types
 
 import numpy as np
 
@@ -63,6 +77,15 @@ _POSITIONS = {'position': (_lib.FIELD_ROW, _lib.FIELD_COL),
 # Registers per entity: sprite record AUX0-AUX2, every word of a plain drape's record.
 MAX_REGISTERS = {'sprite': 3, 'drape': _lib.DRAPE_WORDS}
 MAX_PLOT_KEYS = 4
+# The generator functions a draw may call: (function, stream, kind).
+_DRAWS = ((np.random.randint, 'numpy', 'randint'), (np.random.choice, 'numpy', 'choice'),
+          (np.random.rand, 'numpy', 'float'), (np.random.random, 'numpy', 'float'),
+          (np.random.random_sample, 'numpy', 'float'),
+          (random.randint, 'python', 'randint'), (random.randrange, 'python', 'randrange'),
+          (random.choice, 'python', 'choice'), (random.random, 'python', 'float'))
+# `x op draw` as `draw op' x`.
+_FLIPPED = {ast.Eq: ast.Eq, ast.NotEq: ast.NotEq, ast.Lt: ast.Gt, ast.LtE: ast.GtE,
+            ast.Gt: ast.Lt, ast.GtE: ast.LtE}
 _TYPE_NAMES = {'int': 'number', 'pos': 'position', 'motion': 'motion result', 'char': 'character'}
 
 
@@ -78,13 +101,15 @@ def _f64_halves(x):
 class Compiled(object):
   """One class's update(), compiled with symbolic operands (`link` resolves them):
   ('attr', name) a register, ('key', name) a plot key, ('ent', char) an entity,
-  ('label', n) a code address, ('rows',) / ('cols',) the board shape."""
+  ('label', n) a code address, ('rows',) / ('cols',) the board shape, ('rng', stream) the
+  RNG slot of a generator."""
 
-  def __init__(self, klass, kind, ir, attrs, keys, float_reward):
+  def __init__(self, klass, kind, ir, attrs, keys, float_reward, streams=()):
     self.klass, self.kind, self.ir = klass, kind, ir
     self.attrs = attrs            # register names, in slot order
     self.keys = keys              # the_plot keys it reads or writes
     self.float_reward = float_reward
+    self.streams = list(streams)  # generators it draws from ('numpy', 'python'), first use first
 
 
 def register(*classes):
@@ -138,6 +163,7 @@ class _Compiler(object):
     except (OSError, TypeError):
       raise NotLoweredError('{}: the source of update() is not available'.format(_name(klass)))
     self.lines = lines
+    self.globals = getattr(fn, '__globals__', {})
     tree = ast.parse(textwrap.dedent(''.join(lines)))
     self.fdef = tree.body[0]
     args = self.fdef.args
@@ -152,11 +178,13 @@ class _Compiler(object):
     self.n_slots = 0
     self.attrs, self.keys = [], []
     self.float_reward = False
+    self.streams = []
 
   def run(self):
     self.stmts(self.fdef.body)
     self.emit('RET')
-    return Compiled(self.klass, self.kind, self.ir, self.attrs, self.keys, self.float_reward)
+    return Compiled(self.klass, self.kind, self.ir, self.attrs, self.keys, self.float_reward,
+                    self.streams)
 
   # -------------------------------------------------------------- helpers
   def refuse(self, node, what):
@@ -207,6 +235,11 @@ class _Compiler(object):
     if name not in self.attrs:
       self.attrs.append(name)
     return ('attr', name)
+
+  def use_stream(self, stream):
+    if stream not in self.streams:
+      self.streams.append(stream)
+    return ('rng', stream)
 
   def need(self, node, kind, what):
     if self.kind != kind:
@@ -602,7 +635,85 @@ class _Compiler(object):
       if owner is not None:
         self.emit('ANY', owner)
         return 'int'
+    draw = self.generator_call(node)
+    if draw is not None:
+      self.draw(node, *draw)
+      return 'int'
     self.refuse(node, 'the call {}()'.format(ast.unparse(f)))
+
+  # ------------------------------------------------------------------ draws
+  def callee(self, f):
+    """What a name or a dotted chain through modules names in update()'s module (the
+    `np.random.randint` of `np.random.randint(4)`), or None.  Only module attributes are
+    looked up, so resolving runs no user code."""
+    parts = []
+    while isinstance(f, ast.Attribute):
+      parts.append(f.attr)
+      f = f.value
+    if not isinstance(f, ast.Name) or f.id in self.role or f.id in self.locals:
+      return None
+    obj = self.globals.get(f.id)
+    for name in reversed(parts):
+      if not isinstance(obj, types.ModuleType):
+        return None
+      obj = getattr(obj, name, None)
+    return obj
+
+  def generator_call(self, node):
+    """(stream, kind) when `node` calls a function of a global generator, else None."""
+    if not isinstance(node, ast.Call):
+      return None
+    fn = self.callee(node.func)
+    for draw, stream, kind in _DRAWS:
+      if fn is draw:
+        return stream, kind
+    return None
+
+  def draw(self, node, stream, kind):
+    """Emit the int draw `node` (generator_call's stream, kind); refuse other forms."""
+    what = 'the call {}()'.format(ast.unparse(node.func))
+    args, n = node.args, len(node.args)
+    if (node.keywords or kind == 'float' or any(isinstance(a, ast.Starred) for a in args) or
+        n not in {'randint': (1, 2) if stream == 'numpy' else (2,), 'randrange': (1, 2),
+                  'choice': (1,)}[kind]):
+      self.refuse(node, what)
+    slot = self.use_stream(stream)
+    rule = _lib.RAND_NUMPY if stream == 'numpy' else _lib.RAND_PYTHON
+    if kind == 'choice' and isinstance(args[0], (ast.Tuple, ast.List)):
+      values = [self.number(e) for e in args[0].elts]
+      if not values or len(values) > 64 or not all(isinstance(v, int) for v in values):
+        self.refuse(node, what)                 # empty, too long, or not int literals
+      self.emit('PUSH', 0)
+      self.emit('PUSH', len(values))
+      self.emit('RANDINT', slot, rule)
+      self.emit('PICK', len(values), *values)
+      return
+    if kind == 'choice':
+      if stream == 'python':
+        self.refuse(node, what)                 # random.choice takes a sequence
+      self.emit('PUSH', 0)
+      try:
+        self.scalar(args[0])
+      except NotLoweredError:
+        self.refuse(node, what)                 # a sequence that is not a literal
+    else:
+      if n == 1:
+        self.emit('PUSH', 0)
+      for a in args:
+        self.scalar(a)
+      if kind == 'randint' and stream == 'python':
+        rule = _lib.RAND_PYTHON_CLOSED
+    self.emit('RANDINT', slot, rule)
+
+  def float_draw(self, node, op, other, where):
+    """`draw op other` for a float draw `node` and a number literal `other`."""
+    what = 'the call {}()'.format(ast.unparse(node.func))
+    value = self.number(other)
+    if node.args or node.keywords or value is None or type(op) not in _CMPOPS:
+      self.refuse(where, what)
+    stream, _ = self.generator_call(node)
+    self.emit('RANDCMP', self.use_stream(stream), list(_CMPOPS).index(type(op)),
+              *_f64_halves(value))
 
   def literal_values(self, node, chars):
     """Codes of a literal tuple / list / string for `in`; `chars`: the left side is chr()."""
@@ -627,6 +738,9 @@ class _Compiler(object):
     self.refuse(node, '`in` over something that is not a literal tuple, list or string')
 
   def compare(self, node):
+    for x in [node.left] + node.comparators:
+      if len(node.ops) > 1 and (self.generator_call(x) or (None, None))[1] == 'float':
+        self.refuse(node, 'the call {}()'.format(ast.unparse(x.func)))   # drawn once, used twice
     if len(node.ops) == 1:
       self.compare1(node.left, node.ops[0], node.comparators[0], node)
       return 'int'
@@ -643,6 +757,11 @@ class _Compiler(object):
     return 'int'
 
   def compare1(self, left, op, right, node):
+    floats = [(self.generator_call(x) or (None, None))[1] == 'float' for x in (left, right)]
+    if floats[0] and not floats[1]:
+      return self.float_draw(left, op, right, node)
+    if floats[1] and not floats[0]:
+      return self.float_draw(right, _FLIPPED.get(type(op), ast.In)(), left, node)
     none = isinstance(right, ast.Constant) and right.value is None
     if isinstance(op, (ast.Is, ast.IsNot)):
       if not none:
@@ -721,9 +840,10 @@ _RESERVED = {
 
 # ------------------------------------------------------------------ linking
 
-def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys):
+def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys, rng_streams=()):
   """Bytecode words for one game.  compiled: char -> `Compiled`; plot_keys: the key
-  order of the plot registers.  Entities of one class share their code."""
+  order of the plot registers; rng_streams: the generator of each RNG slot.  Entities of
+  one class share their code."""
   chars = list(sprite_chars) + list(drape_chars)
   S = len(sprite_chars)
   words = [len(chars)] + [0] * len(chars)
@@ -732,7 +852,7 @@ def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys):
     comp = compiled[ch]
     if comp.klass not in entry:
       entry[comp.klass] = len(words)
-      words += _encode(comp, len(words), chars, S, rows, cols, plot_keys)
+      words += _encode(comp, len(words), chars, S, rows, cols, plot_keys, rng_streams)
     words[1 + i] = entry[comp.klass]
   if len(words) > _lib.MAX_CODE_WORDS:
     raise NotLoweredError('the compiled game needs {} code words, more than {}'.format(
@@ -740,7 +860,7 @@ def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys):
   return np.array(words, dtype=np.int32)
 
 
-def _encode(comp, base, chars, S, rows, cols, plot_keys):
+def _encode(comp, base, chars, S, rows, cols, plot_keys, rng_streams):
   addr, pc = {}, base
   for ins in comp.ir:                 # pass 1: label addresses
     if ins[0] == 'LABEL':
@@ -757,6 +877,8 @@ def _encode(comp, base, chars, S, rows, cols, plot_keys):
       return comp.attrs.index(x[1])
     if x[0] == 'key':
       return plot_keys.index(x[1])
+    if x[0] == 'rng':
+      return list(rng_streams).index(x[1])
     if x[0] == 'rows':
       return rows
     if x[0] == 'cols':

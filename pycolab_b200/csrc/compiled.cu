@@ -7,7 +7,11 @@
 // in shared memory.  Interpretation is warp-uniform: every lane runs the same
 // instruction on the same values, and the operand stack and locals live in shared
 // memory.  The lanes split up only for a render, a walker's neighbourhood, a curtain
-// fill and a curtain's any().
+// fill, a curtain's any() and an MT19937 twist.
+//
+// Draws (PCL_OP_RANDINT / RANDCMP) continue the env's generator words in d_rng, in global
+// memory as marauders.cu and shockwave.cu keep theirs: a draw reads one or two words and
+// the position, and every 624th output the warp twists the 624 words together.
 //
 // Semantics restated from upstream:
 //   - update() runs on the its_showtime() frame too, with actions=None (engine.py:581);
@@ -16,6 +20,7 @@
 //   - Plot directives apply in call order: rewards sum (plot.py:201-214), the last
 //     discount-setting call wins, terminate_episode() does not stop later updates.
 #include "pcl_board.cuh"
+#include "pcl_mt.cuh"
 
 #include <vector>
 
@@ -42,14 +47,15 @@ struct LaneSlots {
   __device__ __forceinline__ int32_t& operator[](int i) const { return base[i * 32]; }
 };
 
-// Operand words of opcode `op` (PCL_OP_IN has its count more).
+// Operand words of opcode `op` (PCL_OP_IN and PCL_OP_PICK have their count more).
 __host__ __device__ __forceinline__ int op_operands(int op) {
   switch (op) {
-    case PCL_OP_FIELD: case PCL_OP_REWARD_F64: return 2;
+    case PCL_OP_RANDCMP: return 4;
+    case PCL_OP_FIELD: case PCL_OP_REWARD_F64: case PCL_OP_RANDINT: return 2;
     case PCL_OP_PUSH: case PCL_OP_LOAD: case PCL_OP_STORE: case PCL_OP_JMP: case PCL_OP_JZ:
     case PCL_OP_JNZ: case PCL_OP_IN: case PCL_OP_GETR: case PCL_OP_SETR: case PCL_OP_GETP:
     case PCL_OP_SETP: case PCL_OP_CURTAIN: case PCL_OP_ANY: case PCL_OP_MOVE:
-    case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: return 1;
+    case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: case PCL_OP_PICK: return 1;
     default: return 0;
   }
 }
@@ -91,8 +97,12 @@ constexpr OpInfo kOps[PCL_OP_COUNT] = {
     {0, 0},  // REWARD_F64
     {0, 0},  // TERMINATE
     {0, 0},  // DISCOUNT
+    {2, 1},  // RANDINT
+    {0, 1},  // RANDCMP
+    {1, 1},  // PICK (+ its values)
 };
-constexpr int kMaxIn = 64;
+static_assert(sizeof(kOps) / sizeof(kOps[0]) == PCL_OP_COUNT, "one kOps entry per opcode");
+constexpr int kMaxIn = 64;            // values of an IN or a PICK
 
 // Python's // and % (floor semantics) on int32 operands, b != 0.
 __device__ __forceinline__ int floordiv(int a, int b) {
@@ -117,13 +127,38 @@ __device__ __forceinline__ uint32_t row_word_mask(int w, int W) {
   return W - first >= 32 ? 0xffffffffu : (1u << (W - first)) - 1u;
 }
 
+// RNG slot `slot` of the env being stepped: d_rng is u32 [B, program_arg[1], PCL_MT_WORDS].
+__device__ __forceinline__ uint32_t* rng_slot(const Ctx& c, int slot) {
+  const StepParams& p = *c.p;
+  return p.st.d_rng + ((int64_t)c.env * p.program_arg[1] + slot) * PCL_MT_WORDS;
+}
+
+// `x cmp y` for cmp 0-5 = == != < <= > >= (PCL_OP_EQ .. PCL_OP_GE in order).
+template <typename T>
+__device__ __forceinline__ int compare(int cmp, T x, T y) {
+  switch (cmp) {
+    case 0: return x == y;
+    case 1: return x != y;
+    case 2: return x < y;
+    case 3: return x <= y;
+    case 4: return x > y;
+    default: return x >= y;
+  }
+}
+
 struct Rewards {
   int has;
   int sum_i;
   double sum_f;
 };
 
-// The update() of entity `ent` (sprites first, then drapes).
+// The twist of a draw, out of line: inlined into the interpreter it makes ptxas spill to
+// local memory.  Only one output in 624 pays for the call.
+__device__ __noinline__ void twist_out_of_line(uint32_t* mt, int lane) { mt_twist(mt, lane); }
+
+// The update() of entity `ent` (sprites first, then drapes).  kDraws: the code may draw
+// (program_arg[1] > 0); games without draws run a kernel without the generator.
+template <bool kDraws>
 __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot,
                            Directives& dir, Rewards& rw) {
   const StepParams& p = *c.p;
@@ -166,12 +201,7 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
             if (y == 0) plot.error |= PCL_ENV_ERR_ARITH;
             else v = op == PCL_OP_MOD ? floormod(x, y) : floordiv(x, y);
             break;
-          case PCL_OP_EQ: v = x == y; break;
-          case PCL_OP_NE: v = x != y; break;
-          case PCL_OP_LT: v = x < y; break;
-          case PCL_OP_LE: v = x <= y; break;
-          case PCL_OP_GT: v = x > y; break;
-          default: v = x >= y; break;
+          default: v = compare(op - PCL_OP_EQ, x, y); break;
         }
         stk[sp - 1] = v;
         break;
@@ -293,12 +323,48 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         break;
       }
       case PCL_OP_TERMINATE: terminate(dir, __int_as_float(a)); break;
-      default: change_default_discount(dir, __int_as_float(a)); break;   // PCL_OP_DISCOUNT
+      case PCL_OP_DISCOUNT: change_default_discount(dir, __int_as_float(a)); break;
+      case PCL_OP_RANDINT: case PCL_OP_RANDCMP: {   // one mt_draw site for both
+        if (!kDraws) break;                           // pcl_bind_code refused them
+        const int b = __ldg(code + pc + 2);           // the rule, or the comparison
+        const bool cmp = op == PCL_OP_RANDCMP;
+        int low = 0;
+        int64_t width = 0;
+        if (!cmp) {
+          const int high = stk[--sp];
+          low = stk[sp - 1];
+          width = (int64_t)high - low + (b == PCL_RAND_PYTHON_CLOSED);
+          if (width <= 0) {                  // ValueError upstream; low stays on the stack
+            plot.error |= PCL_ENV_ERR_RANGE;
+            break;
+          }
+          --sp;
+        }
+        const MtRule rule = cmp ? kMtRandom53 : b == PCL_RAND_NUMPY ? kMtNumpyBelow : kMtPythonBelow;
+        const uint64_t r = mt_draw<twist_out_of_line>(rng_slot(c, a), rule, (uint64_t)width, lane);
+        if (cmp) {
+          const double x = __dmul_rn(__ull2double_rn(r), 1.0 / 9007199254740992.0);
+          stk[sp++] = compare(b, x, __hiloint2double(__ldg(code + pc + 4), __ldg(code + pc + 3)));
+        } else {
+          stk[sp++] = (int)((uint32_t)low + (uint32_t)r);
+        }
+        break;
+      }
+      default: {                               // PCL_OP_PICK
+        const int i = stk[sp - 1];
+        int v = 0;
+        if ((unsigned)i < (unsigned)a) v = __ldg(code + pc + 2 + i);
+        else plot.error |= PCL_ENV_ERR_INDEX;
+        stk[sp - 1] = v;
+        next += a;
+        break;
+      }
     }
     pc = next;
   }
 }
 
+template <bool kDraws>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 compiled_step(const StepParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -368,7 +434,7 @@ compiled_step(const StepParams p) {
       int ent = 0;
       for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
       for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
-      run_update(c, vm, ent, action, plot, dir, rw);
+      run_update<kDraws>(c, vm, ent, action, plot, dir, rw);
     }
     board::render(c);
   }
@@ -410,6 +476,7 @@ int check_spec(const pcl_spec& s) {
   for (int d = 0; d < s.n_drapes; ++d)
     if (s.drape_kind[d]) return PCL_ERR_UNSUPPORTED;
   if (s.program_arg[0] != 0 && s.program_arg[0] != 1) return PCL_ERR_INVALID;
+  if (s.program_arg[1] < 0 || s.program_arg[1] > 2) return PCL_ERR_INVALID;   // RNG slots
   if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
   return PCL_OK;
 }
@@ -418,6 +485,7 @@ int check_state(const pcl_spec& s, const pcl_state& st) {
   if (!st.d_z_order || !st.d_z_order_init) return PCL_ERR_INVALID;
   for (int d = 0; d < s.n_drapes; ++d)
     if (!st.d_bits[d] || !st.d_bits_init[d]) return PCL_ERR_INVALID;
+  if (s.program_arg[1] > 0 && !st.d_rng) return PCL_ERR_INVALID;
   return PCL_OK;
 }
 
@@ -460,10 +528,18 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (a <= pc || a >= end) return PCL_ERR_INVALID;
         targets.push_back(a);
         break;
-      case PCL_OP_IN:
-        if (a < 0 || a > kMaxIn) return PCL_ERR_INVALID;
+      case PCL_OP_IN: case PCL_OP_PICK:
+        if (a < (op == PCL_OP_PICK ? 1 : 0) || a > kMaxIn) return PCL_ERR_INVALID;
         len += a;
         if (pc + len > end) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_RANDINT:
+        if (a < 0 || a >= s.program_arg[1]) return PCL_ERR_INVALID;
+        if (w[pc + 2] < PCL_RAND_NUMPY || w[pc + 2] > PCL_RAND_PYTHON_CLOSED) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_RANDCMP:
+        if (a < 0 || a >= s.program_arg[1]) return PCL_ERR_INVALID;
+        if (w[pc + 2] < 0 || w[pc + 2] > 5) return PCL_ERR_INVALID;
         break;
       case PCL_OP_FIELD:
         if (a < 0 ? !sprite : a >= S) return PCL_ERR_INVALID;
@@ -521,7 +597,8 @@ int actions_per_env(const pcl_spec&) { return 1; }
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (sizeof(WarpState) + sizeof(Vm) + board::board_bytes(p.H, p.pitch)) *
                       kWarpsPerBlock;
-  return launch_step(compiled_step, p, kWarpsPerBlock, smem, s);
+  return p.program_arg[1] > 0 ? launch_step(compiled_step<true>, p, kWarpsPerBlock, smem, s)
+                              : launch_step(compiled_step<false>, p, kWarpsPerBlock, smem, s);
 }
 
 }  // namespace

@@ -10,6 +10,7 @@ directly; this class is the drop-in single-env view of the same machinery.
 """
 
 import collections
+import random
 
 import numpy as np
 
@@ -133,7 +134,12 @@ class Engine(object):
                             'terminate_episode, change_default_discount, change_z_order) are '
                             'not carried into the device\'s first frame')
     rng_states = None
-    if 'python' in lowered.rng_streams:
+    if lowered.rng_from_globals:
+      # Compiled update() code draws from the GLOBAL generators, as the game's Python
+      # would: the device continues their words and hands them back after every step.
+      if lowered.needs_rng:
+        rng_states = np.concatenate([_global_words(s) for s in lowered.rng_streams])[None]
+    elif 'python' in lowered.rng_streams:
       # apprehend.py:103 draws in the sprite's constructor, which has already run
       # (from the global `random`, as upstream): the device takes the drawn value
       # from the template and needs no generator for this one episode.
@@ -177,7 +183,12 @@ class Engine(object):
     discount = float(result.discount[0])
     self._game_over = bool(int(result.done[0]))
     self._sync_things()
-    if self._batched.rng is not None:
+    if self._batched.game.rng_from_globals:
+      if self._batched.rng is not None:
+        words = self._batched.rng[0].cpu().numpy().view(np.uint32).reshape(-1, _lib.MT_WORDS)
+        for stream, slot in zip(self._batched.game.rng_streams, words):
+          _set_global_words(stream, slot)
+    elif self._batched.rng is not None:
       words = self._batched.rng[0].cpu().numpy().view(np.uint32)
       old = np.random.get_state()
       np.random.set_state((old[0], words[:624].copy(), int(words[624]), old[3], old[4]))
@@ -194,6 +205,8 @@ class Engine(object):
       raise IndexError('a board look-up fell off the array')
     if errors & _lib.ENV_ERR_ARITH:
       raise ZeroDivisionError('integer division or modulo by zero in a compiled update()')
+    if errors & _lib.ENV_ERR_RANGE:
+      raise ValueError('empty range for a random draw in a compiled update()')
     if self._occlusion_in_layers:
       layers = rendering.LazyLayers(board, self._chars)
     else:
@@ -297,6 +310,28 @@ class Engine(object):
         ord(char)
       except TypeError:
         raise ValueError('Character {} is not an ASCII character'.format(char))
+
+
+def _global_words(stream):
+  """u32 [625]: the MT19937 words (624 key words + position) of the global generator
+  `stream`: NumPy's legacy RandomState ('numpy') or Python's random.Random ('python')."""
+  if stream == 'python':
+    return np.array(random.getstate()[1], dtype=np.uint32)
+  kind, key, pos = np.random.get_state()[:3]
+  if kind != 'MT19937':
+    raise RuntimeError('global NumPy RNG is not MT19937')
+  return np.append(key, pos).astype(np.uint32)
+
+
+def _set_global_words(stream, words):
+  """Continue the global generator `stream` from `words` (u32 [625]), keeping the
+  Gaussian each one may hold back."""
+  if stream == 'python':
+    version, _, gauss_next = random.getstate()
+    random.setstate((version, tuple(int(w) for w in words), gauss_next))
+  else:
+    old = np.random.get_state()
+    np.random.set_state((old[0], words[:624].copy(), int(words[624]), old[3], old[4]))
 
 
 class Palette(object):

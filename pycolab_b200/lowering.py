@@ -216,6 +216,8 @@ class LoweredGame(object):
     self.rng_streams = ()       # the MT19937 streams the device continues, one RNG slot each
                                 # in this order: NumPy's legacy RandomState ('numpy') or
                                 # Python's `random` ('python')
+    self.rng_from_globals = False  # the facade hands the global generators of rng_streams to
+                                # the device and takes them back after every step (compiled)
     self.actions_per_env = 1    # action words per env and step
     self.backdrop_chars = ''
     self.drape_kind = None      # per drape: 1 = Scrolly (fixture program only)

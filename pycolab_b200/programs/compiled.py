@@ -93,7 +93,17 @@ def lower(engine, roles):
   game.plot = np.array(_plot_record(**{'aux%d' % i: v for i, v in enumerate(plot_regs)}),
                        dtype=np.int32)
   game.dynamic_z = True                  # the kernel renders from the per-env z-order
-  game.code = compiler.link(comp, sprite_chars, drape_chars, engine.rows, engine.cols, keys)
+  # RNG slots: the generators the code draws from, in order of first use
+  streams = []
+  for ch in order:
+    for stream in comp[ch].streams:
+      if stream not in streams:
+        streams.append(stream)
+  game.rng_streams = tuple(streams)
+  game.rng_from_globals = True
+  game.program_arg[1] = len(streams)
+  game.code = compiler.link(comp, sprite_chars, drape_chars, engine.rows, engine.cols, keys,
+                            game.rng_streams)
   game.float_reward = any(c.float_reward for c in comp.values())
   game.reward_type = float if game.float_reward else int
   game.program_arg[0] = 1 if game.float_reward else 0

@@ -1,0 +1,245 @@
+"""CPU oracle of compiled code that draws from the global generators (include/pcl.h
+PCL_OP_RANDINT, PCL_OP_RANDCMP, PCL_OP_PICK).  TEST INFRASTRUCTURE ONLY.
+
+The draws are restated from the 625 MT19937 words (624 key words + position), with the
+algorithms the device runs, rather than by calling NumPy or `random`: test_drawn.py pins
+the restatement against the real generators, and the oracle then shows that the words
+the device continues give what the generators would.
+
+`make_world(game, words)` is oracle/compiled.py's `make_world` with the env's generator
+words attached: `words` is one mutable list of 625 ints per RNG slot (`game.rng_streams`
+order), and it is kept, not copied, so a trajectory that makes a new world per episode
+continues the same words, as the device does across auto-resets.  `drawn_program`
+interprets the same words as oracle/compiled.py's `compiled_program`, plus the draws.
+"""
+
+import random
+import struct
+
+import numpy as np
+
+from oracle import compiled as ocompiled
+from oracle import engine_model as em
+from pycolab_b200 import _lib
+
+_ERR_INDEX, _ERR_ARITH, _ERR_RANGE = 0x8, 0x20, 0x40
+_CMP = ('EQ', 'NE', 'LT', 'LE', 'GT', 'GE')
+
+
+# ------------------------------------------------------------------ MT19937
+def _twist(mt):
+  for j in range(624):
+    y = (mt[j] & 0x80000000) | (mt[(j + 1) % 624] & 0x7fffffff)
+    mt[j] = mt[(j + 397) % 624] ^ (y >> 1) ^ (0x9908b0df if y & 1 else 0)
+
+
+def next32(mt):
+  """One tempered output; mt[624] is the position."""
+  if mt[624] >= 624:
+    _twist(mt)
+    mt[624] = 0
+  y = mt[mt[624]]
+  mt[624] += 1
+  y ^= y >> 11
+  y ^= (y << 7) & 0x9d2c5680
+  y ^= (y << 15) & 0xefc60000
+  return y ^ (y >> 18)
+
+
+def numpy_below(mt, n):
+  """RandomState.randint(0, n), 1 <= n < 2^32: masked rejection, no output for n == 1."""
+  if n == 1:
+    return 0
+  mask = (1 << (n - 1).bit_length()) - 1
+  while True:
+    v = next32(mt) & mask
+    if v < n:
+      return v
+
+
+def python_below(mt, n):
+  """Random._randbelow(n), 1 <= n <= 2^32: getrandbits(n.bit_length()) until < n."""
+  k = n.bit_length()
+  while True:
+    if k <= 32:
+      r = next32(mt) >> (32 - k)
+    else:
+      lo = next32(mt)
+      r = lo | (next32(mt) >> 31) << 32
+    if r < n:
+      return r
+
+
+def random53(mt):
+  """NumPy's random_sample() and Python's random(): 53 bits of two outputs."""
+  a, b = next32(mt) >> 5, next32(mt) >> 6
+  return (a * 67108864.0 + b) * (1.0 / 9007199254740992.0)
+
+
+def randint(mt, rule, low, high):
+  """PCL_OP_RANDINT: the drawn int, or None for an empty range (nothing consumed)."""
+  width = high - low + (1 if rule == _lib.RAND_PYTHON_CLOSED else 0)
+  if width <= 0:
+    return None
+  return low + (numpy_below(mt, width) if rule == _lib.RAND_NUMPY else python_below(mt, width))
+
+
+# ------------------------------------------------------------------ words
+def seeded_words(game, seed):
+  """One list of words per RNG slot of `game`, seeded as BatchedEngine seeds env `seed`."""
+  from pycolab_b200 import batched
+  return [[int(w) for w in batched._mt_state(s, seed)] for s in game.rng_streams]
+
+
+def global_words(stream):
+  """The words of a global generator now."""
+  if stream == 'python':
+    return [int(w) for w in random.getstate()[1]]
+  _, key, pos = np.random.get_state()[:3]
+  return [int(w) for w in key] + [int(pos)]
+
+
+def make_world(game, words):
+  world = ocompiled.make_world(game)
+  world.program = drawn_program
+  world.rng = words
+  return world
+
+
+# ------------------------------------------------------------------ interpreter
+def _f64(lo, hi):
+  return struct.unpack('<d', struct.pack('<ii', lo, hi))[0]
+
+
+def drawn_program(world, ch, actions):
+  code, plot = world.code, world.plot
+  chars = world.entity_chars
+  me = world.things[ch]
+  action = _lib.ACTION_NONE if actions is None else int(actions)
+  stack, local = [], [0] * _lib.CODE_LOCALS
+  pc = code[1 + chars.index(ch)]
+
+  def ent(k):
+    return me if k < 0 else world.things[chars[k]]
+
+  def cell(r, c):
+    r = r + world.rows if r < 0 else r
+    c = c + world.cols if c < 0 else c
+    if 0 <= r < world.rows and 0 <= c < world.cols:
+      return r, c
+    world.error |= _ERR_INDEX
+    return None
+
+  while True:
+    op = code[pc]
+    name = _lib.OPS[op]
+    a = code[pc + 1] if pc + 1 < len(code) else 0
+    nxt = pc + 1 + _lib.OPERANDS[op]
+    if name == 'RET':
+      return
+    elif name == 'RANDINT':
+      high, low = stack.pop(), stack.pop()
+      v = randint(world.rng[a], code[pc + 2], low, high)
+      if v is None:
+        world.error |= _ERR_RANGE
+        v = low
+      stack.append(v)
+    elif name == 'RANDCMP':
+      x, y = random53(world.rng[a]), _f64(code[pc + 3], code[pc + 4])
+      stack.append(int({'EQ': x == y, 'NE': x != y, 'LT': x < y, 'LE': x <= y, 'GT': x > y,
+                        'GE': x >= y}[_CMP[code[pc + 2]]]))
+    elif name == 'PICK':
+      i = stack.pop()
+      if 0 <= i < a:
+        stack.append(code[pc + 2 + i])
+      else:
+        world.error |= _ERR_INDEX
+        stack.append(0)
+      nxt += a
+    elif name == 'PUSH':
+      stack.append(a)
+    elif name == 'POP':
+      stack.pop()
+    elif name == 'DUP':
+      stack.append(stack[-1])
+    elif name == 'LOAD':
+      stack.append(local[a])
+    elif name == 'STORE':
+      local[a] = stack.pop()
+    elif name == 'JMP':
+      nxt = a
+    elif name in ('JZ', 'JNZ'):
+      if (stack.pop() == 0) == (name == 'JZ'):
+        nxt = a
+    elif name in ('ADD', 'SUB', 'MUL', 'FLOORDIV', 'MOD', 'EQ', 'NE', 'LT', 'LE', 'GT', 'GE'):
+      y, x = stack.pop(), stack.pop()
+      if name in ('FLOORDIV', 'MOD') and y == 0:
+        world.error |= _ERR_ARITH
+        v = 0
+      else:
+        v = {'ADD': lambda: x + y, 'SUB': lambda: x - y, 'MUL': lambda: x * y,
+             'FLOORDIV': lambda: x // y, 'MOD': lambda: x % y, 'EQ': lambda: x == y,
+             'NE': lambda: x != y, 'LT': lambda: x < y, 'LE': lambda: x <= y,
+             'GT': lambda: x > y, 'GE': lambda: x >= y}[name]()
+      stack.append(ocompiled._wrap32(v))
+    elif name == 'NEG':
+      stack.append(ocompiled._wrap32(-stack.pop()))
+    elif name == 'NOT':
+      stack.append(int(stack.pop() == 0))
+    elif name == 'EQ2':
+      c2, r2, c1, r1 = stack.pop(), stack.pop(), stack.pop(), stack.pop()
+      stack.append(int(r1 == r2 and c1 == c2))
+    elif name == 'IN':
+      stack.append(int(stack.pop() in code[pc + 2:pc + 2 + a]))
+      nxt += a
+    elif name == 'ACTION':
+      stack.append(action)
+    elif name == 'FRAME':
+      stack.append(plot.frame)
+    elif name == 'FIELD':
+      w = ent(a)
+      stack.append((w.row, w.col, w.vrow, w.vcol, int(bool(w.visible)))[code[pc + 2]])
+    elif name == 'GETR':
+      stack.append(me.regs[a])
+    elif name == 'SETR':
+      me.regs[a] = stack.pop()
+    elif name == 'GETP':
+      stack.append(plot.regs[a])
+    elif name == 'SETP':
+      plot.regs[a] = stack.pop()
+    elif name in ('BOARD', 'BACKDROP', 'CURTAIN'):
+      c, r = stack.pop(), stack.pop()
+      at = cell(r, c)
+      if at is None:
+        stack.append(0)
+      elif name == 'BOARD':
+        stack.append(int(world.board[at]))
+      elif name == 'BACKDROP':
+        stack.append(int(world.backdrop[at]))
+      else:
+        stack.append(int(ent(a).curtain[at]))
+    elif name == 'SETCELL':
+      v, c, r = stack.pop(), stack.pop(), stack.pop()
+      at = cell(r, c)
+      if at is not None:
+        me.curtain[at] = v != 0
+    elif name == 'FILL':
+      me.curtain[:] = stack.pop() != 0
+    elif name == 'ANY':
+      stack.append(int(ent(a).curtain.any()))
+    elif name == 'MOVE':
+      stack.append(0 if em.walker_move(me, world.board, plot, a) is None else 1)
+    elif name == 'TELEPORT':
+      c, r = stack.pop(), stack.pop()
+      em.walker_teleport(me, r, c)
+    elif name == 'REWARD':
+      plot.add_reward(stack.pop())
+    elif name == 'REWARD_F64':
+      plot.add_reward(_f64(a, code[pc + 2]))
+    elif name == 'TERMINATE':
+      plot.terminate_episode(ocompiled._f32(a))
+    elif name == 'DISCOUNT':
+      plot.discount = ocompiled._f32(a)
+    else:
+      raise AssertionError('opcode %d' % op)
+    pc = nxt

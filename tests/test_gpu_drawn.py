@@ -1,0 +1,172 @@
+"""GPU tests of draws from the global generators in compiled code (csrc/compiled.cu
+PCL_OP_RANDINT / RANDCMP / PICK): tests/drawn_games.py on the H100, against the
+reference's trajectories (tests/golden/drawn_*.npz) and the oracle
+(tests/drawn_oracle.py)."""
+
+import os
+import random
+import sys
+
+import numpy as np
+import pytest
+
+import drawn_oracle as do
+import golden_cases as gc
+import trajectory as tj
+from pycolab_b200 import _lib, compat, compiler, lowering
+
+pytestmark = pytest.mark.gpu
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+
+@pytest.fixture(scope='module')
+def games():
+  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
+  compat.uninstall()
+  try:
+    mod = compat.load_example(os.path.join(HERE, 'drawn_games.py'))
+  finally:
+    compat.uninstall()
+    sys.modules.update(saved)
+  compiler.register(*mod.CLASSES)
+  yield mod
+  compiler.unregister(*mod.CLASSES)
+
+
+@pytest.fixture
+def global_generators():
+  """Leave NumPy's and Python's global generators as the test found them."""
+  np_state, py_state = np.random.get_state(), random.getstate()
+  yield
+  np.random.set_state(np_state)
+  random.setstate(py_state)
+
+
+@pytest.mark.parametrize('name', gc.names('drawn_'))
+def test_facade_replays_drawn_golden(games, global_generators, name):
+  g = gc.load(name)
+  game, level = bytes(g['game']).decode(), int(g['level'][0])
+  regs = games.REGISTERS[game]
+  sprites, registers, types = [], [], []
+
+  def on_frame(env, out):
+    sprites.append([[s.position[0], s.position[1], int(bool(s.visible)),
+                     s.virtual_position[0], s.virtual_position[1]]
+                    for s in (env.things[ch] for ch in games.SPRITES[game])])
+    registers.append([int(getattr(env.things[ch], attr)) for ch, attr in regs])
+    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
+  np.random.seed(int(g['rng_seed'][0]))
+  random.seed(int(g['rng_seed'][0]))
+  got = tj.run_trajectory(lambda: games.GAMES[game](level), g['actions'].tolist(),
+                          on_frame=on_frame)
+  tj.assert_same_trajectory(g, got, name)
+  np.testing.assert_array_equal(g['sprites'].reshape(len(types), -1),
+                                np.array(sprites).reshape(len(types), -1))
+  np.testing.assert_array_equal(g['registers'], np.array(registers))
+  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
+  # the generators the game drew from continue where the reference's stopped
+  assert do.global_words('numpy') == g['numpy_words'].tolist()
+  assert do.global_words('python') == g['python_words'].tolist()
+
+
+def _oracle_run(lowered, words, actions):
+  """Every frame of one env under the batched auto-reset protocol, with its registers
+  (sprite AUX0-AUX2, drape words, plot AUX0-AUX3) per frame under 'regs'."""
+  regs = []
+
+  def on_frame(world, out):
+    regs.append([r for ch in lowered.sprite_chars for r in world.things[ch].regs] +
+                [r for ch in lowered.drape_chars for r in world.things[ch].regs] +
+                list(world.plot.regs))
+    assert world.error == 0
+  traj = tj.run_trajectory(lambda: do.make_world(lowered, words), actions, on_frame=on_frame)
+  traj['regs'] = np.array(regs, dtype=np.int64)
+  return traj
+
+
+def _device_regs(eng, envs):
+  S = len(eng.sprite_chars)
+  sprites = eng.sprites[envs].cpu().numpy()[:, :, _lib.S_AUX0:].reshape(len(envs), -1)
+  drapes = eng.drapes[envs].cpu().numpy().reshape(len(envs), -1)
+  plot = eng.plot[envs].cpu().numpy()[:, _lib.P_AUX0:_lib.P_AUX0 + 4]
+  assert sprites.shape[1] == 3 * S
+  return np.concatenate([sprites, drapes, plot], axis=1).astype(np.int64)
+
+
+def test_batched_monsters_vs_oracle(games):
+  """B = 4096, both levels alternating, auto-reset, 300 steps: 128 sampled envs (the
+  first and last of each level among them) against oracle worlds whose generators are
+  seeded rng_seed + env, every step, then their final generator words."""
+  import torch
+  from pycolab_b200 import batched
+  B, T, seed = 4096, 300, 40
+  levels = [lowering.lower(games.make_monsters(k)) for k in range(2)]
+  eng = batched.BatchedEngine(levels, batch=B, rng_seed=seed)
+  rs = np.random.RandomState(13)
+  table = rs.randint(0, games.N_ACTIONS['monsters'], size=(T, B)).astype(np.int32)
+  sample = [int(e) for e in np.unique(np.concatenate(
+      [[0, 1, B - 2, B - 1], rs.choice(np.arange(2, B - 2), 124, replace=False)]))]
+  assert len(sample) == 128
+  words = {e: do.seeded_words(levels[e % 2], seed + e) for e in sample}
+  want = {e: _oracle_run(levels[e % 2], words[e], table[:, e].tolist()) for e in sample}
+  actions = torch.from_numpy(table).cuda()
+  res = eng.its_showtime()
+  episodes = 0
+  for t in range(T + 1):
+    if t > 0:
+      res = eng.play(actions[t - 1])
+    torch.cuda.synchronize()
+    boards = res.board.cpu().numpy()
+    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
+    disc, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
+    regs = _device_regs(eng, sample)
+    for k, e in enumerate(sample):
+      w = want[e]
+      assert (boards[e] == w['boards'][t]).all(), (t, e)
+      assert has[e] == w['has_reward'][t] and reward[e] == w['reward'][t], (t, e)
+      assert done[e] == w['game_over'][t], (t, e)
+      assert disc[e] == np.float32(w['discount'][t]), (t, e)
+      assert (regs[k] == w['regs'][t]).all(), (t, e, regs[k], w['regs'][t])
+    episodes += int(done.sum())
+  assert episodes > B                       # the streams run on across auto-resets
+  rng = eng.rng.cpu().numpy().view(np.uint32).reshape(B, 2, _lib.MT_WORDS)
+  for e in sample:
+    assert rng[e].tolist() == words[e], e
+  assert int((eng.error_codes() != 0).sum()) == 0
+  assert int(eng._board[:, :, eng.cols:].sum()) == 0        # the pitch padding stays zero
+
+
+def test_shards_reproduce_one_engine(games):
+  """Engines of env_offset 0 and B / 2 step as the two halves of one engine of B."""
+  import torch
+  from pycolab_b200 import batched
+  B, T = 1024, 120
+  levels = [lowering.lower(games.make_monsters(k)) for k in range(2)]
+  whole = batched.BatchedEngine(levels, batch=B, rng_seed=5)
+  halves = [batched.BatchedEngine(levels, batch=B // 2, rng_seed=5, env_offset=off)
+            for off in (0, B // 2)]
+  rs = np.random.RandomState(2)
+  outs = [whole.its_showtime()] + [h.its_showtime() for h in halves]
+  for t in range(T + 1):
+    if t > 0:
+      a = torch.from_numpy(rs.randint(0, 6, size=B).astype(np.int32)).cuda()
+      outs = [whole.play(a), halves[0].play(a[:B // 2].contiguous()),
+              halves[1].play(a[B // 2:].contiguous())]
+    torch.cuda.synchronize()
+    for field in ('board', 'reward', 'has_reward', 'discount', 'done'):
+      joined = torch.cat([getattr(outs[1], field), getattr(outs[2], field)])
+      assert bool((getattr(outs[0], field) == joined).all()), (t, field)
+  assert bool((whole.rng == torch.cat([h.rng for h in halves])).all())
+
+
+@pytest.mark.parametrize('which', [0, 1, 2], ids=['numpy_randint', 'python_randrange',
+                                                  'numpy_choice'])
+def test_empty_range_raises_value_error(games, global_generators, which):
+  engine = games.make_empty(which)
+  engine.its_showtime()
+  before = (do.global_words('numpy'), do.global_words('python'))
+  engine.play(0)
+  with pytest.raises(ValueError):
+    engine.play(1)
+  assert (do.global_words('numpy'), do.global_words('python')) == before  # nothing drawn
