@@ -8,6 +8,12 @@ same words the device runs, one instruction at a time, over the oracle's registe
 Python reference semantics it restates: NumPy cell indexing, floor `//` and `%`, rewards
 summed in call order as Python sums them (an int sum stays int), the Plot directives of
 plot.py:176-260 and MazeWalker motion (sprites.py:315-546 via engine_model).
+
+Draws from the global generators (PCL_OP_RANDINT, RANDCMP, PICK) are restated from the
+625 MT19937 words (624 key words + position), with the algorithms the device runs, rather
+than by calling NumPy or `random`: test_drawn.py pins the restatement against the real
+generators, and the oracle then shows that the words the device continues give what the
+generators would.
 """
 
 import struct
@@ -18,7 +24,8 @@ from oracle import engine_model as em
 from pycolab_b200 import _lib, lowering
 
 OP = _lib.OP
-_ERR_INDEX, _ERR_ARITH = 0x8, 0x20
+_ERR_INDEX, _ERR_ARITH, _ERR_RANGE = 0x8, 0x20, 0x40
+_CMP = ('EQ', 'NE', 'LT', 'LE', 'GT', 'GE')
 
 
 def _wrap32(x):
@@ -33,8 +40,77 @@ def _f64(lo, hi):
   return struct.unpack('<d', struct.pack('<ii', lo, hi))[0]
 
 
-def make_world(game):
-  """A fresh oracle env (the its_showtime() state) of lowered compiled game `game`."""
+# ------------------------------------------------------------------ MT19937
+def _twist(mt):
+  for j in range(624):
+    y = (mt[j] & 0x80000000) | (mt[(j + 1) % 624] & 0x7fffffff)
+    mt[j] = mt[(j + 397) % 624] ^ (y >> 1) ^ (0x9908b0df if y & 1 else 0)
+
+
+def next32(mt):
+  """One tempered output; mt[624] is the position."""
+  if mt[624] >= 624:
+    _twist(mt)
+    mt[624] = 0
+  y = mt[mt[624]]
+  mt[624] += 1
+  y ^= y >> 11
+  y ^= (y << 7) & 0x9d2c5680
+  y ^= (y << 15) & 0xefc60000
+  return y ^ (y >> 18)
+
+
+def numpy_below(mt, n):
+  """RandomState.randint(0, n), 1 <= n < 2^32: masked rejection, no output for n == 1."""
+  if n == 1:
+    return 0
+  mask = (1 << (n - 1).bit_length()) - 1
+  while True:
+    v = next32(mt) & mask
+    if v < n:
+      return v
+
+
+def python_below(mt, n):
+  """Random._randbelow(n), 1 <= n <= 2^32: getrandbits(n.bit_length()) until < n."""
+  k = n.bit_length()
+  while True:
+    if k <= 32:
+      r = next32(mt) >> (32 - k)
+    else:
+      lo = next32(mt)
+      r = lo | (next32(mt) >> 31) << 32
+    if r < n:
+      return r
+
+
+def random53(mt):
+  """NumPy's random_sample() and Python's random(): 53 bits of two outputs."""
+  a, b = next32(mt) >> 5, next32(mt) >> 6
+  return (a * 67108864.0 + b) * (1.0 / 9007199254740992.0)
+
+
+def randint(mt, rule, low, high):
+  """PCL_OP_RANDINT: the drawn int, or None for an empty range (nothing consumed)."""
+  width = high - low + (1 if rule == _lib.RAND_PYTHON_CLOSED else 0)
+  if width <= 0:
+    return None
+  return low + (numpy_below(mt, width) if rule == _lib.RAND_NUMPY else python_below(mt, width))
+
+
+def seeded_words(game, seed):
+  """One list of words per RNG slot of `game`, seeded as BatchedEngine seeds env `seed`."""
+  from pycolab_b200 import batched
+  return [[int(w) for w in batched._mt_state(s, seed)] for s in game.rng_streams]
+
+
+# ------------------------------------------------------------------ worlds
+def make_world(game, words=None):
+  """A fresh oracle env (the its_showtime() state) of lowered compiled game `game`.
+
+  `words`: for a game that draws, one mutable list of 625 ints per RNG slot
+  (`game.rng_streams` order).  It is kept, not copied, so a trajectory that makes a new
+  world per episode continues the same words, as the device does across auto-resets."""
   rows, cols = game.rows, game.cols
   ents = {}
   for s, ch in enumerate(game.sprite_chars):
@@ -58,6 +134,7 @@ def make_world(game):
   world.entity_chars = game.sprite_chars + game.drape_chars
   world.plot.regs = [int(x) for x in game.plot[_lib.P_AUX0:_lib.P_AUX0 + 4]]
   world.error = 0
+  world.rng = words
   return world
 
 
@@ -88,6 +165,25 @@ def compiled_program(world, ch, actions):
     nxt = pc + 1 + _lib.OPERANDS[op]
     if name == 'RET':
       return
+    elif name == 'RANDINT':
+      high, low = stack.pop(), stack.pop()
+      v = randint(world.rng[a], code[pc + 2], low, high)
+      if v is None:
+        world.error |= _ERR_RANGE
+        v = low
+      stack.append(v)
+    elif name == 'RANDCMP':
+      x, y = random53(world.rng[a]), _f64(code[pc + 3], code[pc + 4])
+      stack.append(int({'EQ': x == y, 'NE': x != y, 'LT': x < y, 'LE': x <= y, 'GT': x > y,
+                        'GE': x >= y}[_CMP[code[pc + 2]]]))
+    elif name == 'PICK':
+      i = stack.pop()
+      if 0 <= i < a:
+        stack.append(code[pc + 2 + i])
+      else:
+        world.error |= _ERR_INDEX
+        stack.append(0)
+      nxt += a
     elif name == 'PUSH':
       stack.append(a)
     elif name == 'POP':

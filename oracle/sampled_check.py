@@ -8,7 +8,7 @@ own level and action stream (auto-reset = a fresh world on game-over, the
 batched stand-in for "one Engine per episode", engine.py:103-104), and compare
 every step's (board, reward, has_reward, discount, done) bit for bit.
 
-Used by tests/test_gpu_sampled_parity.py and by bench.py's post-timing
+Used by the batched-vs-oracle tests and by bench.py's post-timing
 `parity_checked` leg (the checker, never the thing measured).
 """
 
@@ -27,22 +27,44 @@ def _compare(t, env, got, want, world):
     raise Mismatch('board differs at step %d env %d, first cell %s: device %r oracle %r' % (
         t, env, tuple(bad[0]), chr(board[tuple(bad[0])]), chr(w_board[tuple(bad[0])])))
   want_has = 0 if w_reward is None else 1
-  want_reward = 0 if w_reward is None else int(w_reward)
-  if (int(has), int(reward)) != (want_has, want_reward):
-    raise Mismatch('reward differs at step %d env %d: device (%d, %d) oracle %r' % (
-        t, env, int(has), int(reward), w_reward))
+  if reward.dtype == np.float64:          # a game with a float reward: the float64 bits
+    bits = np.float64(0.0 if w_reward is None else w_reward).view(np.int64)
+    same = int(has) == want_has and np.float64(reward).view(np.int64) == bits
+  else:
+    same = (int(has), int(reward)) == (want_has, 0 if w_reward is None else int(w_reward))
+  if not same:
+    raise Mismatch('reward differs at step %d env %d: device (%d, %r) oracle %r' % (
+        t, env, int(has), reward, w_reward))
   if float(disc) != float(w_disc):
     raise Mismatch('discount differs at step %d env %d: %r vs %r' % (t, env, disc, w_disc))
   if bool(done) != bool(world.game_over):
     raise Mismatch('game_over differs at step %d env %d' % (t, env))
 
 
-def lockstep(engine, make_world, env_ids, actions, crop=None):
+def sprite_words(walker):
+  """Words 0-4 of a sprite's device record for an oracle MazeWalker: row, col, vrow, vcol
+  and the flags (bit 0 visible, bits 1-2 prior visible: 0 None, 1 False, 2 True)."""
+  prior = 0 if walker.prior_visible is None else 2 if walker.prior_visible else 1
+  return (walker.row, walker.col, walker.vrow, walker.vcol,
+          int(bool(walker.visible)) | prior << 1)
+
+
+def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprites='',
+             pad_columns=False, on_step=None):
   """Step `engine` (a BatchedEngine after its_showtime(), B envs) with
   actions int32 [T, B] and, for every env in `env_ids`, an oracle world built by
-  make_world(env) in lockstep.  crop: optional (crop_spec, crop_state,
-  make_oracle_cropper) to compare a cropper view too.  Returns the number of
-  (env, step) pairs compared, resets included."""
+  make_world(env) in lockstep.  Returns the number of (env, step) pairs compared,
+  resets included.  Every step compares board, reward, has_reward, discount and done;
+  on request also:
+    crop: (crop_spec, crop_state, make_oracle_cropper): engine.crop(crop_spec,
+      state=crop_state) against a cropper that follows each oracle world.  crop_spec may
+      instead be the view engine.attach_cropper() returned (crop_state unused).
+    curtains: drape chars whose engine.curtain(ch) must equal the oracle drape's.
+    sprites: sprite chars whose record words 0-4 must equal `sprite_words` of the
+      oracle walker.
+    pad_columns: the board's pitch padding stays 0.
+    on_step(t, engine, worlds, outs): called after the comparison of step t (0 is
+      its_showtime()), with the oracle worlds and their outputs keyed by env."""
   import torch
   env_ids = [int(e) for e in env_ids]
   idx = torch.as_tensor(env_ids, dtype=torch.long, device=engine.device)
@@ -55,27 +77,42 @@ def lockstep(engine, make_world, env_ids, actions, crop=None):
     croppers = {e: make_cropper() for e in env_ids}
     for e in env_ids:
       croppers[e].set_engine(worlds[e])
+  slots = [engine.sprite_chars.index(ch) for ch in sprites]
   acts_dev = torch.from_numpy(np.ascontiguousarray(actions, dtype=np.int32)).to(engine.device)
-  compared = 0
+
+  def pick(x):
+    return x.index_select(0, idx).cpu().numpy()
 
   def check(t):
-    boards = engine.board.index_select(0, idx).cpu().numpy()
-    reward = engine.reward.index_select(0, idx).cpu().numpy()
-    has = engine.has_reward.index_select(0, idx).cpu().numpy()
-    disc = engine.discount.index_select(0, idx).cpu().numpy()
-    done = engine.done.index_select(0, idx).cpu().numpy()
+    boards, reward, has = pick(engine.board), pick(engine.reward), pick(engine.has_reward)
+    disc, done = pick(engine.discount), pick(engine.done)
     views = None
     if crop is not None:
-      views = engine.crop(crop_spec, state=crop_state).index_select(0, idx).cpu().numpy()
+      views = pick(crop_spec if torch.is_tensor(crop_spec) else
+                   engine.crop(crop_spec, state=crop_state))
+    planes = {ch: pick(engine.curtain(ch)) for ch in curtains}
+    records = pick(engine.sprites) if sprites else None
+    pad = pick(engine._board)[:, :, engine.cols:] if pad_columns else None
     for k, e in enumerate(env_ids):
-      _compare(t, e, (boards[k], reward[k], has[k], disc[k], done[k]), outs[e], worlds[e])
-      if views is not None:
-        want = croppers[e].crop(outs[e][0])
-        if not np.array_equal(views[k], want):
-          raise Mismatch('crop differs at step %d env %d' % (t, e))
+      world = worlds[e]
+      _compare(t, e, (boards[k], reward[k], has[k], disc[k], done[k]), outs[e], world)
+      if views is not None and not np.array_equal(views[k], croppers[e].crop(outs[e][0])):
+        raise Mismatch('crop differs at step %d env %d' % (t, e))
+      for ch in curtains:
+        if not np.array_equal(planes[ch][k], world.things[ch].curtain):
+          raise Mismatch('curtain %s differs at step %d env %d' % (ch, t, e))
+      for i, ch in zip(slots, sprites):
+        got, want = tuple(int(x) for x in records[k, i, :5]), sprite_words(world.things[ch])
+        if got != want:
+          raise Mismatch('sprite %s differs at step %d env %d: device %r oracle %r' % (
+              ch, t, e, got, want))
+      if pad is not None and pad[k].any():
+        raise Mismatch('pad columns differ from 0 at step %d env %d' % (t, e))
+    if on_step is not None:
+      on_step(t, engine, worlds, outs)
     return len(env_ids)
 
-  compared += check(0)
+  compared = check(0)
   for t in range(T):
     engine.play(acts_dev[t])
     for e in env_ids:

@@ -14,6 +14,7 @@ import golden_cases as gc
 import refdriver
 import trajectory as tj
 from oracle import games as ogames
+from oracle import sampled_check
 
 NAMES = gc.names('apprehend_')
 
@@ -66,7 +67,6 @@ def test_facade_apprehend_golden(name):
 def test_batched_apprehend_device_rng_vs_oracle():
   """Auto-resetting batch: env e's slopes come from random.Random(seed + e), drawn by
   the kernel at every restart; boards, rewards, float registers bit-exact."""
-  import torch
   from pycolab_b200 import _lib, batched
   from pycolab_b200.games import apprehend
   art = apprehend.GAME_ART
@@ -74,40 +74,22 @@ def test_batched_apprehend_device_rng_vs_oracle():
   eng = batched.BatchedEngine([apprehend.make_game(art)], batch=B, rng_seed=seed)
   assert eng.rng is not None
   rngs = [random.Random(seed + e) for e in range(B)]
-  worlds = [ogames.make_apprehend(art, rngs[e]) for e in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(3)
-  episodes = 0
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    spr = eng.sprites.cpu().numpy()
-    plot = eng.plot.cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e][:, :len(art[0])], outs[e][0],
-                                    err_msg='t=%d env=%d' % (t, e))
-      want = outs[e][1]
-      assert (int(res.has_reward[e]), int(res.reward[e])) == (
-          (0, 0) if want is None else (1, int(want))), (t, e)
-      assert float(res.discount[e]) == float(outs[e][2])
-      assert bool(res.done[e]) == worlds[e].game_over
-      ball = worlds[e].things['b']
+  actions = np.stack([rs.randint(0, 3, size=B) for _ in range(T)]).astype(np.int32)
+  episodes = [0]
+
+  def same_floats(t, eng, worlds, outs):
+    spr, plot = eng.sprites.cpu().numpy(), eng.plot.cpu().numpy()
+    for e, w in worlds.items():
+      ball = w.things['b']
       dx = np.array([spr[e, 1, _lib.S_AUX0], spr[e, 1, _lib.S_AUX1]], dtype='<i4').view('<f8')[0]
       acc = np.array([plot[e, _lib.P_AUX0], plot[e, _lib.P_AUX1]], dtype='<i4').view('<f8')[0]
       assert dx == ball.aux['dx'] and acc == ball.aux['acc'], (t, e, dx, ball.aux)
-    if t == T:
-      break
-    act = rs.randint(0, 3, size=B).astype(np.int32)
-    res = eng.play(torch.from_numpy(act).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        episodes += 1
-        worlds[e] = ogames.make_apprehend(art, rngs[e])
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(act[e]))
-  assert episodes > 2 * B
+      episodes[0] += int(t < T and w.game_over)
+  sampled_check.lockstep(eng, lambda e: ogames.make_apprehend(art, rngs[e]), range(B), actions,
+                         on_step=same_floats)
+  assert episodes[0] > 2 * B
   assert int(eng.error_codes().abs().max()) == 0
 
 

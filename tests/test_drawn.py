@@ -3,7 +3,7 @@
 
   - the draw forms the compiler accepts, through aliased imports too, and the forms it
     refuses, with the class, the source line and the construct;
-  - the oracle (tests/drawn_oracle.py) reproduces the reference's trajectories of
+  - the oracle (oracle/compiled.py) reproduces the reference's trajectories of
     tests/drawn_games.py (tests/golden/drawn_*.npz), down to both generators' final words;
   - the oracle's restatement of the draws equals NumPy's RandomState and Python's Random
     in value and in the words consumed, over the edge ranges and across a twist;
@@ -22,9 +22,9 @@ import numpy as np
 import pytest
 
 import boundary_sweep
-import drawn_oracle as do
 import golden_cases as gc
 import trajectory as tj
+from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compat, compiler, lowering
 from pycolab_b200.prefab_parts import sprites as b_sprites
 
@@ -205,7 +205,7 @@ def run_oracle(games, g):
   """The oracle's trajectory of golden `g`, its per-frame records and final words."""
   game, level = bytes(g['game']).decode(), int(g['level'][0])
   lowered = lowering.lower(games.GAMES[game](level))
-  words = do.seeded_words(lowered, int(g['rng_seed'][0]))
+  words = ocompiled.seeded_words(lowered, int(g['rng_seed'][0]))
   regs = games.REGISTERS[game]
   slot = {(ch, attr): compiler.registered(type(games.GAMES[game](level).things[ch])).attrs.index(
       attr) for ch, attr in regs}
@@ -217,7 +217,7 @@ def run_oracle(games, g):
     registers.append([world.things[ch].regs[slot[ch, attr]] for ch, attr in regs])
     types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
     assert world.error == 0
-  got = tj.run_trajectory(lambda: do.make_world(lowered, words), g['actions'].tolist(),
+  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered, words), g['actions'].tolist(),
                           on_frame=on_frame)
   final = dict(zip(lowered.rng_streams, words))
   return got, sprites, registers, types, final
@@ -259,14 +259,14 @@ def test_numpy_restatement_matches_random_state(seed):
         want = int(rs.randint(low, high))
       except ValueError:
         pass
-      assert do.randint(words, _lib.RAND_NUMPY, low, high) == want, (seed, rep, low, high)
+      assert ocompiled.randint(words, _lib.RAND_NUMPY, low, high) == want, (seed, rep, low, high)
       assert words == _numpy_words(rs), (seed, rep, low, high)
-    assert int(rs.choice(1)) == do.randint(words, _lib.RAND_NUMPY, 0, 1) == 0
+    assert int(rs.choice(1)) == ocompiled.randint(words, _lib.RAND_NUMPY, 0, 1) == 0
     with pytest.raises(ValueError):
       rs.choice(0)
-    assert do.randint(words, _lib.RAND_NUMPY, 0, 0) is None
-    assert rs.choice((4, -1, 6)) == (4, -1, 6)[do.randint(words, _lib.RAND_NUMPY, 0, 3)]
-    assert rs.random_sample() == do.random53(words)
+    assert ocompiled.randint(words, _lib.RAND_NUMPY, 0, 0) is None
+    assert rs.choice((4, -1, 6)) == (4, -1, 6)[ocompiled.randint(words, _lib.RAND_NUMPY, 0, 3)]
+    assert rs.random_sample() == ocompiled.random53(words)
     assert words == _numpy_words(rs)
 
 
@@ -281,17 +281,17 @@ def test_python_restatement_matches_random(seed):
         want = r.randrange(low, high)
       except ValueError:
         pass
-      assert do.randint(words, _lib.RAND_PYTHON, low, high) == want, (seed, rep, low, high)
+      assert ocompiled.randint(words, _lib.RAND_PYTHON, low, high) == want, (seed, rep, low, high)
       assert words == list(r.getstate()[1]), (seed, rep, low, high)
       if high - 1 >= low:                   # randint(a, b) over [a, b]: up to 2^32 values
-        assert (r.randint(low, high) ==
-                do.randint(words, _lib.RAND_PYTHON_CLOSED, low, high)), (seed, rep, low, high)
+        assert r.randint(low, high) == ocompiled.randint(
+            words, _lib.RAND_PYTHON_CLOSED, low, high), (seed, rep, low, high)
         assert words == list(r.getstate()[1])
-    assert r.randint(-2 ** 31, 2 ** 31 - 1) == do.randint(
+    assert r.randint(-2 ** 31, 2 ** 31 - 1) == ocompiled.randint(
         words, _lib.RAND_PYTHON_CLOSED, -2 ** 31, 2 ** 31 - 1)
-    assert r.randrange(1) == do.randint(words, _lib.RAND_PYTHON, 0, 1) == 0
-    assert r.choice((4, -1, 6)) == (4, -1, 6)[do.randint(words, _lib.RAND_PYTHON, 0, 3)]
-    assert r.random() == do.random53(words)
+    assert r.randrange(1) == ocompiled.randint(words, _lib.RAND_PYTHON, 0, 1) == 0
+    assert r.choice((4, -1, 6)) == (4, -1, 6)[ocompiled.randint(words, _lib.RAND_PYTHON, 0, 3)]
+    assert r.random() == ocompiled.random53(words)
     assert words == list(r.getstate()[1])
 
 

@@ -8,6 +8,7 @@ import pytest
 import golden_cases as gc
 import trajectory as tj
 from oracle import games as ogames
+from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
@@ -39,47 +40,28 @@ def test_facade_aperture_golden(name):
 
 @pytest.mark.parametrize('which', ['aperture_stock_L1', 'aperture_stock_L2', 'other'])
 def test_batched_aperture_vs_oracle(which):
-  import torch
   from pycolab_b200 import batched, levels
   from pycolab_b200.games import aperture
   art = levels.aperture_level() if which == 'other' else tj.u8_to_art(gc.load(which)['art'])
   B, T = 96, 400
   eng = batched.BatchedEngine([aperture.make_game(art)], batch=B)
-  worlds = [ogames.make_aperture(art) for _ in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(11)
   actions = rs.choice(list(range(10)), size=(T, B),
                       p=[.14, .14, .14, .14, .04, .1, .1, .1, .095, .005]).astype(np.int32)
-  episodes = teleports = 0
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    discount, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
-    sprites = eng.sprites.cpu().numpy()
-    curtain = eng.curtain('X').cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d e=%d' % (t, e))
-      want = outs[e][1]
-      assert (int(has[e]), int(reward[e])) == ((0, 0) if want is None else (1, int(want)))
-      assert float(discount[e]) == float(outs[e][2])
-      assert bool(done[e]) == worlds[e].game_over
-      w = worlds[e].things['A']
-      assert tuple(sprites[e, 0, :4]) == (w.row, w.col, w.vrow, w.vcol)
-      np.testing.assert_array_equal(curtain[e], worlds[e].things['X'].curtain)
-    if t == T:
-      break
-    res = eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        episodes += 1
-        worlds[e] = ogames.make_aperture(art)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        before = worlds[e].things['A'].position
-        outs[e] = worlds[e].play(int(actions[t, e]))
-        after = worlds[e].things['A'].position
-        teleports += abs(before[0] - after[0]) + abs(before[1] - after[1]) > 1
-  assert episodes > 0 and teleports > 0
+  last = {}
+  count = {'episodes': 0, 'teleports': 0}
+
+  def count_episodes_and_teleports(t, eng, worlds, outs):
+    for e, w in worlds.items():
+      now = w.things['A'].position
+      if e in last and last[e][0] is not w:   # the world was rebuilt: an episode ended
+        count['episodes'] += 1
+      elif e in last:
+        before = last[e][1]
+        count['teleports'] += abs(before[0] - now[0]) + abs(before[1] - now[1]) > 1
+      last[e] = (w, now)
+  sampled_check.lockstep(eng, lambda e: ogames.make_aperture(art), range(B), actions,
+                         curtains='X', sprites='A', on_step=count_episodes_and_teleports)
+  assert count['episodes'] > 0 and count['teleports'] > 0
   assert int(eng.error_codes().abs().max()) == 0

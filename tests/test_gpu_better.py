@@ -8,6 +8,7 @@ import golden_cases as gc
 import trajectory as tj
 from oracle import engine_model as em
 from oracle import games as ogames
+from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
@@ -48,47 +49,20 @@ def test_facade_better_scrolly_golden_with_croppers(name):
 
 
 def test_batched_better_scrolly_vs_oracle():
-  import torch
   from pycolab_b200 import batched
   from pycolab_b200.games import better_scrolly_maze as bsm
   g = gc.load('better_stock_L1')
   art = tj.u8_to_art(g['art'])
   B, T = 20, 300
   eng = batched.BatchedEngine([bsm.make_game(art)], batch=B)
-  worlds = [ogames.make_better_scrolly(art) for _ in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(8)
   actions = rs.randint(0, 6, size=(T, B)).astype(np.int32)
   actions[rs.random_sample(actions.shape) < 0.97] %= 5
   spec = batched.scrolling_crop_spec(7, 10, eng.sprite_chars.index('c'), pad_char=' ',
                                      scroll_margins=(None, 3))
-  crops = [em.ScrollingCrop(7, 10, ['c'], pad_char=' ', scroll_margins=(None, 3))
-           for _ in range(B)]
-  for c, w in zip(crops, worlds):
-    c.set_engine(w)
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    view = eng.crop(spec).cpu().numpy()
-    cur = eng.curtain('@').cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d e=%d' % (t, e))
-      want = outs[e][1]
-      assert (int(res.has_reward[e]), int(res.reward[e])) == (
-          (0, 0) if want is None else (1, int(want)))
-      assert float(res.discount[e]) == float(outs[e][2])
-      assert bool(res.done[e]) == worlds[e].game_over
-      np.testing.assert_array_equal(view[e], crops[e].crop(outs[e][0]))
-      np.testing.assert_array_equal(cur[e], worlds[e].things['@'].curtain)
-    if t == T:
-      break
-    res = eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        worlds[e] = ogames.make_better_scrolly(art)
-        crops[e].set_engine(worlds[e])
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
+  sampled_check.lockstep(
+      eng, lambda e: ogames.make_better_scrolly(art), range(B), actions, curtains='@',
+      crop=(spec, None, lambda: em.ScrollingCrop(7, 10, ['c'], pad_char=' ',
+                                                 scroll_margins=(None, 3))))
   assert int(eng.error_codes().abs().max()) == 0

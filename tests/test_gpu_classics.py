@@ -10,6 +10,7 @@ import pytest
 import golden_cases as gc
 import trajectory as tj
 from oracle import games as ogames
+from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
@@ -40,47 +41,34 @@ def test_facade_classics_golden(name):
   np.testing.assert_array_equal(g['reward_type'][:n + 1], np.array(types, dtype=np.uint8))
 
 
+def _batched_vs_oracle(game, make_world, actions):
+  """Auto-resetting batch against one oracle world per env: boards, rewards, discounts,
+  done flags and the player's sprite record every step.  Returns the episodes that ended."""
+  from pycolab_b200 import batched
+  T, B = actions.shape
+  eng = batched.BatchedEngine([game], batch=B)
+  eng.its_showtime()
+  episodes = [0]
+
+  def count(t, eng, worlds, outs):
+    episodes[0] += sum(w.game_over for w in worlds.values()) if t < T else 0
+  sampled_check.lockstep(eng, lambda e: make_world(), range(B), actions, sprites='P',
+                         on_step=count)
+  assert int(eng.error_codes().abs().max()) == 0
+  return episodes[0]
+
+
 @pytest.mark.parametrize('kind', ogames.CLASSIC_KINDS)
 @pytest.mark.parametrize('which', ['stock', 'other'])
 def test_batched_classics_vs_oracle(kind, which):
-  import torch
-  from pycolab_b200 import batched, levels
+  from pycolab_b200 import levels
   mod = _module(kind)
   art = list(mod.GAME_ART) if which == 'stock' else levels.classic_level(kind)
   B, T = 67, 300
-  eng = batched.BatchedEngine([mod.make_game(art)], batch=B)
-  worlds = [ogames.make_classic(kind, art) for _ in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
   n_actions = 3 if kind == 'chain_walk' else 6
   actions = np.random.RandomState(B).randint(0, n_actions, size=(T, B)).astype(np.int32)
-  episodes = 0
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    discount, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
-    sprites = eng.sprites.cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d e=%d' % (t, e))
-      want = outs[e][1]
-      assert (int(has[e]), int(reward[e])) == ((0, 0) if want is None else (1, int(want)))
-      assert float(discount[e]) == float(outs[e][2])
-      assert bool(done[e]) == worlds[e].game_over
-      w = worlds[e].things['P']
-      assert tuple(sprites[e, 0, :4]) == (w.row, w.col, w.vrow, w.vcol)
-    if t == T:
-      break
-    res = eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        episodes += 1
-        worlds[e] = ogames.make_classic(kind, art)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
-  assert episodes > 0
-  assert int(eng.error_codes().abs().max()) == 0
+  assert _batched_vs_oracle(mod.make_game(art), lambda: ogames.make_classic(kind, art),
+                            actions) > 0
 
 
 @pytest.mark.parametrize('name', gc.names('fluvial_'))
@@ -110,41 +98,10 @@ def test_facade_fluvial_natation_golden(name):
 
 @pytest.mark.parametrize('which', ['stock', 'other'])
 def test_batched_fluvial_natation_vs_oracle(which):
-  import torch
-  from pycolab_b200 import batched, levels
+  from pycolab_b200 import levels
   from pycolab_b200.games import fluvial_natation
   art = list(fluvial_natation.GAME_ART) if which == 'stock' else levels.fluvial_level()
   B, T = 45, 260
-  eng = batched.BatchedEngine([fluvial_natation.make_game(art)], batch=B)
-  worlds = [ogames.make_fluvial(art) for _ in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
   actions = np.random.RandomState(3).choice([0, 1, 2], size=(T, B), p=[.2, .6, .2]).astype(np.int32)
-  episodes = 0
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    discount, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
-    sprites = eng.sprites.cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d e=%d' % (t, e))
-      want = outs[e][1]
-      assert (int(has[e]), int(reward[e])) == ((0, 0) if want is None else (1, int(want)))
-      assert float(discount[e]) == float(outs[e][2])
-      assert bool(done[e]) == worlds[e].game_over
-      w = worlds[e].things['P']
-      assert tuple(sprites[e, 0, :5]) == (w.row, w.col, w.vrow, w.vcol,
-                                          int(bool(w.visible)) | ((0 if w.prior_visible is None else 2 if w.prior_visible else 1) << 1))
-    if t == T:
-      break
-    res = eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        episodes += 1
-        worlds[e] = ogames.make_fluvial(art)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
-  assert episodes > 0
-  assert int(eng.error_codes().abs().max()) == 0
+  assert _batched_vs_oracle(fluvial_natation.make_game(art), lambda: ogames.make_fluvial(art),
+                            actions) > 0

@@ -1,7 +1,7 @@
 """GPU tests of draws from the global generators in compiled code (csrc/compiled.cu
 PCL_OP_RANDINT / RANDCMP / PICK): tests/drawn_games.py on the H100, against the
 reference's trajectories (tests/golden/drawn_*.npz) and the oracle
-(tests/drawn_oracle.py)."""
+(oracle/compiled.py)."""
 
 import os
 import random
@@ -10,9 +10,10 @@ import sys
 import numpy as np
 import pytest
 
-import drawn_oracle as do
 import golden_cases as gc
 import trajectory as tj
+from oracle import compiled as ocompiled
+from oracle import sampled_check
 from pycolab_b200 import _lib, compat, compiler, lowering
 
 pytestmark = pytest.mark.gpu
@@ -32,6 +33,14 @@ def games():
   compiler.register(*mod.CLASSES)
   yield mod
   compiler.unregister(*mod.CLASSES)
+
+
+def global_words(stream):
+  """The words of a global generator now."""
+  if stream == 'python':
+    return [int(w) for w in random.getstate()[1]]
+  _, key, pos = np.random.get_state()[:3]
+  return [int(w) for w in key] + [int(pos)]
 
 
 @pytest.fixture
@@ -66,23 +75,8 @@ def test_facade_replays_drawn_golden(games, global_generators, name):
   np.testing.assert_array_equal(g['registers'], np.array(registers))
   np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
   # the generators the game drew from continue where the reference's stopped
-  assert do.global_words('numpy') == g['numpy_words'].tolist()
-  assert do.global_words('python') == g['python_words'].tolist()
-
-
-def _oracle_run(lowered, words, actions):
-  """Every frame of one env under the batched auto-reset protocol, with its registers
-  (sprite AUX0-AUX2, drape words, plot AUX0-AUX3) per frame under 'regs'."""
-  regs = []
-
-  def on_frame(world, out):
-    regs.append([r for ch in lowered.sprite_chars for r in world.things[ch].regs] +
-                [r for ch in lowered.drape_chars for r in world.things[ch].regs] +
-                list(world.plot.regs))
-    assert world.error == 0
-  traj = tj.run_trajectory(lambda: do.make_world(lowered, words), actions, on_frame=on_frame)
-  traj['regs'] = np.array(regs, dtype=np.int64)
-  return traj
+  assert global_words('numpy') == g['numpy_words'].tolist()
+  assert global_words('python') == g['python_words'].tolist()
 
 
 def _device_regs(eng, envs):
@@ -97,8 +91,8 @@ def _device_regs(eng, envs):
 def test_batched_monsters_vs_oracle(games):
   """B = 4096, both levels alternating, auto-reset, 300 steps: 128 sampled envs (the
   first and last of each level among them) against oracle worlds whose generators are
-  seeded rng_seed + env, every step, then their final generator words."""
-  import torch
+  seeded rng_seed + env, every step, registers included, then their final generator
+  words."""
   from pycolab_b200 import batched
   B, T, seed = 4096, 300, 40
   levels = [lowering.lower(games.make_monsters(k)) for k in range(2)]
@@ -108,28 +102,22 @@ def test_batched_monsters_vs_oracle(games):
   sample = [int(e) for e in np.unique(np.concatenate(
       [[0, 1, B - 2, B - 1], rs.choice(np.arange(2, B - 2), 124, replace=False)]))]
   assert len(sample) == 128
-  words = {e: do.seeded_words(levels[e % 2], seed + e) for e in sample}
-  want = {e: _oracle_run(levels[e % 2], words[e], table[:, e].tolist()) for e in sample}
-  actions = torch.from_numpy(table).cuda()
-  res = eng.its_showtime()
-  episodes = 0
-  for t in range(T + 1):
-    if t > 0:
-      res = eng.play(actions[t - 1])
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    disc, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
+  words = {e: ocompiled.seeded_words(levels[e % 2], seed + e) for e in sample}
+  eng.its_showtime()
+  episodes = [0]
+
+  def same_registers(t, eng, worlds, outs):
     regs = _device_regs(eng, sample)
     for k, e in enumerate(sample):
-      w = want[e]
-      assert (boards[e] == w['boards'][t]).all(), (t, e)
-      assert has[e] == w['has_reward'][t] and reward[e] == w['reward'][t], (t, e)
-      assert done[e] == w['game_over'][t], (t, e)
-      assert disc[e] == np.float32(w['discount'][t]), (t, e)
-      assert (regs[k] == w['regs'][t]).all(), (t, e, regs[k], w['regs'][t])
-    episodes += int(done.sum())
-  assert episodes > B                       # the streams run on across auto-resets
+      w = worlds[e]
+      want = ([r for ch in eng.sprite_chars for r in w.things[ch].regs] +
+              [r for ch in eng.drape_chars for r in w.things[ch].regs] + list(w.plot.regs))
+      assert (regs[k] == want).all(), (t, e, regs[k], want)
+      assert w.error == 0
+    episodes[0] += int(eng.done.sum())
+  sampled_check.lockstep(eng, lambda e: ocompiled.make_world(levels[e % 2], words[e]), sample,
+                         table, pad_columns=True, on_step=same_registers)
+  assert episodes[0] > B                    # the streams run on across auto-resets
   rng = eng.rng.cpu().numpy().view(np.uint32).reshape(B, 2, _lib.MT_WORDS)
   for e in sample:
     assert rng[e].tolist() == words[e], e
@@ -165,8 +153,8 @@ def test_shards_reproduce_one_engine(games):
 def test_empty_range_raises_value_error(games, global_generators, which):
   engine = games.make_empty(which)
   engine.its_showtime()
-  before = (do.global_words('numpy'), do.global_words('python'))
+  before = (global_words('numpy'), global_words('python'))
   engine.play(0)
   with pytest.raises(ValueError):
     engine.play(1)
-  assert (do.global_words('numpy'), do.global_words('python')) == before  # nothing drawn
+  assert (global_words('numpy'), global_words('python')) == before  # nothing drawn

@@ -127,9 +127,9 @@ def test_batched_unoccluded_layers_vs_oracle():
   """`pcl_layers` over a batch of scrolly_maze envs == the oracle's un-occluded
   layers (backdrop characters, both Scrolly curtains incl. the stale coin cell,
   every sprite) at every step."""
-  import torch
   from oracle import engine_model as em
   from oracle import games as ogames
+  from oracle import sampled_check
   from pycolab_b200 import batched, levels, lowering
   from pycolab_b200.games import scrolly_maze as g
   arts = [levels.scrolly_maze_level(60 + i, world_shape=(65, 65), board_shape=(24, 40))
@@ -137,24 +137,17 @@ def test_batched_unoccluded_layers_vs_oracle():
   games = [lowering.lower(g.make_game(*a)) for a in arts]
   B, T = 12, 60
   eng = batched.BatchedEngine(games, batch=B)
-  worlds = [ogames.make_scrolly_maze(arts[e % 3][0], arts[e % 3][1], '+', arts[e % 3][2])
-            for e in range(B)]
-  for w in worlds:
-    w.its_showtime()
   eng.its_showtime()
   chars = eng.chars
   rs = np.random.RandomState(3)
-  for t in range(T):
+  actions = np.stack([rs.randint(0, 5, size=B) for _ in range(T)]).astype(np.int32)
+
+  def same_layers(t, eng, worlds, outs):
     planes = eng.unoccluded_layers().cpu().numpy()
-    for e in range(B):
-      want = em.unoccluded_layers_of(worlds[e].backdrop, worlds[e].things, list(chars))
+    for e, w in worlds.items():
+      want = em.unoccluded_layers_of(w.backdrop, w.things, list(chars))
       for k, ch in enumerate(chars):
         np.testing.assert_array_equal(planes[e, k], want[ch], err_msg='t=%d env=%d %r' % (t, e, ch))
-    act = rs.randint(0, 5, size=B).astype(np.int32)
-    eng.play(torch.from_numpy(act).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        worlds[e] = ogames.make_scrolly_maze(arts[e % 3][0], arts[e % 3][1], '+', arts[e % 3][2])
-        worlds[e].its_showtime()
-      else:
-        worlds[e].play(int(act[e]))
+  sampled_check.lockstep(
+      eng, lambda e: ogames.make_scrolly_maze(arts[e % 3][0], arts[e % 3][1], '+', arts[e % 3][2]),
+      range(B), actions, on_step=same_layers)

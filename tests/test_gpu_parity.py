@@ -12,6 +12,7 @@ import golden_cases as gc
 import trajectory as tj
 from oracle import engine_model as em
 from oracle import games as ogames
+from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
@@ -86,45 +87,16 @@ def test_facade_marauders_golden(name):
 # ------------------------------------------------- batched engine vs oracle
 
 def _batched_vs_oracle(make_facade_game, make_oracle, actions, n_levels=1,
-                       rng_seed=None, check_curtains=()):
+                       rng_seed=None, check_curtains=''):
   """Step a BatchedEngine (auto-reset) and B oracle worlds in lockstep.
 
   actions: int array [T, B].  make_* take the level index (env % n_levels)."""
   from pycolab_b200 import batched
-  T, B = actions.shape
+  B = actions.shape[1]
   games = [make_facade_game(i) for i in range(n_levels)]
   eng = batched.BatchedEngine(games, batch=B, rng_seed=rng_seed or 0)
-  worlds = [make_oracle(e) for e in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
-  torch = _torch()
-  acts = torch.from_numpy(actions.astype(np.int32)).cuda()
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    disc, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d env=%d' % (t, e))
-      want_r = outs[e][1]
-      assert (int(has[e]), int(reward[e])) == (
-          (0, 0) if want_r is None else (1, int(want_r))), (t, e)
-      assert float(disc[e]) == float(outs[e][2]), (t, e)
-      assert bool(done[e]) == worlds[e].game_over, (t, e)
-    for ch in check_curtains:
-      cur = eng.curtain(ch).cpu().numpy()
-      for e in range(B):
-        np.testing.assert_array_equal(cur[e], worlds[e].things[ch].curtain,
-                                      err_msg='curtain %s t=%d env=%d' % (ch, t, e))
-    if t == T:
-      break
-    res = eng.play(acts[t])
-    for e in range(B):
-      if worlds[e].game_over:               # the auto-reset rule
-        worlds[e] = make_oracle(e)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
+  eng.its_showtime()
+  sampled_check.lockstep(eng, make_oracle, range(B), actions, curtains=check_curtains)
   assert int(eng.error_codes().max()) == 0
   return eng
 
@@ -245,32 +217,12 @@ def test_batched_crop_vs_oracle():
   B, T = 16, 80
   eng = batched.BatchedEngine([scrolly_maze.make_game(*art)], batch=B)
   spec = batched.scrolling_crop_spec(9, 9, 0, pad_char=' ', scroll_margins=(None, None))
-  worlds = [ogames.make_scrolly_maze(art[0], art[1], '+', art[2]) for _ in range(B)]
-  crops = [em.ScrollingCrop(9, 9, ['P'], pad_char=' ', scroll_margins=(None, None))
-           for _ in range(B)]
-  outs = []
-  for w, c in zip(worlds, crops):
-    c.set_engine(w)
-    outs.append(w.its_showtime())
   eng.its_showtime()
-  rs = np.random.RandomState(5)
-  actions = rs.randint(0, 5, size=(T, B)).astype(np.int32)
-  torch = _torch()
-  for t in range(T + 1):
-    got = eng.crop(spec).cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(got[e], crops[e].crop(outs[e][0]),
-                                    err_msg='t=%d env=%d' % (t, e))
-    if t == T:
-      break
-    eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        worlds[e] = ogames.make_scrolly_maze(art[0], art[1], '+', art[2])
-        crops[e].set_engine(worlds[e])
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
+  actions = np.random.RandomState(5).randint(0, 5, size=(T, B)).astype(np.int32)
+  sampled_check.lockstep(
+      eng, lambda e: ogames.make_scrolly_maze(art[0], art[1], '+', art[2]), range(B), actions,
+      crop=(spec, None, lambda: em.ScrollingCrop(9, 9, ['P'], pad_char=' ',
+                                                 scroll_margins=(None, None))))
 
 
 @pytest.mark.parametrize('pad,margins,rows,cols', [(' ', (None, None), 9, 9), (None, (2, 3), 11, 13),
@@ -288,41 +240,25 @@ def test_attached_cropper_vs_oracle(pad, margins, rows, cols):
   view = eng.attach_cropper(spec)
   assert eng._attached[3], 'the scrolly program runs the cropper inside the step kernel'
   twin_state = eng.new_crop_state()
-  worlds = [ogames.make_scrolly_maze(art[0], art[1], '+', art[2]) for _ in range(B)]
-  crops = [em.ScrollingCrop(rows, cols, ['P'], pad_char=pad, scroll_margins=margins)
-           for _ in range(B)]
-  outs = []
-  for w, c in zip(worlds, crops):
-    c.set_engine(w)
-    outs.append(w.its_showtime())
-  l0 = eng.launch_count()
+  l0 = [eng.launch_count()]
   eng.its_showtime()
-  rs = np.random.RandomState(6)
-  actions = rs.randint(0, 5, size=(T, B)).astype(np.int32)
-  torch = _torch()
-  for t in range(T + 1):
-    assert eng.launch_count() == l0 + t + 1                    # one launch per step, crop included
+  actions = np.random.RandomState(6).randint(0, 5, size=(T, B)).astype(np.int32)
+
+  def same_as_the_crop_kernel(t, eng, worlds, outs):
+    assert eng.launch_count() == l0[0] + t + 1                 # one launch per step, crop included
     got = view.cpu().numpy()
     l1 = eng.launch_count()
     twin = eng.crop(spec, state=twin_state).cpu().numpy()      # the stand-alone kernel
-    l0 += eng.launch_count() - l1
+    l0[0] += eng.launch_count() - l1
     np.testing.assert_array_equal(got, twin)
-    for e in range(B):
-      np.testing.assert_array_equal(got[e], crops[e].crop(outs[e][0]),
-                                    err_msg='t=%d env=%d' % (t, e))
-    if t == T:
-      break
-    eng.play(torch.from_numpy(actions[t]).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        worlds[e] = ogames.make_scrolly_maze(art[0], art[1], '+', art[2])
-        crops[e].set_engine(worlds[e])
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
+  sampled_check.lockstep(
+      eng, lambda e: ogames.make_scrolly_maze(art[0], art[1], '+', art[2]), range(B), actions,
+      crop=(view, None, lambda: em.ScrollingCrop(rows, cols, ['P'], pad_char=pad,
+                                                 scroll_margins=margins)),
+      on_step=same_as_the_crop_kernel)
   eng.attach_cropper(None)
   before = view.clone()
-  eng.play(torch.from_numpy(actions[0]).cuda())
+  eng.play(_torch().from_numpy(actions[0]).cuda())
   assert bool((view == before).all())                          # detached: untouched
 
 

@@ -17,6 +17,7 @@ import pytest
 import scrolly_shapes as ss
 from oracle import engine_model as em
 from oracle import games as ogames
+from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
@@ -48,64 +49,19 @@ def _step_vs_oracle(games, make_oracle, actions, check_curtains, sprite_chars, r
   """Step a BatchedEngine (auto-reset) and B oracle worlds in lockstep; compare everything.
 
   games: lowered games or facade Engines (env e plays games[e % len(games)]).
-  on_step(eng, worlds): called after every comparison.  crop: (spec, make_crop(world))
-  to attach a cropper to the step kernel and compare its view every step too."""
+  on_step: sampled_check.lockstep's hook.  crop: (spec, make_crop()) to attach a cropper
+  to the step kernel and compare its view every step too."""
   from pycolab_b200 import batched
-  torch = _torch()
-  T, B = actions.shape
+  B = actions.shape[1]
   eng = batched.BatchedEngine(games, batch=B, rng_seed=rng_seed)
-  H, W, pitch = eng.rows, eng.cols, eng.pitch
-  worlds = [make_oracle(e) for e in range(B)]
-  crops = view = None
+  assert eng._board.shape == (B, eng.rows, eng.pitch)
   if crop is not None:
     view = eng.attach_cropper(crop[0])
     assert eng._attached[3], 'the cropper runs inside the step kernel'
-    crops = [crop[1](w) for w in worlds]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
-  acts = torch.from_numpy(actions.astype(np.int32)).cuda()
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    full = eng._board.cpu().numpy()
-    assert full.shape == (B, H, pitch)
-    assert not full[:, :, W:].any(), 't=%d: pad columns are not 0' % t
-    reward, has = res.reward.cpu().numpy(), res.has_reward.cpu().numpy()
-    disc, done = res.discount.cpu().numpy(), res.done.cpu().numpy()
-    sprites = eng.sprites.cpu().numpy()
-    got_view = None if view is None else view.cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(full[e, :, :W], outs[e][0], err_msg='t=%d env=%d' % (t, e))
-      want_r = outs[e][1]
-      assert (int(has[e]), int(reward[e])) == ((0, 0) if want_r is None else (1, int(want_r))), (t, e)
-      assert float(disc[e]) == float(outs[e][2]), (t, e)
-      assert bool(done[e]) == worlds[e].game_over, (t, e)
-      for i, ch in enumerate(sprite_chars):
-        w = worlds[e].things[ch]
-        rec = sprites[e, i]
-        assert (rec[0], rec[1], rec[4] & 1) == (w.row, w.col, int(bool(w.visible))), (t, e, ch)
-        if hasattr(w, 'vrow'):
-          assert (rec[2], rec[3]) == (w.vrow, w.vcol), (t, e, ch)
-      if crops is not None:
-        np.testing.assert_array_equal(got_view[e], crops[e].crop(outs[e][0]),
-                                      err_msg='crop t=%d env=%d' % (t, e))
-    for ch in check_curtains:
-      cur = eng.curtain(ch).cpu().numpy()
-      for e in range(B):
-        np.testing.assert_array_equal(cur[e], worlds[e].things[ch].curtain,
-                                      err_msg='curtain %s t=%d env=%d' % (ch, t, e))
-    if on_step is not None:
-      on_step(eng, worlds)
-    if t == T:
-      break
-    res = eng.play(acts[t])
-    for e in range(B):
-      if worlds[e].game_over:               # the auto-reset rule
-        worlds[e] = make_oracle(e)
-        if crops is not None:
-          crops[e] = crop[1](worlds[e])
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(actions[t, e]))
+    crop = (view, None, crop[1])
+  eng.its_showtime()
+  sampled_check.lockstep(eng, make_oracle, range(B), actions, crop=crop, curtains=check_curtains,
+                         sprites=sprite_chars, pad_columns=True, on_step=on_step)
   assert int(eng.error_codes().abs().max()) == 0
   return eng
 
@@ -172,7 +128,7 @@ def test_scrolly_window_corner_crosses_word_boundaries():
   both halves of the staged 64-bit word pair (wsh & 32) and many shifts within it."""
   seen = set()
 
-  def record(eng, worlds):
+  def record(t, eng, worlds, outs):
     seen.update((eng.drapes[:, 0, 1].cpu().numpy() & 63).tolist())
   _scrolly_case('12x20_sweep', B=10, T=150, corners=[(5, 20), (5, 56), (5, 84)], on_step=record,
                 shape=((12, 20), (22, 161), ss.DEFAULT_MARGINS))
@@ -186,10 +142,10 @@ def test_scrolly_different_margins_per_drape(name):
   drape never issues an order of its own here: it runs after the player, whose motion
   permits are by then for the next frame.  So both corners stay equal, and the kernel's
   restage of the coin window never runs; the registers must say so."""
-  def same_corners(eng, worlds):
+  def same_corners(t, eng, worlds, outs):
     d = eng.drapes.cpu().numpy()
     np.testing.assert_array_equal(d[:, 0, :2], d[:, 1, :2])
-    for e, w in enumerate(worlds):
+    for e, w in worlds.items():
       assert tuple(d[e, 0, :2]) == w.things['#'].corner == w.things['@'].corner
   _scrolly_case(name, corners=[(5, 52), (5, 60), (5, 20)], on_step=same_corners)
 
@@ -211,10 +167,8 @@ def test_scrolly_attached_cropper_board_shapes(name, pitch, rows, cols, pad):
   margins = (1, 1)
   spec = batched.scrolling_crop_spec(rows, cols, 0, pad_char=pad, scroll_margins=margins)
 
-  def make_crop(world):
-    c = em.ScrollingCrop(rows, cols, ['P'], pad_char=pad, scroll_margins=margins)
-    c.set_engine(world)
-    return c
+  def make_crop():
+    return em.ScrollingCrop(rows, cols, ['P'], pad_char=pad, scroll_margins=margins)
   _scrolly_case(name, B=7, T=100, pitch=pitch, crop=(spec, make_crop))
 
 

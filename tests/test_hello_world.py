@@ -11,6 +11,7 @@ import golden_cases as gc
 import refdriver
 import trajectory as tj
 from oracle import games as ogames
+from oracle import sampled_check
 
 NAMES = gc.names('hello_')
 
@@ -60,37 +61,16 @@ def test_facade_hello_golden(name):
 
 @pytest.mark.gpu
 def test_batched_hello_vs_oracle():
-  import torch
   from pycolab_b200 import batched
   from pycolab_b200.games import hello_world
   art = hello_world.HELLO_ART
   B, T = 19, 200
   eng = batched.BatchedEngine([hello_world.make_game(art)], batch=B)
-  worlds = [ogames.make_hello(art) for _ in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(8)
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    cur = eng.curtain('@').cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d env=%d' % (t, e))
-      np.testing.assert_array_equal(cur[e], worlds[e].things['@'].curtain)
-      want = outs[e][1]
-      assert (int(res.has_reward[e]), int(res.reward[e])) == (
-          (0, 0) if want is None else (1, int(want))), (t, e)
-      assert float(res.discount[e]) == float(outs[e][2]) and bool(res.done[e]) == worlds[e].game_over
-    if t == T:
-      break
-    act = rs.choice([0, 1, 2, 3, 4, 5], size=B, p=[.23, .23, .23, .23, .03, .05]).astype(np.int32)
-    res = eng.play(torch.from_numpy(act).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        worlds[e] = ogames.make_hello(art)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(act[e]))
+  actions = np.stack([rs.choice([0, 1, 2, 3, 4, 5], size=B, p=[.23, .23, .23, .23, .03, .05])
+                      for _ in range(T)]).astype(np.int32)
+  sampled_check.lockstep(eng, lambda e: ogames.make_hello(art), range(B), actions, curtains='@')
   assert int(eng.error_codes().abs().max()) == 0
 
 

@@ -14,6 +14,7 @@ import golden_cases as gc
 import refdriver
 import trajectory as tj
 from oracle import games as ogames
+from oracle import sampled_check
 
 NAMES = gc.names('shockwave_')
 
@@ -66,45 +67,23 @@ def test_facade_shockwave_golden(name):
 def test_batched_shockwave_vs_oracle(shape):
   """Auto-resetting batch over several generated levels, one NumPy generator per env
   (RandomState(seed + e)), boards / curtains / rewards / discounts every step."""
-  import torch
   from pycolab_b200 import batched, levels
   from pycolab_b200.games import shockwave
   arts = [levels.shockwave_level(30 + i, shape[0], shape[1], 0.45) for i in range(3)]
   B, T, seed = 13, 220, 9
   eng = batched.BatchedEngine([shockwave.make_game(a) for a in arts], batch=B, rng_seed=seed)
   rngs = [np.random.RandomState(seed + e) for e in range(B)]
-  make = lambda e: ogames.make_shockwave(arts[e % len(arts)], rngs[e])
-  worlds = [make(e) for e in range(B)]
-  outs = [w.its_showtime() for w in worlds]
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(4)
-  episodes = wins = 0
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    cur = eng.curtain('@').cpu().numpy()
-    for e in range(B):
-      np.testing.assert_array_equal(boards[e][:, :shape[1]], outs[e][0],
-                                    err_msg='t=%d env=%d' % (t, e))
-      np.testing.assert_array_equal(cur[e], worlds[e].things['@'].curtain)
-      want = outs[e][1]
-      assert (int(res.has_reward[e]), int(res.reward[e])) == (
-          (0, 0) if want is None else (1, int(want))), (t, e)
-      assert float(res.discount[e]) == float(outs[e][2])
-      assert bool(res.done[e]) == worlds[e].game_over
-    if t == T:
-      break
-    act = rs.choice([0, 1, 2, 3, 4], size=B, p=[.6, .12, .12, .12, .04]).astype(np.int32)
-    res = eng.play(torch.from_numpy(act).cuda())
-    for e in range(B):
-      if worlds[e].game_over:
-        episodes += 1
-        wins += outs[e][1] == 1
-        worlds[e] = make(e)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(act[e]))
-  assert episodes > B
+  actions = np.stack([rs.choice([0, 1, 2, 3, 4], size=B, p=[.6, .12, .12, .12, .04])
+                      for _ in range(T)]).astype(np.int32)
+  episodes = [0]
+
+  def count(t, eng, worlds, outs):
+    episodes[0] += sum(w.game_over for w in worlds.values()) if t < T else 0
+  sampled_check.lockstep(eng, lambda e: ogames.make_shockwave(arts[e % len(arts)], rngs[e]),
+                         range(B), actions, curtains='@', on_step=count)
+  assert episodes[0] > B
   assert int(eng.error_codes().abs().max()) == 0
 
 

@@ -20,6 +20,7 @@ import refdriver
 import trajectory as tj
 from oracle import engine_model as em
 from oracle import games as ogames
+from oracle import sampled_check
 from oracle import t_maze as otm
 
 NAMES = gc.names('t_maze_')
@@ -335,7 +336,8 @@ def test_facade_t_maze_golden(name):
 def _batched_vs_oracle(B, T, seed, cfg, n_worlds, check_envs=None, policy_seed=3):
   """Auto-resetting batch over generated worlds (env e plays world e % n_worlds, one set of
   make_game arguments for the handle): env e's cue and speckle come from
-  random.Random(seed + e) and RandomState(seed + e), drawn by the kernel at every restart."""
+  random.Random(seed + e) and RandomState(seed + e), drawn by the kernel at every restart.
+  Rewards are compared as float64 bits."""
   import torch
   from pycolab_b200 import batched, levels
   from pycolab_b200.games import t_maze
@@ -349,41 +351,20 @@ def _batched_vs_oracle(B, T, seed, cfg, n_worlds, check_envs=None, policy_seed=3
   def make(e):
     maze, cue = arts[e % n_worlds]
     return otm.make_t_maze(maze, cue, *cfg, rng=rngs[e][0], np_rng=rngs[e][1])
-  worlds = {e: make(e) for e in envs}
-  outs = {e: w.its_showtime() for e, w in worlds.items()}
-  res = eng.its_showtime()
+  eng.its_showtime()
   rs = np.random.RandomState(policy_seed)
   policy = np.array([rs.choice([1, 2, 3, 4, 5, 0, 6], size=B,
                                p=[.35, .1, .2, .2, .13, .01, .01]) for _ in range(T)], np.int32)
-  episodes, paid = 0, set()
-  for t in range(T + 1):
-    torch.cuda.synchronize()
-    boards = res.board.cpu().numpy()
-    reward = res.reward.cpu().numpy()
-    has = res.has_reward.cpu().numpy()
-    disc = res.discount.cpu().numpy()
-    done = res.done.cpu().numpy()
-    for e in envs:
-      np.testing.assert_array_equal(boards[e], outs[e][0], err_msg='t=%d env=%d' % (t, e))
-      want = outs[e][1]
-      assert int(has[e]) == (want is not None), (t, e)
-      want_bits = np.float64(0.0 if want is None else want).view(np.int64)
-      assert reward[e:e + 1].view(np.int64)[0] == want_bits, (t, e, reward[e], want)
-      assert float(disc[e]) == float(outs[e][2]) and bool(done[e]) == worlds[e].game_over, (t, e)
-      if want is not None:
-        paid.add(round(float(want), 3))
-    if t == T:
-      break
-    res = eng.play(torch.from_numpy(policy[t]).cuda())
-    for e in envs:
-      if worlds[e].game_over:
-        episodes += 1
-        worlds[e] = make(e)
-        outs[e] = worlds[e].its_showtime()
-      else:
-        outs[e] = worlds[e].play(int(policy[t][e]))
+  episodes, paid = [0], set()
+
+  def count(t, eng, worlds, outs):
+    for e, w in worlds.items():
+      episodes[0] += int(t < T and w.game_over)
+      if outs[e][1] is not None:
+        paid.add(round(float(outs[e][1]), 3))
+  sampled_check.lockstep(eng, make, envs, policy, on_step=count)
   assert int(eng.error_codes().abs().max()) == 0
-  return eng, episodes, paid
+  return eng, episodes[0], paid
 
 
 @pytest.mark.gpu

@@ -10,7 +10,7 @@ monsters), two more when the fruit is eaten; a float draw takes two MT19937 outp
 an int draw one or more.  Both step the same seeded actions through `pcl_run` (one C call
 per timed window), timed with CUDA events after a warm-up, three alternating repeats per
 batch size.  The same run steps a fresh drawing engine and checks sampled envs against the
-oracle (tests/drawn_oracle.py) every step, and reads the card's name, power limit and
+oracle (oracle/compiled.py) every step, and reads the card's name, power limit and
 maximum SM clock (the clock the kernels ran at is not sampled).
 
     python tools/drawn_bench.py [--batch 4096 65536] [--steps 1000] [--warmup 100]
@@ -31,8 +31,8 @@ sys.path.insert(0, os.path.join(ROOT, 'tools'))
 
 import numpy as np                                                # noqa: E402
 
-import drawn_oracle                                               # noqa: E402
 import trajectory                                                 # noqa: E402
+from oracle import compiled as ocompiled                          # noqa: E402
 from compiled_bench import card, time_run                         # noqa: E402
 from pycolab_b200 import batched, compat, compiler, lowering      # noqa: E402
 
@@ -130,8 +130,8 @@ def check_against_oracle(levels, B, steps, seed=3):
   table = rs.randint(0, 6, size=(steps, B)).astype(np.int32)
   sample = sorted({0, 1, B - 2, B - 1} | set(rs.randint(2, B - 2, size=4).tolist()))
   want = {e: trajectory.run_trajectory(
-      lambda e=e, w=drawn_oracle.seeded_words(levels[e % 2], seed + e):
-      drawn_oracle.make_world(levels[e % 2], w), table[:, e].tolist()) for e in sample}
+      lambda e=e, w=ocompiled.seeded_words(levels[e % 2], seed + e):
+      ocompiled.make_world(levels[e % 2], w), table[:, e].tolist()) for e in sample}
   res = eng.its_showtime()
   actions = torch.from_numpy(table).cuda()
   for t in range(steps + 1):
