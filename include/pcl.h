@@ -61,6 +61,7 @@ typedef enum pcl_status {
 #define PCL_ENV_ERR_BAD_Z            0x10 /* change_z_order names a missing entity, engine.py:802-812 */
 #define PCL_ENV_ERR_ARITH            0x20 /* ZeroDivisionError: `//` or `%` by zero in compiled code */
 #define PCL_ENV_ERR_RANGE            0x40 /* ValueError: a compiled draw from an empty range */
+#define PCL_ENV_ERR_POSTSCROLL       0x80 /* pattern_position_postscroll before the Scrolly moved, drapes.py:434-438 */
 
 /* Which game program advances the envs.  One fused kernel per program; the
  * host "lowering" recognises the reference's entity classes and picks one. */
@@ -100,10 +101,17 @@ typedef enum pcl_program {
                                 teleportation_order.  d_rng, when bound, is u32 [B, 2, PCL_MT_WORDS]: slot 0
                                 Python random.Random words (the cue), slot 1 NumPy RandomState words (the
                                 speckle); d_pattern_init[2] then holds the UN-speckled '*' pattern */
-  PCL_PROG_COMPILED = 14,    /* any registered MazeWalker / plain Drape classes: their update() bodies
-                                compiled to the bytecode below (pcl_bind_code) and interpreted one warp
-                                per env.  Registers: sprite AUX0-AUX2, all eight words of a drape record,
-                                plot AUX0-AUX3 (the_plot keys).  program_arg[0] = 1: rewards are float64
+  PCL_PROG_COMPILED = 14,    /* any registered MazeWalker / Scrolly / plain Drape classes: their update()
+                                bodies compiled to the bytecode below (pcl_bind_code) and interpreted one
+                                warp per env, in one scrolling group.  Registers: sprite AUX0-AUX2 (an
+                                egocentric walker: AUX2 only; AUX0 / AUX1 hold its permits), a Scrolly's
+                                AUX0-AUX2 (words 0-4 are its corners and last move frame), all eight
+                                words of a plain drape record, plot AUX0-AUX3 (the_plot keys).
+                                program_arg[2]: bit d set = Scrolly d writes its pattern (PCL_OP_SETPAT):
+                                d_pattern[d] is then per env and reset from d_pattern_init[d] (per level),
+                                and its curtain, the pattern window as of its last motion helper
+                                (drapes.py:689-695), is kept in d_bits[d] (reset from d_bits_init[d]).
+                                Other Scrolly patterns are static.  program_arg[0] = 1: rewards are float64
                                 (pcl_outputs.d_reward_f64 is required), 0: int32.  program_arg[1] =
                                 the number of RNG slots the code draws from (0-2); with slots,
                                 pcl_state.d_rng is required and is u32 [B, program_arg[1],
@@ -199,6 +207,18 @@ enum {
                            float64 with bit halves lo / hi, cmp 0-5 = == != < <= > >=          */
   PCL_OP_PICK,          /* k, v_1 .. v_k: pop i; push v_(i+1) (1 <= k <= 64); i outside 0 .. k-1
                            latches PCL_ENV_ERR_INDEX and pushes 0                              */
+  /* Scrollys (drapes.py:378-695).  `scrolly` operands name a Scrolly drape, -1 only inside a
+   * Scrolly's own update.  CURTAIN and ANY on a Scrolly read its curtain. */
+  PCL_OP_SCROLL,        /* motion: _maybe_move of the updated Scrolly (drapes.py:487-659)       */
+  PCL_OP_PRESCROLL,     /* scrolly: pop r, c; refresh its pre-scroll corner if it has not moved
+                           in this frame (drapes.py:407-408); push (r + pre_r, c + pre_c)      */
+  PCL_OP_POSTSCROLL,    /* scrolly: pop r, c; push (r + corner_r, c + corner_c); if it has not
+                           moved in this frame, latch PCL_ENV_ERR_POSTSCROLL                   */
+  PCL_OP_PATTERN,       /* scrolly: pop r, c; push its whole_pattern at (r, c) (NumPy indexing
+                           over pattern_rows x pattern_cols)                                  */
+  PCL_OP_SETPAT,        /* pop r, c, v: the updated Scrolly's whole_pattern at (r, c) = v != 0
+                           (its program_arg[2] bit must be set)                                */
+  PCL_OP_PATANY,        /* scrolly: push whether its whole_pattern has a cell set             */
   PCL_OP_COUNT
 };
 

@@ -37,6 +37,7 @@ ENV_ERR_INDEX = 0x8
 ENV_ERR_BAD_Z = 0x10
 ENV_ERR_ARITH = 0x20
 ENV_ERR_RANGE = 0x40
+ENV_ERR_POSTSCROLL = 0x80
 
 PROG_NONE, PROG_SCROLLY_MAZE, PROG_WAREHOUSE, PROG_MARAUDERS, PROG_FIXTURE = 0, 1, 2, 3, 4
 PROG_BETTER_SCROLLY, PROG_CLASSICS, PROG_APERTURE, PROG_ORDEAL, PROG_HELLO = 5, 6, 7, 8, 9
@@ -54,13 +55,17 @@ OPS = ('RET', 'PUSH', 'POP', 'DUP', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'ADD', 
        'FLOORDIV', 'MOD', 'EQ', 'NE', 'LT', 'LE', 'GT', 'GE', 'NEG', 'NOT', 'EQ2', 'IN', 'ACTION',
        'FRAME', 'FIELD', 'GETR', 'SETR', 'GETP', 'SETP', 'BOARD', 'BACKDROP', 'CURTAIN',
        'SETCELL', 'FILL', 'ANY', 'MOVE', 'TELEPORT', 'REWARD', 'REWARD_F64', 'TERMINATE',
-       'DISCOUNT', 'RANDINT', 'RANDCMP', 'PICK')
+       'DISCOUNT', 'RANDINT', 'RANDCMP', 'PICK',
+       # Scrollys: SCROLL motion; PRESCROLL / POSTSCROLL / PATTERN / PATANY a Scrolly (-1 =
+       # the updated one); SETPAT writes the updated Scrolly's pattern.
+       'SCROLL', 'PRESCROLL', 'POSTSCROLL', 'PATTERN', 'SETPAT', 'PATANY')
 OP = {name: code for code, name in enumerate(OPS)}
 OPERANDS = {OP[n]: (4 if n == 'RANDCMP' else
                     2 if n in ('FIELD', 'REWARD_F64', 'RANDINT') else
                     1 if n in ('PUSH', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'IN', 'GETR', 'SETR',
                                'GETP', 'SETP', 'CURTAIN', 'ANY', 'MOVE', 'TERMINATE',
-                               'DISCOUNT', 'PICK') else 0) for n in OPS}
+                               'DISCOUNT', 'PICK', 'SCROLL', 'PRESCROLL', 'POSTSCROLL',
+                               'PATTERN', 'PATANY') else 0) for n in OPS}
 RAND_NUMPY, RAND_PYTHON, RAND_PYTHON_CLOSED = 0, 1, 2     # PCL_OP_RANDINT rules
 MAX_RNG_SLOTS = 2                                         # compiled program_arg[1]
 FIELD_ROW, FIELD_COL, FIELD_VROW, FIELD_VCOL, FIELD_VISIBLE = range(5)

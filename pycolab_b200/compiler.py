@@ -11,15 +11,20 @@ as before.
 
 The subset (everything else raises `NotLoweredError` naming the class, the source line
 and the construct):
-  entities    MazeWalker subclasses (any impassable set, confined or not, default
-              scrolling group, not egocentric) and plain Drape subclasses;
+  entities    MazeWalker subclasses (any impassable set, confined or not, egocentric or
+              not), Scrolly subclasses and plain Drape subclasses, all in one scrolling
+              group; the Scrollys' patterns all of one shape;
   statements  if / elif / else, return, pass; `del` and docstrings compile to nothing;
               local variables holding an int, a bool, a position or a motion result;
+              `r, c = <position>`;
               `self.<attr>` and `the_plot['key']` with =, +=, -=, *=, //=, %=;
-              motion helpers (`self._north(board, the_plot)` ... `self._stay(...)`),
+              motion helpers (`self._north(board, the_plot)` ... `self._stay(...)`; on
+              Scrollys `self._north(the_plot)` ...), also as
+              `(self._east if c else self._west)(...)`,
               `self._teleport(pos)`, `the_plot.add_reward(x)`,
               `the_plot.terminate_episode([discount])`, `the_plot.change_default_discount(c)`;
-              on drapes `self.curtain[cell] = v` and `self.curtain[:] = v`;
+              on plain drapes `self.curtain[cell] = v` and `self.curtain[:] = v`;
+              on Scrollys `self.whole_pattern[cell] = v` (their own pattern only);
   values      `actions` (==, !=, in, is None only), int and bool literals (float literals
               only as a reward or a discount), + - * // % and unary -, comparisons
               (chained, position against position or tuple), `in` over a literal
@@ -29,7 +34,10 @@ and the construct):
               `.visible`, `the_plot.frame`, `the_plot['key']`, `the_plot.get('key')`,
               `board[cell]`, `backdrop.curtain[cell]`, `layers['X'][cell]`,
               `self.curtain[cell]`, `things['X'].position / .visible / .curtain[cell]`,
-              `.curtain.any()`.
+              `.curtain.any()` (a Scrolly's curtain is its pattern window);
+              of Scrollys (`self` or `things['X']`): `.pattern_position_prescroll(pos,
+              the_plot)`, `.pattern_position_postscroll(pos, the_plot)`,
+              `.whole_pattern[cell]`, `.whole_pattern.any()`.
   draws       from the global generators, whose functions are found through update()'s
               module globals and compared by identity (so `import numpy as np`,
               `from numpy import random as npr` and `from random import randint` all
@@ -43,7 +51,8 @@ and the construct):
               Each draw continues the env's copy of that generator on the device
               (include/pcl.h PCL_OP_RANDINT) and yields what the generator would.
 Int and bool attributes of `self` become per-entity registers and `the_plot` keys plot
-registers; their values are read from the live objects when the game is lowered.
+registers; their values are read from the live objects when the game is lowered.  A walker
+and a Scrolly have 3 registers, an egocentric walker 1, a plain drape 8, the plot 4.
 Integers are 32 bits on the device; values outside int32 wrap.  After a facade step a
 register is written back with the type (bool or int) its value had at lowering.
 """
@@ -74,8 +83,12 @@ _CMPOPS = {ast.Eq: 'EQ', ast.NotEq: 'NE', ast.Lt: 'LT', ast.LtE: 'LE', ast.Gt: '
            ast.GtE: 'GE'}
 _POSITIONS = {'position': (_lib.FIELD_ROW, _lib.FIELD_COL),
               'virtual_position': (_lib.FIELD_VROW, _lib.FIELD_VCOL)}
-# Registers per entity: sprite record AUX0-AUX2, every word of a plain drape's record.
-MAX_REGISTERS = {'sprite': 3, 'drape': _lib.DRAPE_WORDS}
+# Registers per entity: sprite record AUX0-AUX2, a Scrolly's AUX0-AUX2, every word of a plain
+# drape's record.  An egocentric walker keeps its permits in AUX0 / AUX1: it has AUX2 only.
+MAX_REGISTERS = {'sprite': 3, 'scrolly': 3, 'drape': _lib.DRAPE_WORDS}
+MAX_EGOCENTRIC_REGISTERS = 1
+_PATTERN_POSITIONS = {'pattern_position_prescroll': 'PRESCROLL',
+                      'pattern_position_postscroll': 'POSTSCROLL'}
 MAX_PLOT_KEYS = 4
 # The generator functions a draw may call: (function, stream, kind).
 _DRAWS = ((np.random.randint, 'numpy', 'randint'), (np.random.choice, 'numpy', 'choice'),
@@ -139,11 +152,13 @@ def compile_class(klass):
     raise TypeError('register() takes classes, got {!r}'.format(klass))
   if issubclass(klass, prefab_sprites.MazeWalker):
     kind = 'sprite'
-  elif issubclass(klass, things.Drape) and not issubclass(klass, prefab_drapes.Scrolly):
+  elif issubclass(klass, prefab_drapes.Scrolly):
+    kind = 'scrolly'
+  elif issubclass(klass, things.Drape):
     kind = 'drape'
   else:
-    raise NotLoweredError('{}: only MazeWalker and plain Drape subclasses are compiled'.format(
-        _name(klass)))
+    raise NotLoweredError('{}: only MazeWalker, Scrolly and plain Drape subclasses are '
+                          'compiled'.format(_name(klass)))
   if klass.update in (prefab_sprites.MazeWalker.update, things.Drape.update):
     raise NotLoweredError('{}: has no update() of its own to compile'.format(_name(klass)))
   return _Compiler(klass, kind).run()
@@ -230,7 +245,9 @@ class _Compiler(object):
     return key
 
   def use_attr(self, node, name):
-    if name in _RESERVED.get(self.kind, ()) or hasattr(self.klass, name):
+    reserved = _RESERVED.get(self.kind, ())
+    if (name in reserved or hasattr(self.klass, name) or
+        any(r.endswith('*') and name.startswith(r[:-1]) for r in reserved)):
       self.refuse(node, 'attribute self.{} (not an int or bool of this object)'.format(name))
     if name not in self.attrs:
       self.attrs.append(name)
@@ -241,8 +258,8 @@ class _Compiler(object):
       self.streams.append(stream)
     return ('rng', stream)
 
-  def need(self, node, kind, what):
-    if self.kind != kind:
+  def need(self, node, kinds, what):
+    if self.kind not in kinds.split():
       self.refuse(node, '{} in a {} class'.format(what, self.kind))
 
   def number(self, node):
@@ -299,26 +316,55 @@ class _Compiler(object):
     else:
       self.refuse(st, type(st).__name__)
 
+  def local(self, name, t, st):
+    """The first slot of local variable `name` holding a `t`."""
+    if name in self.role:
+      self.refuse(st, 'assigning an update() argument')
+    if t == 'char':
+      self.refuse(st, 'a character in a variable')
+    slot, have = self.locals.get(name, (None, None))
+    if have is None:
+      slot = self.n_slots
+      self.n_slots += 2 if t == 'pos' else 1
+      if self.n_slots > _lib.CODE_LOCALS:
+        self.refuse(st, 'more than {} local slots'.format(_lib.CODE_LOCALS))
+      self.locals[name] = (slot, t)
+    elif have != t:
+      self.refuse(st, 'variable {} holding a {} and a {}'.format(
+          name, _TYPE_NAMES[have], _TYPE_NAMES[t]))
+    return slot
+
   def assign(self, target, value, st):
     if isinstance(target, ast.Name):
       if target.id in self.role:
         self.refuse(st, 'assigning an update() argument')
       t = self.expr(value)
-      if t == 'char':
-        self.refuse(st, 'a character in a variable')
-      slot, have = self.locals.get(target.id, (None, None))
-      if have is None:
-        slot = self.n_slots
-        self.n_slots += 2 if t == 'pos' else 1
-        if self.n_slots > _lib.CODE_LOCALS:
-          self.refuse(st, 'more than {} local slots'.format(_lib.CODE_LOCALS))
-        self.locals[target.id] = (slot, t)
-      elif have != t:
-        self.refuse(st, 'variable {} holding a {} and a {}'.format(
-            target.id, _TYPE_NAMES[have], _TYPE_NAMES[t]))
+      slot = self.local(target.id, t, st)
       if t == 'pos':
         self.emit('STORE', slot + 1)
       self.emit('STORE', slot)
+      return
+    if isinstance(target, ast.Tuple):
+      # `r, c = <position>`
+      names = target.elts
+      if len(names) != 2 or not all(isinstance(n, ast.Name) for n in names):
+        self.refuse(st, 'unpacking into anything but two names')
+      if any(n.id in self.role for n in names):
+        self.refuse(st, 'assigning an update() argument')
+      if self.expr(value) != 'pos':
+        self.refuse(st, 'unpacking something that is not a position')
+      slots = [self.local(n.id, 'int', st) for n in names]
+      self.emit('STORE', slots[1])
+      self.emit('STORE', slots[0])
+      return
+    if isinstance(target, ast.Subscript) and self.pattern_owner(target.value) is not None:
+      if self.pattern_owner(target.value) != -1:
+        self.refuse(st, "a write to another entity's whole_pattern")
+      if _sliced(target.slice):
+        self.refuse(st, 'a whole_pattern slice')
+      self.cell(target.slice, st)
+      self.scalar(value)
+      self.emit('SETPAT')
       return
     if isinstance(target, ast.Attribute) and self.is_self(target.value):
       reg = self.use_attr(target, target.attr)
@@ -332,7 +378,7 @@ class _Compiler(object):
       return
     if (isinstance(target, ast.Subscript) and isinstance(target.value, ast.Attribute) and
         self.is_self(target.value.value) and target.value.attr == 'curtain'):
-      self.need(st, 'drape', 'a curtain write')
+      self.need(st, 'drape', 'a curtain write')   # a Scrolly's curtain is its pattern's
       sl = target.slice
       if isinstance(sl, ast.Slice):
         if sl.lower is not None or sl.upper is not None or sl.step is not None:
@@ -369,6 +415,23 @@ class _Compiler(object):
 
   def call_stmt(self, call):
     f = call.func
+    if self.motion_choice(f):
+      # `(self._east if c else self._west)(...)` as if / else
+      other, end = self.label(), self.label()
+      self.truth(f.test)
+      self.emit('JZ', other)
+      self.call_stmt(ast.copy_location(ast.Call(f.body, call.args, call.keywords), call))
+      self.emit('JMP', end)
+      self.place(other)
+      self.call_stmt(ast.copy_location(ast.Call(f.orelse, call.args, call.keywords), call))
+      self.place(end)
+      return
+    if (isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS and
+        self.kind == 'scrolly'):
+      if len(call.args) != 1 or call.keywords or not self.is_param(call.args[0], 'the_plot'):
+        self.refuse(call, 'a Scrolly motion helper not called as (the_plot)')
+      self.emit('SCROLL', _MOTIONS[f.attr])
+      return
     if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS:
       self.expr(call)
       self.emit('POP')
@@ -452,6 +515,8 @@ class _Compiler(object):
     if isinstance(node, ast.Name) and self.locals.get(node.id, (0, None))[1] == 'pos':
       slot = self.locals[node.id][0]
       return (lambda: self.emit('LOAD', slot), lambda: self.emit('LOAD', slot + 1))
+    if self.pattern_position(node) is not None:   # one call pushes both
+      return (lambda: self.pattern_position(node, emit=True), lambda: None)
     if isinstance(node, ast.Tuple) and len(node.elts) == 2:
       return (lambda: self.scalar(node.elts[0]), lambda: self.scalar(node.elts[1]))
     return None
@@ -460,6 +525,15 @@ class _Compiler(object):
     parts = self.pos_parts(node)
     if parts is None or isinstance(node, ast.Tuple):
       self.refuse(where, 'indexing something that is not a position')
+    if self.pattern_position(node) is not None:
+      self.pattern_position(node, emit=True)
+      if index == 1:                      # keep the column: through a fresh local slot
+        slot = self.local(' tmp%d' % self.n_slots, 'int', where)
+        self.emit('STORE', slot)
+      self.emit('POP')
+      if index == 1:
+        self.emit('LOAD', slot)
+      return 'int'
     parts[index]()
     return 'int'
 
@@ -559,11 +633,53 @@ class _Compiler(object):
       return 'int'
     self.refuse(node, 'the attribute .' + node.attr)
 
+  def owner(self, node):
+    """-1 for `self`, ('ent', X) for `things['X']`, else None."""
+    if self.is_self(node):
+      return -1
+    ch = self.thing_char(node)
+    return None if ch is None else ('ent', ch)
+
+  def pattern_owner(self, node):
+    """-1 for `self.whole_pattern` (of a Scrolly), ('ent', X) for `things['X'].whole_pattern`,
+    else None."""
+    if isinstance(node, ast.Attribute) and node.attr == 'whole_pattern':
+      owner = self.owner(node.value)
+      if owner == -1:
+        self.need(node, 'scrolly', 'self.whole_pattern')
+      return owner
+    return None
+
+  def pattern_position(self, node, emit=False):
+    """The opcode of `<scrolly>.pattern_position_prescroll / _postscroll(pos, the_plot)`,
+    else None; `emit`: push the (row, col) it yields."""
+    if not (isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and
+            node.func.attr in _PATTERN_POSITIONS):
+      return None
+    owner = self.owner(node.func.value)
+    if owner is None:
+      return None
+    if emit:
+      if owner == -1:
+        self.need(node, 'scrolly', node.func.attr)
+      if (len(node.args) != 2 or node.keywords or
+          not self.is_param(node.args[1], 'the_plot')):
+        self.refuse(node, node.func.attr + ' not called as (position, the_plot)')
+      self.pos(node.args[0], node)
+      self.emit(_PATTERN_POSITIONS[node.func.attr], owner)
+    return _PATTERN_POSITIONS[node.func.attr]
+
+  def motion_choice(self, f):
+    """Is callee `f` `(self._a if c else self._b)` over two motion helpers?"""
+    return (isinstance(f, ast.IfExp) and
+            all(isinstance(x, ast.Attribute) and self.is_self(x.value) and x.attr in _MOTIONS
+                for x in (f.body, f.orelse)))
+
   def curtain_owner(self, node):
     """-1 for `self.curtain`, ('ent', X) for `things['X'].curtain`, else None."""
     if isinstance(node, ast.Attribute) and node.attr == 'curtain':
       if self.is_self(node.value):
-        self.need(node, 'drape', 'self.curtain')
+        self.need(node, 'drape scrolly', 'self.curtain')
         return -1
       ch = self.thing_char(node.value)
       if ch is not None:
@@ -593,6 +709,13 @@ class _Compiler(object):
       self.cell(sl, node)
       self.emit('BACKDROP')
       return 'int'
+    owner = self.pattern_owner(base)
+    if owner is not None:
+      if _sliced(sl):
+        self.refuse(node, 'a whole_pattern slice')
+      self.cell(sl, node)
+      self.emit('PATTERN', owner)
+      return 'int'
     owner = self.curtain_owner(base)
     if owner is not None:
       if isinstance(sl, ast.Slice):
@@ -606,6 +729,13 @@ class _Compiler(object):
 
   def call(self, node):
     f = node.func
+    if self.motion_choice(f):
+      self.need(node, 'sprite', 'a motion result')
+      return self.expr(ast.copy_location(ast.IfExp(
+          f.test, ast.copy_location(ast.Call(f.body, node.args, node.keywords), node),
+          ast.copy_location(ast.Call(f.orelse, node.args, node.keywords), node)), node))
+    if self.pattern_position(node, emit=True) is not None:
+      return 'pos'
     if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS:
       self.need(node, 'sprite', f.attr)
       if (len(node.args) != 2 or node.keywords or not self.is_param(node.args[0], 'board') or
@@ -631,6 +761,10 @@ class _Compiler(object):
       self.emit('GETP', ('key', self.use_key(node.args[0].value)))
       return 'int'
     if isinstance(f, ast.Attribute) and f.attr == 'any' and not node.args and not node.keywords:
+      owner = self.pattern_owner(f.value)
+      if owner is not None:
+        self.emit('PATANY', owner)
+        return 'int'
       owner = self.curtain_owner(f.value)
       if owner is not None:
         self.emit('ANY', owner)
@@ -829,12 +963,22 @@ class _Compiler(object):
     self.emit(name)
 
 
+def _sliced(index):
+  """Does a subscript index take a slice on some axis?"""
+  return any(isinstance(x, ast.Slice) for x in
+             (index.elts if isinstance(index, ast.Tuple) else [index]))
+
+
 # Attributes the prefabs keep for themselves (their state lives in the device records).
 _RESERVED = {
     'sprite': {'_virtual_row', '_virtual_col', '_position', '_visible', '_prior_visible',
                '_c_h_a_r_a_c_t_e_r', '_c_o_r_n_e_r', '_impassable', '_confined_to_board',
                '_egocentric_scroller', '_scrolling_group'},
     'drape': {'_c_u_r_t_a_i_n', '_c_h_a_r_a_c_t_e_r'},
+    'scrolly': {'_c_u_r_t_a_i_n', '_c_h_a_r_a_c_t_e_r', '_w_h_o_l_e_p_a_t_t_e_r_n',
+                '_northwest_corner', '_prescroll_northwest_corner', '_last_maybe_move_frame',
+                '_northwest_corner_limit', '_scroll_margins', '_have_margins', '_board_shape',
+                '_scrolling_group', '_pattern_at_init', '_margin_*'},
 }
 
 
@@ -888,7 +1032,7 @@ def _encode(comp, base, chars, S, rows, cols, plot_keys, rng_streams):
       raise NotLoweredError('{}: things[{!r}] names no entity of the game'.format(
           _name(comp.klass), ch))
     k = chars.index(ch)
-    if (op == 'FIELD') != (k < S):
+    if (op == 'FIELD') != (k < S):     # FIELD names a sprite; the others a drape / Scrolly
       raise NotLoweredError('{}: things[{!r}] is not a {}'.format(
           _name(comp.klass), ch, 'sprite' if op == 'FIELD' else 'drape'))
     return k

@@ -505,7 +505,8 @@ int resolve_curtain(const pcl_handle* h, int d, pcl::LayersParams* p) {
     p->row_words[d] = sp.pattern_words;
     const bool coins = at == pcl::CurtainAt::kStaleWindow;
     p->stale_slot[d] = coins;
-    p->per_level[d] = !coins && h->st.d_level != nullptr;   // read-only patterns: per level
+    // a pattern with a reset template is per env; the others are read-only, per level
+    p->per_level[d] = !coins && h->st.d_level != nullptr && h->st.d_pattern_init[d] == nullptr;
   } else if (at == pcl::CurtainAt::kBits) {
     p->bits[d] = h->st.d_bits[d]; p->bits_bstride[d] = h->st.bits_bstride[d];
     p->row_words[d] = sp.bits_words;

@@ -1,5 +1,13 @@
-// compiled.cu — the compiled step program: MazeWalkers and plain drapes whose update()
-// bodies `pycolab_b200.compiler` translated into the bytecode of include/pcl.h (PCL_OP_*).
+// compiled.cu — the compiled step program: MazeWalkers (egocentric or not), Scrollys and
+// plain drapes whose update() bodies `pycolab_b200.compiler` translated into the bytecode
+// of include/pcl.h (PCL_OP_*).
+//
+// Scrollys scroll with fixture.cu's motion helper (board::scrolly_move_dyn), in the one
+// scrolling group whose order words live in the plot record.  A Scrolly's curtain is the
+// window of its pattern as of its last motion helper (drapes.py:689-695): read from the
+// static pattern at its corner, or, for a Scrolly whose code writes its pattern, kept in
+// d_bits and copied from the per-env pattern at each motion helper, so a write shows on
+// the board only after the next one, as upstream.
 //
 // The kernel is fixture.cu's frame — one warp per env, a real board in shared memory,
 // rendered after every update group (engine.py:725-735) — with an interpreter where the
@@ -55,7 +63,9 @@ __host__ __device__ __forceinline__ int op_operands(int op) {
     case PCL_OP_PUSH: case PCL_OP_LOAD: case PCL_OP_STORE: case PCL_OP_JMP: case PCL_OP_JZ:
     case PCL_OP_JNZ: case PCL_OP_IN: case PCL_OP_GETR: case PCL_OP_SETR: case PCL_OP_GETP:
     case PCL_OP_SETP: case PCL_OP_CURTAIN: case PCL_OP_ANY: case PCL_OP_MOVE:
-    case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: case PCL_OP_PICK: return 1;
+    case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: case PCL_OP_PICK: case PCL_OP_SCROLL:
+    case PCL_OP_PRESCROLL: case PCL_OP_POSTSCROLL: case PCL_OP_PATTERN: case PCL_OP_PATANY:
+      return 1;
     default: return 0;
   }
 }
@@ -100,6 +110,12 @@ constexpr OpInfo kOps[PCL_OP_COUNT] = {
     {2, 1},  // RANDINT
     {0, 1},  // RANDCMP
     {1, 1},  // PICK (+ its values)
+    {0, 0},  // SCROLL
+    {2, 2},  // PRESCROLL
+    {2, 2},  // POSTSCROLL
+    {2, 1},  // PATTERN
+    {3, 0},  // SETPAT
+    {0, 1},  // PATANY
 };
 static_assert(sizeof(kOps) / sizeof(kOps[0]) == PCL_OP_COUNT, "one kOps entry per opcode");
 constexpr int kMaxIn = 64;            // values of an IN or a PICK
@@ -127,6 +143,32 @@ __device__ __forceinline__ uint32_t row_word_mask(int w, int W) {
   return W - first >= 32 ? 0xffffffffu : (1u << (W - first)) - 1u;
 }
 
+// Scrolly d's whole pattern in the env being stepped: per env when the code writes it
+// (program_arg[2] bit d), else static per level.  Not read through __ldg: the same launch
+// may write it.
+__device__ __forceinline__ uint32_t* pattern_of(const Ctx& c, int d) {
+  const StepParams& p = *c.p;
+  const int64_t at = ((p.program_arg[2] >> d) & 1) ? (int64_t)c.env : c.lvl;
+  return p.st.d_pattern[d] + at * p.st.pattern_bstride[d];
+}
+
+// Word w of row r of Scrolly d's pattern window at its corner: curtain cells 32w .. 32w + 31
+// (pattern rows carry two zero words past the last column, so the second load stays in
+// the row).
+__device__ __forceinline__ uint32_t window_word(const Ctx& c, int d, int r, int w) {
+  const StepParams& p = *c.p;
+  const int32_t* rec = c.st->drapes[d];
+  const uint32_t* row = pattern_of(c, d) + (int64_t)(rec[PCL_D_CORNER_R] + r) * p.PWW;
+  const int col = rec[PCL_D_CORNER_C] + 32 * w;
+  return __funnelshift_r(row[col >> 5], row[(col >> 5) + 1], col & 31) & row_word_mask(w, p.W);
+}
+
+// Word w of row r of drape d's curtain: its bits, or a Scrolly's window (drapes.py:689-695).
+__device__ __forceinline__ uint32_t curtain_word(const Ctx& c, int d, int r, int w) {
+  if (c.p->drape_kind[d] && !((c.kept >> d) & 1)) return window_word(c, d, r, w);
+  return board::bits_row(c, d, r)[w];
+}
+
 // RNG slot `slot` of the env being stepped: d_rng is u32 [B, program_arg[1], PCL_MT_WORDS].
 __device__ __forceinline__ uint32_t* rng_slot(const Ctx& c, int slot) {
   const StepParams& p = *c.p;
@@ -146,6 +188,21 @@ __device__ __forceinline__ int compare(int cmp, T x, T y) {
   }
 }
 
+// A motion helper of Scrolly d (drapes.py:487-659).  Every path ends in _update_curtain, so
+// a Scrolly whose curtain is kept in d_bits copies its new window there; the others are
+// read from their static pattern at their corner, which only this call moves.
+__device__ __forceinline__ void scroll(const Ctx& c, int d, int motion, Plot& plot) {
+  board::scrolly_move_dyn(c, d, motion, plot);
+  if ((c.kept >> d) & 1) {
+    const StepParams& p = *c.p;
+    for (int i = c.lane; i < p.H * p.BW; i += 32) {
+      const int r = i / p.BW, w = i - r * p.BW;
+      board::bits_row(c, d, r)[w] = window_word(c, d, r, w);
+    }
+    __syncwarp();
+  }
+}
+
 struct Rewards {
   int has;
   int sum_i;
@@ -157,8 +214,10 @@ struct Rewards {
 __device__ __noinline__ void twist_out_of_line(uint32_t* mt, int lane) { mt_twist(mt, lane); }
 
 // The update() of entity `ent` (sprites first, then drapes).  kDraws: the code may draw
-// (program_arg[1] > 0); games without draws run a kernel without the generator.
-template <bool kDraws>
+// (program_arg[1] > 0); games without draws run a kernel without the generator.  kScroll:
+// the game scrolls (has Scrollys or egocentric walkers); the others run a kernel without
+// the Scrolly motion helper and egocentric moves, which cost ptxas 23 more registers.
+template <bool kDraws, bool kScroll>
 __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot,
                            Directives& dir, Rewards& rw) {
   const StepParams& p = *c.p;
@@ -166,7 +225,10 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
   const int S = p.S, H = p.H, W = p.W, lane = c.lane;
   const int32_t* code = p.code;
   const bool is_sprite = ent < S;
-  int32_t* regs = is_sprite ? &st->sprites[ent][PCL_S_AUX0] : st->drapes[ent - S];
+  // Registers: a walker's AUX0-AUX2 (an egocentric one's permits fill AUX0 / AUX1), a
+  // Scrolly's AUX0-AUX2, a plain drape's whole record.
+  int32_t* regs = is_sprite ? &st->sprites[ent][kScroll && p.egocentric[ent] ? PCL_S_AUX2 : PCL_S_AUX0]
+                            : &st->drapes[ent - S][kScroll && p.drape_kind[ent - S] ? PCL_D_AUX0 : 0];
   const LaneSlots stk = {&vm->stack[0][lane]};
   const LaneSlots loc = {&vm->local[0][lane]};
   int sp = 0;
@@ -251,6 +313,7 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         if (cell_index(r, H) && cell_index(col, W)) {
           if (op == PCL_OP_BOARD) v = c.board[r * p.pitch + col];
           else if (op == PCL_OP_BACKDROP) v = c.backdrop[(int64_t)r * p.pitch + col];
+          else if (kScroll) v = board::drape_bit(c, (a < 0 ? ent : a) - S, r, col);
           else v = bit_at(board::bits_row(c, (a < 0 ? ent : a) - S, r), col);
         } else {
           plot.error |= PCL_ENV_ERR_INDEX;
@@ -290,7 +353,7 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         bool any = false;
         for (int i = lane; i < H * p.BW; i += 32) {
           const int r = i / p.BW, w = i - r * p.BW;
-          any |= board::bits_row(c, d, r)[w] != 0u;
+          any |= (kScroll ? curtain_word(c, d, r, w) : board::bits_row(c, d, r)[w]) != 0u;
         }
         stk[sp++] = __any_sync(PCL_FULL, any) ? 1 : 0;
         break;
@@ -300,7 +363,8 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         const uint32_t* imp = st->impassable[ent];
         const uint8_t* bd = c.board;
         const int pitch = p.pitch;
-        const bool moved = walker_move(s, ent, a, plot, H, W, p.confined[ent] != 0, false, lane,
+        const bool moved = walker_move(s, ent, a, plot, H, W, p.confined[ent] != 0,
+                                       kScroll && p.egocentric[ent] != 0, lane,
                                        [&](int r, int col) { return in_set(imp, bd[r * pitch + col]); });
         board::store_sprite(st->sprites[ent], s, lane);
         stk[sp++] = moved ? 0 : 1;
@@ -350,6 +414,59 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         }
         break;
       }
+      case PCL_OP_SCROLL: if (kScroll) scroll(c, ent - S, a, plot); break;
+      case PCL_OP_PRESCROLL: case PCL_OP_POSTSCROLL: {
+        if (!kScroll) break;                   // pcl_bind_code refused them
+        int32_t* rec = st->drapes[(a < 0 ? ent : a) - S];
+        const bool stale = rec[PCL_D_LAST_FRAME] < plot.frame;
+        int dr = rec[PCL_D_CORNER_R], dc = rec[PCL_D_CORNER_C];
+        if (op == PCL_OP_PRESCROLL) {
+          if (stale) {                         // drapes.py:407-408
+            __syncwarp();
+            if (lane == 0) { rec[PCL_D_PRE_R] = dr; rec[PCL_D_PRE_C] = dc; }
+            __syncwarp();
+          }
+          dr = rec[PCL_D_PRE_R]; dc = rec[PCL_D_PRE_C];
+        } else if (stale) {
+          plot.error |= PCL_ENV_ERR_POSTSCROLL;   // RuntimeError upstream, drapes.py:434-438
+        }
+        stk[sp - 2] = (int)((unsigned)stk[sp - 2] + (unsigned)dr);
+        stk[sp - 1] = (int)((unsigned)stk[sp - 1] + (unsigned)dc);
+        break;
+      }
+      case PCL_OP_PATTERN: case PCL_OP_SETPAT: {
+        if (!kScroll) break;
+        const bool set = op == PCL_OP_SETPAT;
+        sp -= set ? 3 : 2;
+        int r = stk[sp], col = stk[sp + 1];
+        const int d = (set || a < 0 ? ent : a) - S;
+        int v = 0;
+        if (cell_index(r, p.PH) && cell_index(col, p.PW)) {
+          uint32_t* row = pattern_of(c, d) + (int64_t)r * p.PWW;
+          if (set) {
+            __syncwarp();
+            if (lane == 0) {
+              const uint32_t bit = 1u << (col & 31);
+              row[col >> 5] = stk[sp + 2] ? (row[col >> 5] | bit) : (row[col >> 5] & ~bit);
+            }
+            __syncwarp();
+          } else {
+            v = bit_at(row, col);
+          }
+        } else {
+          plot.error |= PCL_ENV_ERR_INDEX;
+        }
+        if (!set) stk[sp++] = v;
+        break;
+      }
+      case PCL_OP_PATANY: {
+        if (!kScroll) break;
+        const uint32_t* pat = pattern_of(c, (a < 0 ? ent : a) - S);
+        bool any = false;
+        for (int i = lane; i < p.PH * p.PWW; i += 32) any |= pat[i] != 0u;
+        stk[sp++] = __any_sync(PCL_FULL, any) ? 1 : 0;
+        break;
+      }
       default: {                               // PCL_OP_PICK
         const int i = stk[sp - 1];
         int v = 0;
@@ -364,7 +481,7 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
   }
 }
 
-template <bool kDraws>
+template <bool kDraws, bool kScroll>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 compiled_step(const StepParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -382,6 +499,7 @@ compiled_step(const StepParams p) {
   c.p = &p; c.st = st; c.board = my + sizeof(WarpState) + sizeof(Vm);
   c.backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
   c.env = env; c.lane = lane; c.lvl = lvl;
+  c.kept = (uint32_t)p.program_arg[2];       // Scrollys that write their pattern
 
   int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
   int32_t* g_drapes = p.st.d_drapes + (int64_t)env * D * PCL_DRAPE_WORDS;
@@ -400,8 +518,15 @@ compiled_step(const StepParams p) {
       restart ? p.st.d_z_order_init + lvl * p.st.z_order_init_bstride : g_z, S, D, lane);
   for (int i = lane; i < S * 4; i += 32) (&st->impassable[0][0])[i] = p.impassable[i >> 2][i & 3];
   if (restart) {
-    // A restart rebuilds every plain curtain from its template (things.py:146-217).
+    // A restart rebuilds every curtain kept in bits from its template (things.py:146-217),
+    // and every pattern the code writes.
     for (int d = 0; d < D; ++d) {
+      if ((c.kept >> d) & 1) {
+        const uint32_t* src = p.st.d_pattern_init[d] + lvl * p.st.pattern_init_bstride[d];
+        uint32_t* dst = p.st.d_pattern[d] + (int64_t)env * p.st.pattern_bstride[d];
+        for (int i = lane; i < p.PH * p.PWW; i += 32) dst[i] = src[i];
+      }
+      if (p.drape_kind[d] && !((c.kept >> d) & 1)) continue;
       const uint32_t* src = p.st.d_bits_init[d] + lvl * p.st.bits_init_bstride[d];
       uint32_t* dst = p.st.d_bits[d] + (int64_t)env * p.st.bits_bstride[d];
       for (int i = lane; i < H * p.BW; i += 32) dst[i] = src[i];
@@ -434,7 +559,7 @@ compiled_step(const StepParams p) {
       int ent = 0;
       for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
       for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
-      run_update<kDraws>(c, vm, ent, action, plot, dir, rw);
+      run_update<kDraws, kScroll>(c, vm, ent, action, plot, dir, rw);
     }
     board::render(c);
   }
@@ -443,6 +568,8 @@ compiled_step(const StepParams p) {
   if (lane == 0) {
     st->plot[PCL_P_FRAME] = plot.frame; st->plot[PCL_P_GAME_OVER] = dir.game_over;
     st->plot[PCL_P_ERROR] = plot.error;
+    st->plot[PCL_P_ORDER_R] = plot.order_r; st->plot[PCL_P_ORDER_C] = plot.order_c;
+    st->plot[PCL_P_ORDER_FRAME] = plot.order_frame; st->plot[PCL_P_EGO_MASK] = plot.ego_mask;
     if (p.program_arg[0]) p.out.d_reward_f64[env] = rw.has ? rw.sum_f : 0.0;
     else p.out.d_reward[env] = rw.has ? rw.sum_i : 0;
     p.out.d_has_reward[env] = (uint8_t)rw.has;
@@ -453,8 +580,8 @@ compiled_step(const StepParams p) {
   board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
 }
 
-// MazeWalkers (default scrolling group, not egocentric) and plain drapes; the entities
-// and the z-order are consistent permutations of each other.
+// MazeWalkers, Scrollys and plain drapes in one scrolling group; the entities and the
+// z-order are consistent permutations of each other.
 int check_spec(const pcl_spec& s) {
   const int n = s.n_sprites + s.n_drapes;
   if (n < 1) return PCL_ERR_INVALID;
@@ -471,22 +598,39 @@ int check_spec(const pcl_spec& s) {
     }
     if (in_z != 1 || in_groups != 1 || ch == 0 || ch > 127) return PCL_ERR_INVALID;
   }
-  for (int i = 0; i < s.n_sprites; ++i)
-    if (s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
-  for (int d = 0; d < s.n_drapes; ++d)
-    if (s.drape_kind[d]) return PCL_ERR_UNSUPPORTED;
+  for (int d = 0; d < s.n_drapes; ++d) {
+    if (s.drape_kind[d] != 0 && s.drape_kind[d] != 1) return PCL_ERR_UNSUPPORTED;
+    if (!s.drape_kind[d]) continue;
+    if (s.pattern_rows < s.rows || s.pattern_cols < s.cols) return PCL_ERR_INVALID;
+    if (s.pattern_words < (s.pattern_cols + 31) / 32 + 2) return PCL_ERR_INVALID;
+    if (!margins_fit(s, d)) return PCL_ERR_INVALID;
+  }
   if (s.program_arg[0] != 0 && s.program_arg[0] != 1) return PCL_ERR_INVALID;
   if (s.program_arg[1] < 0 || s.program_arg[1] > 2) return PCL_ERR_INVALID;   // RNG slots
+  // Written patterns: Scrollys only.
+  const uint32_t kept = (uint32_t)s.program_arg[2];
+  for (int d = 0; d < 32; ++d)
+    if (((kept >> d) & 1) && (d >= s.n_drapes || !s.drape_kind[d])) return PCL_ERR_INVALID;
   if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
   return PCL_OK;
 }
 
 int check_state(const pcl_spec& s, const pcl_state& st) {
   if (!st.d_z_order || !st.d_z_order_init) return PCL_ERR_INVALID;
-  for (int d = 0; d < s.n_drapes; ++d)
-    if (!st.d_bits[d] || !st.d_bits_init[d]) return PCL_ERR_INVALID;
+  for (int d = 0; d < s.n_drapes; ++d) {
+    const bool kept = (s.program_arg[2] >> d) & 1;
+    if (s.drape_kind[d] && !st.d_pattern[d]) return PCL_ERR_INVALID;
+    if (kept && (!st.d_pattern_init[d] || st.pattern_bstride[d] == 0)) return PCL_ERR_INVALID;
+    if ((!s.drape_kind[d] || kept) && (!st.d_bits[d] || !st.d_bits_init[d])) return PCL_ERR_INVALID;
+  }
   if (s.program_arg[1] > 0 && !st.d_rng) return PCL_ERR_INVALID;
   return PCL_OK;
+}
+
+// Scrollys' curtains: kept in bits when their pattern is written, else their window.
+CurtainAt curtain(const pcl_spec& s, int d) {
+  return s.drape_kind[d] && !((s.program_arg[2] >> d) & 1) ? CurtainAt::kPatternWindow
+                                                            : CurtainAt::kBits;
 }
 
 // The checks pcl_bind_code promises (include/pcl.h): after them the kernel can run any
@@ -495,22 +639,42 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
   const int S = s.n_sprites, ents = s.n_sprites + s.n_drapes, body = 1 + ents;
   if (n <= body || n > PCL_MAX_CODE_WORDS || w[0] != ents) return PCL_ERR_INVALID;
   enum { kNone = 0, kSprite = 1, kDrape = 2 };
-  std::vector<int8_t> starts(n, kNone);          // kind of the function starting at a word
+  // What the entities sharing a function allow it: their kind, the fewest registers any of
+  // them has (1 for an egocentric walker, 3 for a walker or a Scrolly, 8 for a plain
+  // drape), whether they are all Scrollys, all plain drapes, all Scrollys that write
+  // their pattern.
+  struct Fn { int8_t kind, regs; bool scrolly, plain, writes; };
+  std::vector<Fn> starts(n, Fn{kNone, 0, false, false, false});   // by first word
   for (int i = 0; i < ents; ++i) {
     const int e = w[1 + i], kind = i < S ? kSprite : kDrape;
     if (e < body || e >= n) return PCL_ERR_INVALID;
-    if (starts[e] != kNone && starts[e] != kind) return PCL_ERR_INVALID;
-    starts[e] = (int8_t)kind;
+    if (starts[e].kind != kNone && starts[e].kind != kind) return PCL_ERR_INVALID;
+    const bool scrolly = kind == kDrape && s.drape_kind[i - S];
+    const bool writes = scrolly && ((s.program_arg[2] >> (i - S)) & 1);
+    const int regs = kind == kSprite ? (s.sprite_egocentric[i] ? 1 : 3)
+                                     : (scrolly ? 3 : PCL_DRAPE_WORDS);
+    Fn& f = starts[e];
+    if (f.kind == kNone) f = Fn{(int8_t)kind, (int8_t)regs, scrolly, !scrolly && kind == kDrape, writes};
+    f.regs = (int8_t)(regs < f.regs ? regs : f.regs);
+    f.scrolly = f.scrolly && scrolly;
+    f.plain = f.plain && !scrolly && kind == kDrape;
+    f.writes = f.writes && writes;
   }
-  if (starts[body] == kNone) return PCL_ERR_INVALID;
+  if (starts[body].kind == kNone) return PCL_ERR_INVALID;
+  // An entity operand naming a Scrolly, or -1 in a function of Scrollys.
+  auto is_scrolly = [&](int a, const Fn& f) {
+    return a < 0 ? f.scrolly : (a >= S && a < ents && s.drape_kind[a - S] != 0);
+  };
   std::vector<int> depth(n, -1);                 // stack depth on arrival, -1 = unreachable
   std::vector<int8_t> boundary(n, 0);
   std::vector<int> targets;
   int kind = kNone, end = 0;
+  Fn fn = starts[body];
   for (int pc = body; pc < n;) {
-    if (starts[pc] != kNone) {                   // a new function
-      kind = starts[pc];
-      for (end = pc + 1; end < n && starts[end] == kNone; ++end) {}
+    if (starts[pc].kind != kNone) {              // a new function
+      fn = starts[pc];
+      kind = fn.kind;
+      for (end = pc + 1; end < n && starts[end].kind == kNone; ++end) {}
       depth[pc] = 0;
     }
     boundary[pc] = 1;
@@ -546,7 +710,7 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (w[pc + 2] < 0 || w[pc + 2] > 4) return PCL_ERR_INVALID;
         break;
       case PCL_OP_GETR: case PCL_OP_SETR:
-        if (a < 0 || a >= (sprite ? 3 : PCL_DRAPE_WORDS)) return PCL_ERR_INVALID;
+        if (a < 0 || a >= fn.regs) return PCL_ERR_INVALID;
         break;
       case PCL_OP_GETP: case PCL_OP_SETP:
         if (a < 0 || a >= 4) return PCL_ERR_INVALID;
@@ -555,7 +719,16 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (a < 0 ? sprite : (a < S || a >= ents)) return PCL_ERR_INVALID;
         break;
       case PCL_OP_SETCELL: case PCL_OP_FILL:
-        if (sprite) return PCL_ERR_INVALID;
+        if (!fn.plain) return PCL_ERR_INVALID;   // a Scrolly's curtain is its pattern's window
+        break;
+      case PCL_OP_SCROLL:
+        if (!fn.scrolly || a < 0 || a > PCL_M_STAY) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_SETPAT:
+        if (!fn.scrolly || !fn.writes) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_PRESCROLL: case PCL_OP_POSTSCROLL: case PCL_OP_PATTERN: case PCL_OP_PATANY:
+        if (!is_scrolly(a, fn)) return PCL_ERR_INVALID;
         break;
       case PCL_OP_MOVE:
         if (!sprite || a < 0 || a > PCL_M_STAY) return PCL_ERR_INVALID;
@@ -597,13 +770,19 @@ int actions_per_env(const pcl_spec&) { return 1; }
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (sizeof(WarpState) + sizeof(Vm) + board::board_bytes(p.H, p.pitch)) *
                       kWarpsPerBlock;
-  return p.program_arg[1] > 0 ? launch_step(compiled_step<true>, p, kWarpsPerBlock, smem, s)
-                              : launch_step(compiled_step<false>, p, kWarpsPerBlock, smem, s);
+  bool scrolls = false;
+  for (int d = 0; d < p.D; ++d) scrolls = scrolls || p.drape_kind[d];
+  for (int i = 0; i < p.S; ++i) scrolls = scrolls || p.egocentric[i];
+  if (scrolls)
+    return p.program_arg[1] > 0 ? launch_step(compiled_step<true, true>, p, kWarpsPerBlock, smem, s)
+                                : launch_step(compiled_step<false, true>, p, kWarpsPerBlock, smem, s);
+  return p.program_arg[1] > 0 ? launch_step(compiled_step<true, false>, p, kWarpsPerBlock, smem, s)
+                              : launch_step(compiled_step<false, false>, p, kWarpsPerBlock, smem, s);
 }
 
 }  // namespace
 
-const Program kCompiled = {check_spec, check_state, curtain_bits, launch, actions_per_env,
+const Program kCompiled = {check_spec, check_state, curtain, launch, actions_per_env,
                            /*float_reward=*/false, /*crop_epilogue=*/false,
                            /*scroll_groups=*/false, check_code, /*float_reward_arg0=*/true};
 

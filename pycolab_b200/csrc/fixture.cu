@@ -35,6 +35,7 @@ using board::Ctx;
 using board::render;
 using board::load_sprite;
 using board::store_sprite;
+using board::scrolly_move_dyn;
 
 // The order / egocentric-set registers of scrolling group g <-> `plot`.
 __device__ __forceinline__ void group_in(Plot& plot, const WarpState* st, int g) {
@@ -48,70 +49,6 @@ __device__ __forceinline__ void group_out(const Plot& plot, WarpState* st, int g
     st->groups[g][PCL_G_ORDER_R] = plot.order_r; st->groups[g][PCL_G_ORDER_C] = plot.order_c;
     st->groups[g][PCL_G_ORDER_FRAME] = plot.order_frame;
     st->groups[g][PCL_G_EGO_MASK] = plot.ego_mask;
-  }
-  __syncwarp();
-}
-
-// scrolling.py:437-482 over the sprites in shared memory.
-__device__ bool is_possible(const Ctx& c, const Plot& plot, int motion) {
-  bool ok = true;
-  for (int i = 0; i < c.p->S; ++i) {
-    if ((plot.ego_mask >> i) & 1) {
-      const int32_t* r = c.st->sprites[i];
-      ok = ok && (r[PCL_S_AUX1] == plot.frame) && ((r[PCL_S_AUX0] >> motion) & 1);
-    }
-  }
-  return ok;
-}
-
-// drapes.py:487-659 for drape d (same logic as pcl::scrolly_move, dynamic S).
-__device__ void scrolly_move_dyn(const Ctx& c, int d, int motion, Plot& plot) {
-  const StepParams& p = *c.p;
-  int32_t* rec = c.st->drapes[d];
-  int corner_r = rec[PCL_D_CORNER_R], corner_c = rec[PCL_D_CORNER_C];
-  int pre_r = rec[PCL_D_PRE_R], pre_c = rec[PCL_D_PRE_C], last = rec[PCL_D_LAST_FRAME];
-  const ScrollyCfg cfg = scrolly_cfg(p.H, p.W, p.PH, p.PW, p.margin[d][0], p.margin[d][1]);
-  if (last < plot.frame) { last = plot.frame; pre_r = corner_r; pre_c = corner_c; }
-  const int dr = motion_dr(motion), dc = motion_dc(motion);
-  if (plot.order_frame == plot.frame) {
-    if (dr != plot.order_r && dc != plot.order_c) plot.error |= PCL_ENV_ERR_ORDER_MISMATCH;
-    corner_r += plot.order_r; corner_c += plot.order_c;
-  } else if (motion != PCL_M_STAY) {
-    if (!cfg.have_margins) {
-      if (is_possible(c, plot, motion)) {
-        const int nr = corner_r + dr, nc = corner_c + dc;
-        const int orr = (0 <= nr && nr <= cfg.limit_r) ? dr : 0;
-        const int occ = (0 <= nc && nc <= cfg.limit_c) ? dc : 0;
-        corner_r += orr; corner_c += occ;
-        plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
-      }
-    } else {
-      bool want_v = false, want_h = false;
-      for (int i = 0; i < p.S; ++i) {
-        if ((plot.ego_mask >> i) & 1) {
-          const int32_t* s = c.st->sprites[i];
-          const int row = s[PCL_S_ROW], col = s[PCL_S_COL];
-          const int nr = row + dr, nc = col + dc;
-          want_v |= (row > nr && nr <= cfg.m_north) || (row < nr && nr >= cfg.m_south);
-          want_h |= (col > nc && nc <= cfg.m_west) || (col < nc && nc >= cfg.m_east);
-        }
-      }
-      if (want_v || want_h) {
-        const int orr = want_v ? dr : 0, occ = want_h ? dc : 0;
-        const int nr = corner_r + orr, nc = corner_c + occ;
-        bool can = (0 <= nr && nr <= cfg.limit_r) && (0 <= nc && nc <= cfg.limit_c);
-        can = can && is_possible(c, plot, motion);
-        if (can) {
-          corner_r = nr; corner_c = nc;
-          plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
-        }
-      }
-    }
-  }
-  __syncwarp();
-  if (c.lane == 0) {
-    rec[PCL_D_CORNER_R] = corner_r; rec[PCL_D_CORNER_C] = corner_c;
-    rec[PCL_D_PRE_R] = pre_r; rec[PCL_D_PRE_C] = pre_c; rec[PCL_D_LAST_FRAME] = last;
   }
   __syncwarp();
 }
@@ -131,7 +68,7 @@ fixture_step(const StepParams p) {
   Ctx c;
   c.p = &p; c.st = st; c.board = my + sizeof(WarpState);
   c.backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  c.env = env; c.lane = lane; c.lvl = lvl;
+  c.env = env; c.lane = lane; c.lvl = lvl; c.kept = 0;
 
   int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
   int32_t* g_drapes = p.st.d_drapes + (int64_t)env * D * PCL_DRAPE_WORDS;

@@ -34,9 +34,11 @@ struct Ctx {
   const uint8_t* backdrop;
   int env, lane;
   int64_t lvl;                       // index of static level data
+  uint32_t kept;                     // bit d: Scrolly d's curtain is kept in d_bits, not read
+                                     // from its pattern (compiled.cu: patterns it writes)
 };
 
-// Row r of plain drape d's curtain bits (d_bits) in env c.env.
+// Row r of drape d's curtain bits (d_bits) in env c.env.
 __device__ __forceinline__ uint32_t* bits_row(const Ctx& c, int d, int r) {
   const StepParams& p = *c.p;
   return p.st.d_bits[d] + (int64_t)c.env * p.st.bits_bstride[d] + (int64_t)r * p.BW;
@@ -44,7 +46,7 @@ __device__ __forceinline__ uint32_t* bits_row(const Ctx& c, int d, int r) {
 
 __device__ __forceinline__ bool drape_bit(const Ctx& c, int d, int r, int col) {
   const StepParams& p = *c.p;
-  if (p.drape_kind[d]) {             // Scrolly: window of the pattern (drapes.py:689-695)
+  if (p.drape_kind[d] && !((c.kept >> d) & 1)) {   // Scrolly: window of the pattern (drapes.py:689-695)
     const uint32_t* pat = p.st.d_pattern[d] + c.lvl * p.st.pattern_bstride[d];
     const int pr = c.st->drapes[d][PCL_D_CORNER_R] + r, pc = c.st->drapes[d][PCL_D_CORNER_C] + col;
     return bit_at(pat + (int64_t)pr * p.PWW, pc);
@@ -86,6 +88,70 @@ __device__ __forceinline__ void store_sprite(int32_t* r, const Sprite& s, int la
   if (lane == 0) {
     r[0] = s.row; r[1] = s.col; r[2] = s.vrow; r[3] = s.vcol;
     r[4] = s.flags; r[5] = s.aux0; r[6] = s.aux1; r[7] = s.aux2;
+  }
+  __syncwarp();
+}
+
+// scrolling.py:437-482 over the sprites in shared memory.
+__device__ inline bool is_possible(const Ctx& c, const Plot& plot, int motion) {
+  bool ok = true;
+  for (int i = 0; i < c.p->S; ++i) {
+    if ((plot.ego_mask >> i) & 1) {
+      const int32_t* r = c.st->sprites[i];
+      ok = ok && (r[PCL_S_AUX1] == plot.frame) && ((r[PCL_S_AUX0] >> motion) & 1);
+    }
+  }
+  return ok;
+}
+
+// drapes.py:487-659 for drape d (same logic as pcl::scrolly_move, dynamic S).
+__device__ inline void scrolly_move_dyn(const Ctx& c, int d, int motion, Plot& plot) {
+  const StepParams& p = *c.p;
+  int32_t* rec = c.st->drapes[d];
+  int corner_r = rec[PCL_D_CORNER_R], corner_c = rec[PCL_D_CORNER_C];
+  int pre_r = rec[PCL_D_PRE_R], pre_c = rec[PCL_D_PRE_C], last = rec[PCL_D_LAST_FRAME];
+  const ScrollyCfg cfg = scrolly_cfg(p.H, p.W, p.PH, p.PW, p.margin[d][0], p.margin[d][1]);
+  if (last < plot.frame) { last = plot.frame; pre_r = corner_r; pre_c = corner_c; }
+  const int dr = motion_dr(motion), dc = motion_dc(motion);
+  if (plot.order_frame == plot.frame) {
+    if (dr != plot.order_r && dc != plot.order_c) plot.error |= PCL_ENV_ERR_ORDER_MISMATCH;
+    corner_r += plot.order_r; corner_c += plot.order_c;
+  } else if (motion != PCL_M_STAY) {
+    if (!cfg.have_margins) {
+      if (is_possible(c, plot, motion)) {
+        const int nr = corner_r + dr, nc = corner_c + dc;
+        const int orr = (0 <= nr && nr <= cfg.limit_r) ? dr : 0;
+        const int occ = (0 <= nc && nc <= cfg.limit_c) ? dc : 0;
+        corner_r += orr; corner_c += occ;
+        plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
+      }
+    } else {
+      bool want_v = false, want_h = false;
+      for (int i = 0; i < p.S; ++i) {
+        if ((plot.ego_mask >> i) & 1) {
+          const int32_t* s = c.st->sprites[i];
+          const int row = s[PCL_S_ROW], col = s[PCL_S_COL];
+          const int nr = row + dr, nc = col + dc;
+          want_v |= (row > nr && nr <= cfg.m_north) || (row < nr && nr >= cfg.m_south);
+          want_h |= (col > nc && nc <= cfg.m_west) || (col < nc && nc >= cfg.m_east);
+        }
+      }
+      if (want_v || want_h) {
+        const int orr = want_v ? dr : 0, occ = want_h ? dc : 0;
+        const int nr = corner_r + orr, nc = corner_c + occ;
+        bool can = (0 <= nr && nr <= cfg.limit_r) && (0 <= nc && nc <= cfg.limit_c);
+        can = can && is_possible(c, plot, motion);
+        if (can) {
+          corner_r = nr; corner_c = nc;
+          plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
+        }
+      }
+    }
+  }
+  __syncwarp();
+  if (c.lane == 0) {
+    rec[PCL_D_CORNER_R] = corner_r; rec[PCL_D_CORNER_C] = corner_c;
+    rec[PCL_D_PRE_R] = pre_r; rec[PCL_D_PRE_C] = pre_c; rec[PCL_D_LAST_FRAME] = last;
   }
   __syncwarp();
 }

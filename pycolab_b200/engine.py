@@ -207,6 +207,10 @@ class Engine(object):
       raise ZeroDivisionError('integer division or modulo by zero in a compiled update()')
     if errors & _lib.ENV_ERR_RANGE:
       raise ValueError('empty range for a random draw in a compiled update()')
+    if errors & _lib.ENV_ERR_POSTSCROLL:
+      raise RuntimeError('The pattern_position_postscroll method was called on a Scrolly '
+                         'instance before that instance had a chance to decide whether or '
+                         'where it would scroll.')
     if self._occlusion_in_layers:
       layers = rendering.LazyLayers(board, self._chars)
     else:

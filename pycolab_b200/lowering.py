@@ -135,7 +135,8 @@ def role_of(entity):
   from pycolab_b200 import compiler
   compiled = compiler.registered(cls)
   if compiled is not None:
-    return 'compiled.walker' if compiled.kind == 'sprite' else 'compiled.drape'
+    return {'sprite': 'compiled.walker', 'scrolly': 'compiled.scrolly',
+            'drape': 'compiled.drape'}[compiled.kind]
   for klass in cls.__mro__:
     key = (klass.__module__.rsplit('.', 1)[-1], klass.__name__)
     if key in LOWERED_CLASSES:
@@ -220,7 +221,7 @@ class LoweredGame(object):
                                 # the device and takes them back after every step (compiled)
     self.actions_per_env = 1    # action words per env and step
     self.backdrop_chars = ''
-    self.drape_kind = None      # per drape: 1 = Scrolly (fixture program only)
+    self.drape_kind = None      # per drape: 1 = Scrolly (fixture and compiled programs)
     self.dynamic_z = False      # per-env z-order array (Plot.change_z_order)
     self.program_arg = [0] * 8  # pcl_spec.program_arg
     self.reward_type = int      # the reference's reward type (classics pay floats)

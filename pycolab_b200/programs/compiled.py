@@ -1,4 +1,4 @@
-"""The compiled program `csrc/compiled.cu`: MazeWalkers and plain drapes of classes
+"""The compiled program `csrc/compiled.cu`: MazeWalkers, Scrollys and plain drapes of classes
 registered with `pycolab_b200.compiler`, whose update() bodies run as device bytecode."""
 
 import numpy as np
@@ -7,8 +7,8 @@ from pycolab_b200 import _lib
 from pycolab_b200 import compiler
 from pycolab_b200 import things
 from pycolab_b200.errors import NotLoweredError
-from pycolab_b200.lowering import (LoweredGame, _common, _plot_record, _set_sprites,
-                                   _sprite_record, pack_rows)
+from pycolab_b200.lowering import (LoweredGame, _common, _plot_record, _scrolly_record,
+                                   _set_sprites, _sprite_record, pack_rows, round_up)
 
 _INT32 = (-2 ** 31, 2 ** 31 - 1)
 
@@ -31,16 +31,31 @@ def lower(engine, roles):
   _common(engine, game, _lib.PROG_COMPILED)
   order = ''.join(game.groups)
   sprite_chars = [c for c in order if roles[c] == 'compiled.walker']
-  drape_chars = [c for c in order if roles[c] == 'compiled.drape']
+  drape_chars = [c for c in order if roles[c] in ('compiled.drape', 'compiled.scrolly')]
   if len(sprite_chars) > _lib.MAX_SPRITES or len(drape_chars) > _lib.MAX_DRAPES:
     raise NotLoweredError('too many entities for the compiled device program')
   comp = {ch: compiler.registered(type(th[ch])) for ch in order}
-  for ch in sprite_chars:
-    if th[ch]._egocentric_scroller:
-      raise NotLoweredError('egocentric MazeWalker {!r} is not compiled'.format(ch))
   for ch in drape_chars:
     if type(th[ch]).curtain is not things.Drape.curtain:
       raise NotLoweredError('drape {!r} overrides `curtain`'.format(ch))
+  scrollys = [ch for ch in drape_chars if roles[ch] == 'compiled.scrolly']
+  # One scrolling group: its order words are the plot record's.
+  groups = {th[ch]._scrolling_group for ch in sprite_chars + scrollys}
+  if len(groups) > 1:
+    raise NotLoweredError('more than one scrolling group ({}): the compiled program keeps '
+                          'one'.format(sorted(groups)))
+  shapes = {th[ch].whole_pattern.shape for ch in scrollys}
+  if len(shapes) > 1:
+    raise NotLoweredError('Scrolly patterns of different shapes {}'.format(sorted(shapes)))
+  for ch in scrollys:
+    if tuple(th[ch]._board_shape) != (engine.rows, engine.cols):
+      raise NotLoweredError('Scrolly {!r}: board_shape differs from the Engine board'.format(ch))
+  for ch in order:                 # pattern operands must name Scrollys
+    for ins in comp[ch].ir:
+      if ins[0] in ('PRESCROLL', 'POSTSCROLL', 'PATTERN', 'PATANY') and isinstance(ins[1], tuple):
+        if ins[1][1] in roles and roles[ins[1][1]] != 'compiled.scrolly':
+          raise NotLoweredError('{}: things[{!r}] is not a Scrolly'.format(
+              compiler._name(comp[ch].klass), ins[1][1]))
 
   # the_plot keys: plot registers AUX0.. in order of first use
   keys = []
@@ -65,9 +80,12 @@ def lower(engine, roles):
   values = {}
   for ch in order:
     c = comp[ch]
-    if len(c.attrs) > compiler.MAX_REGISTERS[c.kind]:
-      raise NotLoweredError('{} needs {} registers; a {} has {}'.format(
-          compiler._name(c.klass), len(c.attrs), c.kind, compiler.MAX_REGISTERS[c.kind]))
+    ego = c.kind == 'sprite' and bool(th[ch]._egocentric_scroller)
+    limit = compiler.MAX_EGOCENTRIC_REGISTERS if ego else compiler.MAX_REGISTERS[c.kind]
+    if len(c.attrs) > limit:
+      raise NotLoweredError('{} {!r} needs {} registers; {} has {}'.format(
+          compiler._name(c.klass), ch, len(c.attrs),
+          'an egocentric walker' if ego else 'a ' + c.kind, limit))
     regs = []
     values[ch] = []
     for name in c.attrs:
@@ -80,15 +98,35 @@ def lower(engine, roles):
     registers[ch] = regs
 
   sprites = [th[c] for c in sprite_chars]
-  _set_sprites(game, sprites, [_sprite_record(s, *(values[s.character] + [0, 0, 0])[:3])
-                               for s in sprites])
+  # an egocentric walker's permits start empty (AUX0 = 0, AUX1 = never), its register in AUX2
+  _set_sprites(game, sprites, [
+      _sprite_record(s, 0, _lib.NEVER, (values[s.character] + [0])[0])
+      if s._egocentric_scroller else _sprite_record(s, *(values[s.character] + [0, 0, 0])[:3])
+      for s in sprites], named_groups=True)
   game.drape_chars = ''.join(drape_chars)
   game.margins = [(-1, -1)] * len(drape_chars)
   game.drape_kind = [0] * len(drape_chars)
+  if shapes:
+    game.pattern_rows, game.pattern_cols = shapes.pop()
+    game.pattern_words = round_up((game.pattern_cols + 31) // 32 + 3, 2)
   recs = []
   for d, ch in enumerate(drape_chars):
-    recs.append((values[ch] + [0] * _lib.DRAPE_WORDS)[:_lib.DRAPE_WORDS])
-    game.bits[d] = pack_rows(th[ch].curtain, game.bits_words)
+    ent = th[ch]
+    if ch in scrollys:
+      rec = _scrolly_record(ent)
+      rec[_lib.D_AUX0:_lib.D_AUX0 + len(values[ch])] = values[ch]
+      recs.append(rec)
+      game.drape_kind[d] = 1
+      game.margins[d] = (-1, -1) if ent._scroll_margins is None else tuple(ent._scroll_margins)
+      game.patterns[d] = pack_rows(ent.whole_pattern, game.pattern_words)
+      # A pattern the code writes is per env; its curtain is kept in bits (csrc/compiled.cu).
+      game.pattern_mutable[d] = any(ins[0] == 'SETPAT' for ins in comp[ch].ir)
+      if game.pattern_mutable[d]:
+        game.program_arg[2] |= 1 << d
+        game.bits[d] = pack_rows(ent.curtain, game.bits_words)
+    else:
+      recs.append((values[ch] + [0] * _lib.DRAPE_WORDS)[:_lib.DRAPE_WORDS])
+      game.bits[d] = pack_rows(ent.curtain, game.bits_words)
   game.drapes = np.array(recs, dtype=np.int32).reshape(len(drape_chars), _lib.DRAPE_WORDS)
   game.plot = np.array(_plot_record(**{'aux%d' % i: v for i, v in enumerate(plot_regs)}),
                        dtype=np.int32)
@@ -123,9 +161,11 @@ def sync(engine):
   th = engine.things
   for ch, regs in game.registers.items():
     if ch in b.sprite_chars:
-      words = sprites[b.sprite_chars.index(ch)][_lib.S_AUX0:]
+      s = b.sprite_chars.index(ch)
+      words = sprites[s][_lib.S_AUX2 if game.egocentric[s] else _lib.S_AUX0:]
     else:
-      words = drapes[b.drape_chars.index(ch)]
+      d = b.drape_chars.index(ch)
+      words = drapes[d][_lib.D_AUX0 if game.drape_kind[d] else 0:]
     for (name, is_bool), word in zip(regs, words):
       setattr(th[ch], name, bool(word) if is_bool else int(word))
   for k, (key, is_bool) in enumerate(game.plot_keys):

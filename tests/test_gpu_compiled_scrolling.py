@@ -1,0 +1,181 @@
+"""GPU tests of scrolling games on the compiled step program (csrc/compiled.cu): the games
+of tests/scrolling_games.py on the H100, against the reference's trajectories
+(tests/golden/scrolly_*.npz, scrolling_*.npz), the hand-written scrolly_maze kernel and the
+oracle interpreter of tests/scrolling_oracle.py."""
+
+import os
+import sys
+
+import numpy as np
+import pytest
+
+import golden_cases as gc
+import scrolling_oracle
+import scrolly_shapes
+import trajectory as tj
+from oracle import sampled_check
+from pycolab_b200 import _lib, compat, compiler, levels, lowering
+
+pytestmark = pytest.mark.gpu
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+
+@pytest.fixture(scope='module')
+def games():
+  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
+  compat.uninstall()
+  try:
+    mod = compat.load_example(os.path.join(HERE, 'scrolling_games.py'))
+  finally:
+    compat.uninstall()
+    sys.modules.update(saved)
+  compiler.register(*mod.CLASSES)
+  yield mod
+  compiler.unregister(*mod.CLASSES)
+
+
+def _margins(name):
+  if name.startswith('scrolly_shape'):
+    return scrolly_shapes.SHAPE[name[len('scrolly_shape'):]][2]
+  return scrolly_shapes.DEFAULT_MARGINS
+
+
+def _sprite_rows(env, chars):
+  return [[s.position[0], s.position[1], int(bool(s.visible)),
+           s.virtual_position[0], s.virtual_position[1]]
+          for s in (env.things[ch] for ch in chars)]
+
+
+@pytest.mark.parametrize('name', gc.names('scrolly_'))
+def test_facade_replays_scrolly_golden(games, name):
+  g = gc.load(name)
+  maze, board, beneath = gc.scrolly_art(g)
+  sprites = []
+  got = tj.run_trajectory(
+      lambda: games.make_maze(maze, board, beneath, margins=_margins(name)),
+      g['actions'].tolist(), on_frame=lambda env, out: sprites.append(_sprite_rows(env, 'Pabc')))
+  tj.assert_same_trajectory(g, got, name)
+  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
+
+
+@pytest.mark.parametrize('name', gc.names('scrolling_'))
+def test_facade_replays_scrolling_golden(games, name):
+  g = gc.load(name)
+  level = int(g['level'][0])
+  sprites, registers, corners, types, envs = [], [], [], [], []
+
+  def on_frame(env, out):
+    sprites.append(_sprite_rows(env, games.SPRITES))
+    registers.append([int(getattr(env.things[ch], attr)) for ch, attr in games.REGISTERS] +
+                     [int(env.the_plot[key]) for key in games.PLOT_KEYS])
+    corners.append([list(env.things[ch]._northwest_corner) for ch in games.SCROLLYS])
+    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
+    if not envs or envs[-1] is not env:
+      envs.append(env)
+    assert isinstance(env.things['e'].sees_gems, bool)
+  got = tj.run_trajectory(lambda: games.make_sampler(level), g['actions'].tolist(),
+                          on_frame=on_frame)
+  tj.assert_same_trajectory(g, got, name)
+  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
+  np.testing.assert_array_equal(g['registers'], np.array(registers))
+  np.testing.assert_array_equal(g['corners'], np.array(corners))
+  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
+  last = envs[-1].things
+  np.testing.assert_array_equal(g['pattern_walls'], last['#'].whole_pattern)
+  np.testing.assert_array_equal(g['pattern_gems'], last['*'].whole_pattern)
+
+
+def test_facade_raises_on_postscroll_before_the_move(games):
+  engine = games.make_early()
+  engine.its_showtime()
+  engine.play(0)
+  with pytest.raises(RuntimeError, match='pattern_position_postscroll'):
+    engine.play(1)
+
+
+B, T = 4096, 300
+
+
+def _levels(n):
+  return [levels.scrolly_maze_level(100 + i, world_shape=(129, 129), board_shape=(64, 64))
+          for i in range(n)]
+
+
+def test_compiled_maze_matches_the_hand_written_kernel(games):
+  """B = 4096 over four generated 64 x 64 levels, auto-reset, 300 steps: every output and
+  every sprite and corner word byte for byte against PCL_PROG_SCROLLY_MAZE."""
+  import torch
+  from pycolab_b200 import batched
+  from pycolab_b200.games import scrolly_maze
+  arts = _levels(4)
+  theirs = batched.BatchedEngine([scrolly_maze.make_game(*a) for a in arts], batch=B)
+  ours = batched.BatchedEngine([games.make_maze(*a) for a in arts], batch=B)
+  assert theirs.game.program == _lib.PROG_SCROLLY_MAZE
+  assert ours.game.program == _lib.PROG_COMPILED
+  rs = np.random.RandomState(5)
+  actions = torch.from_numpy(rs.randint(0, 6, size=(T, B)).astype(np.int32)).cuda()
+  # the compiled program keeps its sprites in update order (abcP), the kernel in PAbc
+  order = torch.tensor([ours.sprite_chars.index(ch) for ch in theirs.sprite_chars]).cuda()
+  assert theirs.drape_chars == ours.drape_chars == '#@'
+
+  def same(t):
+    torch.cuda.synchronize()
+    for name in ('_board', 'reward', 'has_reward', 'discount', 'done'):
+      a, b = getattr(theirs, name), getattr(ours, name)
+      assert torch.equal(a, b), (name, t)
+    assert torch.equal(theirs.sprites[:, :, :5], ours.sprites[:, order, :5]), ('sprites', t)
+    assert torch.equal(theirs.drapes[:, :, :2], ours.drapes[:, :, :2]), ('corners', t)
+  theirs.its_showtime()
+  ours.its_showtime()
+  same(0)
+  dones = 0
+  for t in range(T):
+    theirs.play(actions[t])
+    ours.play(actions[t])
+    same(t + 1)
+    dones += int(ours.done.sum())
+  assert dones > 0                            # episodes end and restart on the way
+  assert int(ours.error_codes().abs().sum()) == 0
+
+
+def test_batched_lockstep_against_the_oracle(games):
+  """B = 4096 over two levels: sampled envs against the oracle every step, curtains,
+  sprite words and pad columns included, then the coins' final whole_pattern."""
+  import torch
+  from pycolab_b200 import batched, lowering as low
+  arts = _levels(2)
+  lowered = [low.lower(games.make_maze(*a)) for a in arts]
+  engine = batched.BatchedEngine(lowered, batch=B)
+  engine.its_showtime()
+  rs = np.random.RandomState(9)
+  actions = rs.randint(0, 6, size=(T, B)).astype(np.int32)
+  env_ids = [0, 1, 2, 3, 1000, 2049, 4094, 4095]
+  worlds = {}
+
+  def make_world(e):
+    worlds[e] = scrolling_oracle.make_world(lowered[e % 2])
+    return worlds[e]
+  n = sampled_check.lockstep(engine, make_world, env_ids, actions, curtains='#@',
+                             sprites='Pabc', pad_columns=True)
+  assert n == len(env_ids) * (T + 1)
+  coins = engine.patterns[1].index_select(
+      0, torch.as_tensor(env_ids, device=engine.device)).cpu().numpy().view(np.uint32)
+  for k, e in enumerate(env_ids):
+    world = worlds[e]
+    got = lowering.unpack_rows(coins[k], lowered[0].pattern_cols)
+    np.testing.assert_array_equal(got, world.things['@'].pattern, err_msg=str(e))
+
+
+def test_batched_sampler_lockstep_against_the_oracle(games):
+  """The sampler (kept Scrolly curtains, two levels) at B = 4096 against the oracle."""
+  from pycolab_b200 import batched, lowering as low
+  lowered = [low.lower(games.make_sampler(level)) for level in (0, 1)]
+  engine = batched.BatchedEngine(lowered, batch=B)
+  engine.its_showtime()
+  rs = np.random.RandomState(3)
+  actions = rs.randint(0, games.N_ACTIONS, size=(T, B)).astype(np.int32)
+  env_ids = [0, 1, 7, 2048, 4095]
+  n = sampled_check.lockstep(engine, lambda e: scrolling_oracle.make_world(lowered[e % 2]),
+                             env_ids, actions, curtains='#*', sprites='Pe', pad_columns=True)
+  assert n == len(env_ids) * (T + 1)

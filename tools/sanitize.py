@@ -117,6 +117,16 @@ def main():
                            '@': dict(pattern=~pattern, corner=(1, 1), margins=None, group='two')},
                           update_schedule=[['#', '@'], ['P', 'q']], z_order='@#Pq')
   run('fixture_step (2 scrolling groups)', [fx], 5, 9)
+  # Compiled scrolling games: Scrollys (one writing its pattern), egocentric walkers.
+  from pycolab_b200 import compat, compiler
+  compat.uninstall()
+  try:
+    sg = compat.load_example(os.path.join(ROOT, 'tests', 'scrolling_games.py'))
+  finally:
+    compat.uninstall()
+  compiler.register(*sg.CLASSES)
+  run('compiled_step scrolly maze', [sg.make_maze(*a) for a in arts], 7, 6, steps=20)
+  run('compiled_step sampler', [sg.make_sampler(0), sg.make_sampler(1)], 5, 10, steps=30)
   print('done')
 
 
