@@ -111,7 +111,11 @@ typedef enum pcl_program {
                                 d_pattern[d] is then per env and reset from d_pattern_init[d] (per level),
                                 and its curtain, the pattern window as of its last motion helper
                                 (drapes.py:689-695), is kept in d_bits[d] (reset from d_bits_init[d]).
-                                Other Scrolly patterns are static.  program_arg[0] = 1: rewards are float64
+                                Other Scrolly patterns are static.  program_arg[3]: bit s set = sprite s
+                                is a plain Sprite (things.py:265-391), not a MazeWalker: its code sets
+                                its own position and visibility (PCL_OP_SETFIELD), its registers are
+                                VROW, VCOL and AUX0-AUX2, and it may stand anywhere, off the board too.
+                                Egocentric sprites may not set the bit.  program_arg[0] = 1: rewards are float64
                                 (pcl_outputs.d_reward_f64 is required), 0: int32.  program_arg[1] =
                                 the number of RNG slots the code draws from (0-2); with slots,
                                 pcl_state.d_rng is required and is u32 [B, program_arg[1],
@@ -181,7 +185,8 @@ enum {
   PCL_OP_ACTION,        /* push the env's action (PCL_ACTION_NONE at a (re)start)            */
   PCL_OP_FRAME,         /* push the_plot.frame                                                */
   PCL_OP_FIELD,         /* sprite, f: push row, col, virtual row, virtual col, visible (f 0-4) */
-  PCL_OP_GETR,          /* k: push register k of the entity being updated (sprite k < 3)      */
+  PCL_OP_GETR,          /* k: push register k of the entity being updated (walker k < 3, plain
+                           sprite k < 5)                                                       */
   PCL_OP_SETR,          /* k: pop into it                                                     */
   PCL_OP_GETP,          /* k: push plot register k (k < 4)                                    */
   PCL_OP_SETP,          /* k: pop into it                                                     */
@@ -219,6 +224,12 @@ enum {
   PCL_OP_SETPAT,        /* pop r, c, v: the updated Scrolly's whole_pattern at (r, c) = v != 0
                            (its program_arg[2] bit must be set)                                */
   PCL_OP_PATANY,        /* scrolly: push whether its whole_pattern has a cell set             */
+  /* Plain Sprites (program_arg[3]).  Their positions are any int32 pair.  A render paints a
+   * visible one at its NumPy-wrapped cell; one still off the board after the wrap latches
+   * PCL_ENV_ERR_INDEX at the render that follows its update group and paints nothing
+   * (rendering.py:139, `board[tuple(position)]`). */
+  PCL_OP_SETFIELD,      /* f: pop v into the updated plain sprite's row (f 0), col (f 1) or
+                           visible bit (f 4, v != 0); the write twin of FIELD                 */
   PCL_OP_COUNT
 };
 

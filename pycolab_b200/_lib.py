@@ -58,14 +58,16 @@ OPS = ('RET', 'PUSH', 'POP', 'DUP', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'ADD', 
        'DISCOUNT', 'RANDINT', 'RANDCMP', 'PICK',
        # Scrollys: SCROLL motion; PRESCROLL / POSTSCROLL / PATTERN / PATANY a Scrolly (-1 =
        # the updated one); SETPAT writes the updated Scrolly's pattern.
-       'SCROLL', 'PRESCROLL', 'POSTSCROLL', 'PATTERN', 'SETPAT', 'PATANY')
+       'SCROLL', 'PRESCROLL', 'POSTSCROLL', 'PATTERN', 'SETPAT', 'PATANY',
+       # Plain Sprites: SETFIELD f sets the updated sprite's row, col or visible bit.
+       'SETFIELD')
 OP = {name: code for code, name in enumerate(OPS)}
 OPERANDS = {OP[n]: (4 if n == 'RANDCMP' else
                     2 if n in ('FIELD', 'REWARD_F64', 'RANDINT') else
                     1 if n in ('PUSH', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'IN', 'GETR', 'SETR',
                                'GETP', 'SETP', 'CURTAIN', 'ANY', 'MOVE', 'TERMINATE',
                                'DISCOUNT', 'PICK', 'SCROLL', 'PRESCROLL', 'POSTSCROLL',
-                               'PATTERN', 'PATANY') else 0) for n in OPS}
+                               'PATTERN', 'PATANY', 'SETFIELD') else 0) for n in OPS}
 RAND_NUMPY, RAND_PYTHON, RAND_PYTHON_CLOSED = 0, 1, 2     # PCL_OP_RANDINT rules
 MAX_RNG_SLOTS = 2                                         # compiled program_arg[1]
 FIELD_ROW, FIELD_COL, FIELD_VROW, FIELD_VCOL, FIELD_VISIBLE = range(5)

@@ -12,8 +12,9 @@ as before.
 The subset (everything else raises `NotLoweredError` naming the class, the source line
 and the construct):
   entities    MazeWalker subclasses (any impassable set, confined or not, egocentric or
-              not), Scrolly subclasses and plain Drape subclasses, all in one scrolling
-              group; the Scrollys' patterns all of one shape;
+              not), plain Sprite subclasses (things.Sprite, not MazeWalker), Scrolly
+              subclasses and plain Drape subclasses, all in one scrolling group; the
+              Scrollys' patterns all of one shape;
   statements  if / elif / else, return, pass; `del` and docstrings compile to nothing;
               local variables holding an int, a bool, a position or a motion result;
               `r, c = <position>`;
@@ -24,6 +25,8 @@ and the construct):
               `self._teleport(pos)`, `the_plot.add_reward(x)`,
               `the_plot.terminate_episode([discount])`, `the_plot.change_default_discount(c)`;
               on plain drapes `self.curtain[cell] = v` and `self.curtain[:] = v`;
+              on plain Sprites `self._position = <position>` (not a bare tuple: upstream
+              `.row` would fail on it later) and `self._visible = <truth value>`;
               on Scrollys `self.whole_pattern[cell] = v` (their own pattern only);
   values      `actions` (==, !=, in, is None only), int and bool literals (float literals
               only as a reward or a discount), + - * // % and unary -, comparisons
@@ -31,7 +34,10 @@ and the construct):
               tuple / list / string, and / or / not, `x if c else y`, `is None` on
               motion results, int(), ord('c'), chr(cell) against characters, positions
               (`.position`, `.virtual_position`, `.corner`, `.row`, `.col`, [0], [1]),
-              `.visible`, `the_plot.frame`, `the_plot['key']`, `the_plot.get('key')`,
+              `.visible`, `self._position` / `self._visible` of a plain Sprite,
+              `self.Position(r, c)` / `Position(row=r, col=c)` (also as `Sprite.Position`
+              through update()'s module globals, e.g. `things.Sprite.Position`),
+              `the_plot.frame`, `the_plot['key']`, `the_plot.get('key')`,
               `board[cell]`, `backdrop.curtain[cell]`, `layers['X'][cell]`,
               `self.curtain[cell]`, `things['X'].position / .visible / .curtain[cell]`,
               `.curtain.any()` (a Scrolly's curtain is its pattern window);
@@ -51,10 +57,14 @@ and the construct):
               Each draw continues the env's copy of that generator on the device
               (include/pcl.h PCL_OP_RANDINT) and yields what the generator would.
 Int and bool attributes of `self` become per-entity registers and `the_plot` keys plot
-registers; their values are read from the live objects when the game is lowered.  A walker
-and a Scrolly have 3 registers, an egocentric walker 1, a plain drape 8, the plot 4.
-Integers are 32 bits on the device; values outside int32 wrap.  After a facade step a
-register is written back with the type (bool or int) its value had at lowering.
+registers; their values are read from the live objects when the game is lowered.  An
+attribute used as a position (`self._start = self.position`, `self._position =
+self._start`, `board[self._start]`) is a position attribute and takes two registers; its
+first use in update() fixes which it is, and a later use as the other is refused.  A walker
+and a Scrolly have 3 registers, an egocentric walker 1, a plain Sprite 5, a plain drape 8,
+the plot 4.  Integers are 32 bits on the device; values outside int32 wrap.  After a facade
+step a register is written back with the type (bool, int, Position or tuple) its value had
+at lowering.
 """
 
 import ast
@@ -85,7 +95,8 @@ _POSITIONS = {'position': (_lib.FIELD_ROW, _lib.FIELD_COL),
               'virtual_position': (_lib.FIELD_VROW, _lib.FIELD_VCOL)}
 # Registers per entity: sprite record AUX0-AUX2, a Scrolly's AUX0-AUX2, every word of a plain
 # drape's record.  An egocentric walker keeps its permits in AUX0 / AUX1: it has AUX2 only.
-MAX_REGISTERS = {'sprite': 3, 'scrolly': 3, 'drape': _lib.DRAPE_WORDS}
+# A plain Sprite has no virtual position: its registers are VROW, VCOL and AUX0-AUX2.
+MAX_REGISTERS = {'sprite': 3, 'plain': 5, 'scrolly': 3, 'drape': _lib.DRAPE_WORDS}
 MAX_EGOCENTRIC_REGISTERS = 1
 _PATTERN_POSITIONS = {'pattern_position_prescroll': 'PRESCROLL',
                       'pattern_position_postscroll': 'POSTSCROLL'}
@@ -100,6 +111,8 @@ _DRAWS = ((np.random.randint, 'numpy', 'randint'), (np.random.choice, 'numpy', '
 _FLIPPED = {ast.Eq: ast.Eq, ast.NotEq: ast.NotEq, ast.Lt: ast.Gt, ast.LtE: ast.GtE,
             ast.Gt: ast.Lt, ast.GtE: ast.LtE}
 _TYPE_NAMES = {'int': 'number', 'pos': 'position', 'motion': 'motion result', 'char': 'character'}
+# A plain Sprite's own state (things.py:339-391), read and written in place.
+_SPRITE_STATE = ('_position', '_visible')
 
 
 def _f32_bits(x):
@@ -117,12 +130,25 @@ class Compiled(object):
   ('label', n) a code address, ('rows',) / ('cols',) the board shape, ('rng', stream) the
   RNG slot of a generator."""
 
-  def __init__(self, klass, kind, ir, attrs, keys, float_reward, streams=()):
+  def __init__(self, klass, kind, ir, attrs, keys, float_reward, streams=(), attr_types=None):
     self.klass, self.kind, self.ir = klass, kind, ir
     self.attrs = attrs            # register names, in slot order
+    # 'int' (ints and bools, one register) or 'pos' (a position, two: row, then col)
+    self.attr_types = dict(attr_types or {})
     self.keys = keys              # the_plot keys it reads or writes
     self.float_reward = float_reward
     self.streams = list(streams)  # generators it draws from ('numpy', 'python'), first use first
+
+  def width(self, name):
+    return 2 if self.attr_types.get(name) == 'pos' else 1
+
+  def slot(self, name):
+    """The first register of attribute `name`."""
+    return sum(self.width(a) for a in self.attrs[:self.attrs.index(name)])
+
+  @property
+  def n_registers(self):
+    return sum(self.width(a) for a in self.attrs)
 
 
 def register(*classes):
@@ -152,14 +178,17 @@ def compile_class(klass):
     raise TypeError('register() takes classes, got {!r}'.format(klass))
   if issubclass(klass, prefab_sprites.MazeWalker):
     kind = 'sprite'
+  elif issubclass(klass, things.Sprite):
+    kind = 'plain'
   elif issubclass(klass, prefab_drapes.Scrolly):
     kind = 'scrolly'
   elif issubclass(klass, things.Drape):
     kind = 'drape'
   else:
-    raise NotLoweredError('{}: only MazeWalker, Scrolly and plain Drape subclasses are '
-                          'compiled'.format(_name(klass)))
-  if klass.update in (prefab_sprites.MazeWalker.update, things.Drape.update):
+    raise NotLoweredError('{}: only Sprite, MazeWalker, Scrolly and plain Drape subclasses '
+                          'are compiled'.format(_name(klass)))
+  if klass.update in (prefab_sprites.MazeWalker.update, things.Sprite.update,
+                      things.Drape.update):
     raise NotLoweredError('{}: has no update() of its own to compile'.format(_name(klass)))
   return _Compiler(klass, kind).run()
 
@@ -192,6 +221,7 @@ class _Compiler(object):
     self.locals = {}              # name -> (first slot, type)
     self.n_slots = 0
     self.attrs, self.keys = [], []
+    self.attr_types = {}
     self.float_reward = False
     self.streams = []
 
@@ -199,7 +229,7 @@ class _Compiler(object):
     self.stmts(self.fdef.body)
     self.emit('RET')
     return Compiled(self.klass, self.kind, self.ir, self.attrs, self.keys, self.float_reward,
-                    self.streams)
+                    self.streams, self.attr_types)
 
   # -------------------------------------------------------------- helpers
   def refuse(self, node, what):
@@ -244,14 +274,62 @@ class _Compiler(object):
       self.keys.append(key)
     return key
 
-  def use_attr(self, node, name):
+  def check_attr(self, node, name):
     reserved = _RESERVED.get(self.kind, ())
     if (name in reserved or hasattr(self.klass, name) or
         any(r.endswith('*') and name.startswith(r[:-1]) for r in reserved)):
       self.refuse(node, 'attribute self.{} (not an int or bool of this object)'.format(name))
+
+  def use_attr(self, node, name, t='int'):
+    """The register of attribute `name` holding a `t` ('int' or 'pos'; a position
+    attribute's registers are ('attr', name, 0) and ('attr', name, 1))."""
+    self.check_attr(node, name)
+    have = self.attr_types.setdefault(name, t)
+    if have != t:
+      self.refuse(node, 'attribute self.{} holding a {} and a {}'.format(
+          name, _TYPE_NAMES[have], _TYPE_NAMES[t]))
     if name not in self.attrs:
       self.attrs.append(name)
     return ('attr', name)
+
+  def register_attr(self, node):
+    """`name` of `self.name` when it is a register attribute, else None."""
+    if (isinstance(node, ast.Attribute) and self.is_self(node.value) and
+        node.attr not in _POSITIONS and node.attr not in ('corner', 'visible', 'Position') and
+        not (self.kind == 'plain' and node.attr in _SPRITE_STATE)):
+      return node.attr
+    return None
+
+  def claim_pos(self, node):
+    """Where a position is needed: an attribute of no type yet becomes a position one."""
+    name = self.register_attr(node)
+    reserved = _RESERVED.get(self.kind, ())
+    if (name is not None and name not in self.attr_types and name not in reserved and
+        not hasattr(self.klass, name) and
+        not any(r.endswith('*') and name.startswith(r[:-1]) for r in reserved)):
+      self.use_attr(node, name, 'pos')
+
+  def position_ctor(self, node):
+    """(row, col) argument nodes of `Position(r, c)` / `Position(row=r, col=c)`, where
+    Position is things.Sprite.Position as `self.Position` or through the module globals,
+    else None."""
+    if not isinstance(node, ast.Call):
+      return None
+    f = node.func
+    if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr == 'Position':
+      fn = inspect.getattr_static(self.klass, 'Position', None)
+    else:
+      fn = self.callee(f)
+    if fn is not things.Sprite.Position:
+      return None
+    args = dict(zip(('row', 'col'), node.args))
+    for k in node.keywords:
+      if k.arg not in ('row', 'col') or k.arg in args:
+        self.refuse(node, 'these arguments of Position()')
+      args[k.arg] = k.value
+    if len(node.args) > 2 or set(args) != {'row', 'col'}:
+      self.refuse(node, 'these arguments of Position()')
+    return args['row'], args['col']
 
   def use_stream(self, stream):
     if stream not in self.streams:
@@ -367,9 +445,32 @@ class _Compiler(object):
       self.emit('SETPAT')
       return
     if isinstance(target, ast.Attribute) and self.is_self(target.value):
-      reg = self.use_attr(target, target.attr)
-      self.scalar(value)
-      self.emit('SETR', reg)
+      if self.kind == 'plain' and target.attr == '_position':
+        if isinstance(value, ast.Tuple):
+          self.refuse(st, 'a bare tuple as a position (upstream its .row fails later; use '
+                      'self.Position(row, col))')
+        self.pos(value, st)
+        self.emit('SETFIELD', _lib.FIELD_COL)
+        self.emit('SETFIELD', _lib.FIELD_ROW)
+        return
+      if self.kind == 'plain' and target.attr == '_visible':
+        self.truth(value)
+        self.emit('SETFIELD', _lib.FIELD_VISIBLE)
+        return
+      self.check_attr(target, target.attr)
+      if self.attr_types.get(target.attr) == 'pos':
+        self.pos(value, st)
+        t = 'pos'
+      else:
+        t = self.expr(value)
+        if t not in ('int', 'pos'):
+          self.refuse(value, 'a {} where a number is needed'.format(_TYPE_NAMES[t]))
+      reg = self.use_attr(target, target.attr, t)
+      if t == 'pos':
+        self.emit('SETR', reg + (1,))
+        self.emit('SETR', reg + (0,))
+      else:
+        self.emit('SETR', reg)
       return
     key = self.plot_key(target)
     if key is not None:
@@ -481,6 +582,7 @@ class _Compiler(object):
       self.refuse(node, 'a {} as a truth value'.format(_TYPE_NAMES[t]))
 
   def pos(self, node, where):
+    self.claim_pos(node)
     parts = self.pos_parts(node)
     if parts is None:
       self.refuse(where, 'something that is not a position')
@@ -508,8 +610,15 @@ class _Compiler(object):
       if owner is not None:
         if node.attr in _POSITIONS:
           if owner == -1:
-            self.need(node, 'sprite', '.' + node.attr)
+            self.need(node, 'sprite plain' if node.attr == 'position' else 'sprite',
+                      '.' + node.attr)
           return tuple(field(owner, f) for f in _POSITIONS[node.attr])
+        if owner == -1 and self.kind == 'plain' and node.attr == '_position':
+          return tuple(field(owner, f) for f in _POSITIONS['position'])
+        name = self.register_attr(node)
+        if name is not None and self.attr_types.get(name) == 'pos':
+          reg = self.use_attr(node, name, 'pos')
+          return (lambda: self.emit('GETR', reg + (0,)), lambda: self.emit('GETR', reg + (1,)))
         if node.attr == 'corner':
           return (lambda: self.emit('PUSH', ('rows',)), lambda: self.emit('PUSH', ('cols',)))
     if isinstance(node, ast.Name) and self.locals.get(node.id, (0, None))[1] == 'pos':
@@ -517,6 +626,9 @@ class _Compiler(object):
       return (lambda: self.emit('LOAD', slot), lambda: self.emit('LOAD', slot + 1))
     if self.pattern_position(node) is not None:   # one call pushes both
       return (lambda: self.pattern_position(node, emit=True), lambda: None)
+    if self.position_ctor(node) is not None:
+      row, col = self.position_ctor(node)
+      return (lambda: self.scalar(row), lambda: self.scalar(col))
     if isinstance(node, ast.Tuple) and len(node.elts) == 2:
       return (lambda: self.scalar(node.elts[0]), lambda: self.scalar(node.elts[1]))
     return None
@@ -618,8 +730,8 @@ class _Compiler(object):
     if node.attr in ('row', 'col'):
       return self.component(node.value, 0 if node.attr == 'row' else 1, node)
     if self.is_self(node.value):
-      if node.attr == 'visible':
-        self.need(node, 'sprite', '.visible')
+      if node.attr == 'visible' or (self.kind == 'plain' and node.attr == '_visible'):
+        self.need(node, 'sprite plain', '.visible')
         self.emit('FIELD', -1, _lib.FIELD_VISIBLE)
         return 'int'
       self.emit('GETR', self.use_attr(node, node.attr))
@@ -736,6 +848,10 @@ class _Compiler(object):
           ast.copy_location(ast.Call(f.orelse, node.args, node.keywords), node)), node))
     if self.pattern_position(node, emit=True) is not None:
       return 'pos'
+    if self.position_ctor(node) is not None:
+      for part in self.pos_parts(node):
+        part()
+      return 'pos'
     if isinstance(f, ast.Attribute) and self.is_self(f.value) and f.attr in _MOTIONS:
       self.need(node, 'sprite', f.attr)
       if (len(node.args) != 2 or node.keywords or not self.is_param(node.args[0], 'board') or
@@ -788,9 +904,12 @@ class _Compiler(object):
       return None
     obj = self.globals.get(f.id)
     for name in reversed(parts):
-      if not isinstance(obj, types.ModuleType):
+      if isinstance(obj, types.ModuleType):
+        obj = getattr(obj, name, None)
+      elif isinstance(obj, type):            # a class attribute, looked up without running code
+        obj = inspect.getattr_static(obj, name, None)
+      else:
         return None
-      obj = getattr(obj, name, None)
     return obj
 
   def generator_call(self, node):
@@ -974,6 +1093,7 @@ _RESERVED = {
     'sprite': {'_virtual_row', '_virtual_col', '_position', '_visible', '_prior_visible',
                '_c_h_a_r_a_c_t_e_r', '_c_o_r_n_e_r', '_impassable', '_confined_to_board',
                '_egocentric_scroller', '_scrolling_group'},
+    'plain': {'_position', '_visible', '_c_h_a_r_a_c_t_e_r', '_c_o_r_n_e_r'},
     'drape': {'_c_u_r_t_a_i_n', '_c_h_a_r_a_c_t_e_r'},
     'scrolly': {'_c_u_r_t_a_i_n', '_c_h_a_r_a_c_t_e_r', '_w_h_o_l_e_p_a_t_t_e_r_n',
                 '_northwest_corner', '_prescroll_northwest_corner', '_last_maybe_move_frame',
@@ -1017,8 +1137,8 @@ def _encode(comp, base, chars, S, rows, cols, plot_keys, rng_streams):
       return int(x)
     if x[0] == 'label':
       return addr[x[1]]
-    if x[0] == 'attr':
-      return comp.attrs.index(x[1])
+    if x[0] == 'attr':                # ('attr', name) or ('attr', name, half) of a position
+      return comp.slot(x[1]) + (x[2] if len(x) > 2 else 0)
     if x[0] == 'key':
       return plot_keys.index(x[1])
     if x[0] == 'rng':

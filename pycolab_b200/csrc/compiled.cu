@@ -1,6 +1,10 @@
-// compiled.cu — the compiled step program: MazeWalkers (egocentric or not), Scrollys and
-// plain drapes whose update() bodies `pycolab_b200.compiler` translated into the bytecode
-// of include/pcl.h (PCL_OP_*).
+// compiled.cu — the compiled step program: MazeWalkers (egocentric or not), plain Sprites,
+// Scrollys and plain drapes whose update() bodies `pycolab_b200.compiler` translated into
+// the bytecode of include/pcl.h (PCL_OP_*).
+//
+// A plain Sprite (program_arg[3]) sets its own position and visibility (PCL_OP_SETFIELD)
+// and may stand anywhere: the render wraps its position as NumPy indexing does, and a
+// visible one off the board latches PCL_ENV_ERR_INDEX after its update group's render.
 //
 // Scrollys scroll with fixture.cu's motion helper (board::scrolly_move_dyn), in the one
 // scrolling group whose order words live in the plot record.  A Scrolly's curtain is the
@@ -65,6 +69,7 @@ __host__ __device__ __forceinline__ int op_operands(int op) {
     case PCL_OP_SETP: case PCL_OP_CURTAIN: case PCL_OP_ANY: case PCL_OP_MOVE:
     case PCL_OP_TERMINATE: case PCL_OP_DISCOUNT: case PCL_OP_PICK: case PCL_OP_SCROLL:
     case PCL_OP_PRESCROLL: case PCL_OP_POSTSCROLL: case PCL_OP_PATTERN: case PCL_OP_PATANY:
+    case PCL_OP_SETFIELD:
       return 1;
     default: return 0;
   }
@@ -116,6 +121,7 @@ constexpr OpInfo kOps[PCL_OP_COUNT] = {
     {2, 1},  // PATTERN
     {3, 0},  // SETPAT
     {0, 1},  // PATANY
+    {1, 0},  // SETFIELD
 };
 static_assert(sizeof(kOps) / sizeof(kOps[0]) == PCL_OP_COUNT, "one kOps entry per opcode");
 constexpr int kMaxIn = 64;            // values of an IN or a PICK
@@ -134,6 +140,21 @@ __device__ __forceinline__ int floormod(int a, int b) {
 __device__ __forceinline__ bool cell_index(int& i, int n) {
   if (i < 0) i += n;
   return (unsigned)i < (unsigned)n;
+}
+
+// Does a visible plain sprite (program_arg[3]) stand off the board, so that upstream's
+// render, `board[tuple(position)] = ...` (rendering.py:139), raises IndexError?
+// Lane s checks sprite s.
+__device__ __forceinline__ bool plain_sprite_off_board(const Ctx& c) {
+  const StepParams& p = *c.p;
+  const int s = c.lane;
+  bool off = false;
+  if (s < p.S && ((p.program_arg[3] >> s) & 1)) {
+    const int32_t* rec = c.st->sprites[s];
+    int r = rec[PCL_S_ROW], col = rec[PCL_S_COL];
+    off = (rec[PCL_S_FLAGS] & 1) && !(cell_index(r, p.H) && cell_index(col, p.W));
+  }
+  return __any_sync(PCL_FULL, off);
 }
 
 // Valid curtain bits of word w of a bit row of W cells.
@@ -225,9 +246,14 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
   const int S = p.S, H = p.H, W = p.W, lane = c.lane;
   const int32_t* code = p.code;
   const bool is_sprite = ent < S;
-  // Registers: a walker's AUX0-AUX2 (an egocentric one's permits fill AUX0 / AUX1), a
-  // Scrolly's AUX0-AUX2, a plain drape's whole record.
-  int32_t* regs = is_sprite ? &st->sprites[ent][kScroll && p.egocentric[ent] ? PCL_S_AUX2 : PCL_S_AUX0]
+  // Registers: a walker's AUX0-AUX2 (an egocentric one's permits fill AUX0 / AUX1), a plain
+  // sprite's VROW, VCOL and AUX0-AUX2 (register k >= `hole` skips FLAGS), a Scrolly's
+  // AUX0-AUX2, a plain drape's whole record.
+  const bool plain = is_sprite && ((p.program_arg[3] >> ent) & 1);
+  const int hole = plain ? PCL_S_FLAGS - PCL_S_VROW : PCL_SPRITE_WORDS;
+  int32_t* regs = is_sprite ? &st->sprites[ent][plain ? PCL_S_VROW
+                                                : kScroll && p.egocentric[ent] ? PCL_S_AUX2
+                                                                               : PCL_S_AUX0]
                             : &st->drapes[ent - S][kScroll && p.drape_kind[ent - S] ? PCL_D_AUX0 : 0];
   const LaneSlots stk = {&vm->stack[0][lane]};
   const LaneSlots loc = {&vm->local[0][lane]};
@@ -291,11 +317,19 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         stk[sp++] = f == 4 ? (rec[PCL_S_FLAGS] & 1) : rec[f];
         break;
       }
-      case PCL_OP_GETR: stk[sp++] = regs[a]; break;
+      case PCL_OP_GETR: stk[sp++] = regs[a + (a >= hole)]; break;
+      case PCL_OP_SETFIELD: {                  // row, col or the visible bit of FLAGS
+        const int v = stk[--sp];
+        int32_t* rec = st->sprites[ent];
+        __syncwarp();
+        if (lane == 0) rec[a] = a == PCL_S_FLAGS ? (rec[a] & ~1) | (v != 0) : v;
+        __syncwarp();
+        break;
+      }
       case PCL_OP_SETR: {
         const int v = stk[--sp];
         __syncwarp();
-        if (lane == 0) regs[a] = v;
+        if (lane == 0) regs[a + (a >= hole)] = v;
         __syncwarp();
         break;
       }
@@ -540,7 +574,7 @@ compiled_step(const StepParams p) {
   // Zero the board's pitch padding too: the whole H * pitch plane goes out to d_board.
   for (int i = lane; i < (int)board_bytes; i += 32) c.board[i] = 0;
   __syncwarp();
-  board::stage_board(c, restart, g_board);
+  board::stage_board</*kWrap=*/true>(c, restart, g_board);
 
   Plot plot;
   plot.frame = st->plot[PCL_P_FRAME] + 1;    // engine.py:716
@@ -561,7 +595,8 @@ compiled_step(const StepParams p) {
       for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
       run_update<kDraws, kScroll>(c, vm, ent, action, plot, dir, rw);
     }
-    board::render(c);
+    board::render</*kWrap=*/true>(c);
+    if (p.program_arg[3] && plain_sprite_off_board(c)) plot.error |= PCL_ENV_ERR_INDEX;
   }
 
   __syncwarp();
@@ -580,7 +615,7 @@ compiled_step(const StepParams p) {
   board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
 }
 
-// MazeWalkers, Scrollys and plain drapes in one scrolling group; the entities and the
+// MazeWalkers, plain Sprites, Scrollys and plain drapes in one scrolling group; the entities and the
 // z-order are consistent permutations of each other.
 int check_spec(const pcl_spec& s) {
   const int n = s.n_sprites + s.n_drapes;
@@ -611,6 +646,10 @@ int check_spec(const pcl_spec& s) {
   const uint32_t kept = (uint32_t)s.program_arg[2];
   for (int d = 0; d < 32; ++d)
     if (((kept >> d) & 1) && (d >= s.n_drapes || !s.drape_kind[d])) return PCL_ERR_INVALID;
+  // Plain Sprites: sprites only, and not egocentric.
+  const uint32_t plain = (uint32_t)s.program_arg[3];
+  for (int i = 0; i < 32; ++i)
+    if (((plain >> i) & 1) && (i >= s.n_sprites || s.sprite_egocentric[i])) return PCL_ERR_INVALID;
   if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
   return PCL_OK;
 }
@@ -638,21 +677,26 @@ CurtainAt curtain(const pcl_spec& s, int d) {
 int check_code(const pcl_spec& s, const int32_t* w, int n) {
   const int S = s.n_sprites, ents = s.n_sprites + s.n_drapes, body = 1 + ents;
   if (n <= body || n > PCL_MAX_CODE_WORDS || w[0] != ents) return PCL_ERR_INVALID;
-  enum { kNone = 0, kSprite = 1, kDrape = 2 };
+  // A walker and a plain Sprite are different kinds: their functions take different opcodes.
+  enum { kNone = 0, kSprite = 1, kDrape = 2, kPlainSprite = 3 };
+  const uint32_t plain_sprites = (uint32_t)s.program_arg[3];
+  auto is_plain_sprite = [&](int k) { return k >= 0 && k < S && ((plain_sprites >> k) & 1); };
   // What the entities sharing a function allow it: their kind, the fewest registers any of
-  // them has (1 for an egocentric walker, 3 for a walker or a Scrolly, 8 for a plain
-  // drape), whether they are all Scrollys, all plain drapes, all Scrollys that write
-  // their pattern.
+  // them has (1 for an egocentric walker, 3 for a walker or a Scrolly, 5 for a plain
+  // sprite, 8 for a plain drape), whether they are all Scrollys, all plain drapes, all
+  // Scrollys that write their pattern.
   struct Fn { int8_t kind, regs; bool scrolly, plain, writes; };
   std::vector<Fn> starts(n, Fn{kNone, 0, false, false, false});   // by first word
   for (int i = 0; i < ents; ++i) {
-    const int e = w[1 + i], kind = i < S ? kSprite : kDrape;
+    const int e = w[1 + i];
+    const int kind = i >= S ? kDrape : is_plain_sprite(i) ? kPlainSprite : kSprite;
     if (e < body || e >= n) return PCL_ERR_INVALID;
     if (starts[e].kind != kNone && starts[e].kind != kind) return PCL_ERR_INVALID;
     const bool scrolly = kind == kDrape && s.drape_kind[i - S];
     const bool writes = scrolly && ((s.program_arg[2] >> (i - S)) & 1);
-    const int regs = kind == kSprite ? (s.sprite_egocentric[i] ? 1 : 3)
-                                     : (scrolly ? 3 : PCL_DRAPE_WORDS);
+    const int regs = kind == kPlainSprite ? 5
+                     : kind == kSprite ? (s.sprite_egocentric[i] ? 1 : 3)
+                                       : (scrolly ? 3 : PCL_DRAPE_WORDS);
     Fn& f = starts[e];
     if (f.kind == kNone) f = Fn{(int8_t)kind, (int8_t)regs, scrolly, !scrolly && kind == kDrape, writes};
     f.regs = (int8_t)(regs < f.regs ? regs : f.regs);
@@ -683,7 +727,8 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
     int len = 1 + op_operands(op);
     if (pc + len > end) return PCL_ERR_INVALID;
     const int a = len > 1 ? w[pc + 1] : 0;
-    const bool sprite = kind == kSprite;
+    const bool walker = kind == kSprite, plain_sprite = kind == kPlainSprite;
+    const bool sprite = walker || plain_sprite;
     switch (op) {
       case PCL_OP_LOAD: case PCL_OP_STORE:
         if (a < 0 || a >= PCL_CODE_LOCALS) return PCL_ERR_INVALID;
@@ -705,9 +750,18 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (a < 0 || a >= s.program_arg[1]) return PCL_ERR_INVALID;
         if (w[pc + 2] < 0 || w[pc + 2] > 5) return PCL_ERR_INVALID;
         break;
-      case PCL_OP_FIELD:
+      case PCL_OP_FIELD: {
         if (a < 0 ? !sprite : a >= S) return PCL_ERR_INVALID;
-        if (w[pc + 2] < 0 || w[pc + 2] > 4) return PCL_ERR_INVALID;
+        const int f = w[pc + 2];
+        if (f < 0 || f > 4) return PCL_ERR_INVALID;
+        // A plain Sprite has no virtual position.
+        if ((f == PCL_S_VROW || f == PCL_S_VCOL) && (a < 0 ? plain_sprite : is_plain_sprite(a)))
+          return PCL_ERR_INVALID;
+        break;
+      }
+      case PCL_OP_SETFIELD:
+        if (!plain_sprite || (a != PCL_S_ROW && a != PCL_S_COL && a != PCL_S_FLAGS))
+          return PCL_ERR_INVALID;
         break;
       case PCL_OP_GETR: case PCL_OP_SETR:
         if (a < 0 || a >= fn.regs) return PCL_ERR_INVALID;
@@ -731,10 +785,10 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (!is_scrolly(a, fn)) return PCL_ERR_INVALID;
         break;
       case PCL_OP_MOVE:
-        if (!sprite || a < 0 || a > PCL_M_STAY) return PCL_ERR_INVALID;
+        if (!walker || a < 0 || a > PCL_M_STAY) return PCL_ERR_INVALID;
         break;
       case PCL_OP_TELEPORT:
-        if (!sprite) return PCL_ERR_INVALID;
+        if (!walker) return PCL_ERR_INVALID;
         break;
       case PCL_OP_REWARD_F64:
         if (!s.program_arg[0]) return PCL_ERR_INVALID;   // an int32 reward cannot carry it

@@ -54,7 +54,11 @@ __device__ __forceinline__ bool drape_bit(const Ctx& c, int d, int r, int col) {
   return bit_at(bits_row(c, d, r), col);
 }
 
-// engine.py:737-759 + rendering.py:98-160 into the smem board.
+// engine.py:737-759 + rendering.py:98-160 into the smem board.  kWrap: sprite positions
+// may lie off the board (compiled.cu's plain Sprites), and a visible sprite paints at its
+// NumPy-wrapped cell, `board[tuple(position)]` (rendering.py:139): a negative row or
+// column counts from the end once, and a position no cell matches paints nothing.
+template <bool kWrap = false>
 __device__ inline void render(const Ctx& c) {
   const StepParams& p = *c.p;
   const int n = p.S + p.D, cells = p.H * p.W;
@@ -66,7 +70,14 @@ __device__ inline void render(const Ctx& c) {
       for (int s = 0; s < p.S; ++s) {
         if (p.sprite_char[s] == ch) {
           const int32_t* rec = c.st->sprites[s];
-          if ((rec[PCL_S_FLAGS] & 1) && rec[PCL_S_ROW] == r && rec[PCL_S_COL] == col) code = ch;
+          if (kWrap) {
+            int sr = rec[PCL_S_ROW], sc = rec[PCL_S_COL];
+            sr += sr < 0 ? p.H : 0;
+            sc += sc < 0 ? p.W : 0;
+            if ((rec[PCL_S_FLAGS] & 1) && sr == r && sc == col) code = ch;
+          } else if ((rec[PCL_S_FLAGS] & 1) && rec[PCL_S_ROW] == r && rec[PCL_S_COL] == col) {
+            code = ch;
+          }
         }
       }
       for (int d = 0; d < p.D; ++d)
@@ -168,9 +179,10 @@ __device__ __forceinline__ void stage_records(WarpState* st, const int32_t* src_
 
 // The board every entity of the first update group reads: the pre-initial render
 // (engine.py:572-578) at a restart, else last step's final board from `g_board`.
+template <bool kWrap = false>
 __device__ __forceinline__ void stage_board(const Ctx& c, bool restart, const uint8_t* g_board) {
   if (restart) {
-    render(c);
+    render<kWrap>(c);
   } else {
     const int n16 = (c.p->H * c.p->pitch) >> 4;
     for (int i = c.lane; i < n16; i += 32)

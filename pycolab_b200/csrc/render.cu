@@ -72,8 +72,14 @@ render_kernel(const RenderParams p) {
   }
   if (threadIdx.x < p.S) {
     const int32_t* rec = p.sprites + ((int64_t)env * p.S + threadIdx.x) * PCL_SPRITE_WORDS;
-    const int row = rec[PCL_S_ROW], col = rec[PCL_S_COL];
-    const bool vis = rec[PCL_S_FLAGS] & 1;                     // engine.py:754
+    // `board[tuple(position)]` (rendering.py:139): a negative row or column counts from
+    // the end once; a position still off the board (a plain Sprite may stand anywhere)
+    // paints nothing.
+    int row = rec[PCL_S_ROW], col = rec[PCL_S_COL];
+    row += row < 0 ? p.H : 0;
+    col += col < 0 ? p.W : 0;
+    const bool vis = (rec[PCL_S_FLAGS] & 1) &&                 // engine.py:754
+                     (unsigned)row < (unsigned)p.H && (unsigned)col < (unsigned)p.W;
     sh.seg[threadIdx.x] = vis ? row * segs_per_row + (col >> 4) : -1;
     sh.word[threadIdx.x] = (col & 15) >> 2;
     sh.cover[threadIdx.x] = 0xffu << ((col & 3) * 8);
@@ -158,8 +164,11 @@ __global__ void __launch_bounds__(256) layers_kernel(const LayersParams p) {
       const int sidx = p.sprite_of[k];
       if (sidx >= 0) {
         const int32_t* rec = p.sprites + ((int64_t)env * p.S + sidx) * PCL_SPRITE_WORDS;
-        const int dc = rec[PCL_S_COL] - c0;
-        if ((rec[PCL_S_FLAGS] & 1) && rec[PCL_S_ROW] == r && (unsigned)dc < 16u) {
+        int sr = rec[PCL_S_ROW], sc = rec[PCL_S_COL];      // wrapped as render_kernel does
+        sr += sr < 0 ? p.H : 0;
+        sc += sc < 0 ? p.W : 0;
+        const int dc = sc - c0;
+        if ((rec[PCL_S_FLAGS] & 1) && sr == r && (unsigned)sc < (unsigned)p.W && (unsigned)dc < 16u) {
           uint32_t* w = dc < 4 ? &px.x : dc < 8 ? &px.y : dc < 12 ? &px.z : &px.w;
           *w |= 1u << ((dc & 3) * 8);
         }

@@ -135,8 +135,8 @@ def role_of(entity):
   from pycolab_b200 import compiler
   compiled = compiler.registered(cls)
   if compiled is not None:
-    return {'sprite': 'compiled.walker', 'scrolly': 'compiled.scrolly',
-            'drape': 'compiled.drape'}[compiled.kind]
+    return {'sprite': 'compiled.walker', 'plain': 'compiled.sprite',
+            'scrolly': 'compiled.scrolly', 'drape': 'compiled.drape'}[compiled.kind]
   for klass in cls.__mro__:
     key = (klass.__module__.rsplit('.', 1)[-1], klass.__name__)
     if key in LOWERED_CLASSES:
@@ -239,7 +239,9 @@ class LoweredGame(object):
                                 # Python objects after a step
     self.action_row = None      # (Engine, facade actions) -> the env's action words
     self.code = None            # i32 bytecode words (pcl_bind_code) of the compiled program
-    self.registers = {}         # compiled: char -> [(attribute, is_bool)] in register order
+    self.registers = {}         # compiled: char -> [(attribute, type)] in register order, type
+                                # the value's at lowering: bool, int, things.Sprite.Position
+                                # or tuple (the last two: a position attribute, two registers)
     self.plot_keys = []         # compiled: [(the_plot key, is_bool)] in plot register order
 
   @property

@@ -1,5 +1,6 @@
-"""The compiled program `csrc/compiled.cu`: MazeWalkers, Scrollys and plain drapes of classes
-registered with `pycolab_b200.compiler`, whose update() bodies run as device bytecode."""
+"""The compiled program `csrc/compiled.cu`: MazeWalkers, plain Sprites, Scrollys and plain
+drapes of classes registered with `pycolab_b200.compiler`, whose update() bodies run as
+device bytecode."""
 
 import numpy as np
 
@@ -8,7 +9,7 @@ from pycolab_b200 import compiler
 from pycolab_b200 import things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.lowering import (LoweredGame, _common, _plot_record, _scrolly_record,
-                                   _set_sprites, _sprite_record, pack_rows, round_up)
+                                   _sprite_record, _walker_meta, pack_rows, round_up)
 
 _INT32 = (-2 ** 31, 2 ** 31 - 1)
 
@@ -25,12 +26,25 @@ def _register_value(owner, value):
       owner, value))
 
 
+def _position_value(owner, value):
+  """The (row, col) of a position attribute and its type (things.Sprite.Position or tuple),
+  or NotLoweredError."""
+  if ((isinstance(value, things.Sprite.Position) or type(value) is tuple) and len(value) == 2 and
+      all(isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+          for x in value)):
+    words = [_register_value(owner, x)[0] for x in value]
+    return words, (things.Sprite.Position if isinstance(value, things.Sprite.Position) else tuple)
+  raise NotLoweredError('{} holds {!r}: a position attribute holds a Position or a tuple of '
+                        'two ints'.format(owner, value))
+
+
 def lower(engine, roles):
   th = engine.things
   game = LoweredGame()
   _common(engine, game, _lib.PROG_COMPILED)
   order = ''.join(game.groups)
-  sprite_chars = [c for c in order if roles[c] == 'compiled.walker']
+  sprite_chars = [c for c in order if roles[c] in ('compiled.walker', 'compiled.sprite')]
+  plain = [c for c in sprite_chars if roles[c] == 'compiled.sprite']
   drape_chars = [c for c in order if roles[c] in ('compiled.drape', 'compiled.scrolly')]
   if len(sprite_chars) > _lib.MAX_SPRITES or len(drape_chars) > _lib.MAX_DRAPES:
     raise NotLoweredError('too many entities for the compiled device program')
@@ -40,7 +54,7 @@ def lower(engine, roles):
       raise NotLoweredError('drape {!r} overrides `curtain`'.format(ch))
   scrollys = [ch for ch in drape_chars if roles[ch] == 'compiled.scrolly']
   # One scrolling group: its order words are the plot record's.
-  groups = {th[ch]._scrolling_group for ch in sprite_chars + scrollys}
+  groups = {th[ch]._scrolling_group for ch in sprite_chars + scrollys if ch not in plain}
   if len(groups) > 1:
     raise NotLoweredError('more than one scrolling group ({}): the compiled program keeps '
                           'one'.format(sorted(groups)))
@@ -56,6 +70,10 @@ def lower(engine, roles):
         if ins[1][1] in roles and roles[ins[1][1]] != 'compiled.scrolly':
           raise NotLoweredError('{}: things[{!r}] is not a Scrolly'.format(
               compiler._name(comp[ch].klass), ins[1][1]))
+      if (ins[0] == 'FIELD' and isinstance(ins[1], tuple) and ins[1][1] in plain and
+          ins[2] in (_lib.FIELD_VROW, _lib.FIELD_VCOL)):
+        raise NotLoweredError('{}: things[{!r}].virtual_position: a plain Sprite has none'.format(
+            compiler._name(comp[ch].klass), ins[1][1]))
 
   # the_plot keys: plot registers AUX0.. in order of first use
   keys = []
@@ -82,27 +100,49 @@ def lower(engine, roles):
     c = comp[ch]
     ego = c.kind == 'sprite' and bool(th[ch]._egocentric_scroller)
     limit = compiler.MAX_EGOCENTRIC_REGISTERS if ego else compiler.MAX_REGISTERS[c.kind]
-    if len(c.attrs) > limit:
+    if c.n_registers > limit:
       raise NotLoweredError('{} {!r} needs {} registers; {} has {}'.format(
-          compiler._name(c.klass), ch, len(c.attrs),
-          'an egocentric walker' if ego else 'a ' + c.kind, limit))
+          compiler._name(c.klass), ch, c.n_registers,
+          'an egocentric walker' if ego else
+          'a plain Sprite' if c.kind == 'plain' else 'a ' + c.kind, limit))
     regs = []
     values[ch] = []
     for name in c.attrs:
       if not hasattr(th[ch], name):
         raise NotLoweredError('{!r}.{} is used by update() but not set when the game is '
                               'lowered'.format(ch, name))
-      value, is_bool = _register_value('{!r}.{}'.format(ch, name), getattr(th[ch], name))
-      regs.append((name, is_bool))
-      values[ch].append(value)
+      owner = '{!r}.{}'.format(ch, name)
+      if c.attr_types.get(name) == 'pos':
+        words, kind = _position_value(owner, getattr(th[ch], name))
+      else:
+        value, is_bool = _register_value(owner, getattr(th[ch], name))
+        words, kind = [value], (bool if is_bool else int)
+      regs.append((name, kind))
+      values[ch] += words
     registers[ch] = regs
 
   sprites = [th[c] for c in sprite_chars]
-  # an egocentric walker's permits start empty (AUX0 = 0, AUX1 = never), its register in AUX2
-  _set_sprites(game, sprites, [
-      _sprite_record(s, 0, _lib.NEVER, (values[s.character] + [0])[0])
-      if s._egocentric_scroller else _sprite_record(s, *(values[s.character] + [0, 0, 0])[:3])
-      for s in sprites], named_groups=True)
+  records = []
+  for s in sprites:
+    v = values[s.character]
+    if s.character in plain:           # registers VROW, VCOL, AUX0-AUX2
+      rec = _sprite_record(s, *(v[2:] + [0, 0, 0])[:3])
+      rec[_lib.S_VROW:_lib.S_VCOL + 1] = (v + [0, 0])[:2]
+    elif s._egocentric_scroller:       # permits start empty (AUX0 = 0, AUX1 = never)
+      rec = _sprite_record(s, 0, _lib.NEVER, (v + [0])[0])
+    else:
+      rec = _sprite_record(s, *(v + [0, 0, 0])[:3])
+    records.append(rec)
+  game.sprite_chars = ''.join(sprite_chars)
+  meta = [([0, 0, 0, 0], False, False) if ch in plain else _walker_meta(th[ch], named_groups=True)
+          for ch in sprite_chars]
+  game.impassable = [m[0] for m in meta]
+  game.confined = [m[1] for m in meta]
+  game.egocentric = [m[2] for m in meta]
+  game.sprites = np.array(records, dtype=np.int32).reshape(len(sprites), _lib.SPRITE_WORDS)
+  for s, ch in enumerate(sprite_chars):
+    if ch in plain:
+      game.program_arg[3] |= 1 << s
   game.drape_chars = ''.join(drape_chars)
   game.margins = [(-1, -1)] * len(drape_chars)
   game.drape_kind = [0] * len(drape_chars)
@@ -152,7 +192,8 @@ def lower(engine, roles):
 
 
 def sync(engine):
-  """Registers back into the entities' attributes and the Plot's keys (bool stays bool)."""
+  """Registers back into the entities' attributes and the Plot's keys, each with the type its
+  value had at lowering (bool stays bool, a Position stays a Position)."""
   b = engine.batched
   game = b.game
   sprites = b.sprites[0].cpu().numpy()
@@ -162,12 +203,20 @@ def sync(engine):
   for ch, regs in game.registers.items():
     if ch in b.sprite_chars:
       s = b.sprite_chars.index(ch)
-      words = sprites[s][_lib.S_AUX2 if game.egocentric[s] else _lib.S_AUX0:]
+      rec = sprites[s]
+      if (game.program_arg[3] >> s) & 1:         # a plain Sprite: VROW, VCOL, AUX0-AUX2
+        words = list(rec[_lib.S_VROW:_lib.S_VCOL + 1]) + list(rec[_lib.S_AUX0:])
+      else:
+        words = list(rec[_lib.S_AUX2 if game.egocentric[s] else _lib.S_AUX0:])
     else:
       d = b.drape_chars.index(ch)
-      words = drapes[d][_lib.D_AUX0 if game.drape_kind[d] else 0:]
-    for (name, is_bool), word in zip(regs, words):
-      setattr(th[ch], name, bool(word) if is_bool else int(word))
+      words = list(drapes[d][_lib.D_AUX0 if game.drape_kind[d] else 0:])
+    for name, kind in regs:
+      if kind in (bool, int):
+        setattr(th[ch], name, kind(words.pop(0)))
+      else:
+        pair = (int(words.pop(0)), int(words.pop(0)))
+        setattr(th[ch], name, pair if kind is tuple else kind(*pair))
   for k, (key, is_bool) in enumerate(game.plot_keys):
     word = plot[_lib.P_AUX0 + k]
     engine.the_plot[key] = bool(word) if is_bool else int(word)
