@@ -120,7 +120,12 @@ typedef enum pcl_program {
                                 the number of RNG slots the code draws from (0-2); with slots,
                                 pcl_state.d_rng is required and is u32 [B, program_arg[1],
                                 PCL_MT_WORDS], each slot the words of NumPy's RandomState or of
-                                Python's random.Random, continued across auto-resets */
+                                Python's random.Random, continued across auto-resets.  program_arg[4] = 1:
+                                the game's Backdrop has compiled update() code (a function of its own,
+                                header word 1 + n of the bytecode) that runs once per step before update
+                                group 0 and writes a per-env live curtain, bound with pcl_bind_backdrop;
+                                d_backdrop is then its per-level reset template (0: the backdrop is
+                                static and d_backdrop is read directly) */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */
@@ -156,7 +161,8 @@ enum { PCL_DIR_NONE = 0,
 
 /* PCL_PROG_COMPILED bytecode (pcl_bind_code): int32 words.  Word 0 = n, the number of entities
  * (n_sprites + n_drapes); words 1..n = the first word of each entity's update() (sprites first,
- * then drapes, in spec order).  Entities of one class share their code.  The entry points split
+ * then drapes, in spec order); with program_arg[4] set, word 1 + n = the first word of the
+ * Backdrop's update().  Entities of one class share their code.  The entry points split
  * the words after the header into functions; each ends with PCL_OP_RET, and its jumps go
  * forward to a word inside it, so every update ends.  The operand stack holds int32 values;
  * "pop r, c" pops c first.  An entity operand of -1 means the entity being updated.  Cell
@@ -230,6 +236,13 @@ enum {
    * (rendering.py:139, `board[tuple(position)]`). */
   PCL_OP_SETFIELD,      /* f: pop v into the updated plain sprite's row (f 0), col (f 1) or
                            visible bit (f 4, v != 0); the write twin of FIELD                 */
+  /* The Backdrop's update() (program_arg[4]): these three appear only in its function, which
+   * has no registers, no motion, no drape or pattern writes and no -1 entity operand.  They
+   * write the env's live curtain; BACKDROP reads it, and every later render paints it. */
+  PCL_OP_SETBACK,       /* pop r, c, v: the live curtain at (r, c) = v (as a byte)             */
+  PCL_OP_FILLBACK,      /* pop v: every cell of the live curtain = v (as a byte)              */
+  PCL_OP_ROLLBACK,      /* axis, lo, hi: pop shift; rows lo .. hi - 1 = np.roll(those rows, shift,
+                           axis) (axis 0 or 1, 0 <= lo <= hi <= rows)                         */
   PCL_OP_COUNT
 };
 
@@ -385,6 +398,13 @@ int pcl_bind_state(pcl_handle* h, const pcl_state* state);
  * safe: the upload first waits for the device.  Other programs: PCL_ERR_UNSUPPORTED.
  * pcl_reset / pcl_step return PCL_ERR_UNBOUND until code is bound. */
 int pcl_bind_code(pcl_handle* h, const int32_t* h_code, int32_t n_words);
+
+/* PCL_PROG_COMPILED with program_arg[4] set: the Backdrop's live curtains, u8 [B, rows, pitch]
+ * (caller-owned DEVICE memory).  A (re)start copies the env's level template (d_backdrop,
+ * indexed through d_level) into its row; the Backdrop's code then writes it, the step's renders
+ * and pcl_layers read it.  PCL_ERR_INVALID for a NULL buffer and for every other handle.  The
+ * step and reset entry points of such a handle return PCL_ERR_UNBOUND until it is bound. */
+int pcl_bind_backdrop(pcl_handle* h, uint8_t* d_backdrop_live);
 
 /* Engine.its_showtime() (engine.py:520-581) for every env whose d_env_mask
  * byte is non-zero (NULL = all): restore the reset templates, then run the

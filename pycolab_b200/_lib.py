@@ -60,9 +60,13 @@ OPS = ('RET', 'PUSH', 'POP', 'DUP', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'ADD', 
        # the updated one); SETPAT writes the updated Scrolly's pattern.
        'SCROLL', 'PRESCROLL', 'POSTSCROLL', 'PATTERN', 'SETPAT', 'PATANY',
        # Plain Sprites: SETFIELD f sets the updated sprite's row, col or visible bit.
-       'SETFIELD')
+       'SETFIELD',
+       # The Backdrop's live curtain: SETBACK a cell, FILLBACK all of it, ROLLBACK axis, lo, hi
+       # a band of rows as np.roll does.
+       'SETBACK', 'FILLBACK', 'ROLLBACK')
 OP = {name: code for code, name in enumerate(OPS)}
 OPERANDS = {OP[n]: (4 if n == 'RANDCMP' else
+                    3 if n == 'ROLLBACK' else
                     2 if n in ('FIELD', 'REWARD_F64', 'RANDINT') else
                     1 if n in ('PUSH', 'LOAD', 'STORE', 'JMP', 'JZ', 'JNZ', 'IN', 'GETR', 'SETR',
                                'GETP', 'SETP', 'CURTAIN', 'ANY', 'MOVE', 'TERMINATE',
@@ -184,6 +188,7 @@ SYMBOLS = {
     'pcl_destroy': (C.c_int, [C.c_void_p]),
     'pcl_bind_state': (C.c_int, [C.c_void_p, C.POINTER(State)]),
     'pcl_bind_code': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
+    'pcl_bind_backdrop': (C.c_int, [C.c_void_p, C.c_void_p]),
     'pcl_reset': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_step': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_run': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs), C.c_void_p]),

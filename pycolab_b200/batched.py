@@ -206,6 +206,11 @@ class BatchedEngine(object):
     if g0.code is not None:       # the compiled program's bytecode, shared by every level
       code = np.ascontiguousarray(g0.code, dtype=np.int32)
       _lib.check(self._lib.pcl_bind_code(self._h, code.ctypes.data, len(code)), 'pcl_bind_code')
+    self.backdrop_live = None   # u8 [B, rows, pitch]: a compiled Backdrop's curtains as they are now
+    if g0.program == _lib.PROG_COMPILED and g0.program_arg[4]:
+      self.backdrop_live = per_env([g.backdrop for g in games], np.uint8)
+      _lib.check(self._lib.pcl_bind_backdrop(self._h, self.backdrop_live.data_ptr()),
+                 'pcl_bind_backdrop')
     self._showtime = False
 
   # ---------------------------------------------------------------- running

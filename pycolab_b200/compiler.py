@@ -14,7 +14,9 @@ and the construct):
   entities    MazeWalker subclasses (any impassable set, confined or not, egocentric or
               not), plain Sprite subclasses (things.Sprite, not MazeWalker), Scrolly
               subclasses and plain Drape subclasses, all in one scrolling group; the
-              Scrollys' patterns all of one shape;
+              Scrollys' patterns all of one shape; a Backdrop subclass with its own
+              update(self, actions, board, layers, things, the_plot), which has no
+              registers and runs before update group 0;
   statements  if / elif / else, return, pass; `del` and docstrings compile to nothing;
               local variables holding an int, a bool, a position or a motion result;
               `r, c = <position>`;
@@ -28,6 +30,12 @@ and the construct):
               on plain Sprites `self._position = <position>` (not a bare tuple: upstream
               `.row` would fail on it later) and `self._visible = <truth value>`;
               on Scrollys `self.whole_pattern[cell] = v` (their own pattern only);
+              on a Backdrop `self.curtain[cell] = v`, `self.curtain[:] = v` and
+              `self.curtain[a:b, :] = np.roll(self.curtain[a:b, :], shift, axis)` (also
+              `[a:b]`, or the whole curtain; int literal bounds, the same band on both
+              sides, the literal axis 0 or 1, np.roll found as draws are), where v is a
+              palette look-up, ord('c'), an int literal 0..255, a board or curtain cell,
+              a bool, or `x if c else y` of these (each lies in 0..255);
   values      `actions` (==, !=, in, is None only), int and bool literals (float literals
               only as a reward or a discount), + - * // % and unary -, comparisons
               (chained, position against position or tuple), `in` over a literal
@@ -41,6 +49,10 @@ and the construct):
               `board[cell]`, `backdrop.curtain[cell]`, `layers['X'][cell]`,
               `self.curtain[cell]`, `things['X'].position / .visible / .curtain[cell]`,
               `.curtain.any()` (a Scrolly's curtain is its pattern window);
+              `board.shape`, `board.shape[0]`, `board.shape[1]`; in a Backdrop also
+              `self.curtain.shape`, `self.curtain[cell]` (its live curtain) and
+              `self.palette.X` / `self.palette['X']` (aliases included; lowering checks
+              the character against the game's palette);
               of Scrollys (`self` or `things['X']`): `.pattern_position_prescroll(pos,
               the_plot)`, `.pattern_position_postscroll(pos, the_plot)`,
               `.whole_pattern[cell]`, `.whole_pattern.any()`.
@@ -77,6 +89,7 @@ import types
 import numpy as np
 
 from pycolab_b200 import _lib
+from pycolab_b200 import engine as engine_lib
 from pycolab_b200 import things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.prefab_parts import drapes as prefab_drapes
@@ -85,6 +98,7 @@ from pycolab_b200.prefab_parts import sprites as prefab_sprites
 _REGISTRY = {}                # class -> Compiled
 
 _PARAMS = ('self', 'actions', 'board', 'layers', 'backdrop', 'things', 'the_plot')
+_BACKDROP_PARAMS = ('self', 'actions', 'board', 'layers', 'things', 'the_plot')
 _MOTIONS = {'_north': 0, '_northeast': 1, '_east': 2, '_southeast': 3, '_south': 4,
             '_southwest': 5, '_west': 6, '_northwest': 7, '_stay': 8}
 _BINOPS = {ast.Add: 'ADD', ast.Sub: 'SUB', ast.Mult: 'MUL', ast.FloorDiv: 'FLOORDIV',
@@ -184,11 +198,13 @@ def compile_class(klass):
     kind = 'scrolly'
   elif issubclass(klass, things.Drape):
     kind = 'drape'
+  elif issubclass(klass, things.Backdrop):
+    kind = 'backdrop'
   else:
-    raise NotLoweredError('{}: only Sprite, MazeWalker, Scrolly and plain Drape subclasses '
-                          'are compiled'.format(_name(klass)))
+    raise NotLoweredError('{}: only Sprite, MazeWalker, Scrolly, plain Drape and Backdrop '
+                          'subclasses are compiled'.format(_name(klass)))
   if klass.update in (prefab_sprites.MazeWalker.update, things.Sprite.update,
-                      things.Drape.update):
+                      things.Drape.update, things.Backdrop.update):
     raise NotLoweredError('{}: has no update() of its own to compile'.format(_name(klass)))
   return _Compiler(klass, kind).run()
 
@@ -211,11 +227,12 @@ class _Compiler(object):
     tree = ast.parse(textwrap.dedent(''.join(lines)))
     self.fdef = tree.body[0]
     args = self.fdef.args
-    if (not isinstance(self.fdef, ast.FunctionDef) or len(args.args) != len(_PARAMS) or
+    params = _BACKDROP_PARAMS if kind == 'backdrop' else _PARAMS
+    if (not isinstance(self.fdef, ast.FunctionDef) or len(args.args) != len(params) or
         args.vararg or args.kwarg or args.kwonlyargs or self.fdef.decorator_list):
-      raise NotLoweredError('{}: update() must take the seven standard arguments'.format(
-          _name(klass)))
-    self.role = {a.arg: role for a, role in zip(args.args, _PARAMS)}
+      raise NotLoweredError('{}: update() must take the {} standard arguments'.format(
+          _name(klass), 'six' if kind == 'backdrop' else 'seven'))
+    self.role = {a.arg: role for a, role in zip(args.args, params)}
     self.ir = []
     self.n_labels = 0
     self.locals = {}              # name -> (first slot, type)
@@ -275,6 +292,9 @@ class _Compiler(object):
     return key
 
   def check_attr(self, node, name):
+    if self.kind == 'backdrop':
+      self.refuse(node, 'attribute self.{} (a Backdrop has no registers; keep its state in '
+                  'the_plot)'.format(name))
     reserved = _RESERVED.get(self.kind, ())
     if (name in reserved or hasattr(self.klass, name) or
         any(r.endswith('*') and name.startswith(r[:-1]) for r in reserved)):
@@ -435,6 +455,12 @@ class _Compiler(object):
       self.emit('STORE', slots[1])
       self.emit('STORE', slots[0])
       return
+    if isinstance(target, ast.Subscript) and self.is_self_curtain(target.value):
+      if self.kind == 'backdrop':
+        return self.backdrop_write(target.slice, value, st)
+    if (isinstance(target, ast.Subscript) and isinstance(target.value, ast.Attribute) and
+        target.value.attr == 'curtain' and self.is_param(target.value.value, 'backdrop')):
+      self.refuse(st, "a write to backdrop.curtain (only the Backdrop's own update() writes it)")
     if isinstance(target, ast.Subscript) and self.pattern_owner(target.value) is not None:
       if self.pattern_owner(target.value) != -1:
         self.refuse(st, "a write to another entity's whole_pattern")
@@ -601,6 +627,8 @@ class _Compiler(object):
     """Two emitters (row, col) of a position expression, else None."""
     def field(ent, f):
       return lambda: self.emit('FIELD', ent, f)
+    if self.is_shape(node):
+      return (lambda: self.emit('PUSH', ('rows',)), lambda: self.emit('PUSH', ('cols',)))
     if isinstance(node, ast.Attribute):
       owner = None
       if self.is_self(node.value):
@@ -619,7 +647,7 @@ class _Compiler(object):
         if name is not None and self.attr_types.get(name) == 'pos':
           reg = self.use_attr(node, name, 'pos')
           return (lambda: self.emit('GETR', reg + (0,)), lambda: self.emit('GETR', reg + (1,)))
-        if node.attr == 'corner':
+        if node.attr == 'corner' and self.kind != 'backdrop':
           return (lambda: self.emit('PUSH', ('rows',)), lambda: self.emit('PUSH', ('cols',)))
     if isinstance(node, ast.Name) and self.locals.get(node.id, (0, None))[1] == 'pos':
       slot = self.locals[node.id][0]
@@ -723,6 +751,12 @@ class _Compiler(object):
     self.refuse(node, type(node).__name__)
 
   def attribute(self, node):
+    ch = self.palette_char(node)
+    if ch is not None:
+      self.emit('PUSH', ('palette', ch))
+      return 'int'
+    if node.attr in ('row', 'col') and self.is_shape(node.value):
+      self.refuse(node, 'the attribute .' + node.attr + ' of a shape')
     if self.pos_parts(node) is not None and not isinstance(node, ast.Tuple):
       for part in self.pos_parts(node):
         part()
@@ -803,7 +837,17 @@ class _Compiler(object):
     if key is not None:
       self.emit('GETP', ('key', key))
       return 'int'
+    ch = self.palette_char(node)
+    if ch is not None:
+      self.emit('PUSH', ('palette', ch))
+      return 'int'
     base, sl = node.value, node.slice
+    if self.kind == 'backdrop' and self.is_self_curtain(base):   # its own live curtain
+      if _sliced(sl):
+        self.refuse(node, 'reading a curtain slice')
+      self.cell(sl, node)
+      self.emit('BACKDROP')
+      return 'int'
     if self.is_param(base, 'board'):
       self.cell(sl, node)
       self.emit('BOARD')
@@ -1082,6 +1126,141 @@ class _Compiler(object):
     self.emit(name)
 
 
+  # ------------------------------------------------------------- Backdrops
+  def is_self_curtain(self, node):
+    return isinstance(node, ast.Attribute) and node.attr == 'curtain' and self.is_self(node.value)
+
+  def is_shape(self, node):
+    """`board.shape`, or `self.curtain.shape` in a Backdrop: (rows, cols)."""
+    return (isinstance(node, ast.Attribute) and node.attr == 'shape' and
+            (self.is_param(node.value, 'board') or
+             (self.kind == 'backdrop' and self.is_self_curtain(node.value))))
+
+  def palette_char(self, node):
+    """The character of `self.palette.X` / `self.palette['X']` in a Backdrop, its alias
+    resolved (engine.py Palette), else None.  Lowering checks it against the palette."""
+    if self.kind != 'backdrop':
+      return None
+    if isinstance(node, ast.Attribute):
+      base, key = node.value, node.attr
+    elif (isinstance(node, ast.Subscript) and isinstance(node.slice, ast.Constant) and
+          isinstance(node.slice.value, str)):
+      base, key = node.value, node.slice.value
+    else:
+      return None
+    if not (isinstance(base, ast.Attribute) and base.attr == 'palette' and self.is_self(base.value)):
+      return None
+    return engine_lib.Palette._ALIASES.get(key, key)
+
+  def is_byte(self, node):
+    """Does `node` always lie in 0..255, so that NumPy stores it in a uint8 cell as it is?"""
+    if isinstance(node, ast.Constant):
+      return isinstance(node.value, bool) or (isinstance(node.value, int) and
+                                               0 <= node.value <= 255)
+    if self.palette_char(node) is not None:
+      return True
+    if (isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id == 'ord'
+        and len(node.args) == 1 and isinstance(node.args[0], ast.Constant) and
+        isinstance(node.args[0].value, str) and len(node.args[0].value) == 1):
+      return ord(node.args[0].value) <= 255
+    if isinstance(node, (ast.Compare, ast.UnaryOp)):
+      return isinstance(node, ast.Compare) or isinstance(node.op, ast.Not)
+    if isinstance(node, ast.Subscript) and not _sliced(node.slice):
+      base = node.value
+      return (self.is_param(base, 'board') or self.is_self_curtain(base) or
+              (isinstance(base, ast.Attribute) and base.attr == 'curtain' and
+               self.thing_char(base.value) is not None) or
+              (isinstance(base, ast.Subscript) and self.is_param(base.value, 'layers')))
+    return False
+
+  def byte(self, node):
+    """A value for a curtain cell: a form that lies in 0..255, or `x if c else y` of them.
+    NumPy 2 raises OverflowError when a Python int outside 0..255 is stored in a uint8 cell
+    but wraps a NumPy int; a device int32 does not say which it was, so no other int is
+    written."""
+    if isinstance(node, ast.IfExp):
+      other, end = self.label(), self.label()
+      self.truth(node.test)
+      self.emit('JZ', other)
+      self.byte(node.body)
+      self.emit('JMP', end)
+      self.place(other)
+      self.byte(node.orelse)
+      self.place(end)
+      return
+    if not self.is_byte(node):
+      self.refuse(node, 'a curtain value that may lie outside 0..255 (write a palette '
+                  "character, ord('c'), an int literal 0..255, a board or curtain cell or a bool)")
+    self.scalar(node)
+
+  def band(self, sl, where):
+    """(lo, hi) of a band of rows `[a:b]` / `[a:b, :]` (None where omitted), or None for a
+    cell index.  Refuses every other slice."""
+    elts = sl.elts if isinstance(sl, ast.Tuple) else [sl]
+    if not any(isinstance(x, ast.Slice) for x in elts):
+      return None
+    rows = elts[0]
+    full = lambda x: (isinstance(x, ast.Slice) and x.lower is None and x.upper is None and
+                      x.step is None)
+    if not isinstance(rows, ast.Slice) or len(elts) > 2 or (len(elts) == 2 and not full(elts[1])):
+      self.refuse(where, 'a row or column slice other than a band of rows [a:b, :]')
+    if rows.step is not None:
+      self.refuse(where, 'a stepped slice')
+    out = []
+    for bound in (rows.lower, rows.upper):
+      value = None if bound is None else self.number(bound)
+      if bound is not None and not isinstance(value, int):
+        self.refuse(where, 'a slice bound that is not an int literal')
+      out.append(value)
+    return tuple(out)
+
+  def roll(self, node, where):
+    """(band, shift node, axis) of `np.roll(<curtain band>, shift, axis)`, else None."""
+    if not (isinstance(node, ast.Call) and self.callee(node.func) is np.roll):
+      return None
+    args = dict(zip(('a', 'shift', 'axis'), node.args))
+    for k in node.keywords:
+      if k.arg not in ('shift', 'axis') or k.arg in args:
+        self.refuse(where, 'these arguments of np.roll()')
+      args[k.arg] = k.value
+    if len(node.args) > 3 or 'shift' not in args:
+      self.refuse(where, 'these arguments of np.roll()')
+    axis = args.get('axis')
+    if not (isinstance(axis, ast.Constant) and type(axis.value) is int and axis.value in (0, 1)):
+      self.refuse(where, 'an np.roll axis that is not the literal 0 or 1')
+    src = args['a']
+    if self.is_self_curtain(src):
+      band = (None, None)
+    elif isinstance(src, ast.Subscript) and self.is_self_curtain(src.value):
+      band = self.band(src.slice, where)
+    else:
+      band = None
+    if band is None:
+      self.refuse(where, "np.roll of something other than a band of the Backdrop's curtain")
+    return band, args['shift'], axis.value
+
+  def backdrop_write(self, sl, value, st):
+    """`self.curtain[cell] = v`, `self.curtain[:] = v` or `self.curtain[band] =
+    np.roll(self.curtain[band], shift, axis)` in a Backdrop's update()."""
+    band = self.band(sl, st)
+    if band is None:
+      self.cell(sl, st)
+      self.byte(value)
+      self.emit('SETBACK')
+      return
+    rolled = self.roll(value, st)
+    if rolled is not None:
+      if rolled[0] != band:
+        self.refuse(st, 'np.roll of another band than the one it is assigned to')
+      self.scalar(rolled[1])
+      self.emit('ROLLBACK', rolled[2], ('lo',) + band, ('hi',) + band)
+      return
+    if band != (None, None):
+      self.refuse(st, 'a write to a band of rows other than np.roll of that band')
+    self.byte(value)
+    self.emit('FILLBACK')
+
+
 def _sliced(index):
   """Does a subscript index take a slice on some axis?"""
   return any(isinstance(x, ast.Slice) for x in
@@ -1104,13 +1283,15 @@ _RESERVED = {
 
 # ------------------------------------------------------------------ linking
 
-def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys, rng_streams=()):
+def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys, rng_streams=(),
+         backdrop=None):
   """Bytecode words for one game.  compiled: char -> `Compiled`; plot_keys: the key
-  order of the plot registers; rng_streams: the generator of each RNG slot.  Entities of
-  one class share their code."""
+  order of the plot registers; rng_streams: the generator of each RNG slot; backdrop: the
+  `Compiled` of the Backdrop, whose entry goes in header word 1 + n (pcl.h program_arg[4]).
+  Entities of one class share their code."""
   chars = list(sprite_chars) + list(drape_chars)
   S = len(sprite_chars)
-  words = [len(chars)] + [0] * len(chars)
+  words = [len(chars)] + [0] * (len(chars) + (backdrop is not None))
   entry = {}
   for i, ch in enumerate(chars):
     comp = compiled[ch]
@@ -1118,6 +1299,9 @@ def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys, rng_streams
       entry[comp.klass] = len(words)
       words += _encode(comp, len(words), chars, S, rows, cols, plot_keys, rng_streams)
     words[1 + i] = entry[comp.klass]
+  if backdrop is not None:
+    words[1 + len(chars)] = len(words)
+    words += _encode(backdrop, len(words), chars, S, rows, cols, plot_keys, rng_streams)
   if len(words) > _lib.MAX_CODE_WORDS:
     raise NotLoweredError('the compiled game needs {} code words, more than {}'.format(
         len(words), _lib.MAX_CODE_WORDS))
@@ -1147,6 +1331,11 @@ def _encode(comp, base, chars, S, rows, cols, plot_keys, rng_streams):
       return rows
     if x[0] == 'cols':
       return cols
+    if x[0] == 'palette':             # lowering checked it against the game's palette
+      return ord(x[1])
+    if x[0] in ('lo', 'hi'):          # a band of rows, clipped as a Python slice
+      lo, hi, _ = slice(x[1], x[2]).indices(rows)
+      return lo if x[0] == 'lo' else max(lo, hi)
     ch = x[1]                         # ('ent', ch)
     if ch not in chars:
       raise NotLoweredError('{}: things[{!r}] names no entity of the game'.format(

@@ -34,6 +34,7 @@ struct pcl_handle {
   int32_t* code_dev;
   int code_dev_words;            // words the device buffer holds room for
   int code_stale;                // code_host changed since the upload
+  uint8_t* backdrop_live;        // pcl_bind_backdrop, or NULL
 };
 
 namespace {
@@ -140,6 +141,12 @@ void fill_params(const pcl_handle* h, StepParams* p) {
   memcpy(p->group_chars, s.group_chars, sizeof(p->group_chars));
   p->st = h->st;
   p->code = h->code_dev;
+  p->backdrop_live = h->backdrop_live;
+}
+
+// Does the handle's Backdrop run compiled code on a live curtain (pcl_bind_backdrop)?
+bool live_backdrop(const pcl_spec& s) {
+  return s.program == PCL_PROG_COMPILED && s.program_arg[4] != 0;
 }
 
 int launch(pcl_handle* h, const StepParams& p, cudaStream_t stream) {
@@ -197,6 +204,7 @@ int check_ready(pcl_handle* h, const pcl_outputs* out, cudaStream_t s) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   if (h->program->check_code && !h->code_host) return PCL_ERR_UNBOUND;
+  if (live_backdrop(h->spec) && !h->backdrop_live) return PCL_ERR_UNBOUND;
   if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
   if (float_rewards(h) && !out->d_reward_f64) return PCL_ERR_INVALID;
   return h->program->check_code ? upload_code(h, s) : PCL_OK;
@@ -254,6 +262,7 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->code_dev = nullptr;
   h->code_dev_words = 0;
   h->code_stale = 0;
+  h->backdrop_live = nullptr;
   *out = h;
   return PCL_OK;
 }
@@ -306,6 +315,13 @@ int pcl_bind_code(pcl_handle* h, const int32_t* h_code, int32_t n_words) {
   h->code_host = copy;
   h->code_words = n_words;
   h->code_stale = 1;
+  return PCL_OK;
+}
+
+int pcl_bind_backdrop(pcl_handle* h, uint8_t* d_backdrop_live) {
+  if (!h || !d_backdrop_live || !live_backdrop(h->spec)) return PCL_ERR_INVALID;
+  h->backdrop_live = d_backdrop_live;
+  h->base.backdrop_live = d_backdrop_live;   // pcl_bind_state's fill_params copies it too
   return PCL_OK;
 }
 
@@ -524,7 +540,12 @@ pcl::LayersParams layers_params(const pcl_handle* h, int n_chars, uint8_t* d_out
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.H = sp.rows; p.W = sp.cols; p.pitch = sp.pitch;
   p.S = sp.n_sprites; p.D = sp.n_drapes; p.n_chars = n_chars;
-  p.backdrop = h->st.d_backdrop; p.backdrop_bstride = h->st.backdrop_bstride;
+  if (live_backdrop(sp)) {       // the Backdrop as its code left it, per env
+    p.backdrop = h->backdrop_live; p.backdrop_bstride = (int64_t)sp.rows * sp.pitch;
+    p.backdrop_per_env = 1;
+  } else {
+    p.backdrop = h->st.d_backdrop; p.backdrop_bstride = h->st.backdrop_bstride;
+  }
   p.level = h->st.d_level; p.sprites = h->st.d_sprites; p.drapes = h->st.d_drapes;
   p.out = d_out;
   return p;
@@ -548,6 +569,7 @@ int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_
   if (!h || !chars || !d_out || n_chars < 1 || n_chars > PCL_MAX_LAYER_CHARS)
     return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
+  if (live_backdrop(h->spec) && !h->backdrop_live) return PCL_ERR_UNBOUND;
   const pcl_spec& sp = h->spec;
   pcl::LayersParams p = layers_params(h, n_chars, d_out);
   for (int d = 0; d < sp.n_drapes; ++d) {

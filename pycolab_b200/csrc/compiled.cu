@@ -75,6 +75,10 @@ __host__ __device__ __forceinline__ int op_operands(int op) {
   }
 }
 
+// Operand words of every opcode, the Backdrop's included (host side: pcl_bind_code).  The
+// interpreter counts ROLLBACK's itself, so that compiled_step's dispatch stays as it was.
+int code_operands(int op) { return op == PCL_OP_ROLLBACK ? 3 : op_operands(op); }
+
 // Stack effect of each opcode (host side: pcl_bind_code's depth check).
 struct OpInfo { int8_t pops, pushes; };
 constexpr OpInfo kOps[PCL_OP_COUNT] = {
@@ -122,6 +126,9 @@ constexpr OpInfo kOps[PCL_OP_COUNT] = {
     {3, 0},  // SETPAT
     {0, 1},  // PATANY
     {1, 0},  // SETFIELD
+    {3, 0},  // SETBACK
+    {1, 0},  // FILLBACK
+    {1, 0},  // ROLLBACK
 };
 static_assert(sizeof(kOps) / sizeof(kOps[0]) == PCL_OP_COUNT, "one kOps entry per opcode");
 constexpr int kMaxIn = 64;            // values of an IN or a PICK
@@ -234,11 +241,61 @@ struct Rewards {
 // local memory.  Only one output in 624 pays for the call.
 __device__ __noinline__ void twist_out_of_line(uint32_t* mt, int lane) { mt_twist(mt, lane); }
 
-// The update() of entity `ent` (sprites first, then drapes).  kDraws: the code may draw
-// (program_arg[1] > 0); games without draws run a kernel without the generator.  kScroll:
+// Rotate the band of cells of rows lo .. hi - 1 of `bd` as np.roll(band, shift, axis) does:
+// along each row (axis 1) or across whole rows (axis 0), by three reversals (all of it, then
+// its first k and its last n - k cells, k = shift mod n), with the warp's lanes swapping
+// pairs and a __syncwarp between reversals.
+__device__ void roll_band(uint8_t* bd, int pitch, int W, int axis, int lo, int hi, int shift,
+                          int lane) {
+  const int n = axis ? W : hi - lo;          // cells along the axis
+  const int lines = axis ? hi - lo : W;      // rows (axis 1) or columns (axis 0) rolled
+  if (n <= 1 || lines <= 0) return;
+  const int k = (int)(((long long)shift % n + n) % n);
+  if (k == 0) return;
+  for (int s = 0; s < 3; ++s) {                // [0, n), then [0, k), then [k, n)
+    const int a = s == 2 ? k : 0, len = (s == 1 ? k : n) - a, half = len / 2;
+    for (int i = lane; i < half * lines; i += 32) {
+      const int line = i / half, j = i - line * half;
+      const int x = a + j, y = a + len - 1 - j;
+      uint8_t* u = axis ? bd + (int64_t)(lo + line) * pitch + x : bd + (int64_t)(lo + x) * pitch + line;
+      uint8_t* v = axis ? bd + (int64_t)(lo + line) * pitch + y : bd + (int64_t)(lo + y) * pitch + line;
+      const uint8_t t = *u;
+      *u = *v;
+      *v = t;
+    }
+    __syncwarp();
+  }
+}
+
+// PCL_OP_SETBACK (x, y, v = r, c, value), FILLBACK (x = value) and ROLLBACK (a = axis, lo, hi,
+// x = shift) on `bd`, the env's live curtain of H x W cells.  Only backdrop_step runs them.
+// False: SETBACK's cell is off the board (nothing written).
+__device__ __forceinline__ bool write_backdrop(uint8_t* bd, int H, int W, int pitch, int lane, int op,
+                                            int a, int lo, int hi, int x, int y, int v) {
+  __syncwarp();                              // every lane has read what it is about to change
+  if (op == PCL_OP_SETBACK) {
+    if (!(cell_index(x, H) && cell_index(y, W))) return false;
+    if (lane == 0) bd[(int64_t)x * pitch + y] = (uint8_t)v;
+  } else if (op == PCL_OP_FILLBACK) {
+    for (int i = lane; i < H * W; i += 32) {
+      const int r = i / W;
+      bd[(int64_t)r * pitch + (i - r * W)] = (uint8_t)x;
+    }
+  } else {
+    roll_band(bd, pitch, W, a, lo, hi, x, lane);
+  }
+  __syncwarp();
+  return true;
+}
+
+// The update() of entity `ent` (sprites first, then drapes; S + D is the Backdrop).  kDraws:
+// the code may draw (program_arg[1] > 0); games without draws run a kernel without the
+// generator.  kScroll:
 // the game scrolls (has Scrollys or egocentric walkers); the others run a kernel without
 // the Scrolly motion helper and egocentric moves, which cost ptxas 23 more registers.
-template <bool kDraws, bool kScroll>
+// kBackdrop: the game has a compiled Backdrop (program_arg[4]); only backdrop_step runs its
+// opcodes, so compiled_step keeps the registers it had without them.
+template <bool kDraws, bool kScroll, bool kBackdrop>
 __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot,
                            Directives& dir, Rewards& rw) {
   const StepParams& p = *c.p;
@@ -254,7 +311,8 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
   int32_t* regs = is_sprite ? &st->sprites[ent][plain ? PCL_S_VROW
                                                 : kScroll && p.egocentric[ent] ? PCL_S_AUX2
                                                                                : PCL_S_AUX0]
-                            : &st->drapes[ent - S][kScroll && p.drape_kind[ent - S] ? PCL_D_AUX0 : 0];
+                 : kBackdrop && ent == S + p.D ? nullptr             // the Backdrop has none
+                 : &st->drapes[ent - S][kScroll && p.drape_kind[ent - S] ? PCL_D_AUX0 : 0];
   const LaneSlots stk = {&vm->stack[0][lane]};
   const LaneSlots loc = {&vm->local[0][lane]};
   int sp = 0;
@@ -501,7 +559,19 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         stk[sp++] = __any_sync(PCL_FULL, any) ? 1 : 0;
         break;
       }
-      default: {                               // PCL_OP_PICK
+      default: {                               // PCL_OP_PICK, and the Backdrop's opcodes
+        // The Backdrop's opcodes take no case labels: with them, compiled_step's dispatch
+        // and register allocation would change.
+        if (kBackdrop && op >= PCL_OP_SETBACK) {
+          const bool set = op == PCL_OP_SETBACK, roll = op == PCL_OP_ROLLBACK;
+          sp -= set ? 3 : 1;
+          if (!write_backdrop(p.backdrop_live + (int64_t)c.env * H * p.pitch, H, W, p.pitch, lane, op,
+                              a, roll ? __ldg(code + pc + 2) : 0, roll ? __ldg(code + pc + 3) : 0,
+                              stk[sp], set ? stk[sp + 1] : 0, set ? stk[sp + 2] : 0))
+            plot.error |= PCL_ENV_ERR_INDEX;
+          if (roll) next += 3;                 // op_operands leaves ROLLBACK's out (code_operands)
+          break;
+        }
         const int i = stk[sp - 1];
         int v = 0;
         if ((unsigned)i < (unsigned)a) v = __ldg(code + pc + 2 + i);
@@ -515,9 +585,10 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
   }
 }
 
-template <bool kDraws, bool kScroll>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32)
-compiled_step(const StepParams p) {
+// One env's step.  kBackdrop: as run_update; compiled_step and backdrop_step are its two
+// kernels.
+template <bool kDraws, bool kScroll, bool kBackdrop>
+__device__ __forceinline__ void step(const StepParams& p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -531,7 +602,9 @@ compiled_step(const StepParams p) {
   Vm* vm = reinterpret_cast<Vm*>(my + sizeof(WarpState));
   Ctx c;
   c.p = &p; c.st = st; c.board = my + sizeof(WarpState) + sizeof(Vm);
-  c.backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
+  // A compiled Backdrop (program_arg[4]) writes its own live copy; the template is per level.
+  const uint8_t* backdrop_init = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
+  c.backdrop = kBackdrop ? p.backdrop_live + (int64_t)env * H * p.pitch : backdrop_init;
   c.env = env; c.lane = lane; c.lvl = lvl;
   c.kept = (uint32_t)p.program_arg[2];       // Scrollys that write their pattern
 
@@ -565,6 +638,11 @@ compiled_step(const StepParams p) {
       uint32_t* dst = p.st.d_bits[d] + (int64_t)env * p.st.bits_bstride[d];
       for (int i = lane; i < H * p.BW; i += 32) dst[i] = src[i];
     }
+    if (kBackdrop) {                         // the Backdrop's curtain, before the first render
+      const uint4* src = reinterpret_cast<const uint4*>(backdrop_init);
+      uint4* dst = reinterpret_cast<uint4*>(p.backdrop_live + (int64_t)env * H * p.pitch);
+      for (int i = lane; i < (H * p.pitch) >> 4; i += 32) dst[i] = src[i];
+    }
   }
   __syncwarp();
   if (restart) {
@@ -587,16 +665,37 @@ compiled_step(const StepParams p) {
 
   // ---- update groups (engine.py:725-735)
   int k = 0;
-  for (int g = 0; g < p.n_groups; ++g) {
-    for (int e = 0; e < p.group_len[g]; ++e, ++k) {
-      const int ch = p.group_chars[k];
-      int ent = 0;
-      for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
-      for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
-      run_update<kDraws, kScroll>(c, vm, ent, action, plot, dir, rw);
+  if (kBackdrop) {
+    // The Backdrop's update() first, as "group -1": on the board of the last render, with no
+    // render after it (engine.py:718-723).  One run_update call site serves it and the
+    // entities, which keeps backdrop_step free of a stack.
+    for (int g = -1; g < p.n_groups; ++g) {
+      for (int e = 0; e < (g < 0 ? 1 : p.group_len[g]); ++e) {
+        int ent = n;
+        if (g >= 0) {
+          const int ch = p.group_chars[k++];
+          ent = 0;
+          for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
+          for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
+        }
+        run_update<kDraws, kScroll, kBackdrop>(c, vm, ent, action, plot, dir, rw);
+      }
+      if (g < 0) continue;
+      board::render</*kWrap=*/true>(c);
+      if (p.program_arg[3] && plain_sprite_off_board(c)) plot.error |= PCL_ENV_ERR_INDEX;
     }
-    board::render</*kWrap=*/true>(c);
-    if (p.program_arg[3] && plain_sprite_off_board(c)) plot.error |= PCL_ENV_ERR_INDEX;
+  } else {
+    for (int g = 0; g < p.n_groups; ++g) {
+      for (int e = 0; e < p.group_len[g]; ++e, ++k) {
+        const int ch = p.group_chars[k];
+        int ent = 0;
+        for (int s = 0; s < S; ++s) if (p.sprite_char[s] == ch) ent = s;
+        for (int d = 0; d < D; ++d) if (p.drape_char[d] == ch) ent = S + d;
+        run_update<kDraws, kScroll, kBackdrop>(c, vm, ent, action, plot, dir, rw);
+      }
+      board::render</*kWrap=*/true>(c);
+      if (p.program_arg[3] && plain_sprite_off_board(c)) plot.error |= PCL_ENV_ERR_INDEX;
+    }
   }
 
   __syncwarp();
@@ -613,6 +712,17 @@ compiled_step(const StepParams p) {
   }
   __syncwarp();
   board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
+}
+
+template <bool kDraws, bool kScroll>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32) compiled_step(const StepParams p) {
+  step<kDraws, kScroll, false>(p);
+}
+
+// Games whose Backdrop has compiled update() code (program_arg[4]).
+template <bool kDraws, bool kScroll>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32) backdrop_step(const StepParams p) {
+  step<kDraws, kScroll, true>(p);
 }
 
 // MazeWalkers, plain Sprites, Scrollys and plain drapes in one scrolling group; the entities and the
@@ -650,6 +760,7 @@ int check_spec(const pcl_spec& s) {
   const uint32_t plain = (uint32_t)s.program_arg[3];
   for (int i = 0; i < 32; ++i)
     if (((plain >> i) & 1) && (i >= s.n_sprites || s.sprite_egocentric[i])) return PCL_ERR_INVALID;
+  if (s.program_arg[4] != 0 && s.program_arg[4] != 1) return PCL_ERR_INVALID;   // a compiled Backdrop
   if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
   return PCL_OK;
 }
@@ -675,10 +786,13 @@ CurtainAt curtain(const pcl_spec& s, int d) {
 // The checks pcl_bind_code promises (include/pcl.h): after them the kernel can run any
 // entity's code without a bounds test.
 int check_code(const pcl_spec& s, const int32_t* w, int n) {
-  const int S = s.n_sprites, ents = s.n_sprites + s.n_drapes, body = 1 + ents;
+  // With a compiled Backdrop, header word 1 + ents is its function's entry.
+  const bool has_backdrop = s.program_arg[4] != 0;
+  const int S = s.n_sprites, ents = s.n_sprites + s.n_drapes, body = 1 + ents + has_backdrop;
   if (n <= body || n > PCL_MAX_CODE_WORDS || w[0] != ents) return PCL_ERR_INVALID;
-  // A walker and a plain Sprite are different kinds: their functions take different opcodes.
-  enum { kNone = 0, kSprite = 1, kDrape = 2, kPlainSprite = 3 };
+  // A walker, a plain Sprite and the Backdrop are different kinds: their functions take
+  // different opcodes.
+  enum { kNone = 0, kSprite = 1, kDrape = 2, kPlainSprite = 3, kBackdrop = 4 };
   const uint32_t plain_sprites = (uint32_t)s.program_arg[3];
   auto is_plain_sprite = [&](int k) { return k >= 0 && k < S && ((plain_sprites >> k) & 1); };
   // What the entities sharing a function allow it: their kind, the fewest registers any of
@@ -704,6 +818,11 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
     f.plain = f.plain && !scrolly && kind == kDrape;
     f.writes = f.writes && writes;
   }
+  if (has_backdrop) {                          // no registers, and a function of its own
+    const int e = w[1 + ents];
+    if (e < body || e >= n || starts[e].kind != kNone) return PCL_ERR_INVALID;
+    starts[e] = Fn{kBackdrop, 0, false, false, false};
+  }
   if (starts[body].kind == kNone) return PCL_ERR_INVALID;
   // An entity operand naming a Scrolly, or -1 in a function of Scrollys.
   auto is_scrolly = [&](int a, const Fn& f) {
@@ -724,11 +843,11 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
     boundary[pc] = 1;
     const int op = w[pc];
     if (op < 0 || op >= PCL_OP_COUNT) return PCL_ERR_INVALID;
-    int len = 1 + op_operands(op);
+    int len = 1 + code_operands(op);
     if (pc + len > end) return PCL_ERR_INVALID;
     const int a = len > 1 ? w[pc + 1] : 0;
     const bool walker = kind == kSprite, plain_sprite = kind == kPlainSprite;
-    const bool sprite = walker || plain_sprite;
+    const bool sprite = walker || plain_sprite, backdrop = kind == kBackdrop;
     switch (op) {
       case PCL_OP_LOAD: case PCL_OP_STORE:
         if (a < 0 || a >= PCL_CODE_LOCALS) return PCL_ERR_INVALID;
@@ -770,7 +889,14 @@ int check_code(const pcl_spec& s, const int32_t* w, int n) {
         if (a < 0 || a >= 4) return PCL_ERR_INVALID;
         break;
       case PCL_OP_CURTAIN: case PCL_OP_ANY:
-        if (a < 0 ? sprite : (a < S || a >= ents)) return PCL_ERR_INVALID;
+        if (a < 0 ? sprite || backdrop : (a < S || a >= ents)) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_SETBACK: case PCL_OP_FILLBACK:
+        if (!backdrop) return PCL_ERR_INVALID;
+        break;
+      case PCL_OP_ROLLBACK:
+        if (!backdrop || (a != 0 && a != 1)) return PCL_ERR_INVALID;
+        if (w[pc + 2] < 0 || w[pc + 2] > w[pc + 3] || w[pc + 3] > s.rows) return PCL_ERR_INVALID;
         break;
       case PCL_OP_SETCELL: case PCL_OP_FILL:
         if (!fn.plain) return PCL_ERR_INVALID;   // a Scrolly's curtain is its pattern's window
@@ -827,11 +953,19 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
   bool scrolls = false;
   for (int d = 0; d < p.D; ++d) scrolls = scrolls || p.drape_kind[d];
   for (int i = 0; i < p.S; ++i) scrolls = scrolls || p.egocentric[i];
+  const bool draws = p.program_arg[1] > 0;
+  if (p.program_arg[4]) {
+    if (scrolls)
+      return draws ? launch_step(backdrop_step<true, true>, p, kWarpsPerBlock, smem, s)
+                   : launch_step(backdrop_step<false, true>, p, kWarpsPerBlock, smem, s);
+    return draws ? launch_step(backdrop_step<true, false>, p, kWarpsPerBlock, smem, s)
+                 : launch_step(backdrop_step<false, false>, p, kWarpsPerBlock, smem, s);
+  }
   if (scrolls)
-    return p.program_arg[1] > 0 ? launch_step(compiled_step<true, true>, p, kWarpsPerBlock, smem, s)
-                                : launch_step(compiled_step<false, true>, p, kWarpsPerBlock, smem, s);
-  return p.program_arg[1] > 0 ? launch_step(compiled_step<true, false>, p, kWarpsPerBlock, smem, s)
-                              : launch_step(compiled_step<false, false>, p, kWarpsPerBlock, smem, s);
+    return draws ? launch_step(compiled_step<true, true>, p, kWarpsPerBlock, smem, s)
+                 : launch_step(compiled_step<false, true>, p, kWarpsPerBlock, smem, s);
+  return draws ? launch_step(compiled_step<true, false>, p, kWarpsPerBlock, smem, s)
+               : launch_step(compiled_step<false, false>, p, kWarpsPerBlock, smem, s);
 }
 
 }  // namespace

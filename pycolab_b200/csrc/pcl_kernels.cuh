@@ -51,6 +51,7 @@ struct StepParams {
   int has_cropper;               // pcl_attach_cropper: crop the new board as the kernel's epilogue
   CropParams cropper;            // (board is taken from `out` at launch time)
   const int32_t* code;           // device copy of the bytecode bound with pcl_bind_code, or NULL
+  uint8_t* backdrop_live;        // pcl_bind_backdrop: u8 [B, H, pitch] live curtains, or NULL
 };
 
 // Launch with the programmatic-stream-serialisation attribute (the kernel calls
@@ -174,6 +175,7 @@ struct LayersParams {
   const int32_t* sprites;
   const int32_t* drapes;
   uint8_t* out;                            // u8 [B, n_chars, H, pitch]
+  int backdrop_per_env;                    // 1: `backdrop` is indexed by env, not level (live)
 };
 cudaError_t launch_layers(const LayersParams& p, cudaStream_t s);
 

@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(256) layers_kernel(const LayersParams p) {
   const int segs_per_row = p.pitch >> 4;
   const int plane_segs = p.H * segs_per_row;
   const int64_t lvl = p.level ? p.level[env] : env;
-  const uint8_t* backdrop = p.backdrop + lvl * p.backdrop_bstride;
+  const uint8_t* backdrop = p.backdrop + (p.backdrop_per_env ? env : lvl) * p.backdrop_bstride;
   uint8_t* out = p.out + (int64_t)env * p.n_chars * p.H * p.pitch;
   for (int i = threadIdx.x; i < p.n_chars * plane_segs; i += blockDim.x) {
     const int k = i / plane_segs, seg = i - k * plane_segs;

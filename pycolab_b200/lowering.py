@@ -226,7 +226,8 @@ class LoweredGame(object):
     self.program_arg = [0] * 8  # pcl_spec.program_arg
     self.reward_type = int      # the reference's reward type (classics pay floats)
     self.float_reward = False   # rewards are not integers: pcl_outputs.d_reward_f64
-    self.backdrop_role = None   # device counterpart of a Backdrop with update() logic
+    self.backdrop_role = None   # device counterpart of a Backdrop with update() logic: 'river'
+                                # (classics) or 'compiled.backdrop' (registered code)
     self.scroll_groups = ['']   # names of the scrolling groups, index = device group id
     self.sprite_group = []      # per sprite: index into scroll_groups
     self.drape_group = []       # per drape
@@ -339,7 +340,10 @@ def _common(engine, game, program, never_reads_layers=False):
                  for _, entities in sorted(engine._update_groups.items())]
   backdrop = engine.backdrop
   game.backdrop_role = None
-  if type(backdrop).update is not things.Backdrop.update:
+  from pycolab_b200 import compiler
+  if compiler.registered(type(backdrop)) is not None:
+    game.backdrop_role = 'compiled.backdrop'    # its code runs on the compiled program only
+  elif type(backdrop).update is not things.Backdrop.update:
     for klass in type(backdrop).__mro__:
       key = (klass.__module__.rsplit('.', 1)[-1], klass.__name__)
       if (key in LOWERED_BACKDROPS and type(backdrop).update is klass.update and
@@ -397,6 +401,8 @@ def lower(engine):
   if family not in programs.BY_FAMILY:
     raise NotLoweredError(family)
   game = programs.BY_FAMILY[family].lower(engine, roles)
-  if game.backdrop_role is not None and family != 'classics':
+  if game.backdrop_role == 'compiled.backdrop' and family != 'compiled':
+    raise NotLoweredError('a registered Backdrop is lowered only with registered entities')
+  if game.backdrop_role not in (None, 'compiled.backdrop') and family != 'classics':
     raise NotLoweredError('a Backdrop with update() logic is lowered only with its own game')
   return game

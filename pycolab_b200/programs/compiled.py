@@ -1,6 +1,6 @@
-"""The compiled program `csrc/compiled.cu`: MazeWalkers, plain Sprites, Scrollys and plain
-drapes of classes registered with `pycolab_b200.compiler`, whose update() bodies run as
-device bytecode."""
+"""The compiled program `csrc/compiled.cu`: MazeWalkers, plain Sprites, Scrollys, plain
+drapes and a Backdrop of classes registered with `pycolab_b200.compiler`, whose update()
+bodies run as device bytecode."""
 
 import numpy as np
 
@@ -49,6 +49,17 @@ def lower(engine, roles):
   if len(sprite_chars) > _lib.MAX_SPRITES or len(drape_chars) > _lib.MAX_DRAPES:
     raise NotLoweredError('too many entities for the compiled device program')
   comp = {ch: compiler.registered(type(th[ch])) for ch in order}
+  # A registered Backdrop: its code runs first and writes a per-env live curtain.
+  backdrop = (compiler.registered(type(engine.backdrop))
+              if game.backdrop_role == 'compiled.backdrop' else None)
+  compiled = [backdrop] * (backdrop is not None) + [comp[ch] for ch in order]
+  if backdrop is not None:
+    game.program_arg[4] = 1
+    for ins in backdrop.ir:
+      for x in ins[1:]:
+        if isinstance(x, tuple) and x[0] == 'palette' and x[1] not in engine.backdrop.palette:
+          raise NotLoweredError('{}: self.palette names {!r}, which is not a legal character of '
+                                "the game's palette".format(compiler._name(backdrop.klass), x[1]))
   for ch in drape_chars:
     if type(th[ch]).curtain is not things.Drape.curtain:
       raise NotLoweredError('drape {!r} overrides `curtain`'.format(ch))
@@ -77,8 +88,8 @@ def lower(engine, roles):
 
   # the_plot keys: plot registers AUX0.. in order of first use
   keys = []
-  for ch in order:
-    for key in comp[ch].keys:
+  for c in compiled:
+    for key in c.keys:
       if key not in keys:
         keys.append(key)
   if len(keys) > compiler.MAX_PLOT_KEYS:
@@ -173,16 +184,16 @@ def lower(engine, roles):
   game.dynamic_z = True                  # the kernel renders from the per-env z-order
   # RNG slots: the generators the code draws from, in order of first use
   streams = []
-  for ch in order:
-    for stream in comp[ch].streams:
+  for c in compiled:
+    for stream in c.streams:
       if stream not in streams:
         streams.append(stream)
   game.rng_streams = tuple(streams)
   game.rng_from_globals = True
   game.program_arg[1] = len(streams)
   game.code = compiler.link(comp, sprite_chars, drape_chars, engine.rows, engine.cols, keys,
-                            game.rng_streams)
-  game.float_reward = any(c.float_reward for c in comp.values())
+                            game.rng_streams, backdrop)
+  game.float_reward = any(c.float_reward for c in compiled)
   game.reward_type = float if game.float_reward else int
   game.program_arg[0] = 1 if game.float_reward else 0
   game.registers = registers
@@ -220,3 +231,5 @@ def sync(engine):
   for k, (key, is_bool) in enumerate(game.plot_keys):
     word = plot[_lib.P_AUX0 + k]
     engine.the_plot[key] = bool(word) if is_bool else int(word)
+  if b.backdrop_live is not None:          # the Backdrop's curtain as its code left it
+    np.copyto(engine.backdrop.curtain, b.backdrop_live[0, :, :b.cols].cpu().numpy())
