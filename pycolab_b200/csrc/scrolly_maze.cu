@@ -58,8 +58,18 @@
 // Sprite order P,a,b,c (indices 0..3); drape order '#','@' (0, 1).
 // Registers: patroller aux0 = moving_east; P aux0/aux1 = scroll permit mask /
 // permit frame; '@' aux0/aux1 = board cell of a coin already removed from the
-// pattern but still on the (not yet refreshed) curtain, or -1; plot aux0 =
-// coins left in the pattern.
+// pattern but still on the (not yet refreshed) curtain, or -1; '@' aux2 = dirty-group
+// mask of the env's coin pattern (below); plot aux0 = coins left in the pattern.
+//
+// Coin groups: every env owns a complete copy of its level's coin pattern
+// (d_pattern[1]), and it differs from the level's template (d_pattern_init[1], shared
+// by all envs of the level and so served from L2) only in the rows of coins picked up
+// this episode.  Bit k of '@' aux2 set means rows [k g, (k + 1) g) of the env's pattern
+// may differ from the template; bit k clear means they are equal.  The step reads a
+// clean group's rows from the template instead of the env's copy (the coin window and
+// the coin patch rows), a pick-up sets its group's bit, and an auto-reset restart
+// copies back only the dirty groups (the reloaded record brings the mask back to 0).
+// A host that writes an env's coin pattern directly sets that env's aux2 to -1.
 #include "pcl_device.cuh"
 #include "pcl_kernels.cuh"
 #include "pcl_crop.cuh"
@@ -89,6 +99,12 @@ __device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
 // from the even word at or below corner_c >> 5 always cover it (<= 31 + 32 + 64
 // bits), and pattern rows are 8-byte aligned (pattern_words is even), so a row is
 // staged with two 8-byte cp.async into a 16-byte smem slot.
+
+// Pattern rows per bit of the coin dirty-group mask: g = 2^s rows, s the smallest shift
+// with 32 g >= PH, so that 32 bits cover every pattern row (g = 8 at 129 rows).
+__device__ __forceinline__ int coin_group_shift(int PH) {
+  return 32 - __clz((PH - 1) >> 5);
+}
 
 // prmt.b32 without __byte_perm's selector masking (the table holds nibbles 0..5).
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
@@ -266,6 +282,16 @@ __device__ __forceinline__ void scrolly_move_p(Drape& d, const ScrollyCfg& cfg, 
   plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
 }
 
+// The env's own coin pattern, and its level's template.  Both are recomputed from the
+// launch parameters where they are used: at 64 registers, no pointer to either stays live
+// through the step.
+__device__ __forceinline__ uint32_t* env_coins(const StepParams& p, int env) {
+  return p.st.d_pattern[1] + (int64_t)env * p.st.pattern_bstride[1];
+}
+__device__ __forceinline__ const uint32_t* level_coins(const StepParams& p, int64_t lvl) {
+  return p.st.d_pattern_init[1] + lvl * p.st.pattern_init_bstride[1];
+}
+
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
 scrolly_maze_step(const StepParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -309,7 +335,6 @@ scrolly_maze_step(const StepParams p) {
   const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
 
   const uint32_t* wall_pat = p.st.d_pattern[0] + lvl * p.st.pattern_bstride[0];
-  uint32_t* coin_pat = p.st.d_pattern[1] + (int64_t)env * p.st.pattern_bstride[1];
 
   // The env's action word does not depend on the records either: issue its load now,
   // beside theirs, instead of one memory round trip later (it is only USED if the env
@@ -339,16 +364,25 @@ scrolly_maze_step(const StepParams p) {
   }
   if (restart) {
     const PlotCarry carry = plot_carry(rec + 48, true);
+    // Groups of the coin pattern to restore, read before the record is reloaded: the
+    // dirty ones at an auto-reset, every one at the host's reset (which so repairs any
+    // pattern).
+    const unsigned dirty = p.mode == MODE_RESET ? ~0u
+                                                : (unsigned)rec[32 + PCL_DRAPE_WORDS + PCL_D_AUX2];
     __syncwarp();
     const int32_t* si = p.st.d_sprites_init + lvl * p.st.sprites_init_bstride;
     const int32_t* di = p.st.d_drapes_init + lvl * p.st.drapes_init_bstride;
     const int32_t* pi = p.st.d_plot_init + lvl * p.st.plot_init_bstride;
     rec[lane] = __ldg(si + lane);
     rec[32 + lane] = lane < 16 ? __ldg(di + lane) : __ldg(pi + lane - 16);
-    // Fresh coins: restore the mutable pattern (one Engine per episode).
-    const uint32_t* src = p.st.d_pattern_init[1] + lvl * p.st.pattern_init_bstride[1];
-    const int n = p.PH * PWW;
-    for (int i = lane; i < n; i += 32) coin_pat[i] = __ldg(src + i);
+    // Fresh coins: restore the mutable pattern (one Engine per episode); the reloaded
+    // record's mask is 0.
+    const uint32_t* src = level_coins(p, lvl);
+    const int n = p.PH * PWW, gw = PWW << coin_group_shift(p.PH);   // words per group
+    for (unsigned m = dirty; m != 0u; m &= m - 1u) {
+      const int lo = (__ffs(m) - 1) * gw, hi = min(lo + gw, n);
+      for (int i = lo + lane; i < hi; i += 32) env_coins(p, env)[i] = __ldg(src + i);
+    }
     __syncwarp();
     if (lane == 0) store_carry(rec + 48, carry);
     __syncwarp();
@@ -427,13 +461,16 @@ scrolly_maze_step(const StepParams p) {
       const int pr = wr + rec[w * PCL_SPRITE_WORDS + PCL_S_VROW] + k - 2;
       c_first = wc + rec[w * PCL_SPRITE_WORDS + PCL_S_VCOL] - 2;
       if ((unsigned)pr < (unsigned)p.PH) { row = wall_pat + (int64_t)pr * PWW; limit = PWW; }
-    } else if (lane < 23) {
-      const int r = p_vrow + (lane - 20) - 1;
-      c_first = c_pre_c + p_vcol - 1;
-      if ((unsigned)r < (unsigned)H) { row = coin_pat + (int64_t)(c_pre_r + r) * PWW; limit = PWW; }
-    } else if (lane == 23) {
-      c_first = c_pre_c;
-      row = coin_pat + (int64_t)c_pre_r * PWW; limit = PWW;
+    } else if (lane < 24) {
+      // A clean group's row comes from the level's template (see "Coin groups").
+      const int r = lane < 23 ? p_vrow + (lane - 20) - 1 : 0;
+      c_first = lane < 23 ? c_pre_c + p_vcol - 1 : c_pre_c;
+      if ((unsigned)r < (unsigned)H) {
+        const int pr = c_pre_r + r;
+        row = ((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> coin_group_shift(p.PH))) & 1u
+                  ? env_coins(p, env) : level_coins(p, lvl);
+        row += (int64_t)pr * PWW; limit = PWW;
+      }
     }
     if (row != nullptr) {
       const int wi = c_first >> 5;           // floor, may be -1
@@ -470,19 +507,25 @@ scrolly_maze_step(const StepParams p) {
 #pragma unroll 4
     for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
   }
-  if (narrow) {
-    const int nhalf = H * 2;                 // two 8-byte halves per window row
+  // Coin window rows of clean groups come from the level's template (see "Coin groups"):
+  // per env that is L2 traffic shared by the level's envs instead of DRAM of its own.
+  {
+    const uint32_t* coin_tpl = level_coins(p, lvl);
+    const int gs = coin_group_shift(p.PH);
+    const int hw = nw >> 1, nhalf = H * hw;  // 8-byte halves per window row
     for (int i = lane; i < nhalf; i += 32) {
-      const int r = i >> 1, k = (i & 1) * 2;
+      const int r = narrow ? i >> 1 : i / hw, k = (i - r * hw) * 2, pr = cr_pred + r;
       cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
-      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
+      if (!(((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u))
+        cp_async8(s_coin + i * 2, coin_tpl + (int64_t)pr * PWW + ce + k);
     }
-  } else {                                   // boards wider than 64 columns
-    const int hw = nw >> 1, nhalf = H * hw;
-    for (int i = lane; i < nhalf; i += 32) {
-      const int r = i / hw, k = (i - r * hw) * 2;
-      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
-      cp_async8(s_coin + i * 2, coin_pat + (int64_t)(cr_pred + r) * PWW + ce + k);
+    if (rec_coins[PCL_D_AUX2] != 0) {
+#pragma unroll 1
+      for (int i = lane; i < nhalf; i += 32) {
+        const int r = narrow ? i >> 1 : i / hw, k = (i - r * hw) * 2, pr = cr_pred + r;
+        if (((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u)
+          cp_async8(s_coin + i * 2, env_coins(p, env) + (int64_t)pr * PWW + ce + k);
+      }
     }
   }
 
@@ -582,10 +625,10 @@ scrolly_maze_step(const StepParams p) {
     else if ((unsigned)(dr + 1) <= 2u && (unsigned)(dc + 1) <= 2u)
       coin = (coin9 >> ((dr + 1) * 3 + dc + 1)) & 1u;
     else
-      coin = bit_at(coin_pat + (int64_t)pr * PWW, pc);   // cannot happen
+      coin = bit_at(env_coins(p, env) + (int64_t)pr * PWW, pc);   // cannot happen
     if (coin) {
       add_reward(dir, 100);
-      if (lane == 0) coin_pat[(int64_t)pr * PWW + (pc >> 5)] &= ~(1u << (pc & 31));
+      if (lane == 0) env_coins(p, env)[(int64_t)pr * PWW + (pc >> 5)] &= ~(1u << (pc & 31));
       picked_r = pr; picked_c = pc;
       plot.aux0 -= 1;
       if (plot.aux0 == 0) terminate(dir);
@@ -621,8 +664,10 @@ scrolly_maze_step(const StepParams p) {
     r[PCL_P_ORDER_FRAME] = plot.order_frame; r[PCL_P_EGO_MASK] = plot.ego_mask;
     r[PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
-    // The coin window was staged before the pick-up: clear the bit there too.
+    // The coin window was staged before the pick-up: clear the bit there too.  The
+    // pick-up's group of the env's pattern now differs from the template.
     if (picked_r >= 0) {
+      rec[32 + PCL_DRAPE_WORDS + PCL_D_AUX2] |= 1 << (picked_r >> coin_group_shift(p.PH));
       const int r2 = picked_r - cr_pred, b = picked_c - (ce << 5);
       if ((unsigned)r2 < (unsigned)H && (unsigned)b < (unsigned)(nw * 32))
         s_coin[r2 * nw + (b >> 5)] &= ~(1u << (b & 31));
@@ -634,7 +679,7 @@ scrolly_maze_step(const StepParams p) {
     __syncwarp();
     ce_final = (cc >> 5) & ~1;
     for (int i = lane; i < H * nw; i += 32)
-      s_coin[i] = coin_pat[(int64_t)(cr + i / nw) * PWW + ce_final + i % nw];
+      s_coin[i] = env_coins(p, env)[(int64_t)(cr + i / nw) * PWW + ce_final + i % nw];
   }
   __syncwarp();
   p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane] = rec[lane];
