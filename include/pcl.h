@@ -546,13 +546,18 @@ int pcl_crop_tracking(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d
  *   ObservationCharacterRepainter: depth 1, u8 table = the character mapping;
  *   ObservationToArray:            the value mapping (scalars or depth-vectors);
  *   ObservationToFeatureArray:     f32 one-hot, table[ch][d] = (ch == layers[d]).
- * d_table is [128, depth] of `dtype`; d_valid u8 [128] marks characters the
- * mapping knows (NULL = all); a board holding an unknown character sets
- * *d_unknown (i32, may be NULL) to 1 (upstream RuntimeError, rendering.py:520-526).
+ * d_table is [128, depth] of `dtype`, 1 <= depth <= 32 (callers split deeper
+ * outputs into launches of <= 32 planes); d_valid u8 [128] marks characters the
+ * mapping knows (NULL = all).  A cell holding a byte >= 128 gets zero elements.
+ * An in-board cell whose byte is >= 128 or not valid sets *d_unknown (i32, may be
+ * NULL) to 1 (upstream RuntimeError, rendering.py:520-526); pad columns are not
+ * read.  Only the element size matters, the bits are copied: any 1-, 2-, 4- or
+ * 8-byte type (bool, int8, float16, uint32, ...) fits the code of its size.
  * Output strides are in ELEMENTS, so any `permute` is just a stride choice. */
 typedef struct pcl_observe_spec {
   int32_t depth;
-  int32_t dtype;              /* 0 uint8, 1 int32, 2 float32, 3 int64, 4 float64 */
+  int32_t dtype;              /* 0 uint8, 1 int32, 2 float32, 3 int64, 4 float64,
+                                 5 any 2-byte type (int16, uint16, float16) */
   int64_t stride_b, stride_d, stride_r, stride_c;
 } pcl_observe_spec;
 int pcl_observe(pcl_handle* h, const pcl_observe_spec* spec, const void* d_table,

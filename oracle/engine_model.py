@@ -570,7 +570,8 @@ class ScrollingCrop(object):
 # --------------------------------------------------------------------------
 
 def observation_to_array(board, value_mapping, dtype=None, permute=None):
-  """rendering.py:409-542."""
+  """rendering.py:409-542: any dtype; a value is stored by masked assignment, one
+  vector component at a time, as upstream stores it."""
   first = next(iter(value_mapping.values()))
   dtype = dtype if dtype is not None else np.array(first).dtype
   try:
@@ -581,22 +582,37 @@ def observation_to_array(board, value_mapping, dtype=None, permute=None):
   for code in np.unique(board):
     if chr(code) not in value_mapping:
       raise RuntimeError('character %r outside the value mapping' % chr(code))
-    out[:, board == code] = np.reshape(value_mapping[chr(code)], (depth, 1))
+    mask = board == code
+    if is_3d:
+      for layer, component in enumerate(value_mapping[chr(code)]):
+        out[layer, mask] = component
+    else:
+      out[:, mask] = value_mapping[chr(code)]
   result = out if is_3d else out[0]
   return result if permute is None else np.transpose(result, permute)
 
 
 def observation_repaint(board, character_mapping):
-  """rendering.py:304-406 (board part)."""
+  """rendering.py:304-406 (board part): upstream repaints through an
+  ObservationToArray of the 128 ASCII codes, so a byte >= 128 raises."""
+  if board.size and int(board.max()) > 127:
+    raise RuntimeError('byte %d outside the ASCII repaint mapping' % int(board.max()))
   lut = np.arange(256, dtype=np.uint8)
   for src, dst in character_mapping.items():
     lut[ord(src)] = ord(dst)
   return lut[board]
 
 
-def observation_to_feature_array(board, layers, permute=None):
-  """rendering.py:545-661 with occluded layers (board == ord(c))."""
-  out = np.stack([(board == ord(c)).astype(np.float32) for c in layers])
+def observation_to_feature_array(board, layers, permute=None, observation_layers=None):
+  """rendering.py:545-661.  `observation_layers` is the observation's layer dict,
+  copied as upstream copies it (a zero plane where a character is missing); None
+  means occluded layers of every character, `board == ord(c)`."""
+  if observation_layers is None:
+    observation_layers = {c: board == ord(c) for c in layers}
+  out = np.zeros((len(layers),) + board.shape, dtype=np.float32)
+  for index, character in enumerate(layers):
+    if character in observation_layers:
+      np.copyto(out[index], observation_layers[character])
   return out if permute is None else np.transpose(out, permute)
 
 

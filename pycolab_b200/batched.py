@@ -514,12 +514,24 @@ class BatchedEngine(object):
   # --- observation post-processors (rendering.py:304-661) over the whole batch
   def to_feature_array(self, layers, permute=None):
     """ObservationToFeatureArray: float32 one-hot planes, [B, C, rows, cols] (or
-    the last three axes permuted)."""
+    the last three axes permuted).  A character the game lacks gives a zero plane.
+    A game made with occlusion_in_layers=False copies its un-occluded layers
+    (`unoccluded_layers`), as upstream copies `observation.layers`."""
     from pycolab_b200 import observers
+    torch = _torch()
     permute = observers.check_permute(permute, True, 'ObservationToFeatureArray')
-    return observers.observe(self._lib, self._h, self._board, self.rows, self.cols,
-                             observers.feature_table(layers), None, True, permute,
-                             self._stream())
+    if self.game.occlusion_in_layers:
+      out = observers.observe(self._lib, self._h, self._board, self.rows, self.cols,
+                              observers.feature_table(layers, present=self.chars), None,
+                              True, permute, self._stream())
+      return out.view(torch.float32)
+    known = [k for k, ch in enumerate(layers) if ch in self.chars]
+    out = torch.zeros((self.batch, len(layers), self.rows, self.cols), dtype=torch.float32,
+                      device=self.device)
+    if known:
+      planes = self.unoccluded_layers(''.join(layers[k] for k in known))
+      out[:, known] = planes.float()
+    return out if permute is None else out.permute([0] + [1 + i for i in permute])
 
   def to_array(self, value_mapping, dtype=None, permute=None):
     """ObservationToArray: map characters to scalars ([B, rows, cols]) or vectors
@@ -536,7 +548,7 @@ class BatchedEngine(object):
           'This ObservationToArray only knows array values for the characters {}, but it '
           'received an observation with a character not in that set'.format(
               ''.join(value_mapping.keys())))
-    return out
+    return out.view(observers.torch_dtype(table.dtype))
 
   def repaint(self, character_mapping):
     """ObservationCharacterRepainter over every board: u8 [B, rows, cols]."""

@@ -744,13 +744,13 @@ int pcl_observe(pcl_handle* h, const pcl_observe_spec* spec, const void* d_table
                 int32_t* d_unknown, void* stream) {
   Range nvtx_range("pcl_observe");
   if (!h || !spec || !d_table || !d_board || !d_out) return PCL_ERR_INVALID;
-  if (spec->depth < 1 || spec->depth > 32 || spec->dtype < 0 || spec->dtype > 4)
+  if (spec->depth < 1 || spec->depth > 32 || spec->dtype < 0 || spec->dtype > 5)
     return PCL_ERR_INVALID;
   pcl::ObserveParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
   p.depth = spec->depth; p.dtype = spec->dtype;
-  p.words = spec->dtype >= 3 ? 2 : 1;
+  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
   p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
   p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
   p.table = d_table; p.valid = d_valid; p.board = d_board; p.out = d_out;

@@ -10,6 +10,10 @@
 // thread converts 4 consecutive cells (one aligned 32-bit board word) and writes
 // depth values per cell through caller-chosen strides, so `permute` costs
 // nothing.  HBM-bound: reads 1 byte, writes depth * sizeof(T) bytes per cell.
+// The kernel only copies bits: an element of 1, 2, 4 or 8 bytes is 1, 2, 1 or 2
+// words of T (uint8 for 1 and 2 bytes, uint32 for 4 and 8).  A byte >= 128 lies
+// outside every mapping (upstream's are keyed by ASCII characters): its cell gets
+// zero elements and the launch flags it as unknown.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -49,12 +53,14 @@ observe_kernel(const ObserveParams p) {
     for (int k = 0; k < 4; ++k) {
       const int c = wcol * 4 + k;
       if (c >= p.W) break;
-      const int ch = (cells >> (8 * k)) & 0x7f;
-      unknown |= !valid[ch] || ((cells >> (8 * k)) & 0x80);
+      const uint32_t byte = (cells >> (8 * k)) & 0xff;
+      const bool ascii = byte < 128;
+      unknown |= !ascii || !valid[byte & 0x7f];
       T* dst = out + b * p.stride_b + (int64_t)r * p.stride_r + (int64_t)c * p.stride_c;
-      const T* src = table + ch * row_words;
+      const T* src = table + (byte & 0x7f) * row_words;
       for (int d = 0; d < p.depth; ++d)
-        for (int w = 0; w < p.words; ++w) dst[d * p.stride_d + w] = src[d * p.words + w];
+        for (int w = 0; w < p.words; ++w)
+          dst[d * p.stride_d + w] = ascii ? src[d * p.words + w] : T(0);
     }
   }
   if (unknown && p.unknown) *p.unknown = 1;
@@ -67,10 +73,10 @@ cudaError_t launch_observe(const ObserveParams& p, cudaStream_t s) {
   int blocks = (int)((total + kThreads - 1) / kThreads);
   if (blocks > 132 * 16) blocks = 132 * 16;       // grid-stride over 16 CTAs per SM (H100: 132 SMs)
   if (blocks < 1) blocks = 1;
-  const size_t elem = p.dtype == 0 ? 1 : 4;
-  const size_t smem = 128 * (size_t)p.depth * p.words * elem;
-  if (p.dtype == 0) observe_kernel<uint8_t><<<blocks, kThreads, smem, s>>>(p);
-  else observe_kernel<uint32_t><<<blocks, kThreads, smem, s>>>(p);   // int32 / float32 bits
+  const bool bytes = p.dtype == 0 || p.dtype == 5;   // 1- and 2-byte elements
+  const size_t smem = 128 * (size_t)p.depth * p.words * (bytes ? 1 : 4);
+  if (bytes) observe_kernel<uint8_t><<<blocks, kThreads, smem, s>>>(p);
+  else observe_kernel<uint32_t><<<blocks, kThreads, smem, s>>>(p);   // 4- / 8-byte bits
   return cudaGetLastError();
 }
 

@@ -181,8 +181,8 @@ cudaError_t launch_layers(const LayersParams& p, cudaStream_t s);
 
 struct ObserveParams {
   int B, H, W, pitch, depth, dtype;
-  int words;                     // 32-bit words per element (2 for int64 / float64)
-  int64_t stride_b, stride_d, stride_r, stride_c;   // in 32-bit words (bytes for uint8)
+  int words;                     // words per element: 2 for 8- and 2-byte elements
+  int64_t stride_b, stride_d, stride_r, stride_c;   // in words (u32, or bytes for dtype 0 / 5)
   const void* table;             // [128, depth]
   const uint8_t* valid;          // u8 [128] or NULL
   const uint8_t* board;          // u8 [B, H, pitch]

@@ -235,6 +235,7 @@ class LoweredGame(object):
     # Host hooks of the program module (pycolab_b200/programs), None where it needs none:
     self.curtain = None         # (BatchedEngine, d) -> u8 [B, rows, pitch] curtain of drape d,
                                 # or None where the device exports it (pcl_export_curtain)
+    self.occlusion_in_layers = True   # False: layers are un-occluded (rendering.py:187-301)
     self.layers = None          # (BatchedEngine, chars) -> bool [B, len(chars), rows, cols]
     self.sync = None            # (Engine): mirror program-private device state into the
                                 # Python objects after a step
@@ -362,6 +363,7 @@ def _common(engine, game, program, never_reads_layers=False):
   if not engine._occlusion_in_layers and not never_reads_layers:
     raise NotLoweredError('occlusion_in_layers=False is lowered only for games whose '
                           'entities never consult `layers`')
+  game.occlusion_in_layers = engine._occlusion_in_layers
 
 
 def _set_sprites(game, sprites, records, named_groups=False):

@@ -14,38 +14,58 @@ import numpy as np
 
 from pycolab_b200 import _lib
 
-_DTYPES = {np.dtype(np.uint8): 0, np.dtype(np.int32): 1, np.dtype(np.float32): 2,
-           np.dtype(np.int64): 3, np.dtype(np.float64): 4}
+# pcl_observe copies bits, so only an element's size picks the launch: the code of
+# each size (include/pcl.h pcl_observe_spec.dtype), and the container it is moved in.
+_CODE_OF_SIZE = {1: 0, 2: 5, 4: 1, 8: 3}
+_CONTAINER = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}
+MAX_PLANES = 32                  # planes one pcl_observe launch writes
+
+
+def check_dtype(dtype):
+  """`dtype` as a NumPy dtype if the device can produce it: bool, integers and
+  floats of 1, 2, 4 or 8 bytes."""
+  dt = np.dtype(dtype)
+  if dt.kind not in 'biuf' or dt.itemsize not in _CODE_OF_SIZE:
+    raise TypeError('ObservationToArray on the device supports bool, integer and float '
+                    'outputs of 1, 2, 4 or 8 bytes, not {}'.format(dt))
+  return dt
 
 
 def value_table(value_mapping, dtype=None):
   """ObservationToArray's mapping (rendering.py:423-470) as (table [128, depth],
-  valid u8 [128], is_3d)."""
+  valid u8 [128], is_3d).  Values are stored exactly as upstream stores them into
+  its output array: masked assignment, one vector component at a time."""
   first = next(iter(value_mapping.values()))
-  dt = np.dtype(dtype) if dtype is not None else np.array(first).dtype
+  dt = check_dtype(dtype if dtype is not None else np.array(first).dtype)
   try:
     depth, is_3d = len(first), True
   except TypeError:
     depth, is_3d = 1, False
-  if dt not in _DTYPES:
-    raise TypeError('ObservationToArray on the device supports uint8, int32, int64, '
-                    'float32 and float64 outputs, not {}'.format(dt))
-  table = np.zeros((128, depth), dtype=dt)
+  planes = np.zeros((depth, 128), dtype=dt)
   valid = np.zeros((128,), dtype=np.uint8)
   for ch, value in value_mapping.items():
     code = ord(ch)
     if code > 127:
       raise ValueError('non-ASCII character {!r} in a value mapping'.format(ch))
-    table[code] = value
+    mask = np.arange(128) == code
+    if is_3d:
+      for layer, component in enumerate(value):
+        planes[layer, mask] = component
+    else:
+      planes[:, mask] = value
     valid[code] = 1
-  return table, valid, is_3d
+  return np.ascontiguousarray(planes.T), valid, is_3d
 
 
-def feature_table(layers):
-  """ObservationToFeatureArray (rendering.py:545-661): one-hot float32 planes."""
+def feature_table(layers, present=None):
+  """ObservationToFeatureArray (rendering.py:545-661) over occluded layers
+  (`board == ord(c)`): one-hot float32 planes.  A character outside `present` (the
+  observation's layers; None = every character) or beyond ASCII gets a zero plane,
+  as upstream fills layers the observation lacks with zeros."""
   table = np.zeros((128, len(layers)), dtype=np.float32)
   for d, ch in enumerate(layers):
-    table[ord(ch), d] = 1.0
+    if ord(ch) < 128 and (present is None or ch in present):
+      table[ord(ch), d] = 1.0
   return table
 
 
@@ -70,30 +90,53 @@ def check_permute(permute, is_3d, who):
   return permute
 
 
+def plane_chunks(depth):
+  """[(first plane, planes)]: the pcl_observe launches of a `depth`-plane output."""
+  return [(k0, min(MAX_PLANES, depth - k0)) for k0 in range(0, depth, MAX_PLANES)]
+
+
 def observe(lib, handle, board, rows, cols, table, valid, is_3d, permute, stream,
             unknown=None):
   """Run pcl_observe over `board` (u8 [B, rows, pitch] CUDA tensor).  Returns a
-  CUDA tensor shaped [B] + permuted([depth,] rows, cols)."""
+  CUDA tensor shaped [B] + permuted([depth,] rows, cols), in the same-size
+  unsigned container of `table.dtype` (`torch_dtype` / `numpy_view` convert it).
+  More than MAX_PLANES planes take one launch per MAX_PLANES."""
   import torch
   B = board.shape[0]
   depth = table.shape[1]
+  size = table.dtype.itemsize
   base = [depth, rows, cols] if is_3d else [rows, cols]
   perm = list(permute) if permute is not None else list(range(len(base)))
   shape = [base[i] for i in perm]
-  torch_dtype = {0: torch.uint8, 1: torch.int32, 2: torch.float32, 3: torch.int64,
-                 4: torch.float64}[_DTYPES[table.dtype]]
-  out = torch.empty([B] + shape, dtype=torch_dtype, device=board.device)
+  container = getattr(torch, np.dtype(_CONTAINER[size]).name)
+  out = torch.empty([B] + shape, dtype=container, device=board.device)
   strides = list(out.stride())[1:]
   at = {base_dim: strides[perm.index(base_dim)] for base_dim in range(len(base))}
-  spec = _lib.ObserveSpec(depth, _DTYPES[table.dtype], out.stride()[0],
-                          at[0] if is_3d else 0,
-                          at[1] if is_3d else at[0], at[2] if is_3d else at[1])
-  t_table = torch.from_numpy(np.ascontiguousarray(table).view(
-      np.uint8 if table.dtype == np.uint8 else np.int32)).to(board.device)
+  t_table = torch.from_numpy(np.ascontiguousarray(table).view(_CONTAINER[size])).to(
+      board.device)
   t_valid = None if valid is None else torch.from_numpy(valid).to(board.device)
-  _lib.check(lib.pcl_observe(handle, C.byref(spec), t_table.data_ptr(),
-                             None if t_valid is None else t_valid.data_ptr(),
-                             board.data_ptr(), out.data_ptr(),
-                             None if unknown is None else unknown.data_ptr(), stream),
-             'pcl_observe')
+  for k0, planes in plane_chunks(depth):
+    spec = _lib.ObserveSpec(planes, _CODE_OF_SIZE[size], out.stride()[0],
+                            at[0] if is_3d else 0,
+                            at[1] if is_3d else at[0], at[2] if is_3d else at[1])
+    chunk = t_table[:, k0:k0 + planes].contiguous()
+    d_out = out.data_ptr() + (k0 * at[0] * size if is_3d else 0)
+    _lib.check(lib.pcl_observe(handle, C.byref(spec), chunk.data_ptr(),
+                               None if t_valid is None else t_valid.data_ptr(),
+                               board.data_ptr(), d_out,
+                               None if unknown is None else unknown.data_ptr(), stream),
+               'pcl_observe')
   return out
+
+
+def torch_dtype(dtype):
+  """The torch dtype of NumPy `dtype` (same size, same meaning)."""
+  import torch
+  dt = np.dtype(dtype)
+  return torch.bool if dt == np.bool_ else getattr(torch, dt.name)
+
+
+def numpy_view(out, dtype):
+  """Host copy of an `observe` result as a NumPy array of `dtype`."""
+  host = out.cpu().numpy()
+  return host.view(dtype)

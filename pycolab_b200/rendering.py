@@ -32,6 +32,11 @@ class LazyLayers(collections.abc.Mapping):
     self._chars = frozenset(chars)
     self._cache = {}
 
+  @property
+  def board(self):
+    """The board these layers are derived from."""
+    return self._board
+
   def __getitem__(self, char):
     if char not in self._chars:
       raise KeyError(char)
@@ -69,7 +74,13 @@ class BaseObservationRenderer(object):
 
   def paint_sprite(self, character, position):
     self._check(character)
-    self._painted.append(('sprite', character, (int(position[0]), int(position[1]))))
+    row, col = int(position[0]), int(position[1])
+    # `self._board[tuple(position)]` upstream: NumPy wraps a negative index once
+    # and raises beyond that.
+    if not (-self._rows <= row < self._rows and -self._cols <= col < self._cols):
+      raise IndexError('sprite position {} is off the {}x{} board'.format(
+          (row, col), self._rows, self._cols))
+    self._painted.append(('sprite', character, (row, col)))
 
   def paint_drape(self, character, curtain):
     self._check(character)
@@ -119,7 +130,8 @@ class _BoardOnDevice(object):
     out = observers.observe(lib, self._handles[key], t_board, rows, cols, table, valid,
                             is_3d, permute, stream, unknown)
     torch.cuda.synchronize(dev)
-    return out[0].cpu().numpy(), (bool(int(unknown[0])) if want_unknown else False)
+    return (observers.numpy_view(out[0], table.dtype),
+            bool(int(unknown[0])) if want_unknown else False)
 
 
 _on_device = _BoardOnDevice()
@@ -163,7 +175,14 @@ class ObservationCharacterRepainter(object):
     self._table = observers.repaint_table(character_mapping)
 
   def __call__(self, original_observation):
-    board, _ = _on_device(original_observation.board, self._table, None, False, None)
+    # Upstream repaints through an ObservationToArray of the 128 ASCII codes, so a
+    # byte >= 128 raises there.
+    board, unknown = _on_device(original_observation.board, self._table, None, False, None,
+                                want_unknown=True)
+    if unknown:
+      raise RuntimeError(
+          'This ObservationCharacterRepainter only repaints ASCII characters, but it '
+          'received an observation with a byte outside that set')
     chars = (set(original_observation.layers) - set(self._character_mapping)).union(
         self._character_mapping.values())
     return Observation(board=board, layers=LazyLayers(board, chars))
@@ -175,7 +194,6 @@ class ObservationToFeatureArray(object):
   def __init__(self, layers, permute=None):
     from pycolab_b200 import observers
     self._layers = layers
-    self._table = observers.feature_table(layers)
     self._permute = observers.check_permute(permute, True, 'ObservationToFeatureArray')
 
   def __call__(self, observation):
@@ -184,8 +202,21 @@ class ObservationToFeatureArray(object):
           'The layers argument to this ObservationToFeatureArray, {!r}, has no entry that '
           'refers to an actual feature in the input observation. Actual features in the '
           'observation are {!r}.'.format(self._layers, ''.join(sorted(observation.layers))))
-    out, _ = _on_device(observation.board, self._table, None, True, self._permute)
-    return out
+    from pycolab_b200 import observers
+    layers = observation.layers
+    if (isinstance(layers, LazyLayers) and layers.board is observation.board and
+        all(ord(c) < 128 for c in self._layers if c in layers)):
+      # Occluded layers are `board == ord(c)`: one look-up per cell on the device.
+      table = observers.feature_table(self._layers, present=layers)
+      out, _ = _on_device(observation.board, table, None, True, self._permute)
+      return out
+    # Any other layers (un-occluded ones, or a user's dict) are copied as upstream
+    # does, with zeros for layers the observation lacks.
+    out = np.zeros((len(self._layers),) + observation.board.shape, dtype=np.float32)
+    for index, character in enumerate(self._layers):
+      if character in layers:
+        np.copyto(out[index], layers[character])
+    return out if self._permute is None else np.transpose(out, self._permute)
 
 
 class BaseUnoccludedObservationRenderer(BaseObservationRenderer):
@@ -209,13 +240,51 @@ class BaseUnoccludedObservationRenderer(BaseObservationRenderer):
     return Observation(board=board, layers=layers)
 
 
+def _launches(painted):
+  """Split `painted` into runs, in order, that fit one pcl_render launch each."""
+  from pycolab_b200 import _lib
+  runs, sprites, drapes = [[]], 0, 0
+  for item in painted:
+    s, d = item[0] == 'sprite', item[0] == 'drape'
+    if sprites + s > _lib.MAX_SPRITES or drapes + d > _lib.MAX_DRAPES:
+      runs.append([])
+      sprites = drapes = 0
+    runs[-1].append(item)
+    sprites, drapes = sprites + s, drapes + d
+  return runs
+
+
 def render_on_device(backdrop, painted, device=0):
-  """One `pcl_render` launch for a single canvas; returns uint8 [rows, cols].
+  """`pcl_render` launches for a single canvas; returns uint8 [rows, cols].
 
   painted: [(kind, char, data)] in z-order, kind 'sprite' (data = (row, col)) or
   'drape' (data = bool mask).  A character painted several times occupies
-  several z slots upstream; here each paint call gets its own slot too.
+  several z slots upstream; here each paint call gets its own slot too.  More
+  paint calls than one launch holds are rendered in successive launches, each
+  painting over the board the previous one made.
   """
+  rows, cols = backdrop.shape
+  # Each paint call gets a private slot code so repeated characters keep their
+  # own z rank; the real character is restored after the launch.  The codes are
+  # bytes that neither the backdrop nor any painted character uses, so the
+  # restore touches painted cells only.
+  used = set(np.unique(backdrop).tolist()) | set(ord(ch) for _, ch, _ in painted)
+  free = [v for v in list(range(128, 256)) + list(range(128)) if v not in used]
+  runs = _launches(painted)
+  need = max(len(run) for run in runs)
+  if need > len(free):
+    raise ValueError('{} paint calls in one launch need {} free byte values for their '
+                     'z slots; the backdrop and the painted characters leave {}'.format(
+                         need, need, len(free)))
+  board = np.array(backdrop, dtype=np.uint8)
+  for run in runs:
+    board = _render_once(board, run, free[:len(run)], device)
+  return board
+
+
+def _render_once(backdrop, painted, slots, device):
+  """One `pcl_render` launch painting `painted` over `backdrop` with z slot codes
+  `slots` (one per paint call)."""
   import torch
   from pycolab_b200 import _lib
   lib = _lib.load()
@@ -223,18 +292,13 @@ def render_on_device(backdrop, painted, device=0):
   pitch = (cols + 15) // 16 * 16
   sprites = [(c, d) for k, c, d in painted if k == 'sprite']
   drapes = [(c, d) for k, c, d in painted if k == 'drape']
-  if len(sprites) > _lib.MAX_SPRITES or len(drapes) > _lib.MAX_DRAPES:
-    raise ValueError('too many paint calls for one pcl_render launch')
-  # Each paint call gets a private slot code so repeated characters keep their
-  # own z rank; the real character is restored after the launch.
   spec = _lib.Spec()
   spec.abi_version, spec.program = _lib.ABI_VERSION, _lib.PROG_NONE
   spec.rows, spec.cols, spec.pitch = rows, cols, pitch
   spec.n_sprites, spec.n_drapes = len(sprites), len(drapes)
-  z_order, slot = [], 128
   sprite_i = drape_i = 0
-  real = {}
-  for kind, ch, _ in painted:
+  real = np.arange(256, dtype=np.uint8)
+  for (kind, ch, _), slot in zip(painted, slots):
     real[slot] = ord(ch)
     if kind == 'sprite':
       spec.sprite_char[sprite_i] = slot
@@ -242,8 +306,6 @@ def render_on_device(backdrop, painted, device=0):
     else:
       spec.drape_char[drape_i] = slot
       drape_i += 1
-    z_order.append(slot)
-    slot += 1
   dev = torch.device('cuda', device)
   handle = C.c_void_p()
   _lib.check(lib.pcl_create(C.byref(spec), 1, device, C.byref(handle)), 'pcl_create')
@@ -259,16 +321,14 @@ def render_on_device(backdrop, painted, device=0):
     t_bd = torch.from_numpy(bd).to(dev)
     t_cur = torch.from_numpy(cur).to(dev)
     t_rec = torch.from_numpy(rec).to(dev)
-    t_z = torch.tensor([z_order or [0]], dtype=torch.uint8, device=dev)
+    t_z = torch.tensor([list(slots) or [0]], dtype=torch.uint8, device=dev)
     t_out = torch.zeros((1, rows, pitch), dtype=torch.uint8, device=dev)
     stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(lib.pcl_render(handle, t_bd.data_ptr(), 0, t_cur.data_ptr(),
                               t_rec.data_ptr(), t_z.data_ptr(), t_out.data_ptr(), stream),
                'pcl_render')
     torch.cuda.synchronize(dev)
-    board = t_out[0, :, :cols].cpu().numpy().copy()
+    board = t_out[0, :, :cols].cpu().numpy()
   finally:
     lib.pcl_destroy(handle)
-  for code, ch in real.items():
-    board[board == code] = ch
-  return board
+  return real[board]
