@@ -126,6 +126,21 @@ typedef enum pcl_program {
                                 group 0 and writes a per-env live curtain, bound with pcl_bind_backdrop;
                                 d_backdrop is then its per-level reset template (0: the backdrop is
                                 static and d_backdrop is read directly) */
+  PCL_PROG_BOX_WORLD = 15,   /* examples/research/box_world/box_world.py:127-271: sprite '.' (MazeWalker,
+                                impassable '#', confined), NO drapes.  Every key 'a'-'t', lock 'A'-'T' and
+                                the gem '*' is a cell of a per-env object grid held in d_bits[0] viewed as
+                                u8 [rows, pitch] (bits_words = pitch / 4): 0 = no object, else the
+                                character, bit 7 set on a distractor lock cell; d_bits_init[0] is the
+                                level's reset template.  A held key sits at (0, 0).  rows <= 32 and
+                                pitch <= 32 (grid_size <= 30).  program_arg[0] = max_num_steps.  Sprite
+                                AUX0 = _step_counter; plot AUX0 = the character of the_plot['over_this']
+                                (0 = unset), AUX1 = its position (row << 16 | col).  Rewards are int32
+                                (the reference's floats 0, +1, -1, +10).  Levels have a '#' ring; without
+                                it a look-up at row or column -1 wraps as NumPy's does, one past the last
+                                row or column latches PCL_ENV_ERR_INDEX (NumPy's IndexError) and skips the
+                                rest of the step's logic, and the walker never leaves the board.  pcl_layers and
+                                pcl_export_curtain see the backdrop and the player only: object planes
+                                are d_bits[0] == character */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */

@@ -80,7 +80,10 @@ class BatchedEngine(object):
     self.auto_reset = bool(auto_reset)
     self.rows, self.cols, self.pitch = g0.rows, g0.cols, g0.pitch
     self.sprite_chars, self.drape_chars = g0.sprite_chars, g0.drape_chars
-    self.chars = ''.join(sorted(set(g0.sprite_chars + g0.drape_chars + g0.backdrop_chars)))
+    # object chars (LoweredGame.object_chars) may differ between the levels of one handle
+    self.object_chars = ''.join(sorted(set(''.join(g.object_chars for g in games))))
+    self.chars = ''.join(sorted(set(g0.sprite_chars + g0.drape_chars + g0.backdrop_chars +
+                                    self.object_chars)))
     n = len(games)
     shared = (n == 1)
     dev = self.device
@@ -350,11 +353,15 @@ class BatchedEngine(object):
 
   # ------------------------------------------------------------- accessors
   def curtain(self, char):
-    """Drape.curtain of every env as bool [B, rows, cols] (things.py:213-217)."""
-    return self._curtain_bytes(self.drape_chars.index(char))[:, :, :self.cols].bool()
+    """Drape.curtain of every env as bool [B, rows, cols] (things.py:213-217), for the
+    spec's drapes and the program's object characters alike."""
+    d = (self.drape_chars + self.object_chars).index(char)
+    return self._curtain_bytes(d)[:, :, :self.cols].bool()
 
   def _curtain_bytes(self, d):
-    """Curtain of drape `d` as u8 [B, rows, pitch] (the pcl_export_curtain layout)."""
+    """Curtain of drape `d` as u8 [B, rows, pitch] (the pcl_export_curtain layout); d >=
+    len(drape_chars) names object_chars[d - len(drape_chars)], which only the program's
+    curtain hook serves."""
     if self.game.curtain is not None:
       out = self.game.curtain(self, d)
       if out is not None:

@@ -86,6 +86,7 @@ const struct {
     {PCL_PROG_SHOCKWAVE, &pcl::kShockwave},
     {PCL_PROG_T_MAZE, &pcl::kTMaze},
     {PCL_PROG_COMPILED, &pcl::kCompiled},
+    {PCL_PROG_BOX_WORLD, &pcl::kBoxWorld},
 };
 
 // The descriptor of program `id`, or nullptr for an id this build does not know.

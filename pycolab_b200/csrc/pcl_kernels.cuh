@@ -105,7 +105,7 @@ struct Program {
   bool float_reward_arg0;        // rewards are float64 when spec.program_arg[0] != 0
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
-    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled;
+    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld;
 
 // Host-side helpers of the programs' check_spec.
 inline bool chars_are(const uint8_t* got, int n, const char* want) {

@@ -259,3 +259,92 @@ def t_maze_level(seed=0, shape=(77, 191)):
   cue[first:, :block] = ord('Q')
   cue[first:, 11 - block:] = ord('Q')
   return _to_art(art), _to_art(cue)
+
+
+BOX_WORLD_KEYS = 'abcdefghijklmnopqrst'      # research/box_world: 20 colours, key 'a' opens 'A'
+BOX_WORLD_LOCKS = BOX_WORLD_KEYS.upper()
+
+
+def _box_world_problem(rand, solution_lengths, num_forward, num_backward, branch_length):
+  """The box graph: solution length and (lock, key) id pairs.  Id 0 is "no lock" (the
+  boxes on the floor), id -1 the gem; ids 1 .. n name colours of the shuffled palette.
+  Rows past the solution length are distractor branches."""
+  n = rand.choice(solution_lengths)
+  forward = rand.choice(num_forward)
+  backward = rand.choice(num_backward)
+  pairs = [(i, i + 1) for i in range(n)] + [(n, -1)]
+  for _ in range(forward):
+    lock = rand.choice(range(1, n + 1))
+    for _ in range(branch_length):
+      key = None
+      while key is None or key == lock:
+        key = rand.choice(range(n + 1, len(BOX_WORLD_KEYS)))
+      pairs.append((lock, key))
+      lock = key
+  for _ in range(backward):              # backward branches ignore branch_length
+    key = rand.choice(range(1, n + 1))
+    lock = rand.choice(range(n + 1, len(BOX_WORLD_KEYS)))
+    pairs.append((lock, key))
+  return n, pairs
+
+
+def _box_world_attempt(rand, grid_size, solution_lengths, num_forward, num_backward,
+                       branch_length, max_tries=200):
+  """One generation attempt, or None when it ran out of placement tries."""
+  n, pairs = _box_world_problem(rand, solution_lengths, num_forward, num_backward,
+                                branch_length)
+  palette = list(range(len(BOX_WORLD_KEYS)))
+  rand.shuffle(palette)
+  size = grid_size + 2
+  art = np.full((size, size), ord(' '), dtype=np.uint8)
+  art[0, :] = art[-1, :] = art[:, 0] = art[:, -1] = ord('#')
+  distractors = []
+  tries = 0
+
+  def room_for_box(x, y):               # the box and its lock, with a free ring around both
+    return (art[y - 1:y + 2, x - 1:x + 3] == ord(' ')).all()
+
+  for i, (lock, key) in enumerate(pairs):
+    while True:
+      if tries > max_tries:
+        return None
+      x = rand.randint(0, grid_size - 3) + 1
+      y = rand.randint(1, grid_size - 1) + 1
+      if room_for_box(x, y):
+        break
+      tries += 1
+    art[y, x] = ord('*') if key == -1 else ord(BOX_WORLD_KEYS[palette[key - 1]])
+    if lock != 0:
+      art[y, x + 1] = ord(BOX_WORLD_LOCKS[palette[lock - 1]])
+      if i > n:
+        distractors.append((x + 1, y))
+  while True:
+    if tries > max_tries:
+      return None
+    x = rand.randint(0, grid_size - 1) + 1
+    y = rand.randint(1, grid_size - 1) + 1
+    if art[y, x] == ord(' '):
+      break
+    tries += 1
+  art[y, x] = ord('.')
+  return _to_art(art), distractors
+
+
+def box_world_level(seed, grid_size=12, solution_length=(1, 2, 3, 4),
+                    num_forward=(0, 1, 2, 3, 4), num_backward=(0,), branch_length=1):
+  """A research/box_world level: (art, distractors).
+
+  `seed` is an int or a `np.random.RandomState`, which the generator continues.  It makes
+  the draws of research/box_world/box_world.py's `make_game` in the same order — the
+  problem's `choice`s, the `shuffle` of the 20 key / lock colours, the `randint`
+  placements and both retry loops — so RandomState(s) gives the level that upstream
+  builds from RandomState(s).  The art is (grid_size + 2)² with a '#' wall, the player
+  '.', keys 'a'-'t', locks 'A'-'T' right of the box they close, and the gem '*';
+  `distractors` lists the (column, row) of every lock that ends the episode."""
+  rand = seed if isinstance(seed, np.random.RandomState) else np.random.RandomState(seed)
+  for _ in range(200):
+    level = _box_world_attempt(rand, grid_size, solution_length, num_forward, num_backward,
+                               branch_length)
+    if level is not None:
+      return level
+  raise RuntimeError('Could not generate game in MAX_GENERATION_TRIES tries.')

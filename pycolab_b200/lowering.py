@@ -65,6 +65,11 @@ LOWERED_CLASSES = {
     ('t_maze', 'SpeckleDrape'): 't_maze.speckle',
     ('t_maze', 'TeleporterDrape'): 't_maze.teleporter',
     ('t_maze', 'GoalDrape'): 't_maze.goal',
+    ('box_world', 'PlayerSprite'): 'box_world.player',
+    ('box_world', 'BoxThing'): 'box_world.thing',
+    ('box_world', 'GemDrape'): 'box_world.gem',
+    ('box_world', 'KeyDrape'): 'box_world.key',
+    ('box_world', 'LockDrape'): 'box_world.lock',
     ('ordeal', 'PlayerSprite'): 'ordeal.player',
     ('ordeal', 'DragonduckSprite'): 'ordeal.dragonduck',
     ('ordeal', 'SwordDrape'): 'ordeal.sword',
@@ -197,6 +202,9 @@ class LoweredGame(object):
     self.rows = self.cols = self.pitch = 0
     self.sprite_chars = ''
     self.drape_chars = ''
+    self.object_chars = ''      # characters of Drapes the program keeps as cells of one object
+                                # grid instead of spec drapes (box_world); the curtain and
+                                # layers hooks serve them
     self.impassable = []
     self.confined = []
     self.egocentric = []

@@ -24,7 +24,7 @@ def main():
   from pycolab_b200 import batched, dist as pdist, levels, lowering
   from pycolab_b200.games import (aperture, better_scrolly_maze, extraterrestrial_marauders,
                                   apprehend, fixtures, fluvial_natation, hello_world, ordeal,
-                                  shockwave, t_maze,
+                                  box_world, shockwave, t_maze,
                                   scrolly_maze, warehouse_manager)
   from pycolab_b200.games.classics import chain_walk, cliff_walk, four_rooms
   rs = np.random.RandomState(0)
@@ -108,6 +108,13 @@ def main():
   run('shockwave_step 9x33', [shockwave.make_game(levels.shockwave_level(3, 9, 33))], 6, 5, steps=40)
   run('t_maze_step (device RNG)', [t_maze.make_game(1, False, 20, 2, 3, *levels.t_maze_level(s))
                                    for s in range(2)], 6, 7, steps=45)
+  run('box_world_step', [box_world.make_game(g, (1, 2, 3, 4), (0, 1, 2, 3, 4), (0,), 1,
+                                              random_state=np.random.RandomState(s),
+                                              max_num_steps=15)
+                          for g, s in ((12, 0), (12, 1), (12, 2))], 7, 6, steps=40)
+  run('box_world_step 32x32', [box_world.make_game(30, (1, 2, 3, 4), (0, 1, 2, 3, 4), (0,), 1,
+                                                   random_state=np.random.RandomState(4),
+                                                   max_num_steps=10)], 5, 6, steps=25)
   pattern = rs.random_sample((17, 23)) < 0.2
   fx = fixtures.make_game(['           ', '   P       ', '      q    ', '           ',
                            '           ', '           '], ' ',
