@@ -476,7 +476,10 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
  * With `crop` non-NULL the step is followed by pcl_crop(crop, d_crop, d_crop_state)
  * and h_view receives the crops u8 [B, crop rows, crop cols] instead of the
  * boards u8 [B, rows, pitch] — only the view the agent consumes crosses PCIe
- * (cropping.py:393-426 applied before the hand-off). */
+ * (cropping.py:393-426 applied before the hand-off).  The crop spec is checked before
+ * anything is enqueued: a spec pcl_crop refuses, and a tracking list that names a drape
+ * (the curtains are not passed here: use pcl_crop_tracking), return their status
+ * (PCL_ERR_UNSUPPORTED for the drape) with no env stepped. */
 #define PCL_HOST_SLOTS 8
 struct pcl_crop_spec;
 int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
@@ -518,8 +521,11 @@ int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_
  * re-initialises itself when the env's episode counter moves on, as
  * ScrollingCropper.set_engine does for a new Engine (cropping.py:375-391).
  * d_crop_state == NULL selects a single built-in cropper slot in the plot record.
- * sprite_index < 0 is a FixedCropper at (offset_rows, offset_cols). */
+ * sprite_index < 0 is a FixedCropper at (offset_rows, offset_cols).
+ * Windows of more than PCL_MAX_CROP_CELLS cells are PCL_ERR_UNSUPPORTED at every cropper
+ * entry point (the kernels divide a cell index by the width with a 16-bit-exact reciprocal). */
 #define PCL_MAX_TRACK 4
+#define PCL_MAX_CROP_CELLS 65535
 typedef struct pcl_crop_spec {
   int32_t rows, cols;          /* window shape */
   int32_t sprite_index;        /* entity to track (a sprite) */

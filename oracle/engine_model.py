@@ -469,11 +469,13 @@ class World(object):
 
 
 # --------------------------------------------------------------------------
-# ScrollingCropper (cropping.py:229-598), board only (layers follow from it).
+# ScrollingCropper (cropping.py:229-598), board and (optionally) a layer dict.
 # --------------------------------------------------------------------------
 
 class ScrollingCrop(object):
-  """cropping.py:313-598 restated for a single tracked-entity list."""
+  """cropping.py:313-598 restated for a single tracked-entity list.  The engine is any
+  object with `rows`, `cols` and `things`: {char: entity with `is_sprite` and either
+  `row`, `col`, `visible` (a sprite) or a bool `curtain` (a drape)}."""
 
   def __init__(self, rows, cols, to_track, pad_char=None,
                scroll_margins=(2, 3), initial_offset=None, saccade=True):
@@ -552,7 +554,8 @@ class ScrollingCrop(object):
     if self.pad is None:
       self._rectify()
 
-  def crop(self, board):            # cropping.py:393-426 + 118-227
+  def crop(self, board, layers=None):   # cropping.py:393-426 + 118-227
+    """The cropped board; with `layers`, (board, layers) as `crop_window` returns."""
     centroid = self._centroid()
     if self.corner is None:
       self._initialise(centroid, (self.rows // 2 + self.offset[0],
@@ -562,7 +565,7 @@ class ScrollingCrop(object):
         self._pan_to(centroid)
       elif self.saccade:
         self._initialise(centroid, (self.rows // 2, self.cols // 2))
-    return crop_window(board, self.corner, self.rows, self.cols, self.pad)
+    return crop_window(board, self.corner, self.rows, self.cols, self.pad, layers)
 
 
 # --------------------------------------------------------------------------
@@ -616,8 +619,9 @@ def observation_to_feature_array(board, layers, permute=None, observation_layers
   return out if permute is None else np.transpose(out, permute)
 
 
-def crop_window(board, corner, rows, cols, pad_char):
-  """cropping.py:118-227 `_do_crop`, board part."""
+def crop_window(board, corner, rows, cols, pad_char, layers=None):
+  """cropping.py:118-227 `_do_crop`.  With `layers` ({char: bool [H, W]}) returns
+  (board, layers): each layer cut at the same window, its pad cells `pad_char == char`."""
   top, left = corner
   H, W = board.shape
   if pad_char is None:
@@ -632,4 +636,10 @@ def crop_window(board, corner, rows, cols, pad_char):
   tr1 = min(rows, max(0, H - top))
   tc1 = min(cols, max(0, W - left))
   out[tr0:tr1, tc0:tc1] = board[fr0:fr1, fc0:fc1]
-  return out
+  if layers is None:
+    return out
+  cut = {}
+  for char, layer in layers.items():
+    cut[char] = np.full((rows, cols), pad_char == char, dtype=bool)
+    cut[char][tr0:tr1, tc0:tc1] = layer[fr0:fr1, fc0:fc1]
+  return out, cut

@@ -15,6 +15,7 @@ ABI_VERSION = 3
 MAX_SPRITES = 16
 MAX_DRAPES = 8
 MAX_TRACK = 4                # entities one ScrollingCropper can follow (pcl_crop_spec.track)
+MAX_CROP_CELLS = 65535       # largest crop window (rows * cols) the cropper entry points serve
 SPRITE_WORDS = 8
 DRAPE_WORDS = 8
 PLOT_WORDS = 16

@@ -15,11 +15,23 @@ import numpy as np
 
 from pycolab_b200 import _lib
 from pycolab_b200 import lowering
+from pycolab_b200.errors import NotLoweredError
 
 
 def _torch():
   import torch
   return torch
+
+
+def _check_crop(status, what, handle, crop_spec):
+  """`_lib.check` for a cropper entry point: a window or tracking list the device does
+  not serve (PCL_ERR_UNSUPPORTED) raises NotLoweredError."""
+  if status == _lib.ERR_UNSUPPORTED:
+    raise NotLoweredError(
+        '%s: the device does not serve this cropper (%dx%d window, at most %d cells; '
+        'tracking list %s; drapes are tracked by crop() on boards up to 128x128 only)' % (
+            what, crop_spec.rows, crop_spec.cols, _lib.MAX_CROP_CELLS, list(crop_spec.track)))
+  _lib.check(status, what, handle)
 
 
 def _mt_state(stream, seed):
@@ -331,14 +343,18 @@ class BatchedEngine(object):
         self._crop_dev = _torch().empty(shape, dtype=_torch().uint8, device=self.device)
     h, n = self._host_buffers(slot, shape)
     n['actions'][:] = np.asarray(actions, dtype=np.int32).reshape(-1)
-    _lib.check(self._lib.pcl_step_host_async(
+    status = self._lib.pcl_step_host_async(
         self._h, h['actions'].data_ptr(), self._actions.data_ptr(), C.byref(self._out),
         None if crop_spec is None else C.addressof(crop_spec),
         None if crop_spec is None else self._crop_dev.data_ptr(),
         None if crop_state is None else crop_state.data_ptr(),
         h['view'].data_ptr(), h['reward'].data_ptr(), h['has_reward'].data_ptr(),
-        h['discount'].data_ptr(), h['done'].data_ptr(), int(slot), self._stream()),
-        'pcl_step_host_async', self._h)
+        h['discount'].data_ptr(), h['done'].data_ptr(), int(slot), self._stream())
+    if crop_spec is not None and not self.game.float_reward:
+      # a refused crop spec (a drape in the tracking list: crop() serves those) is
+      # refused before the step is enqueued: no env has moved
+      _check_crop(status, 'pcl_step_host_async', self._h, crop_spec)
+    _lib.check(status, 'pcl_step_host_async', self._h)
     self._slot_shape[slot] = shape
 
   def host_wait(self, slot=0):
@@ -433,6 +449,9 @@ class BatchedEngine(object):
       _lib.check(self._lib.pcl_attach_cropper(self._h, None, None, None), 'pcl_attach_cropper')
       self._attached = None
       return None
+    if crop_spec.rows * crop_spec.cols > _lib.MAX_CROP_CELLS:
+      # no entry point serves it: refuse now rather than at the first step
+      _check_crop(_lib.ERR_UNSUPPORTED, 'attach_cropper', self._h, crop_spec)
     if out is None:
       out = torch.zeros((self.batch, crop_spec.rows, crop_spec.cols), dtype=torch.uint8,
                         device=self.device)
@@ -440,7 +459,11 @@ class BatchedEngine(object):
       state = self.new_crop_state()
     status = self._lib.pcl_attach_cropper(self._h, C.byref(crop_spec), out.data_ptr(),
                                           state.data_ptr())
-    if status == _lib.ERR_UNSUPPORTED:          # no epilogue in this program: crop after the step
+    if status == _lib.ERR_UNSUPPORTED:
+      # No epilogue in this program, or a tracked drape: crop after the step.  A refused
+      # spec leaves the handle's previous cropper attached; detach it, or the step kernel
+      # would go on writing into that cropper's view and state after they are released.
+      _lib.check(self._lib.pcl_attach_cropper(self._h, None, None, None), 'pcl_attach_cropper')
       self._attached = (crop_spec, state, out, False)
     else:
       _lib.check(status, 'pcl_attach_cropper', self._h)
@@ -478,12 +501,14 @@ class BatchedEngine(object):
         if code < 0:
           curtains.append(self._curtain_bytes(-code - 1))
           ptrs[i] = curtains[-1].data_ptr()
-      _lib.check(self._lib.pcl_crop_tracking(self._h, C.byref(crop_spec),
-                                             self._board.data_ptr(), out.data_ptr(), state_ptr,
-                                             ptrs, self._stream()), 'pcl_crop_tracking', self._h)
+      _check_crop(self._lib.pcl_crop_tracking(self._h, C.byref(crop_spec),
+                                              self._board.data_ptr(), out.data_ptr(), state_ptr,
+                                              ptrs, self._stream()),
+                  'pcl_crop_tracking', self._h, crop_spec)
     else:
-      _lib.check(self._lib.pcl_crop(self._h, C.byref(crop_spec), self._board.data_ptr(),
-                                    out.data_ptr(), state_ptr, self._stream()), 'pcl_crop', self._h)
+      _check_crop(self._lib.pcl_crop(self._h, C.byref(crop_spec), self._board.data_ptr(),
+                                     out.data_ptr(), state_ptr, self._stream()),
+                  'pcl_crop', self._h, crop_spec)
     return out
 
   def pack_handoff(self, view, packed):

@@ -9,6 +9,8 @@ batch-1 engine behind a `pycolab_b200.engine.Engine`.
 
 import copy
 
+import numpy as np
+
 from pycolab_b200 import rendering
 from pycolab_b200.errors import NotLoweredError
 
@@ -43,8 +45,7 @@ class ObservationCropper(object):
         raise ValueError("An `ObservationCropper` tried to fill empty space with a "
                          "character that isn't used by the current game engine.")
 
-  def _device_crop(self, spec):
-    from pycolab_b200 import batched
+  def _device_crop(self, spec, observation):
     self._check_pad()
     b = self._engine.batched
     if b is None:
@@ -52,8 +53,35 @@ class ObservationCropper(object):
     if getattr(self, '_state', None) is None:
       self._state = b.new_crop_state()
     board = b.crop(spec, state=self._state)[0].cpu().numpy().copy()
-    chars = set(self._engine.things) | set(self._engine.backdrop.palette)
-    return rendering.Observation(board=board, layers=rendering.LazyLayers(board, chars))
+    layers = getattr(observation, 'layers', None)
+    if layers is None or isinstance(layers, rendering.LazyLayers):
+      # occluded layers: those of the cropped board, pad cells included
+      chars = set(self._engine.things) | set(self._engine.backdrop.palette)
+      return rendering.Observation(board=board, layers=rendering.LazyLayers(board, chars))
+    # Un-occluded layers (occlusion_in_layers=False) are not a function of the board:
+    # crop each as _do_crop does (cropping.py:189-219), at the corner the device chose.
+    if spec.sprite_index < 0:
+      corner = (spec.offset_rows, spec.offset_cols)
+    else:
+      corner = tuple(int(v) for v in self._state[0, :2].cpu())
+    return rendering.Observation(board=board, layers=crop_layers(
+        layers, corner, spec.rows, spec.cols, self._pad_char))
+
+
+def crop_layers(layers, corner, rows, cols, pad_char):
+  """`_do_crop`'s layer part (cropping.py:189-219): each layer's rows x cols window at
+  `corner`, cells off the board set where the layer's character is `pad_char`."""
+  top, left = corner
+  out = {}
+  for char, layer in layers.items():
+    H, W = layer.shape
+    got = np.full((rows, cols), pad_char == char, dtype=bool)
+    r0, c0 = max(0, top), max(0, left)
+    r1, c1 = max(0, min(H, top + rows)), max(0, min(W, left + cols))
+    if r1 > r0 and c1 > c0:
+      got[r0 - top:r1 - top, c0 - left:c1 - left] = layer[r0:r1, c0:c1]
+    out[char] = got
+  return out
 
 
 class FixedCropper(ObservationCropper):
@@ -77,7 +105,7 @@ class FixedCropper(ObservationCropper):
     spec = _lib.CropSpec(self._rows, self._cols, -1,
                          -1 if self._pad_char is None else ord(self._pad_char),
                          0, 0, self._top_row, self._left_col, 0)
-    return self._device_crop(spec)
+    return self._device_crop(spec, observation)
 
   @property
   def rows(self):
@@ -128,11 +156,16 @@ class ScrollingCropper(ObservationCropper):
       if char not in self._engine.things:
         raise RuntimeError('ScrollingCropper was told to track a nonexistent game entity '
                            '{!r}.'.format(char))
-      codes.append(b.sprite_chars.index(char) + 1 if char in b.sprite_chars
-                   else -(b.drape_chars.index(char) + 1))
+      if char in b.sprite_chars:
+        codes.append(b.sprite_chars.index(char) + 1)
+      elif char in b.drape_chars:
+        codes.append(-(b.drape_chars.index(char) + 1))
+      else:                      # e.g. a box_world key: an object of the program, no drape
+        raise NotLoweredError('the device cropper tracks sprites and drapes only; {!r} is '
+                              'neither in this game'.format(char))
     spec = batched.scrolling_crop_spec(self._rows, self._cols, 0, track=codes,
                                        **self._spec_args)
-    return self._device_crop(spec)
+    return self._device_crop(spec, observation)
 
   @property
   def rows(self):

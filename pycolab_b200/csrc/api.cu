@@ -423,6 +423,34 @@ int host_pipeline_ready(pcl_handle* h) {
   return PCL_OK;
 }
 
+// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts, for every
+// cropper entry point.
+int crop_spec_ok(const pcl_handle* h, const pcl_crop_spec* crop) {
+  if (crop->rows <= 0 || crop->cols <= 0) return PCL_ERR_INVALID;
+  // sprite_index names the tracked sprite only when no priority list is given (a
+  // cropper may track a drape in a game without sprites).
+  if (crop->track[0] == 0 && crop->sprite_index >= h->spec.n_sprites) return PCL_ERR_INVALID;
+  if (crop->sprite_index >= 0 &&
+      (2 * crop->margin_rows >= crop->rows || 2 * crop->margin_cols >= crop->cols))
+    return PCL_ERR_INVALID;                                  // cropping.py:374-380
+  if (crop->pad_char < 0 && (crop->rows > h->spec.rows || crop->cols > h->spec.cols))
+    return PCL_ERR_INVALID;                                  // cropping.py:384-391
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
+    if (crop->sprite_index < 0) return PCL_ERR_INVALID;      // a FixedCropper tracks nothing
+    if (crop->track[i] > h->spec.n_sprites || crop->track[i] < -h->spec.n_drapes)
+      return PCL_ERR_INVALID;                                // no such sprite / drape
+  }
+  // A legal window upstream, but crop_word's reciprocal division is exact only below it.
+  if ((int64_t)crop->rows * crop->cols > PCL_MAX_CROP_CELLS) return PCL_ERR_UNSUPPORTED;
+  return PCL_OK;
+}
+
+bool tracks_drape(const pcl_crop_spec* crop) {
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i)
+    if (crop->track[i] < 0) return true;
+  return false;
+}
+
 }  // namespace
 
 int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
@@ -455,6 +483,11 @@ int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_acti
   if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
   if (!h_actions || !d_actions || slot < 0 || slot >= PCL_HOST_SLOTS) return PCL_ERR_INVALID;
   if (crop && !d_crop) return PCL_ERR_INVALID;
+  if (crop) {                    // refuse the crop before the step, not after it
+    const int ok = crop_spec_ok(h, crop);
+    if (ok != PCL_OK) return ok;
+    if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;      // no curtains here: pcl_crop_tracking
+  }
   int e = host_pipeline_ready(h);
   if (e != PCL_OK) return e;
   cudaStream_t s = (cudaStream_t)stream;
@@ -587,32 +620,6 @@ int pcl_layers(pcl_handle* h, const uint8_t* chars, int32_t n_chars, uint8_t* d_
 }
 
 namespace {
-// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts, for every
-// cropper entry point.
-int crop_spec_ok(const pcl_handle* h, const pcl_crop_spec* crop) {
-  if (crop->rows <= 0 || crop->cols <= 0) return PCL_ERR_INVALID;
-  // sprite_index names the tracked sprite only when no priority list is given (a
-  // cropper may track a drape in a game without sprites).
-  if (crop->track[0] == 0 && crop->sprite_index >= h->spec.n_sprites) return PCL_ERR_INVALID;
-  if (crop->sprite_index >= 0 &&
-      (2 * crop->margin_rows >= crop->rows || 2 * crop->margin_cols >= crop->cols))
-    return PCL_ERR_INVALID;                                  // cropping.py:374-380
-  if (crop->pad_char < 0 && (crop->rows > h->spec.rows || crop->cols > h->spec.cols))
-    return PCL_ERR_INVALID;                                  // cropping.py:384-391
-  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
-    if (crop->sprite_index < 0) return PCL_ERR_INVALID;      // a FixedCropper tracks nothing
-    if (crop->track[i] > h->spec.n_sprites || crop->track[i] < -h->spec.n_drapes)
-      return PCL_ERR_INVALID;                                // no such sprite / drape
-  }
-  return PCL_OK;
-}
-
-bool tracks_drape(const pcl_crop_spec* crop) {
-  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i)
-    if (crop->track[i] < 0) return true;
-  return false;
-}
-
 pcl::CropParams crop_params(const pcl_handle* h, const pcl_crop_spec* crop,
                             const uint8_t* d_board, uint8_t* d_crop, int32_t* d_crop_state) {
   pcl::CropParams p;
@@ -639,7 +646,6 @@ int pcl_attach_cropper(pcl_handle* h, const pcl_crop_spec* crop, uint8_t* d_crop
   if (!h->program->crop_epilogue) return PCL_ERR_UNSUPPORTED;
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
-  if ((int64_t)crop->rows * crop->cols >= 65536) return PCL_ERR_UNSUPPORTED;
   if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape medians need scratch memory
   h->base.cropper = crop_params(h, crop, nullptr, d_crop, d_crop_state);
   h->base.has_cropper = 1;

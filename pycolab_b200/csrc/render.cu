@@ -337,11 +337,11 @@ cudaError_t launch_layers(const LayersParams& p, cudaStream_t s) {
   return cudaGetLastError();
 }
 cudaError_t launch_crop(const CropParams& p, cudaStream_t s) {
-  if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols >= 65536) return cudaErrorInvalidValue;
+  if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols > PCL_MAX_CROP_CELLS) return cudaErrorInvalidValue;
   return launch_pdl(crop_kernel, (p.B + 3) / 4, 128, 0, s, p);
 }
 cudaError_t launch_crop_handoff(const CropParams& p, const HandoffParams& x, cudaStream_t s) {
-  if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols >= 65536) return cudaErrorInvalidValue;
+  if (p.crop.cols < 1 || (int64_t)p.crop.rows * p.crop.cols > PCL_MAX_CROP_CELLS) return cudaErrorInvalidValue;
   cudaError_t e = launch_pdl(crop_handoff_kernel, (p.B + 3) / 4, 128, 0, s, p, x);
   if (e != cudaSuccess || !x.signal_kernel) return e;
   handoff_signal_kernel<<<1, 32, 0, s>>>(x);          // plain stream order: after the grid above retires

@@ -50,6 +50,12 @@ def main():
   spec = batched.scrolling_crop_spec(9, 9, 0, pad_char=' ', scroll_margins=(None, None))
   eng.crop(spec)
   eng.crop(spec, state=eng.new_crop_state())
+  # drape tracking (pcl_crop_tracking): the warp-histogram medians of both curtains, on a
+  # 37-column board so the column loop takes its second pass
+  drapes = batched.scrolling_crop_spec(5, 7, 0, pad_char=' ', scroll_margins=(1, 2),
+                                       track=[-1, 1, -2])
+  eng.crop(drapes, state=eng.new_crop_state())
+  eng.crop(drapes)
   eng.unoccluded_layers()
   eng.curtain('#'), eng.curtain('@')
   eng.to_feature_array('P#@ ')
