@@ -398,7 +398,10 @@ typedef struct pcl_handle pcl_handle;
 int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out);
 int pcl_destroy(pcl_handle* h);
 
-/* Attach the caller's device buffers. */
+/* Attach the caller's device buffers.  The static level data (backdrop, read-only
+ * patterns, reset templates) may be read into the handle's own derived copies before
+ * the first step or reset after this call; a host that rewrites it afterwards calls
+ * pcl_bind_state again. */
 int pcl_bind_state(pcl_handle* h, const pcl_state* state);
 
 /* PCL_PROG_COMPILED: the bytecode every env runs, h_code a HOST array of n_words int32 words

@@ -35,6 +35,10 @@ struct pcl_handle {
   int code_dev_words;            // words the device buffer holds room for
   int code_stale;                // code_host changed since the upload
   uint8_t* backdrop_live;        // pcl_bind_backdrop, or NULL
+  // Program::derive: its allocation for the bound state, and whether the state was bound
+  // since it was built
+  void* derived_dev;
+  int derive_stale;
 };
 
 namespace {
@@ -200,7 +204,25 @@ int upload_code(pcl_handle* h, cudaStream_t s) {
   return PCL_OK;
 }
 
-// Everything a step or reset on `s` needs is in place; uploads bound code on the way.
+// Build the program's derived copies of the state bound since the last launch (the
+// first launch after pcl_bind_state reads the static level data; binding itself touches
+// no device memory).  Launches still in flight may read the previous copies: wait first.
+int derive_state(pcl_handle* h) {
+  if (!h->derive_stale) return PCL_OK;
+  if (h->derived_dev) {
+    PCL_CUDA(h, cudaDeviceSynchronize());
+    PCL_CUDA(h, cudaFree(h->derived_dev));
+    h->derived_dev = nullptr;
+  }
+  const int r = h->program->derive(h->spec, h->st, h->batch, &h->base, &h->derived_dev);
+  if (r == PCL_ERR_CUDA) return cuda_failed(h, cudaGetLastError(), "Program::derive");
+  if (r != PCL_OK) return r;
+  h->derive_stale = 0;
+  return PCL_OK;
+}
+
+// Everything a step or reset on `s` needs is in place; uploads bound code and builds
+// derived copies on the way.
 int check_ready(pcl_handle* h, const pcl_outputs* out, cudaStream_t s) {
   if (!h || !out) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
@@ -208,6 +230,8 @@ int check_ready(pcl_handle* h, const pcl_outputs* out, cudaStream_t s) {
   if (live_backdrop(h->spec) && !h->backdrop_live) return PCL_ERR_UNBOUND;
   if (!out->d_board || !outputs_set(*out)) return PCL_ERR_INVALID;
   if (float_rewards(h) && !out->d_reward_f64) return PCL_ERR_INVALID;
+  const int r = derive_state(h);
+  if (r != PCL_OK) return r;
   return h->program->check_code ? upload_code(h, s) : PCL_OK;
 }
 
@@ -264,6 +288,8 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->code_dev_words = 0;
   h->code_stale = 0;
   h->backdrop_live = nullptr;
+  h->derived_dev = nullptr;
+  h->derive_stale = 0;
   *out = h;
   return PCL_OK;
 }
@@ -278,6 +304,7 @@ int pcl_destroy(pcl_handle* h) {
   }
   if (h) {
     if (h->code_dev) cudaFree(h->code_dev);
+    if (h->derived_dev) cudaFree(h->derived_dev);
     delete[] h->code_host;
   }
   delete h;
@@ -299,6 +326,7 @@ int pcl_bind_state(pcl_handle* h, const pcl_state* st) {
   }
   h->st = *st;
   fill_params(h, &h->base);      // the per-step calls only patch mode / actions / outputs
+  h->derive_stale = h->program->derive != nullptr;
   h->bound = 1;
   return PCL_OK;
 }

@@ -52,6 +52,11 @@ struct StepParams {
   CropParams cropper;            // (board is taken from `out` at launch time)
   const int32_t* code;           // device copy of the bytecode bound with pcl_bind_code, or NULL
   uint8_t* backdrop_live;        // pcl_bind_backdrop: u8 [B, H, pitch] live curtains, or NULL
+  // Program::derive: device copies the program builds from the static level data bound
+  // with pcl_bind_state, in formats only that program knows (indexed like the arrays they
+  // come from: per level, or one copy when the stride is 0).
+  const uint32_t* derived[2];
+  int64_t derived_bstride[2];    // in words
 };
 
 // Launch with the programmatic-stream-serialisation attribute (the kernel calls
@@ -103,6 +108,11 @@ struct Program {
   // PCL_OK / PCL_ERR_INVALID.  nullptr: the program takes no code.
   int (*check_code)(const pcl_spec&, const int32_t* words, int n_words);
   bool float_reward_arg0;        // rewards are float64 when spec.program_arg[0] != 0
+  // Called before the first step or reset after each pcl_bind_state: builds
+  // StepParams::derived* from the bound state for a handle of `batch` envs, in one device
+  // allocation returned in *owned (the handle frees it when it rebuilds and at
+  // pcl_destroy).  May synchronise the device.  nullptr: the program derives nothing.
+  int (*derive)(const pcl_spec&, const pcl_state&, int batch, StepParams* base, void** owned);
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
     kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld;

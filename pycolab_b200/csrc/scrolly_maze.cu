@@ -22,9 +22,10 @@
 //      wherever the scroll order moves the walker first) and the 3x3 patch of coin bits
 //      around the player;
 //   4. once those bits are in, cp.async of the backdrop tile and of the two windows of
-//      the bit-packed patterns (4 words per row, two 8-byte copies) -> smem, no
-//      registers held; groups 1 and 2 run on registers + shuffles of the patch bits
-//      while the copies fly;
+//      the bit-packed patterns (4 words per row, one 16-byte copy from the row-blocked
+//      copies of the bound patterns, see "Row-blocked windows") -> smem, no registers
+//      held; groups 1 and 2 run on registers + shuffles of the patch bits while the
+//      copies fly;
 //   5. each lane shifts whole window rows once into one word per 16-cell board
 //      segment (wall16 << 16 | coin16); the paint loop then composes 16-byte
 //      segments from smem (prmt with a 256-entry selector table) and streams them
@@ -70,6 +71,9 @@
 // the coin patch rows), a pick-up sets its group's bit, and an auto-reset restart
 // copies back only the dirty groups (the reloaded record brings the mask back to 0).
 // A host that writes an env's coin pattern directly sets that env's aux2 to -1.
+#include <algorithm>
+#include <new>
+
 #include "pcl_device.cuh"
 #include "pcl_kernels.cuh"
 #include "pcl_crop.cuh"
@@ -282,9 +286,12 @@ __device__ __forceinline__ void scrolly_move_p(Drape& d, const ScrollyCfg& cfg, 
   plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
 }
 
-// The env's own coin pattern, and its level's template.  Both are recomputed from the
-// launch parameters where they are used: at 64 registers, no pointer to either stays live
-// through the step.
+// The env's own coin pattern, its level's template and its level's wall pattern.  All are
+// recomputed from the launch parameters where they are used: at 64 registers, no pointer
+// to any of them stays live through the step.
+__device__ __forceinline__ const uint32_t* level_walls(const StepParams& p, int64_t lvl) {
+  return p.st.d_pattern[0] + lvl * p.st.pattern_bstride[0];
+}
 __device__ __forceinline__ uint32_t* env_coins(const StepParams& p, int env) {
   return p.st.d_pattern[1] + (int64_t)env * p.st.pattern_bstride[1];
 }
@@ -333,8 +340,6 @@ scrolly_maze_step(const StepParams p) {
     return;
   }
   const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
-
-  const uint32_t* wall_pat = p.st.d_pattern[0] + lvl * p.st.pattern_bstride[0];
 
   // The env's action word does not depend on the records either: issue its load now,
   // beside theirs, instead of one memory round trip later (it is only USED if the env
@@ -460,7 +465,7 @@ scrolly_maze_step(const StepParams p) {
       const int w = lane / 5, k = lane - w * 5;
       const int pr = wr + rec[w * PCL_SPRITE_WORDS + PCL_S_VROW] + k - 2;
       c_first = wc + rec[w * PCL_SPRITE_WORDS + PCL_S_VCOL] - 2;
-      if ((unsigned)pr < (unsigned)p.PH) { row = wall_pat + (int64_t)pr * PWW; limit = PWW; }
+      if ((unsigned)pr < (unsigned)p.PH) { row = level_walls(p, lvl) + (int64_t)pr * PWW; limit = PWW; }
     } else if (lane < 24) {
       // A clean group's row comes from the level's template (see "Coin groups").
       const int r = lane < 23 ? p_vrow + (lane - 20) - 1 : 0;
@@ -507,17 +512,32 @@ scrolly_maze_step(const StepParams p) {
 #pragma unroll 4
     for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
   }
-  // Coin window rows of clean groups come from the level's template (see "Coin groups"):
-  // per env that is L2 traffic shared by the level's envs instead of DRAM of its own.
+  // Both windows come from the row-blocked copies (see "Row-blocked windows"): the H rows
+  // of a window are one contiguous run there.  Coin window rows of clean groups come from
+  // the level's template (see "Coin groups"): per env that is L2 traffic shared by the
+  // level's envs instead of DRAM of its own.
   {
-    const uint32_t* coin_tpl = level_coins(p, lvl);
     const int gs = coin_group_shift(p.PH);
+    const uint32_t* wsrc =
+        p.derived[0] + lvl * p.derived_bstride[0] + ((int64_t)(we >> 1) * p.PH + wr) * nw;
+    const uint32_t* csrc =
+        p.derived[1] + lvl * p.derived_bstride[1] + ((int64_t)(ce >> 1) * p.PH + cr_pred) * nw;
     const int hw = nw >> 1, nhalf = H * hw;  // 8-byte halves per window row
-    for (int i = lane; i < nhalf; i += 32) {
-      const int r = narrow ? i >> 1 : i / hw, k = (i - r * hw) * 2, pr = cr_pred + r;
-      cp_async8(s_wall + i * 2, wall_pat + (int64_t)(wr + r) * PWW + we + k);
-      if (!(((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u))
-        cp_async8(s_coin + i * 2, coin_tpl + (int64_t)pr * PWW + ce + k);
+    if (narrow) {                            // one 16-byte row per copy
+#pragma unroll 1
+      for (int r = lane; r < H; r += 32) {
+        cp_async16(s_wall + r * 4, wsrc + r * 4);
+        if (!(((unsigned)rec_coins[PCL_D_AUX2] >> ((cr_pred + r) >> gs)) & 1u))
+          cp_async16(s_coin + r * 4, csrc + r * 4);
+      }
+    } else {
+#pragma unroll 1
+      for (int i = lane; i < nhalf; i += 32) {
+        const int pr = cr_pred + i / hw;
+        cp_async8(s_wall + i * 2, wsrc + i * 2);
+        if (!(((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u))
+          cp_async8(s_coin + i * 2, csrc + i * 2);
+      }
     }
     if (rec_coins[PCL_D_AUX2] != 0) {
 #pragma unroll 1
@@ -558,7 +578,7 @@ scrolly_maze_step(const StepParams p) {
       if (pr < 0) pr += p.PH;
       if (pc < 0) pc += p.PW;
       if ((unsigned)pr < (unsigned)p.PH && (unsigned)pc < (unsigned)p.PW)
-        next_to_wall = bit_at(wall_pat + (int64_t)pr * PWW, pc);
+        next_to_wall = bit_at(level_walls(p, lvl) + (int64_t)pr * PWW, pc);
       else
         my_err |= PCL_ENV_ERR_INDEX;
     }
@@ -836,11 +856,68 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(scrolly_maze_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);
 }
 
+// ---- Row-blocked windows (built by derive() for each pcl_bind_state) -----------------
+// Block k of a pattern holds words [2k, 2k + window_words(W)) of every pattern row, rows
+// contiguous, so the window at first word 2k and row r0 is ONE run of H * window_words(W)
+// words.  Staged from the pattern itself, a 16-byte window row fills only half of the
+// 32-byte L2 sector it is read from whenever pattern rows are 32 bytes or more apart.
+// Blocks exist for every first word a window can stage, 0 .. ((PW - W) >> 5) & ~1.  One
+// copy of the wall pattern d_pattern[0] (derived[0]) and one of the coin template
+// d_pattern_init[1] (derived[1]), each indexed like the array it comes from.
+
+__global__ void build_blocked(const uint32_t* src, int64_t src_bstride, uint32_t* dst, int PH,
+                              int PWW, int nw, int nblk, int64_t total) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t t = i / nw;
+    const int w = (int)(i - t * nw);
+    const int row = (int)(t % PH);
+    t /= PH;
+    const int k = (int)(t % nblk);
+    dst[i] = src[(t / nblk) * src_bstride + (int64_t)row * PWW + 2 * k + w];
+  }
+}
+
+int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, void** owned) {
+  // Copies of per-level data: as many as the level index can name (one per env without
+  // one), or a single one when the array has no stride.
+  int64_t levels = batch;
+  if (st.d_level) {
+    int32_t* lv = new (std::nothrow) int32_t[batch];
+    if (!lv) return PCL_ERR_NOMEM;
+    const cudaError_t e = cudaMemcpy(lv, st.d_level, sizeof(int32_t) * batch, cudaMemcpyDeviceToHost);
+    levels = 1;
+    for (int i = 0; e == cudaSuccess && i < batch; ++i) levels = std::max<int64_t>(levels, lv[i] + 1);
+    delete[] lv;
+    if (e != cudaSuccess) return PCL_ERR_CUDA;
+  }
+  const int W = s.cols, PH = s.pattern_rows;
+  const int nw = window_words(W), nblk = ((((s.pattern_cols - W) >> 5) & ~1) >> 1) + 1;
+  const int64_t blk_words = (int64_t)nblk * PH * nw;              // one blocked copy
+  const int64_t n_wall = st.pattern_bstride[0] == 0 ? 1 : levels;
+  const int64_t n_coin = st.pattern_init_bstride[1] == 0 ? 1 : levels;
+  const int64_t off_coin = (n_wall * blk_words * 4 + 255) & ~(int64_t)255;
+  uint8_t* buf = nullptr;
+  if (cudaMalloc(&buf, off_coin + n_coin * blk_words * 4) != cudaSuccess) return PCL_ERR_NOMEM;
+  *owned = buf;
+  uint32_t* wall = reinterpret_cast<uint32_t*>(buf);
+  uint32_t* coin = reinterpret_cast<uint32_t*>(buf + off_coin);
+  build_blocked<<<1024, 256>>>(st.d_pattern[0], st.pattern_bstride[0], wall, PH, s.pattern_words,
+                               nw, nblk, n_wall * blk_words);
+  build_blocked<<<1024, 256>>>(st.d_pattern_init[1], st.pattern_init_bstride[1], coin, PH,
+                               s.pattern_words, nw, nblk, n_coin * blk_words);
+  p->derived[0] = wall; p->derived_bstride[0] = n_wall > 1 ? blk_words : 0;
+  p->derived[1] = coin; p->derived_bstride[1] = n_coin > 1 ? blk_words : 0;
+  return cudaDeviceSynchronize() == cudaSuccess && cudaGetLastError() == cudaSuccess ? PCL_OK
+                                                                                     : PCL_ERR_CUDA;
+}
+
 }  // namespace
 
 const Program kScrollyMaze = {check_spec, check_state, curtain, launch, nullptr,
                               /*float_reward=*/false, /*crop_epilogue=*/true,
-                              /*scroll_groups=*/false};
+                              /*scroll_groups=*/false, /*check_code=*/nullptr,
+                              /*float_reward_arg0=*/false, derive};
 
 }  // namespace pcl
 
