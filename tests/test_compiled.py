@@ -18,9 +18,10 @@ import pytest
 import boundary_sweep
 import golden_cases as gc
 import refdriver
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
-from pycolab_b200 import _lib, compat, compiler, lowering
+from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.prefab_parts import sprites as b_sprites
@@ -28,23 +29,9 @@ from pycolab_b200.prefab_parts import sprites as b_sprites
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def _load(path):
-  """Import a pycolab module through compat, leaving sys.modules as it was."""
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    return compat.load_example(path)
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-
-
 @pytest.fixture(scope='module')
 def games():
-  mod = _load(os.path.join(HERE, 'compiled_games.py'))
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('compiled_games.py')
 
 
 @pytest.mark.parametrize('name', gc.names('compiled_'))
@@ -251,8 +238,8 @@ needs_ref = pytest.mark.skipif(not refdriver.available(), reason='/root/referenc
 def test_reference_classics_compile_and_match_golden(name):
   g = gc.load(name)
   kind, art = bytes(g['kind']).decode(), tj.u8_to_art(g['art'])
-  mod = _load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'classics',
-                           kind + '.py'))
+  mod = rg.load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'classics',
+                             kind + '.py'))
   compiler.register(mod.PlayerSprite)
   try:
     saved, mod.GAME_ART = mod.GAME_ART, art
@@ -279,17 +266,6 @@ def test_reference_classics_compile_and_match_golden(name):
 
 # ------------------------------------------------------------ pcl_bind_code --
 
-def _handle(lib, spec):
-  h = C.c_void_p()
-  assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
-  return h
-
-
-def _bind(lib, h, words):
-  words = np.ascontiguousarray(words, dtype=np.int32)
-  return lib.pcl_bind_code(h, words.ctypes.data, len(words))
-
-
 def _outputs():
   f = boundary_sweep.FAKE
   return _lib.Outputs(f, f, f, f, f, f)
@@ -300,14 +276,14 @@ def test_bind_code_checks(games):
   lowered = lowering.lower(games.make_coins(0))
   spec = lowered.make_spec(True)
   code = lowered.code.copy()
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
     # step and reset before any code is bound
     assert lib.pcl_bind_state(h, C.byref(boundary_sweep._full_state())) == _lib.OK
     out = _outputs()
     assert lib.pcl_step(h, boundary_sweep.FAKE, C.byref(out), None) == _lib.ERR_UNBOUND
     assert lib.pcl_reset(h, None, C.byref(out), None) == _lib.ERR_UNBOUND
-    assert _bind(lib, h, code) == _lib.OK
+    assert rg.bind(lib, h, code) == _lib.OK
     n_ent = code[0]
     body = 1 + n_ent
     first = code[1]                    # the player's update (sprite 0)
@@ -328,44 +304,35 @@ def test_bind_code_checks(games):
         'oversize': np.zeros(_lib.MAX_CODE_WORDS + 1, dtype=np.int32),
         'empty': code[:body],
     }
-    pc = _instructions(code, first, code[2])
+    pc = ocompiled.instructions(code, first, code[2])
     jz = [i for i in pc if code[i] == op('JZ')][0]
     cases['backward jump'] = mutated(jz + 1, jz)
     cases['jump out of the function'] = mutated(jz + 1, len(code) + 5)
     cases['jump into an operand'] = mutated(jz + 1, jz + 1)
-    getr = [i for i in _instructions(code, code[2], code[3]) if code[i] == op('GETR')][0]
+    getr = [i for i in ocompiled.instructions(code, code[2], code[3]) if code[i] == op('GETR')][0]
     cases['register out of range'] = mutated(getr + 1, 3)     # sprites have 3 registers
-    field = [i for i in _instructions(code, code[3], len(code)) if code[i] == op('FIELD')][0]
+    field = [i for i in ocompiled.instructions(code, code[3], len(code))
+             if code[i] == op('FIELD')][0]
     cases['entity out of range'] = mutated(field + 1, 2)      # drape 'c' is entity 2
     cases['sprite entity past the end'] = mutated(field + 1, 7)
-    load = _instructions(code, first, code[2])
+    load = ocompiled.instructions(code, first, code[2])
     store = [i for i in load if code[i] == op('STORE')][0]
     cases['local out of range'] = mutated(store + 1, _lib.CODE_LOCALS)
     cases['no RET at the end'] = mutated(len(code) - 1, op('POP'))
     cases['stack underflow'] = mutated(first, op('POP'))
     for label, words in cases.items():
-      assert _bind(lib, h, words) == _lib.ERR_INVALID, label
+      assert rg.bind(lib, h, words) == _lib.ERR_INVALID, label
     assert lib.pcl_bind_code(h, None, 4) == _lib.ERR_INVALID
   finally:
     lib.pcl_destroy(h)
 
 
-def _instructions(code, start, end):
-  """Word indices of the instructions in [start, end)."""
-  out, pc = [], start
-  while pc < end:
-    out.append(pc)
-    op = code[pc]
-    pc += 1 + _lib.OPERANDS[op] + (code[pc + 1] if op == _lib.OP['IN'] else 0)
-  return out
-
-
 def test_bind_code_is_refused_by_other_programs():
   lib = _lib.load()
   from pycolab_b200.games.classics import four_rooms
-  h = _handle(lib, lowering.lower(four_rooms.make_game()).make_spec(True))
+  h = rg.handle(lib, lowering.lower(four_rooms.make_game()).make_spec(True))
   try:
-    assert _bind(lib, h, [1, 2, 0]) == _lib.ERR_UNSUPPORTED
+    assert rg.bind(lib, h, [1, 2, 0]) == _lib.ERR_UNSUPPORTED
   finally:
     lib.pcl_destroy(h)
 
@@ -390,8 +357,8 @@ def test_bench_player_compiles_like_the_reference_four_rooms():
     import compiled_bench
   finally:
     sys.path.pop(0)
-  mod = _load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'classics',
-                           'four_rooms.py'))
+  mod = rg.load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'classics',
+                             'four_rooms.py'))
   theirs = compiler.compile_class(mod.PlayerSprite)
   ours = compiler.compile_class(compiled_bench.FourRoomsPlayer)
   link = lambda c: compiler.link({'P': c}, 'P', '', 13, 13, []).tolist()

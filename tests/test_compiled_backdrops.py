@@ -1,7 +1,7 @@
 """CPU tests of Backdrops with registered update() code on the compiled step program
 (`pycolab_b200.compiler` kind 'backdrop', PCL_OP_SETBACK / FILLBACK / ROLLBACK, program_arg[4]):
 
-  - the test interpreter of tests/backdrop_oracle.py running the games of
+  - the oracle interpreter (oracle/compiled.py) running the games of
     tests/backdrop_games.py reproduces the reference's trajectories (tests/golden/backdrop_*),
     the Backdrop's curtain, Plot keys and NumPy's generator included;
   - with the reference present, its own fluvial_natation classes, registered, lower to the
@@ -15,43 +15,27 @@
 
 import ctypes as C
 import os
-import sys
 
 import numpy as np
 import pytest
 
-import backdrop_oracle
 import golden_cases as gc
 import refdriver
+import registered_games as rg
 import test_kernel_resources as resources
 import trajectory as tj
 from oracle import compiled as ocompiled
-from pycolab_b200 import _lib, ascii_art, compat, compiler, lowering
+from pycolab_b200 import _lib, ascii_art, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.prefab_parts import sprites as b_sprites
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 needs_ref = pytest.mark.skipif(not refdriver.available(), reason='reference not present')
-
-
-def _load(path):
-  """Import a pycolab module through compat, leaving sys.modules as it was."""
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    return compat.load_example(path)
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
 
 
 @pytest.fixture(scope='module')
 def games():
-  mod = _load(os.path.join(HERE, 'backdrop_games.py'))
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('backdrop_games.py')
 
 
 def _oracle_trajectory(make_engine, actions, rng_seed=None, keys=()):
@@ -70,7 +54,7 @@ def _oracle_trajectory(make_engine, actions, rng_seed=None, keys=()):
     curtains.append(world.backdrop.copy())
     plot.append([world.plot.regs[plot_keys.index(k)] for k in keys])
     assert world.error == 0
-  got = tj.run_trajectory(lambda: backdrop_oracle.make_world(lowered, words), actions,
+  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered, words), actions,
                           on_frame=on_frame)
   return got, sprites, curtains, plot, words
 
@@ -103,7 +87,8 @@ def test_oracle_runs_the_fluvial_pair_like_the_reference(games, name):
 
 @pytest.fixture(scope='module')
 def ref_fluvial():
-  mod = _load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'fluvial_natation.py'))
+  mod = rg.load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples',
+                             'fluvial_natation.py'))
   compiler.register(mod.PlayerSprite, mod.RiverBackdrop)
   yield mod
   compiler.unregister(mod.PlayerSprite, mod.RiverBackdrop)
@@ -320,17 +305,6 @@ def test_a_registered_backdrop_needs_registered_entities(games):
 
 # ------------------------------------------------------------ the C boundary --
 
-def _handle(lib, spec):
-  h = C.c_void_p()
-  assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
-  return h
-
-
-def _bind(lib, h, words):
-  words = np.ascontiguousarray(words, dtype=np.int32)
-  return lib.pcl_bind_code(h, words.ctypes.data, len(words))
-
-
 def test_bind_code_checks_the_backdrop_function(games):
   lib = _lib.load()
   lowered = lowering.lower(games.make_flow(0))
@@ -339,9 +313,9 @@ def test_bind_code_checks_the_backdrop_function(games):
   n = len(lowered.sprite_chars + lowered.drape_chars)
   op = lambda name: _lib.OP[name]
   entry = int(code[1 + n])
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
-    assert _bind(lib, h, code) == _lib.OK
+    assert rg.bind(lib, h, code) == _lib.OK
     roll = entry + [i for i, w in enumerate(code[entry:].tolist()) if w == op('ROLLBACK')][0]
     fill = entry + [i for i, w in enumerate(code[entry:].tolist()) if w == op('FILLBACK')][0]
     walker = int(code[1])
@@ -365,8 +339,8 @@ def test_bind_code_checks_the_backdrop_function(games):
         'FILL in the Backdrop': mutated((fill, op('FILL'))),
     }
     for label, words in cases.items():
-      assert _bind(lib, h, words) == _lib.ERR_INVALID, label
-    assert _bind(lib, h, mutated((roll + 2, 0), (roll + 3, lowered.rows))) == _lib.OK
+      assert rg.bind(lib, h, words) == _lib.ERR_INVALID, label
+    assert rg.bind(lib, h, mutated((roll + 2, 0), (roll + 3, lowered.rows))) == _lib.OK
   finally:
     lib.pcl_destroy(h)
 
@@ -375,7 +349,7 @@ def test_bind_backdrop_and_create_checks(games):
   lib = _lib.load()
   lowered = lowering.lower(games.make_flow(0))
   spec = lowered.make_spec(True)
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
     assert lib.pcl_bind_backdrop(h, None) == _lib.ERR_INVALID
     assert lib.pcl_bind_backdrop(h, 0x1000) == _lib.OK
@@ -385,13 +359,13 @@ def test_bind_backdrop_and_create_checks(games):
   # handles without a compiled Backdrop refuse it
   spec0 = lowered.make_spec(True)
   spec0.program_arg[4] = 0
-  h = _handle(lib, spec0)
+  h = rg.handle(lib, spec0)
   try:
     assert lib.pcl_bind_backdrop(h, 0x1000) == _lib.ERR_INVALID
   finally:
     lib.pcl_destroy(h)
   from pycolab_b200.games import fluvial_natation
-  h = _handle(lib, lowering.lower(fluvial_natation.make_game()).make_spec(True))
+  h = rg.handle(lib, lowering.lower(fluvial_natation.make_game()).make_spec(True))
   try:
     assert lib.pcl_bind_backdrop(h, 0x1000) == _lib.ERR_INVALID
   finally:
@@ -408,14 +382,14 @@ def test_steps_wait_for_the_live_backdrop(games):
   every step and reset entry point before it launches anything."""
   lib = _lib.load()
   lowered = lowering.lower(games.make_flow(0))
-  h = _handle(lib, lowered.make_spec(True))
+  h = rg.handle(lib, lowered.make_spec(True))
   try:
     st = _lib.State()
     fake = 0x1000
     st.d_backdrop = st.d_plot = st.d_plot_init = st.d_sprites = st.d_sprites_init = fake
     st.d_z_order = st.d_z_order_init = st.d_rng = fake
     assert lib.pcl_bind_state(h, C.byref(st)) == _lib.OK
-    assert _bind(lib, h, lowered.code) == _lib.OK
+    assert rg.bind(lib, h, lowered.code) == _lib.OK
     out = _lib.Outputs(fake, fake, fake, fake, fake)
     assert lib.pcl_reset(h, None, C.byref(out), None) == _lib.ERR_UNBOUND
     assert lib.pcl_step(h, fake, C.byref(out), None) == _lib.ERR_UNBOUND

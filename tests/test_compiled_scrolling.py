@@ -3,7 +3,7 @@ MazeWalkers in registered update() code (`pycolab_b200.compiler`, csrc/compiled.
 
   - the forms the compiler accepts for them and the ones it refuses, with the source line;
   - limits refused at lowering: registers, scrolling groups, pattern shapes;
-  - the oracle interpreter of tests/scrolling_oracle.py running the compiled maze of
+  - the oracle interpreter (oracle/compiled.py) running the compiled maze of
     tests/scrolling_games.py reproduces the reference's scrolly_maze trajectories
     (tests/golden/scrolly_*.npz), and the compiled sampler those of tests/golden/scrolling_*;
   - with the reference present, its own scrolly_maze classes compile unchanged;
@@ -13,7 +13,6 @@ MazeWalkers in registered update() code (`pycolab_b200.compiler`, csrc/compiled.
 import ctypes as C
 import inspect
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -21,36 +20,22 @@ import pytest
 import boundary_sweep
 import golden_cases as gc
 import refdriver
-import scrolling_oracle
+import registered_games as rg
 import scrolly_shapes
 import trajectory as tj
-from pycolab_b200 import _lib, compat, compiler, lowering
+from oracle import compiled as ocompiled
+from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.prefab_parts import drapes as b_drapes
 from pycolab_b200.prefab_parts import sprites as b_sprites
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 needs_ref = pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
-
-
-def _load(path):
-  """Import a pycolab module through compat, leaving sys.modules as it was."""
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    return compat.load_example(path)
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
 
 
 @pytest.fixture(scope='module')
 def games():
-  mod = _load(os.path.join(HERE, 'scrolling_games.py'))
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('scrolling_games.py')
 
 
 def _margins(name):
@@ -79,7 +64,7 @@ def test_oracle_runs_compiled_maze_like_the_reference(games, name):
   def on_frame(world, out):
     sprites.append(_sprite_rows(world, 'Pabc'))
     assert world.error == 0
-  got = tj.run_trajectory(lambda: scrolling_oracle.make_world(lowered), g['actions'].tolist(),
+  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist(),
                           on_frame=on_frame)
   tj.assert_same_trajectory(g, got, name)
   np.testing.assert_array_equal(g['sprites'], np.array(sprites))
@@ -102,7 +87,7 @@ def _sampler_trajectory(games, g):
     assert world.error == 0
 
   def make():
-    worlds.append(scrolling_oracle.make_world(lowered))
+    worlds.append(ocompiled.make_world(lowered))
     return worlds[-1]
   got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
   patterns = [worlds[-1].things[ch].pattern for ch in games.SCROLLYS]
@@ -122,24 +107,8 @@ def test_oracle_runs_compiled_sampler_like_the_reference(games, name):
     np.testing.assert_array_equal(g['pattern_' + {'#': 'walls', '*': 'gems'}[ch]], pattern)
 
 
-@pytest.mark.parametrize('name', gc.names('compiled_'))
-def test_scrolling_oracle_runs_the_compiled_goldens_too(name):
-  """The interpreter of tests/scrolling_oracle.py on games without Scrollys: the reference's
-  trajectories of tests/compiled_games.py, as oracle/compiled.py reproduces them."""
-  mod = _load(os.path.join(HERE, 'compiled_games.py'))
-  compiler.register(*mod.CLASSES)
-  try:
-    g = gc.load(name)
-    game, level = bytes(g['game']).decode(), int(g['level'][0])
-    lowered = lowering.lower(mod.GAMES[game](level))
-  finally:
-    compiler.unregister(*mod.CLASSES)
-  got = tj.run_trajectory(lambda: scrolling_oracle.make_world(lowered), g['actions'].tolist())
-  tj.assert_same_trajectory(g, got, name)
-
-
 def test_oracle_raises_on_postscroll_before_the_move(games):
-  world = scrolling_oracle.make_world(lowering.lower(games.make_early()))
+  world = ocompiled.make_world(lowering.lower(games.make_early()))
   world.its_showtime()
   world.play(0)
   with pytest.raises(RuntimeError, match='postscroll'):
@@ -323,7 +292,7 @@ def test_groups_and_pattern_shapes_are_refused_at_lowering(games):
 
 @needs_ref
 def test_reference_scrolly_maze_classes_compile_and_match_golden(games):
-  mod = _load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'scrolly_maze.py'))
+  mod = rg.load(os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'scrolly_maze.py'))
   with pytest.raises(NotLoweredError, match=r'the_plot\.log\(\)'):
     compiler.compile_class(mod.CashDrape)
   ours = (mod.PlayerSprite, mod.PatrollerSprite, mod.MazeDrape)
@@ -345,7 +314,7 @@ def test_reference_scrolly_maze_classes_compile_and_match_golden(games):
           update_schedule=[['#'], ['a', 'b', 'c', 'P'], ['@']], z_order='abc@#P')
       lowered = lowering.lower(engine)
       assert lowered.program == _lib.PROG_COMPILED
-      got = tj.run_trajectory(lambda: scrolling_oracle.make_world(lowered), g['actions'].tolist())
+      got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist())
       tj.assert_same_trajectory(g, got, name)
   finally:
     compiler.unregister(*ours)
@@ -353,38 +322,18 @@ def test_reference_scrolly_maze_classes_compile_and_match_golden(games):
 
 # ------------------------------------------------------------ pcl_bind_code --
 
-def _handle(lib, spec):
-  h = C.c_void_p()
-  assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
-  return h
-
-
-def _bind(lib, h, words):
-  words = np.ascontiguousarray(words, dtype=np.int32)
-  return lib.pcl_bind_code(h, words.ctypes.data, len(words))
-
-
-def _instructions(code, start, end):
-  out, pc = [], start
-  while pc < end:
-    out.append(pc)
-    op = code[pc]
-    pc += 1 + _lib.OPERANDS[op] + (code[pc + 1] if op in (_lib.OP['IN'], _lib.OP['PICK']) else 0)
-  return out
-
-
 def test_bind_code_checks_the_scrolly_opcodes(games):
   lib = _lib.load()
   lowered = lowering.lower(games.make_sampler(0))
   spec = lowered.make_spec(True)
   code = lowered.code.copy()
   op = lambda name: _lib.OP[name]
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
-    assert _bind(lib, h, code) == _lib.OK
+    assert rg.bind(lib, h, code) == _lib.OK
     fn = {ch: code[1 + i] for i, ch in enumerate(lowered.sprite_chars + lowered.drape_chars)}
     starts = sorted(set(fn.values())) + [len(code)]
-    span = lambda ch: _instructions(code, fn[ch], starts[starts.index(fn[ch]) + 1])
+    span = lambda ch: ocompiled.instructions(code, fn[ch], starts[starts.index(fn[ch]) + 1])
     find = lambda ch, name: [i for i in span(ch) if code[i] == op(name)][0]
 
     def mutated(at, value):
@@ -407,7 +356,7 @@ def test_bind_code_checks_the_scrolly_opcodes(games):
     }
     cases['PATTERN of self in a walker'][watcher_curtain + 1] = -1
     for label, words in cases.items():
-      assert _bind(lib, h, words) == _lib.ERR_INVALID, label
+      assert rg.bind(lib, h, words) == _lib.ERR_INVALID, label
   finally:
     lib.pcl_destroy(h)
 
@@ -434,7 +383,7 @@ def test_create_checks_written_patterns(games):
 def test_bind_state_needs_the_written_pattern_template(games):
   lib = _lib.load()
   spec = lowering.lower(games.make_sampler(0)).make_spec(True)
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
     st = boundary_sweep._full_state()
     for d in range(2):

@@ -2,7 +2,7 @@
 registered update() code sets their own position and visibility (`pycolab_b200.compiler`,
 PCL_OP_SETFIELD in csrc/compiled.cu).
 
-  - the test interpreter of tests/sprite_oracle.py running the games of
+  - the oracle interpreter (oracle/compiled.py) running the games of
     tests/sprite_games.py reproduces the reference's trajectories (tests/golden/sprite_*),
     registers and position attributes included, and raises IndexError where it did;
   - the forms the compiler accepts and the ones it refuses, with the source line;
@@ -14,41 +14,24 @@ PCL_OP_SETFIELD in csrc/compiled.cu).
 
 import ctypes as C
 import os
-import sys
 
 import numpy as np
 import pytest
 
 import golden_cases as gc
-import sprite_oracle
+import registered_games as rg
 import test_kernel_resources as resources
 import trajectory as tj
 from oracle import compiled as ocompiled
-from pycolab_b200 import _lib, compat, compiler, lowering
+from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
 from pycolab_b200.prefab_parts import sprites as b_sprites
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _load(path):
-  """Import a pycolab module through compat, leaving sys.modules as it was."""
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    return compat.load_example(path)
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-
 
 @pytest.fixture(scope='module')
 def games():
-  mod = _load(os.path.join(HERE, 'sprite_games.py'))
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('sprite_games.py')
 
 
 def _world_registers(world, engine, regs, keys, plot_keys):
@@ -84,7 +67,7 @@ def _oracle_trajectory(games, g):
                                       games.PLOT_KEYS[game], keys))
     types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
     assert world.error == 0
-  make = lambda: sprite_oracle.make_world(lowered, words)
+  make = lambda: ocompiled.make_world(lowered, words)
   return lowered, make, on_frame, sprites, registers, types, words
 
 
@@ -296,38 +279,18 @@ def test_lowering_refuses_virtual_position_of_a_plain_sprite(games):
 
 # ------------------------------------------------------------ pcl_bind_code --
 
-def _handle(lib, spec):
-  h = C.c_void_p()
-  assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
-  return h
-
-
-def _bind(lib, h, words):
-  words = np.ascontiguousarray(words, dtype=np.int32)
-  return lib.pcl_bind_code(h, words.ctypes.data, len(words))
-
-
-def _instructions(code, start, end):
-  out, pc = [], start
-  while pc < end:
-    out.append(pc)
-    op = code[pc]
-    pc += 1 + _lib.OPERANDS[op] + (code[pc + 1] if op in (_lib.OP['IN'], _lib.OP['PICK']) else 0)
-  return out
-
-
 def test_bind_code_checks_setfield(games):
   lib = _lib.load()
   lowered = lowering.lower(games.make_bounce(0))
   spec = lowered.make_spec(True)
   code = lowered.code.copy()
   op = lambda name: _lib.OP[name]
-  h = _handle(lib, spec)
+  h = rg.handle(lib, spec)
   try:
-    assert _bind(lib, h, code) == _lib.OK
+    assert rg.bind(lib, h, code) == _lib.OK
     fn = {ch: code[1 + i] for i, ch in enumerate(lowered.sprite_chars + lowered.drape_chars)}
     starts = sorted(set(fn.values())) + [len(code)]
-    span = lambda ch: _instructions(code, fn[ch], starts[starts.index(fn[ch]) + 1])
+    span = lambda ch: ocompiled.instructions(code, fn[ch], starts[starts.index(fn[ch]) + 1])
     find = lambda ch, name: [i for i in span(ch) if code[i] == op(name)][0]
 
     def mutated(*changes):
@@ -352,12 +315,12 @@ def test_bind_code_checks_setfield(games):
     }
     # a TELEPORT pops two: keep the stack balanced so only the opcode is wrong
     for label, words in cases.items():
-      assert _bind(lib, h, words) == _lib.ERR_INVALID, label
-    assert _bind(lib, h, mutated((ball_getr + 1, 4))) == _lib.OK     # AUX2, the fifth
+      assert rg.bind(lib, h, words) == _lib.ERR_INVALID, label
+    assert rg.bind(lib, h, mutated((ball_getr + 1, 4))) == _lib.OK     # AUX2, the fifth
     # the paddle and the ball may not share a function
     shared = code.copy()
     shared[1 + lowered.sprite_chars.index('o')] = fn['P']
-    assert _bind(lib, h, shared) == _lib.ERR_INVALID
+    assert rg.bind(lib, h, shared) == _lib.ERR_INVALID
   finally:
     lib.pcl_destroy(h)
 

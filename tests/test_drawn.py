@@ -14,41 +14,25 @@
 
 import ctypes as C
 import inspect
-import os
 import random
-import sys
 
 import numpy as np
 import pytest
 
 import boundary_sweep
 import golden_cases as gc
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
-from pycolab_b200 import _lib, compat, compiler, lowering
+from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200.prefab_parts import sprites as b_sprites
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 SEQ = (1, 2, 3)
-
-
-def _load(name):
-  """Import a test game module through compat, leaving sys.modules as it was."""
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    return compat.load_example(os.path.join(HERE, name))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
 
 
 @pytest.fixture(scope='module')
 def games():
-  mod = _load('drawn_games.py')
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('drawn_games.py')
 
 
 # ------------------------------------------------------------------ the subset --
@@ -188,7 +172,7 @@ def test_refused_draw_names_class_line_and_construct(update, what):
 
 
 def test_games_without_draws_lower_with_no_streams():
-  mod = _load('compiled_games.py')
+  mod = rg.load('compiled_games.py')
   compiler.register(*mod.CLASSES)
   try:
     for make in mod.GAMES.values():
@@ -297,10 +281,6 @@ def test_python_restatement_matches_random(seed):
 
 # ------------------------------------------------------------ the C boundary --
 
-def _op(name):
-  return _lib.OP[name]
-
-
 def test_rng_slots_are_checked_at_the_boundary(games):
   lib = _lib.load()
   lowered = lowering.lower(games.make_edges(0))
@@ -318,13 +298,9 @@ def test_rng_slots_are_checked_at_the_boundary(games):
     assert lib.pcl_bind_state(h, C.byref(state)) == _lib.ERR_INVALID
     assert lib.pcl_bind_state(h, C.byref(boundary_sweep._full_state())) == _lib.OK
     code = lowered.code.copy()
-
-    def bind(words):
-      words = np.ascontiguousarray(words, dtype=np.int32)
-      return lib.pcl_bind_code(h, words.ctypes.data, len(words))
-    assert bind(code) == _lib.OK
-    at = {name: [i for i in _instructions(code, code[1], len(code)) if code[i] == _op(name)]
-          for name in ('RANDINT', 'RANDCMP', 'PICK')}
+    assert rg.bind(lib, h, code) == _lib.OK
+    at = {name: [i for i in ocompiled.instructions(code, code[1], len(code))
+                 if code[i] == _lib.OP[name]] for name in ('RANDINT', 'RANDCMP', 'PICK')}
     cases = []
     for i in at['RANDINT'][:1]:
       cases += [(i + 1, 2), (i + 1, -1), (i + 2, 3), (i + 2, -1)]    # slot, rule
@@ -336,8 +312,8 @@ def test_rng_slots_are_checked_at_the_boundary(games):
     for where, value in cases:
       bad = code.copy()
       bad[where] = value
-      assert bind(bad) == _lib.ERR_INVALID, (where, value)
-    assert bind(code) == _lib.OK
+      assert rg.bind(lib, h, bad) == _lib.ERR_INVALID, (where, value)
+    assert rg.bind(lib, h, code) == _lib.OK
   finally:
     lib.pcl_destroy(h)
   # a game without draws may not hold a draw
@@ -345,17 +321,6 @@ def test_rng_slots_are_checked_at_the_boundary(games):
   assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
   try:
     assert lib.pcl_bind_state(h, C.byref(boundary_sweep._full_state())) == _lib.OK
-    words = np.ascontiguousarray(lowered.code, dtype=np.int32)
-    assert lib.pcl_bind_code(h, words.ctypes.data, len(words)) == _lib.ERR_INVALID
+    assert rg.bind(lib, h, lowered.code) == _lib.ERR_INVALID
   finally:
     lib.pcl_destroy(h)
-
-
-def _instructions(code, start, end):
-  """Word indices of the instructions in [start, end)."""
-  out, pc = [], start
-  while pc < end:
-    out.append(pc)
-    op = code[pc]
-    pc += 1 + _lib.OPERANDS[op] + (code[pc + 1] if op in (_op('IN'), _op('PICK')) else 0)
-  return out

@@ -2,34 +2,21 @@
 tests/compiled_games.py on the H100, against the reference's trajectories
 (tests/golden/compiled_*.npz) and the oracle interpreter (oracle/compiled.py)."""
 
-import os
-import sys
-
 import numpy as np
 import pytest
 
 import golden_cases as gc
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
-from pycolab_b200 import _lib, compat, compiler, lowering
+from pycolab_b200 import _lib, lowering
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope='module')
 def games():
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    mod = compat.load_example(os.path.join(HERE, 'compiled_games.py'))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-  compiler.register(*mod.CLASSES, mod.OffBoardDrape, mod.DivideDrape)
-  yield mod
-  compiler.unregister(*mod.CLASSES, mod.OffBoardDrape, mod.DivideDrape)
+  yield from rg.registered('compiled_games.py', 'OffBoardDrape', 'DivideDrape')
 
 
 @pytest.mark.parametrize('name', gc.names('compiled_'))

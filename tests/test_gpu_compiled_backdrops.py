@@ -1,40 +1,27 @@
 """GPU tests of Backdrops with registered update() code on the compiled step program
 (csrc/compiled.cu backdrop_step): the games of tests/backdrop_games.py on the H100, against
 the reference's trajectories (tests/golden/backdrop_*.npz, fluvial_*.npz), the hand-written
-PCL_PROG_CLASSICS river and the test interpreter of tests/backdrop_oracle.py."""
-
-import os
-import sys
+PCL_PROG_CLASSICS river and the oracle interpreter (oracle/compiled.py)."""
 
 import numpy as np
 import pytest
 
-import backdrop_oracle
 import golden_cases as gc
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
 from oracle import engine_model as em
 from oracle import sampled_check
-from pycolab_b200 import _lib, compat, compiler, levels, lowering
+from pycolab_b200 import _lib, levels, lowering
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 B, T = 4096, 300
 
 
 @pytest.fixture(scope='module')
 def games():
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    mod = compat.load_example(os.path.join(HERE, 'backdrop_games.py'))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('backdrop_games.py')
 
 
 def _facade_replay(make, g, keys=()):
@@ -134,7 +121,7 @@ def test_backdrop_games_lockstep_against_the_oracle(games, game):
                else None) for e in sample}
   eng.its_showtime()
   n = sampled_check.lockstep(
-      eng, lambda e: backdrop_oracle.make_world(lowered[e % 2], words[e]), sample, actions,
+      eng, lambda e: ocompiled.make_world(lowered[e % 2], words[e]), sample, actions,
       curtains=lowered[0].drape_chars, sprites='P', pad_columns=True, on_step=_backdrop_check)
   assert n == len(sample) * (T + 1)
   if lowered[0].rng_streams:

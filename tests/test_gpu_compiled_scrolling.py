@@ -1,38 +1,25 @@
 """GPU tests of scrolling games on the compiled step program (csrc/compiled.cu): the games
 of tests/scrolling_games.py on the H100, against the reference's trajectories
 (tests/golden/scrolly_*.npz, scrolling_*.npz), the hand-written scrolly_maze kernel and the
-oracle interpreter of tests/scrolling_oracle.py."""
-
-import os
-import sys
+oracle interpreter (oracle/compiled.py)."""
 
 import numpy as np
 import pytest
 
 import golden_cases as gc
-import scrolling_oracle
+import registered_games as rg
 import scrolly_shapes
 import trajectory as tj
+from oracle import compiled as ocompiled
 from oracle import sampled_check
-from pycolab_b200 import _lib, compat, compiler, levels, lowering
+from pycolab_b200 import _lib, levels, lowering
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope='module')
 def games():
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    mod = compat.load_example(os.path.join(HERE, 'scrolling_games.py'))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('scrolling_games.py')
 
 
 def _margins(name):
@@ -154,7 +141,7 @@ def test_batched_lockstep_against_the_oracle(games):
   worlds = {}
 
   def make_world(e):
-    worlds[e] = scrolling_oracle.make_world(lowered[e % 2])
+    worlds[e] = ocompiled.make_world(lowered[e % 2])
     return worlds[e]
   n = sampled_check.lockstep(engine, make_world, env_ids, actions, curtains='#@',
                              sprites='Pabc', pad_columns=True)
@@ -176,6 +163,6 @@ def test_batched_sampler_lockstep_against_the_oracle(games):
   rs = np.random.RandomState(3)
   actions = rs.randint(0, games.N_ACTIONS, size=(T, B)).astype(np.int32)
   env_ids = [0, 1, 7, 2048, 4095]
-  n = sampled_check.lockstep(engine, lambda e: scrolling_oracle.make_world(lowered[e % 2]),
+  n = sampled_check.lockstep(engine, lambda e: ocompiled.make_world(lowered[e % 2]),
                              env_ids, actions, curtains='#*', sprites='Pe', pad_columns=True)
   assert n == len(env_ids) * (T + 1)

@@ -1,40 +1,27 @@
 """GPU tests of plain Sprites on the compiled step program (csrc/compiled.cu): the games of
 tests/sprite_games.py on the H100, against the reference's trajectories
-(tests/golden/sprite_*.npz) and the test interpreter of tests/sprite_oracle.py."""
-
-import os
-import sys
+(tests/golden/sprite_*.npz) and the oracle interpreter (oracle/compiled.py)."""
 
 import numpy as np
 import pytest
 
 import golden_cases as gc
-import sprite_oracle
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
 from oracle import engine_model as em
 from oracle import sampled_check
-from pycolab_b200 import _lib, compat, compiler, lowering, rendering
+from pycolab_b200 import _lib, lowering, rendering
 from pycolab_b200 import things as b_things
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 B, T = 4096, 300
 
 
 @pytest.fixture(scope='module')
 def games():
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    mod = compat.load_example(os.path.join(HERE, 'sprite_games.py'))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('sprite_games.py')
 
 
 def _sprite_rows(env, chars):
@@ -141,7 +128,7 @@ def test_bounce_lockstep_against_the_oracle(games):
   words = {e: ocompiled.seeded_words(lowered[e % 2], seed + e) for e in sample}
   eng.its_showtime()
   n = sampled_check.lockstep(
-      eng, lambda e: sprite_oracle.make_world(lowered[e % 2], words[e]), sample, actions,
+      eng, lambda e: ocompiled.make_world(lowered[e % 2], words[e]), sample, actions,
       curtains='=', sprites='P', pad_columns=True,
       on_step=_plain_check(lambda e: lowered[e % 2]))
   assert n == len(sample) * (T + 1)
@@ -182,7 +169,7 @@ def test_sampler_lockstep_against_the_oracle(games):
     np.testing.assert_array_equal(board, w.board, err_msg=str(t))
     np.testing.assert_array_equal(engine.board[sample[0]].cpu().numpy(), w.board)
   n = sampled_check.lockstep(
-      eng, lambda e: sprite_oracle.make_world(lowered[e % 2]), sample, actions,
+      eng, lambda e: ocompiled.make_world(lowered[e % 2]), sample, actions,
       curtains='#x', sprites='Pw', pad_columns=True,
       on_step=_plain_check(lambda e: lowered[e % 2], render_check))
   assert n == len(sample) * (T + 1)
@@ -199,7 +186,7 @@ def test_only_the_envs_that_fall_latch_index_errors(games):
   lowered = lowering.lower(games.make_fallen())
   eng = batched.BatchedEngine([lowered], batch=n_envs, auto_reset=False)
   falls = np.arange(n_envs) % 3 == 0
-  worlds = [sprite_oracle.make_world(lowered) for _ in range(n_envs)]
+  worlds = [ocompiled.make_world(lowered) for _ in range(n_envs)]
   outs = [w.its_showtime() for w in worlds]
   eng.its_showtime()
   for t in range(6):

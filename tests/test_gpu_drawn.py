@@ -3,36 +3,24 @@ PCL_OP_RANDINT / RANDCMP / PICK): tests/drawn_games.py on the H100, against the
 reference's trajectories (tests/golden/drawn_*.npz) and the oracle
 (oracle/compiled.py)."""
 
-import os
 import random
-import sys
 
 import numpy as np
 import pytest
 
 import golden_cases as gc
+import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
 from oracle import sampled_check
-from pycolab_b200 import _lib, compat, compiler, lowering
+from pycolab_b200 import _lib, lowering
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope='module')
 def games():
-  saved = {k: v for k, v in sys.modules.items() if k == 'pycolab' or k.startswith('pycolab.')}
-  compat.uninstall()
-  try:
-    mod = compat.load_example(os.path.join(HERE, 'drawn_games.py'))
-  finally:
-    compat.uninstall()
-    sys.modules.update(saved)
-  compiler.register(*mod.CLASSES)
-  yield mod
-  compiler.unregister(*mod.CLASSES)
+  yield from rg.registered('drawn_games.py')
 
 
 def global_words(stream):
