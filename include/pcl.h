@@ -141,6 +141,43 @@ typedef enum pcl_program {
                                 rest of the step's logic, and the walker never leaves the board.  pcl_layers and
                                 pcl_export_curtain see the backdrop and the player only: object planes
                                 are d_bits[0] == character */
+  PCL_PROG_CUED_CATCH = 16,  /* examples/research/lp-rnn/cued_catch.py:96-317: sprites 'P' (MazeWalker, impassable '',
+                                confined), 'a' and 'b' (plain Sprites: record VROW / VCOL = the start position),
+                                drape 'Q' (curtain bit rows in d_bits[0]; d_bits_init[0] = the art's 'Q', which
+                                stays in every row outside the bands 1:3, 3:5 and -2: that update() rewrites).
+                                rows <= 32, cols <= 64.  Records: P AUX0 = _trials_till_reward; Q CORNER_R =
+                                phase (0 first, 1 second), CORNER_C = first-phase tick, PRE_R = second-phase cue
+                                choice, PRE_C = second-phase tick, LAST_FRAME = last reset frame (PCL_NEVER =
+                                -inf), AUX0 = trials left, AUX1 = the cue->ball pairings (bit k set: cue k is
+                                'top').  Plot AUX0 = programming_complete, AUX1 = which_ball (0 unset, 1 top,
+                                2 bottom), AUX2 = last_ball_reset (PCL_NEVER = unset), AUX3 = 1 when this step's
+                                reward is a Python float (the normalvariate branch), 0 for an int.
+                                program_arg[0] = reward_sigma != 0: rewards are then float64
+                                (pcl_outputs.d_reward_f64 is required), else int32; [1] =
+                                initial_cue_duration (>= 1), [2] = cue_duration, [3] bit 0 =
+                                always_show_ball_symbol, bit 1 = take the pairings from the template at a
+                                start instead of drawing them (a facade whose Python CueDrape drew them);
+                                [4] / [5] = reward_sigma as float64 bits (lo / hi), [6] / [7] = Lib/random.py's
+                                NV_MAGICCONST as float64 bits (lo / hi).  d_rng is required: u32 [B,
+                                PCL_MT_WORDS], the words of Python's random.Random, continued across steps and
+                                auto-resets (random.sample at a start, randrange(4) per trial, normalvariate
+                                per paid frame).  normalvariate's accept test zz <= -log(u2) uses the device's
+                                double log (1 ulp), so it can decide otherwise than the host's libm only when
+                                zz lies within an ulp of -log(u2) */
+  PCL_PROG_SEQUENCE_RECALL = 17, /* examples/research/lp-rnn/sequence_recall.py:107-317: sprite 'P' (MazeWalker,
+                                impassable '#', confined), drapes 'M' (bit rows in d_bits[0], rewritten
+                                whenever its record's AUX0, the set of covered lights '1'-'4' as bits 0-3,
+                                changes) and '%' (art mask in d_bits_init[1], live rows in d_bits[1], record
+                                AUX0 = cleared).  Backdrop characters are ' #1234' only.  rows <= 32,
+                                cols <= 64.  Plot AUX0 = the program counter over _make_program's list (pc 2k
+                                / 2k+1: OFF / ON of light k; 2L: the pause OFF; 2L+1+2k / 2L+2+2k: SEEK /
+                                EXIT of light k; 4L: QUIT), AUX1 = frames_in_state, AUX2 = timeout_frames
+                                (PCL_SEQUENCE_RECALL_NO_TIMEOUT = inf), AUX3 = the light sequence, light k in
+                                bits 2k..2k+1 (0-3 for '1'-'4').  program_arg = sequence_length L (1-16),
+                                demo_light_on_frames, demo_light_off_frames, max(1, pause_frames).  Rewards
+                                are float64: pcl_outputs.d_reward_f64 is required.  With d_rng bound (u32 [B,
+                                PCL_MT_WORDS], Python random.Random words) the sequence is redrawn at every
+                                (re)start as L calls to random.choice('1234'), else taken from the template */
   PCL_PROG_ORDEAL = 8        /* examples/ordeal.py:74-266: program_arg[0] = PCL_ORDEAL_* chapter;
                                 plot words AUX0 has_sword, AUX1 last_position (row << 16 | col,
                                 -1 unset), AUX2 next_chapter chosen on the device, AUX3 prior chapter */
@@ -154,6 +191,9 @@ enum { PCL_ORDEAL_NEXT_UNSET = -1, PCL_ORDEAL_NEXT_NONE = 0,
 
 /* PCL_PROG_T_MAZE: program_arg[2] for timeout_frames = -1 (never times out). */
 #define PCL_T_MAZE_NO_TIMEOUT 0x7fffffff
+
+/* PCL_PROG_SEQUENCE_RECALL: plot AUX2 for timeout_frames = inf (never times out). */
+#define PCL_SEQUENCE_RECALL_NO_TIMEOUT 0x7fffffff
 
 /* PCL_PROG_CLASSICS: pcl_spec.program_arg[0] selects the rule set; the games
  * pay float rewards (1.0, -1.0, -100.0, 100.0) which d_reward carries as the

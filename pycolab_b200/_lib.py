@@ -45,7 +45,9 @@ PROG_BETTER_SCROLLY, PROG_CLASSICS, PROG_APERTURE, PROG_ORDEAL, PROG_HELLO = 5, 
 PROG_APPREHEND, PROG_SHOCKWAVE, PROG_T_MAZE = 10, 11, 12
 PROG_COMPILED = 14
 PROG_BOX_WORLD = 15
+PROG_CUED_CATCH, PROG_SEQUENCE_RECALL = 16, 17
 T_MAZE_NO_TIMEOUT = 0x7fffffff   # program_arg[2] for timeout_frames = inf
+SEQUENCE_RECALL_NO_TIMEOUT = 0x7fffffff   # plot AUX2 for timeout_frames = inf
 ORDEAL_NEXT_UNSET, ORDEAL_NEXT_NONE, ORDEAL_CASTLE, ORDEAL_CAVERN, ORDEAL_KANSAS = -1, 0, 1, 2, 3
 CLASSIC_FOUR_ROOMS, CLASSIC_CLIFF_WALK, CLASSIC_CHAIN_WALK, CLASSIC_FLUVIAL = 0, 1, 2, 3
 

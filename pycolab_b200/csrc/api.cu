@@ -91,6 +91,8 @@ const struct {
     {PCL_PROG_T_MAZE, &pcl::kTMaze},
     {PCL_PROG_COMPILED, &pcl::kCompiled},
     {PCL_PROG_BOX_WORLD, &pcl::kBoxWorld},
+    {PCL_PROG_CUED_CATCH, &pcl::kCuedCatch},
+    {PCL_PROG_SEQUENCE_RECALL, &pcl::kSequenceRecall},
 };
 
 // The descriptor of program `id`, or nullptr for an id this build does not know.

@@ -115,7 +115,8 @@ struct Program {
   int (*derive)(const pcl_spec&, const pcl_state&, int batch, StepParams* base, void** owned);
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
-    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld;
+    kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld,
+    kCuedCatch, kSequenceRecall;
 
 // Host-side helpers of the programs' check_spec.
 inline bool chars_are(const uint8_t* got, int n, const char* want) {

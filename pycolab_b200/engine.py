@@ -139,6 +139,11 @@ class Engine(object):
       # would: the device continues their words and hands them back after every step.
       if lowered.needs_rng:
         rng_states = np.concatenate([_global_words(s) for s in lowered.rng_streams])[None]
+      if lowered.template_draws is not None:
+        # cued_catch.py:235 drew in the drape's constructor, which has already run: the
+        # device takes that draw from the template and continues the stream in update().
+        index, bit = lowered.template_draws
+        lowered.program_arg[index] |= bit
     elif 'python' in lowered.rng_streams:
       # apprehend.py:103 draws in the sprite's constructor, which has already run
       # (from the global `random`, as upstream): the device takes the drawn value
@@ -180,6 +185,8 @@ class Engine(object):
     value = result.reward[0]
     value = float(value) if self._batched.game.float_reward else int(value)
     reward = self._batched.game.reward_type(value) if int(result.has_reward[0]) else None
+    if reward is not None and self._batched.game.python_reward is not None:
+      reward = self._batched.game.python_reward(self, value)
     discount = float(result.discount[0])
     self._game_over = bool(int(result.done[0]))
     self._sync_things()

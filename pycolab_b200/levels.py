@@ -348,3 +348,37 @@ def box_world_level(seed, grid_size=12, solution_length=(1, 2, 3, 4),
     if level is not None:
       return level
   raise RuntimeError('Could not generate game in MAX_GENERATION_TRIES tries.')
+
+
+def cued_catch_art(rows=7, cols=12, player=(1, 3), balls=((1, 8), (2, 8)), cue_cells=()):
+  """A research/lp-rnn/cued_catch.py board of `rows` x `cols` (the device takes up to
+  32 x 64): the player 'P' and the balls 'a' / 'b' at the given cells, and 'Q' at
+  `cue_cells`.  The defaults are the reference's 7 x 12 layout.  The player only moves
+  between rows 1 and 2 (cued_catch.py:138-141), and a ball left of the player's column
+  is put back at its start (:190-192)."""
+  art = np.full((rows, cols), ord(' '), dtype=np.uint8)
+  for r, c in cue_cells:
+    art[r, c] = ord('Q')
+  art[player] = ord('P')
+  art[balls[0]] = ord('a')
+  art[balls[1]] = ord('b')
+  return _to_art(art)
+
+
+def sequence_recall_art(rows=17, cols=21):
+  """A research/lp-rnn/sequence_recall.py board of `rows` x `cols` (9 x 9 up to 32 x 64):
+  a '#' ring, the player 'P' in the middle inside a 3 x 3 start box '%', and the four light
+  pads, each one step past a free cell from the box: '2' above, '4' below, '1' left and '3'
+  right of it.  Moving straight from the player's start enters a pad in three steps."""
+  assert 9 <= rows and 9 <= cols
+  cr, cc = rows // 2, cols // 2
+  art = np.full((rows, cols), ord(' '), dtype=np.uint8)
+  art[0, :] = art[-1, :] = art[:, 0] = art[:, -1] = ord('#')
+  w = min(3, cc - 2)
+  art[1:cr - 2, cc - w:cc + w + 1] = ord('2')
+  art[cr + 3:rows - 1, cc - w:cc + w + 1] = ord('4')
+  art[cr - 1:cr + 2, 1:cc - 2] = ord('1')
+  art[cr - 1:cr + 2, cc + 3:cols - 1] = ord('3')
+  art[cr - 1:cr + 2, cc - 1:cc + 2] = ord('%')
+  art[cr, cc] = ord('P')
+  return _to_art(art)

@@ -65,6 +65,12 @@ LOWERED_CLASSES = {
     ('t_maze', 'SpeckleDrape'): 't_maze.speckle',
     ('t_maze', 'TeleporterDrape'): 't_maze.teleporter',
     ('t_maze', 'GoalDrape'): 't_maze.goal',
+    ('cued_catch', 'PlayerSprite'): 'cued_catch.player',
+    ('cued_catch', 'BallSprite'): 'cued_catch.ball',
+    ('cued_catch', 'CueDrape'): 'cued_catch.cue',
+    ('sequence_recall', 'PlayerSprite'): 'sequence_recall.player',
+    ('sequence_recall', 'MaskDrape'): 'sequence_recall.mask',
+    ('sequence_recall', 'WaitForSeekDrape'): 'sequence_recall.wait',
     ('box_world', 'PlayerSprite'): 'box_world.player',
     ('box_world', 'BoxThing'): 'box_world.thing',
     ('box_world', 'GemDrape'): 'box_world.gem',
@@ -85,6 +91,12 @@ LOWERED_CLASSES = {
 # Backdrop subclasses whose update() has a device counterpart.
 LOWERED_BACKDROPS = {
     ('fluvial_natation', 'RiverBackdrop'): 'river',
+}
+
+# Module-level functions a device program restates besides the entities' update():
+# sequence_recall's restart draw is _make_program's.
+LOWERED_FUNCTIONS = {
+    ('sequence_recall', '_make_program'),
 }
 
 def source_fingerprint(text):
@@ -226,7 +238,12 @@ class LoweredGame(object):
                                 # in this order: NumPy's legacy RandomState ('numpy') or
                                 # Python's `random` ('python')
     self.rng_from_globals = False  # the facade hands the global generators of rng_streams to
-                                # the device and takes them back after every step (compiled)
+                                # the device and takes them back after every step (compiled,
+                                # cued_catch)
+    self.template_draws = None  # (program_arg index, bit) the facade sets when its Python
+                                # constructors have drawn already: the device then takes those
+                                # draws from the template at a start and draws only in steps
+                                # (cued_catch); a batched engine leaves it clear and draws both
     self.actions_per_env = 1    # action words per env and step
     self.backdrop_chars = ''
     self.drape_kind = None      # per drape: 1 = Scrolly (fixture and compiled programs)
@@ -247,6 +264,8 @@ class LoweredGame(object):
     self.layers = None          # (BatchedEngine, chars) -> bool [B, len(chars), rows, cols]
     self.sync = None            # (Engine): mirror program-private device state into the
                                 # Python objects after a step
+    self.python_reward = None   # (Engine, value): the reference's reward of a step that has one,
+                                # where its Python type varies by step (cued_catch: int or float)
     self.action_row = None      # (Engine, facade actions) -> the env's action words
     self.code = None            # i32 bytecode words (pcl_bind_code) of the compiled program
     self.registers = {}         # compiled: char -> [(attribute, type)] in register order, type

@@ -24,7 +24,7 @@ def main():
   from pycolab_b200 import batched, dist as pdist, levels, lowering
   from pycolab_b200.games import (aperture, better_scrolly_maze, extraterrestrial_marauders,
                                   apprehend, fixtures, fluvial_natation, hello_world, ordeal,
-                                  box_world, shockwave, t_maze,
+                                  box_world, cued_catch, sequence_recall, shockwave, t_maze,
                                   scrolly_maze, warehouse_manager)
   from pycolab_b200.games.classics import chain_walk, cliff_walk, four_rooms
   rs = np.random.RandomState(0)
@@ -121,6 +121,13 @@ def main():
   run('box_world_step 32x32', [box_world.make_game(30, (1, 2, 3, 4), (0, 1, 2, 3, 4), (0,), 1,
                                                    random_state=np.random.RandomState(4),
                                                    max_num_steps=10)], 5, 6, steps=25)
+  run('cued_catch_step (device RNG)', [cued_catch.make_game(1, 2, 4, True, 0.5, 1,
+                                                           art=levels.cued_catch_art(5, 14))],
+      6, 3, steps=40)
+  for shape in ((9, 13), (32, 64)):
+    run('sequence_recall_step %dx%d' % shape,
+        [sequence_recall.make_game(3, 1, 1, 0, 30, art=levels.sequence_recall_art(*shape))],
+        6, 6, steps=40)
   pattern = rs.random_sample((17, 23)) < 0.2
   fx = fixtures.make_game(['           ', '   P       ', '      q    ', '           ',
                            '           ', '           '], ' ',
