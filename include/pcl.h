@@ -419,7 +419,12 @@ typedef struct pcl_outputs {
   uint8_t* d_board;       /* u8 [B, rows, pitch]; Observation.board.  PCL_PROG_FIXTURE reads the
                              board of the LAST render back from here at the next step (its
                              entities may test any character, engine.py:725-735): pass the same
-                             d_board to consecutive steps of a handle running that program. */
+                             d_board to consecutive steps of a handle running that program.
+                             PCL_PROG_SCROLLY_MAZE repaints only the cells that can have changed
+                             when d_board holds the env's last render (the buffer of the handle's
+                             previous step or reset) and neither window scrolls: a host that writes
+                             into a step's board buffer passes a different buffer to the next step
+                             or reset, or calls pcl_bind_state again, which paints every board. */
   int32_t* d_reward;      /* i32 [B]; summed reward (plot.py:201-214), 0 if none */
   uint8_t* d_has_reward;  /* u8 [B]; 0 = reference returned reward None */
   float*   d_discount;    /* f32 [B]; 1.0 running / 0.0 terminated unless a directive said otherwise

@@ -39,6 +39,9 @@ struct pcl_handle {
   // since it was built
   void* derived_dev;
   int derive_stale;
+  // StepParams::board_epoch: the board buffer of the last launch, and its epoch
+  const uint8_t* last_board;
+  uint32_t board_epoch;
 };
 
 namespace {
@@ -156,8 +159,13 @@ bool live_backdrop(const pcl_spec& s) {
   return s.program == PCL_PROG_COMPILED && s.program_arg[4] != 0;
 }
 
-int launch(pcl_handle* h, const StepParams& p, cudaStream_t stream) {
+int launch(pcl_handle* h, StepParams p, cudaStream_t stream) {
   if (!h->program->launch) return PCL_ERR_UNSUPPORTED;
+  if (p.out.d_board != h->last_board) {
+    h->last_board = p.out.d_board;
+    h->board_epoch += 1;
+  }
+  p.board_epoch = h->board_epoch;
   const cudaError_t e = h->program->launch(p, stream);
   if (e != cudaSuccess) return cuda_failed(h, e, "step kernel launch");
   h->launches += 1;              // only launches that were accepted count
@@ -292,6 +300,8 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->backdrop_live = nullptr;
   h->derived_dev = nullptr;
   h->derive_stale = 0;
+  h->last_board = nullptr;
+  h->board_epoch = 0;
   *out = h;
   return PCL_OK;
 }

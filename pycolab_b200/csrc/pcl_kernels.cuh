@@ -57,6 +57,13 @@ struct StepParams {
   // come from: per level, or one copy when the stride is 0).
   const uint32_t* derived[2];
   int64_t derived_bstride[2];    // in words
+  // Program::derive: per-env words the program keeps from one launch to the next (also in
+  // the derived allocation, so every pcl_bind_state starts them afresh), or NULL.
+  // scrolly_maze: what the board of each env was last drawn from.
+  int32_t* render_key;
+  // The handle's count of board-buffer changes: a launch whose out.d_board differs from
+  // the previous launch's gets the next value, so each value names one buffer.
+  uint32_t board_epoch;
 };
 
 // Launch with the programmatic-stream-serialisation attribute (the kernel calls

@@ -71,6 +71,23 @@
 // the coin patch rows), a pick-up sets its group's bit, and an auto-reset restart
 // copies back only the dirty groups (the reloaded record brings the mask back to 0).
 // A host that writes an env's coin pattern directly sets that env's aux2 to -1.
+//
+// Delta rendering: with the example's margins a window scrolls only when the player comes
+// within 2 rows or 3 columns of the board's edge, which the bench workload never did in
+// 19 200 env-steps (tools/scroll_census.py).  Then the new board differs from the last one
+// in at most the sprites' old and new cells, the old and new stale coin and a picked-up
+// coin.  Each env's render key (StepParams::render_key, built by derive(), invalid after
+// every pcl_bind_state) records what its last render was drawn from: the frame, the board
+// buffer's epoch (StepParams::board_epoch), both corners, each sprite's visible cell, the
+// stale coin and the coin mask.  A step that is no restart or reset, whose records match
+// the key, whose mask is not -1 and whose windows stay where they are after group 0 takes
+// the delta path: it stages nothing; in the patch trip, spare loads fetch the 3x3 coin
+// bits and backdrop bytes around each sprite's start cell (the 5x5 wall patches cover the
+// walls); after group 2 one lane per candidate cell composes its final value and stores
+// that byte.  If '@' then issues its own order, or a candidate lies outside every loaded
+// neighbourhood, the warp stages the full paint's copies there and paints in full.  Every
+// path that paints writes the key; frozen envs touch neither board nor key.  A host that
+// writes into a step's board buffer passes another buffer or binds again (include/pcl.h).
 #include <algorithm>
 #include <new>
 
@@ -131,13 +148,45 @@ __host__ __device__ constexpr int window_words(int W) {
 // segments (pitch >= W, so W <= 64 too).
 __host__ __device__ constexpr bool narrow_board(int pitch) { return pitch <= 64; }
 
-__host__ __device__ constexpr size_t warp_smem_bytes(int H, int W, int pitch) {
-  // records, backdrop tile, two window rows of window_words(W) per board row, and one
-  // word per 16-cell segment.  On narrow boards the segment words (pitch / 16 <= 4 per
-  // row) take the place of the wall window rows (4 words per row), which are dead by then.
-  return kRecWords * 4 + (size_t)H * pitch +
-         2 * ((((size_t)H * window_words(W) * 4) + 15) & ~(size_t)15) +
+// Render key (see "Delta rendering"): words per env in the handle's key array, and the
+// words in use.  Word i is key_word(rec, i, epoch) of the records the board was drawn from:
+// words 0..7 are record words (frame, both corners, the stale coin cell, the coin mask),
+// word 8 the board epoch, words 9..12 each sprite's cell row * pitch + col, or -1 if hidden.
+constexpr int kKeyStride = 16;
+enum { kKeyRecWords = 8, kKeyEpoch = 8, kKeySprites = 9, kKeyWords = kKeySprites + kS };
+// Record offsets of key words 0..7, one byte each.
+constexpr uint64_t kKeyRec =
+    (uint64_t)(48 + PCL_P_FRAME) | (uint64_t)(32 + PCL_D_CORNER_R) << 8 |
+    (uint64_t)(32 + PCL_D_CORNER_C) << 16 | (uint64_t)(40 + PCL_D_CORNER_R) << 24 |
+    (uint64_t)(40 + PCL_D_CORNER_C) << 32 | (uint64_t)(40 + PCL_D_AUX0) << 40 |
+    (uint64_t)(40 + PCL_D_AUX1) << 48 | (uint64_t)(40 + PCL_D_AUX2) << 56;
+static_assert(kKeyWords <= kKeyStride, "the render key outgrew its slot");
+
+// Delta rendering's scratch words, in the (then idle) staging area of the warp: the 5x5
+// wall patch rows (one per patch lane), the 3x3 coin rows and backdrop rows around each
+// sprite's start cell, and what the last render drew from the records.
+enum {
+  kNbWall = 0,                     // 20 words: rowbits of patch lanes 0..19
+  kNbCoin = 32,                    // 12 words: 3 coin bits per row, sprite s row k at 3 s + k
+  kNbBackdrop = 44,                // 12 words: 3 backdrop bytes per row, likewise
+  kNbStart = 56,                   // 4 words per sprite: vrow, vcol, and row, col (-1: hidden)
+  kNbStale = kNbStart + 4 * kS,    // 2 words: the stale coin cell (AUX0, AUX1)
+  kNbWords = (kNbStale + 2 + 3) & ~3   // whole 16-byte units: warp regions stay 16-byte aligned
+};
+
+__host__ __device__ constexpr size_t staging_bytes(int H, int W, int pitch) {
+  // backdrop tile, two window rows of window_words(W) per board row, and one word per
+  // 16-cell segment.  On narrow boards the segment words (pitch / 16 <= 4 per row) take
+  // the place of the wall window rows (4 words per row), which are dead by then.
+  return (size_t)H * pitch + 2 * ((((size_t)H * window_words(W) * 4) + 15) & ~(size_t)15) +
          (narrow_board(pitch) ? 0 : (((size_t)H * (pitch >> 2) + 15) & ~(size_t)15));
+}
+
+__host__ __device__ constexpr size_t warp_smem_bytes(int H, int W, int pitch) {
+  // records, then the staging area; the delta path's scratch (kNbWords) reuses the
+  // staging area, which tiny boards pad to its size.
+  return kRecWords * 4 + (staging_bytes(H, W, pitch) > (size_t)kNbWords * 4
+                             ? staging_bytes(H, W, pitch) : (size_t)kNbWords * 4);
 }
 
 // Programmatic dependent launch: let the next kernel of the stream begin its
@@ -172,8 +221,8 @@ __device__ __align__(16) const SelTable g_sel = make_sel_table();
 // at each phase boundary, and of %globaltimer (ns) at entry and exit, to
 // g_stamps[env].  Differences of these 32-bit stamps, taken modulo 2^32, are exact.
 // Without the switch PCL_STAMP expands to nothing and the kernel is the production one.
-// The stamp build needs 8 bytes of spill at 64 registers; tools/step_phases.py reports
-// its step time beside the production build's.
+// The stamp build also fits 64 registers without spills; tools/step_phases.py reports its
+// step time beside the production build's.
 #ifdef PCL_STEP_STAMPS
 constexpr int kStampEnvs = 8192;
 enum {
@@ -212,6 +261,8 @@ constexpr size_t kMaxBlockSmem = 227 * 1024 - 2048;
 static_assert(8 * (kWarpsPerBlock * (warp_smem_bytes(64, 64, 64) + sizeof(SelTable)) + 1024) <=
                   228 * 1024,
               "a 64x64 scrolly_maze block no longer fits 8 times per SM");
+static_assert(warp_smem_bytes(1, 1, 16) == kRecWords * 4 + kNbWords * 4,
+              "delta rendering's scratch must fit a warp's region on the smallest board");
 static_assert(kMaxBlockSmem + kWarpsPerBlock * sizeof(SelTable) == 227 * 1024,
               "kMaxBlockSmem must leave room for the static selector tables");
 
@@ -289,6 +340,11 @@ __device__ __forceinline__ void scrolly_move_p(Drape& d, const ScrollyCfg& cfg, 
 // The env's own coin pattern, its level's template and its level's wall pattern.  All are
 // recomputed from the launch parameters where they are used: at 64 registers, no pointer
 // to any of them stays live through the step.
+// The index of the env's static level data.  Re-read where it is used after the patch
+// trip: at 64 registers the 64-bit index is not held through groups 1 and 2 either.
+__device__ __forceinline__ int64_t level_of(const StepParams& p, int env) {
+  return p.st.d_level ? p.st.d_level[env] : env;
+}
 __device__ __forceinline__ const uint32_t* level_walls(const StepParams& p, int64_t lvl) {
   return p.st.d_pattern[0] + lvl * p.st.pattern_bstride[0];
 }
@@ -297,6 +353,15 @@ __device__ __forceinline__ uint32_t* env_coins(const StepParams& p, int env) {
 }
 __device__ __forceinline__ const uint32_t* level_coins(const StepParams& p, int64_t lvl) {
   return p.st.d_pattern_init[1] + lvl * p.st.pattern_init_bstride[1];
+}
+
+// Word i of the render key of records `rec` (kKey*), for a board of row pitch `pitch` in
+// the buffer of epoch `epoch`.  Lane i computes word i: no branch on i.
+__device__ __forceinline__ int32_t key_word(const int32_t* rec, int i, uint32_t epoch, int pitch) {
+  const int32_t r = rec[i < kKeyRecWords ? (int)((kKeyRec >> (8 * i)) & 0xffu) : 0];
+  const int32_t* q = rec + min(max(i - kKeySprites, 0), kS - 1) * PCL_SPRITE_WORDS;
+  const int32_t cell = q[PCL_S_FLAGS] & 1 ? q[PCL_S_ROW] * pitch + q[PCL_S_COL] : -1;
+  return i < kKeyRecWords ? r : i == kKeyEpoch ? (int32_t)epoch : cell;
 }
 
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
@@ -339,12 +404,14 @@ scrolly_maze_step(const StepParams p) {
     cp_async_wait_all();
     return;
   }
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
+  const int64_t lvl = level_of(p, env);     // index of static level data
 
   // The env's action word does not depend on the records either: issue its load now,
   // beside theirs, instead of one memory round trip later (it is only USED if the env
   // neither restarts nor is frozen).
   int action = env_action(p, env);
+  // The render key, in the same trip as the records.
+  const int32_t key = lane < kKeyWords ? p.render_key[(int64_t)env * kKeyStride + lane] : 0;
   // ---- 1. records -> smem (coalesced) ------------------------------------
   rec[lane] = p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane];
   rec[32 + lane] = lane < 16 ? p.st.d_drapes[(int64_t)env * 2 * PCL_DRAPE_WORDS + lane]
@@ -367,6 +434,9 @@ scrolly_maze_step(const StepParams p) {
     cp_async_wait_all();
     return;
   }
+  // The board in d_board was drawn from these very records (see "Delta rendering").
+  const bool key_ok = __all_sync(PCL_FULL, lane >= kKeyWords ||
+                                               key == key_word(rec, lane, p.board_epoch, pitch));
   if (restart) {
     const PlotCarry carry = plot_carry(rec + 48, true);
     // Groups of the coin pattern to restore, read before the record is reloaded: the
@@ -484,6 +554,34 @@ scrolly_maze_step(const StepParams p) {
       rowbits = __funnelshift_r(lo, hi, c_first & 31) & 31u;
     }
   }
+  // Delta rendering: neither window moves and the board is this env's last render.  In
+  // the same trip, the 3x3 coin bits (lanes 0..11) and backdrop bytes (lanes 12..23)
+  // around each sprite's start cell, row k of sprite s at lane 3 s + k (+ 12).
+  bool delta = key_ok && !restart && wr == rec[32 + PCL_D_CORNER_R] &&
+               wc == rec[32 + PCL_D_CORNER_C] && cr_pred == rec_coins[PCL_D_CORNER_R] &&
+               cc_pred == rec_coins[PCL_D_CORNER_C] && rec_coins[PCL_D_AUX2] != -1;
+  unsigned nb = 0;
+  if (delta && lane < 24) {
+    const int s = (lane < 12 ? lane : lane - 12) / 3;
+    const int vr = rec[s * PCL_SPRITE_WORDS + PCL_S_VROW], vc = rec[s * PCL_SPRITE_WORDS + PCL_S_VCOL];
+    const int r = vr + (lane < 12 ? lane : lane - 12) - 3 * s - 1;
+    if ((unsigned)r < (unsigned)H) {
+      if (lane < 12) {
+        const int pr = cr_pred + r, c_first = cc_pred + vc - 1, wi = c_first >> 5;
+        const uint32_t* row = ((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> coin_group_shift(p.PH))) & 1u
+                                  ? env_coins(p, env) : level_coins(p, lvl);
+        row += (int64_t)pr * PWW;
+        const uint32_t lo = (unsigned)wi < (unsigned)PWW ? row[wi] : 0u;
+        const uint32_t hi = (unsigned)(wi + 1) < (unsigned)PWW ? row[wi + 1] : 0u;
+        nb = __funnelshift_r(lo, hi, c_first & 31) & 7u;
+      } else {
+        const uint8_t* bd = p.st.d_backdrop + lvl * p.st.backdrop_bstride + (int64_t)r * pitch;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+          if ((unsigned)(vc - 1 + j) < (unsigned)W) nb |= (unsigned)__ldg(bd + vc - 1 + j) << (8 * j);
+      }
+    }
+  }
   // Pattern columns past PW are zero padding and negative ones read as zero, so
   // the wall bits need no further masking; coin bits are masked to the board.
   unsigned field = 0;                        // my walker's 5x5 patch, bit (dr+2)*5 + dc+2
@@ -500,53 +598,69 @@ scrolly_maze_step(const StepParams p) {
     coin9 |= (__shfl_sync(PCL_FULL, rowbits, 23) & 1u) << 9;
   }
   PCL_STAMP(kStPatch);
+  uint32_t* s_nb = reinterpret_cast<uint32_t*>(s_bd);   // delta rendering's scratch
   // The bulk copies: the backdrop tile and the two windows -> smem, no registers held.
   // They are first needed after group 2, so they are issued only now: issued ahead of
   // the record and patch loads (as before), every warp's 6 KB of copies queued in front of
   // those two dependent round trips, and in a full wave each trip took 2-4x as long as
-  // in a lone warp (tools/step_phases.py; DESIGN.md section 5).
-  {
-    const uint8_t* src = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * 16;
-    uint8_t* dst = s_bd + lane * 16;
-    const int n16 = (H * pitch) >> 4;
+  // in a lone warp (tools/step_phases.py; DESIGN.md section 5).  Delta rendering stages
+  // nothing unless it falls back to the full paint after group 2.
+  auto stage = [&](int64_t lvl) {
+    {
+      const uint8_t* src = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * 16;
+      uint8_t* dst = s_bd + lane * 16;
+      const int n16 = (H * pitch) >> 4;
 #pragma unroll 4
-    for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
-  }
-  // Both windows come from the row-blocked copies (see "Row-blocked windows"): the H rows
-  // of a window are one contiguous run there.  Coin window rows of clean groups come from
-  // the level's template (see "Coin groups"): per env that is L2 traffic shared by the
-  // level's envs instead of DRAM of its own.
-  {
-    const int gs = coin_group_shift(p.PH);
-    const uint32_t* wsrc =
-        p.derived[0] + lvl * p.derived_bstride[0] + ((int64_t)(we >> 1) * p.PH + wr) * nw;
-    const uint32_t* csrc =
-        p.derived[1] + lvl * p.derived_bstride[1] + ((int64_t)(ce >> 1) * p.PH + cr_pred) * nw;
-    const int hw = nw >> 1, nhalf = H * hw;  // 8-byte halves per window row
-    if (narrow) {                            // one 16-byte row per copy
+      for (int i = lane; i < n16; i += 32, src += 512, dst += 512) cp_async16(dst, src);
+    }
+    // Both windows come from the row-blocked copies (see "Row-blocked windows"): the H rows
+    // of a window are one contiguous run there.  Coin window rows of clean groups come from
+    // the level's template (see "Coin groups"): per env that is L2 traffic shared by the
+    // level's envs instead of DRAM of its own.
+    {
+      const int gs = coin_group_shift(p.PH);
+      const uint32_t* wsrc =
+          p.derived[0] + lvl * p.derived_bstride[0] + ((int64_t)(we >> 1) * p.PH + wr) * nw;
+      const uint32_t* csrc =
+          p.derived[1] + lvl * p.derived_bstride[1] + ((int64_t)(ce >> 1) * p.PH + cr_pred) * nw;
+      const int hw = nw >> 1, nhalf = H * hw;  // 8-byte halves per window row
+      if (narrow) {                            // one 16-byte row per copy
 #pragma unroll 1
-      for (int r = lane; r < H; r += 32) {
-        cp_async16(s_wall + r * 4, wsrc + r * 4);
-        if (!(((unsigned)rec_coins[PCL_D_AUX2] >> ((cr_pred + r) >> gs)) & 1u))
-          cp_async16(s_coin + r * 4, csrc + r * 4);
+        for (int r = lane; r < H; r += 32) {
+          cp_async16(s_wall + r * 4, wsrc + r * 4);
+          if (!(((unsigned)rec_coins[PCL_D_AUX2] >> ((cr_pred + r) >> gs)) & 1u))
+            cp_async16(s_coin + r * 4, csrc + r * 4);
+        }
+      } else {
+#pragma unroll 1
+        for (int i = lane; i < nhalf; i += 32) {
+          const int pr = cr_pred + i / hw;
+          cp_async8(s_wall + i * 2, wsrc + i * 2);
+          if (!(((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u))
+            cp_async8(s_coin + i * 2, csrc + i * 2);
+        }
       }
-    } else {
+      if (rec_coins[PCL_D_AUX2] != 0) {
 #pragma unroll 1
-      for (int i = lane; i < nhalf; i += 32) {
-        const int pr = cr_pred + i / hw;
-        cp_async8(s_wall + i * 2, wsrc + i * 2);
-        if (!(((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u))
-          cp_async8(s_coin + i * 2, csrc + i * 2);
+        for (int i = lane; i < nhalf; i += 32) {
+          const int r = narrow ? i >> 1 : i / hw, k = (i - r * hw) * 2, pr = cr_pred + r;
+          if (((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u)
+            cp_async8(s_coin + i * 2, env_coins(p, env) + (int64_t)pr * PWW + ce + k);
+        }
       }
     }
-    if (rec_coins[PCL_D_AUX2] != 0) {
-#pragma unroll 1
-      for (int i = lane; i < nhalf; i += 32) {
-        const int r = narrow ? i >> 1 : i / hw, k = (i - r * hw) * 2, pr = cr_pred + r;
-        if (((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> gs)) & 1u)
-          cp_async8(s_coin + i * 2, env_coins(p, env) + (int64_t)pr * PWW + ce + k);
-      }
+  };
+  if (delta) {
+    if (lane < 20) s_nb[kNbWall + lane] = rowbits;
+    if (lane < 24) s_nb[kNbCoin + lane] = nb;
+    if (lane < 4) {
+      uint32_t* q = s_nb + kNbStart + 4 * lane;
+      q[0] = mine.vrow; q[1] = mine.vcol;
+      q[2] = visible(mine) ? mine.row : -1; q[3] = mine.col;
     }
+    if (lane < 2) s_nb[kNbStale + lane] = rec_coins[PCL_D_AUX0 + lane];
+  } else {
+    stage(lvl);
   }
 
   // ---- 4a. update group 1: patrollers a, b, c then P, ONE WALKER PER LANE ----
@@ -578,7 +692,7 @@ scrolly_maze_step(const StepParams p) {
       if (pr < 0) pr += p.PH;
       if (pc < 0) pc += p.PW;
       if ((unsigned)pr < (unsigned)p.PH && (unsigned)pc < (unsigned)p.PW)
-        next_to_wall = bit_at(level_walls(p, lvl) + (int64_t)pr * PWW, pc);
+        next_to_wall = bit_at(level_walls(p, level_of(p, env)) + (int64_t)pr * PWW, pc);
       else
         my_err |= PCL_ENV_ERR_INDEX;
     }
@@ -684,16 +798,82 @@ scrolly_maze_step(const StepParams p) {
     r[PCL_P_ORDER_FRAME] = plot.order_frame; r[PCL_P_EGO_MASK] = plot.ego_mask;
     r[PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
-    // The coin window was staged before the pick-up: clear the bit there too.  The
-    // pick-up's group of the env's pattern now differs from the template.
-    if (picked_r >= 0) {
-      rec[32 + PCL_DRAPE_WORDS + PCL_D_AUX2] |= 1 << (picked_r >> coin_group_shift(p.PH));
-      const int r2 = picked_r - cr_pred, b = picked_c - (ce << 5);
-      if ((unsigned)r2 < (unsigned)H && (unsigned)b < (unsigned)(nw * 32))
-        s_coin[r2 * nw + (b >> 5)] &= ~(1u << (b & 31));
-    }
+    // The pick-up's group of the env's pattern now differs from the template.
+    if (picked_r >= 0) rec[32 + PCL_DRAPE_WORDS + PCL_D_AUX2] |= 1 << (picked_r >> coin_group_shift(p.PH));
   }
   const int cr = coins.corner_r, cc = coins.corner_c;
+
+  // ---- 4c. delta rendering: store the final value of every cell that can have changed.
+  // Candidates, one per lane: the old (lanes 0..3) and new (4..7) cells of the sprites,
+  // the old (8) and new (9) stale coin, and the coin picked up (10).  With both windows
+  // where they were, every other cell shows the walls, coins, backdrop and sprites it
+  // showed in the last render.  A cell listed twice gets the same value twice.  A moved
+  // '@' window or a candidate outside the loaded neighbourhoods falls back to the full
+  // paint, staged only now.
+  if (delta) {
+    __syncwarp();                            // the new records are in rec
+    bool fall = cr != cr_pred || cc != cc_pred;
+    int cell = -1;
+    uint32_t val = 0;
+    if (!fall) {
+      int r = -1, c = -1;
+      if (lane < 4) {
+        r = (int)s_nb[kNbStart + 4 * lane + 2]; c = (int)s_nb[kNbStart + 4 * lane + 3];
+      } else if (lane < 8) {
+        const int32_t* s = rec + (lane - 4) * PCL_SPRITE_WORDS;
+        if (s[PCL_S_FLAGS] & 1) { r = s[PCL_S_ROW]; c = s[PCL_S_COL]; }
+      } else if (lane == 8) {
+        r = (int)s_nb[kNbStale]; c = (int)s_nb[kNbStale + 1];
+      } else if (lane == 9) {
+        r = rec_coins[PCL_D_AUX0]; c = rec_coins[PCL_D_AUX1];
+      } else if (lane == 10 && picked_r >= 0) {
+        r = picked_r - cr; c = picked_c - cc;
+      }
+      bool outside = false;
+      if (r >= 0) {
+        int s = -1, dr = 0, dc = 0;          // a sprite whose 3x3 holds (r, c), at (dr, dc)
+#pragma unroll
+        for (int t = kS - 1; t >= 0; --t) {
+          const int a = r - (int)s_nb[kNbStart + 4 * t] + 1, b = c - (int)s_nb[kNbStart + 4 * t + 1] + 1;
+          if ((unsigned)a <= 2u && (unsigned)b <= 2u) { s = t; dr = a; dc = b; }
+        }
+        outside = s < 0 || !on_board(r, c, H, W);
+        if (!outside) {
+          // z-order a b c @ # P, as the full paint composes it
+          const bool wall = (s_nb[kNbWall + 5 * s + dr + 1] >> (dc + 1)) & 1u;
+          bool coin = (s_nb[kNbCoin + 3 * s + dr] >> dc) & 1u;
+          if (picked_r - cr == r && picked_c - cc == c) coin = false;
+          if (rec_coins[PCL_D_AUX0] == r && rec_coins[PCL_D_AUX1] == c) coin = true;
+          val = (s_nb[kNbBackdrop + 3 * s + dr] >> (8 * dc)) & 0xffu;
+          // t = 1..3: a, b, c; t = 4: '@', '#', then P (sprite 0) on top
+#pragma unroll
+          for (int t = 1; t <= kS; ++t) {
+            const int32_t* q = rec + (t & 3) * PCL_SPRITE_WORDS;
+            if (t == kS && coin) val = '@';
+            if (t == kS && wall) val = '#';
+            if ((q[PCL_S_FLAGS] & 1) && q[PCL_S_ROW] == r && q[PCL_S_COL] == c) val = p.sprite_char[t & 3];
+          }
+          cell = r * pitch + c;
+        }
+      }
+      fall = __any_sync(PCL_FULL, outside);
+    }
+    if (fall) {
+      __syncwarp();                          // every lane is done with the scratch words
+      delta = false;
+      stage(level_of(p, env));
+      cp_async_wait_all();
+    } else if (cell >= 0) {
+      p.out.d_board[(int64_t)env * H * pitch + cell] = (uint8_t)val;
+    }
+  }
+
+  // The coin window was staged before the pick-up: clear the bit there too.
+  if (!delta && lane == 0 && picked_r >= 0) {
+    const int r2 = picked_r - cr_pred, b = picked_c - (ce << 5);
+    if ((unsigned)r2 < (unsigned)H && (unsigned)b < (unsigned)(nw * 32))
+      s_coin[r2 * nw + (b >> 5)] &= ~(1u << (b & 31));
+  }
   int ce_final = ce;
   if (cr != cr_pred || cc != cc_pred) {      // '@' issued its own order: restage
     __syncwarp();
@@ -705,6 +885,19 @@ scrolly_maze_step(const StepParams p) {
   p.st.d_sprites[(int64_t)env * kS * PCL_SPRITE_WORDS + lane] = rec[lane];
   if (lane < 16) p.st.d_drapes[(int64_t)env * 2 * PCL_DRAPE_WORDS + lane] = rec[32 + lane];
   else p.st.d_plot[(int64_t)env * PCL_PLOT_WORDS + lane - 16] = rec[32 + lane];
+  if (lane < kKeyWords)                      // what the board in d_board is now drawn from
+    p.render_key[(int64_t)env * kKeyStride + lane] = key_word(rec, lane, p.board_epoch, pitch);
+  if (delta) {                               // 4c stored every cell that changed
+    PCL_STAMP(kStPatched);
+    PCL_STAMP(kStPaint);
+    if (p.has_cropper) {
+      __syncwarp();
+      crop_epilogue(p.cropper, p.out.d_board, env, lane, rec, rec + 48);
+    }
+    PCL_STAMP(kStEnd);
+    PCL_STAMP_TIME(kStTimeOut);
+    return;
+  }
 
   // ---- 5. final render, z-order a b c @ # P (engine.py:737-759) ----------
   // 5a. Window rows -> ONE word per 16-cell board segment (wall16 << 16 | coin16),
@@ -897,11 +1090,15 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
   const int64_t n_wall = st.pattern_bstride[0] == 0 ? 1 : levels;
   const int64_t n_coin = st.pattern_init_bstride[1] == 0 ? 1 : levels;
   const int64_t off_coin = (n_wall * blk_words * 4 + 255) & ~(int64_t)255;
+  const int64_t off_key = (off_coin + n_coin * blk_words * 4 + 255) & ~(int64_t)255;
   uint8_t* buf = nullptr;
-  if (cudaMalloc(&buf, off_coin + n_coin * blk_words * 4) != cudaSuccess) return PCL_ERR_NOMEM;
+  if (cudaMalloc(&buf, off_key + (int64_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_NOMEM;
   *owned = buf;
   uint32_t* wall = reinterpret_cast<uint32_t*>(buf);
   uint32_t* coin = reinterpret_cast<uint32_t*>(buf + off_coin);
+  // Render keys of no render (frame -1): the first launch paints every board.
+  p->render_key = reinterpret_cast<int32_t*>(buf + off_key);
+  if (cudaMemset(p->render_key, 0xff, (size_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_CUDA;
   build_blocked<<<1024, 256>>>(st.d_pattern[0], st.pattern_bstride[0], wall, PH, s.pattern_words,
                                nw, nblk, n_wall * blk_words);
   build_blocked<<<1024, 256>>>(st.d_pattern_init[1], st.pattern_init_bstride[1], coin, PH,

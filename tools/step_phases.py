@@ -20,6 +20,8 @@ Phases (cycles between consecutive stamps of one warp):
   seg_patch    -> records written back, segment words built, sprites patched
   paint        -> board stored
   cropper      -> cropper epilogue done (zero without a cropper)
+A warp on the delta-rendering path stages nothing: its copy_wait is empty, seg_patch holds
+the records write-back and the changed cells' stores, and paint is empty.
 
     python tools/step_phases.py [--steps 1000] [--sizes 4096,128] [--rounds 2]
 """
