@@ -68,6 +68,31 @@ and the construct):
                 `random.random()`, only as one side of a comparison with a number literal.
               Each draw continues the env's copy of that generator on the device
               (include/pcl.h PCL_OP_RANDINT) and yields what the generator would.
+  helpers     calls of the game's own code, inlined where they stand (there is no call
+              opcode, so every jump stays forward and a helper costs nothing at run time):
+              `self.name(...)` where `name` resolves along the entity class's MRO to a plain
+              function of the game's code (methods of this package's classes keep the
+              treatment above; a game's override of one, `_north` say, is inlined as Python
+              would call it), and `name(...)` of a plain function of the game's code, found
+              through the module globals as draws are.  The game's code is every function
+              but this package's, NumPy's and the standard library's.  Arguments are positional or keyword,
+              defaults int / bool / None / one-character string literals.  An update()
+              argument (board, layers, things, backdrop, the_plot, actions) passed under any
+              parameter name stands for it inside the helper; a one-character string literal
+              is a constant of the body, specialised per call site (`things[ch]`,
+              `layers[ch]`, `board[p] == ch`); any other argument is an int, bool, position or
+              motion result, evaluated once, left to right, into fresh local slots that are
+              freed when the call ends (PCL_CODE_LOCALS bounds the deepest chain of live
+              slots).  A helper returns nothing (`return`, `return None`, `return <call
+              returning nothing>` such as `return self._teleport(p)`), or a value of one type
+              on every path: a number or a position, which may not fall off the end, or a
+              motion result, which falls off as None.  A value used as a statement is
+              discarded.  Helpers nest up to MAX_HELPER_DEPTH deep; recursion, `*args`,
+              `**kwargs`, keyword-only parameters, decorators (staticmethod, classmethod,
+              property), lambdas, closures, generators, `super()` and another entity's methods
+              are refused, naming the helper, its line and each call site.  Inside a helper
+              `self.<attr>`, Plot keys, draws and entity look-ups are update()'s.  When a
+              subclass overrides a helper, `registered` compiles update() for it again.
 Int and bool attributes of `self` become per-entity registers and `the_plot` keys plot
 registers; their values are read from the live objects when the game is lowered.  An
 attribute used as a position (`self._start = self.position`, `self._position =
@@ -81,10 +106,13 @@ at lowering.
 
 import ast
 import inspect
+import os
 import random
 import struct
+import sysconfig
 import textwrap
 import types
+import weakref
 
 import numpy as np
 
@@ -96,6 +124,7 @@ from pycolab_b200.prefab_parts import drapes as prefab_drapes
 from pycolab_b200.prefab_parts import sprites as prefab_sprites
 
 _REGISTRY = {}                # class -> Compiled
+_VARIANTS = {}                # registered class -> {subclass: its Compiled}, weak in the subclass
 
 _PARAMS = ('self', 'actions', 'board', 'layers', 'backdrop', 'things', 'the_plot')
 _BACKDROP_PARAMS = ('self', 'actions', 'board', 'layers', 'things', 'the_plot')
@@ -125,6 +154,13 @@ _DRAWS = ((np.random.randint, 'numpy', 'randint'), (np.random.choice, 'numpy', '
 _FLIPPED = {ast.Eq: ast.Eq, ast.NotEq: ast.NotEq, ast.Lt: ast.Gt, ast.LtE: ast.GtE,
             ast.Gt: ast.Lt, ast.GtE: ast.LtE}
 _TYPE_NAMES = {'int': 'number', 'pos': 'position', 'motion': 'motion result', 'char': 'character'}
+# Stack words of the values a helper takes or returns.
+_WIDTH = {'int': 1, 'motion': 1, 'pos': 2}
+# update() arguments a helper may take, under any parameter name.
+_ROLES = ('actions', 'board', 'layers', 'backdrop', 'things', 'the_plot')
+# What the compiler keeps of the function whose body it compiles, saved around an inlined helper.
+_FRAME = ('lines', 'first', 'globals', 'role', 'locals', 'where', 'short', 'ret')
+MAX_HELPER_DEPTH = 8
 # A plain Sprite's own state (things.py:339-391), read and written in place.
 _SPRITE_STATE = ('_position', '_visible')
 
@@ -144,7 +180,8 @@ class Compiled(object):
   ('label', n) a code address, ('rows',) / ('cols',) the board shape, ('rng', stream) the
   RNG slot of a generator."""
 
-  def __init__(self, klass, kind, ir, attrs, keys, float_reward, streams=(), attr_types=None):
+  def __init__(self, klass, kind, ir, attrs, keys, float_reward, streams=(), attr_types=None,
+               methods=None):
     self.klass, self.kind, self.ir = klass, kind, ir
     self.attrs = attrs            # register names, in slot order
     # 'int' (ints and bools, one register) or 'pos' (a position, two: row, then col)
@@ -152,6 +189,8 @@ class Compiled(object):
     self.keys = keys              # the_plot keys it reads or writes
     self.float_reward = float_reward
     self.streams = list(streams)  # generators it draws from ('numpy', 'python'), first use first
+    # name -> the class attribute each inlined `self.name(...)` resolved to on `klass`
+    self.methods = dict(methods or {})
 
   def width(self, name):
     return 2 if self.attr_types.get(name) == 'pos' else 1
@@ -170,20 +209,38 @@ def register(*classes):
   Returns its argument (so `@compiler.register` decorates a class)."""
   for klass in classes:
     _REGISTRY[klass] = compile_class(klass)
+    _VARIANTS.pop(klass, None)
   return classes[0] if len(classes) == 1 else classes
 
 
 def unregister(*classes):
   for klass in classes:
     _REGISTRY.pop(klass, None)
+    _VARIANTS.pop(klass, None)
 
 
 def registered(cls):
   """The `Compiled` of the registered class along `cls`'s MRO whose update() `cls` uses,
-  or None."""
+  or None.  When a method that update() calls as `self.name(...)` resolves differently on
+  `cls` (a subclass overrides a helper or a motion helper), this is a compilation for `cls`,
+  shared with every class whose methods resolve as `cls`'s do.  Its `klass` is the
+  registered class, and the cache holds subclasses weakly, so classes made at run time
+  can be freed."""
   for klass in cls.__mro__:
     if klass in _REGISTRY:
-      return _REGISTRY[klass] if cls.update is klass.update else None
+      if cls.update is not klass.update:
+        return None
+      variants = _VARIANTS.setdefault(klass, weakref.WeakKeyDictionary())
+      if cls not in variants:
+        for comp in [_REGISTRY[klass]] + list(variants.values()):
+          if all(inspect.getattr_static(cls, name, None) is obj
+                 for name, obj in comp.methods.items()):
+            break
+        else:
+          comp = compile_class(cls)
+          comp.klass = klass
+        variants[cls] = comp
+      return variants[cls]
   return None
 
 
@@ -241,19 +298,34 @@ class _Compiler(object):
     self.attr_types = {}
     self.float_reward = False
     self.streams = []
+    # The function being compiled (update() or an inlined helper): see _FRAME.
+    self.where = _name(klass) + '.update'
+    self.short = klass.__qualname__ + '.update'
+    self.ret = None               # an inlined helper's _Return, None in update()
+    self.callers = []             # (short name, line) of each call site being inlined
+    self.active = []              # the helpers being inlined, outermost first
+    self.methods = {}             # name -> class attribute of each inlined self.name()
+    self.helper_types = {}        # call node -> what the helper it inlines returns
 
   def run(self):
     self.stmts(self.fdef.body)
     self.emit('RET')
     return Compiled(self.klass, self.kind, self.ir, self.attrs, self.keys, self.float_reward,
-                    self.streams, self.attr_types)
+                    self.streams, self.attr_types, self.methods)
 
   # -------------------------------------------------------------- helpers
   def refuse(self, node, what):
     line = self.first + getattr(node, 'lineno', 1) - 1
     text = self.lines[getattr(node, 'lineno', 1) - 1].strip()
-    raise NotLoweredError('{}.update, line {}: {} is not compiled: {}'.format(
-        _name(self.klass), line, what, text))
+    raise NotLoweredError('{}, line {}: {} is not compiled: {}{}'.format(
+        self.where, line, what, text, self.called_from()))
+
+  def called_from(self):
+    """' (called from Case.update, line N)' inside an inlined helper, else ''."""
+    if not self.callers:
+      return ''
+    return ' (called from {})'.format(', called from '.join(
+        '{}, line {}'.format(name, line) for name, line in reversed(self.callers)))
 
   def emit(self, *ins):
     self.ir.append(ins)
@@ -370,6 +442,226 @@ class _Compiler(object):
       return sign * node.value
     return None
 
+  # -------------------------------------------------------- inlined helpers
+  def helper(self, node):
+    """What a call of one of the game's own helpers runs, else None: for `self.name(...)`
+    the attribute `name` of the entity's class along its MRO when it is the game's code
+    (methods of this package's classes keep their own treatment), for `name(...)` a
+    function of the game's code found through the module globals (`_user_code` decides
+    both)."""
+    if not isinstance(node, ast.Call):
+      return None
+    f = node.func
+    if isinstance(f, ast.Attribute) and self.is_self(f.value):
+      obj = inspect.getattr_static(self.klass, f.attr, None)
+      self.methods[f.attr] = obj        # every resolution, for `registered` to compare
+      fn = obj
+      if isinstance(obj, property):
+        fn = obj.fget
+      elif isinstance(obj, (staticmethod, classmethod)):
+        fn = obj.__func__
+      return obj if isinstance(fn, types.FunctionType) and _user_code(fn) else None
+    fn = self.callee(f)
+    if isinstance(fn, types.FunctionType) and _user_code(fn):
+      return fn
+    return None
+
+  def helper_type(self, node):
+    """What the helper `node` calls returns ('int', 'pos', 'motion' or 'nothing'), found by
+    inlining it into code that is thrown away; None when `node` calls no helper.  The
+    call is then inlined again, so a chain of helpers each asked for its type costs up to
+    2 ** depth inlines; MAX_HELPER_DEPTH bounds that at 256."""
+    if self.helper(node) is None:
+      return None
+    if node not in self.helper_types:
+      at = len(self.ir)
+      self.helper_types[node] = self.inline(node)
+      del self.ir[at:]
+    return self.helper_types[node]
+
+  def refuse_helper(self, fn, call, what):
+    """Refuse the helper `fn` that `call`, in the function being compiled, runs."""
+    site = (self.short, self.first + call.lineno - 1)
+    self.callers.append(site)
+    msg = '{}.{}, line {}: {} is not compiled{}'.format(
+        fn.__module__, fn.__qualname__, fn.__code__.co_firstlineno, what, self.called_from())
+    self.callers.pop()
+    raise NotLoweredError(msg)
+
+  def helper_def(self, obj, call):
+    """(function, its def, source lines, first line) of the helper `obj`; refuses the forms
+    that are not inlined."""
+    fn = obj
+    for kind in (staticmethod, classmethod, property):
+      if isinstance(obj, kind):
+        fn = obj.fget if kind is property else obj.__func__
+        if isinstance(fn, types.FunctionType):
+          self.refuse_helper(fn, call, 'a {} helper'.format(kind.__name__))
+        self.refuse(call, 'the call {}()'.format(ast.unparse(call.func)))
+    if fn.__name__ == '<lambda>':
+      self.refuse_helper(fn, call, 'a lambda')
+    if fn in self.active:
+      cycle = self.active[self.active.index(fn):] + [fn]
+      self.refuse_helper(fn, call, 'recursion ({})'.format(
+          ' -> '.join(g.__qualname__ for g in cycle)))
+    if len(self.active) >= MAX_HELPER_DEPTH:
+      self.refuse_helper(fn, call, 'helpers nested more than {} deep'.format(MAX_HELPER_DEPTH))
+    if fn.__code__.co_flags & (inspect.CO_GENERATOR | inspect.CO_COROUTINE |
+                               inspect.CO_ASYNC_GENERATOR):
+      self.refuse_helper(fn, call, 'a generator')
+    free = [v for v in fn.__code__.co_freevars if v != '__class__']   # __class__: super()
+    if free:
+      self.refuse_helper(fn, call, 'a closure over {}'.format(', '.join(free)))
+    try:
+      lines, first = inspect.getsourcelines(fn)
+    except (OSError, TypeError):
+      self.refuse_helper(fn, call, 'a helper whose source is not available')
+    fdef = ast.parse(textwrap.dedent(''.join(lines))).body[0]
+    if not isinstance(fdef, ast.FunctionDef):
+      self.refuse_helper(fn, call, type(fdef).__name__)
+    if fdef.decorator_list:
+      self.refuse_helper(fn, call, 'a decorated helper')
+    a = fdef.args
+    if a.vararg or a.kwarg or a.kwonlyargs:
+      self.refuse_helper(fn, call, '*args, **kwargs or a keyword-only parameter')
+    params = a.posonlyargs + a.args
+    for p, d in zip(params[len(params) - len(a.defaults):], a.defaults):
+      if not (type(self.number(d)) is int or isinstance(d, ast.Constant) and (
+          d.value is None or type(d.value) is bool or (type(d.value) is str and len(d.value) == 1))):
+        self.refuse_helper(fn, call, 'the default {}={}'.format(p.arg, ast.unparse(d)))
+    return fn, fdef, lines, first
+
+  def inline(self, call):
+    """Emit the body of the helper `call` runs in place of the call.  Returns what it
+    leaves on the stack: the type of its value, or 'nothing'."""
+    fn, fdef, lines, first = self.helper_def(self.helper(call), call)
+    what = '{}()'.format(ast.unparse(call.func))
+    params = [p.arg for p in fdef.args.posonlyargs + fdef.args.args]
+    defaults = dict(zip(params[len(params) - len(fdef.args.defaults):], fdef.args.defaults))
+    role = {}
+    if isinstance(call.func, ast.Attribute):       # a method: its first parameter is self
+      if not params:
+        self.refuse_helper(fn, call, 'a method without a self parameter')
+      role[params.pop(0)] = 'self'
+    bound = dict(zip(params, call.args))
+    if len(call.args) > len(params) or any(isinstance(x, ast.Starred) for x in call.args):
+      self.refuse(call, 'these arguments of ' + what)
+    positional_only = {p.arg for p in fdef.args.posonlyargs}
+    for k in call.keywords:
+      if k.arg not in params or k.arg in bound or k.arg in positional_only:
+        self.refuse(call, 'these arguments of ' + what)
+      bound[k.arg] = k.value
+    for p in params:
+      if p not in bound and p not in defaults:
+        self.refuse(call, '{} without its argument {}'.format(what, p))
+    # Arguments in the caller's frame, left to right, then the defaults.
+    n_slots, local, consts = self.n_slots, {}, {}
+    for p in [p for p in bound] + [p for p in params if p not in bound]:
+      arg = bound.get(p, defaults.get(p))
+      if isinstance(arg, ast.Name) and self.role.get(arg.id) in _ROLES:
+        role[p] = self.role[arg.id]
+        continue
+      if isinstance(arg, ast.Constant) and type(arg.value) is str and len(arg.value) == 1:
+        consts[p] = arg.value
+        continue
+      if isinstance(arg, ast.Constant) and arg.value is None:
+        self.emit('PUSH', 0)                        # None as a motion result
+        t = 'motion'
+      elif self.helper(arg) is not None or p not in bound:
+        t = self.value(arg)
+      else:
+        try:
+          t = self.value(arg)
+        except NotLoweredError:                     # refused below, naming the argument
+          t = None
+      if t not in _WIDTH:
+        self.refuse(call, 'the argument {}={} of {}'.format(p, ast.unparse(arg), what))
+      slot = self.n_slots
+      self.n_slots += _WIDTH[t]
+      if self.n_slots > _lib.CODE_LOCALS:
+        self.refuse(call, 'more than {} local slots'.format(_lib.CODE_LOCALS))
+      for s in reversed(range(slot, self.n_slots)):
+        self.emit('STORE', s)
+      local[p] = (slot, t)
+    # The helper's own frame.
+    constants = _Constants(consts)
+    body = [constants.visit(st) for st in fdef.body]
+    saved = {k: getattr(self, k) for k in _FRAME}
+    self.callers.append((self.short, self.first + call.lineno - 1))
+    self.active.append(fn)
+    self.lines, self.first, self.globals = lines, first, fn.__globals__
+    self.role, self.locals, self.ret = role, local, _Return(self.label())
+    self.where, self.short = '{}.{}'.format(fn.__module__, fn.__qualname__), fn.__qualname__
+    try:
+      if constants.stored is not None:
+        self.refuse(constants.stored, 'assigning the argument ' + constants.stored.id)
+      self.stmts(body)
+      ret = self.ret
+      if ret.type is not None and ret.bare:
+        if ret.type != 'motion':
+          self.refuse(ret.bare[0][1], 'a bare return in a helper that returns a ' +
+                      _TYPE_NAMES[ret.type])
+        for at, _ in reversed(ret.bare):         # None as a motion result
+          self.ir.insert(at, ('PUSH', 0))
+      if ret.type is not None and _falls_off(body):
+        if ret.type != 'motion':
+          self.refuse(fdef, 'a helper that returns a {} and can fall off its end'.format(
+              _TYPE_NAMES[ret.type]))
+        self.emit('PUSH', 0)
+      # A jump to the label that immediately follows is not emitted.
+      at = len(self.ir)
+      while at and (self.ir[at - 1][0] == 'LABEL' or self.ir[at - 1] == ('JMP', ret.label)):
+        if self.ir[at - 1][0] == 'JMP':
+          del self.ir[at - 1]
+        at -= 1
+      self.place(ret.label)
+      return ret.type or 'nothing'
+    finally:
+      for k, v in saved.items():
+        setattr(self, k, v)
+      self.callers.pop()
+      self.active.pop()
+      self.n_slots = n_slots
+
+  def helper_return(self, st):
+    """`return`, `return None`, `return <call returning None>` or `return <value>` in an
+    inlined helper: a jump to its end, with the value on the stack."""
+    ret, v = self.ret, st.value
+    if v is None or (isinstance(v, ast.Constant) and v.value is None):
+      t = None
+    elif isinstance(v, ast.Call) and self.returns_nothing(v):
+      self.call_stmt(v)
+      t = None
+    else:
+      t = self.value(v)
+      if t not in _WIDTH:
+        self.refuse(st, 'returning a ' + _TYPE_NAMES[t])
+    self.emit('JMP', ret.label)
+    if t is None:
+      ret.bare.append((len(self.ir) - 1, st))
+    elif ret.type is None:
+      ret.type = t
+    elif ret.type != t:
+      self.refuse(st, 'returning a {} and a {}'.format(_TYPE_NAMES[ret.type], _TYPE_NAMES[t]))
+
+  def value(self, node):
+    """Push a value a helper takes or returns: as expr(), and a tuple as a position."""
+    if isinstance(node, ast.Tuple):
+      self.pos(node, node)
+      return 'pos'
+    return self.expr(node)
+
+  def returns_nothing(self, call):
+    """Is `call` a statement call: a helper that returns nothing, `_teleport`, a Scrolly's
+    motion helper or a `the_plot` method?"""
+    f = call.func
+    if self.helper(call) is not None:
+      return self.helper_type(call) == 'nothing'
+    if isinstance(f, ast.Attribute) and self.is_self(f.value):
+      return f.attr == '_teleport' or (f.attr in _MOTIONS and self.kind == 'scrolly')
+    return (isinstance(f, ast.Attribute) and self.is_param(f.value, 'the_plot') and
+            f.attr in ('add_reward', 'terminate_episode', 'change_default_discount'))
+
   # ----------------------------------------------------------- statements
   def stmts(self, body):
     for st in body:
@@ -390,6 +682,8 @@ class _Compiler(object):
         return
       self.refuse(st, '`del` of anything but names')
     elif isinstance(st, ast.Return):
+      if self.ret is not None:
+        return self.helper_return(st)
       if st.value is not None and not (isinstance(st.value, ast.Constant) and
                                        st.value.value is None):
         self.refuse(st, 'returning a value')
@@ -542,6 +836,11 @@ class _Compiler(object):
 
   def call_stmt(self, call):
     f = call.func
+    if self.helper(call) is not None:      # first: a game's override of a motion helper too
+      t = self.inline(call)
+      for _ in range(_WIDTH.get(t, 0)):       # a value used as a statement is discarded
+        self.emit('POP')
+      return
     if self.motion_choice(f):
       # `(self._east if c else self._west)(...)` as if / else
       other, end = self.label(), self.label()
@@ -659,14 +958,16 @@ class _Compiler(object):
       return (lambda: self.scalar(row), lambda: self.scalar(col))
     if isinstance(node, ast.Tuple) and len(node.elts) == 2:
       return (lambda: self.scalar(node.elts[0]), lambda: self.scalar(node.elts[1]))
+    if self.helper_type(node) == 'pos':           # one inlined call pushes both
+      return (lambda: self.inline(node), lambda: None)
     return None
 
   def component(self, node, index, where):
     parts = self.pos_parts(node)
     if parts is None or isinstance(node, ast.Tuple):
       self.refuse(where, 'indexing something that is not a position')
-    if self.pattern_position(node) is not None:
-      self.pattern_position(node, emit=True)
+    if self.pattern_position(node) is not None or self.helper_type(node) == 'pos':
+      parts[0]()
       if index == 1:                      # keep the column: through a fresh local slot
         slot = self.local(' tmp%d' % self.n_slots, 'int', where)
         self.emit('STORE', slot)
@@ -803,7 +1104,7 @@ class _Compiler(object):
             node.func.attr in _PATTERN_POSITIONS):
       return None
     owner = self.owner(node.func.value)
-    if owner is None:
+    if owner is None or (owner == -1 and self.helper(node) is not None):
       return None
     if emit:
       if owner == -1:
@@ -885,6 +1186,11 @@ class _Compiler(object):
 
   def call(self, node):
     f = node.func
+    if self.helper(node) is not None:      # first: a game's override of a motion helper too
+      t = self.inline(node)
+      if t == 'nothing':
+        self.refuse(node, 'the value of {}(), which returns nothing'.format(ast.unparse(f)))
+      return t
     if self.motion_choice(f):
       self.need(node, 'sprite', 'a motion result')
       return self.expr(ast.copy_location(ast.IfExp(
@@ -1261,6 +1567,62 @@ class _Compiler(object):
     self.emit('FILLBACK')
 
 
+class _Return(object):
+  """The end of an inlined helper: its label, the type of the value it returns (None
+  until a `return <value>`), and (IR index, node) of each `return` without a value."""
+
+  def __init__(self, label):
+    self.label, self.type, self.bare = label, None, []
+
+
+class _Constants(ast.NodeTransformer):
+  """A helper's body with each parameter bound to a one-character string literal read as
+  that literal; `stored` is the first name node that assigns such a parameter."""
+
+  def __init__(self, consts):
+    self.consts, self.stored = consts, None
+
+  def visit_Name(self, node):
+    if node.id not in self.consts:
+      return node
+    if not isinstance(node.ctx, ast.Load):
+      self.stored = self.stored or node
+      return node
+    return ast.copy_location(ast.Constant(self.consts[node.id]), node)
+
+
+def _falls_off(body):
+  """Can control reach the end of the statements `body`?"""
+  if not body:
+    return True
+  last = body[-1]
+  if isinstance(last, ast.Return):
+    return False
+  if isinstance(last, ast.If):
+    return _falls_off(last.body) or _falls_off(last.orelse)
+  return True
+
+
+_STDLIB = tuple(os.path.realpath(sysconfig.get_paths()[k]) + os.sep
+                for k in ('stdlib', 'platstdlib'))
+
+
+def _user_code(fn):
+  """Is the Python function `fn` the game's code, to be inlined?  One rule for methods
+  and module functions: every function qualifies except this package's, NumPy's and the
+  standard library's (by the file that defines it, so a game module named like a standard
+  one, or a game installed as a package, qualifies).  A function of another library
+  qualifies too, and compiles if its body lies in the subset."""
+  if (fn.__module__ or '').split('.')[0] in ('numpy', 'pycolab_b200'):
+    return False
+  path = fn.__code__.co_filename
+  if path.startswith('<frozen'):                 # standard modules frozen into Python
+    return False
+  path = os.path.realpath(path)
+  return not (path.startswith(_STDLIB) and 'site-packages' not in path and
+              'dist-packages' not in path)
+
+
 def _sliced(index):
   """Does a subscript index take a slice on some axis?"""
   return any(isinstance(x, ast.Slice) for x in
@@ -1288,17 +1650,18 @@ def link(compiled, sprite_chars, drape_chars, rows, cols, plot_keys, rng_streams
   """Bytecode words for one game.  compiled: char -> `Compiled`; plot_keys: the key
   order of the plot registers; rng_streams: the generator of each RNG slot; backdrop: the
   `Compiled` of the Backdrop, whose entry goes in header word 1 + n (pcl.h program_arg[4]).
-  Entities of one class share their code."""
+  Entities of one `Compiled` share their code: those of one class, and those of subclasses
+  that inline the same helpers (`registered`)."""
   chars = list(sprite_chars) + list(drape_chars)
   S = len(sprite_chars)
   words = [len(chars)] + [0] * (len(chars) + (backdrop is not None))
   entry = {}
   for i, ch in enumerate(chars):
     comp = compiled[ch]
-    if comp.klass not in entry:
-      entry[comp.klass] = len(words)
+    if comp not in entry:
+      entry[comp] = len(words)
       words += _encode(comp, len(words), chars, S, rows, cols, plot_keys, rng_streams)
-    words[1 + i] = entry[comp.klass]
+    words[1 + i] = entry[comp]
   if backdrop is not None:
     words[1 + len(chars)] = len(words)
     words += _encode(backdrop, len(words), chars, S, rows, cols, plot_keys, rng_streams)
