@@ -35,15 +35,15 @@
 // arithmetic, set the step's length: with the copies issued first, every warp's 6 KB of
 // copies queued in front of them (DESIGN.md section 5, tools/step_phases.py).
 //
-// Tried and rejected in an A/B on the project's earlier target GPU, not re-measured on
-// H100: HALF a warp per env (two envs per warp, every warp primitive on the half's
-// 16-lane mask; the warp instructions of game logic per env issued once per two envs).
-// Bit-exact on the whole GPU suite, but slower per 4096-env step there; the reading then
-// was that the step is bound by the length of ONE warp's dependent chain, not by issue
-// slots, and that halving the lanes doubles every staging / paint loop on that chain.
-// The phase stamps (PCL_STEP_STAMPS) do not support that reading on H100: there a lone
-// warp's step is ~7 500 cycles, but in the full wave the records and patch-row trips
-// alone took ~12 000 (DESIGN.md section 5).
+// Not built: several envs per warp.  Packing E envs into a warp divides the warp-uniform
+// game logic per env by E, and leaves a 4096-env launch with the warps per SM of a
+// 4096 / E-env launch today.  The delta-path kernel at 1024 and 2048 envs (8 and 16 warps
+// per SM; an optimistic bound for E = 4 and 2, with fewer loads per warp) steps in 7.89
+// and 7.30 us against 8.26 at 4096 (H100 SXM, 700 W, tools/step_sweep.py; DESIGN.md
+// section 5): at most ~12 %, and E = 4 would not beat E = 2.  The wave's length is not
+// issue contention between the SM's warps.  (An earlier GPU's A/B of two envs per warp
+// was slower too, but for another reason: before delta rendering, halving the lanes
+// doubled the staging and paint loops on each warp's chain.)
 //
 // Residency on H100 (64x64 board): 64 registers x 128 threads allow 8 blocks of the
 // 65 536 registers, and 6400 B of dynamic shared memory per warp (25 KB per block) + 2 KB
@@ -113,6 +113,12 @@ __device__ __forceinline__ int action_to_motion(int a) {   // scrolly_maze.py:26
 
 __device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::
+               "r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+// 16 bytes through L1, for data every warp of an SM reads (the selector table): the SM's
+// warps hit its L1 instead of all sending the same lines to L2 (cp_async16 bypasses L1).
+__device__ __forceinline__ void cp_async16_l1(void* smem, const void* gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;\n" ::
                "r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
 }
 
@@ -200,7 +206,7 @@ __device__ __forceinline__ void pdl_wait_prior_grids() {
 }
 
 // Selector table of the paint loop (see the kernel): 256 x u16, built at compile
-// time and pulled into shared memory with one cp.async per lane of warp 0.
+// time and pulled into shared memory with one cp.async per lane by each warp that paints.
 struct SelTable { uint16_t v[256]; };
 constexpr SelTable make_sel_table() {
   SelTable t = {};
@@ -221,14 +227,17 @@ __device__ __align__(16) const SelTable g_sel = make_sel_table();
 // at each phase boundary, and of %globaltimer (ns) at entry and exit, to
 // g_stamps[env].  Differences of these 32-bit stamps, taken modulo 2^32, are exact.
 // Without the switch PCL_STAMP expands to nothing and the kernel is the production one.
-// The stamp build also fits 64 registers without spills; tools/step_phases.py reports its
-// step time beside the production build's.
+// The stamp build also fits 64 registers, with a 4-byte spill since the path word;
+// tools/step_phases.py reports its step time beside the production build's.
+// Slot kStPath names the path the warp took (kPath*), so the tool can tell which path's
+// warps end a launch.
 #ifdef PCL_STEP_STAMPS
 constexpr int kStampEnvs = 8192;
 enum {
   kStEntry, kStPrior, kStRecords, kStPatch, kStGroup2, kStWait, kStPatched, kStPaint, kStEnd,
-  kStTimeIn, kStTimeOut, kStampWords
+  kStTimeIn, kStTimeOut, kStPath, kStampWords
 };
+enum { kPathDelta, kPathDeltaPickup, kPathFellBack, kPathFull, kPathRestart };
 __device__ uint32_t g_stamps[kStampEnvs][kStampWords];
 __device__ __forceinline__ uint32_t global_ns() {
   uint32_t t;
@@ -245,9 +254,11 @@ __device__ __forceinline__ void stamp(int k, uint32_t v) {
 }
 #define PCL_STAMP(k) stamp(k, (uint32_t)clock())
 #define PCL_STAMP_TIME(k) stamp(k, global_ns())
+#define PCL_STAMP_PATH(v) stamp(kStPath, (uint32_t)(v))
 #else
 #define PCL_STAMP(k) do {} while (0)
 #define PCL_STAMP_TIME(k) do {} while (0)
+#define PCL_STAMP_PATH(v) do {} while (0)
 #endif
 
 // The most dynamic shared memory a block may ask for on the H100: 227 KB per block less
@@ -373,13 +384,12 @@ scrolly_maze_step(const StepParams p) {
   // nibble; selector nibble k picks byte 5 ('#') if wall_k, else byte 4 ('@') if
   // coin_k, else byte k of the backdrop word (z-order ... '@' '#' ...).
   // One copy per WARP: a warp then needs no block barrier before it paints (warps of a
-  // block leave at different points: ragged tail, frozen envs).
+  // block leave at different points: ragged tail, frozen envs).  Only a warp that paints
+  // in full copies it, with its staging copies (stage() below).
   __shared__ __align__(16) uint16_t s_sel_all[kWarpsPerBlock][256];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   uint16_t* s_sel = s_sel_all[warp];
-  cp_async16(reinterpret_cast<uint8_t*>(s_sel) + lane * 16,
-             reinterpret_cast<const uint8_t*>(g_sel.v) + lane * 16);
   pdl_launch_dependents();
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   const bool live = env < p.B;
@@ -393,17 +403,14 @@ scrolly_maze_step(const StepParams p) {
   uint32_t* s_wall = reinterpret_cast<uint32_t*>(s_bd + (size_t)H * pitch);
   uint32_t* s_coin = s_wall + ((H * nw + 3) & ~3);
   // Everything above ran without touching state earlier kernels may have
-  // produced (g_sel is a constant); from here on the kernel reads such state.
+  // produced; from here on the kernel reads such state.
   pdl_wait_prior_grids();
   PCL_STAMP(kStPrior);
   // An attached cropper reads its corner state at the very end: start that line's trip
   // from DRAM now (a hint, no register held).
   if (p.has_cropper && p.cropper.state && live && lane == 0)
     asm volatile("prefetch.global.L2 [%0];" :: "l"(p.cropper.state + (int64_t)env * 4));
-  if (!live) {                 // ragged last block: only the selector copy to drain
-    cp_async_wait_all();
-    return;
-  }
+  if (!live) return;           // ragged last block
   const int64_t lvl = level_of(p, env);     // index of static level data
 
   // The env's action word does not depend on the records either: issue its load now,
@@ -430,10 +437,7 @@ scrolly_maze_step(const StepParams p) {
     restart = was_over && p.auto_reset;
     frozen = was_over && !p.auto_reset;
   }
-  if (frozen) {                              // warp-uniform
-    cp_async_wait_all();
-    return;
-  }
+  if (frozen) return;                        // warp-uniform
   // The board in d_board was drawn from these very records (see "Delta rendering").
   const bool key_ok = __all_sync(PCL_FULL, lane >= kKeyWords ||
                                                key == key_word(rec, lane, p.board_epoch, pitch));
@@ -604,8 +608,12 @@ scrolly_maze_step(const StepParams p) {
   // the record and patch loads (as before), every warp's 6 KB of copies queued in front of
   // those two dependent round trips, and in a full wave each trip took 2-4x as long as
   // in a lone warp (tools/step_phases.py; DESIGN.md section 5).  Delta rendering stages
-  // nothing unless it falls back to the full paint after group 2.
+  // nothing unless it falls back to the full paint after group 2.  The paint loop's selector
+  // table travels with these copies: the delta path never reads it, and copied at entry
+  // by every warp of a wave it was 2 MB per 4096-env launch, all from the same 512 bytes.
   auto stage = [&](int64_t lvl) {
+    cp_async16_l1(reinterpret_cast<uint8_t*>(s_sel) + lane * 16,
+                  reinterpret_cast<const uint8_t*>(g_sel.v) + lane * 16);
     {
       const uint8_t* src = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * 16;
       uint8_t* dst = s_bd + lane * 16;
@@ -661,6 +669,7 @@ scrolly_maze_step(const StepParams p) {
     if (lane < 2) s_nb[kNbStale + lane] = rec_coins[PCL_D_AUX0 + lane];
   } else {
     stage(lvl);
+    PCL_STAMP_PATH(restart ? kPathRestart : kPathFull);
   }
 
   // ---- 4a. update group 1: patrollers a, b, c then P, ONE WALKER PER LANE ----
@@ -762,7 +771,9 @@ scrolly_maze_step(const StepParams p) {
       coin = bit_at(env_coins(p, env) + (int64_t)pr * PWW, pc);   // cannot happen
     if (coin) {
       add_reward(dir, 100);
-      if (lane == 0) env_coins(p, env)[(int64_t)pr * PWW + (pc >> 5)] &= ~(1u << (pc & 31));
+      // A reduction with no result (RED): nothing on this warp waits for the word's old
+      // value, where a read-modify-write put one more round trip on the pick-up's step.
+      if (lane == 0) atomicAnd(env_coins(p, env) + (int64_t)pr * PWW + (pc >> 5), ~(1u << (pc & 31)));
       picked_r = pr; picked_c = pc;
       plot.aux0 -= 1;
       if (plot.aux0 == 0) terminate(dir);
@@ -863,6 +874,7 @@ scrolly_maze_step(const StepParams p) {
       delta = false;
       stage(level_of(p, env));
       cp_async_wait_all();
+      PCL_STAMP_PATH(kPathFellBack);
     } else if (cell >= 0) {
       p.out.d_board[(int64_t)env * H * pitch + cell] = (uint8_t)val;
     }
@@ -888,6 +900,7 @@ scrolly_maze_step(const StepParams p) {
   if (lane < kKeyWords)                      // what the board in d_board is now drawn from
     p.render_key[(int64_t)env * kKeyStride + lane] = key_word(rec, lane, p.board_epoch, pitch);
   if (delta) {                               // 4c stored every cell that changed
+    PCL_STAMP_PATH(picked_r >= 0 ? kPathDeltaPickup : kPathDelta);
     PCL_STAMP(kStPatched);
     PCL_STAMP(kStPaint);
     if (p.has_cropper) {
@@ -1120,7 +1133,7 @@ const Program kScrollyMaze = {check_spec, check_state, curtain, launch, nullptr,
 
 #ifdef PCL_STEP_STAMPS
 // Copies the stamps of the last scrolly_maze_step launch for envs [0, n) to host memory
-// (n * 11 u32, in the order of the kSt* slots).  Only the stamp build exports it.
+// (n * 12 u32, in the order of the kSt* slots).  Only the stamp build exports it.
 extern "C" int pcl_step_stamps(uint32_t* host, int n) {
   if (n < 0 || n > pcl::kStampEnvs) return -1;
   return cudaMemcpyFromSymbol(host, pcl::g_stamps, sizeof(pcl::g_stamps[0]) * n) == cudaSuccess

@@ -23,6 +23,10 @@ Phases (cycles between consecutive stamps of one warp):
 A warp on the delta-rendering path stages nothing: its copy_wait is empty, seg_patch holds
 the records write-back and the changed cells' stores, and paint is empty.
 
+`paths` splits the warps by the path each took (PATHS below, one stamp word per warp):
+their count, and the median and max of their work cycles (entry to end, less prior_grid)
+and of their exit time, so the path whose warps end the launch shows.
+
     python tools/step_phases.py [--steps 1000] [--sizes 4096,128] [--rounds 2]
 """
 import argparse
@@ -40,7 +44,9 @@ sys.path.insert(0, os.path.join(ROOT, 'tools'))
 PHASES = ('prior_grid', 'records', 'patch_bits', 'groups', 'copy_wait', 'seg_patch', 'paint',
           'cropper')
 N_CLOCKS = len(PHASES) + 1          # slots 0..8: cycle stamps at the phase boundaries
-T_IN, T_OUT, WORDS = 9, 10, 11
+T_IN, T_OUT, PATH, WORDS = 9, 10, 11, 12
+# Values of the path slot (kPath* in scrolly_maze.cu).
+PATHS = ('delta', 'delta_pickup', 'fell_back', 'full_paint', 'restart')
 
 
 def build_stamps(out_dir):
@@ -73,6 +79,13 @@ def stamp_stats(raw):
   ref = t0.min() if len(t0) else 0
   t_in = (t0 - ref) % (1 << 32)
   t_out = (done[:, T_OUT].astype(np.int64) - ref) % (1 << 32)
+  work = tot - d[:, 0]
+  paths = {}
+  for k, name in enumerate(PATHS):
+    sel = done[:, PATH] == k
+    paths[name] = {'warps': int(sel.sum()),
+                   'work_cycles': {'median': pct(work[sel], 50), 'max': pct(work[sel], 100)},
+                   'exit_ns': {'median': pct(t_out[sel], 50), 'max': pct(t_out[sel], 100)}}
   return {
       'warps': int(len(done)),
       'cycles': {name: {'median': pct(d[:, i], 50), 'p90': pct(d[:, i], 90)}
@@ -82,6 +95,7 @@ def stamp_stats(raw):
                    'max': pct(t_in, 100)},
       'exit_ns': {'min': pct(t_out, 0), 'p10': pct(t_out, 10), 'p50': pct(t_out, 50),
                   'p90': pct(t_out, 90), 'max': pct(t_out, 100)},
+      'paths': paths,
   }
 
 
