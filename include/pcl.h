@@ -432,8 +432,10 @@ typedef struct pcl_outputs {
   uint8_t* d_done;        /* u8 [B]; Engine.game_over after this step */
   double*  d_reward_f64;  /* f64 [B]; the summed reward exactly as the reference's float sum produces
                              it, 0.0 if none.  Written only by programs whose rewards are not integers
-                             (today PCL_PROG_T_MAZE, which then leaves d_reward alone); required by
-                             them (PCL_ERR_INVALID when NULL), ignored by every other program. */
+                             (PCL_PROG_T_MAZE and PCL_PROG_SEQUENCE_RECALL always, PCL_PROG_COMPILED
+                             and PCL_PROG_CUED_CATCH when program_arg[0] is set), which then leave
+                             d_reward alone; required by them (PCL_ERR_INVALID when NULL), ignored by
+                             every other program. */
 } pcl_outputs;
 
 typedef struct pcl_handle pcl_handle;

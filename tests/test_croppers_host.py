@@ -209,9 +209,17 @@ def _spec(rows, cols, track=None, pad='.'):
 FAKE = boundary_sweep.FAKE
 
 
+def _step_host_async(lib, h, spec):
+  out = _lib.Outputs(FAKE, FAKE, FAKE, FAKE, FAKE)
+  return lib.pcl_step_host_async(h, FAKE, FAKE, C.byref(out), C.byref(spec), FAKE, FAKE, FAKE,
+                                 FAKE, FAKE, FAKE, FAKE, 0, None)
+
+
 def _calls(lib, h, spec):
-  """{entry point: status} of every cropper entry point for `spec`; none of them may get
-  as far as a launch (the handle's device is -1)."""
+  """{entry point: status} of every cropper entry point for `spec`, which every one of them
+  must refuse: a spec one of them accepts would launch on the made-up addresses (device -1
+  only means the handle selects no device; where a GPU is present the launch runs on the
+  current one)."""
   curtains = (C.c_void_p * _lib.MAX_TRACK)(*([FAKE] * _lib.MAX_TRACK))
   out = _lib.Outputs(FAKE, FAKE, FAKE, FAKE, FAKE)
   x = _lib.HandoffState()
@@ -224,9 +232,7 @@ def _calls(lib, h, spec):
                                                    curtains, None)
   got['pcl_crop_handoff'] = lib.pcl_crop_handoff(h, C.byref(spec), FAKE, FAKE, C.byref(out),
                                                  C.byref(x), None)
-  got['pcl_step_host_async'] = lib.pcl_step_host_async(
-      h, FAKE, FAKE, C.byref(out), C.byref(spec), FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, 0,
-      None)
+  got['pcl_step_host_async'] = _step_host_async(lib, h, spec)
   return got
 
 
@@ -269,11 +275,12 @@ def test_drape_tracking_past_128_rows_or_columns_is_unsupported(shape):
 def test_step_host_async_refuses_drape_tracking_before_the_step(track):
   """pcl_step_host_async passes no curtains: a tracking list naming a drape is refused
   with PCL_ERR_UNSUPPORTED before the step is enqueued (here: before the device -1
-  handle would fail to create its copy stream)."""
+  handle would fail to create its copy stream).  pcl_crop_tracking accepts the same spec,
+  so it is not called here: it would launch on the made-up addresses."""
   lib, h = _none_handle(16, 16)
   try:
-    assert _calls(lib, h, _spec(5, 7, track))['pcl_step_host_async'] == _lib.ERR_UNSUPPORTED
+    assert _step_host_async(lib, h, _spec(5, 7, track)) == _lib.ERR_UNSUPPORTED
     bad = _spec(5, 7, [3])                                      # no sprite 2
-    assert _calls(lib, h, bad)['pcl_step_host_async'] == _lib.ERR_INVALID
+    assert set(_calls(lib, h, bad).values()) == {_lib.ERR_INVALID}
   finally:
     lib.pcl_destroy(h)

@@ -423,122 +423,7 @@ def test_large_batch_invariants():
 
 
 # --------------------------------------------------- engine-level behaviours
-
-# Every step program starts and ends an env's step with the same reset / freeze
-# protocol; each is checked here with a game its own tests use.  Per program: the
-# game factory, draw(rs, shape) -> random action words, and the action row that
-# ends an episode at once (None: the drawn actions end episodes on their own).
-
-def _fixture_game():
-  from pycolab_b200.games import fixtures
-  kw, _ = gc.fixture_kwargs(gc.load('fixture_walkers_0'))
-  return fixtures.make_game(kw['art'], kw['what_lies_beneath'], kw['walkers'], kw['scrollys'],
-                            kw['drapes'], kw['update_schedule'], kw['z_order'])
-
-
-def _protocol_program(name):
-  from pycolab_b200 import _lib, levels, lowering
-  from pycolab_b200.games import (aperture, apprehend, better_scrolly_maze, hello_world, ordeal,
-                                  scrolly_maze, shockwave, warehouse_manager)
-  from pycolab_b200.games import extraterrestrial_marauders as marauders
-  from pycolab_b200.games.classics import cliff_walk
-  below = lambda n: (lambda rs, shape: rs.randint(0, n, size=shape))
-  if name == 'fixture':
-    low = lowering.lower(_fixture_game())
-    n_ent, n_dir = len(low.sprite_chars) + len(low.drape_chars), _lib.FIXTURE_DIRECTIVES
-
-    def draw(rs, shape):                      # a motion per entity, no Plot directives
-      rows = np.zeros(tuple(shape) + (n_ent + 2 * n_dir,), dtype=np.int64)
-      rows[..., :n_ent] = rs.randint(0, 9, size=tuple(shape) + (n_ent,))
-      return rows
-    quit_row = np.zeros(n_ent + 2 * n_dir, dtype=np.int64)
-    quit_row[:n_ent] = 8
-    quit_row[n_ent] = _lib.DIR_TERMINATE      # terminate_episode(discount 0.0)
-    return _fixture_game, draw, quit_row
-  return {
-      'scrolly_maze': (lambda: scrolly_maze.make_game(*levels.scrolly_maze_level(
-          4, world_shape=(65, 65), board_shape=(32, 32))), below(4), 5),
-      'warehouse': (lambda: warehouse_manager.make_game(levels.warehouse_level(3)), below(5), 5),
-      'marauders': (lambda: marauders.make_game(levels.marauders_level()), below(4), 4),
-      'better_scrolly': (lambda: better_scrolly_maze.make_game(
-          tj.u8_to_art(gc.load('better_stock_L1')['art'])), below(5), 5),
-      'classics': (lambda: cliff_walk.make_game(), below(4), 3),   # east off the start: the cliff
-      'aperture': (lambda: aperture.make_game(
-          tj.u8_to_art(gc.load('aperture_stock_L1')['art'])), below(9), 9),
-      'ordeal': (ordeal.make_castle, below(4), 4),
-      'hello': (hello_world.make_game, below(4), 4),
-      'apprehend': (apprehend.make_game, below(3), None),   # the ball lands within a board height
-      'shockwave': (lambda: shockwave.make_game(levels.shockwave_level(30, 12, 15, 0.45)),
-                    lambda rs, shape: rs.choice(5, size=shape, p=[.6, .12, .12, .12, .04]), None),
-  }[name]
-
-
-PROTOCOL_PROGRAMS = ['scrolly_maze', 'warehouse', 'marauders', 'better_scrolly', 'fixture',
-                     'classics', 'aperture', 'ordeal', 'hello', 'apprehend', 'shockwave']
-
-
-@pytest.mark.parametrize('program', PROTOCOL_PROGRAMS)
-def test_partial_reset_touches_only_masked_envs(program):
-  """A masked reset rebuilds the selected envs as a fresh Engine would (its_showtime,
-  frame 0) and leaves every other env's board and frame as they were."""
-  from pycolab_b200 import batched
-  torch = _torch()
-  make, draw, _ = _protocol_program(program)
-  B = 6
-  eng = batched.BatchedEngine([make()], batch=B, auto_reset=False)
-  first = eng.its_showtime().board.clone()
-  rs = np.random.RandomState(0)
-  for _ in range(25):
-    eng.play(draw(rs, (B,)).astype(np.int32).reshape(-1))
-  before = eng.board.clone()
-  frames = eng.frames().tolist()
-  # A fresh Engine draws from where each env's random stream stands now.
-  rng = None if eng.rng is None else eng.rng.cpu().numpy().view(np.uint32).copy()
-  mask = torch.tensor([1, 0, 0, 1, 0, 0], dtype=torch.uint8, device='cuda')
-  eng.reset(mask)
-  fresh = batched.BatchedEngine([make()], batch=B, auto_reset=False, rng_states=rng)
-  want = fresh.its_showtime().board
-  torch.cuda.synchronize()
-  if rng is None:
-    assert bool((want == first).all())
-  assert bool((eng.board[[0, 3]] == want[[0, 3]]).all())
-  assert bool((eng.board[[1, 2, 4, 5]] == before[[1, 2, 4, 5]]).all())
-  assert eng.frames().tolist() == [0, frames[1], frames[2], 0, frames[4], frames[5]]
-
-
-@pytest.mark.parametrize('program', PROTOCOL_PROGRAMS)
-def test_finished_env_freezes_without_auto_reset(program):
-  """Upstream raises on play() after the episode ended (engine.py:622-624); the
-  batched engine leaves such an env untouched instead, and steps the others."""
-  from pycolab_b200 import batched
-  torch = _torch()
-  make, draw, quit_row = _protocol_program(program)
-  B, T = 4, 12
-  eng = batched.BatchedEngine([make()], batch=B, auto_reset=False)
-  eng.its_showtime()
-  rs = np.random.RandomState(4)
-  actions = draw(rs, (T, B))
-  if quit_row is not None:
-    for e in range(B - 1):                    # env e quits at step 2e, the last env never
-      actions[2 * e, e] = quit_row
-  frozen_steps = 0
-  for t in range(T):
-    done = eng.done.cpu().numpy().astype(bool)
-    board = eng.board.cpu().numpy()
-    frames = eng.frames().cpu().numpy()
-    res = eng.play(actions[t].astype(np.int32).reshape(-1))
-    torch.cuda.synchronize()
-    now = res.done.cpu().numpy().astype(bool)
-    assert now[done].all(), (t, done, now)
-    np.testing.assert_array_equal(res.board.cpu().numpy()[done], board[done], err_msg='t=%d' % t)
-    new_frames = eng.frames().cpu().numpy()
-    np.testing.assert_array_equal(new_frames[done], frames[done], err_msg='t=%d' % t)
-    np.testing.assert_array_equal(new_frames[~done], frames[~done] + 1, err_msg='t=%d' % t)
-    discount = res.discount.cpu().numpy()
-    np.testing.assert_array_equal(discount[~done], np.where(now[~done], 0.0, 1.0))
-    frozen_steps += int(done.sum())
-  assert frozen_steps > 0                     # some env really was frozen
-
+# (the per-env reset / freeze protocol of every step program: test_gpu_protocol.py)
 
 def test_facade_raises_like_the_reference():
   from pycolab_b200 import levels
