@@ -2,7 +2,7 @@
 code, whose classes the tests register with `pycolab_b200.compiler`.
 
 This module imports `pycolab.*` only, so it runs unchanged on the reference (the golden
-maker, tests/golden/make_backdrop_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  Three games:
 
   fluvial  a swimmer in a river whose middle rows flow one cell west on even frames: the
@@ -216,12 +216,19 @@ class Flow(plab_things.Backdrop):
     self.curtain[-1, 0] = self.palette['#'] if layers['P'][3, 5] else self.palette.tilde
 
 
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (Swimmer, River, Walker, Trail, Purse, Rower, Flow)
 
-# (golden name, game, level, action seed, np.random seed, steps)
+# (golden name, game, level, action seed, generator seed, steps)
 CASES = [('backdrop_trail_0', 'trail', 0, 41, 3, 300), ('backdrop_trail_1', 'trail', 1, 42, 4, 300),
          ('backdrop_flow_0', 'flow', 0, 43, 5, 300), ('backdrop_flow_1', 'flow', 1, 44, 6, 300)]
 GAMES = {'trail': make_trail, 'flow': make_flow}
 N_ACTIONS = {'trail': 6, 'flow': 6}
 SPRITES = {'trail': 'P', 'flow': 'P'}
+REGISTERS = {'trail': [], 'flow': []}
 PLOT_KEYS = {'trail': ['prev_row', 'prev_col', 'dots'], 'flow': ['tide']}
+GENERATORS = ('numpy',)
+RAISES = {}
+FIELDS = ('game', 'level', 'rng_seed', 'actions', 'sprites', 'backdrops', 'plot_keys',
+          'reward_type', 'numpy_words')

@@ -2,7 +2,7 @@
 tests register with `pycolab_b200.compiler`.
 
 This module imports `pycolab.*` only, so it runs unchanged on the reference (the golden
-maker, tests/golden/make_compiled_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  Between them the games use every kind of construct the compiler
 accepts: curtain reads and writes, `.any()`, registers flipped by blocked moves, Plot keys,
 a float reward stream, backdrop and layer reads, diagonal moves, leaving the board,
@@ -232,7 +232,8 @@ def make_fault(drape_class):
                                      drapes={'x': drape_class})
 
 
-# The classes a test registers, and what the golden maker records every frame.
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (CoinPlayer, Patroller, CoinDrape, LavaWalker, GemDrape)
 GAMES = {'coins': make_coins, 'lava': make_lava}
 SPRITES = {'coins': 'Pe', 'lava': 'P'}
@@ -240,11 +241,14 @@ REGISTERS = {'coins': (('P', 'bumps'), ('e', 'eastward'), ('c', 'collected')),
              'lava': (('P', 'home_row'), ('P', 'home_col'), ('P', 'steps'), ('x', 'phase'))}
 PLOT_KEYS = {'coins': ('countdown', 'caught'), 'lava': ()}
 N_ACTIONS = {'coins': 6, 'lava': 7}
+GENERATORS = ()
+RAISES = {}
+FIELDS = ('game', 'level', 'actions', 'sprites', 'registers', 'reward_type', 'reward_f64')
 
-# (golden name, game, level, action seed, steps)
+# (golden name, game, level, action seed, generator seed, steps)
 CASES = (
-    ('compiled_coins_0', 'coins', 0, 1, 320),
-    ('compiled_coins_1', 'coins', 1, 2, 320),
-    ('compiled_lava_0', 'lava', 0, 3, 320),
-    ('compiled_lava_1', 'lava', 1, 4, 320),
+    ('compiled_coins_0', 'coins', 0, 1, None, 320),
+    ('compiled_coins_1', 'coins', 1, 2, None, 320),
+    ('compiled_lava_0', 'lava', 0, 3, None, 320),
+    ('compiled_lava_1', 'lava', 1, 4, None, 320),
 )

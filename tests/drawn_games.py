@@ -3,7 +3,7 @@ pycolab code, whose entity classes the tests register with `pycolab_b200.compile
 
 This module imports `pycolab.*`, `numpy` and `random` only, the way a game author would
 (with aliases and `from` imports too), so it runs unchanged on the reference (the golden
-maker, tests/golden/make_drawn_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  No constructor draws.
 """
 
@@ -230,13 +230,19 @@ def make_empty(which):
   return game
 
 
-# The classes a test registers, and what the golden maker records every frame.
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (Player, NumpyMonster, PythonMonster, Fruit, Edges, EmptyRange)
 GAMES = {'monsters': make_monsters, 'edges': make_edges}
 SPRITES = {'monsters': 'Pab', 'edges': ''}
 REGISTERS = {'monsters': (('P', 'bonuses'), ('f', 'eaten')),
              'edges': (('x', 'case'), ('x', 'out'))}
+PLOT_KEYS = {'monsters': (), 'edges': ()}
 N_ACTIONS = {'monsters': 6, 'edges': 2}
+GENERATORS = ('numpy', 'python')
+RAISES = {}
+FIELDS = ('game', 'level', 'rng_seed', 'actions', 'sprites', 'registers', 'reward_type',
+          'numpy_words', 'python_words')
 
 # (golden name, game, level, action seed, generator seed, steps)
 CASES = (

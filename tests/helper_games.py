@@ -3,7 +3,7 @@ ordinary pycolab code, whose entity classes the tests register with `pycolab_b20
 (which inlines each helper call).
 
 This module imports `pycolab.*` only, so it runs unchanged on the reference (the golden
-maker, tests/golden/make_helper_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  Three games:
 
   bolts    marauders-like: the bolts share one registered `Bolt` base whose update() calls
@@ -425,9 +425,11 @@ class Divider(prefab_sprites.MazeWalker):
     return total // parts
 
 
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (Cannon, Marauders, Bolt, Runner, Chaser, Coins, Trail, Scout, Maze, Divider)
 
-# Golden cases of tests/golden/make_helper_golden.py: (name, game, level, seed, rng seed, steps).
+# (golden name, game, level, action seed, generator seed, steps)
 CASES = [('helper_bolts_0', 'bolts', 0, 41, 3, 400), ('helper_bolts_1', 'bolts', 1, 42, 4, 400),
          ('helper_chaser_0', 'chaser', 0, 43, 0, 300),
          ('helper_chaser_1', 'chaser', 1, 44, 0, 300),
@@ -440,3 +442,7 @@ REGISTERS = {'bolts': [('X', 'hits')], 'chaser': [('P', 'bumps')],
              'divzero': [('P', 'left'), ('P', 'share')]}
 PLOT_KEYS = {'bolts': ['hit_frame', 'last_player_shot', 'last_marauder_shot'], 'chaser': [],
              'divzero': []}
+GENERATORS = ('numpy',)
+RAISES = {'divzero': ZeroDivisionError}
+FIELDS = ('game', 'level', 'rng_seed', 'actions', 'sprites', 'registers', 'reward_type',
+          'numpy_words', 'raised_at')

@@ -2,7 +2,7 @@
 classes the tests register with `pycolab_b200.compiler`.
 
 This module imports `pycolab.*` only, so it runs unchanged on the reference (the golden
-maker, tests/golden/make_scrolling_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  Three games:
 
   maze     a scrolly maze in this project's own words: an egocentric player, patrollers
@@ -325,14 +325,24 @@ class EarlyAsker(prefab_drapes.Scrolly):
     self._stay(the_plot)
 
 
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (MazePlayer, MazePatroller, MazeWalls, MazeCoins, SamplerPlayer, Watcher,
            SamplerWalls, Gems, EarlyAsker)
 
-# Golden cases of tests/golden/make_scrolling_golden.py: (name, level, seed, steps).
-CASES = [('scrolling_sampler_0', 0, 11, 400), ('scrolling_sampler_1', 1, 12, 400)]
-N_ACTIONS = 10                      # sampler actions; the last quits
-SPRITES = 'Pe'
-SCROLLYS = '#*'
-REGISTERS = [('P', 'steps'), ('e', 'on_gem'), ('e', 'sees_gems'), ('#', 'calls'),
-             ('*', 'taken')]
-PLOT_KEYS = ['gems']
+# (golden name, game, level, action seed, generator seed, steps)
+CASES = [('scrolling_sampler_0', 'sampler', 0, 11, None, 400),
+         ('scrolling_sampler_1', 'sampler', 1, 12, None, 400)]
+GAMES = {'sampler': make_sampler}
+N_ACTIONS = {'sampler': 10}         # the last quits
+SPRITES = {'sampler': 'Pe'}
+REGISTERS = {'sampler': [('P', 'steps'), ('e', 'on_gem'), ('e', 'sees_gems'), ('#', 'calls'),
+                         ('*', 'taken')]}
+PLOT_KEYS = {'sampler': ['gems']}
+GENERATORS = ()
+RAISES = {}
+# Each Scrolly's corner every frame, and its whole_pattern at the end, under 'pattern_' + name.
+SCROLLYS = {'sampler': '#*'}
+PATTERNS = {'sampler': {'walls': '#', 'gems': '*'}}
+FIELDS = ('level', 'actions', 'sprites', 'registers', 'corners', 'reward_type',
+          'pattern_walls', 'pattern_gems')

@@ -2,7 +2,7 @@
 classes the tests register with `pycolab_b200.compiler`.
 
 This module imports `pycolab.*` only, so it runs unchanged on the reference (the golden
-maker, tests/golden/make_sprite_golden.py) and on this package (loaded through
+maker, tests/golden/make_registered_golden.py) and on this package (loaded through
 `compat.load_example`).  Three games:
 
   bounce   a breakout-like game on two levels: the ball is a plain Sprite with dy / dx
@@ -313,9 +313,11 @@ class Faller(plab_things.Sprite):
       self._position = self.Position(self._position.row + 1, self._position.col)
 
 
+# The classes a test registers, and the tables of the golden maker and the replays
+# (tests/registered_games.py).
 CLASSES = (Paddle, Ball, Bricks, Player, Walls, Wanderer, Blinker, Edge, Ghost, Marker, Faller)
 
-# Golden cases of tests/golden/make_sprite_golden.py: (name, game, level, seed, rng seed, steps).
+# (golden name, game, level, action seed, generator seed, steps)
 CASES = [('sprite_bounce_0', 'bounce', 0, 21, 5, 400), ('sprite_bounce_1', 'bounce', 1, 22, 6, 400),
          ('sprite_sampler_0', 'sampler', 0, 23, 0, 300),
          ('sprite_sampler_1', 'sampler', 1, 24, 0, 300),
@@ -330,3 +332,7 @@ REGISTERS = {'bounce': [('o', 'dy'), ('o', 'dx'), ('o', '_serve')],
                          ('c', 'step'), ('c', 'walked'), ('x', '_mark')],
              'fallen': []}
 PLOT_KEYS = {'bounce': ['lives'], 'sampler': ['marks'], 'fallen': []}
+GENERATORS = ('numpy',)
+RAISES = {'fallen': IndexError}
+FIELDS = ('game', 'level', 'rng_seed', 'actions', 'sprites', 'registers', 'reward_type',
+          'numpy_words', 'raised_at')

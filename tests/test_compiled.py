@@ -1,9 +1,9 @@
 """CPU tests of the compiled step program (`pycolab_b200.compiler`, csrc/compiled.cu).
 
   - what the compiler accepts and refuses, with the source line in the message;
-  - the oracle interpreter (oracle/compiled.py) running the compiled words reproduces the
-    reference's trajectories of tests/compiled_games.py (tests/golden/compiled_*.npz) and,
-    with the reference present, of its own classics examples;
+  - with the reference present, the oracle interpreter (oracle/compiled.py) running the
+    compiled words of its own classics examples reproduces their goldens (the games of
+    tests/compiled_games.py replay theirs in test_registered_goldens.py);
   - pcl_bind_code's checks, on handles that never reach a device;
   - the kernel keeps its operand stack out of local memory.
 """
@@ -24,7 +24,6 @@ from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
-from pycolab_b200.prefab_parts import sprites as b_sprites
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -32,35 +31,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 @pytest.fixture(scope='module')
 def games():
   yield from rg.registered('compiled_games.py')
-
-
-@pytest.mark.parametrize('name', gc.names('compiled_'))
-def test_oracle_reproduces_compiled_golden(games, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  engine = games.GAMES[game](level)
-  lowered = lowering.lower(engine)
-  assert lowered.program == _lib.PROG_COMPILED
-  assert lowered.float_reward == (game == 'lava')
-  regs, keys = games.REGISTERS[game], games.PLOT_KEYS[game]
-  slot = {(ch, attr): compiler.registered(type(engine.things[ch])).attrs.index(attr)
-          for ch, attr in regs}
-  order = [key for key, _ in lowered.plot_keys]
-  sprites, registers, types = [], [], []
-
-  def on_frame(world, out):
-    sprites.append([[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]
-                    for w in (world.things[ch] for ch in games.SPRITES[game])])
-    registers.append([world.things[ch].regs[slot[ch, attr]] for ch, attr in regs] +
-                     [world.plot.regs[order.index(key)] for key in keys])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    assert world.error == 0
-  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
 
 
 def test_registered_class_wins_and_unregistered_is_refused(games):
@@ -105,16 +75,6 @@ def test_float_rewards_select_the_float64_output(games):
 
 
 # ---------------------------------------------------------------- the subset --
-
-class _W(b_sprites.MazeWalker):
-  def __init__(self, corner, position, character):
-    super(_W, self).__init__(corner, position, character, impassable='#')
-    self.n = 0
-
-
-def _walker(update):
-  return type('Case', (_W,), {'update': update, '__module__': __name__})
-
 
 # Each refused construct, as a walker whose update() has it on the marked line.
 def _loop(self, actions, board, layers, backdrop, things, the_plot):
@@ -179,13 +139,7 @@ REFUSED = [(_loop, 'For'), (_float_math, 'literal 0.5'), (_other_call, 'the_plot
 
 @pytest.mark.parametrize('update,what', REFUSED, ids=[u.__name__ for u, _ in REFUSED])
 def test_refused_construct_names_class_line_and_construct(update, what):
-  import inspect
-  lines, first = inspect.getsourcelines(update)
-  marked = [first + i for i, line in enumerate(lines) if '# REFUSED' in line]
-  with pytest.raises(NotLoweredError) as e:
-    compiler.compile_class(_walker(update))
-  msg = str(e.value)
-  assert 'Case' in msg and 'line %d' % marked[0] in msg and what in msg, msg
+  msg = rg.assert_refused(rg.walker(update), what)
   assert '# REFUSED' in msg, msg                  # the source line itself
 
 
@@ -209,7 +163,7 @@ def _accepted(self, actions, board, layers, backdrop, things, the_plot):
 
 
 def test_accepted_constructs_compile():
-  comp = compiler.compile_class(_walker(_accepted))
+  comp = compiler.compile_class(rg.walker(_accepted))
   assert comp.attrs == ['n'] and comp.keys == ['k'] and not comp.float_reward
   ops = {ins[0] for ins in comp.ir}
   assert {'MOVE', 'TELEPORT', 'IN', 'EQ2', 'FLOORDIV', 'MOD', 'BACKDROP', 'BOARD', 'FRAME',
@@ -220,7 +174,7 @@ def test_drape_only_and_sprite_only_constructs_are_checked():
   def fill(self, actions, board, layers, backdrop, things, the_plot):
     self.curtain[:] = True
   with pytest.raises(NotLoweredError, match='curtain write in a sprite class'):
-    compiler.compile_class(_walker(fill))
+    compiler.compile_class(rg.walker(fill))
 
   def move(self, actions, board, layers, backdrop, things, the_plot):
     self._north(board, the_plot)

@@ -1,9 +1,8 @@
 """CPU tests of Backdrops with registered update() code on the compiled step program
 (`pycolab_b200.compiler` kind 'backdrop', PCL_OP_SETBACK / FILLBACK / ROLLBACK, program_arg[4]):
 
-  - the oracle interpreter (oracle/compiled.py) running the games of
-    tests/backdrop_games.py reproduces the reference's trajectories (tests/golden/backdrop_*),
-    the Backdrop's curtain, Plot keys and NumPy's generator included;
+  - the oracle interpreter (oracle/compiled.py) running the fluvial pair of
+    tests/backdrop_games.py reproduces the reference's fluvial goldens (tests/golden/fluvial_*);
   - with the reference present, its own fluvial_natation classes, registered, lower to the
     compiled program and replay its goldens (tests/golden/fluvial_*), and the fluvial pair of
     tests/backdrop_games.py compiles to the same words;
@@ -57,21 +56,6 @@ def _oracle_trajectory(make_engine, actions, rng_seed=None, keys=()):
   got = tj.run_trajectory(lambda: ocompiled.make_world(lowered, words), actions,
                           on_frame=on_frame)
   return got, sprites, curtains, plot, words
-
-
-@pytest.mark.parametrize('name', gc.names('backdrop_'))
-def test_oracle_runs_backdrop_games_like_the_reference(games, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  got, sprites, curtains, plot, words = _oracle_trajectory(
-      lambda: games.GAMES[game](level), g['actions'].tolist(), int(g['rng_seed'][0]),
-      games.PLOT_KEYS[game])
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['backdrops'], np.stack(curtains))
-  np.testing.assert_array_equal(g['plot_keys'], np.array(plot))
-  if words is not None:
-    assert words[0] == g['numpy_words'].tolist()
 
 
 @pytest.mark.parametrize('name', gc.names('fluvial_'))
@@ -237,14 +221,7 @@ REFUSED = [(_attribute, 'a Backdrop has no registers'), (_column_slice, 'a band 
 
 @pytest.mark.parametrize('update,what', REFUSED, ids=[u.__name__ for u, _ in REFUSED])
 def test_refused_construct_names_class_line_and_construct(update, what):
-  import inspect
-  lines, first = inspect.getsourcelines(update)
-  line = first + [i for i, l in enumerate(lines) if '# REFUSED' in l][0]
-  with pytest.raises(NotLoweredError) as e:
-    compiler.compile_class(_backdrop(update))
-  msg = str(e.value)
-  assert 'Case.update, line {}:'.format(line) in msg, msg
-  assert what in msg, msg
+  rg.assert_refused(_backdrop(update), what)
 
 
 def _sprite_writes_backdrop(self, actions, board, layers, backdrop, things, the_plot):

@@ -1,9 +1,8 @@
 """CPU tests of helper calls in compiled update() code: the game's own methods and module
 functions, inlined by `pycolab_b200.compiler` into the words the interpreter already runs.
 
-  - the oracle interpreter (oracle/compiled.py) running the games of tests/helper_games.py
-    reproduces the reference's trajectories (tests/golden/helper_*), registers included,
-    and latches PCL_ENV_ERR_ARITH where the reference raised ZeroDivisionError;
+  - the oracle interpreter (oracle/compiled.py) latches PCL_ENV_ERR_ARITH where the reference
+    raised ZeroDivisionError (tests/golden/helper_divzero.npz), after every frame before it;
   - virtual dispatch: subclasses overriding a helper get their own code, the others share;
   - role-only helpers without an early return link to the words of their pasted-in twin;
   - a helper's local slots are freed when its call ends;
@@ -18,8 +17,6 @@ import pytest
 
 import golden_cases as gc
 import registered_games as rg
-import trajectory as tj
-from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
 from pycolab_b200.errors import NotLoweredError
@@ -31,64 +28,10 @@ def games():
   yield from rg.registered('helper_games.py')
 
 
-def _world_registers(world, engine, regs, keys, plot_keys):
-  out = []
-  for ch, name in regs:
-    comp = compiler.registered(type(engine.things[ch]))
-    slot = comp.slot(name)
-    out += world.things[ch].regs[slot:slot + comp.width(name)]
-  return out + [world.plot.regs[plot_keys.index(k)] for k in keys]
-
-
-def _world_sprites(world, chars):
-  return [[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]
-          for w in (world.things[ch] for ch in chars)]
-
-
-def _oracle(games, g):
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  engine = games.GAMES[game](level)
-  lowered = lowering.lower(engine)
-  keys = [k for k, _ in lowered.plot_keys]
-  words = ocompiled.seeded_words(lowered, int(g['rng_seed'][0])) if lowered.rng_streams else None
-  sprites, registers, types = [], [], []
-
-  def on_frame(world, out):
-    sprites.append(_world_sprites(world, games.SPRITES[game]))
-    registers.append(_world_registers(world, engine, games.REGISTERS[game],
-                                      games.PLOT_KEYS[game], keys))
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    assert world.error == 0
-  make = lambda: ocompiled.make_world(lowered, words)
-  return make, on_frame, sprites, registers, types, words
-
-
-@pytest.mark.parametrize('name', [n for n in gc.names('helper_') if n != 'helper_divzero'])
-def test_oracle_runs_helper_games_like_the_reference(games, name):
-  g = gc.load(name)
-  make, on_frame, sprites, registers, types, words = _oracle(games, g)
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers).reshape(len(types), -1))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  if words is not None:
-    assert words[0] == g['numpy_words'].tolist()
-
-
 def test_oracle_latches_arith_where_the_reference_divided_by_zero(games):
-  g = gc.load('helper_divzero')
-  make, on_frame, sprites, registers, types, _ = _oracle(games, g)
-  world = make()
-  boards = [world.its_showtime()[0]]
-  at = int(g['raised_at'][0])
-  for a in g['actions'][:at].tolist():
-    boards.append(world.play(a)[0])
-    on_frame(world, (None, None))
-  np.testing.assert_array_equal(g['boards'], np.array(boards))
-  np.testing.assert_array_equal(g['registers'][1:], np.array(registers))
-  world.play(int(g['actions'][at]))
-  assert world.error & _lib.ENV_ERR_ARITH
+  """helper_divzero on the oracle: every frame before the reference's ZeroDivisionError,
+  then PCL_ENV_ERR_ARITH (a case of test_registered_goldens too)."""
+  rg.assert_oracle_replays(games, 'helper_divzero')
 
 
 # ------------------------------------------------------------ virtual dispatch --

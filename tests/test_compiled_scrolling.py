@@ -5,13 +5,12 @@ MazeWalkers in registered update() code (`pycolab_b200.compiler`, csrc/compiled.
   - limits refused at lowering: registers, scrolling groups, pattern shapes;
   - the oracle interpreter (oracle/compiled.py) running the compiled maze of
     tests/scrolling_games.py reproduces the reference's scrolly_maze trajectories
-    (tests/golden/scrolly_*.npz), and the compiled sampler those of tests/golden/scrolling_*;
+    (tests/golden/scrolly_*.npz); the sampler's goldens replay in test_registered_goldens.py;
   - with the reference present, its own scrolly_maze classes compile unchanged;
   - pcl_bind_code / pcl_create checks of the new opcodes, on handles that reach no device.
 """
 
 import ctypes as C
-import inspect
 import os
 
 import numpy as np
@@ -68,43 +67,6 @@ def test_oracle_runs_compiled_maze_like_the_reference(games, name):
                           on_frame=on_frame)
   tj.assert_same_trajectory(g, got, name)
   np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-
-
-def _sampler_trajectory(games, g):
-  engine = games.make_sampler(int(g['level'][0]))
-  attrs = {ch: compiler.registered(type(ent)).attrs for ch, ent in engine.things.items()}
-  lowered = lowering.lower(engine)
-  keys = [k for k, _ in lowered.plot_keys]
-  sprites, registers, corners, types, worlds = [], [], [], [], []
-
-  def on_frame(world, out):
-    sprites.append(_sprite_rows(world, games.SPRITES))
-    registers.append([world.things[ch].regs[attrs[ch].index(attr)]
-                      for ch, attr in games.REGISTERS] +
-                     [world.plot.regs[keys.index(k)] for k in games.PLOT_KEYS])
-    corners.append([list(world.things[ch].corner) for ch in games.SCROLLYS])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    assert world.error == 0
-
-  def make():
-    worlds.append(ocompiled.make_world(lowered))
-    return worlds[-1]
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  patterns = [worlds[-1].things[ch].pattern for ch in games.SCROLLYS]
-  return got, sprites, registers, corners, types, patterns
-
-
-@pytest.mark.parametrize('name', gc.names('scrolling_'))
-def test_oracle_runs_compiled_sampler_like_the_reference(games, name):
-  g = gc.load(name)
-  got, sprites, registers, corners, types, patterns = _sampler_trajectory(games, g)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['corners'], np.array(corners))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  for ch, pattern in zip(games.SCROLLYS, patterns):
-    np.testing.assert_array_equal(g['pattern_' + {'#': 'walls', '*': 'gems'}[ch]], pattern)
 
 
 def test_oracle_raises_on_postscroll_before_the_move(games):
@@ -218,12 +180,7 @@ WALKER_REFUSED = [(_walker_pattern, 'self.whole_pattern in a sprite class'),
                          [(u, w, _walker) for u, w in WALKER_REFUSED],
                          ids=[u.__name__ for u, _ in SCROLLY_REFUSED + WALKER_REFUSED])
 def test_refused_construct_names_class_line_and_construct(update, what, make):
-  lines, first = inspect.getsourcelines(update)
-  marked = [first + i for i, line in enumerate(lines) if '# REFUSED' in line]
-  with pytest.raises(NotLoweredError) as e:
-    compiler.compile_class(make(update))
-  msg = str(e.value)
-  assert 'Case' in msg and 'line %d' % marked[0] in msg and what in msg, msg
+  rg.assert_refused(make(update), what)
 
 
 def test_plain_drapes_keep_refusing_motion_helpers_and_patterns():

@@ -2,9 +2,8 @@
 registered update() code sets their own position and visibility (`pycolab_b200.compiler`,
 PCL_OP_SETFIELD in csrc/compiled.cu).
 
-  - the oracle interpreter (oracle/compiled.py) running the games of
-    tests/sprite_games.py reproduces the reference's trajectories (tests/golden/sprite_*),
-    registers and position attributes included, and raises IndexError where it did;
+  - the oracle interpreter (oracle/compiled.py) raises IndexError where the reference fell
+    (tests/golden/sprite_fallen.npz), after every frame before it;
   - the forms the compiler accepts and the ones it refuses, with the source line;
   - what lowering refuses: registers, position values, a plain Sprite's virtual_position;
   - pcl_bind_code / pcl_create checks of SETFIELD and program_arg[3], on handles that reach
@@ -15,13 +14,10 @@ PCL_OP_SETFIELD in csrc/compiled.cu).
 import ctypes as C
 import os
 
-import numpy as np
 import pytest
 
-import golden_cases as gc
 import registered_games as rg
 import test_kernel_resources as resources
-import trajectory as tj
 from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
@@ -34,67 +30,10 @@ def games():
   yield from rg.registered('sprite_games.py')
 
 
-def _world_registers(world, engine, regs, keys, plot_keys):
-  out = []
-  for ch, name in regs:
-    comp = compiler.registered(type(engine.things[ch]))
-    slot = comp.slot(name)
-    out += world.things[ch].regs[slot:slot + comp.width(name)]
-  return out + [world.plot.regs[plot_keys.index(k)] for k in keys]
-
-
-def _world_sprites(world, lowered, chars):
-  rows = []
-  for ch in chars:
-    w = world.things[ch]
-    plain = (lowered.program_arg[3] >> lowered.sprite_chars.index(ch)) & 1
-    v = (w.row, w.col) if plain else (w.vrow, w.vcol)   # a plain Sprite has no virtual position
-    rows.append([w.row, w.col, int(bool(w.visible)), v[0], v[1]])
-  return rows
-
-
-def _oracle_trajectory(games, g):
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  engine = games.GAMES[game](level)
-  lowered = lowering.lower(engine)
-  keys = [k for k, _ in lowered.plot_keys]
-  words = ocompiled.seeded_words(lowered, int(g['rng_seed'][0])) if lowered.rng_streams else None
-  sprites, registers, types = [], [], []
-
-  def on_frame(world, out):
-    sprites.append(_world_sprites(world, lowered, games.SPRITES[game]))
-    registers.append(_world_registers(world, engine, games.REGISTERS[game],
-                                      games.PLOT_KEYS[game], keys))
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    assert world.error == 0
-  make = lambda: ocompiled.make_world(lowered, words)
-  return lowered, make, on_frame, sprites, registers, types, words
-
-
-@pytest.mark.parametrize('name', [n for n in gc.names('sprite_') if n != 'sprite_fallen'])
-def test_oracle_runs_sprite_games_like_the_reference(games, name):
-  g = gc.load(name)
-  lowered, make, on_frame, sprites, registers, types, words = _oracle_trajectory(games, g)
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers).reshape(len(types), -1))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  if words is not None:
-    assert words[0] == g['numpy_words'].tolist()
-
-
 def test_oracle_raises_where_the_reference_fell(games):
-  g = gc.load('sprite_fallen')
-  lowered, make, on_frame, sprites, registers, types, _ = _oracle_trajectory(games, g)
-  world = make()
-  boards = [world.its_showtime()[0]]
-  at = int(g['raised_at'][0])
-  for a in g['actions'][:at].tolist():
-    boards.append(world.play(a)[0])
-  np.testing.assert_array_equal(g['boards'], np.array(boards))
-  with pytest.raises(IndexError):
-    world.play(int(g['actions'][at]))
+  """sprite_fallen on the oracle: every frame before the reference's IndexError, then the
+  IndexError (a case of test_registered_goldens too)."""
+  rg.assert_oracle_replays(games, 'sprite_fallen')
 
 
 # ------------------------------------------------------------ the subset --
@@ -185,14 +124,7 @@ SPRITE_REFUSED = [(_bare_tuple, 'bare tuple'), (_north, '_north in a plain class
 @pytest.mark.parametrize('update,what', SPRITE_REFUSED,
                          ids=[u.__name__ for u, _ in SPRITE_REFUSED])
 def test_refused_construct_names_class_line_and_construct(update, what):
-  import inspect
-  lines, first = inspect.getsourcelines(update)
-  line = first + [i for i, l in enumerate(lines) if '# REFUSED' in l][0]
-  with pytest.raises(NotLoweredError) as e:
-    compiler.compile_class(_sprite(update))
-  msg = str(e.value)
-  assert 'Case.update, line {}:'.format(line) in msg, msg
-  assert what in msg, msg
+  rg.assert_refused(_sprite(update), what)
 
 
 def _walker_writes_position(self, actions, board, layers, backdrop, things, the_plot):

@@ -3,8 +3,6 @@
 
   - the draw forms the compiler accepts, through aliased imports too, and the forms it
     refuses, with the class, the source line and the construct;
-  - the oracle (oracle/compiled.py) reproduces the reference's trajectories of
-    tests/drawn_games.py (tests/golden/drawn_*.npz), down to both generators' final words;
   - the oracle's restatement of the draws equals NumPy's RandomState and Python's Random
     in value and in the words consumed, over the edge ranges and across a twist;
   - pcl_create / pcl_bind_state / pcl_bind_code refuse bad RNG slots, on handles that never
@@ -13,19 +11,15 @@
 """
 
 import ctypes as C
-import inspect
 import random
 
 import numpy as np
 import pytest
 
 import boundary_sweep
-import golden_cases as gc
 import registered_games as rg
-import trajectory as tj
 from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compiler, lowering
-from pycolab_b200.prefab_parts import sprites as b_sprites
 
 SEQ = (1, 2, 3)
 
@@ -59,20 +53,10 @@ def test_float_draw_on_either_side_of_the_comparison():
       self.n = 1
     if random.random() != -1:
       self.n = 2
-  comp = compiler.compile_class(_walker(update))
+  comp = compiler.compile_class(rg.walker(update))
   cmps = [ins for ins in comp.ir if ins[0] == 'RANDCMP']
   assert [c[2] for c in cmps] == [2, 1]          # 0.25 > x as x < 0.25; x != -1
   assert [c[1] for c in cmps] == [('rng', 'numpy'), ('rng', 'python')]
-
-
-class _W(b_sprites.MazeWalker):
-  def __init__(self, corner, position, character):
-    super(_W, self).__init__(corner, position, character, impassable='#')
-    self.n = 0
-
-
-def _walker(update):
-  return type('Case', (_W,), {'update': update, '__module__': __name__})
 
 
 # Each refused draw, as a walker whose update() has it on the marked line.
@@ -162,12 +146,7 @@ REFUSED = [(_size, 'the call np.random.randint()'), (_dtype, 'the call np.random
 
 @pytest.mark.parametrize('update,what', REFUSED, ids=[u.__name__ for u, _ in REFUSED])
 def test_refused_draw_names_class_line_and_construct(update, what):
-  lines, first = inspect.getsourcelines(update)
-  marked = [first + i for i, line in enumerate(lines) if '# REFUSED' in line]
-  with pytest.raises(compiler.NotLoweredError) as e:
-    compiler.compile_class(_walker(update))
-  msg = str(e.value)
-  assert 'Case' in msg and 'line %d' % marked[0] in msg and what in msg, msg
+  msg = rg.assert_refused(rg.walker(update), what)
   assert '# REFUSED' in msg, msg
 
 
@@ -181,43 +160,6 @@ def test_games_without_draws_lower_with_no_streams():
       assert not lowered.needs_rng
   finally:
     compiler.unregister(*mod.CLASSES)
-
-
-# ------------------------------------------------------------------ the oracle --
-
-def run_oracle(games, g):
-  """The oracle's trajectory of golden `g`, its per-frame records and final words."""
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  lowered = lowering.lower(games.GAMES[game](level))
-  words = ocompiled.seeded_words(lowered, int(g['rng_seed'][0]))
-  regs = games.REGISTERS[game]
-  slot = {(ch, attr): compiler.registered(type(games.GAMES[game](level).things[ch])).attrs.index(
-      attr) for ch, attr in regs}
-  sprites, registers, types = [], [], []
-
-  def on_frame(world, out):
-    sprites.append([[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]
-                    for w in (world.things[ch] for ch in games.SPRITES[game])])
-    registers.append([world.things[ch].regs[slot[ch, attr]] for ch, attr in regs])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    assert world.error == 0
-  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered, words), g['actions'].tolist(),
-                          on_frame=on_frame)
-  final = dict(zip(lowered.rng_streams, words))
-  return got, sprites, registers, types, final
-
-
-@pytest.mark.parametrize('name', gc.names('drawn_'))
-def test_oracle_reproduces_drawn_golden(games, name):
-  g = gc.load(name)
-  got, sprites, registers, types, final = run_oracle(games, g)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'].reshape(len(types), -1),
-                                np.array(sprites).reshape(len(types), -1))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  assert final['numpy'] == g['numpy_words'].tolist()
-  assert final['python'] == g['python_words'].tolist()
 
 
 # ------------------------------------------------------- the draw restatement --

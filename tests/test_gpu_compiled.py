@@ -1,11 +1,10 @@
 """GPU tests of the compiled step program (csrc/compiled.cu): registered update() code of
-tests/compiled_games.py on the H100, against the reference's trajectories
-(tests/golden/compiled_*.npz) and the oracle interpreter (oracle/compiled.py)."""
+tests/compiled_games.py on the H100, against the oracle interpreter (oracle/compiled.py).
+Its goldens replay in test_gpu_registered_goldens.py."""
 
 import numpy as np
 import pytest
 
-import golden_cases as gc
 import registered_games as rg
 import trajectory as tj
 from oracle import compiled as ocompiled
@@ -17,36 +16,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope='module')
 def games():
   yield from rg.registered('compiled_games.py', 'OffBoardDrape', 'DivideDrape')
-
-
-@pytest.mark.parametrize('name', gc.names('compiled_'))
-def test_facade_replays_compiled_golden(games, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  regs, keys = games.REGISTERS[game], games.PLOT_KEYS[game]
-  sprites, registers, types, rewards, reg_types = [], [], [], [], []
-
-  def on_frame(env, out):
-    sprites.append([[s.position[0], s.position[1], int(bool(s.visible)),
-                     s.virtual_position[0], s.virtual_position[1]]
-                    for s in (env.things[ch] for ch in games.SPRITES[game])])
-    values = ([getattr(env.things[ch], attr) for ch, attr in regs] +
-              [env.the_plot[key] for key in keys])
-    registers.append([int(v) for v in values])
-    reg_types.append([type(v) for v in values])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-  got = tj.run_trajectory(lambda: games.GAMES[game](level), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  np.testing.assert_array_equal(g['reward_f64'], np.array(rewards))      # bit-exact sums
-  first = games.GAMES[game](0)            # the registers keep their Python types
-  want = [type(getattr(first.things[ch], attr)) for ch, attr in regs] + \
-         [type(first.the_plot[key]) for key in keys]
-  assert all(t == want for t in reg_types)
 
 
 def _oracle_frames(lowered, actions):

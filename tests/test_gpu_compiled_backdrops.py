@@ -1,6 +1,7 @@
 """GPU tests of Backdrops with registered update() code on the compiled step program
 (csrc/compiled.cu backdrop_step): the games of tests/backdrop_games.py on the H100, against
-the reference's trajectories (tests/golden/backdrop_*.npz, fluvial_*.npz), the hand-written
+the reference's fluvial trajectories (tests/golden/fluvial_*.npz; the others replay in
+test_gpu_registered_goldens.py), the hand-written
 PCL_PROG_CLASSICS river and the oracle interpreter (oracle/compiled.py)."""
 
 import numpy as np
@@ -40,17 +41,6 @@ def _facade_replay(make, g, keys=()):
   return plot
 
 
-@pytest.mark.parametrize('name', gc.names('backdrop_'))
-def test_facade_replays_backdrop_golden(games, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  np.random.seed(int(g['rng_seed'][0]))
-  plot = _facade_replay(lambda: games.GAMES[game](level), g, games.PLOT_KEYS[game])
-  np.testing.assert_array_equal(g['plot_keys'], np.array(plot))
-  _, key, pos = np.random.get_state()[:3]
-  assert np.append(key, pos).astype(np.uint32).tolist() == g['numpy_words'].tolist()
-
-
 @pytest.mark.parametrize('name', gc.names('fluvial_'))
 def test_facade_replays_fluvial_golden_with_the_compiled_pair(games, name):
   g = gc.load(name)
@@ -86,11 +76,6 @@ def test_compiled_fluvial_matches_the_classics_kernel(games, which):
   assert int((compiled.error_codes() != 0).sum()) == 0
 
 
-def _sample(rs):
-  return [int(e) for e in np.unique(np.concatenate(
-      [[0, 1, B - 2, B - 1], rs.choice(np.arange(2, B - 2), 28, replace=False)]))]
-
-
 def _backdrop_check(t, engine, worlds, outs):
   """Each sampled env's live curtain and un-occluded layers against its oracle world."""
   import torch
@@ -116,7 +101,7 @@ def test_backdrop_games_lockstep_against_the_oracle(games, game):
   eng = batched.BatchedEngine(lowered, batch=B, rng_seed=seed)
   rs = np.random.RandomState(9)
   actions = rs.randint(0, games.N_ACTIONS[game], size=(T, B)).astype(np.int32)
-  sample = _sample(rs)
+  sample = rg.sample_envs(rs, B)
   words = {e: (ocompiled.seeded_words(lowered[e % 2], seed + e) if lowered[0].rng_streams
                else None) for e in sample}
   eng.its_showtime()

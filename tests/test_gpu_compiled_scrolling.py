@@ -1,6 +1,7 @@
 """GPU tests of scrolling games on the compiled step program (csrc/compiled.cu): the games
 of tests/scrolling_games.py on the H100, against the reference's trajectories
-(tests/golden/scrolly_*.npz, scrolling_*.npz), the hand-written scrolly_maze kernel and the
+(tests/golden/scrolly_*.npz; the sampler's replay in test_gpu_registered_goldens.py), the
+hand-written scrolly_maze kernel and the
 oracle interpreter (oracle/compiled.py)."""
 
 import numpy as np
@@ -44,33 +45,6 @@ def test_facade_replays_scrolly_golden(games, name):
       g['actions'].tolist(), on_frame=lambda env, out: sprites.append(_sprite_rows(env, 'Pabc')))
   tj.assert_same_trajectory(g, got, name)
   np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-
-
-@pytest.mark.parametrize('name', gc.names('scrolling_'))
-def test_facade_replays_scrolling_golden(games, name):
-  g = gc.load(name)
-  level = int(g['level'][0])
-  sprites, registers, corners, types, envs = [], [], [], [], []
-
-  def on_frame(env, out):
-    sprites.append(_sprite_rows(env, games.SPRITES))
-    registers.append([int(getattr(env.things[ch], attr)) for ch, attr in games.REGISTERS] +
-                     [int(env.the_plot[key]) for key in games.PLOT_KEYS])
-    corners.append([list(env.things[ch]._northwest_corner) for ch in games.SCROLLYS])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-    if not envs or envs[-1] is not env:
-      envs.append(env)
-    assert isinstance(env.things['e'].sees_gems, bool)
-  got = tj.run_trajectory(lambda: games.make_sampler(level), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['corners'], np.array(corners))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  last = envs[-1].things
-  np.testing.assert_array_equal(g['pattern_walls'], last['#'].whole_pattern)
-  np.testing.assert_array_equal(g['pattern_gems'], last['*'].whole_pattern)
 
 
 def test_facade_raises_on_postscroll_before_the_move(games):
@@ -161,7 +135,7 @@ def test_batched_sampler_lockstep_against_the_oracle(games):
   engine = batched.BatchedEngine(lowered, batch=B)
   engine.its_showtime()
   rs = np.random.RandomState(3)
-  actions = rs.randint(0, games.N_ACTIONS, size=(T, B)).astype(np.int32)
+  actions = rs.randint(0, games.N_ACTIONS['sampler'], size=(T, B)).astype(np.int32)
   env_ids = [0, 1, 7, 2048, 4095]
   n = sampled_check.lockstep(engine, lambda e: ocompiled.make_world(lowered[e % 2]),
                              env_ids, actions, curtains='#*', sprites='Pe', pad_columns=True)

@@ -1,18 +1,15 @@
 """GPU tests of plain Sprites on the compiled step program (csrc/compiled.cu): the games of
-tests/sprite_games.py on the H100, against the reference's trajectories
-(tests/golden/sprite_*.npz) and the oracle interpreter (oracle/compiled.py)."""
+tests/sprite_games.py on the H100, against the oracle interpreter (oracle/compiled.py).
+Their goldens replay in test_gpu_registered_goldens.py."""
 
 import numpy as np
 import pytest
 
-import golden_cases as gc
 import registered_games as rg
-import trajectory as tj
+from registered_games import global_generators  # noqa: F401  (a fixture)
 from oracle import compiled as ocompiled
-from oracle import engine_model as em
 from oracle import sampled_check
 from pycolab_b200 import _lib, lowering, rendering
-from pycolab_b200 import things as b_things
 
 pytestmark = pytest.mark.gpu
 
@@ -24,97 +21,6 @@ def games():
   yield from rg.registered('sprite_games.py')
 
 
-def _sprite_rows(env, chars):
-  rows = []
-  for s in (env.things[ch] for ch in chars):
-    vp = getattr(s, 'virtual_position', s.position)
-    rows.append([s.position[0], s.position[1], int(bool(s.visible)), vp[0], vp[1]])
-  return rows
-
-
-def _register_row(env, regs, keys):
-  out = []
-  for ch, name in regs:
-    value = getattr(env.things[ch], name)
-    out += [int(x) for x in value] if isinstance(value, tuple) else [int(value)]
-  return out + [int(env.the_plot[key]) for key in keys]
-
-
-@pytest.mark.parametrize('name', [n for n in gc.names('sprite_') if n != 'sprite_fallen'])
-def test_facade_replays_sprite_golden(games, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  np.random.seed(int(g['rng_seed'][0]))
-  sprites, registers = [], []
-  types = {('o', '_serve'): b_things.Sprite.Position, ('w', '_home'): b_things.Sprite.Position,
-           ('x', '_mark'): tuple, ('o', 'dy'): int, ('w', 'seen'): int}
-
-  def on_frame(env, out):
-    sprites.append(_sprite_rows(env, games.SPRITES[game]))
-    registers.append(_register_row(env, games.REGISTERS[game], games.PLOT_KEYS[game]))
-    for (ch, name), t in types.items():        # written back with the type it had
-      if ch in env.things:
-        assert type(getattr(env.things[ch], name)) is t, (ch, name)
-  got = tj.run_trajectory(lambda: games.GAMES[game](level), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['registers'], np.array(registers).reshape(len(sprites), -1))
-  _, key, pos = np.random.get_state()[:3]
-  assert np.append(key, pos).astype(np.uint32).tolist() == g['numpy_words'].tolist()
-
-
-def test_facade_raises_index_error_where_the_reference_did(games):
-  g = gc.load('sprite_fallen')
-  engine = games.make_fallen()
-  boards = [engine.its_showtime()[0].board.copy()]
-  at = int(g['raised_at'][0])
-  for a in g['actions'][:at].tolist():
-    boards.append(engine.play(a)[0].board.copy())
-  np.testing.assert_array_equal(g['boards'], np.array(boards))
-  with pytest.raises(IndexError):
-    engine.play(int(g['actions'][at]))
-
-
-def _plain_check(lowered_by_env, extra=None):
-  """on_step for lockstep: each plain Sprite's row, col and visible bit, every register
-  word, and the un-occluded layers, against the oracle worlds."""
-  def on_step(t, engine, worlds, outs):
-    import torch
-    ids = sorted(worlds)
-    idx = torch.as_tensor(ids, device=engine.device)
-    sprites = engine.sprites.index_select(0, idx).cpu().numpy()
-    drapes = engine.drapes.index_select(0, idx).cpu().numpy()
-    plot = engine.plot.index_select(0, idx).cpu().numpy()
-    layers = engine.unoccluded_layers(engine.chars).index_select(0, idx).cpu().numpy()
-    for k, e in enumerate(ids):
-      w, game = worlds[e], lowered_by_env(e)
-      assert w.error == 0
-      for s, ch in enumerate(engine.sprite_chars):
-        ent, rec = w.things[ch], sprites[k, s]
-        if (game.program_arg[3] >> s) & 1:
-          assert [rec[0], rec[1], rec[4] & 1] == [ent.row, ent.col, int(bool(ent.visible))], (t, e, ch)
-          words = list(rec[2:4]) + list(rec[5:])
-        else:
-          words = list(rec[_lib.S_AUX2 if game.egocentric[s] else _lib.S_AUX0:])
-        assert words[:len(ent.regs)] == ent.regs[:len(words)], (t, e, ch)
-      for d, ch in enumerate(engine.drape_chars):
-        if not game.drape_kind[d]:
-          assert list(drapes[k, d]) == w.things[ch].regs, (t, e, ch)
-      assert list(plot[k, _lib.P_AUX0:_lib.P_AUX0 + 4]) == w.plot.regs, (t, e)
-      want = em.unoccluded_layers_of(w.backdrop, w.things, engine.chars)
-      for c, ch in enumerate(engine.chars):
-        np.testing.assert_array_equal(layers[k, c], want[ch], err_msg=str((t, e, ch)))
-    if extra is not None:
-      extra(t, engine, worlds, outs)
-  return on_step
-
-
-def _sample(rs):
-  return [int(e) for e in np.unique(np.concatenate(
-      [[0, 1, B - 2, B - 1], rs.choice(np.arange(2, B - 2), 28, replace=False)]))]
-
-
 def test_bounce_lockstep_against_the_oracle(games):
   """B = 4096, both levels, auto-reset: sampled envs every step, the bricks' curtain, the
   ball's words and registers, and the generators' words at the end."""
@@ -124,13 +30,13 @@ def test_bounce_lockstep_against_the_oracle(games):
   eng = batched.BatchedEngine(lowered, batch=B, rng_seed=seed)
   rs = np.random.RandomState(7)
   actions = rs.randint(0, 4, size=(T, B)).astype(np.int32)
-  sample = _sample(rs)
+  sample = rg.sample_envs(rs, B)
   words = {e: ocompiled.seeded_words(lowered[e % 2], seed + e) for e in sample}
   eng.its_showtime()
   n = sampled_check.lockstep(
       eng, lambda e: ocompiled.make_world(lowered[e % 2], words[e]), sample, actions,
       curtains='=', sprites='P', pad_columns=True,
-      on_step=_plain_check(lambda e: lowered[e % 2]))
+      on_step=rg.register_check(lambda e: lowered[e % 2], layers=True))
   assert n == len(sample) * (T + 1)
   rng = eng.rng.cpu().numpy().view(np.uint32).reshape(B, 1, _lib.MT_WORDS)
   for e in sample:
@@ -148,7 +54,7 @@ def test_sampler_lockstep_against_the_oracle(games):
   eng.its_showtime()
   rs = np.random.RandomState(8)
   actions = rs.randint(0, 9, size=(T, B)).astype(np.int32)
-  sample = _sample(rs)
+  sample = rg.sample_envs(rs, B)
   seen = {'wrapped': 0, 'far': 0}
 
   def render_check(t, engine, worlds, outs):
@@ -171,10 +77,16 @@ def test_sampler_lockstep_against_the_oracle(games):
   n = sampled_check.lockstep(
       eng, lambda e: ocompiled.make_world(lowered[e % 2]), sample, actions,
       curtains='#x', sprites='Pw', pad_columns=True,
-      on_step=_plain_check(lambda e: lowered[e % 2], render_check))
+      on_step=rg.register_check(lambda e: lowered[e % 2], layers=True, extra=render_check))
   assert n == len(sample) * (T + 1)
   assert seen['wrapped'] > 0 and seen['far'] > 0
   assert int((eng.error_codes() != 0).sum()) == 0
+
+
+def test_facade_raises_index_error_where_the_reference_did(games, global_generators):  # noqa: F811
+  """sprite_fallen through the facade: every frame before the reference's IndexError, then
+  the IndexError (a case of test_gpu_registered_goldens too)."""
+  rg.assert_facade_replays(games, 'sprite_fallen')
 
 
 def test_only_the_envs_that_fall_latch_index_errors(games):

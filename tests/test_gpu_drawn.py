@@ -1,16 +1,12 @@
 """GPU tests of draws from the global generators in compiled code (csrc/compiled.cu
-PCL_OP_RANDINT / RANDCMP / PICK): tests/drawn_games.py on the H100, against the
-reference's trajectories (tests/golden/drawn_*.npz) and the oracle
-(oracle/compiled.py)."""
-
-import random
+PCL_OP_RANDINT / RANDCMP / PICK): tests/drawn_games.py on the H100, against the oracle
+(oracle/compiled.py).  Its goldens replay in test_gpu_registered_goldens.py."""
 
 import numpy as np
 import pytest
 
-import golden_cases as gc
 import registered_games as rg
-import trajectory as tj
+from registered_games import global_generators  # noqa: F401  (a fixture)
 from oracle import compiled as ocompiled
 from oracle import sampled_check
 from pycolab_b200 import _lib, lowering
@@ -21,50 +17,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope='module')
 def games():
   yield from rg.registered('drawn_games.py')
-
-
-def global_words(stream):
-  """The words of a global generator now."""
-  if stream == 'python':
-    return [int(w) for w in random.getstate()[1]]
-  _, key, pos = np.random.get_state()[:3]
-  return [int(w) for w in key] + [int(pos)]
-
-
-@pytest.fixture
-def global_generators():
-  """Leave NumPy's and Python's global generators as the test found them."""
-  np_state, py_state = np.random.get_state(), random.getstate()
-  yield
-  np.random.set_state(np_state)
-  random.setstate(py_state)
-
-
-@pytest.mark.parametrize('name', gc.names('drawn_'))
-def test_facade_replays_drawn_golden(games, global_generators, name):
-  g = gc.load(name)
-  game, level = bytes(g['game']).decode(), int(g['level'][0])
-  regs = games.REGISTERS[game]
-  sprites, registers, types = [], [], []
-
-  def on_frame(env, out):
-    sprites.append([[s.position[0], s.position[1], int(bool(s.visible)),
-                     s.virtual_position[0], s.virtual_position[1]]
-                    for s in (env.things[ch] for ch in games.SPRITES[game])])
-    registers.append([int(getattr(env.things[ch], attr)) for ch, attr in regs])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-  np.random.seed(int(g['rng_seed'][0]))
-  random.seed(int(g['rng_seed'][0]))
-  got = tj.run_trajectory(lambda: games.GAMES[game](level), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'].reshape(len(types), -1),
-                                np.array(sprites).reshape(len(types), -1))
-  np.testing.assert_array_equal(g['registers'], np.array(registers))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-  # the generators the game drew from continue where the reference's stopped
-  assert global_words('numpy') == g['numpy_words'].tolist()
-  assert global_words('python') == g['python_words'].tolist()
 
 
 def _device_regs(eng, envs):
@@ -138,11 +90,11 @@ def test_shards_reproduce_one_engine(games):
 
 @pytest.mark.parametrize('which', [0, 1, 2], ids=['numpy_randint', 'python_randrange',
                                                   'numpy_choice'])
-def test_empty_range_raises_value_error(games, global_generators, which):
+def test_empty_range_raises_value_error(games, global_generators, which):  # noqa: F811
   engine = games.make_empty(which)
   engine.its_showtime()
-  before = (global_words('numpy'), global_words('python'))
+  before = (rg.global_words('numpy'), rg.global_words('python'))
   engine.play(0)
   with pytest.raises(ValueError):
     engine.play(1)
-  assert (global_words('numpy'), global_words('python')) == before  # nothing drawn
+  assert (rg.global_words('numpy'), rg.global_words('python')) == before  # nothing drawn
