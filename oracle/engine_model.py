@@ -387,7 +387,8 @@ def layers_of(board, chars):
 def unoccluded_layers_of(backdrop, things, chars):
   """rendering.py:187-301 (`BaseUnoccludedObservationRenderer`): every layer is
   painted on its own — backdrop characters where the backdrop has them, a visible
-  sprite's cell, a drape's whole curtain — so several layers may be set at one
+  sprite's cell on top of that, a drape's whole curtain in place of it (paint_drape
+  copies the curtain over the layer, :278) — so several layers may be set at one
   position."""
   layers = {c: np.asarray(backdrop) == ord(c) for c in chars}
   for ch, ent in things.items():
@@ -397,7 +398,7 @@ def unoccluded_layers_of(backdrop, things, chars):
         layer[ent.row, ent.col] = True
       layers[ch] = layers[ch] | layer
     else:
-      layers[ch] = layers[ch] | ent.curtain
+      layers[ch] = np.array(ent.curtain, dtype=bool)
   return layers
 
 

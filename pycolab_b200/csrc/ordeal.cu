@@ -215,7 +215,7 @@ ordeal_step(const StepParams p) {
       unsigned m = 0;
       if (ch == p.sprite_char[0]) m = sprite_bit(pl, r, c0);
       else if (S > 1 && ch == p.sprite_char[1]) m = sprite_bit(dd, r, c0);
-      else if (D && ch == p.drape_char[0])
+      else if (D && ch == p.drape_char[0] && c0 < W)    // a segment past the board is pad
         m = bits16(sword + (int64_t)r * BW, c0) & ((1u << min(16, W - c0)) - 1u);
       if (m) paint_bits(px, m, ch);
     }

@@ -144,7 +144,11 @@ __global__ void __launch_bounds__(256) layers_kernel(const LayersParams p) {
     const int ncols = min(16, p.W - c0);
     uint4 px = make_uint4(0, 0, 0, 0);
     const int d = p.drape_of[k];
-    if (d >= 0) {
+    if (ncols <= 0) {
+      // A segment wholly past the board (pitch > ceil16(W)) is pad: zeros, and nothing is
+      // read.  (1u << ncols) would not mask it: the shift of a negative count gives 0, so
+      // the mask would be all ones and copy the bits past the window or the row.
+    } else if (d >= 0) {
       const int32_t* drec = p.drapes + ((int64_t)env * p.D + d) * PCL_DRAPE_WORDS;
       const int cr = p.scrolly[d] ? drec[PCL_D_CORNER_R] : 0;
       const int cc = p.scrolly[d] ? drec[PCL_D_CORNER_C] : 0;

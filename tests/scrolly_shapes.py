@@ -85,7 +85,7 @@ def shape_level(name, seed, corner=None):
   return open_level(seed, board, world, corner=corner)
 
 
-def facade_game(maze, board, beneath, margins=DEFAULT_MARGINS):
+def facade_game(maze, board, beneath, margins=DEFAULT_MARGINS, occlusion_in_layers=True):
   """pycolab_b200.games.scrolly_maze.make_game with scroll margins per drape ('#', '@')."""
   from pycolab_b200 import ascii_art
   from pycolab_b200.games import scrolly_maze as g
@@ -100,7 +100,24 @@ def facade_game(maze, board, beneath, margins=DEFAULT_MARGINS):
       drapes={'#': ascii_art.Partial(g.MazeDrape, scroll_margins=margins[0], **info.kwargs('#')),
               '@': ascii_art.Partial(g.CashDrape, scroll_margins=margins[1], **info.kwargs('@'))},
       update_schedule=[['#'], ['a', 'b', 'c', 'P'], ['@']],
-      z_order='abc@#P')
+      z_order='abc@#P', occlusion_in_layers=occlusion_in_layers)
+
+
+def lowered(game, pitch=None, repack=False):
+  """Lower a facade game; optionally widen its pitch (re-padding the backdrop) or re-pack
+  its patterns at the smallest pattern_words pcl_create accepts."""
+  from pycolab_b200 import lowering
+  low = lowering.lower(game)
+  if pitch is not None:
+    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
+    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
+    low.backdrop, low.pitch = backdrop, pitch
+  if repack:
+    words = min_pattern_words(low.cols, low.pattern_cols)
+    low.patterns = {d: lowering.pack_rows(lowering.unpack_rows(p, low.pattern_cols), words)
+                    for d, p in low.patterns.items()}
+    low.pattern_words = words
+  return low
 
 
 def oracle_world(maze, board, beneath, margins=DEFAULT_MARGINS):

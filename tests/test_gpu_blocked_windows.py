@@ -13,7 +13,7 @@ import pytest
 
 import scrolly_shapes as ss
 from oracle import sampled_check
-from test_gpu_shapes import _lowered, _walk
+from test_gpu_shapes import _walk
 
 pytestmark = pytest.mark.gpu
 
@@ -24,7 +24,7 @@ def test_share_levels_false(name):
   from pycolab_b200 import batched
   board, world, margins = ss.SHAPE[name]
   arts = [ss.open_level(60 + i, board, world, coin_density=0.4) for i in range(3)]
-  games = [_lowered(ss.facade_game(*a, margins=margins)) for a in arts]
+  games = [ss.lowered(ss.facade_game(*a, margins=margins)) for a in arts]
   B = 9
   eng = batched.BatchedEngine(games, batch=B, share_levels=False)
   assert eng.level is None
@@ -41,7 +41,7 @@ def test_rewritten_wall_pattern_is_read_again_after_rebinding():
   from pycolab_b200 import _lib, batched
   board, world, margins = ss.SHAPE['11x33']
   arts = [ss.open_level(70 + i, board, world) for i in range(2)]
-  games = [_lowered(ss.facade_game(*a, margins=margins)) for a in arts]
+  games = [ss.lowered(ss.facade_game(*a, margins=margins)) for a in arts]
   B = 6
   eng = batched.BatchedEngine(games, batch=B)
   eng.its_showtime()

@@ -17,7 +17,7 @@ import pytest
 import scrolly_shapes as ss
 from oracle import games as ogames
 from oracle import sampled_check
-from test_gpu_shapes import _lowered, _walk
+from test_gpu_shapes import _walk
 
 pytestmark = pytest.mark.gpu
 
@@ -136,7 +136,7 @@ def test_scripted_walks_scroll_both_windows(name):
   the 4-word fast paths."""
   board, world, margins = WIDE if name == 'wide_20x80' else ss.SHAPE[name]
   arts = [ss.open_level(80 + i, board, world, coin_density=0.3) for i in range(3)]
-  games = [_lowered(ss.facade_game(*a, margins=margins)) for a in arts]
+  games = [ss.lowered(ss.facade_game(*a, margins=margins)) for a in arts]
   B = 10
   pair = Pair(games, B)
   pair.lockstep(lambda e: ss.oracle_world(*arts[e % 3], margins=margins),

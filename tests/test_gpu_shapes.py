@@ -27,23 +27,6 @@ def _torch():
   return torch
 
 
-def _lowered(game, pitch=None, min_pattern_words=False):
-  """Lower a facade game; optionally widen its pitch (re-padding the backdrop) or re-pack
-  its patterns at the smallest pattern_words pcl_create accepts."""
-  from pycolab_b200 import lowering
-  low = lowering.lower(game)
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
-  if min_pattern_words:
-    words = ss.min_pattern_words(low.cols, low.pattern_cols)
-    low.patterns = {d: lowering.pack_rows(lowering.unpack_rows(p, low.pattern_cols), words)
-                    for d, p in low.patterns.items()}
-    low.pattern_words = words
-  return low
-
-
 def _step_vs_oracle(games, make_oracle, actions, check_curtains, sprite_chars, rng_seed=0,
                     on_step=None, crop=None):
   """Step a BatchedEngine (auto-reset) and B oracle worlds in lockstep; compare everything.
@@ -80,7 +63,7 @@ def _scrolly_case(name, B=10, T=150, n_levels=3, pitch=None, min_pattern_words=F
   board, world, margins = shape or ss.SHAPE[name]
   arts = [ss.open_level(40 + i, board, world, corner=None if corners is None else corners[i])
           for i in range(n_levels)]
-  games = [_lowered(ss.facade_game(*a, margins=margins), pitch, min_pattern_words) for a in arts]
+  games = [ss.lowered(ss.facade_game(*a, margins=margins), pitch, min_pattern_words) for a in arts]
   return _step_vs_oracle(
       games, lambda e: ss.oracle_world(*arts[e % n_levels], margins=margins),
       _walk(len(name), T, B), '#@', 'Pabc', on_step=on_step, crop=crop)
@@ -115,7 +98,7 @@ def test_scrolly_pitch_wider_than_the_board(name, pitch):
     from pycolab_b200 import levels
     from pycolab_b200.games import scrolly_maze
     arts = [levels.scrolly_maze_level(60 + i, world_shape=(97, 97)) for i in range(2)]
-    games = [_lowered(scrolly_maze.make_game(*a), pitch) for a in arts]
+    games = [ss.lowered(scrolly_maze.make_game(*a), pitch) for a in arts]
     _step_vs_oracle(games, lambda e: ogames.make_scrolly_maze(arts[e % 2][0], arts[e % 2][1], '+',
                                                               arts[e % 2][2]),
                     _walk(64, 100, 6), '#@', 'Pabc')

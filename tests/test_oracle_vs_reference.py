@@ -446,3 +446,57 @@ def test_shockwave_board_shapes(rows, cols):
   finally:
     ref_shock.LEVELS.pop()
   assert steps > 100
+
+
+# ----------------------------------------------- un-occluded layers, hand-built
+
+class _Thing(object):
+  def __init__(self, **kw):
+    self.__dict__.update(kw)
+
+
+def _unoccluded_scene(case):
+  """(backdrop, things, z_order) of a 5 x 7 board with drape 'D', sprites 'P' and 'a'."""
+  backdrop = np.full((5, 7), ord(' '), np.uint8)
+  backdrop[0, :] = ord('#')
+  curtain = np.zeros((5, 7), bool)
+  curtain[2, 1:5] = curtain[4, 6] = True
+  things = {'D': _Thing(is_sprite=False, curtain=curtain),
+            'P': _Thing(is_sprite=True, row=3, col=1, visible=True),
+            'a': _Thing(is_sprite=True, row=1, col=5, visible=True)}
+  if case == 'backdrop_holds_the_drape_character':
+    backdrop[1, :3] = backdrop[2, 1] = ord('D')
+  elif case == 'invisible_sprite_on_its_backdrop_character':
+    backdrop[3, 2:5] = ord('a')
+    things['a'].row, things['a'].col, things['a'].visible = 3, 3, False
+  elif case == 'sprite_under_a_drape':
+    things['a'].row, things['a'].col = 2, 3
+  return backdrop, things, 'aPD'
+
+
+@pytest.mark.parametrize('case', ['backdrop_holds_the_drape_character',
+                                  'invisible_sprite_on_its_backdrop_character',
+                                  'sprite_under_a_drape'])
+def test_unoccluded_layers_of_vs_reference_renderer(case):
+  """oracle.engine_model.unoccluded_layers_of == the reference's
+  BaseUnoccludedObservationRenderer painted as Engine._render paints it (engine.py:749-757):
+  the backdrop, then each visible sprite and each drape in z-order.  A drape's layer is its
+  curtain alone even where the backdrop holds the drape's character."""
+  refdriver._import()
+  from pycolab import rendering as ref_rendering
+  backdrop, things, z_order = _unoccluded_scene(case)
+  chars = sorted(set(chr(c) for c in np.unique(backdrop)) | set(things))
+  ref = ref_rendering.BaseUnoccludedObservationRenderer(5, 7, chars)
+  ref.clear()
+  ref.paint_all_of(backdrop)
+  for ch in z_order:
+    ent = things[ch]
+    if not ent.is_sprite:
+      ref.paint_drape(ch, ent.curtain)
+    elif ent.visible:
+      ref.paint_sprite(ch, (ent.row, ent.col))
+  want = ref.render().layers
+  got = em.unoccluded_layers_of(backdrop, things, chars)
+  assert sorted(got) == sorted(want)
+  for ch in chars:
+    np.testing.assert_array_equal(got[ch], want[ch], err_msg=ch)

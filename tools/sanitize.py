@@ -108,6 +108,15 @@ def main():
     g = mk()
     g.the_plot.this_chapter = mk.__name__[5:]
     run('ordeal_step ' + mk.__name__[5:], [g], 5, 5)
+  # pcl_layers and pcl_export_curtain at pitch 80 > ceil16(15): the sword is a bit-row drape,
+  # and the segments wholly past the board must read nothing of the rows behind the last one
+  g = ordeal.make_cavern()
+  g.the_plot.this_chapter = 'cavern'
+  eng = run('ordeal_step cavern pitch 80', [ss.lowered(g, pitch=80)], 5, 5)
+  eng.unoccluded_layers()
+  eng._curtain_bytes(0)
+  torch.cuda.synchronize()
+  print('ok layers / export at pitch 80')
   run('hello_step', [hello_world.make_game()], 5, 6)
   run('apprehend_step (device RNG)', [apprehend.make_game()], 5, 3, steps=30)
   run('shockwave_step', [shockwave.make_game(0), shockwave.make_game(levels.shockwave_level(3, 9, 33))][:1], 5, 5, steps=40)
