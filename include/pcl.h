@@ -162,8 +162,8 @@ typedef enum pcl_program {
                                 PCL_MT_WORDS], the words of Python's random.Random, continued across steps and
                                 auto-resets (random.sample at a start, randrange(4) per trial, normalvariate
                                 per paid frame).  normalvariate's accept test zz <= -log(u2) uses the device's
-                                double log (1 ulp), so it can decide otherwise than the host's libm only when
-                                zz lies within an ulp of -log(u2) */
+                                double log (1 ulp) away from the boundary, and the correctly rounded
+                                -log(u2) when zz lies within a few ulps of it */
   PCL_PROG_SEQUENCE_RECALL = 17, /* examples/research/lp-rnn/sequence_recall.py:107-317: sprite 'P' (MazeWalker,
                                 impassable '#', confined), drapes 'M' (bit rows in d_bits[0], rewritten
                                 whenever its record's AUX0, the set of covered lights '1'-'4' as bits 0-3,

@@ -24,7 +24,9 @@
 // (the pool method: _randbelow(4), (3), (2), (1)); with it set they come from the template
 // (the Python CueDrape drew them) and only update()'s draws come from d_rng.  normalvariate
 // is Lib/random.py's Kinderman-Monahan loop with correctly rounded f64 operations (no FMA
-// contraction); its accept test uses the device's double log (1 ulp), see include/pcl.h.
+// contraction).  Its accept test zz <= -log(u2) takes the device's double log (within 1 ulp)
+// unless zz lies within a few ulps of it; there it compares with the correctly rounded
+// -log(u2), as CPython's (glibc's) log gives it, from a double-double log.
 #include "pcl_device.cuh"
 #include "pcl_kernels.cuh"
 #include "pcl_mt.cuh"
@@ -44,8 +46,68 @@ __device__ __forceinline__ uint64_t cols_bits(int lo, int hi) {
   return upto & ~((1ull << lo) - 1ull);
 }
 
-// The minimum-blocks bound lets ptxas take the registers it needs (76): with the block size
-// alone it aims lower and spills around the draw loop.
+// Double-double arithmetic (Dekker / Knuth error-free transformations) for minus_log_rn.
+struct DD { double hi, lo; };
+__device__ __forceinline__ DD two_sum(double a, double b) {
+  const double s = __dadd_rn(a, b), bb = __dsub_rn(s, a);
+  return {s, __dadd_rn(__dsub_rn(a, __dsub_rn(s, bb)), __dsub_rn(b, bb))};
+}
+__device__ __forceinline__ DD fast_two_sum(double a, double b) {
+  const double s = __dadd_rn(a, b);
+  return {s, __dsub_rn(b, __dsub_rn(s, a))};
+}
+__device__ __forceinline__ DD dd_add(DD x, DD y) {
+  const DD s = two_sum(x.hi, y.hi);
+  return fast_two_sum(s.hi, __dadd_rn(s.lo, __dadd_rn(x.lo, y.lo)));
+}
+__device__ __forceinline__ DD dd_mul(DD x, DD y) {
+  const double p = __dmul_rn(x.hi, y.hi);
+  const double e = __fma_rn(x.hi, y.hi, -p);
+  return fast_two_sum(p, __dadd_rn(e, __dadd_rn(__dmul_rn(x.hi, y.lo), __dmul_rn(x.lo, y.hi))));
+}
+__device__ __forceinline__ DD dd_div(DD x, DD y) {
+  const double q1 = __ddiv_rn(x.hi, y.hi);
+  DD r = dd_add(x, dd_mul({-q1, 0.0}, y));
+  const double q2 = __ddiv_rn(r.hi, y.hi);
+  r = dd_add(r, dd_mul({-q2, 0.0}, y));
+  return dd_add(fast_two_sum(q1, q2), {__ddiv_rn(r.hi, y.hi), 0.0});
+}
+// 1 / (2j + 1), j = 0..22, as double-doubles.
+__constant__ DD kOddRecip[23] = {
+    {1.0, 0.0}, {0.3333333333333333, 1.850371707708594e-17},
+    {0.2, -1.1102230246251566e-17}, {0.14285714285714285, 7.93016446160826e-18},
+    {0.1111111111111111, 6.1679056923619804e-18}, {0.09090909090909091, -2.523234146875356e-18},
+    {0.07692307692307693, -4.270088556250602e-18}, {0.06666666666666667, 9.251858538542971e-19},
+    {0.058823529411764705, 8.163404592832033e-19}, {0.05263157894736842, 2.921639538487254e-18},
+    {0.047619047619047616, 2.64338815386942e-18}, {0.043478260869565216, 1.206764157201257e-18},
+    {0.04, -8.326672684688674e-19}, {0.037037037037037035, 2.05596856412066e-18},
+    {0.034482758620689655, 4.785444071660157e-19}, {0.03225806451612903, 8.953411488912552e-19},
+    {0.030303030303030304, -8.410780489584519e-19}, {0.02857142857142857, 8.921435019309293e-19},
+    {0.02702702702702703, -1.50030138462859e-18}, {0.02564102564102564, 8.896017825522087e-19},
+    {0.024390243902439025, -8.46206573647223e-19}, {0.023255813953488372, 3.2273925134452225e-19},
+    {0.022222222222222223, -8.480870326997723e-19}};
+// -log(u2) correctly rounded, 0 < u2 <= 1: log to about 100 bits as k ln 2 + 2 atanh(s),
+// u2 = 2^k m, m in [sqrt(1/2), sqrt(2)), s = (m - 1) / (m + 1), |s| < 0.172, summed to s^45.
+// Called only when zz lies within 2^-50 relative of the device's -log(u2), so kept out of line.
+__device__ __noinline__ double minus_log_rn(double u2) {
+  int k;
+  double m = frexp(u2, &k);
+  if (m < 0.70710678118654752) { m = __dmul_rn(m, 2.0); k -= 1; }
+  const DD s = dd_div({__dsub_rn(m, 1.0), 0.0}, two_sum(m, 1.0));
+  const DD s2 = dd_mul(s, s);
+  DD p = kOddRecip[22];
+#pragma unroll 1
+  for (int j = 21; j >= 0; --j) p = dd_add(dd_mul(p, s2), kOddRecip[j]);
+  const DD ln2 = {0.6931471805599452862, 2.3190468138462996154e-17};
+  const DD lg = dd_add(dd_mul(ln2, {(double)k, 0.0}), dd_mul(dd_mul(s, p), {2.0, 0.0}));
+  return -__dadd_rn(lg.hi, lg.lo);
+}
+
+// The minimum-blocks bound lets ptxas take the registers it needs (72, 87 with kNoisy): with
+// the block size alone it aims lower and spills around the draw loop.  kNoisy (reward_sigma
+// set) compiles the normal draws in; the noiseless kernel leaves them, and the registers of
+// their exact accept test, out.
+template <bool kNoisy>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, 4)
 cued_catch_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
@@ -83,7 +145,7 @@ cued_catch_step(const StepParams p) {
   int ttr = sp[SP].aux0;                           // PlayerSprite._trials_till_reward
 
   uint32_t* mt = reinterpret_cast<uint32_t*>(p.st.d_rng) + (int64_t)env * PCL_MT_WORDS;
-  const bool noisy = p.program_arg[0] != 0;
+  const bool noisy = kNoisy;                       // program_arg[0] != 0
   const int icd = p.program_arg[1], cd = p.program_arg[2];
   const bool always_show = p.program_arg[3] & 1;
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
@@ -138,14 +200,16 @@ cued_catch_step(const StepParams p) {
       pairs |= (int)((pool >> j) & 1u) << i;
       pool = (pool & ~(1u << j)) | (((pool >> (3 - i)) & 1u) << j);
       stage = i < 3 ? i + 1 : noisy_pay ? kU1 : trial_reset ? kTrial : kDone;
-    } else if (stage == kU1) {
+    } else if (kNoisy && stage == kU1) {
       u1 = __dmul_rn((double)r, 1.0 / 9007199254740992.0);
       stage = kU2;
-    } else if (stage == kU2) {                     // Lib/random.py normalvariate()
+    } else if (kNoisy && stage == kU2) {           // Lib/random.py normalvariate()
       const double u2 = __dsub_rn(1.0, __dmul_rn((double)r, 1.0 / 9007199254740992.0));
       z = __ddiv_rn(__dmul_rn(magic, __dsub_rn(u1, 0.5)), u2);
       const double zz = __dmul_rn(__dmul_rn(z, z), 0.25);   // z * z / 4.0, exactly
-      stage = zz <= -log(u2) ? (trial_reset ? kTrial : kDone) : kU1;
+      double bound = -log(u2);
+      if (fabs(__dsub_rn(zz, bound)) <= __dmul_rn(bound, 0x1p-50)) bound = minus_log_rn(u2);
+      stage = zz <= bound ? (trial_reset ? kTrial : kDone) : kU1;
     } else {
       choice = (int)r;
       stage = kDone;
@@ -301,7 +365,8 @@ int check_state(const pcl_spec&, const pcl_state& st) {
 }
 
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
-  return launch_step(cued_catch_step, p, kWarpsPerBlock, 0, s);
+  return launch_step(p.program_arg[0] ? cued_catch_step<true> : cued_catch_step<false>, p,
+                     kWarpsPerBlock, 0, s);
 }
 
 }  // namespace

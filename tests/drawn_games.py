@@ -202,6 +202,81 @@ def make_edges(level):
                                      drapes={'x': Edges})
 
 
+# ----------------------------------------------------------------- thresholds --
+# Twelve float draws from each generator every frame, each against a literal with one of the
+# six comparisons: against 0.5 with the draw on the left, then against 0.25 with the literal
+# on the left.  Bit k of `hits` is draw k's outcome, NumPy's draws first.
+
+class Thresholds(plab_things.Drape):
+
+  def __init__(self, curtain, character):
+    super(Thresholds, self).__init__(curtain, character)
+    self.hits = 0
+
+  def update(self, actions, board, layers, backdrop, things, the_plot):
+    self.hits = 0
+    if np.random.rand() < 0.5:
+      self.hits += 1
+    if np.random.rand() <= 0.5:
+      self.hits += 2
+    if np.random.rand() > 0.5:
+      self.hits += 4
+    if np.random.rand() >= 0.5:
+      self.hits += 8
+    if np.random.rand() == 0.5:
+      self.hits += 16
+    if np.random.rand() != 0.5:
+      self.hits += 32
+    if 0.25 < np.random.rand():
+      self.hits += 64
+    if 0.25 <= np.random.rand():
+      self.hits += 128
+    if 0.25 > np.random.rand():
+      self.hits += 256
+    if 0.25 >= np.random.rand():
+      self.hits += 512
+    if 0.25 == np.random.rand():
+      self.hits += 1024
+    if 0.25 != np.random.rand():
+      self.hits += 2048
+    if random.random() < 0.5:
+      self.hits += 4096
+    if random.random() <= 0.5:
+      self.hits += 8192
+    if random.random() > 0.5:
+      self.hits += 16384
+    if random.random() >= 0.5:
+      self.hits += 32768
+    if random.random() == 0.5:
+      self.hits += 65536
+    if random.random() != 0.5:
+      self.hits += 131072
+    if 0.25 < random.random():
+      self.hits += 262144
+    if 0.25 <= random.random():
+      self.hits += 524288
+    if 0.25 > random.random():
+      self.hits += 1048576
+    if 0.25 >= random.random():
+      self.hits += 2097152
+    if 0.25 == random.random():
+      self.hits += 4194304
+    if 0.25 != random.random():
+      self.hits += 8388608
+    if actions == 1:
+      the_plot.terminate_episode()
+
+
+# The literal each generator's draws of Thresholds.update are compared with, in order.
+THRESHOLDS = (0.5,) * 6 + (0.25,) * 6
+
+
+def make_thresholds(level):
+  del level    # one level
+  return ascii_art.ascii_art_to_game(['....', '.t..'], what_lies_beneath='.',
+                                     drapes={'t': Thresholds})
+
+
 # ---------------------------------------------------------------------- empty --
 # Draws from an empty range on action 1: NumPy's randint, Python's randrange, choice(0).
 
@@ -232,13 +307,13 @@ def make_empty(which):
 
 # The classes a test registers, and the tables of the golden maker and the replays
 # (tests/registered_games.py).
-CLASSES = (Player, NumpyMonster, PythonMonster, Fruit, Edges, EmptyRange)
-GAMES = {'monsters': make_monsters, 'edges': make_edges}
-SPRITES = {'monsters': 'Pab', 'edges': ''}
+CLASSES = (Player, NumpyMonster, PythonMonster, Fruit, Edges, Thresholds, EmptyRange)
+GAMES = {'monsters': make_monsters, 'edges': make_edges, 'thresholds': make_thresholds}
+SPRITES = {'monsters': 'Pab', 'edges': '', 'thresholds': ''}
 REGISTERS = {'monsters': (('P', 'bonuses'), ('f', 'eaten')),
-             'edges': (('x', 'case'), ('x', 'out'))}
-PLOT_KEYS = {'monsters': (), 'edges': ()}
-N_ACTIONS = {'monsters': 6, 'edges': 2}
+             'edges': (('x', 'case'), ('x', 'out')), 'thresholds': (('t', 'hits'),)}
+PLOT_KEYS = {'monsters': (), 'edges': (), 'thresholds': ()}
+N_ACTIONS = {'monsters': 6, 'edges': 2, 'thresholds': 2}
 GENERATORS = ('numpy', 'python')
 RAISES = {}
 FIELDS = ('game', 'level', 'rng_seed', 'actions', 'sprites', 'registers', 'reward_type',
@@ -249,4 +324,5 @@ CASES = (
     ('drawn_monsters_0', 'monsters', 0, 1, 7, 320),
     ('drawn_monsters_1', 'monsters', 1, 2, 8, 320),
     ('drawn_edges_0', 'edges', 0, 3, 9, 320),
+    ('drawn_thresholds_0', 'thresholds', 0, 4, 10, 120),
 )

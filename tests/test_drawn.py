@@ -35,7 +35,8 @@ def test_accepted_draws_compile_through_aliases(games):
   streams = {k.__name__: compiler.registered(k).streams for k in games.CLASSES}
   assert streams == {'Player': ['numpy', 'python'], 'NumpyMonster': ['numpy'],
                      'PythonMonster': ['python'], 'Fruit': ['python', 'numpy'],
-                     'Edges': ['numpy', 'python'], 'EmptyRange': ['numpy', 'python']}
+                     'Edges': ['numpy', 'python'], 'Thresholds': ['numpy', 'python'],
+                     'EmptyRange': ['numpy', 'python']}
   ops = {ins[0] for k in games.CLASSES for ins in compiler.registered(k).ir}
   assert {'RANDINT', 'RANDCMP', 'PICK'} <= ops
   lowered = lowering.lower(games.make_monsters(0))
