@@ -55,8 +55,8 @@ struct StepParams {
   // Program::derive: device copies the program builds from the static level data bound
   // with pcl_bind_state, in formats only that program knows (indexed like the arrays they
   // come from: per level, or one copy when the stride is 0).
-  const uint32_t* derived[2];
-  int64_t derived_bstride[2];    // in words
+  const uint32_t* derived[3];
+  int64_t derived_bstride[3];    // in words
   // Program::derive: per-env words the program keeps from one launch to the next (also in
   // the derived allocation, so every pcl_bind_state starts them afresh), or NULL.
   // scrolly_maze: what the board of each env was last drawn from.

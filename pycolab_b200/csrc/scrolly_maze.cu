@@ -17,10 +17,12 @@
 //   2. group 0 ('#' MazeDrape) is pure register arithmetic and fixes BOTH
 //      final window corners (the '@' drape can only obey an order, never issue
 //      one: by the time it runs, the player's permit is already for frame+1);
-//   3. plain loads, one pattern row per lane: a 5x5 patch of wall bits around each of
-//      the 4 walkers (covers every cell any _check_motion of this step can consult,
-//      wherever the scroll order moves the walker first) and the 3x3 patch of coin bits
-//      around the player;
+//   3. the patch trip, one job and at most two words per lane, every load issued before
+//      any is used: each of the 4 walkers' 5x5 patch of wall bits as one word of the
+//      level's wall-neighbourhood table (covers every cell any _check_motion of this step
+//      can consult, wherever the scroll order moves the walker first), the 3x3 patch of
+//      coin bits around the player, and on the delta path the coin and backdrop rows
+//      around each sprite;
 //   4. once those bits are in, cp.async of the backdrop tile and of the two windows of
 //      the bit-packed patterns (4 words per row, one 16-byte copy from the row-blocked
 //      copies of the bound patterns, see "Row-blocked windows") -> smem, no registers
@@ -122,6 +124,20 @@ __device__ __forceinline__ void cp_async16_l1(void* smem, const void* gmem) {
                "r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
 }
 
+// The patch trip's loads, with an L2 policy that evicts their lines last: a full paint
+// streams ~10 KB per env through L2 (staged tile and windows, the board), which would
+// otherwise push the wall-neighbourhood table out and put a DRAM round trip on the step.
+__device__ __forceinline__ uint64_t l2_evict_last() {
+  uint64_t policy;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(policy));
+  return policy;
+}
+__device__ __forceinline__ uint32_t ld_keep(const uint32_t* p, uint64_t policy) {
+  uint32_t v;
+  asm volatile("ld.global.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(policy) : "memory");
+  return v;
+}
+
 // A 64-cell window row starts at bit corner_c of its pattern row; the four words
 // from the even word at or below corner_c >> 5 always cover it (<= 31 + 32 + 64
 // bits), and pattern rows are 8-byte aligned (pattern_words is even), so a row is
@@ -169,16 +185,17 @@ constexpr uint64_t kKeyRec =
 static_assert(kKeyWords <= kKeyStride, "the render key outgrew its slot");
 
 // Delta rendering's scratch words, in the (then idle) staging area of the warp: the 5x5
-// wall patch rows (one per patch lane), the 3x3 coin rows and backdrop rows around each
-// sprite's start cell, and what the last render drew from the records.
+// wall words of the walkers, the 3x3 coin rows and backdrop rows around each sprite's
+// start cell, and what the last render drew from the records.
 enum {
-  kNbWall = 0,                     // 20 words: rowbits of patch lanes 0..19
+  kNbWall = 0,                     // 4 words: walker s's 5x5 wall word at s
   kNbCoin = 32,                    // 12 words: 3 coin bits per row, sprite s row k at 3 s + k
-  kNbBackdrop = 44,                // 12 words: 3 backdrop bytes per row, likewise
+  kNbBackdrop = 44,                // 12 words: 3 backdrop bytes per row, likewise (kNbCoin + 12)
   kNbStart = 56,                   // 4 words per sprite: vrow, vcol, and row, col (-1: hidden)
   kNbStale = kNbStart + 4 * kS,    // 2 words: the stale coin cell (AUX0, AUX1)
   kNbWords = (kNbStale + 2 + 3) & ~3   // whole 16-byte units: warp regions stay 16-byte aligned
 };
+static_assert(kNbBackdrop == kNbCoin + 12, "the patch trip stores coin and backdrop rows as one run");
 
 __host__ __device__ constexpr size_t staging_bytes(int H, int W, int pitch) {
   // backdrop tile, two window rows of window_words(W) per board row, and one word per
@@ -526,71 +543,68 @@ scrolly_maze_step(const StepParams p) {
   const bool c_touch = rec_coins[PCL_D_LAST_FRAME] < plot.frame;
   const int c_pre_r = rec_coins[c_touch ? PCL_D_CORNER_R : PCL_D_PRE_R];
   const int c_pre_c = rec_coins[c_touch ? PCL_D_CORNER_C : PCL_D_PRE_C];
-  // Look-up bits, one pattern ROW per lane: lanes 0..19 = row k of the 5x5 wall
-  // patch of walker w (lane = 5 w + k; covers every cell any _check_motion of this
-  // step can consult, wherever the scroll order moves the walker first), lanes
-  // 20..22 = the 3 rows of the coin patch around the player, lane 23 = the coin
-  // bit at the pre-scroll corner (an off-board player sits at (0, 0)).
-  unsigned rowbits = 0;
-  {
-    const uint32_t* row = nullptr;
-    int c_first = 0, limit = 0;              // first pattern column, words in the row
-    if (lane < 20) {
-      const int w = lane / 5, k = lane - w * 5;
-      const int pr = wr + rec[w * PCL_SPRITE_WORDS + PCL_S_VROW] + k - 2;
-      c_first = wc + rec[w * PCL_SPRITE_WORDS + PCL_S_VCOL] - 2;
-      if ((unsigned)pr < (unsigned)p.PH) { row = level_walls(p, lvl) + (int64_t)pr * PWW; limit = PWW; }
-    } else if (lane < 24) {
-      // A clean group's row comes from the level's template (see "Coin groups").
-      const int r = lane < 23 ? p_vrow + (lane - 20) - 1 : 0;
-      c_first = lane < 23 ? c_pre_c + p_vcol - 1 : c_pre_c;
-      if ((unsigned)r < (unsigned)H) {
-        const int pr = c_pre_r + r;
-        row = ((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> coin_group_shift(p.PH))) & 1u
-                  ? env_coins(p, env) : level_coins(p, lvl);
-        row += (int64_t)pr * PWW; limit = PWW;
-      }
-    }
-    if (row != nullptr) {
-      const int wi = c_first >> 5;           // floor, may be -1
-      const uint32_t lo = (unsigned)wi < (unsigned)limit ? row[wi] : 0u;
-      const uint32_t hi = (unsigned)(wi + 1) < (unsigned)limit ? row[wi + 1] : 0u;
-      rowbits = __funnelshift_r(lo, hi, c_first & 31) & 31u;
-    }
-  }
-  // Delta rendering: neither window moves and the board is this env's last render.  In
-  // the same trip, the 3x3 coin bits (lanes 0..11) and backdrop bytes (lanes 12..23)
-  // around each sprite's start cell, row k of sprite s at lane 3 s + k (+ 12).
+  // Delta rendering: neither window moves and the board is this env's last render.
   bool delta = key_ok && !restart && wr == rec[32 + PCL_D_CORNER_R] &&
                wc == rec[32 + PCL_D_CORNER_C] && cr_pred == rec_coins[PCL_D_CORNER_R] &&
                cc_pred == rec_coins[PCL_D_CORNER_C] && rec_coins[PCL_D_AUX2] != -1;
-  unsigned nb = 0;
-  if (delta && lane < 24) {
-    const int s = (lane < 12 ? lane : lane - 12) / 3;
+  // The patch trip: one job and at most two words per lane.  Every lane computes its
+  // address, predicates, shift and mask with selects, issues both loads, and only then
+  // combines them, so the step waits on one round trip here, not one per kind of job.
+  //   lanes 0..3    walker `lane`'s 5x5 wall word (see "Wall neighbourhoods"): covers
+  //                 every cell any _check_motion of this step can consult, wherever the
+  //                 scroll order moves the walker first;
+  //   lanes 4..6    row lane - 4 of the 3x3 coin patch around the player at the pre-scroll
+  //                 corner, lane 7 the coin bit at that corner (an off-board player sits
+  //                 at (0, 0));
+  //   lanes 8..19   delta only: 3 coin bits of row k around sprite s's start cell
+  //                 (lane 8 + 3 s + k);
+  //   lanes 20..31  delta only: 3 backdrop bytes of row k around sprite s's start cell
+  //                 (lane 20 + 3 s + k), from the two aligned words that hold them.
+  // A clean group's coin row comes from the level's template (see "Coin groups").
+  uint32_t got;
+  {
+    const bool wall_lane = lane < 4, coin_lane = lane < 20, pc_lane = lane < 8;
+    const int j = coin_lane ? lane - 8 : lane - 20;          // delta jobs: 3 s + k
+    const int s = wall_lane ? lane : pc_lane ? 0 : j / 3;
     const int vr = rec[s * PCL_SPRITE_WORDS + PCL_S_VROW], vc = rec[s * PCL_SPRITE_WORDS + PCL_S_VCOL];
-    const int r = vr + (lane < 12 ? lane : lane - 12) - 3 * s - 1;
-    if ((unsigned)r < (unsigned)H) {
-      if (lane < 12) {
-        const int pr = cr_pred + r, c_first = cc_pred + vc - 1, wi = c_first >> 5;
-        const uint32_t* row = ((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> coin_group_shift(p.PH))) & 1u
-                                  ? env_coins(p, env) : level_coins(p, lvl);
-        row += (int64_t)pr * PWW;
-        const uint32_t lo = (unsigned)wi < (unsigned)PWW ? row[wi] : 0u;
-        const uint32_t hi = (unsigned)(wi + 1) < (unsigned)PWW ? row[wi + 1] : 0u;
-        nb = __funnelshift_r(lo, hi, c_first & 31) & 7u;
-      } else {
-        const uint8_t* bd = p.st.d_backdrop + lvl * p.st.backdrop_bstride + (int64_t)r * pitch;
+    // board row of a coin or backdrop job, and the first column it reads
+    const int r = pc_lane ? (lane < 7 ? p_vrow + lane - 5 : 0) : vr + j - 3 * (j / 3) - 1;
+    const int c = pc_lane ? (lane < 7 ? c_pre_c + p_vcol - 1 : c_pre_c)
+                          : coin_lane ? cc_pred + vc - 1 : vc - 1;
+    const bool row_ok = (unsigned)r < (unsigned)H && (pc_lane || delta);
+    // coin jobs
+    const int pr = (pc_lane ? c_pre_r : cr_pred) + r;
+    const uint32_t* coin_row =
+        (((unsigned)rec_coins[PCL_D_AUX2] >> (pr >> coin_group_shift(p.PH))) & 1u
+             ? env_coins(p, env) : level_coins(p, lvl)) + (int64_t)pr * PWW;
+    // wall jobs: the centre (pattern row, column) of the walker's patch
+    const int wr_c = wr + vr + 2, wc_c = wc + vc + 2;       // + the table's 2-cell margin
+    const int tw = p.PW + 4;
+    const uint32_t* base =
+        wall_lane ? p.derived[2] + lvl * p.derived_bstride[2] + (int64_t)wr_c * tw + wc_c
+        : coin_lane ? coin_row
+                    : reinterpret_cast<const uint32_t*>(p.st.d_backdrop + lvl * p.st.backdrop_bstride +
+                                                        (int64_t)r * pitch);
+    const int words = coin_lane ? PWW : pitch >> 2;          // words in a coin or backdrop row
+    const int wi = wall_lane ? 0 : coin_lane ? c >> 5 : c >> 2;   // floor, may be -1
+    const bool ok0 = wall_lane ? (unsigned)wr_c < (unsigned)(p.PH + 4) && (unsigned)wc_c < (unsigned)tw
+                               : row_ok && (unsigned)wi < (unsigned)words;
+    const bool ok1 = !wall_lane && row_ok && (unsigned)(wi + 1) < (unsigned)words;
+    const int sh = wall_lane ? 0 : coin_lane ? c & 31 : (c & 3) * 8;
+    // coin bits are not masked to the board here (coin9 is, below; delta candidates off
+    // the board fall back); backdrop bytes off the board read 0
+    uint32_t mask = wall_lane ? ~0u : lane == 7 ? 1u : 7u;
+    if (!coin_lane) {
+      mask = 0;
 #pragma unroll
-        for (int j = 0; j < 3; ++j)
-          if ((unsigned)(vc - 1 + j) < (unsigned)W) nb |= (unsigned)__ldg(bd + vc - 1 + j) << (8 * j);
-      }
+      for (int i = 0; i < 3; ++i) mask |= ((unsigned)(c + i) < (unsigned)W ? 0xffu : 0u) << (8 * i);
     }
+    const uint64_t keep = l2_evict_last();
+    const uint32_t lo = ok0 ? ld_keep(base + wi, keep) : 0u;
+    const uint32_t hi = ok1 ? ld_keep(base + wi + 1, keep) : 0u;
+    got = __funnelshift_r(lo, hi, sh) & mask;
   }
-  // Pattern columns past PW are zero padding and negative ones read as zero, so
-  // the wall bits need no further masking; coin bits are masked to the board.
-  unsigned field = 0;                        // my walker's 5x5 patch, bit (dr+2)*5 + dc+2
-#pragma unroll
-  for (int k = 0; k < 5; ++k) field |= __shfl_sync(PCL_FULL, rowbits, me * 5 + k) << (5 * k);
+  const unsigned field = __shfl_sync(PCL_FULL, got, me);   // my walker's 5x5, bit (dr+2)*5 + dc+2
   unsigned coin9 = 0;                        // 3x3 around the player's start + the (0,0) cell
   {
     unsigned colmask = 0;
@@ -598,8 +612,8 @@ scrolly_maze_step(const StepParams p) {
     for (int i = 0; i < 3; ++i)
       colmask |= ((unsigned)(p_vcol - 1 + i) < (unsigned)W ? 1u : 0u) << i;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) coin9 |= (__shfl_sync(PCL_FULL, rowbits, 20 + k) & colmask) << (3 * k);
-    coin9 |= (__shfl_sync(PCL_FULL, rowbits, 23) & 1u) << 9;
+    for (int k = 0; k < 3; ++k) coin9 |= (__shfl_sync(PCL_FULL, got, 4 + k) & colmask) << (3 * k);
+    coin9 |= __shfl_sync(PCL_FULL, got, 7) << 9;
   }
   PCL_STAMP(kStPatch);
   uint32_t* s_nb = reinterpret_cast<uint32_t*>(s_bd);   // delta rendering's scratch
@@ -659,8 +673,8 @@ scrolly_maze_step(const StepParams p) {
     }
   };
   if (delta) {
-    if (lane < 20) s_nb[kNbWall + lane] = rowbits;
-    if (lane < 24) s_nb[kNbCoin + lane] = nb;
+    if (lane < 4) s_nb[kNbWall + lane] = got;
+    if (lane >= 8) s_nb[kNbCoin + lane - 8] = got;   // coin rows, then backdrop rows
     if (lane < 4) {
       uint32_t* q = s_nb + kNbStart + 4 * lane;
       q[0] = mine.vrow; q[1] = mine.vcol;
@@ -851,7 +865,7 @@ scrolly_maze_step(const StepParams p) {
         outside = s < 0 || !on_board(r, c, H, W);
         if (!outside) {
           // z-order a b c @ # P, as the full paint composes it
-          const bool wall = (s_nb[kNbWall + 5 * s + dr + 1] >> (dc + 1)) & 1u;
+          const bool wall = (s_nb[kNbWall + s] >> ((dr + 1) * 5 + dc + 1)) & 1u;
           bool coin = (s_nb[kNbCoin + 3 * s + dr] >> dc) & 1u;
           if (picked_r - cr == r && picked_c - cc == c) coin = false;
           if (rec_coins[PCL_D_AUX0] == r && rec_coins[PCL_D_AUX1] == c) coin = true;
@@ -1084,6 +1098,38 @@ __global__ void build_blocked(const uint32_t* src, int64_t src_bstride, uint32_t
   }
 }
 
+// ---- Wall neighbourhoods (built by derive() beside the row-blocked windows) ----------
+// One word per pattern cell (pr, pc), with a 2-cell margin: word (pr + 2) * (PW + 4) +
+// pc + 2 of a copy has bit (dr + 2) * 5 + dc + 2 set iff the wall pattern has a wall at
+// (pr + dr, pc + dc), where rows outside [0, PH), negative columns and columns past the
+// row's PWW words read 0 (columns in [PW, 32 PWW) read the row's zero padding).  So a
+// walker's whole 5x5 patch is one load.  A centre outside the margin reads 0 in all 25
+// cells: the kernel loads nothing for it.  (PH + 4) * (PW + 4) words per copy, one per
+// level (one per env without a level index), or a single one when the pattern has no
+// stride: derived[2].
+__global__ void build_neighbourhoods(const uint32_t* src, int64_t src_bstride, uint32_t* dst, int PH,
+                                     int PW, int PWW, int64_t total) {
+  const int tw = PW + 4;
+  const int64_t per_copy = (int64_t)(PH + 4) * tw;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t t = i / per_copy;
+    const int cell = (int)(i - t * per_copy);
+    const int pr = cell / tw - 2, c_first = cell % tw - 4;   // first column of each patch row
+    const int wi = c_first >> 5;                             // floor, may be -1
+    uint32_t word = 0;
+    for (int k = 0; k < 5; ++k) {
+      const int r = pr + k - 2;
+      if ((unsigned)r >= (unsigned)PH) continue;
+      const uint32_t* row = src + t * src_bstride + (int64_t)r * PWW;
+      const uint32_t lo = (unsigned)wi < (unsigned)PWW ? row[wi] : 0u;
+      const uint32_t hi = (unsigned)(wi + 1) < (unsigned)PWW ? row[wi + 1] : 0u;
+      word |= (__funnelshift_r(lo, hi, c_first & 31) & 31u) << (5 * k);
+    }
+    dst[i] = word;
+  }
+}
+
 int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, void** owned) {
   // Copies of per-level data: as many as the level index can name (one per env without
   // one), or a single one when the array has no stride.
@@ -1102,13 +1148,16 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
   const int64_t blk_words = (int64_t)nblk * PH * nw;              // one blocked copy
   const int64_t n_wall = st.pattern_bstride[0] == 0 ? 1 : levels;
   const int64_t n_coin = st.pattern_init_bstride[1] == 0 ? 1 : levels;
+  const int64_t nbh_words = (int64_t)(PH + 4) * (s.pattern_cols + 4);   // one neighbourhood copy
   const int64_t off_coin = (n_wall * blk_words * 4 + 255) & ~(int64_t)255;
-  const int64_t off_key = (off_coin + n_coin * blk_words * 4 + 255) & ~(int64_t)255;
+  const int64_t off_nbh = (off_coin + n_coin * blk_words * 4 + 255) & ~(int64_t)255;
+  const int64_t off_key = (off_nbh + n_wall * nbh_words * 4 + 255) & ~(int64_t)255;
   uint8_t* buf = nullptr;
   if (cudaMalloc(&buf, off_key + (int64_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_NOMEM;
   *owned = buf;
   uint32_t* wall = reinterpret_cast<uint32_t*>(buf);
   uint32_t* coin = reinterpret_cast<uint32_t*>(buf + off_coin);
+  uint32_t* nbh = reinterpret_cast<uint32_t*>(buf + off_nbh);
   // Render keys of no render (frame -1): the first launch paints every board.
   p->render_key = reinterpret_cast<int32_t*>(buf + off_key);
   if (cudaMemset(p->render_key, 0xff, (size_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_CUDA;
@@ -1116,8 +1165,11 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
                                nw, nblk, n_wall * blk_words);
   build_blocked<<<1024, 256>>>(st.d_pattern_init[1], st.pattern_init_bstride[1], coin, PH,
                                s.pattern_words, nw, nblk, n_coin * blk_words);
+  build_neighbourhoods<<<1024, 256>>>(st.d_pattern[0], st.pattern_bstride[0], nbh, PH,
+                                      s.pattern_cols, s.pattern_words, n_wall * nbh_words);
   p->derived[0] = wall; p->derived_bstride[0] = n_wall > 1 ? blk_words : 0;
   p->derived[1] = coin; p->derived_bstride[1] = n_coin > 1 ? blk_words : 0;
+  p->derived[2] = nbh; p->derived_bstride[2] = n_wall > 1 ? nbh_words : 0;
   return cudaDeviceSynchronize() == cudaSuccess && cudaGetLastError() == cudaSuccess ? PCL_OK
                                                                                      : PCL_ERR_CUDA;
 }
@@ -1130,6 +1182,17 @@ const Program kScrollyMaze = {check_spec, check_state, curtain, launch, nullptr,
                               /*float_reward_arg0=*/false, derive};
 
 }  // namespace pcl
+
+// The wall-neighbourhood table derive() builds (see "Wall neighbourhoods"), for `copies`
+// wall patterns of rows x words words, `bstride` words apart, into d_dst ((rows + 4) x
+// (cols + 4) words per copy), so that tests can hold the table against its rule.  Not
+// part of include/pcl.h.  0, or -3 on a CUDA error.
+extern "C" int pcl_scrolly_wall_neighbourhoods(const uint32_t* d_pattern, int64_t bstride, int rows,
+                                               int cols, int words, int64_t copies, uint32_t* d_dst) {
+  pcl::build_neighbourhoods<<<1024, 256>>>(d_pattern, bstride, d_dst, rows, cols, words,
+                                           copies * (rows + 4) * (cols + 4));
+  return cudaDeviceSynchronize() == cudaSuccess && cudaGetLastError() == cudaSuccess ? 0 : -3;
+}
 
 #ifdef PCL_STEP_STAMPS
 // Copies the stamps of the last scrolly_maze_step launch for envs [0, n) to host memory
