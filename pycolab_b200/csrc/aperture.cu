@@ -66,16 +66,9 @@ aperture_step(const StepParams p) {
   cp_async_wait_all();
   __syncwarp();
 
-  Sprite sp;
-  sp.row = rec[PCL_S_ROW]; sp.col = rec[PCL_S_COL];
-  sp.vrow = rec[PCL_S_VROW]; sp.vcol = rec[PCL_S_VCOL];
-  sp.flags = rec[PCL_S_FLAGS]; sp.aux0 = sp.aux1 = sp.aux2 = 0;
+  Sprite sp = load_sprite(rec);
   int ap0 = rec[8 + PCL_D_AUX0], ap1 = rec[8 + PCL_D_AUX1];    // _apertures[0], [1]
-  Plot plot;
-  plot.frame = rec[16 + PCL_P_FRAME] + 1;                      // engine.py:716
-  plot.error = rec[16 + PCL_P_ERROR];
-  plot.aux0 = 0;
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
+  Plot plot = step_plot(rec + 16, rec[16 + PCL_P_ERROR]);
   Directives dir = fresh_directives();
 
   // ---- group 0: PlayerSprite.update on the stale board -------------------
@@ -143,11 +136,9 @@ aperture_step(const StepParams p) {
   // ---- _apply_and_clear_plot (engine.py:761-847) + records back
   __syncwarp();                 // every lane has read the staged records (racecheck: WAR)
   if (lane == 0) {
-    rec[PCL_S_ROW] = sp.row; rec[PCL_S_COL] = sp.col;
-    rec[PCL_S_VROW] = sp.vrow; rec[PCL_S_VCOL] = sp.vcol; rec[PCL_S_FLAGS] = sp.flags;
+    store_sprite(rec, sp, PCL_S_AUX0);
     rec[8 + PCL_D_AUX0] = ap0; rec[8 + PCL_D_AUX1] = ap1;
-    rec[16 + PCL_P_FRAME] = plot.frame; rec[16 + PCL_P_GAME_OVER] = dir.game_over;
-    rec[16 + PCL_P_ERROR] = plot.error;
+    store_plot<ORDER_KEEP>(rec + 16, plot, dir);
     store_outputs(p.out, env, dir);
     // final render, z-order X then A: patch the staged tile (engine.py:737-759)
     if (ap0 >= 0) s_bd[(ap0 >> 16) * pitch + (ap0 & 0xffff)] = p.drape_char[0];

@@ -46,21 +46,11 @@ apprehend_step(const StepParams p) {
   const bool restart = run == ENV_RESTART;
   const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprites;
   const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
-  Sprite pl, ball;
-  {
-    const int32_t* r = src_s;
-    pl.row = r[PCL_S_ROW]; pl.col = r[PCL_S_COL]; pl.vrow = r[PCL_S_VROW]; pl.vcol = r[PCL_S_VCOL];
-    pl.flags = r[PCL_S_FLAGS]; pl.aux0 = pl.aux1 = pl.aux2 = 0;
-    r += PCL_SPRITE_WORDS;
-    ball.row = r[PCL_S_ROW]; ball.col = r[PCL_S_COL]; ball.vrow = r[PCL_S_VROW];
-    ball.vcol = r[PCL_S_VCOL]; ball.flags = r[PCL_S_FLAGS];
-    ball.aux0 = r[PCL_S_AUX0]; ball.aux1 = r[PCL_S_AUX1]; ball.aux2 = 0;
-  }
-  Plot plot;
-  plot.frame = src_p[PCL_P_FRAME] + 1;                                // engine.py:716
+  Sprite pl = load_sprite(src_s), ball = load_sprite(src_s + PCL_SPRITE_WORDS);
+  pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
+  ball.aux2 = 0;
   const PlotCarry carry = plot_carry(g_plot, restart);
-  plot.error = carry.error;
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
+  Plot plot = step_plot(src_p, carry.error);
   double dx = f64_of(ball.aux0, ball.aux1);
   double acc = f64_of(src_p[PCL_P_AUX0], src_p[PCL_P_AUX1]);
   if (restart && p.st.d_rng != nullptr) {                             // BallSprite.__init__ :103
@@ -92,16 +82,11 @@ apprehend_step(const StepParams p) {
 
   __syncwarp();
   if (lane == 0) {
-    int32_t* r = g_sprites;
-    r[PCL_S_ROW] = pl.row; r[PCL_S_COL] = pl.col; r[PCL_S_VROW] = pl.vrow; r[PCL_S_VCOL] = pl.vcol;
-    r[PCL_S_FLAGS] = pl.flags; r[PCL_S_AUX0] = 0; r[PCL_S_AUX1] = 0; r[PCL_S_AUX2] = 0;
-    r += PCL_SPRITE_WORDS;
-    r[PCL_S_ROW] = ball.row; r[PCL_S_COL] = ball.col; r[PCL_S_VROW] = ball.vrow;
-    r[PCL_S_VCOL] = ball.vcol; r[PCL_S_FLAGS] = ball.flags;
-    r[PCL_S_AUX0] = __double2loint(dx); r[PCL_S_AUX1] = __double2hiint(dx); r[PCL_S_AUX2] = 0;
-    g_plot[PCL_P_FRAME] = plot.frame; g_plot[PCL_P_GAME_OVER] = dir.game_over;
-    g_plot[PCL_P_EPISODES] = carry.episodes; g_plot[PCL_P_ERROR] = plot.error;
-    g_plot[PCL_P_ORDER_FRAME] = PCL_NEVER;
+    ball.aux0 = __double2loint(dx); ball.aux1 = __double2hiint(dx);
+    store_sprite(g_sprites, pl);
+    store_sprite(g_sprites + PCL_SPRITE_WORDS, ball);
+    store_carry(g_plot, carry);
+    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
     g_plot[PCL_P_AUX0] = __double2loint(acc); g_plot[PCL_P_AUX1] = __double2hiint(acc);
     store_outputs(p.out, env, dir);
   }

@@ -86,17 +86,9 @@ better_scrolly_step(const StepParams p) {
 
   Sprite sp[kS];
 #pragma unroll
-  for (int i = 0; i < kS; ++i) {
-    const int32_t* r = rec + i * PCL_SPRITE_WORDS;
-    sp[i].row = r[PCL_S_ROW]; sp[i].col = r[PCL_S_COL];
-    sp[i].vrow = r[PCL_S_VROW]; sp[i].vcol = r[PCL_S_VCOL];
-    sp[i].flags = r[PCL_S_FLAGS]; sp[i].aux0 = r[PCL_S_AUX0]; sp[i].aux1 = sp[i].aux2 = 0;
-  }
-  Plot plot;
-  plot.frame = rec[48 + PCL_P_FRAME] + 1;                  // engine.py:716
-  plot.error = rec[48 + PCL_P_ERROR];
+  for (int i = 0; i < kS; ++i) sp[i] = load_sprite(rec + i * PCL_SPRITE_WORDS);
+  Plot plot = step_plot(rec + 48, rec[48 + PCL_P_ERROR]);
   plot.aux0 = rec[48 + PCL_P_AUX0];
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
   Directives dir = fresh_directives();
 
   // Snapshot of the previous render's sprites (z-order a b c @ P).
@@ -163,14 +155,9 @@ better_scrolly_step(const StepParams p) {
   __syncwarp();
   if (lane == 0) {
 #pragma unroll
-    for (int i = 0; i < kS; ++i) {
-      int32_t* r = rec + i * PCL_SPRITE_WORDS;
-      r[PCL_S_ROW] = sp[i].row; r[PCL_S_COL] = sp[i].col;
-      r[PCL_S_VROW] = sp[i].vrow; r[PCL_S_VCOL] = sp[i].vcol;
-      r[PCL_S_FLAGS] = sp[i].flags; r[PCL_S_AUX0] = sp[i].aux0;
-    }
-    rec[48 + PCL_P_FRAME] = plot.frame; rec[48 + PCL_P_GAME_OVER] = dir.game_over;
-    rec[48 + PCL_P_ERROR] = plot.error; rec[48 + PCL_P_AUX0] = plot.aux0;
+    for (int i = 0; i < kS; ++i) store_sprite(rec + i * PCL_SPRITE_WORDS, sp[i], PCL_S_AUX1);
+    store_plot<ORDER_KEEP>(rec + 48, plot, dir);
+    rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
   }
   __syncwarp();

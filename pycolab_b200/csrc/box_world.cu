@@ -60,13 +60,11 @@ box_world_step(const StepParams p) {
       reinterpret_cast<uint4*>(grid + lane * pitch)[q] =
           reinterpret_cast<const uint4*>(src_g + lane * pitch)[q];
 
-  Sprite pl;
-  pl.row = src_s[PCL_S_ROW]; pl.col = src_s[PCL_S_COL];
-  pl.vrow = src_s[PCL_S_VROW]; pl.vcol = src_s[PCL_S_VCOL];
-  pl.flags = src_s[PCL_S_FLAGS];
-  int steps = src_s[PCL_S_AUX0];                   // PlayerSprite._step_counter
-  const int frame = src_p[PCL_P_FRAME] + 1;        // engine.py:716
-  PlotCarry carry = plot_carry(g_plot, restart);
+  Sprite pl = load_sprite(src_s);
+  pl.aux1 = pl.aux2 = 0;                           // stored as zeros
+  int steps = pl.aux0;                             // PlayerSprite._step_counter
+  const PlotCarry carry = plot_carry(g_plot, restart);
+  Plot plot = step_plot(src_p, carry.error);
   int over_ch = src_p[PCL_P_AUX0];                 // the_plot['over_this']: 0 = unset
   int over_at = src_p[PCL_P_AUX1];
   const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
@@ -109,7 +107,7 @@ box_world_step(const StepParams p) {
       if (move && on) { pl.row = pl.vrow = tr; pl.col = pl.vcol = tc; }
       if (thing && !raised) { over_ch = thing; over_at = (pl.row << 16) | pl.col; }
     }
-    if (raised) carry.error |= PCL_ENV_ERR_INDEX;
+    if (raised) plot.error |= PCL_ENV_ERR_INDEX;
     else if (++steps > p.program_arg[0]) terminate(dir);
   }
 
@@ -141,12 +139,10 @@ box_world_step(const StepParams p) {
 
   // ---- records, outputs and the grid rows that changed
   if (lane == 0) {
-    g_sprite[PCL_S_ROW] = pl.row; g_sprite[PCL_S_COL] = pl.col;
-    g_sprite[PCL_S_VROW] = pl.vrow; g_sprite[PCL_S_VCOL] = pl.vcol;
-    g_sprite[PCL_S_FLAGS] = pl.flags; g_sprite[PCL_S_AUX0] = steps;
-    g_sprite[PCL_S_AUX1] = 0; g_sprite[PCL_S_AUX2] = 0;
-    g_plot[PCL_P_FRAME] = frame; g_plot[PCL_P_GAME_OVER] = dir.game_over;
+    pl.aux0 = steps;
+    store_sprite(g_sprite, pl);
     store_carry(g_plot, carry);
+    store_plot<ORDER_KEEP>(g_plot, plot, dir);
     g_plot[PCL_P_AUX0] = over_ch; g_plot[PCL_P_AUX1] = over_at;
     store_outputs(p.out, env, dir);
   }

@@ -73,15 +73,9 @@ classics_step(const StepParams p) {
   cp_async_wait_all();
   __syncwarp();
 
-  Sprite sp;
-  sp.row = rec[PCL_S_ROW]; sp.col = rec[PCL_S_COL];
-  sp.vrow = rec[PCL_S_VROW]; sp.vcol = rec[PCL_S_VCOL];
-  sp.flags = rec[PCL_S_FLAGS]; sp.aux0 = sp.aux1 = sp.aux2 = 0;
-  Plot plot;
-  plot.frame = rec[16 + PCL_P_FRAME] + 1;                    // engine.py:716
-  plot.error = rec[16 + PCL_P_ERROR];
+  Sprite sp = load_sprite(rec);
+  Plot plot = step_plot(rec + 16, rec[16 + PCL_P_ERROR]);
   plot.aux0 = rec[16 + PCL_P_AUX0];                          // river rotation count
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
   Directives dir = fresh_directives();
 
   const int rule = p.program_arg[0];
@@ -131,10 +125,9 @@ classics_step(const StepParams p) {
   // ---- _apply_and_clear_plot (engine.py:761-847) + records back
   __syncwarp();                 // every lane has read the staged records (racecheck: WAR)
   if (lane == 0) {
-    rec[PCL_S_ROW] = sp.row; rec[PCL_S_COL] = sp.col;
-    rec[PCL_S_VROW] = sp.vrow; rec[PCL_S_VCOL] = sp.vcol; rec[PCL_S_FLAGS] = sp.flags;
-    rec[16 + PCL_P_FRAME] = plot.frame; rec[16 + PCL_P_GAME_OVER] = dir.game_over;
-    rec[16 + PCL_P_ERROR] = plot.error; rec[16 + PCL_P_AUX0] = plot.aux0;
+    store_sprite(rec, sp, PCL_S_AUX0);
+    store_plot<ORDER_KEEP>(rec + 16, plot, dir);
+    rec[16 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
   }
   __syncwarp();

@@ -451,22 +451,22 @@ __device__ void run_update(const Ctx& c, Vm* vm, int ent, int action, Plot& plot
         break;
       }
       case PCL_OP_MOVE: {
-        Sprite s = board::load_sprite(st->sprites[ent]);
+        Sprite s = load_sprite(st->sprites[ent]);
         const uint32_t* imp = st->impassable[ent];
         const uint8_t* bd = c.board;
         const int pitch = p.pitch;
         const bool moved = walker_move(s, ent, a, plot, H, W, p.confined[ent] != 0,
                                        kScroll && p.egocentric[ent] != 0, lane,
                                        [&](int r, int col) { return in_set(imp, bd[r * pitch + col]); });
-        board::store_sprite(st->sprites[ent], s, lane);
+        board::warp_store_sprite(st->sprites[ent], s, lane);
         stk[sp++] = moved ? 0 : 1;
         break;
       }
       case PCL_OP_TELEPORT: {
         sp -= 2;
-        Sprite s = board::load_sprite(st->sprites[ent]);
+        Sprite s = load_sprite(st->sprites[ent]);
         walker_teleport(s, H, W, stk[sp], stk[sp + 1]);
-        board::store_sprite(st->sprites[ent], s, lane);
+        board::warp_store_sprite(st->sprites[ent], s, lane);
         break;
       }
       case PCL_OP_REWARD: case PCL_OP_REWARD_F64: {
@@ -654,11 +654,7 @@ __device__ __forceinline__ void step(const StepParams& p) {
   __syncwarp();
   board::stage_board</*kWrap=*/true>(c, restart, g_board);
 
-  Plot plot;
-  plot.frame = st->plot[PCL_P_FRAME] + 1;    // engine.py:716
-  plot.error = st->plot[PCL_P_ERROR];
-  plot.order_r = st->plot[PCL_P_ORDER_R]; plot.order_c = st->plot[PCL_P_ORDER_C];
-  plot.order_frame = st->plot[PCL_P_ORDER_FRAME]; plot.ego_mask = st->plot[PCL_P_EGO_MASK];
+  Plot plot = step_plot</*kOrder=*/true>(st->plot, carry.error);
   Directives dir = fresh_directives();
   Rewards rw = {0, 0, 0.0};
   const int action = restart ? PCL_ACTION_NONE : p.actions[(int64_t)env * p.actions_per_env];
@@ -700,15 +696,10 @@ __device__ __forceinline__ void step(const StepParams& p) {
 
   __syncwarp();
   if (lane == 0) {
-    st->plot[PCL_P_FRAME] = plot.frame; st->plot[PCL_P_GAME_OVER] = dir.game_over;
-    st->plot[PCL_P_ERROR] = plot.error;
-    st->plot[PCL_P_ORDER_R] = plot.order_r; st->plot[PCL_P_ORDER_C] = plot.order_c;
-    st->plot[PCL_P_ORDER_FRAME] = plot.order_frame; st->plot[PCL_P_EGO_MASK] = plot.ego_mask;
-    if (p.program_arg[0]) p.out.d_reward_f64[env] = rw.has ? rw.sum_f : 0.0;
-    else p.out.d_reward[env] = rw.has ? rw.sum_i : 0;
-    p.out.d_has_reward[env] = (uint8_t)rw.has;
-    p.out.d_discount[env] = dir.discount;
-    p.out.d_done[env] = (uint8_t)dir.game_over;
+    store_plot<ORDER_ALL>(st->plot, plot, dir);
+    dir.reward = rw.has ? rw.sum_i : 0; dir.has_reward = rw.has;   // the code's own sums
+    if (p.program_arg[0]) store_outputs(p.out, env, dir, rw.has ? rw.sum_f : 0.0);
+    else store_outputs(p.out, env, dir);
   }
   __syncwarp();
   board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);

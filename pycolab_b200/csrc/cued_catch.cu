@@ -129,18 +129,17 @@ cued_catch_step(const StepParams p) {
   Sprite sp[3];
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
-    const int32_t* r = src_s + i * PCL_SPRITE_WORDS;
-    sp[i].row = r[PCL_S_ROW]; sp[i].col = r[PCL_S_COL];
-    sp[i].vrow = r[PCL_S_VROW]; sp[i].vcol = r[PCL_S_VCOL];
-    sp[i].flags = r[PCL_S_FLAGS]; sp[i].aux0 = r[PCL_S_AUX0]; sp[i].aux1 = sp[i].aux2 = 0;
+    sp[i] = load_sprite(src_s + i * PCL_SPRITE_WORDS);
+    sp[i].aux1 = sp[i].aux2 = 0;                                       // stored as zeros
   }
   // CueDrape (:229-245): phase, ticks, trial choice, last reset, trials left, pairings
   int phase = src_q[PCL_D_CORNER_R], tick1 = src_q[PCL_D_CORNER_C];
   int choice = src_q[PCL_D_PRE_R], tick2 = src_q[PCL_D_PRE_C];
   int last_reset = src_q[PCL_D_LAST_FRAME], trials = src_q[PCL_D_AUX0];
   int pairs = src_q[PCL_D_AUX1];
-  const int f = src_p[PCL_P_FRAME] + 1;                                // engine.py:716
   const PlotCarry carry = plot_carry(g_plot, restart);
+  const Plot plot = step_plot(src_p, carry.error);
+  const int f = plot.frame;
   int programmed = src_p[PCL_P_AUX0], which = src_p[PCL_P_AUX1], ball_reset = src_p[PCL_P_AUX2];
   int ttr = sp[SP].aux0;                           // PlayerSprite._trials_till_reward
 
@@ -294,26 +293,17 @@ cued_catch_step(const StepParams p) {
   if (lane == 0) {
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
-      int32_t* r = g_sprites + i * PCL_SPRITE_WORDS;
-      r[PCL_S_ROW] = sp[i].row; r[PCL_S_COL] = sp[i].col;
-      r[PCL_S_VROW] = sp[i].vrow; r[PCL_S_VCOL] = sp[i].vcol;
-      r[PCL_S_FLAGS] = sp[i].flags; r[PCL_S_AUX0] = i == SP ? ttr : 0;
-      r[PCL_S_AUX1] = 0; r[PCL_S_AUX2] = 0;
+      sp[i].aux0 = i == SP ? ttr : 0;
+      store_sprite(g_sprites + i * PCL_SPRITE_WORDS, sp[i]);
     }
-    g_q[PCL_D_CORNER_R] = phase; g_q[PCL_D_CORNER_C] = tick1;
-    g_q[PCL_D_PRE_R] = choice; g_q[PCL_D_PRE_C] = tick2;
-    g_q[PCL_D_LAST_FRAME] = last_reset; g_q[PCL_D_AUX0] = trials;
-    g_q[PCL_D_AUX1] = pairs; g_q[PCL_D_AUX2] = 0;
-    g_plot[PCL_P_FRAME] = f; g_plot[PCL_P_GAME_OVER] = dir.game_over;
+    store_drape(g_q, {phase, tick1, choice, tick2, last_reset, trials, pairs, 0});
     store_carry(g_plot, carry);
-    g_plot[PCL_P_ORDER_FRAME] = PCL_NEVER;
+    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
     g_plot[PCL_P_AUX0] = programmed; g_plot[PCL_P_AUX1] = which;
     g_plot[PCL_P_AUX2] = ball_reset; g_plot[PCL_P_AUX3] = noisy_pay ? 1 : 0;
-    if (noisy) p.out.d_reward_f64[env] = noisy_pay ? reward_f64 : (double)dir.reward;
-    else p.out.d_reward[env] = dir.reward;
-    p.out.d_has_reward[env] = 1;
-    p.out.d_discount[env] = dir.discount;
-    p.out.d_done[env] = (uint8_t)dir.game_over;
+    // has_reward is 1: PlayerSprite.update pays (possibly 0) at every step
+    if (noisy) store_outputs(p.out, env, dir, noisy_pay ? reward_f64 : (double)dir.reward);
+    else store_outputs(p.out, env, dir);
   }
 
   // ---- render (engine.py:737-759): backdrop, P, a, b, Q; lane r paints row r.  A ball

@@ -33,8 +33,7 @@ using board::kMaxEnt;
 using board::WarpState;
 using board::Ctx;
 using board::render;
-using board::load_sprite;
-using board::store_sprite;
+using board::warp_store_sprite;
 using board::scrolly_move_dyn;
 
 // The order / egocentric-set registers of scrolling group g <-> `plot`.
@@ -110,9 +109,7 @@ fixture_step(const StepParams p) {
   }
   board::stage_board(c, restart, g_board);
 
-  Plot plot;
-  plot.frame = st->plot[PCL_P_FRAME] + 1;    // engine.py:716
-  plot.error = st->plot[PCL_P_ERROR];
+  Plot plot = step_plot(st->plot, carry.error);
   group_in(plot, st, 0);
   Directives dir = fresh_directives();
   const int32_t* act = restart ? nullptr : p.actions + (int64_t)env * p.actions_per_env;
@@ -134,7 +131,7 @@ fixture_step(const StepParams p) {
         walker_move(sp, s, motion, plot, H, W, p.confined[s] != 0, p.egocentric[s] != 0, lane,
                     [&](int r, int col) { return in_set(imp, board[r * pitch + col]); });
         group_out(plot, st, p.sprite_group[s], lane);
-        store_sprite(st->sprites[s], sp, lane);
+        warp_store_sprite(st->sprites[s], sp, lane);
       }
       for (int d = 0; d < D; ++d) {
         if (p.drape_char[d] == ch && p.drape_kind[d]) {
@@ -194,9 +191,8 @@ fixture_step(const StepParams p) {
 
   __syncwarp();
   if (lane == 0) {
-    st->plot[PCL_P_FRAME] = plot.frame; st->plot[PCL_P_GAME_OVER] = dir.game_over;
-    st->plot[PCL_P_ERROR] = plot.error;
-    for (int w = 0; w < PCL_GROUP_WORDS; ++w) st->plot[PCL_P_ORDER_R + w] = st->groups[0][w];
+    group_in(plot, st, 0);
+    store_plot<ORDER_ALL>(st->plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
   __syncwarp();

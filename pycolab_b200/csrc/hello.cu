@@ -39,14 +39,12 @@ hello_step(const StepParams p) {
   const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drape;
   const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
   // lane s < S owns sprite s; every lane knows the drape's roll counters
-  int row = 0, col = 0, flags = 0, kset = 0;
-  if (lane < S) {
-    const int32_t* r = src_s + lane * PCL_SPRITE_WORDS;
-    row = r[PCL_S_ROW]; col = r[PCL_S_COL]; flags = r[PCL_S_FLAGS]; kset = r[PCL_S_AUX0];
-  }
+  Sprite sp = {};
+  if (lane < S) sp = load_sprite(src_s + lane * PCL_SPRITE_WORDS);
+  const int kset = sp.aux0;
   int roll_r = src_d[PCL_D_AUX0], roll_c = src_d[PCL_D_AUX1];
-  const int frame = src_p[PCL_P_FRAME] + 1;                           // engine.py:716
   const PlotCarry carry = plot_carry(g_plot, restart);
+  const Plot plot = step_plot(src_p, carry.error);
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   Directives dir = fresh_directives();
 
@@ -58,8 +56,8 @@ hello_step(const StepParams p) {
       const int dy0 = (action == 1 || action == 2) ? 1 : -1;
       const int dx = (kset >= 2) ? -dx0 : dx0;
       const int dy = (kset == 1 || kset == 2) ? -dy0 : dy0;
-      col = (col + dx + W) % W;
-      row = (row + dy + H) % H;
+      sp.col = (sp.col + dx + W) % W;
+      sp.row = (sp.row + dy + H) % H;
     }
     // RollingDrape.update: axes (0, 0, 1, 1), shifts (-1, 1, -1, 1)
     if (action < 2) roll_r = (roll_r + (action == 0 ? H - 1 : 1)) % H;
@@ -70,17 +68,15 @@ hello_step(const StepParams p) {
   }
 
   __syncwarp();
-  if (lane < S) {
-    int32_t* r = g_sprites + lane * PCL_SPRITE_WORDS;
-    r[PCL_S_ROW] = row; r[PCL_S_COL] = col; r[PCL_S_VROW] = row; r[PCL_S_VCOL] = col;
-    r[PCL_S_FLAGS] = flags; r[PCL_S_AUX0] = kset;
+  if (lane < S) {                                   // a plain Sprite: virtual = true position
+    sp.vrow = sp.row; sp.vcol = sp.col;
+    store_sprite(g_sprites + lane * PCL_SPRITE_WORDS, sp, PCL_S_AUX1);
   }
   if (lane == 0) {
     g_drape[PCL_D_AUX0] = roll_r; g_drape[PCL_D_AUX1] = roll_c;
     g_drape[PCL_D_LAST_FRAME] = src_d[PCL_D_LAST_FRAME];
-    g_plot[PCL_P_FRAME] = frame; g_plot[PCL_P_GAME_OVER] = dir.game_over;
     store_carry(g_plot, carry);
-    g_plot[PCL_P_ORDER_FRAME] = PCL_NEVER;
+    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
 
@@ -89,9 +85,9 @@ hello_step(const StepParams p) {
   int s_row[4], s_col[4], s_vis[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    s_row[k] = __shfl_sync(PCL_FULL, row, k);
-    s_col[k] = __shfl_sync(PCL_FULL, col, k);
-    s_vis[k] = k < S ? (__shfl_sync(PCL_FULL, flags, k) & 1) : 0;
+    s_row[k] = __shfl_sync(PCL_FULL, sp.row, k);
+    s_col[k] = __shfl_sync(PCL_FULL, sp.col, k);
+    s_vis[k] = k < S ? (__shfl_sync(PCL_FULL, sp.flags, k) & 1) : 0;
   }
   const int n = S + 1;
   uint8_t* board = p.out.d_board + (int64_t)env * H * pitch;

@@ -90,20 +90,12 @@ marauders_step(const StepParams p) {
   }
   Sprite sp[kS];
 #pragma unroll
-  for (int i = 0; i < kS; ++i) {
-    const int32_t* r = rec + i * PCL_SPRITE_WORDS;
-    sp[i].row = r[PCL_S_ROW]; sp[i].col = r[PCL_S_COL];
-    sp[i].vrow = r[PCL_S_VROW]; sp[i].vcol = r[PCL_S_VCOL];
-    sp[i].flags = r[PCL_S_FLAGS]; sp[i].aux0 = sp[i].aux1 = sp[i].aux2 = 0;
-  }
+  for (int i = 0; i < kS; ++i) sp[i] = load_sprite(rec + i * PCL_SPRITE_WORDS);
   Drape marauders;
   marauders.aux0 = rec[56 + PCL_DRAPE_WORDS + PCL_D_AUX0];
-  Plot plot;
-  plot.frame = rec[72 + PCL_P_FRAME]; plot.error = rec[72 + PCL_P_ERROR];
+  Plot plot = step_plot(rec + 72, rec[72 + PCL_P_ERROR]);
   plot.aux0 = rec[72 + PCL_P_AUX0]; plot.aux1 = rec[72 + PCL_P_AUX1];
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
   Directives dir = fresh_directives();
-  plot.frame += 1;
 
   // ---- the stale board, as far as anybody looks at it --------------------
   // top[i]: bolt i is the visible character of its cell (layers[c] = board==c,
@@ -230,14 +222,9 @@ marauders_step(const StepParams p) {
   __syncwarp();
   if (lane == 0) {
 #pragma unroll
-    for (int i = 0; i < kS; ++i) {
-      int32_t* r = rec + i * PCL_SPRITE_WORDS;
-      r[PCL_S_ROW] = sp[i].row; r[PCL_S_COL] = sp[i].col;
-      r[PCL_S_VROW] = sp[i].vrow; r[PCL_S_VCOL] = sp[i].vcol; r[PCL_S_FLAGS] = sp[i].flags;
-    }
+    for (int i = 0; i < kS; ++i) store_sprite(rec + i * PCL_SPRITE_WORDS, sp[i], PCL_S_AUX0);
     rec[56 + PCL_DRAPE_WORDS + PCL_D_AUX0] = marauders.aux0;
-    rec[72 + PCL_P_FRAME] = plot.frame; rec[72 + PCL_P_GAME_OVER] = dir.game_over;
-    rec[72 + PCL_P_ERROR] = plot.error;
+    store_plot<ORDER_KEEP>(rec + 72, plot, dir);
     rec[72 + PCL_P_AUX0] = plot.aux0; rec[72 + PCL_P_AUX1] = plot.aux1;
     store_outputs(p.out, env, dir);
   }

@@ -72,18 +72,9 @@ ordeal_step(const StepParams p) {
   cp_async_wait_all();
   __syncwarp();
 
-  Sprite pl, dd;
-  pl.row = rec[PCL_S_ROW]; pl.col = rec[PCL_S_COL]; pl.vrow = rec[PCL_S_VROW];
-  pl.vcol = rec[PCL_S_VCOL]; pl.flags = rec[PCL_S_FLAGS]; pl.aux0 = pl.aux1 = pl.aux2 = 0;
-  dd = pl;
-  if (S > 1) {
-    dd.row = rec[8 + PCL_S_ROW]; dd.col = rec[8 + PCL_S_COL]; dd.vrow = rec[8 + PCL_S_VROW];
-    dd.vcol = rec[8 + PCL_S_VCOL]; dd.flags = rec[8 + PCL_S_FLAGS];
-  }
-  Plot plot;
-  plot.frame = rec[32 + PCL_P_FRAME] + 1;                    // engine.py:716
-  plot.error = rec[32 + PCL_P_ERROR];
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
+  Sprite pl = load_sprite(rec);
+  Sprite dd = S > 1 ? load_sprite(rec + 8) : pl;
+  Plot plot = step_plot(rec + 32, rec[32 + PCL_P_ERROR]);
   int has_sword = rec[32 + PCL_P_AUX0], last_pos = rec[32 + PCL_P_AUX1];
   int next_chapter = rec[32 + PCL_P_AUX2];
   const int prior = rec[32 + PCL_P_AUX3];
@@ -182,14 +173,9 @@ ordeal_step(const StepParams p) {
   // ---- _apply_and_clear_plot (engine.py:761-847) + records back
   __syncwarp();
   if (lane == 0) {
-    rec[PCL_S_ROW] = pl.row; rec[PCL_S_COL] = pl.col; rec[PCL_S_VROW] = pl.vrow;
-    rec[PCL_S_VCOL] = pl.vcol; rec[PCL_S_FLAGS] = pl.flags;
-    if (S > 1) {
-      rec[8 + PCL_S_ROW] = dd.row; rec[8 + PCL_S_COL] = dd.col; rec[8 + PCL_S_VROW] = dd.vrow;
-      rec[8 + PCL_S_VCOL] = dd.vcol; rec[8 + PCL_S_FLAGS] = dd.flags;
-    }
-    rec[32 + PCL_P_FRAME] = plot.frame; rec[32 + PCL_P_GAME_OVER] = dir.game_over;
-    rec[32 + PCL_P_ERROR] = plot.error;
+    store_sprite(rec, pl, PCL_S_AUX0);
+    if (S > 1) store_sprite(rec + 8, dd, PCL_S_AUX0);
+    store_plot<ORDER_KEEP>(rec + 32, plot, dir);
     rec[32 + PCL_P_AUX0] = has_sword; rec[32 + PCL_P_AUX1] = last_pos;
     rec[32 + PCL_P_AUX2] = next_chapter;
     store_outputs(p.out, env, dir);

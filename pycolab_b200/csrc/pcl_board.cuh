@@ -88,18 +88,10 @@ __device__ inline void render(const Ctx& c) {
   __syncwarp();
 }
 
-__device__ __forceinline__ Sprite load_sprite(const int32_t* r) {
-  Sprite s;
-  s.row = r[0]; s.col = r[1]; s.vrow = r[2]; s.vcol = r[3];
-  s.flags = r[4]; s.aux0 = r[5]; s.aux1 = r[6]; s.aux2 = r[7];
-  return s;
-}
-__device__ __forceinline__ void store_sprite(int32_t* r, const Sprite& s, int lane) {
+// Write a sprite back to its record in the warp's state (one lane, between warp barriers).
+__device__ __forceinline__ void warp_store_sprite(int32_t* r, const Sprite& s, int lane) {
   __syncwarp();
-  if (lane == 0) {
-    r[0] = s.row; r[1] = s.col; r[2] = s.vrow; r[3] = s.vcol;
-    r[4] = s.flags; r[5] = s.aux0; r[6] = s.aux1; r[7] = s.aux2;
-  }
+  if (lane == 0) store_sprite(r, s);
   __syncwarp();
 }
 
@@ -119,21 +111,22 @@ __device__ inline bool is_possible(const Ctx& c, const Plot& plot, int motion) {
 __device__ inline void scrolly_move_dyn(const Ctx& c, int d, int motion, Plot& plot) {
   const StepParams& p = *c.p;
   int32_t* rec = c.st->drapes[d];
-  int corner_r = rec[PCL_D_CORNER_R], corner_c = rec[PCL_D_CORNER_C];
-  int pre_r = rec[PCL_D_PRE_R], pre_c = rec[PCL_D_PRE_C], last = rec[PCL_D_LAST_FRAME];
+  Drape dp = load_drape(rec);
   const ScrollyCfg cfg = scrolly_cfg(p.H, p.W, p.PH, p.PW, p.margin[d][0], p.margin[d][1]);
-  if (last < plot.frame) { last = plot.frame; pre_r = corner_r; pre_c = corner_c; }
+  if (dp.last_frame < plot.frame) {
+    dp.last_frame = plot.frame; dp.pre_r = dp.corner_r; dp.pre_c = dp.corner_c;
+  }
   const int dr = motion_dr(motion), dc = motion_dc(motion);
   if (plot.order_frame == plot.frame) {
     if (dr != plot.order_r && dc != plot.order_c) plot.error |= PCL_ENV_ERR_ORDER_MISMATCH;
-    corner_r += plot.order_r; corner_c += plot.order_c;
+    dp.corner_r += plot.order_r; dp.corner_c += plot.order_c;
   } else if (motion != PCL_M_STAY) {
     if (!cfg.have_margins) {
       if (is_possible(c, plot, motion)) {
-        const int nr = corner_r + dr, nc = corner_c + dc;
+        const int nr = dp.corner_r + dr, nc = dp.corner_c + dc;
         const int orr = (0 <= nr && nr <= cfg.limit_r) ? dr : 0;
         const int occ = (0 <= nc && nc <= cfg.limit_c) ? dc : 0;
-        corner_r += orr; corner_c += occ;
+        dp.corner_r += orr; dp.corner_c += occ;
         plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
       }
     } else {
@@ -149,21 +142,18 @@ __device__ inline void scrolly_move_dyn(const Ctx& c, int d, int motion, Plot& p
       }
       if (want_v || want_h) {
         const int orr = want_v ? dr : 0, occ = want_h ? dc : 0;
-        const int nr = corner_r + orr, nc = corner_c + occ;
+        const int nr = dp.corner_r + orr, nc = dp.corner_c + occ;
         bool can = (0 <= nr && nr <= cfg.limit_r) && (0 <= nc && nc <= cfg.limit_c);
         can = can && is_possible(c, plot, motion);
         if (can) {
-          corner_r = nr; corner_c = nc;
+          dp.corner_r = nr; dp.corner_c = nc;
           plot.order_r = orr; plot.order_c = occ; plot.order_frame = plot.frame;
         }
       }
     }
   }
   __syncwarp();
-  if (c.lane == 0) {
-    rec[PCL_D_CORNER_R] = corner_r; rec[PCL_D_CORNER_C] = corner_c;
-    rec[PCL_D_PRE_R] = pre_r; rec[PCL_D_PRE_C] = pre_c; rec[PCL_D_LAST_FRAME] = last;
-  }
+  if (c.lane == 0) store_drape(rec, dp, PCL_D_AUX0);
   __syncwarp();
 }
 

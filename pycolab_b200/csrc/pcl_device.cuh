@@ -10,6 +10,7 @@
 #pragma once
 
 #include <stdint.h>
+#include <stddef.h>
 #include <limits.h>
 
 #include "../../include/pcl.h"
@@ -34,6 +35,65 @@ struct Plot {                       // plot.py:69-104 + scrolling.py:198-241
   int aux0, aux1, aux2, aux3;
   int crop_r, crop_c, crop_init, reserved;
 };
+
+// The structs are the records' word layout (include/pcl.h), so the codec below is the
+// one place that knows it.  It takes a plain int32 pointer: a global record or one
+// staged in shared memory.
+static_assert(sizeof(Sprite) == PCL_SPRITE_WORDS * 4 && offsetof(Sprite, row) == PCL_S_ROW * 4 &&
+              offsetof(Sprite, col) == PCL_S_COL * 4 && offsetof(Sprite, vrow) == PCL_S_VROW * 4 &&
+              offsetof(Sprite, vcol) == PCL_S_VCOL * 4 && offsetof(Sprite, flags) == PCL_S_FLAGS * 4 &&
+              offsetof(Sprite, aux0) == PCL_S_AUX0 * 4 && offsetof(Sprite, aux1) == PCL_S_AUX1 * 4 &&
+              offsetof(Sprite, aux2) == PCL_S_AUX2 * 4, "Sprite is not the sprite record");
+static_assert(sizeof(Drape) == PCL_DRAPE_WORDS * 4 &&
+              offsetof(Drape, corner_r) == PCL_D_CORNER_R * 4 &&
+              offsetof(Drape, corner_c) == PCL_D_CORNER_C * 4 &&
+              offsetof(Drape, pre_r) == PCL_D_PRE_R * 4 && offsetof(Drape, pre_c) == PCL_D_PRE_C * 4 &&
+              offsetof(Drape, last_frame) == PCL_D_LAST_FRAME * 4 &&
+              offsetof(Drape, aux0) == PCL_D_AUX0 * 4 && offsetof(Drape, aux1) == PCL_D_AUX1 * 4 &&
+              offsetof(Drape, aux2) == PCL_D_AUX2 * 4, "Drape is not the drape record");
+static_assert(sizeof(Plot) == PCL_PLOT_WORDS * 4 && offsetof(Plot, frame) == PCL_P_FRAME * 4 &&
+              offsetof(Plot, game_over) == PCL_P_GAME_OVER * 4 &&
+              offsetof(Plot, error) == PCL_P_ERROR * 4 && offsetof(Plot, episodes) == PCL_P_EPISODES * 4 &&
+              offsetof(Plot, order_r) == PCL_P_ORDER_R * 4 && offsetof(Plot, order_c) == PCL_P_ORDER_C * 4 &&
+              offsetof(Plot, order_frame) == PCL_P_ORDER_FRAME * 4 &&
+              offsetof(Plot, ego_mask) == PCL_P_EGO_MASK * 4 && offsetof(Plot, aux0) == PCL_P_AUX0 * 4 &&
+              offsetof(Plot, aux1) == PCL_P_AUX1 * 4 && offsetof(Plot, aux2) == PCL_P_AUX2 * 4 &&
+              offsetof(Plot, aux3) == PCL_P_AUX3 * 4 && offsetof(Plot, crop_r) == PCL_P_CROP_R * 4 &&
+              offsetof(Plot, crop_c) == PCL_P_CROP_C * 4 &&
+              offsetof(Plot, crop_init) == PCL_P_CROP_INIT * 4 &&
+              offsetof(Plot, reserved) == PCL_P_RESERVED * 4, "Plot is not the plot record");
+
+__device__ __forceinline__ Sprite load_sprite(const int32_t* r) {
+  Sprite s;
+  s.row = r[PCL_S_ROW]; s.col = r[PCL_S_COL]; s.vrow = r[PCL_S_VROW]; s.vcol = r[PCL_S_VCOL];
+  s.flags = r[PCL_S_FLAGS]; s.aux0 = r[PCL_S_AUX0]; s.aux1 = r[PCL_S_AUX1]; s.aux2 = r[PCL_S_AUX2];
+  return s;
+}
+// The stores write the words before `end` (a PCL_S_* / PCL_D_* index), all eight by
+// default.  A kernel that leaves a staged record's AUX words alone stores up to AUX0 and
+// need not hold them in registers.
+__device__ __forceinline__ void store_sprite(int32_t* r, const Sprite& s, int end = PCL_SPRITE_WORDS) {
+  r[PCL_S_ROW] = s.row; r[PCL_S_COL] = s.col; r[PCL_S_VROW] = s.vrow; r[PCL_S_VCOL] = s.vcol;
+  r[PCL_S_FLAGS] = s.flags;
+  if (end > PCL_S_AUX0) r[PCL_S_AUX0] = s.aux0;
+  if (end > PCL_S_AUX1) r[PCL_S_AUX1] = s.aux1;
+  if (end > PCL_S_AUX2) r[PCL_S_AUX2] = s.aux2;
+}
+__device__ __forceinline__ Drape load_drape(const int32_t* r) {
+  Drape d;
+  d.corner_r = r[PCL_D_CORNER_R]; d.corner_c = r[PCL_D_CORNER_C];
+  d.pre_r = r[PCL_D_PRE_R]; d.pre_c = r[PCL_D_PRE_C]; d.last_frame = r[PCL_D_LAST_FRAME];
+  d.aux0 = r[PCL_D_AUX0]; d.aux1 = r[PCL_D_AUX1]; d.aux2 = r[PCL_D_AUX2];
+  return d;
+}
+__device__ __forceinline__ void store_drape(int32_t* r, const Drape& d, int end = PCL_DRAPE_WORDS) {
+  r[PCL_D_CORNER_R] = d.corner_r; r[PCL_D_CORNER_C] = d.corner_c;
+  r[PCL_D_PRE_R] = d.pre_r; r[PCL_D_PRE_C] = d.pre_c; r[PCL_D_LAST_FRAME] = d.last_frame;
+  if (end > PCL_D_AUX0) r[PCL_D_AUX0] = d.aux0;
+  if (end > PCL_D_AUX1) r[PCL_D_AUX1] = d.aux1;
+  if (end > PCL_D_AUX2) r[PCL_D_AUX2] = d.aux2;
+}
+
 // Engine directives accumulated during one step (plot.py:69-104).
 struct Directives {
   int reward;
@@ -384,9 +444,52 @@ __device__ __forceinline__ void store_carry(int32_t* plot, const PlotCarry& c) {
   plot[PCL_P_EPISODES] = c.episodes; plot[PCL_P_ERROR] = c.error;
 }
 
+// The Plot a step starts from: the frame after the source record's (engine.py:716), the
+// carried error word, and the source record's scrolling order (kOrder) or no order.  The
+// AUX words are the program's to read.
+template <bool kOrder = false>
+__device__ __forceinline__ Plot step_plot(const int32_t* src, int error) {
+  Plot q;
+  q.frame = src[PCL_P_FRAME] + 1;
+  q.error = error;
+  if (kOrder) {
+    q.order_r = src[PCL_P_ORDER_R]; q.order_c = src[PCL_P_ORDER_C];
+    q.order_frame = src[PCL_P_ORDER_FRAME]; q.ego_mask = src[PCL_P_EGO_MASK];
+  } else {
+    q.order_r = q.order_c = 0; q.order_frame = PCL_NEVER; q.ego_mask = 0;
+  }
+  return q;
+}
+
+// Which scrolling-order words store_plot writes: none (the record keeps its own), only
+// the order frame, back to PCL_NEVER (programs that never scroll), or all four.
+enum PlotOrder { ORDER_KEEP, ORDER_CLEAR, ORDER_ALL };
+
+// The engine's words of the plot record after a step: frame, game_over, the error word
+// and the order words kOrder names.  The episode count is the carry's (store_carry); the
+// AUX words are the program's to store, and the CROP words the cropper epilogue's.
+template <PlotOrder kOrder>
+__device__ __forceinline__ void store_plot(int32_t* rec, const Plot& q, const Directives& dir) {
+  rec[PCL_P_FRAME] = q.frame; rec[PCL_P_GAME_OVER] = dir.game_over; rec[PCL_P_ERROR] = q.error;
+  if (kOrder == ORDER_CLEAR) rec[PCL_P_ORDER_FRAME] = PCL_NEVER;
+  if (kOrder == ORDER_ALL) {
+    rec[PCL_P_ORDER_R] = q.order_r; rec[PCL_P_ORDER_C] = q.order_c;
+    rec[PCL_P_ORDER_FRAME] = q.order_frame; rec[PCL_P_EGO_MASK] = q.ego_mask;
+  }
+}
+
 // The step's outputs for env `env` (one lane stores them).
 __device__ __forceinline__ void store_outputs(const pcl_outputs& out, int env, const Directives& dir) {
   out.d_reward[env] = dir.reward;
+  out.d_has_reward[env] = (uint8_t)dir.has_reward;
+  out.d_discount[env] = dir.discount;
+  out.d_done[env] = (uint8_t)dir.game_over;
+}
+// The same for a program whose rewards are float64 (Program::float_reward): `reward` goes
+// to d_reward_f64 and d_reward is not written.
+__device__ __forceinline__ void store_outputs(const pcl_outputs& out, int env, const Directives& dir,
+                                              double reward) {
+  out.d_reward_f64[env] = reward;
   out.d_has_reward[env] = (uint8_t)dir.has_reward;
   out.d_discount[env] = dir.discount;
   out.d_done[env] = (uint8_t)dir.game_over;

@@ -488,14 +488,7 @@ scrolly_maze_step(const StepParams p) {
   // ---- registers: the drapes / plot / player fields every lane needs, plus ONE
   // walker per lane (lane & 3: P, a, b, c) for the SIMT part of group 1 ---------
   const int me = lane & 3;
-  Sprite mine;
-  {
-    const int32_t* r = rec + me * PCL_SPRITE_WORDS;
-    mine.row = r[PCL_S_ROW]; mine.col = r[PCL_S_COL];
-    mine.vrow = r[PCL_S_VROW]; mine.vcol = r[PCL_S_VCOL];
-    mine.flags = r[PCL_S_FLAGS]; mine.aux0 = r[PCL_S_AUX0]; mine.aux1 = r[PCL_S_AUX1];
-    mine.aux2 = 0;
-  }
+  Sprite mine = load_sprite(rec + me * PCL_SPRITE_WORDS);
   // The player as every lane sees it (previous render + permits).
   const int p_row = rec[PCL_S_ROW], p_col = rec[PCL_S_COL];
   const int p_vrow = rec[PCL_S_VROW], p_vcol = rec[PCL_S_VCOL];
@@ -504,14 +497,8 @@ scrolly_maze_step(const StepParams p) {
   // The '@' drape and the plot's coin count stay in the records until group 2: they
   // are not held in registers through group 1.
   const int32_t* rec_coins = rec + 32 + PCL_DRAPE_WORDS;
-  Drape walls;
-  {
-    const int32_t* r = rec + 32;
-    walls.corner_r = r[PCL_D_CORNER_R]; walls.corner_c = r[PCL_D_CORNER_C];
-    walls.pre_r = r[PCL_D_PRE_R]; walls.pre_c = r[PCL_D_PRE_C];
-    walls.last_frame = r[PCL_D_LAST_FRAME];
-  }
-  Plot plot;
+  Drape walls = load_drape(rec + 32);
+  Plot plot;                                 // not step_plot(): it reorders this kernel's code
   {
     const int32_t* r = rec + 48;
     plot.frame = r[PCL_P_FRAME]; plot.error = r[PCL_P_ERROR];
@@ -747,13 +734,8 @@ scrolly_maze_step(const StepParams p) {
     }
   }
   __syncwarp();                              // every lane has read the records it needs (racecheck)
-  if (lane < 4) {                            // write my walker back
-    int32_t* r = rec + me * PCL_SPRITE_WORDS;
-    r[PCL_S_ROW] = mine.row; r[PCL_S_COL] = mine.col;
-    r[PCL_S_VROW] = mine.vrow; r[PCL_S_VCOL] = mine.vcol;
-    r[PCL_S_FLAGS] = mine.flags; r[PCL_S_AUX0] = mine.aux0;
-    if (is_p) r[PCL_S_AUX1] = mine.aux1;
-  }
+  if (lane < 4)                              // write my walker back
+    store_sprite(rec + me * PCL_SPRITE_WORDS, mine, is_p ? PCL_S_AUX2 : PCL_S_AUX1);
   if (motion != PCL_M_NONE) plot.ego_mask |= 1;             // sprites.py:443 (P only)
   plot.error |= __reduce_or_sync(PCL_FULL, (unsigned)(lane < 4 ? my_err : 0));
   if (__any_sync(PCL_FULL, lane < 4 && hit)) terminate(dir);
@@ -765,11 +747,7 @@ scrolly_maze_step(const StepParams p) {
   pl.aux0 = __shfl_sync(PCL_FULL, mine.aux0, 0); pl.aux1 = __shfl_sync(PCL_FULL, mine.aux1, 0);
 
   // ---- 4b. update group 2: '@' CashDrape (scrolly_maze.py:341-364) -------
-  Drape coins;
-  coins.corner_r = rec_coins[PCL_D_CORNER_R]; coins.corner_c = rec_coins[PCL_D_CORNER_C];
-  coins.pre_r = rec_coins[PCL_D_PRE_R]; coins.pre_c = rec_coins[PCL_D_PRE_C];
-  coins.last_frame = rec_coins[PCL_D_LAST_FRAME];
-  coins.aux0 = rec_coins[PCL_D_AUX0]; coins.aux1 = rec_coins[PCL_D_AUX1];
+  Drape coins = load_drape(rec_coins);
   scrolly_touch_prescroll(coins, plot);
   plot.aux0 = rec[48 + PCL_P_AUX0];
   int picked_r = -1, picked_c = -1;          // pattern cell cleared this frame
@@ -807,21 +785,10 @@ scrolly_maze_step(const StepParams p) {
   PCL_STAMP(kStWait);
   __syncwarp();
   if (lane == 0) {
-    int32_t* r = rec + 32;
-    r[PCL_D_CORNER_R] = walls.corner_r; r[PCL_D_CORNER_C] = walls.corner_c;
-    r[PCL_D_PRE_R] = walls.pre_r; r[PCL_D_PRE_C] = walls.pre_c;
-    r[PCL_D_LAST_FRAME] = walls.last_frame;
-    r += PCL_DRAPE_WORDS;
-    r[PCL_D_CORNER_R] = coins.corner_r; r[PCL_D_CORNER_C] = coins.corner_c;
-    r[PCL_D_PRE_R] = coins.pre_r; r[PCL_D_PRE_C] = coins.pre_c;
-    r[PCL_D_LAST_FRAME] = coins.last_frame;
-    r[PCL_D_AUX0] = coins.aux0; r[PCL_D_AUX1] = coins.aux1;
-    r = rec + 48;
-    r[PCL_P_FRAME] = plot.frame; r[PCL_P_GAME_OVER] = dir.game_over;
-    r[PCL_P_ERROR] = plot.error;
-    r[PCL_P_ORDER_R] = plot.order_r; r[PCL_P_ORDER_C] = plot.order_c;
-    r[PCL_P_ORDER_FRAME] = plot.order_frame; r[PCL_P_EGO_MASK] = plot.ego_mask;
-    r[PCL_P_AUX0] = plot.aux0;
+    store_drape(rec + 32, walls, PCL_D_AUX0);
+    store_drape(rec + 32 + PCL_DRAPE_WORDS, coins, PCL_D_AUX2);
+    store_plot<ORDER_ALL>(rec + 48, plot, dir);
+    rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
     // The pick-up's group of the env's pattern now differs from the template.
     if (picked_r >= 0) rec[32 + PCL_DRAPE_WORDS + PCL_D_AUX2] |= 1 << (picked_r >> coin_group_shift(p.PH));

@@ -57,18 +57,13 @@ sequence_recall_step(const StepParams p) {
   const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
   const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
 
-  Sprite pl;
-  pl.row = src_s[PCL_S_ROW]; pl.col = src_s[PCL_S_COL];
-  pl.vrow = src_s[PCL_S_VROW]; pl.vcol = src_s[PCL_S_VCOL];
-  pl.flags = src_s[PCL_S_FLAGS]; pl.aux0 = pl.aux1 = pl.aux2 = 0;
+  Sprite pl = load_sprite(src_s);
+  pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
   const int covered0 = src_d[PCL_D_AUX0];
   int covered = covered0;
   int cleared = src_d[PCL_DRAPE_WORDS + PCL_D_AUX0];
-  Plot plot;
-  plot.frame = src_p[PCL_P_FRAME] + 1;                                // engine.py:716
   const PlotCarry carry = plot_carry(g_plot, restart);
-  plot.error = carry.error;
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
+  Plot plot = step_plot(src_p, carry.error);
   int pc = src_p[PCL_P_AUX0], fis = src_p[PCL_P_AUX1], timeout = src_p[PCL_P_AUX2];
   uint32_t seq = (uint32_t)src_p[PCL_P_AUX3];
   const int L = p.program_arg[0];
@@ -160,10 +155,7 @@ sequence_recall_step(const StepParams p) {
   }
 
   if (lane == 0) {
-    g_sprite[PCL_S_ROW] = pl.row; g_sprite[PCL_S_COL] = pl.col;
-    g_sprite[PCL_S_VROW] = pl.vrow; g_sprite[PCL_S_VCOL] = pl.vcol;
-    g_sprite[PCL_S_FLAGS] = pl.flags; g_sprite[PCL_S_AUX0] = 0;
-    g_sprite[PCL_S_AUX1] = 0; g_sprite[PCL_S_AUX2] = 0;
+    store_sprite(g_sprite, pl);
     const int32_t* init_d = p.st.d_drapes_init + lvl * p.st.drapes_init_bstride;
 #pragma unroll
     for (int d = 0; d < 2; ++d) {
@@ -172,16 +164,11 @@ sequence_recall_step(const StepParams p) {
       for (int w = 0; w < PCL_DRAPE_WORDS; ++w) r[w] = r0[w];
       r[PCL_D_AUX0] = d == DM ? covered : cleared;
     }
-    g_plot[PCL_P_FRAME] = f; g_plot[PCL_P_GAME_OVER] = dir.game_over;
     store_carry(g_plot, carry);
-    g_plot[PCL_P_ERROR] = plot.error;
-    g_plot[PCL_P_ORDER_FRAME] = PCL_NEVER;
+    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
     g_plot[PCL_P_AUX0] = pc; g_plot[PCL_P_AUX1] = fis;
     g_plot[PCL_P_AUX2] = timeout; g_plot[PCL_P_AUX3] = (int)seq;
-    p.out.d_reward_f64[env] = dir.has_reward ? reward : 0.0;
-    p.out.d_has_reward[env] = (uint8_t)dir.has_reward;
-    p.out.d_discount[env] = dir.discount;
-    p.out.d_done[env] = (uint8_t)dir.game_over;
+    store_outputs(p.out, env, dir, dir.has_reward ? reward : 0.0);
   }
 
   // ---- render (engine.py:737-759): backdrop, M over the covered lights, P, '%'

@@ -61,15 +61,11 @@ shockwave_step(const StepParams p) {
   const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprite;
   const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
   const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
-  Sprite pl;
-  pl.row = src_s[PCL_S_ROW]; pl.col = src_s[PCL_S_COL]; pl.vrow = src_s[PCL_S_VROW];
-  pl.vcol = src_s[PCL_S_VCOL]; pl.flags = src_s[PCL_S_FLAGS]; pl.aux0 = pl.aux1 = pl.aux2 = 0;
+  Sprite pl = load_sprite(src_s);
+  pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
   int impact = src_d[PCL_D_AUX0], steps = src_d[PCL_D_AUX1];
-  Plot plot;
-  plot.frame = src_p[PCL_P_FRAME] + 1;                                // engine.py:716
   const PlotCarry carry = plot_carry(g_plot, restart);
-  plot.error = carry.error;
-  plot.order_frame = PCL_NEVER; plot.order_r = plot.order_c = 0; plot.ego_mask = 0;
+  Plot plot = step_plot(src_p, carry.error);
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   Directives dir = fresh_directives();
   // Row `lane` of the curtain the LAST render showed (the art's '@' cells after a restart).
@@ -123,14 +119,11 @@ shockwave_step(const StepParams p) {
     if (BW > 1) row[1] = (uint32_t)(new_row >> 32);
   }
   if (lane == 0) {
-    g_sprite[PCL_S_ROW] = pl.row; g_sprite[PCL_S_COL] = pl.col; g_sprite[PCL_S_VROW] = pl.vrow;
-    g_sprite[PCL_S_VCOL] = pl.vcol; g_sprite[PCL_S_FLAGS] = pl.flags;
-    g_sprite[PCL_S_AUX0] = 0; g_sprite[PCL_S_AUX1] = 0; g_sprite[PCL_S_AUX2] = 0;
+    store_sprite(g_sprite, pl);
     g_drapes[PCL_D_AUX0] = impact; g_drapes[PCL_D_AUX1] = steps;
     g_drapes[PCL_D_LAST_FRAME] = PCL_NEVER;
-    g_plot[PCL_P_FRAME] = plot.frame; g_plot[PCL_P_GAME_OVER] = dir.game_over;
-    g_plot[PCL_P_EPISODES] = carry.episodes; g_plot[PCL_P_ERROR] = plot.error;
-    g_plot[PCL_P_ORDER_FRAME] = PCL_NEVER;
+    store_carry(g_plot, carry);
+    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
 

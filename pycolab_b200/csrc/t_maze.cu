@@ -139,26 +139,13 @@ t_maze_step(const StepParams p) {
   const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
   const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
 
-  Sprite pl[1];
-  pl[0].row = src_s[PCL_S_ROW]; pl[0].col = src_s[PCL_S_COL];
-  pl[0].vrow = src_s[PCL_S_VROW]; pl[0].vcol = src_s[PCL_S_VCOL];
-  pl[0].flags = src_s[PCL_S_FLAGS]; pl[0].aux0 = src_s[PCL_S_AUX0]; pl[0].aux1 = src_s[PCL_S_AUX1];
-  pl[0].aux2 = 0;
+  Sprite pl[1] = {load_sprite(src_s)};
+  pl[0].aux2 = 0;                                                     // stored as zero
   Drape dr[ND];
 #pragma unroll
-  for (int d = 0; d < ND; ++d) {
-    const int32_t* r = src_d + d * PCL_DRAPE_WORDS;
-    dr[d].corner_r = r[PCL_D_CORNER_R]; dr[d].corner_c = r[PCL_D_CORNER_C];
-    dr[d].pre_r = r[PCL_D_PRE_R]; dr[d].pre_c = r[PCL_D_PRE_C];
-    dr[d].last_frame = r[PCL_D_LAST_FRAME];
-    dr[d].aux0 = r[PCL_D_AUX0]; dr[d].aux1 = r[PCL_D_AUX1]; dr[d].aux2 = r[PCL_D_AUX2];
-  }
-  Plot plot;
-  plot.frame = src_p[PCL_P_FRAME] + 1;                                // engine.py:716
+  for (int d = 0; d < ND; ++d) dr[d] = load_drape(src_d + d * PCL_DRAPE_WORDS);
   const PlotCarry carry = plot_carry(g_plot, restart);
-  plot.error = carry.error;
-  plot.order_r = src_p[PCL_P_ORDER_R]; plot.order_c = src_p[PCL_P_ORDER_C];
-  plot.order_frame = src_p[PCL_P_ORDER_FRAME]; plot.ego_mask = src_p[PCL_P_EGO_MASK];
+  Plot plot = step_plot</*kOrder=*/true>(src_p, carry.error);
   int timeout = src_p[PCL_P_AUX0];                 // the_plot['timeout_frames']
   int tele_frame = src_p[PCL_P_AUX1];              // the_plot.get('teleportation_order_frame', -1)
   int tele_r = src_p[PCL_P_AUX2], tele_c = src_p[PCL_P_AUX3];   // the_plot['teleportation_order']
@@ -308,32 +295,16 @@ t_maze_step(const StepParams p) {
 
   __syncwarp();
   if (lane == 0) {
-    g_sprite[PCL_S_ROW] = pl[0].row; g_sprite[PCL_S_COL] = pl[0].col;
-    g_sprite[PCL_S_VROW] = pl[0].vrow; g_sprite[PCL_S_VCOL] = pl[0].vcol;
-    g_sprite[PCL_S_FLAGS] = pl[0].flags; g_sprite[PCL_S_AUX0] = pl[0].aux0;
-    g_sprite[PCL_S_AUX1] = pl[0].aux1; g_sprite[PCL_S_AUX2] = 0;
+    store_sprite(g_sprite, pl[0]);
     dr[DQ].aux0 = which_goal; dr[DQ].aux1 = yo ? 1 : 0; dr[DQ].aux2 = in_limbo ? 1 : 0;
     dr[DTELE].aux1 = delay; dr[DTELE].aux2 = countdown;
 #pragma unroll
-    for (int d = 0; d < ND; ++d) {
-      int32_t* r = g_drapes + d * PCL_DRAPE_WORDS;
-      r[PCL_D_CORNER_R] = dr[d].corner_r; r[PCL_D_CORNER_C] = dr[d].corner_c;
-      r[PCL_D_PRE_R] = dr[d].pre_r; r[PCL_D_PRE_C] = dr[d].pre_c;
-      r[PCL_D_LAST_FRAME] = dr[d].last_frame;
-      r[PCL_D_AUX0] = dr[d].aux0; r[PCL_D_AUX1] = dr[d].aux1; r[PCL_D_AUX2] = dr[d].aux2;
-    }
-    g_plot[PCL_P_FRAME] = plot.frame; g_plot[PCL_P_GAME_OVER] = dir.game_over;
+    for (int d = 0; d < ND; ++d) store_drape(g_drapes + d * PCL_DRAPE_WORDS, dr[d]);
     store_carry(g_plot, carry);
-    g_plot[PCL_P_ERROR] = plot.error;
-    g_plot[PCL_P_ORDER_R] = plot.order_r; g_plot[PCL_P_ORDER_C] = plot.order_c;
-    g_plot[PCL_P_ORDER_FRAME] = plot.order_frame; g_plot[PCL_P_EGO_MASK] = plot.ego_mask;
+    store_plot<ORDER_ALL>(g_plot, plot, dir);
     g_plot[PCL_P_AUX0] = timeout; g_plot[PCL_P_AUX1] = tele_frame;
     g_plot[PCL_P_AUX2] = tele_r; g_plot[PCL_P_AUX3] = tele_c;
-    // the step's outputs; the reward is float64 (d_reward is not written)
-    p.out.d_reward_f64[env] = dir.has_reward ? reward : 0.0;
-    p.out.d_has_reward[env] = (uint8_t)dir.has_reward;
-    p.out.d_discount[env] = dir.discount;
-    p.out.d_done[env] = (uint8_t)dir.game_over;
+    store_outputs(p.out, env, dir, dir.has_reward ? reward : 0.0);
   }
 
   // ---- render (engine.py:737-759): backdrop, then * # l t r Q P; lane k paints four cells

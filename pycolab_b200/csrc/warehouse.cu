@@ -86,20 +86,11 @@ warehouse_step(const StepParams p) {
   mbar_wait(bar, 0);
   __syncwarp();
 
-  Plot plot;
-  plot.frame = r_plot[PCL_P_FRAME] + 1;                    // engine.py:716
-  plot.error = r_plot[PCL_P_ERROR];
-  plot.order_frame = PCL_NEVER; plot.order_r = 0; plot.order_c = 0; plot.ego_mask = 0;
+  Plot plot = step_plot(r_plot, r_plot[PCL_P_ERROR]);
   Directives dir = fresh_directives();
 
   // Player as of the previous render; box i's record sits in lane i.
-  Sprite player;
-  {
-    const int32_t* r = rec + NB * PCL_SPRITE_WORDS;
-    player.row = r[PCL_S_ROW]; player.col = r[PCL_S_COL];
-    player.vrow = r[PCL_S_VROW]; player.vcol = r[PCL_S_VCOL];
-    player.flags = r[PCL_S_FLAGS]; player.aux0 = player.aux1 = player.aux2 = 0;
-  }
+  Sprite player = load_sprite(rec + NB * PCL_SPRITE_WORDS);
   const bool pl_vis = visible(player);
   const int pl_row = player.row, pl_col = player.col;
   // Sprite characters -> smem (rec words 88..95 are padding); static indices only,
@@ -144,11 +135,7 @@ warehouse_step(const StepParams p) {
     const unsigned who = __ballot_sync(PCL_FULL, pushed);
     if (who) {                               // at most one box can be next to P
       const int j = __ffs(who) - 1;
-      const int32_t* r = rec + j * PCL_SPRITE_WORDS;
-      Sprite box;
-      box.row = r[PCL_S_ROW]; box.col = r[PCL_S_COL];
-      box.vrow = r[PCL_S_VROW]; box.vcol = r[PCL_S_VCOL];
-      box.flags = r[PCL_S_FLAGS]; box.aux0 = r[PCL_S_AUX0]; box.aux1 = box.aux2 = 0;
+      Sprite box = load_sprite(rec + j * PCL_SPRITE_WORDS);
       uint32_t imp[4];
 #pragma unroll
       for (int w = 0; w < 4; ++w) imp[w] = p.impassable[0][w];
@@ -161,11 +148,7 @@ warehouse_step(const StepParams p) {
       walker_move(box, j, motion_of_action(action), plot, H, W, false, false, lane,
                   [&](int r2, int c2) { return in_set(imp, stale_cell(r2, c2)); });
       __syncwarp();
-      if (lane == 0) {
-        int32_t* w = rec + j * PCL_SPRITE_WORDS;
-        w[PCL_S_ROW] = box.row; w[PCL_S_COL] = box.col;
-        w[PCL_S_VROW] = box.vrow; w[PCL_S_VCOL] = box.vcol; w[PCL_S_FLAGS] = box.flags;
-      }
+      if (lane == 0) store_sprite(rec + j * PCL_SPRITE_WORDS, box, PCL_S_AUX0);
       __syncwarp();
       if (lane == j) { b_row = box.row; b_col = box.col; }
     }
@@ -205,12 +188,9 @@ warehouse_step(const StepParams p) {
   // ---- _apply_and_clear_plot + records back
   __syncwarp();
   if (lane == 0) {
-    int32_t* w = rec + NB * PCL_SPRITE_WORDS;
-    w[PCL_S_ROW] = player.row; w[PCL_S_COL] = player.col;
-    w[PCL_S_VROW] = player.vrow; w[PCL_S_VCOL] = player.vcol; w[PCL_S_FLAGS] = player.flags;
+    store_sprite(rec + NB * PCL_SPRITE_WORDS, player, PCL_S_AUX0);
     r_judge[PCL_D_AUX0] = on_goals;
-    r_plot[PCL_P_FRAME] = plot.frame; r_plot[PCL_P_GAME_OVER] = dir.game_over;
-    r_plot[PCL_P_ERROR] = plot.error;
+    store_plot<ORDER_KEEP>(r_plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
   __syncwarp();
