@@ -20,7 +20,7 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from make_golden import refdriver, save, sprite_recorder, tj  # noqa: E402
+from make_golden import refdriver, save, tj  # noqa: E402
 import lp_rnn_cases as lc                                      # noqa: E402
 
 # (name, art (None = the reference's), make_game args, seed, T, policy kwargs)
@@ -61,10 +61,9 @@ def cued_catch():
   for name, art, args, seed, T, kw in CUED_CATCH_CASES:
     art = list(ref.GAME_ART) if art is None else small_cued_catch_art()
     sprites, rewards, types, states = [], [], [], []
-    rec = sprite_recorder('Pab', sprites)
 
     def on_frame(env, out):
-      rec(env, out)
+      sprites.append(tj.sprite_rows(env, 'Pab'))
       rewards.append(np.nan if out[1] is None else float(out[1]))
       types.append(lc.reward_code(out[1]))
       states.append(lc.cued_catch_state(env))
@@ -91,10 +90,9 @@ def sequence_recall():
     art = list(ref.GAME_ART) if art == 'ref' else levels.sequence_recall_art(*art)
     centre = tuple(int(x[0]) for x in np.where(tj.art_to_u8(art) == ord('P')))
     sprites, rewards, states = [], [], []
-    rec = sprite_recorder('P', sprites)
 
     def on_frame(env, out):
-      rec(env, out)
+      sprites.append(tj.sprite_rows(env, 'P'))
       rewards.append(np.nan if out[1] is None else float(out[1]))
       states.append(lc.sequence_recall_state(env))
     random.seed(900 + seed)

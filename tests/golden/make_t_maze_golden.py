@@ -15,7 +15,7 @@ import os
 
 import numpy as np
 
-from make_golden import refdriver, save, sprite_recorder, tj
+from make_golden import refdriver, save, tj
 
 
 def ref_t_maze_module():
@@ -64,10 +64,9 @@ def t_mazes():
     if name.endswith('_quit'):
       actions = [6 if a == 5 and i % 3 == 0 else a for i, a in enumerate(actions)]
     sprites, rewards, goals = [], [], []
-    rec = sprite_recorder('P', sprites)
 
     def on_frame(env, out):
-      rec(env, out)
+      sprites.append(tj.sprite_rows(env, 'P'))
       rewards.append(np.nan if out[1] is None else float(out[1]))
       goals.append(0 if env.things['Q'].which_goal == 'left' else 1)
     random.seed(900 + seed)

@@ -55,14 +55,6 @@ def fixture_kwargs(g):
               update_schedule=cfg['schedule'], z_order=cfg['z_order']), cfg
 
 
-def oracle_sprite_rows(world, chars):
-  rows = []
-  for ch in chars:
-    w = world.things[ch]
-    rows.append([w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol])
-  return rows
-
-
 def new_directive_row(row, n):
   """A stored action row of the `fixture_directives_*` goldens (n motions, reward
   or INT32_MIN, terminate 0/1, z_move_this or -1, z_in_front_of or 0) in the

@@ -169,11 +169,6 @@ def global_generators():
 
 # ----------------------------------------------------------------- recorders --
 
-def reward_type(reward):
-  """0 for no reward, 1 for an int, 2 for a float."""
-  return 0 if reward is None else (2 if isinstance(reward, float) else 1)
-
-
 def value_types(games, game, env):
   """The Python types of a game's registers and Plot keys in an Engine."""
   return ([type(getattr(env.things[ch], name)) for ch, name in games.REGISTERS[game]] +
@@ -197,7 +192,7 @@ class _Recorder(object):
     rows['sprites'].append(self.sprites(env, games.SPRITES[game]))
     rows['registers'].append(self.registers(env, games.REGISTERS[game]) + plot)
     rows['plot_keys'].append(plot)
-    rows['reward_type'].append(reward_type(out[1]))
+    rows['reward_type'].append(tj.reward_type(out[1]))
     rows['reward_f64'].append(np.nan if out[1] is None else float(out[1]))
     rows['corners'].append([self.corner(env, ch)
                             for ch in getattr(games, 'SCROLLYS', {}).get(game, '')])
@@ -232,12 +227,7 @@ class EngineRecorder(_Recorder):
     self.types.append(value_types(self.games, self.game, env))
 
   def sprites(self, env, chars):
-    rows = []
-    for s in (env.things[ch] for ch in chars):
-      vp = getattr(s, 'virtual_position', s.position)     # a plain Sprite has none
-      rows.append([int(s.position[0]), int(s.position[1]), int(bool(s.visible)),
-                   int(vp[0]), int(vp[1])])
-    return rows
+    return tj.sprite_rows(env, chars)
 
   def registers(self, env, regs):
     out = []
@@ -282,13 +272,9 @@ class WorldRecorder(_Recorder):
     super(WorldRecorder, self).__call__(world, out)
 
   def sprites(self, world, chars):
-    rows = []
-    for ch in chars:
-      w = world.things[ch]
-      plain = (self.lowered.program_arg[3] >> self.lowered.sprite_chars.index(ch)) & 1
-      v = (w.row, w.col) if plain else (w.vrow, w.vcol)   # a plain Sprite has no virtual position
-      rows.append([w.row, w.col, int(bool(w.visible)), v[0], v[1]])
-    return rows
+    lowered = self.lowered
+    plain = [ch for s, ch in enumerate(lowered.sprite_chars) if (lowered.program_arg[3] >> s) & 1]
+    return tj.world_sprite_rows(world, chars, plain)
 
   def registers(self, world, regs):
     out = []
@@ -335,10 +321,7 @@ def _assert_replays(games, name, g, make_env, recorder, check_raise):
   if at >= 0:
     check_raise(recorder.env, actions[at], games.RAISES[game])
   got.update(recorder.arrays(), raised_at=np.array([at], dtype=np.int32))
-  missing = sorted(set(g) - set(INPUTS) - set(got))
-  assert not missing, '%s: the replay recorded no %s' % (name, ', '.join(missing))
-  for key in sorted(set(g) - set(INPUTS)):
-    np.testing.assert_array_equal(got[key], g[key], err_msg='%s: %s' % (name, key), strict=True)
+  tj.assert_golden_arrays(name, g, got, INPUTS)
 
 
 def _oracle_raise(world, action, exception):

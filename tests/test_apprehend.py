@@ -1,8 +1,8 @@
 """examples/apprehend.py (SURVEY.md §8f-4): two MazeWalkers, a float64 accumulator and
-one draw from Python's `random` per episode.  Goldens are the reference's own
-trajectories (tests/golden/apprehend_stock_*: 30 episodes each, `random.seed` fixed);
-CPU: the oracle; GPU: the facade Engine (B = 1, slopes drawn by the Python sprites) and
-a batched lock-step whose slopes are drawn ON THE DEVICE from per-env MT19937 states."""
+one draw from Python's `random` per episode.  The replays of its goldens
+(tests/golden/apprehend_stock_*: 30 episodes each, `random.seed` fixed) are in
+test_example_goldens.py and test_gpu_example_goldens.py; here a batched lock-step whose
+slopes are drawn ON THE DEVICE from per-env MT19937 states, and lowering."""
 
 import os
 import random
@@ -10,57 +10,9 @@ import random
 import numpy as np
 import pytest
 
-import golden_cases as gc
 import refdriver
-import trajectory as tj
 from oracle import games as ogames
 from oracle import sampled_check
-
-NAMES = gc.names('apprehend_')
-
-
-def _rows(env, chars='Pb'):
-  out = []
-  for ch in chars:
-    s = env.things[ch]
-    vp = getattr(s, 'virtual_position', s.position)
-    out.append([int(s.position[0]), int(s.position[1]), int(bool(s.visible)),
-                int(vp[0]), int(vp[1])])
-  return out
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_apprehend_matches_reference_golden(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  rng = random.Random(int(g['random_seed'][0]))
-  sprites, floats = [], []
-
-  def on_frame(env, out):
-    sprites.append(_rows(env))
-    floats.append([env.things['b'].aux['dx'], env.things['b'].aux['acc']])
-  got = tj.run_trajectory(lambda: ogames.make_apprehend(art, rng), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  # float64 registers at 0 ulp: slope and accumulator, every frame
-  np.testing.assert_array_equal(g['floats'].view(np.int64), np.array(floats).view(np.int64))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES)
-def test_facade_apprehend_golden(name):
-  """B = 1 facade: the twin's BallSprite draws from the global `random` exactly as
-  upstream, one Engine per episode; the device only integrates."""
-  from pycolab_b200.games import apprehend
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites = []
-  random.seed(int(g['random_seed'][0]))
-  got = tj.run_trajectory(lambda: apprehend.make_game(art), g['actions'].tolist(),
-                          on_frame=lambda env, out: sprites.append(_rows(env)))
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
 
 
 @pytest.mark.gpu

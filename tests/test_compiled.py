@@ -16,6 +16,7 @@ import numpy as np
 import pytest
 
 import boundary_sweep
+import example_games as eg
 import golden_cases as gc
 import refdriver
 import registered_games as rg
@@ -205,17 +206,7 @@ def test_reference_classics_compile_and_match_golden(name):
     compiler.unregister(mod.PlayerSprite)
   assert lowered.program == _lib.PROG_COMPILED
   assert lowered.float_reward and lowered.reward_type is float
-  sprites, types = [], []
-
-  def on_frame(world, out):
-    w = world.things['P']
-    sprites.append([[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]])
-    types.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
+  eg.assert_replays('oracle', name, make_env=lambda: ocompiled.make_world(lowered))
 
 
 # ------------------------------------------------------------ pcl_bind_code --

@@ -18,6 +18,7 @@ import os
 import numpy as np
 import pytest
 
+import example_games as eg
 import golden_cases as gc
 import refdriver
 import registered_games as rg
@@ -37,36 +38,19 @@ def games():
   yield from rg.registered('backdrop_games.py')
 
 
-def _oracle_trajectory(make_engine, actions, rng_seed=None, keys=()):
-  """The oracle's trajectory of a lowered game, with per-frame sprites, Backdrop curtains and
-  Plot keys; returns (trajectory, sprites, curtains, keys, words)."""
-  engine = make_engine()
+def _assert_oracle_replays(name, engine):
+  """The oracle runs lowered `engine` like golden `name`, latching no error."""
   lowered = lowering.lower(engine)
-  plot_keys = [k for k, _ in lowered.plot_keys]
-  words = (ocompiled.seeded_words(lowered, rng_seed)
-           if lowered.rng_streams and rng_seed is not None else None)
-  sprites, curtains, plot = [], [], []
 
-  def on_frame(world, out):
-    w = world.things['P']
-    sprites.append([[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]])
-    curtains.append(world.backdrop.copy())
-    plot.append([world.plot.regs[plot_keys.index(k)] for k in keys])
+  def no_error(world, out):
     assert world.error == 0
-  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered, words), actions,
-                          on_frame=on_frame)
-  return got, sprites, curtains, plot, words
+  eg.assert_replays('oracle', name, make_env=lambda: ocompiled.make_world(lowered),
+                    check=no_error)
 
 
 @pytest.mark.parametrize('name', gc.names('fluvial_'))
 def test_oracle_runs_the_fluvial_pair_like_the_reference(games, name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  got, sprites, curtains, _, _ = _oracle_trajectory(lambda: games.make_fluvial(art),
-                                                    g['actions'].tolist())
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['backdrops'], np.stack(curtains))
+  _assert_oracle_replays(name, games.make_fluvial(tj.u8_to_art(gc.load(name)['art'])))
 
 
 @pytest.fixture(scope='module')
@@ -88,10 +72,7 @@ def test_reference_fluvial_classes_compile_and_replay(ref_fluvial, name):
                                              backdrop=ref_fluvial.RiverBackdrop)
   lowered = lowering.lower(make())
   assert lowered.program == _lib.PROG_COMPILED and lowered.program_arg[4] == 1
-  got, sprites, curtains, _, _ = _oracle_trajectory(make, g['actions'].tolist())
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['backdrops'], np.stack(curtains))
+  _assert_oracle_replays(name, make())
 
 
 @needs_ref

@@ -17,11 +17,11 @@ import numpy as np
 import pytest
 
 import boundary_sweep
+import example_games as eg
 import golden_cases as gc
 import refdriver
 import registered_games as rg
 import scrolly_shapes
-import trajectory as tj
 from oracle import compiled as ocompiled
 from pycolab_b200 import _lib, compiler, lowering
 from pycolab_b200 import things as b_things
@@ -44,9 +44,8 @@ def _margins(name):
   return scrolly_shapes.DEFAULT_MARGINS
 
 
-def _sprite_rows(world, chars):
-  return [[w.row, w.col, int(bool(w.visible)), w.vrow, w.vcol]
-          for w in (world.things[ch] for ch in chars)]
+def _no_error(world, out):
+  assert world.error == 0
 
 
 # ------------------------------------------------------------- the goldens --
@@ -58,15 +57,8 @@ def test_oracle_runs_compiled_maze_like_the_reference(games, name):
   lowered = lowering.lower(games.make_maze(maze, board, beneath, margins=_margins(name)))
   assert lowered.program == _lib.PROG_COMPILED
   assert list(lowered.drape_kind) == [1, 1] and lowered.program_arg[2] == 0b10
-  sprites = []
-
-  def on_frame(world, out):
-    sprites.append(_sprite_rows(world, 'Pabc'))
-    assert world.error == 0
-  got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
+  eg.assert_replays('oracle', name, make_env=lambda: ocompiled.make_world(lowered),
+                    check=_no_error)
 
 
 def test_oracle_raises_on_postscroll_before_the_move(games):
@@ -271,8 +263,7 @@ def test_reference_scrolly_maze_classes_compile_and_match_golden(games):
           update_schedule=[['#'], ['a', 'b', 'c', 'P'], ['@']], z_order='abc@#P')
       lowered = lowering.lower(engine)
       assert lowered.program == _lib.PROG_COMPILED
-      got = tj.run_trajectory(lambda: ocompiled.make_world(lowered), g['actions'].tolist())
-      tj.assert_same_trajectory(g, got, name)
+      eg.assert_replays('oracle', name, make_env=lambda: ocompiled.make_world(lowered))
   finally:
     compiler.unregister(*ours)
 

@@ -1,6 +1,6 @@
 """GPU parity of the aperture program (SURVEY.md §8f-4: two update groups, a
-Drape with logic, ray casting, teleports) against the reference's golden
-trajectories and the oracle."""
+Drape with logic, ray casting, teleports) against the oracle.  The facade's replays of
+its goldens are in test_gpu_example_goldens.py."""
 
 import numpy as np
 import pytest
@@ -11,31 +11,6 @@ from oracle import games as ogames
 from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.mark.parametrize('name', gc.names('aperture_'))
-def test_facade_aperture_golden(name):
-  from pycolab_b200.games import aperture
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  n = min(len(g['actions']), 350)
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    s = env.things['A']
-    sprites.append([[s.position[0], s.position[1], int(bool(s.visible)),
-                     s.virtual_position[0], s.virtual_position[1]]])
-    drape = env.things['X']
-    curtains.append(drape.curtain.copy())
-    assert sorted(drape.apertures) == sorted(zip(*np.nonzero(drape.curtain)))
-
-  got = tj.run_trajectory(lambda: aperture.make_game(art), g['actions'][:n].tolist(),
-                          on_frame=on_frame)
-  want = {k: g[k][:n + 1] for k in ('boards', 'reward', 'has_reward', 'discount',
-                                    'game_over')}
-  tj.assert_same_trajectory(want, got, name)
-  np.testing.assert_array_equal(g['sprites'][:n + 1], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'][:n + 1], np.stack(curtains).astype(np.uint8))
 
 
 @pytest.mark.parametrize('which', ['aperture_stock_L1', 'aperture_stock_L2', 'other'])

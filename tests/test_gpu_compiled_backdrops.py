@@ -7,6 +7,7 @@ PCL_PROG_CLASSICS river and the oracle interpreter (oracle/compiled.py)."""
 import numpy as np
 import pytest
 
+import example_games as eg
 import golden_cases as gc
 import registered_games as rg
 import trajectory as tj
@@ -25,28 +26,11 @@ def games():
   yield from rg.registered('backdrop_games.py')
 
 
-def _facade_replay(make, g, keys=()):
-  sprites, curtains, plot = [], [], []
-
-  def on_frame(env, out):
-    s = env.things['P']
-    sprites.append([[s.position[0], s.position[1], int(bool(s.visible)),
-                     s.virtual_position[0], s.virtual_position[1]]])
-    curtains.append(env.backdrop.curtain.copy())
-    plot.append([int(env.the_plot[k]) for k in keys])
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['backdrops'], np.stack(curtains))
-  return plot
-
-
 @pytest.mark.parametrize('name', gc.names('fluvial_'))
 def test_facade_replays_fluvial_golden_with_the_compiled_pair(games, name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
+  art = tj.u8_to_art(gc.load(name)['art'])
   assert lowering.lower(games.make_fluvial(art)).program == _lib.PROG_COMPILED
-  _facade_replay(lambda: games.make_fluvial(art), g)
+  eg.assert_replays('facade', name, make_env=lambda: games.make_fluvial(art))
 
 
 @pytest.mark.parametrize('which', ['stock', 'other'])

@@ -7,10 +7,10 @@ oracle interpreter (oracle/compiled.py)."""
 import numpy as np
 import pytest
 
+import example_games as eg
 import golden_cases as gc
 import registered_games as rg
 import scrolly_shapes
-import trajectory as tj
 from oracle import compiled as ocompiled
 from oracle import sampled_check
 from pycolab_b200 import _lib, levels, lowering
@@ -29,22 +29,11 @@ def _margins(name):
   return scrolly_shapes.DEFAULT_MARGINS
 
 
-def _sprite_rows(env, chars):
-  return [[s.position[0], s.position[1], int(bool(s.visible)),
-           s.virtual_position[0], s.virtual_position[1]]
-          for s in (env.things[ch] for ch in chars)]
-
-
 @pytest.mark.parametrize('name', gc.names('scrolly_'))
 def test_facade_replays_scrolly_golden(games, name):
-  g = gc.load(name)
-  maze, board, beneath = gc.scrolly_art(g)
-  sprites = []
-  got = tj.run_trajectory(
-      lambda: games.make_maze(maze, board, beneath, margins=_margins(name)),
-      g['actions'].tolist(), on_frame=lambda env, out: sprites.append(_sprite_rows(env, 'Pabc')))
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
+  maze, board, beneath = gc.scrolly_art(gc.load(name))
+  eg.assert_replays('facade', name,
+                    make_env=lambda: games.make_maze(maze, board, beneath, margins=_margins(name)))
 
 
 def test_facade_raises_on_postscroll_before_the_move(games):

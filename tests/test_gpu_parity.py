@@ -1,4 +1,5 @@
-"""GPU parity: the CUDA step engine vs the golden fixtures and the oracle.
+"""GPU parity: the CUDA step engine vs the oracle (the facade's golden replays are in
+test_gpu_example_goldens.py).
 
 All of these call through the C ABI (libpcl.so via ctypes).  Bar: bit-exact
 boards (uint8), rewards (incl. None-ness), discounts, game_over and sprite
@@ -9,7 +10,6 @@ import numpy as np
 import pytest
 
 import golden_cases as gc
-import trajectory as tj
 from oracle import engine_model as em
 from oracle import games as ogames
 from oracle import sampled_check
@@ -20,68 +20,6 @@ pytestmark = pytest.mark.gpu
 def _torch():
   import torch
   return torch
-
-
-def _facade_sprites(chars, sink):
-  def on_frame(env, out):
-    rows = []
-    for ch in chars:
-      s = env.things[ch]
-      vp = s.virtual_position
-      rows.append([s.position[0], s.position[1], int(bool(s.visible)), vp[0], vp[1]])
-    sink.append(rows)
-  return on_frame
-
-
-# --------------------------------------------------------------- facade, B=1
-
-@pytest.mark.parametrize('name', gc.names('scrolly_'))
-def test_facade_scrolly_golden(name):
-  from pycolab_b200.games import scrolly_maze
-  g = gc.load(name)
-  maze, board, beneath = gc.scrolly_art(g)
-  sprites = []
-  n = len(g['actions'])            # the whole golden (BASELINE configs[0]: 1000 steps)
-  got = tj.run_trajectory(lambda: scrolly_maze.make_game(maze, board, beneath),
-                          g['actions'][:n].tolist(),
-                          on_frame=_facade_sprites('Pabc', sprites))
-  want = {k: g[k][:n + 1] for k in ('boards', 'reward', 'has_reward', 'discount',
-                                    'game_over')}
-  tj.assert_same_trajectory(want, got, name)
-  np.testing.assert_array_equal(g['sprites'][:n + 1], np.array(sprites))
-
-
-@pytest.mark.parametrize('name', gc.names('warehouse_'))
-def test_facade_warehouse_golden(name):
-  from pycolab_b200.games import warehouse_manager
-  g = gc.load(name)
-  art, wlb = gc.warehouse_art(g)
-  chars = bytes(g['sprite_chars']).decode()
-  sprites = []
-  n = len(g['actions'])
-  got = tj.run_trajectory(lambda: warehouse_manager.make_game(art, wlb),
-                          g['actions'][:n].tolist(),
-                          on_frame=_facade_sprites(chars, sprites))
-  want = {k: g[k][:n + 1] for k in ('boards', 'reward', 'has_reward', 'discount',
-                                    'game_over')}
-  tj.assert_same_trajectory(want, got, name)
-  np.testing.assert_array_equal(g['sprites'][:n + 1], np.array(sprites))
-
-
-@pytest.mark.parametrize('name', gc.names('marauders_'))
-def test_facade_marauders_golden(name):
-  from pycolab_b200.games import extraterrestrial_marauders as marauders
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  np.random.seed(int(g['rng_seed'][0]))     # facade mirrors the global NumPy RNG
-  sprites = []
-  n = len(g['actions'])
-  got = tj.run_trajectory(lambda: marauders.make_game(art), g['actions'][:n].tolist(),
-                          on_frame=_facade_sprites('Pabcdyz', sprites))
-  want = {k: g[k][:n + 1] for k in ('boards', 'reward', 'has_reward', 'discount',
-                                    'game_over')}
-  tj.assert_same_trajectory(want, got, name)
-  np.testing.assert_array_equal(g['sprites'][:n + 1], np.array(sprites))
 
 
 # ------------------------------------------------- batched engine vs oracle
@@ -181,34 +119,6 @@ def test_batched_marauders():
 
 
 # ------------------------------------------------------------------ cropper
-
-@pytest.mark.parametrize('name', gc.names('crop_'))
-def test_crop_golden(name):
-  from pycolab_b200 import cropping
-  from pycolab_b200.games import scrolly_maze
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  maze, board, beneath = gc.scrolly_art(g)
-  crop = cropping.ScrollingCropper(
-      cfg['rows'], cfg['cols'], ['P'], pad_char=cfg['pad'],
-      scroll_margins=tuple(cfg['margins']),
-      initial_offset=None if cfg['offset'] is None else tuple(cfg['offset']),
-      saccade=cfg['saccade'])
-  crops = []
-
-  def make():
-    eng = scrolly_maze.make_game(maze, board, beneath)
-    crop.set_engine(eng)
-    return eng
-
-  n = 150
-  got = tj.run_trajectory(make, g['actions'][:n].tolist(),
-                          on_frame=lambda env, out: crops.append(crop.crop(out[0]).board))
-  want = {k: g[k][:n + 1] for k in ('boards', 'reward', 'has_reward', 'discount',
-                                    'game_over')}
-  tj.assert_same_trajectory(want, got, name)
-  np.testing.assert_array_equal(g['crops'][:n + 1], np.stack(crops))
-
 
 def test_batched_crop_vs_oracle():
   from pycolab_b200 import batched, levels

@@ -1,53 +1,16 @@
 """`storytelling.Story` over device-backed Engines (and device croppers) against
 the golden trajectories the reference's Story produced (SURVEY.md §8f-4)."""
 
-import importlib
-
-import numpy as np
 import pytest
 
-import golden_cases as gc
-import story_cases
-import trajectory as tj
+import example_games as eg
 
 pytestmark = pytest.mark.gpu
 
 
-def _game(kind, art=None):
-  return importlib.import_module('pycolab_b200.games.classics.' + kind).make_game(art)
-
-
-def _run(name, make):
-  g = gc.load(name)
-  chapters = []
-  got = tj.run_trajectory(make, g['actions'].tolist(),
-                          on_frame=lambda env, out: chapters.append(str(env.the_plot.this_chapter)))
-  tj.assert_same_trajectory(g, got, name)
-  assert chapters == g['chapters'].tolist()
-
-
 def test_list_story_of_device_games():
-  from pycolab_b200 import storytelling
-  _run('story_classics_list',
-       lambda: storytelling.Story([lambda k=k, a=a: _game(k, a)
-                                   for k, a in story_cases.LIST_CHAPTERS]))
+  eg.assert_replays('facade', 'story_classics_list')
 
 
 def test_dict_story_with_device_croppers():
-  from pycolab_b200 import cropping, storytelling
-
-  def then(kind, target):
-    def build():
-      game = _game(kind)
-      game.the_plot.next_chapter = target
-      return game
-    return build
-
-  def make():
-    return storytelling.Story(
-        {'rooms': then('four_rooms', 'cliff'), 'cliff': then('cliff_walk', 'chain'),
-         'chain': lambda: _game('chain_walk')},
-        first_chapter='rooms',
-        croppers={'rooms': cropping.FixedCropper((1, 0), 4, 12), 'cliff': None,
-                  'chain': cropping.FixedCropper((0, 0), 4, 12, pad_char='.')})
-  _run('story_classics_cropped', make)
+  eg.assert_replays('facade', 'story_classics_cropped')

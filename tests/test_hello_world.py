@@ -1,62 +1,16 @@
 """examples/hello_world.py (SURVEY.md §8f-4): plain wrapping Sprites + a rolling
-Drape.  Goldens are the reference's own trajectories (tests/golden/hello_stock_*);
-CPU: the oracle; GPU: the facade Engine (B = 1) and a batched lockstep."""
+Drape.  The replays of its goldens (tests/golden/hello_stock_*) are in
+test_example_goldens.py and test_gpu_example_goldens.py; here a batched lockstep and
+lowering."""
 
 import os
 
 import numpy as np
 import pytest
 
-import golden_cases as gc
 import refdriver
-import trajectory as tj
 from oracle import games as ogames
 from oracle import sampled_check
-
-NAMES = gc.names('hello_')
-
-
-def _rows(env, chars='1234'):
-  out = []
-  for ch in chars:
-    s = env.things[ch]
-    out.append([int(s.position[0]), int(s.position[1]), int(bool(s.visible)),
-                int(s.position[0]), int(s.position[1])])
-  return out
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_hello_matches_reference_golden(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    sprites.append(_rows(env))
-    curtains.append(env.things['@'].curtain.copy())
-  got = tj.run_trajectory(lambda: ogames.make_hello(art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'].astype(bool), np.stack(curtains))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES)
-def test_facade_hello_golden(name):
-  from pycolab_b200.games import hello_world
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    sprites.append(_rows(env))
-    curtains.append(env.things['@'].curtain.copy())
-  got = tj.run_trajectory(lambda: hello_world.make_game(art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'].astype(bool), np.stack(curtains))
 
 
 @pytest.mark.gpu

@@ -1,7 +1,8 @@
-"""Pin the oracle against the golden fixtures the real reference produced.
+"""Pin the oracle against the fixture_* goldens the real reference produced (the
+example-game goldens replay in test_example_goldens.py).
 
 CPU-only; runs everywhere (the fixtures travel with the repo, /root/reference
-does not).  Every board, reward, discount, game_over, sprite register and crop
+does not).  Every board, reward, discount, game_over, sprite register and curtain
 must match bit-for-bit.
 """
 
@@ -10,52 +11,7 @@ import pytest
 
 import golden_cases as gc
 import trajectory as tj
-from oracle import engine_model as em
 from oracle import games
-
-
-def _sprite_sink(chars, sink):
-  def on_frame(env, out):
-    sink.append(gc.oracle_sprite_rows(env, chars))
-  return on_frame
-
-
-@pytest.mark.parametrize('name', gc.names('scrolly_'))
-def test_scrolly(name):
-  g = gc.load(name)
-  maze, board, beneath = gc.scrolly_art(g)
-  sprites = []
-  got = tj.run_trajectory(
-      lambda: games.make_scrolly_maze(maze, board, '+', beneath),
-      g['actions'].tolist(), on_frame=_sprite_sink('Pabc', sprites))
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-
-
-@pytest.mark.parametrize('name', gc.names('warehouse_'))
-def test_warehouse(name):
-  g = gc.load(name)
-  art, wlb = gc.warehouse_art(g)
-  chars = bytes(g['sprite_chars']).decode()
-  sprites = []
-  got = tj.run_trajectory(lambda: games.make_warehouse(art, wlb),
-                          g['actions'].tolist(),
-                          on_frame=_sprite_sink(chars, sprites))
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-
-
-@pytest.mark.parametrize('name', gc.names('marauders_'))
-def test_marauders(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  rng = np.random.RandomState(int(g['rng_seed'][0]))
-  sprites = []
-  got = tj.run_trajectory(lambda: games.make_marauders(art, rng),
-                          g['actions'].tolist(),
-                          on_frame=_sprite_sink('Pabcdyz', sprites))
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
 
 
 @pytest.mark.parametrize('name', gc.names('fixture_walkers_'))
@@ -67,7 +23,7 @@ def test_fixture_walkers(name):
   got = tj.run_trajectory(
       lambda: games.make_fixture_world(**kw), g['actions'],
       convert_action=lambda m: {ch: int(v) for ch, v in zip(chars, m)},
-      on_frame=_sprite_sink(chars, sprites))
+      on_frame=lambda env, out: sprites.append(tj.world_sprite_rows(env, chars)))
   tj.assert_same_trajectory(g, got, name)
   np.testing.assert_array_equal(g['sprites'], np.array(sprites))
 
@@ -81,7 +37,7 @@ def test_fixture_scrolly(name):
   for t in range(len(g['actions']) + 1):
     np.testing.assert_array_equal(g['boards'][t], out[0], err_msg='t=%d' % t)
     np.testing.assert_array_equal(g['sprites'][t],
-                                  gc.oracle_sprite_rows(world, 'Pq'))
+                                  tj.world_sprite_rows(world, 'Pq'))
     np.testing.assert_array_equal(
         g['curtains'][t],
         np.stack([world.things['#'].curtain, world.things['@'].curtain]))
@@ -99,52 +55,12 @@ def test_fixture_two_scrolling_groups(name):
   out = world.its_showtime()
   for t in range(len(g['actions']) + 1):
     np.testing.assert_array_equal(g['boards'][t], out[0], err_msg='t=%d' % t)
-    np.testing.assert_array_equal(g['sprites'][t], gc.oracle_sprite_rows(world, 'Pq'))
+    np.testing.assert_array_equal(g['sprites'][t], tj.world_sprite_rows(world, 'Pq'))
     np.testing.assert_array_equal(
         g['curtains'][t],
         np.stack([world.things['#'].curtain, world.things['@'].curtain]))
     if t < len(g['actions']):
       out = world.play({ch: int(g['actions'][t][k]) for ch, k in cfg['motion_of'].items()})
-
-
-def better_croppers(g, world_or_engine, make_scrolling, make_fixed):
-  """The three better_scrolly_maze views (better_scrolly_maze.py:224-251)."""
-  views = [
-      make_scrolling(10, 30, ['P'], initial_offset=tuple(int(x) for x in g['starter_offset'])),
-      make_scrolling(7, 10, ['c'], pad_char=' ', scroll_margins=(None, 3)),
-      make_fixed(tuple(int(x) for x in g['teaser_corner']), 12, 20, ' '),
-  ]
-  return views
-
-
-@pytest.mark.parametrize('name', gc.names('better_'))
-def test_better_scrolly(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, views = [], [[], [], []]
-  crops = better_croppers(
-      g, None,
-      lambda r, c, t, **kw: em.ScrollingCrop(r, c, t, **kw),
-      lambda corner, r, c, pad: ('fixed', corner, r, c, pad))
-
-  def make():
-    w = games.make_better_scrolly(art)
-    for c in crops[:2]:
-      c.set_engine(w)
-    return w
-
-  def on_frame(env, out):
-    sprites.append(gc.oracle_sprite_rows(env, 'Pabc'))
-    views[0].append(crops[0].crop(out[0]))
-    views[1].append(crops[1].crop(out[0]))
-    _, corner, r, c, pad = crops[2]
-    views[2].append(em.crop_window(out[0], corner, r, c, pad))
-
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  for key, v in zip(('view_player', 'view_patroller', 'view_teaser'), views):
-    np.testing.assert_array_equal(g[key], np.stack(v), err_msg=key)
 
 
 def directive_actions(row, order):
@@ -176,82 +92,3 @@ def test_fixture_directives(name):
     assert [chr(c) for c in g['z_orders'][t]] == world.z_order
     if t < len(g['actions']):
       out = world.play(directive_actions(g['actions'][t], order))
-
-
-@pytest.mark.parametrize('name', gc.names('crop_'))
-def test_cropper(name):
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  maze, board, beneath = gc.scrolly_art(g)
-  crop = em.ScrollingCrop(cfg['rows'], cfg['cols'], ['P'], pad_char=cfg['pad'],
-                          scroll_margins=tuple(cfg['margins']),
-                          initial_offset=cfg['offset'], saccade=cfg['saccade'])
-  crops, corners = [], []
-
-  def make():
-    w = games.make_scrolly_maze(maze, board, '+', beneath)
-    crop.set_engine(w)
-    return w
-
-  def on_frame(env, out):
-    crops.append(crop.crop(out[0]))
-    corners.append(list(crop.corner))
-
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['crops'], np.stack(crops))
-  np.testing.assert_array_equal(g['corners'], np.array(corners))
-
-
-def reward_types(sink):
-  def on_frame(env, out):
-    sink.append(0 if out[1] is None else (2 if isinstance(out[1], float) else 1))
-  return on_frame
-
-
-@pytest.mark.parametrize('name', gc.names('classic_'))
-def test_classics(name):
-  g = gc.load(name)
-  kind, art = bytes(g['kind']).decode(), tj.u8_to_art(g['art'])
-  sprites, types = [], []
-
-  def on_frame(env, out):
-    _sprite_sink('P', sprites)(env, out)
-    reward_types(types)(env, out)
-  got = tj.run_trajectory(lambda: games.make_classic(kind, art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['reward_type'], np.array(types, dtype=np.uint8))
-
-
-@pytest.mark.parametrize('name', gc.names('fluvial_'))
-def test_fluvial_natation(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    _sprite_sink('P', sprites)(env, out)
-    curtains.append(env.backdrop.copy())
-  got = tj.run_trajectory(lambda: games.make_fluvial(art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['backdrops'], np.stack(curtains))
-
-
-@pytest.mark.parametrize('name', gc.names('aperture_'))
-def test_aperture(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    _sprite_sink('A', sprites)(env, out)
-    curtains.append(env.things['X'].curtain.copy())
-  got = tj.run_trajectory(lambda: games.make_aperture(art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'], np.stack(curtains).astype(np.uint8))

@@ -310,7 +310,7 @@ def test_ordeal_story_random_walks(seed):
   chapter name, game over), random walks across all three sub-games."""
   refdriver.ref_storytelling()
   from pycolab.examples import ordeal as ref_ordeal
-  from test_ordeal import OracleOrdeal
+  from example_games import OracleOrdeal
   rs = np.random.RandomState(500 + seed)
   story, mine = ref_ordeal.make_game(), OracleOrdeal()
   story.its_showtime()

@@ -1,9 +1,9 @@
 """examples/shockwave.py (SURVEY.md §8f-4): a walker, two static drapes and a ring of
 fire around `np.random.randint` impact points whose update() reads the STALE board.
 Goldens are the reference's own trajectories (tests/golden/shockwave_*: the stock level
-and two generated ones, policy-driven so that some episodes are won); CPU: the oracle;
-GPU: the facade Engine (B = 1, global NumPy generator handed to the device) and a
-batched lock-step with per-env generators."""
+and generated ones, policy-driven so that some episodes are won), replayed in
+test_example_goldens.py and test_gpu_example_goldens.py; here a batched lock-step with
+per-env generators, and lowering."""
 
 import os
 
@@ -12,54 +12,13 @@ import pytest
 
 import golden_cases as gc
 import refdriver
-import trajectory as tj
 from oracle import games as ogames
 from oracle import sampled_check
 
-NAMES = gc.names('shockwave_')
 
-
-def _rows(env):
-  s = env.things['P']
-  vp = getattr(s, 'virtual_position', s.position)
-  return [[int(s.position[0]), int(s.position[1]), int(bool(s.visible)), int(vp[0]), int(vp[1])]]
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_shockwave_matches_reference_golden(name):
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  rng = np.random.RandomState(int(g['numpy_seed'][0]))
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    sprites.append(_rows(env))
-    curtains.append(env.things['@'].curtain.copy())
-  got = tj.run_trajectory(lambda: ogames.make_shockwave(art, rng), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'].astype(bool), np.stack(curtains))
-  assert int((g['reward'] == 1).sum()) >= 1          # the safe-zone path is on the tape
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES)
-def test_facade_shockwave_golden(name):
-  from pycolab_b200.games import shockwave
-  g = gc.load(name)
-  art = tj.u8_to_art(g['art'])
-  sprites, curtains = [], []
-
-  def on_frame(env, out):
-    sprites.append(_rows(env))
-    curtains.append(np.asarray(env.things['@'].curtain).copy())
-  np.random.seed(int(g['numpy_seed'][0]))
-  got = tj.run_trajectory(lambda: shockwave.make_game(art), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['curtains'].astype(bool), np.stack(curtains))
+@pytest.mark.parametrize('name', gc.names('shockwave_'))
+def test_goldens_hold_a_win(name):
+  assert int((gc.load(name)['reward'] == 1).sum()) >= 1          # the safe-zone path
 
 
 @pytest.mark.gpu

@@ -1,89 +1,28 @@
 """`storytelling.Story` (host-side caller of the path) on CPU.
 
-The Story logic is driven here by oracle Worlds dressed as Engines, against the
-golden trajectory the reference's own Story produced for the same chapters
+The Story logic is driven here by oracle Worlds dressed as Engines (OracleEngine),
+against the golden trajectory the reference's own Story produced for the same chapters
 (tests/golden/story_classics_list.npz); plus the constructor's argument checks
 (storytelling.py:493-622).
 """
 
-import importlib
-
 import numpy as np
 import pytest
 
-import golden_cases as gc
+import example_games as eg
 import story_cases
-import trajectory as tj
+from story_cases import OracleEngine, oracle_chapter
 from oracle import games as ogames
-from pycolab_b200 import engine as engine_lib
-from pycolab_b200 import plot as plot_lib
-from pycolab_b200 import rendering
 from pycolab_b200 import storytelling
 from pycolab_b200 import things
 
 
-class _Walker(things.Sprite):
-  def update(self, *args, **kwargs):
-    raise AssertionError('never called')
-
-
-class OracleEngine(object):
-  """An oracle World with the attributes Story reads from an Engine."""
-
-  def __init__(self, world, palette):
-    self._world = world
-    self.the_plot = plot_lib.Plot()
-    self.rows, self.cols = world.rows, world.cols
-    self._palette = palette
-
-  def _obs(self, out):
-    board = np.asarray(out[0], dtype=np.uint8)
-    chars = set(self._palette) | set(self._world.things)
-    return rendering.Observation(board=board, layers=rendering.LazyLayers(board, chars)), out[1], out[2]
-
-  def its_showtime(self):
-    return self._obs(self._world.its_showtime())
-
-  def play(self, actions):
-    return self._obs(self._world.play(actions))
-
-  @property
-  def game_over(self):
-    return self._world.game_over
-
-  @property
-  def z_order(self):
-    return list(self._world.things)
-
-  @property
-  def backdrop(self):
-    return things.Backdrop(curtain=self._world.backdrop, palette=engine_lib.Palette(self._palette))
-
-  @property
-  def things(self):
-    return {ch: _Walker(things.Sprite.Position(self.rows, self.cols),
-                        things.Sprite.Position(w.row, w.col), ch)
-            for ch, w in self._world.things.items()}
-
-
-def _oracle_chapter(kind, art):
-  stock = importlib.import_module('pycolab_b200.games.classics.' + kind).GAME_ART
-  palette = ' #' if kind == 'four_rooms' else '.'
-  return lambda: OracleEngine(ogames.make_classic(kind, art or list(stock)), palette)
-
-
 def test_list_story_matches_reference_golden():
-  g = gc.load('story_classics_list')
-  chapters = []
-  make = lambda: storytelling.Story([_oracle_chapter(k, a) for k, a in story_cases.LIST_CHAPTERS])
-  got = tj.run_trajectory(make, g['actions'].tolist(),
-                          on_frame=lambda env, out: chapters.append(str(env.the_plot.this_chapter)))
-  tj.assert_same_trajectory(g, got, 'story_classics_list')
-  assert chapters == g['chapters'].tolist()
+  eg.assert_replays('oracle', 'story_classics_list')
 
 
 def test_story_views_and_plot_hand_over():
-  story = storytelling.Story([_oracle_chapter(k, a) for k, a in story_cases.LIST_CHAPTERS])
+  story = storytelling.Story([oracle_chapter(k, a) for k, a in story_cases.LIST_CHAPTERS])
   story.its_showtime()
   assert (story.rows, story.cols) == (4, 12)
   assert story.z_order == ['P'] and set(story.backdrop.palette) == {'.'}
@@ -102,7 +41,7 @@ def test_story_views_and_plot_hand_over():
 
 
 def test_story_ends_after_last_chapter_and_refuses_more_play():
-  story = storytelling.Story([_oracle_chapter('chain_walk', None)])
+  story = storytelling.Story([oracle_chapter('chain_walk', None)])
   story.its_showtime()
   for _ in range(2):
     obs, reward, discount = story.play(0)
@@ -114,7 +53,7 @@ def test_story_ends_after_last_chapter_and_refuses_more_play():
 def test_dict_story_follows_next_chapter_and_rejects_unknown_keys():
   def cliff_then(target):
     def build():
-      game = _oracle_chapter('cliff_walk', None)()
+      game = oracle_chapter('cliff_walk', None)()
       game.the_plot.next_chapter = target
       return game
     return build
@@ -129,7 +68,7 @@ def test_dict_story_follows_next_chapter_and_rejects_unknown_keys():
 
 
 def test_constructor_argument_checks():
-  rooms, cliff = _oracle_chapter('four_rooms', None), _oracle_chapter('cliff_walk', None)
+  rooms, cliff = oracle_chapter('four_rooms', None), oracle_chapter('cliff_walk', None)
   with pytest.raises(ValueError):
     storytelling.Story([])
   with pytest.raises(ValueError):

@@ -70,6 +70,48 @@ def run_until_raise(make_env, actions, exception, on_frame=None):
   raise AssertionError('play() never raised %s' % exception.__name__)
 
 
+def reward_type(reward):
+  """A golden's `reward_type`: 0 for no reward, 1 for an int, 2 for a float."""
+  return 0 if reward is None else (2 if isinstance(reward, float) else 1)
+
+
+def sprite_rows(env, chars):
+  """A golden's `sprites` row of an Engine with the pycolab API: (row, col, visible,
+  virtual row, virtual col) of each sprite of `chars`.  A plain Sprite has no virtual
+  position: its position stands in."""
+  rows = []
+  for s in (env.things[ch] for ch in chars):
+    vp = getattr(s, 'virtual_position', s.position)
+    rows.append([int(s.position[0]), int(s.position[1]), int(bool(s.visible)),
+                 int(vp[0]), int(vp[1])])
+  return rows
+
+
+def world_sprite_rows(world, chars, plain=''):
+  """sprite_rows() of an oracle world.  A plain sprite (oracle.games.PlainSprite) has no
+  vrow and vcol, and a compiled plain Sprite, one of `plain`, holds registers there: the
+  position stands in for both."""
+  rows = []
+  for ch in chars:
+    w = world.things[ch]
+    v = (w.row, w.col) if ch in plain or not hasattr(w, 'vrow') else (w.vrow, w.vcol)
+    rows.append([w.row, w.col, int(bool(w.visible)), v[0], v[1]])
+  return rows
+
+
+def assert_golden_arrays(name, g, got, inputs):
+  """Every array golden `name`'s `g` holds apart from its `inputs` equals `got`'s, dtype
+  and shape included, floats bit for bit.  A key `got` lacks fails, and is named."""
+  keys = sorted(set(g) - set(inputs))
+  missing = [key for key in keys if key not in got]
+  assert not missing, '%s: the replay recorded no %s' % (name, ', '.join(missing))
+  for key in keys:
+    msg = '%s: %s' % (name, key)
+    np.testing.assert_array_equal(got[key], g[key], err_msg=msg, strict=True)
+    if g[key].dtype.kind == 'f':
+      assert got[key].tobytes() == g[key].tobytes(), msg + ': float bits differ'
+
+
 def art_to_u8(art):
   return np.vstack([np.frombuffer(l.encode('ascii'), dtype=np.uint8) for l in art])
 
