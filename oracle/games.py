@@ -188,8 +188,9 @@ def warehouse_program(world, ch, actions):
   else:                                           # BoxSprite.update :208-226
     r, c = ent.position
     is_p = lambda rr, cc: board[rr, cc] == ord('P')   # layers['P'][rr, cc]
-    # NumPy index semantics: -1 wraps, >= size raises (the stock and generated
-    # levels keep boxes away from the rim, so only the wrap can occur).
+    # NumPy index semantics: -1 wraps, >= size raises.  Boxes are unconfined, so
+    # one pushed off the board sits at position (0, 0) (and is marked there by the
+    # judge), and every box at (0, 0) moves together when P stands next to it.
     if actions == 0:
       if is_p(r + 1, c): em.walker_move(ent, board, plot, em.M_N)
     elif actions == 1:

@@ -50,7 +50,7 @@ def sprite_words(walker):
 
 
 def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprites='',
-             pad_columns=False, on_step=None):
+             pad_columns=False, on_step=None, raised=None):
   """Step `engine` (a BatchedEngine after its_showtime(), B envs) with
   actions int32 [T, B] and, for every env in `env_ids`, an oracle world built by
   make_world(env) in lockstep.  Returns the number of (env, step) pairs compared,
@@ -64,7 +64,12 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       oracle walker.
     pad_columns: the board's pitch padding stays 0.
     on_step(t, engine, worlds, outs): called after the comparison of step t (0 is
-      its_showtime()), with the oracle worlds and their outputs keyed by env."""
+      its_showtime()), with the oracle worlds and their outputs keyed by env.
+    raised: a dict, to compare the latched error words too.  Each env's word
+      (engine.error_codes()) stays 0 while its oracle world raises nothing.  A world
+      whose play() raises IndexError (a NumPy look-up off the board) at step t must find
+      exactly ENV_ERR_INDEX latched after step t; lockstep then sets raised[env] = t and
+      compares that env no further, as the reference's Engine would play no further."""
   import torch
   env_ids = [int(e) for e in env_ids]
   idx = torch.as_tensor(env_ids, dtype=torch.long, device=engine.device)
@@ -84,6 +89,16 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
     return x.index_select(0, idx).cpu().numpy()
 
   def check(t):
+    if raised is not None:
+      from pycolab_b200 import _lib
+      codes = pick(engine.error_codes())
+      for k, e in enumerate(env_ids):
+        if e in raised and raised[e] < t:
+          continue
+        want = _lib.ENV_ERR_INDEX if e in raised else 0
+        if int(codes[k]) != want:
+          raise Mismatch('error word at step %d env %d: device %#x oracle %#x' % (
+              t, e, int(codes[k]), want))
     boards, reward, has = pick(engine.board), pick(engine.reward), pick(engine.has_reward)
     disc, done = pick(engine.discount), pick(engine.done)
     views = None
@@ -94,6 +109,8 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
     records = pick(engine.sprites) if sprites else None
     pad = pick(engine._board)[:, :, engine.cols:] if pad_columns else None
     for k, e in enumerate(env_ids):
+      if raised is not None and e in raised:
+        continue
       world = worlds[e]
       _compare(t, e, (boards[k], reward[k], has[k], disc[k], done[k]), outs[e], world)
       if views is not None and not np.array_equal(views[k], croppers[e].crop(outs[e][0])):
@@ -110,19 +127,26 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
         raise Mismatch('pad columns differ from 0 at step %d env %d' % (t, e))
     if on_step is not None:
       on_step(t, engine, worlds, outs)
-    return len(env_ids)
+    return len(env_ids) - (len(raised) if raised is not None else 0)
 
   compared = check(0)
   for t in range(T):
     engine.play(acts_dev[t])
     for e in env_ids:
+      if raised is not None and e in raised:
+        continue
       if worlds[e].game_over:                 # the auto-reset rule
         worlds[e] = make_world(e)
         if croppers is not None:
           croppers[e].set_engine(worlds[e])
         outs[e] = worlds[e].its_showtime()
-      else:
+      elif raised is None:
         outs[e] = worlds[e].play(int(actions[t, e]))
+      else:
+        try:
+          outs[e] = worlds[e].play(int(actions[t, e]))
+        except IndexError:
+          raised[e] = t + 1
     compared += check(t + 1)
   return compared
 

@@ -109,14 +109,20 @@ warehouse_step(const StepParams p) {
   int b_row = mine[PCL_S_ROW], b_col = mine[PCL_S_COL];
 
   // Character of the stale board (= previous final render) at (r, c): P on top,
-  // then a box (drawn 'X' when the judge marked it), else the backdrop.
+  // then 'X' where the judge marked a box, else the last visible box there, else
+  // the backdrop.  A box off the board sits at (0, 0) and the judge marks it there
+  // too, but only a visible box paints its own character.  The judge's mark is a
+  // property of the cell, so every box at (r, c) carries the same AUX0.
   // Box positions are still the old ones in `rec` while this is used.
   auto stale_cell = [&](int r, int c) -> int {
     if (pl_vis && r == pl_row && c == pl_col) return P_CHAR;
     int code = s_bd[r * pitch + c];
     for (int i = 0; i < NB; ++i) {
       const int32_t* b = rec + i * PCL_SPRITE_WORDS;
-      if (b[PCL_S_ROW] == r && b[PCL_S_COL] == c) code = b[PCL_S_AUX0] ? 'X' : s_chars[i];
+      if (b[PCL_S_ROW] == r && b[PCL_S_COL] == c) {
+        if (b[PCL_S_AUX0]) code = 'X';
+        else if (b[PCL_S_FLAGS] & 1) code = s_chars[i];
+      }
     }
     return code;
   };
@@ -133,8 +139,12 @@ warehouse_step(const StepParams p) {
     const bool pushed = is_box && !oob && pl_vis && rr == pl_row && cc == pl_col;
     if (__any_sync(PCL_FULL, oob)) plot.error |= PCL_ENV_ERR_INDEX;
     const unsigned who = __ballot_sync(PCL_FULL, pushed);
-    if (who) {                               // at most one box can be next to P
-      const int j = __ffs(who) - 1;
+    // One box on the board can be next to P, but every box off the board sits at
+    // (0, 0), so several can be pushed at once.  Each moves against the stale board:
+    // its lane keeps the new record in registers until all of them have moved.
+    Sprite moved = {};
+    for (unsigned left = who; left; left &= left - 1) {
+      const int j = __ffs(left) - 1;
       Sprite box = load_sprite(rec + j * PCL_SPRITE_WORDS);
       uint32_t imp[4];
 #pragma unroll
@@ -147,24 +157,35 @@ warehouse_step(const StepParams p) {
         }
       walker_move(box, j, motion_of_action(action), plot, H, W, false, false, lane,
                   [&](int r2, int c2) { return in_set(imp, stale_cell(r2, c2)); });
+      if (lane == j) moved = box;
+    }
+    if (who) {
       __syncwarp();
-      if (lane == 0) store_sprite(rec + j * PCL_SPRITE_WORDS, box, PCL_S_AUX0);
+      if (pushed) {
+        store_sprite(rec + lane * PCL_SPRITE_WORDS, moved, PCL_S_AUX0);
+        b_row = moved.row; b_col = moved.col;
+      }
       __syncwarp();
-      if (lane == j) { b_row = box.row; b_col = box.col; }
     }
   }
 
-  // ---- group 1: JudgeDrape.update (:245-266), one lane per box
-  bool first = is_box, goal = false;
+  // ---- group 1: JudgeDrape.update (:245-266), one lane per box.  The curtain counts a
+  // cell once: the last box in it counts.  Boxes share a cell while off the board (at
+  // (0, 0)), or after two of them came back onto it from one virtual cell; `covered`:
+  // a later box (higher in z-order) is visible in this box's cell.
+  bool last = is_box, covered = false, goal = false;
   if (is_box) {
-    for (int i = 0; i < lane; ++i) {
+    for (int i = lane + 1; i < NB; ++i) {
       const int32_t* b = rec + i * PCL_SPRITE_WORDS;
-      if (b[PCL_S_ROW] == b_row && b[PCL_S_COL] == b_col) first = false;
+      if (b[PCL_S_ROW] == b_row && b[PCL_S_COL] == b_col) {
+        last = false;
+        covered |= b[PCL_S_FLAGS] & 1;
+      }
     }
     goal = s_bd[b_row * pitch + b_col] == '_';
   }
-  const int num_boxes = __popc(__ballot_sync(PCL_FULL, first));
-  const int on_goals = __popc(__ballot_sync(PCL_FULL, first && goal));
+  const int num_boxes = __popc(__ballot_sync(PCL_FULL, last));
+  const int on_goals = __popc(__ballot_sync(PCL_FULL, last && goal));
   if (is_box) rec[lane * PCL_SPRITE_WORDS + PCL_S_AUX0] = goal ? 1 : 0;
   add_reward(dir, on_goals - r_judge[PCL_D_AUX0]);
   if (action == 5 || on_goals == num_boxes) terminate(dir);
@@ -199,9 +220,10 @@ warehouse_step(const StepParams p) {
   if (lane >= 16) g_plot[lane - 16] = r_plot[lane - 16];
 
   // ---- final render: patch the sprite cells into the staged tile, stream it out.
-  // Boxes never share a cell with each other or with P (each is impassable to
-  // the others), so the patches are independent; P goes last to keep z-order.
-  if (is_box && (mine[PCL_S_FLAGS] & 1))
+  // The judge marks every box's position, (0, 0) for a box off the board, so a
+  // marked box paints 'X' whether it is visible or not.  An unmarked box paints
+  // its own character if it is visible and not covered.  P goes last, on top.
+  if (is_box && (goal || ((mine[PCL_S_FLAGS] & 1) && !covered)))
     s_bd[b_row * pitch + b_col] = goal ? 'X' : s_chars[lane];
   __syncwarp();
   if (lane == 0 && visible(player)) s_bd[player.row * pitch + player.col] = (uint8_t)P_CHAR;
@@ -215,9 +237,21 @@ warehouse_step(const StepParams p) {
   }
 }
 
+// Dynamic shared memory of one block (kWarpsPerBlock envs): each warp stages its
+// records and its whole backdrop tile.
+size_t block_smem(int H, int pitch) {
+  return (kRecWords * 4 + (size_t)H * pitch) * kWarpsPerBlock;
+}
+
+// The most dynamic shared memory a block may ask for on the H100 (227 KB; the kernel
+// has no static shared memory).  check_spec accepts a spec only if its block fits,
+// so an accepted spec always launches.
+constexpr size_t kMaxBlockSmem = 227 * 1024;
+
 int check_spec(const pcl_spec& s) {
   const int nb = s.n_sprites - 1;
   if (nb < 1 || nb > 10) return PCL_ERR_UNSUPPORTED;
+  if (block_smem(s.rows, s.pitch) > kMaxBlockSmem) return PCL_ERR_UNSUPPORTED;
   if (s.sprite_char[nb] != 'P') return PCL_ERR_UNSUPPORTED;
   if (!chars_are(s.drape_char, s.n_drapes, "X")) return PCL_ERR_UNSUPPORTED;
   const char* order = "1234567890";
@@ -239,8 +273,7 @@ int check_spec(const pcl_spec& s) {
 }
 
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
-  const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch) * kWarpsPerBlock;
-  return launch_step(warehouse_step, p, kWarpsPerBlock, smem, s);
+  return launch_step(warehouse_step, p, kWarpsPerBlock, block_smem(p.H, p.pitch), s);
 }
 
 }  // namespace

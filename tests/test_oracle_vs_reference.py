@@ -24,13 +24,16 @@ pytestmark = pytest.mark.skipif(not refdriver.available(),
                                 reason='/root/reference not present')
 
 
-def _lockstep(make_ref, make_oracle, actions, check_sprites=True):
-  """Step both with auto-reset on game over; compare everything each frame."""
+def _lockstep(make_ref, make_oracle, actions, check_sprites=True, check=None):
+  """Step both with auto-reset on game over; compare everything each frame, and call
+  check(ref, ora, t) after each comparison."""
   ref, ora = make_ref(), make_oracle()
   r_out, o_out = ref.its_showtime(), ora.its_showtime()
   episodes = 0
   for t, a in enumerate(actions):
     _compare(ref, ora, r_out, o_out, t, check_sprites)
+    if check is not None:
+      check(ref, ora, t)
     if ref.game_over:
       episodes += 1
       ref, ora = make_ref(), make_oracle()

@@ -13,7 +13,11 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden',
                       'boundary_statuses.json')
 
 
-def test_every_lowered_level_keeps_its_boundary_statuses():
+def test_boundary_statuses_of_every_lowered_level():
+  """The statuses of the golden file, case for case.  Among them, warehouse refuses a
+  board whose block of four staged backdrop tiles would exceed the 227 KB of shared
+  memory a block can opt in to (rows or pitch 32768 on the 80-column level): such a spec
+  could never launch."""
   with open(GOLDEN) as f:
     encoded = json.load(f)
   got = boundary_sweep.sweep()
@@ -26,6 +30,8 @@ def test_every_lowered_level_keeps_its_boundary_statuses():
                                                           '; '.join(differ[:10]))
   for level in encoded:
     assert want[level + '/create'] == want[level + '/bind'] == _lib.OK, level
+  for case in ('warehouse/spec.rows=32768', 'warehouse/spec.pitch=32768'):
+    assert want[case] == got[case] == _lib.ERR_UNSUPPORTED, case
   programs = set(spec.program for _, spec in boundary_sweep.lowered_specs())
   assert programs == set(range(1, 13))
 
