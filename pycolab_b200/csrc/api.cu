@@ -3,6 +3,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <mutex>
 #include <new>
 
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: ranges show up in nsys / ncu timelines
@@ -20,6 +21,7 @@ struct pcl_handle {
   int actions_per_env;
   pcl_state st;
   long long launches;
+  long long chained_launches;    // of those, step launches with StepParams::chain CHAIN_FOLLOWS
   pcl::StepParams base;          // everything fill_params derives from spec + state, built once at bind
   char last_error[256];          // text of the last failed CUDA call (pcl_last_error)
   // pcl_step_host_async: a copy stream so that the D2H of one step overlaps the next kernel
@@ -159,16 +161,137 @@ bool live_backdrop(const pcl_spec& s) {
   return s.program == PCL_PROG_COMPILED && s.program_arg[4] != 0;
 }
 
-int launch(pcl_handle* h, StepParams p, cudaStream_t stream) {
+// ---- Block chaining (StepParams::chain; scrolly_maze.cu, "Block chaining") -------------
+// A step of a Program::block_chaining program may skip the wait for the whole previous
+// grid (CHAIN_FOLLOWS) when the stream's previous kernel is a step launch of this library
+// that kept the per-block counters (HEAD or FOLLOWS) and cannot have written anything the
+// step reads, nor read anything it writes, but its own envs' state: a launch of the same
+// handle, or of another handle whose per-env memory (its footprint) is disjoint from this
+// one's.  The previous kernel is known in two cases: between the launches of one pcl_run
+// or pcl_run_many call, and under stream capture when the stream's only dependency is the
+// node of the last such launch captured on it.  A step launch after any other step launch
+// keeps the full wait but the counters too (CHAIN_HEAD), so that the next may chain to it.
+// Every other launch (eager pcl_step and pcl_reset, a step after another kernel, the first
+// of a run) is CHAIN_NONE: the kernel as it ran before chaining, at no extra cost.
+
+// The per-env memory one step launch touches: [lo, hi) byte ranges, and which it writes.
+struct Footprint {
+  const pcl_handle* h;           // nullptr: no step launch to chain to
+  bool counted;                  // the launch kept the per-block counters (HEAD, FOLLOWS)
+  int n;
+  struct { uintptr_t lo, hi; bool written; } span[16 + PCL_MAX_DRAPES];
+};
+
+Footprint footprint(const pcl_handle* h, const StepParams& p) {
+  Footprint f;
+  f.h = h;
+  f.counted = false;
+  f.n = 0;
+  const size_t B = (size_t)h->batch;
+  auto add = [&f](const void* ptr, size_t bytes, bool written) {
+    if (ptr && bytes) f.span[f.n++] = {(uintptr_t)ptr, (uintptr_t)ptr + bytes, written};
+  };
+  const pcl_spec& s = h->spec;
+  add(p.st.d_sprites, B * s.n_sprites * PCL_SPRITE_WORDS * 4, true);
+  add(p.st.d_drapes, B * s.n_drapes * PCL_DRAPE_WORDS * 4, true);
+  add(p.st.d_plot, B * PCL_PLOT_WORDS * 4, true);
+  for (int d = 0; d < s.n_drapes; ++d)      // a pattern with a reset template is per env
+    if (p.st.d_pattern_init[d]) add(p.st.d_pattern[d], B * p.st.pattern_bstride[d] * 4, true);
+  add(p.out.d_board, B * s.rows * s.pitch, true);
+  add(p.out.d_reward, B * 4, true);
+  add(p.out.d_has_reward, B, true);
+  add(p.out.d_discount, B * 4, true);
+  add(p.out.d_done, B, true);
+  add(p.out.d_reward_f64, B * 8, true);
+  if (p.has_cropper) {
+    add(p.cropper.out, B * p.cropper.crop.rows * p.cropper.crop.cols, true);
+    add(p.cropper.state, B * 4 * 4, true);
+  }
+  add(p.mode == pcl::MODE_STEP ? p.actions : nullptr, B * h->actions_per_env * 4, false);
+  add(p.mode == pcl::MODE_RESET ? p.env_mask : nullptr, B, false);
+  return f;
+}
+
+// May a launch with footprint `b` follow the launch with footprint `a` without waiting for
+// all of it?
+bool chainable(const Footprint& a, const Footprint& b) {
+  if (!a.h || !a.counted) return false;
+  if (a.h == b.h) return true;
+  for (int i = 0; i < a.n; ++i)
+    for (int j = 0; j < b.n; ++j)
+      if ((a.span[i].written || b.span[j].written) && a.span[i].lo < b.span[j].hi &&
+          b.span[j].lo < a.span[i].hi) return false;
+  return true;
+}
+
+// The last block-chaining step launch captured on each of a few streams.
+struct CapturedStep {
+  cudaStream_t stream;
+  unsigned long long capture;
+  cudaGraphNode_t node;
+  Footprint f;
+};
+std::mutex g_captured_mu;
+CapturedStep g_captured[8];
+int g_captured_next;
+
+// The footprint of the last step launch captured on `s`, if it is `dep` of capture
+// `capture`; else one with h == nullptr.
+Footprint captured_step(cudaStream_t s, unsigned long long capture, cudaGraphNode_t dep) {
+  std::lock_guard<std::mutex> lock(g_captured_mu);
+  for (const CapturedStep& c : g_captured)
+    if (c.node == dep && c.stream == s && c.capture == capture) return c.f;
+  Footprint none;
+  none.h = nullptr;
+  return none;
+}
+
+// A step launch.  `run`: the footprint of the previous launch of the same pcl_run /
+// pcl_run_many call (h == nullptr before its first), updated to this launch's.
+int launch(pcl_handle* h, StepParams p, cudaStream_t stream, Footprint* run = nullptr) {
   if (!h->program->launch) return PCL_ERR_UNSUPPORTED;
   if (p.out.d_board != h->last_board) {
     h->last_board = p.out.d_board;
     h->board_epoch += 1;
   }
   p.board_epoch = h->board_epoch;
+  Footprint f;
+  f.h = nullptr;
+  bool captured = false;
+  if (h->program->block_chaining) {
+    f = footprint(h, p);
+    cudaStreamCaptureStatus status;
+    unsigned long long capture = 0;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t n = 0;
+    PCL_CUDA(h, cudaStreamGetCaptureInfo(stream, &status, &capture, nullptr, &deps, &n));
+    captured = status == cudaStreamCaptureStatusActive;
+    Footprint prev;
+    prev.h = nullptr;
+    if (run) prev = *run;
+    else if (captured && n == 1) prev = captured_step(stream, capture, deps[0]);
+    p.chain = chainable(prev, f) ? pcl::CHAIN_FOLLOWS : prev.h ? pcl::CHAIN_HEAD : pcl::CHAIN_NONE;
+    f.counted = p.chain != pcl::CHAIN_NONE;
+  }
   const cudaError_t e = h->program->launch(p, stream);
   if (e != cudaSuccess) return cuda_failed(h, e, "step kernel launch");
   h->launches += 1;              // only launches that were accepted count
+  if (p.chain == pcl::CHAIN_FOLLOWS) h->chained_launches += 1;
+  if (run) *run = f;
+  if (captured) {                // the node just captured is now the stream's dependency
+    cudaStreamCaptureStatus status;
+    unsigned long long capture = 0;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t n = 0;
+    PCL_CUDA(h, cudaStreamGetCaptureInfo(stream, &status, &capture, nullptr, &deps, &n));
+    if (status == cudaStreamCaptureStatusActive && n == 1) {
+      std::lock_guard<std::mutex> lock(g_captured_mu);
+      int slot = -1;
+      for (int i = 0; i < 8 && slot < 0; ++i) if (g_captured[i].stream == stream) slot = i;
+      if (slot < 0) slot = g_captured_next++ & 7;
+      g_captured[slot] = {stream, capture, deps[0], f};
+    }
+  }
   return PCL_OK;
 }
 
@@ -289,6 +412,7 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->bound = 0;
   h->actions_per_env = h->program->actions_per_env ? h->program->actions_per_env(*spec) : 1;
   h->launches = 0;
+  h->chained_launches = 0;
   h->last_error[0] = 0;
   h->host_ready = 0;
   h->pending_slot = -1;
@@ -398,9 +522,11 @@ int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_output
   StepParams p = h->base;
   p.mode = pcl::MODE_STEP;
   p.out = *out;
+  Footprint run;
+  run.h = nullptr;
   for (int t = 0; t < steps; ++t) {
     p.actions = d_actions + (int64_t)t * h->batch * h->actions_per_env;
-    const int e = launch(h, p, (cudaStream_t)stream);
+    const int e = launch(h, p, (cudaStream_t)stream, &run);
     if (e != PCL_OK) return e;
   }
   return PCL_OK;
@@ -414,6 +540,8 @@ int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const
     const int r = check_ready(handles[i], outs[i], (cudaStream_t)stream);
     if (r != PCL_OK) return r;
   }
+  Footprint run;
+  run.h = nullptr;
   for (int t = 0; t < steps; ++t) {
     if (!d_actions[t]) return PCL_ERR_INVALID;
     pcl_handle* h = handles[t % n_handles];
@@ -421,7 +549,7 @@ int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const
     p.mode = pcl::MODE_STEP;
     p.out = *outs[t % n_handles];
     p.actions = d_actions[t];
-    const int e = launch(h, p, (cudaStream_t)stream);
+    const int e = launch(h, p, (cudaStream_t)stream, &run);
     if (e != PCL_OK) return e;
   }
   return PCL_OK;
@@ -816,6 +944,15 @@ int pcl_error_codes(pcl_handle* h, int32_t* d_out, void* stream) {
 int pcl_launch_count(pcl_handle* h, int64_t* out) {
   if (!h || !out) return PCL_ERR_INVALID;
   *out = h->launches;
+  return PCL_OK;
+}
+
+// The handle's step launches enqueued or captured as chained (StepParams::chain
+// CHAIN_FOLLOWS), so that tests can tell which launches skipped the full wait.  Not part
+// of include/pcl.h.
+int pcl_chained_launch_count(pcl_handle* h, int64_t* out) {
+  if (!h || !out) return PCL_ERR_INVALID;
+  *out = h->chained_launches;
   return PCL_OK;
 }
 

@@ -64,7 +64,20 @@ struct StepParams {
   // The handle's count of board-buffer changes: a launch whose out.d_board differs from
   // the previous launch's gets the next value, so each value names one buffer.
   uint32_t board_epoch;
+  // Program::block_chaining: u32 [blocks, 2] per block of the handle's launches, the
+  // launches whose block has begun and those whose block has ended (in the derived
+  // allocation, so every pcl_bind_state starts them at zero).
+  uint32_t* block_sync;
+  // Program::block_chaining: how this launch waits for the kernels before it (CHAIN_*).
+  int chain;
 };
+
+// StepParams::chain (launch, api.cu; scrolly_maze.cu, "Block chaining").  CHAIN_NONE: the
+// full wait, the kernel as before chaining.  CHAIN_HEAD: the full wait, and the per-block
+// counters kept, so that the next step launch may chain to this one.  CHAIN_FOLLOWS: the
+// stream's previous kernel is a HEAD or FOLLOWS step launch whose per-env memory is this
+// handle's own or disjoint from it, so each block waits only for its own envs' last step.
+enum { CHAIN_NONE = 0, CHAIN_HEAD = 1, CHAIN_FOLLOWS = 2 };
 
 // Launch with the programmatic-stream-serialisation attribute (the kernel calls
 // griddepcontrol.wait before its first global access).
@@ -120,6 +133,10 @@ struct Program {
   // allocation returned in *owned (the handle frees it when it rebuilds and at
   // pcl_destroy).  May synchronise the device.  nullptr: the program derives nothing.
   int (*derive)(const pcl_spec&, const pcl_state&, int batch, StepParams* base, void** owned);
+  // The step kernel honours StepParams::chain with the per-block counters its
+  // derive() builds in StepParams::block_sync, and touches per env only the arrays
+  // footprint() (api.cu) lists.
+  bool block_chaining;
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
     kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld,

@@ -222,6 +222,56 @@ __device__ __forceinline__ void pdl_wait_prior_grids() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
+// ---- Block chaining (StepParams::chain, block_sync) ------------------------------------
+// Step t + 1 of an env reads only what step t of the same env wrote, static level data and
+// inputs written before the chain of step launches began.  So when the stream's previous
+// kernel is a step launch of this library that shares no per-env memory with this one
+// (CHAIN_FOLLOWS, set by api.cu), a block need not wait in griddepcontrol.wait for every
+// block of the previous grid to finish and flush: block b waits only for block b of its own
+// handle's previous launch.  Freed SM slots then take the next launch's blocks at once, and
+// the wave's slowest warps no longer hold every SM idle.  Two counters per block, begin[b]
+// and end[b]: the handle's launches whose block b has begun, and those whose block b ended.
+//   CHAIN_FOLLOWS  entry: thread 0 takes begun = begin[b]++ with an atomic, waits until
+//                  end[b] == begun (block b of every earlier launch of the handle that
+//                  counts is done) and acquires what those blocks wrote; the block barrier
+//                  passes that on to every warp.  Only then does the block call
+//                  launch_dependents.
+//   CHAIN_HEAD     the full wait, and the counters kept as above: a step launch whose
+//                  predecessor is a step launch it may not chain to (the first of a run, or
+//                  a batch sharing memory with the one before).  Thread 0's atomic is issued
+//                  before the wait and overlaps it; the block calls launch_dependents after
+//                  the wait, so a chained successor starts only once every kernel before
+//                  this one has completed.
+//   CHAIN_NONE     the kernel as before chaining (launch_dependents at entry, the full
+//                  wait), counters untouched: every other launch, such as eager pcl_step or
+//                  a step after another kernel.  api.cu never chains a launch to it: the
+//                  next step launch is then CHAIN_HEAD at most.
+//   exit (HEAD, FOLLOWS): after a block barrier (every warp has left the step: frozen,
+//                  ragged-block and early-return warps too), thread 0 stores end[b] =
+//                  begun + 1 with st.release.gpu.
+// No deadlock: a chained launch may start only once every block of the previous one has
+// called launch_dependents, so once each of them is resident and past its own wait; by
+// induction the same holds back to the CHAIN_HEAD launch that began the chain, whose wait
+// saw every kernel before it complete.  A spinning block
+// therefore waits on blocks that are resident and need nothing more to finish, and never
+// holds a slot one of them still needs.  The full griddepcontrol.wait waits for every
+// prerequisite grid in flight, chained ones included, so a launch after a chain needs
+// nothing more.  Inputs another kernel wrote before the chain (actions, the reset mask) are
+// read from L2 (ld.global.cg), never from a line an SM's L1 kept from before.
+__device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
+}
+
 // Selector table of the paint loop (see the kernel): 256 x u16, built at compile
 // time and pulled into shared memory with one cp.async per lane by each warp that paints.
 struct SelTable { uint16_t v[256]; };
@@ -392,11 +442,10 @@ __device__ __forceinline__ int32_t key_word(const int32_t* rec, int i, uint32_t 
   return i < kKeyRecWords ? r : i == kKeyEpoch ? (int32_t)epoch : cell;
 }
 
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
-scrolly_maze_step(const StepParams p) {
+// One warp's env of one step; scrolly_maze_step runs it between the block's entry and exit
+// of "Block chaining".  Every return leaves the step for that warp only.
+__device__ __forceinline__ void step_env(const StepParams& p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  PCL_STAMP(kStEntry);
-  PCL_STAMP_TIME(kStTimeIn);
   // Byte-permute selectors for 4 cells at once: index = wall nibble << 4 | coin
   // nibble; selector nibble k picks byte 5 ('#') if wall_k, else byte 4 ('@') if
   // coin_k, else byte k of the backdrop word (z-order ... '@' '#' ...).
@@ -407,7 +456,6 @@ scrolly_maze_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   uint16_t* s_sel = s_sel_all[warp];
-  pdl_launch_dependents();
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   const bool live = env < p.B;
   const int H = p.H, W = p.W, PWW = p.PWW;
@@ -419,10 +467,6 @@ scrolly_maze_step(const StepParams p) {
   uint8_t* s_bd = my + kRecWords * 4;
   uint32_t* s_wall = reinterpret_cast<uint32_t*>(s_bd + (size_t)H * pitch);
   uint32_t* s_coin = s_wall + ((H * nw + 3) & ~3);
-  // Everything above ran without touching state earlier kernels may have
-  // produced; from here on the kernel reads such state.
-  pdl_wait_prior_grids();
-  PCL_STAMP(kStPrior);
   // An attached cropper reads its corner state at the very end: start that line's trip
   // from DRAM now (a hint, no register held).
   if (p.has_cropper && p.cropper.state && live && lane == 0)
@@ -433,7 +477,8 @@ scrolly_maze_step(const StepParams p) {
   // The env's action word does not depend on the records either: issue its load now,
   // beside theirs, instead of one memory round trip later (it is only USED if the env
   // neither restarts nor is frozen).
-  int action = env_action(p, env);
+  int action = p.mode == MODE_STEP ? __ldcg(p.actions + (int64_t)env * p.actions_per_env)
+                                   : PCL_ACTION_NONE;
   // The render key, in the same trip as the records.
   const int32_t key = lane < kKeyWords ? p.render_key[(int64_t)env * kKeyStride + lane] : 0;
   // ---- 1. records -> smem (coalesced) ------------------------------------
@@ -448,7 +493,7 @@ scrolly_maze_step(const StepParams p) {
   bool restart;
   bool frozen = false;
   if (p.mode == MODE_RESET) {
-    restart = (p.env_mask == nullptr) || (p.env_mask[env] != 0);
+    restart = (p.env_mask == nullptr) || (__ldcg(p.env_mask + env) != 0);
     frozen = !restart;
   } else {
     restart = was_over && p.auto_reset;
@@ -992,6 +1037,37 @@ scrolly_maze_step(const StepParams p) {
   PCL_STAMP_TIME(kStTimeOut);
 }
 
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, 8)
+scrolly_maze_step(const StepParams p) {
+  PCL_STAMP(kStEntry);
+  PCL_STAMP_TIME(kStTimeIn);
+  // Entry of "Block chaining": nothing before it reads state earlier kernels may produce.
+  // begin[b], end[b] at block_sync[2 b], [2 b + 1]
+  __shared__ uint32_t s_begun;
+  if (p.chain == CHAIN_NONE) {
+    pdl_launch_dependents();
+    pdl_wait_prior_grids();
+    PCL_STAMP(kStPrior);
+    step_env(p);
+    return;
+  }
+  uint32_t* const sync = p.block_sync + 2 * blockIdx.x;
+  if (threadIdx.x == 0) s_begun = atomicAdd(sync, 1u);
+  if (p.chain == CHAIN_HEAD) {
+    pdl_wait_prior_grids();
+  } else if (threadIdx.x == 0) {
+    while (ld_relaxed_gpu(sync + 1) != s_begun) __nanosleep(64);
+    ld_acquire_gpu(sync + 1);              // reads that same count: what those blocks wrote
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  PCL_STAMP(kStPrior);
+  step_env(p);
+  __syncthreads();
+  // end[b] == begun before this launch (the full wait, or the spin): now one more.
+  if (threadIdx.x == 0) st_release_gpu(p.block_sync + 2 * blockIdx.x + 1, s_begun + 1u);
+}
+
 // Dynamic shared memory of one block (kWarpsPerBlock envs).
 size_t block_smem(int H, int W, int pitch) {
   return warp_smem_bytes(H, W, pitch) * kWarpsPerBlock;
@@ -1119,8 +1195,10 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
   const int64_t off_coin = (n_wall * blk_words * 4 + 255) & ~(int64_t)255;
   const int64_t off_nbh = (off_coin + n_coin * blk_words * 4 + 255) & ~(int64_t)255;
   const int64_t off_key = (off_nbh + n_wall * nbh_words * 4 + 255) & ~(int64_t)255;
+  const int64_t off_sync = (off_key + (int64_t)batch * kKeyStride * 4 + 255) & ~(int64_t)255;
+  const int64_t sync_bytes = (int64_t)(batch + kWarpsPerBlock - 1) / kWarpsPerBlock * 2 * 4;
   uint8_t* buf = nullptr;
-  if (cudaMalloc(&buf, off_key + (int64_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_NOMEM;
+  if (cudaMalloc(&buf, off_sync + sync_bytes) != cudaSuccess) return PCL_ERR_NOMEM;
   *owned = buf;
   uint32_t* wall = reinterpret_cast<uint32_t*>(buf);
   uint32_t* coin = reinterpret_cast<uint32_t*>(buf + off_coin);
@@ -1128,6 +1206,9 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
   // Render keys of no render (frame -1): the first launch paints every board.
   p->render_key = reinterpret_cast<int32_t*>(buf + off_key);
   if (cudaMemset(p->render_key, 0xff, (size_t)batch * kKeyStride * 4) != cudaSuccess) return PCL_ERR_CUDA;
+  // No launch of the new binding has begun or ended (see "Block chaining").
+  p->block_sync = reinterpret_cast<uint32_t*>(buf + off_sync);
+  if (cudaMemset(p->block_sync, 0, sync_bytes) != cudaSuccess) return PCL_ERR_CUDA;
   build_blocked<<<1024, 256>>>(st.d_pattern[0], st.pattern_bstride[0], wall, PH, s.pattern_words,
                                nw, nblk, n_wall * blk_words);
   build_blocked<<<1024, 256>>>(st.d_pattern_init[1], st.pattern_init_bstride[1], coin, PH,
@@ -1146,7 +1227,7 @@ int derive(const pcl_spec& s, const pcl_state& st, int batch, StepParams* p, voi
 const Program kScrollyMaze = {check_spec, check_state, curtain, launch, nullptr,
                               /*float_reward=*/false, /*crop_epilogue=*/true,
                               /*scroll_groups=*/false, /*check_code=*/nullptr,
-                              /*float_reward_arg0=*/false, derive};
+                              /*float_reward_arg0=*/false, derive, /*block_chaining=*/true};
 
 }  // namespace pcl
 
