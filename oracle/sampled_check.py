@@ -69,19 +69,33 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       (engine.error_codes()) stays 0 while its oracle world raises nothing.  A world
       whose play() raises IndexError (a NumPy look-up off the board) at step t must find
       exactly ENV_ERR_INDEX latched after step t; lockstep then sets raised[env] = t and
-      compares that env no further, as the reference's Engine would play no further."""
+      compares that env no further, as the reference's Engine would play no further.
+      The same holds for a world whose its_showtime() raises, at the first launch (t = 0)
+      or at the launch that auto-resets the env."""
   import torch
   env_ids = [int(e) for e in env_ids]
   idx = torch.as_tensor(env_ids, dtype=torch.long, device=engine.device)
   T = actions.shape[0]
-  worlds = {e: make_world(e) for e in env_ids}
-  outs = {e: worlds[e].its_showtime() for e in env_ids}
+  def showtime(e, t):
+    """A fresh world for env e at step t, and its its_showtime() output."""
+    worlds[e] = make_world(e)
+    if croppers is not None:
+      croppers[e].set_engine(worlds[e])
+    if raised is None:
+      outs[e] = worlds[e].its_showtime()
+      return
+    try:
+      outs[e] = worlds[e].its_showtime()
+    except IndexError:
+      raised[e] = t
+
+  worlds, outs = {}, {}
   croppers = None
   if crop is not None:
     crop_spec, crop_state, make_cropper = crop
     croppers = {e: make_cropper() for e in env_ids}
-    for e in env_ids:
-      croppers[e].set_engine(worlds[e])
+  for e in env_ids:
+    showtime(e, 0)
   slots = [engine.sprite_chars.index(ch) for ch in sprites]
   acts_dev = torch.from_numpy(np.ascontiguousarray(actions, dtype=np.int32)).to(engine.device)
 
@@ -136,10 +150,7 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       if raised is not None and e in raised:
         continue
       if worlds[e].game_over:                 # the auto-reset rule
-        worlds[e] = make_world(e)
-        if croppers is not None:
-          croppers[e].set_engine(worlds[e])
-        outs[e] = worlds[e].its_showtime()
+        showtime(e, t + 1)
       elif raised is None:
         outs[e] = worlds[e].play(int(actions[t, e]))
       else:

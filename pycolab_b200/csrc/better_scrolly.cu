@@ -168,7 +168,9 @@ better_scrolly_step(const StepParams p) {
   // ---- final render, z-order a b c @ P (engine.py:737-759).  a, b, c lie under
   // the coins: patch them into the staged tile up front; coins come from the
   // bit rows (segment sg of a row = its sg-th 16-bit half-word); P is the top
-  // layer, patched into the one segment that holds it.
+  // layer, patched into the one segment that holds it.  A row holds 2*BW
+  // half-words; a pitch wider than that has segments of pad columns past them,
+  // which hold no coins and must not read the next row's bits.
   __syncwarp();
   if (lane == 0) {
 #pragma unroll
@@ -186,7 +188,8 @@ better_scrolly_step(const StepParams p) {
   const int dr = 32 / spr, dsg = 32 - dr * spr;
   for (int seg = lane; seg < total; seg += 32) {
     uint4 px = src[seg];
-    const unsigned coin_bits = reinterpret_cast<const uint16_t*>(s_coin + r * BW)[sg];
+    const unsigned coin_bits =
+        sg < 2 * BW ? reinterpret_cast<const uint16_t*>(s_coin + r * BW)[sg] : 0u;
     if (coin_bits) paint_bits(px, coin_bits, '@');
     if (seg == p_seg) paint_bits(px, p_bit, p.sprite_char[0]);
     dst[seg] = px;
@@ -194,6 +197,18 @@ better_scrolly_step(const StepParams p) {
     if (sg >= spr) { sg -= spr; ++r; }
   }
 }
+
+// Dynamic shared memory of one block (kWarpsPerBlock envs): each warp stages its
+// records, its whole backdrop tile and its coin bit rows (rounded up to 16 bytes).
+size_t block_smem(int H, int pitch, int BW) {
+  const size_t bits_bytes = (((size_t)H * BW * 4) + 15) & ~(size_t)15;
+  return (kRecWords * 4 + (size_t)H * pitch + bits_bytes) * kWarpsPerBlock;
+}
+
+// The most dynamic shared memory a block may ask for on the H100 (227 KB; the kernel
+// has no static shared memory).  check_spec accepts a spec only if its block fits,
+// so an accepted spec always launches.
+constexpr size_t kMaxBlockSmem = 227 * 1024;
 
 int check_spec(const pcl_spec& s) {
   if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
@@ -204,6 +219,7 @@ int check_spec(const pcl_spec& s) {
   for (int i = 0; i < 4; ++i)
     if (s.sprite_confined[i] || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
   if (!bit_rows_fit(s)) return PCL_ERR_INVALID;
+  if (block_smem(s.rows, s.pitch, s.bits_words) > kMaxBlockSmem) return PCL_ERR_UNSUPPORTED;
   return PCL_OK;
 }
 
@@ -213,9 +229,7 @@ int check_state(const pcl_spec&, const pcl_state& st) {
 }
 
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
-  const size_t bits_bytes = (((size_t)p.H * p.BW * 4) + 15) & ~(size_t)15;
-  const size_t smem = (kRecWords * 4 + (size_t)p.H * p.pitch + bits_bytes) * kWarpsPerBlock;
-  return launch_step(better_scrolly_step, p, kWarpsPerBlock, smem, s);
+  return launch_step(better_scrolly_step, p, kWarpsPerBlock, block_smem(p.H, p.pitch, p.BW), s);
 }
 
 }  // namespace
