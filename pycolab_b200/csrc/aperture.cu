@@ -36,31 +36,27 @@ aperture_step(const StepParams p) {
   const int warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, 1);
   const int H = p.H, W = p.W, pitch = p.pitch;
   const int tile = H * pitch;
   uint8_t* my = smem_raw + warp * (kRecWords * 4 + tile);
   int32_t* rec = reinterpret_cast<int32_t*>(my);
   uint8_t* s_bd = my + kRecWords * 4;
 
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_drape = p.st.d_drapes + (int64_t)env * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, backdrop + i * 16);
+  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, e.backdrop + i * 16);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
   const bool restart = run == ENV_RESTART;
   if (restart) {                                   // a fresh Engine (engine.py:520-581)
-    const PlotCarry carry = plot_carry(g_plot, true);
-    if (lane < 8) rec[lane] = __ldg(p.st.d_sprites_init + lvl * p.st.sprites_init_bstride + lane);
-    else if (lane < 16) rec[lane] = __ldg(p.st.d_drapes_init + lvl * p.st.drapes_init_bstride + lane - 8);
-    else rec[lane] = __ldg(p.st.d_plot_init + lvl * p.st.plot_init_bstride + lane - 16);
+    const PlotCarry carry = plot_carry(e.plot, true);
+    if (lane < 8) rec[lane] = __ldg(e.level(p.st.d_sprites_init, p.st.sprites_init_bstride) + lane);
+    else if (lane < 16) rec[lane] = __ldg(e.level(p.st.d_drapes_init, p.st.drapes_init_bstride) + lane - 8);
+    else rec[lane] = __ldg(e.level(p.st.d_plot_init, p.st.plot_init_bstride) + lane - 16);
     __syncwarp();
     if (lane == 0) store_carry(rec + 16, carry);
   } else {
-    rec[lane] = lane < 8 ? g_sprite[lane] : lane < 16 ? g_drape[lane - 8] : g_plot[lane - 16];
+    rec[lane] = lane < 8 ? e.sprites[lane] : lane < 16 ? e.drapes[lane - 8] : e.plot[lane - 16];
   }
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   cp_async_wait_all();
@@ -146,9 +142,9 @@ aperture_step(const StepParams p) {
     if (visible(sp)) s_bd[sp.row * pitch + sp.col] = p.sprite_char[0];
   }
   __syncwarp();
-  if (lane < 8) g_sprite[lane] = rec[lane];
-  else if (lane < 16) g_drape[lane - 8] = rec[lane];
-  else g_plot[lane - 16] = rec[lane];
+  if (lane < 8) e.sprites[lane] = rec[lane];
+  else if (lane < 16) e.drapes[lane - 8] = rec[lane];
+  else e.plot[lane - 16] = rec[lane];
 
   const uint4* src = reinterpret_cast<const uint4*>(s_bd);
   uint4* dst = reinterpret_cast<uint4*>(p.out.d_board + (int64_t)env * tile);

@@ -35,21 +35,18 @@ apprehend_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 2, 0);
   const int H = p.H, W = p.W, pitch = p.pitch;
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * 2 * PCL_SPRITE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprites;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
   Sprite pl = load_sprite(src_s), ball = load_sprite(src_s + PCL_SPRITE_WORDS);
   pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
   ball.aux2 = 0;
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   Plot plot = step_plot(src_p, carry.error);
   double dx = f64_of(ball.aux0, ball.aux1);
   double acc = f64_of(src_p[PCL_P_AUX0], src_p[PCL_P_AUX1]);
@@ -83,28 +80,22 @@ apprehend_step(const StepParams p) {
   __syncwarp();
   if (lane == 0) {
     ball.aux0 = __double2loint(dx); ball.aux1 = __double2hiint(dx);
-    store_sprite(g_sprites, pl);
-    store_sprite(g_sprites + PCL_SPRITE_WORDS, ball);
-    store_carry(g_plot, carry);
-    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
-    g_plot[PCL_P_AUX0] = __double2loint(acc); g_plot[PCL_P_AUX1] = __double2hiint(acc);
+    store_sprite(e.sprites, pl);
+    store_sprite(e.sprites + PCL_SPRITE_WORDS, ball);
+    store_carry(e.plot, carry);
+    store_plot<ORDER_CLEAR>(e.plot, plot, dir);
+    e.plot[PCL_P_AUX0] = __double2loint(acc); e.plot[PCL_P_AUX1] = __double2hiint(acc);
     store_outputs(p.out, env, dir);
   }
 
   // ---- render (engine.py:737-759): backdrop, 'b', then 'P' on top
-  uint8_t* board = p.out.d_board + (int64_t)env * H * pitch;
-  const int segs_per_row = pitch >> 4;
-  const int total = H * segs_per_row;
-  for (int seg = lane; seg < total; seg += 32) {
-    const int r = seg / segs_per_row;
-    const int c0 = (seg - r * segs_per_row) << 4;
-    uint4 px = *reinterpret_cast<const uint4*>(backdrop + r * pitch + c0);
+  paint_segments(p.out.d_board + (int64_t)env * H * pitch, e.backdrop, H, pitch, lane,
+                 [&](uint4& px, int r, int c0) {
     unsigned m = sprite_bit(ball, r, c0);
     if (m) paint_bits(px, m, p.sprite_char[1]);
     m = sprite_bit(pl, r, c0);
     if (m) paint_bits(px, m, p.sprite_char[0]);
-    *reinterpret_cast<uint4*>(board + r * pitch + c0) = px;
-  }
+  });
 }
 
 int check_spec(const pcl_spec& s) {

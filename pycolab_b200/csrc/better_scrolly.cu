@@ -39,7 +39,7 @@ better_scrolly_step(const StepParams p) {
   const int warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
+  const EnvAt e = env_at(p, env, kS, 1);
   const int H = p.H, W = p.W, pitch = p.pitch, BW = p.BW;
   const size_t tile = (size_t)H * pitch;
   const size_t bits_bytes = (((size_t)H * BW * 4) + 15) & ~(size_t)15;
@@ -48,36 +48,31 @@ better_scrolly_step(const StepParams p) {
   uint8_t* s_bd = my + kRecWords * 4;
   uint32_t* s_coin = reinterpret_cast<uint32_t*>(s_bd + tile);
 
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * kS * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
   uint32_t* g_coin = p.st.d_bits[0] + (int64_t)env * p.st.bits_bstride[0];
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
 
   {
     const int n16 = (int)(tile >> 4);
-    for (int i = lane; i < n16; i += 32) cp_async16(s_bd + i * 16, backdrop + i * 16);
+    for (int i = lane; i < n16; i += 32) cp_async16(s_bd + i * 16, e.backdrop + i * 16);
   }
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
   const bool restart = run == ENV_RESTART;
   const int nbits = H * BW;
   if (restart) {
-    const PlotCarry carry = plot_carry(g_plot, true);
-    rec[lane] = __ldg(p.st.d_sprites_init + lvl * p.st.sprites_init_bstride + lane);
-    if (lane < 8) rec[32 + lane] = __ldg(p.st.d_drapes_init +
-                                         lvl * p.st.drapes_init_bstride + lane);
-    if (lane >= 16) rec[32 + lane] = __ldg(p.st.d_plot_init +
-                                           lvl * p.st.plot_init_bstride + lane - 16);
+    const PlotCarry carry = plot_carry(e.plot, true);
+    rec[lane] = __ldg(e.level(p.st.d_sprites_init, p.st.sprites_init_bstride) + lane);
+    if (lane < 8) rec[32 + lane] = __ldg(e.level(p.st.d_drapes_init, p.st.drapes_init_bstride) + lane);
+    if (lane >= 16)
+      rec[32 + lane] = __ldg(e.level(p.st.d_plot_init, p.st.plot_init_bstride) + lane - 16);
     // Fresh coins (one Engine per episode): template -> live curtain and smem.
-    const uint32_t* src = p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0];
+    const uint32_t* src = e.level(p.st.d_bits_init[0], p.st.bits_init_bstride[0]);
     for (int i = lane; i < nbits; i += 32) { const uint32_t w = __ldg(src + i); g_coin[i] = w; s_coin[i] = w; }
     __syncwarp();
     if (lane == 0) store_carry(rec + 48, carry);
   } else {
-    rec[lane] = g_sprites[lane];
-    if (lane < 8) rec[32 + lane] = g_drapes[lane];
-    if (lane >= 16) rec[32 + lane] = g_plot[lane - 16];
+    rec[lane] = e.sprites[lane];
+    if (lane < 8) rec[32 + lane] = e.drapes[lane];
+    if (lane >= 16) rec[32 + lane] = e.plot[lane - 16];
     for (int i = lane; i < nbits; i += 32) cp_async4(s_coin + i, g_coin + i);
   }
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
@@ -161,9 +156,9 @@ better_scrolly_step(const StepParams p) {
     store_outputs(p.out, env, dir);
   }
   __syncwarp();
-  g_sprites[lane] = rec[lane];
-  if (lane < 8) g_drapes[lane] = rec[32 + lane];
-  if (lane >= 16) g_plot[lane - 16] = rec[32 + lane];
+  e.sprites[lane] = rec[lane];
+  if (lane < 8) e.drapes[lane] = rec[32 + lane];
+  if (lane >= 16) e.plot[lane - 16] = rec[32 + lane];
 
   // ---- final render, z-order a b c @ P (engine.py:737-759).  a, b, c lie under
   // the coins: patch them into the staged tile up front; coins come from the

@@ -40,19 +40,17 @@ box_world_step(const StepParams p) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, 0);
   const int H = p.H, pitch = p.pitch, segs = p.pitch >> 4;
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
   uint8_t* g_grid = reinterpret_cast<uint8_t*>(p.st.d_bits[0] + (int64_t)env * p.st.bits_bstride[0]);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprite;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
   const uint8_t* src_g = restart
-      ? reinterpret_cast<const uint8_t*>(p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0])
+      ? reinterpret_cast<const uint8_t*>(e.level(p.st.d_bits_init[0], p.st.bits_init_bstride[0]))
       : g_grid;
   uint8_t* grid = s_grid[warp];
   if (lane < H)
@@ -63,17 +61,16 @@ box_world_step(const StepParams p) {
   Sprite pl = load_sprite(src_s);
   pl.aux1 = pl.aux2 = 0;                           // stored as zeros
   int steps = pl.aux0;                             // PlayerSprite._step_counter
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   Plot plot = step_plot(src_p, carry.error);
   int over_ch = src_p[PCL_P_AUX0];                 // the_plot['over_this']: 0 = unset
   int over_at = src_p[PCL_P_AUX1];
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
   __syncwarp();
 
   // the board of the last render where the player is not: an object, else the backdrop
   auto board_at = [&](int r, int c) -> int {
     const int g = grid[r * pitch + c] & 0x7f;
-    return g ? g : backdrop[r * pitch + c];
+    return g ? g : e.backdrop[r * pitch + c];
   };
   const int held = board_at(0, 0);                 // inventory_item
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
@@ -96,7 +93,7 @@ box_world_step(const StepParams p) {
       const int thing = grid[at] & 0x7f;
       bool move;
       if (!thing) {
-        move = !in_set(p.impassable[0], backdrop[at]);
+        move = !in_set(p.impassable[0], e.backdrop[at]);
       } else {
         move = is_lock(thing) && held == thing + ('a' - 'A');
         if (move && on) { pl.row = pl.vrow = tr; pl.col = pl.vcol = tc; }
@@ -140,10 +137,10 @@ box_world_step(const StepParams p) {
   // ---- records, outputs and the grid rows that changed
   if (lane == 0) {
     pl.aux0 = steps;
-    store_sprite(g_sprite, pl);
-    store_carry(g_plot, carry);
-    store_plot<ORDER_KEEP>(g_plot, plot, dir);
-    g_plot[PCL_P_AUX0] = over_ch; g_plot[PCL_P_AUX1] = over_at;
+    store_sprite(e.sprites, pl);
+    store_carry(e.plot, carry);
+    store_plot<ORDER_KEEP>(e.plot, plot, dir);
+    e.plot[PCL_P_AUX0] = over_ch; e.plot[PCL_P_AUX1] = over_at;
     store_outputs(p.out, env, dir);
   }
   if (lane < H && (restart || (changed >= 0 && (lane == 0 || lane == changed))))
@@ -154,7 +151,7 @@ box_world_step(const StepParams p) {
   // ---- render (engine.py:737-759): backdrop, objects, then the player; lane r paints row r
   if (lane < H) {
     uint8_t* board = p.out.d_board + (int64_t)env * H * pitch + lane * pitch;
-    const uint8_t* bd = backdrop + lane * pitch;
+    const uint8_t* bd = e.backdrop + lane * pitch;
     for (int q = 0; q < segs; ++q) {
       const uint4 g4 = reinterpret_cast<const uint4*>(grid + lane * pitch)[q];
       const uint4 b4 = reinterpret_cast<const uint4*>(bd)[q];

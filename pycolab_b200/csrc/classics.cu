@@ -44,30 +44,27 @@ classics_step(const StepParams p) {
   const int warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, 0);
   const int H = p.H, W = p.W, pitch = p.pitch;
   const int tile = H * pitch;
   uint8_t* my = smem_raw + warp * (kRecWords * 4 + tile);
   int32_t* rec = reinterpret_cast<int32_t*>(my);
   uint8_t* s_bd = my + kRecWords * 4;
 
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, backdrop + i * 16);
+  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, e.backdrop + i * 16);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
   const bool restart = run == ENV_RESTART;
   if (restart) {                                   // a fresh Engine (engine.py:520-581)
-    const PlotCarry carry = plot_carry(g_plot, true);
-    if (lane < 8) rec[lane] = __ldg(p.st.d_sprites_init + lvl * p.st.sprites_init_bstride + lane);
-    if (lane >= 16) rec[lane] = __ldg(p.st.d_plot_init + lvl * p.st.plot_init_bstride + lane - 16);
+    const PlotCarry carry = plot_carry(e.plot, true);
+    if (lane < 8) rec[lane] = __ldg(e.level(p.st.d_sprites_init, p.st.sprites_init_bstride) + lane);
+    if (lane >= 16) rec[lane] = __ldg(e.level(p.st.d_plot_init, p.st.plot_init_bstride) + lane - 16);
     __syncwarp();
     if (lane == 0) store_carry(rec + 16, carry);
   } else {
-    if (lane < 8) rec[lane] = g_sprite[lane];
-    if (lane >= 16) rec[lane] = g_plot[lane - 16];
+    if (lane < 8) rec[lane] = e.sprites[lane];
+    if (lane >= 16) rec[lane] = e.plot[lane - 16];
   }
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   cp_async_wait_all();
@@ -93,7 +90,7 @@ classics_step(const StepParams p) {
       const int r = r0 + i / W, c = i - (r - r0) * W;
       int src = c + k;
       if (src >= W) src -= W;
-      s_bd[r * pitch + c] = __ldg(backdrop + r * pitch + src);
+      s_bd[r * pitch + c] = __ldg(e.backdrop + r * pitch + src);
     }
     __syncwarp();               // the walker's neighbourhood test reads cells other lanes wrote
     if (even) walker_move(sp, 0, PCL_M_W, plot, H, W, p.confined[0] != 0, false, lane, blocked);
@@ -131,8 +128,8 @@ classics_step(const StepParams p) {
     store_outputs(p.out, env, dir);
   }
   __syncwarp();
-  if (lane < 8) g_sprite[lane] = rec[lane];
-  if (lane >= 16) g_plot[lane - 16] = rec[lane];
+  if (lane < 8) e.sprites[lane] = rec[lane];
+  if (lane >= 16) e.plot[lane - 16] = rec[lane];
 
   // ---- final render: backdrop + P (engine.py:737-759)
   uint8_t* board = p.out.d_board + (int64_t)env * tile;

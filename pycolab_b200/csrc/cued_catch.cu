@@ -113,18 +113,15 @@ cued_catch_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 3, 1);
   const int H = p.H, W = p.W, BW = p.BW, pitch = p.pitch;
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * 3 * PCL_SPRITE_WORDS;
-  int32_t* g_q = p.st.d_drapes + (int64_t)env * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprites;
-  const int32_t* src_q = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_q;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_q = e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
 
   Sprite sp[3];
 #pragma unroll
@@ -137,7 +134,7 @@ cued_catch_step(const StepParams p) {
   int choice = src_q[PCL_D_PRE_R], tick2 = src_q[PCL_D_PRE_C];
   int last_reset = src_q[PCL_D_LAST_FRAME], trials = src_q[PCL_D_AUX0];
   int pairs = src_q[PCL_D_AUX1];
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   const Plot plot = step_plot(src_p, carry.error);
   const int f = plot.frame;
   int programmed = src_p[PCL_P_AUX0], which = src_p[PCL_P_AUX1], ball_reset = src_p[PCL_P_AUX2];
@@ -260,7 +257,7 @@ cued_catch_step(const StepParams p) {
   uint64_t qrow = 0;
   bool banded = false;
   if (lane < H) {
-    const uint32_t* init = p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0] + lane * BW;
+    const uint32_t* init = e.level(p.st.d_bits_init[0], p.st.bits_init_bstride[0]) + lane * BW;
     qrow = (uint64_t)init[0] | (W > 32 ? (uint64_t)init[1] << 32 : 0ull);
     const bool in_symbol = lane >= 3 && lane < 5;
     const uint64_t symbol_row = symbol == kWhichTop ? cols_bits(0, min(6, W))
@@ -294,13 +291,13 @@ cued_catch_step(const StepParams p) {
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       sp[i].aux0 = i == SP ? ttr : 0;
-      store_sprite(g_sprites + i * PCL_SPRITE_WORDS, sp[i]);
+      store_sprite(e.sprites + i * PCL_SPRITE_WORDS, sp[i]);
     }
-    store_drape(g_q, {phase, tick1, choice, tick2, last_reset, trials, pairs, 0});
-    store_carry(g_plot, carry);
-    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
-    g_plot[PCL_P_AUX0] = programmed; g_plot[PCL_P_AUX1] = which;
-    g_plot[PCL_P_AUX2] = ball_reset; g_plot[PCL_P_AUX3] = noisy_pay ? 1 : 0;
+    store_drape(e.drapes, {phase, tick1, choice, tick2, last_reset, trials, pairs, 0});
+    store_carry(e.plot, carry);
+    store_plot<ORDER_CLEAR>(e.plot, plot, dir);
+    e.plot[PCL_P_AUX0] = programmed; e.plot[PCL_P_AUX1] = which;
+    e.plot[PCL_P_AUX2] = ball_reset; e.plot[PCL_P_AUX3] = noisy_pay ? 1 : 0;
     // has_reward is 1: PlayerSprite.update pays (possibly 0) at every step
     if (noisy) store_outputs(p.out, env, dir, noisy_pay ? reward_f64 : (double)dir.reward);
     else store_outputs(p.out, env, dir);
@@ -312,10 +309,9 @@ cued_catch_step(const StepParams p) {
     Sprite shown[3] = {sp[SP], sp[SA], sp[SB]};
 #pragma unroll
     for (int i = 1; i < 3; ++i) if (shown[i].col < 0) shown[i].col += W;
-    const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride + lane * pitch;
     uint8_t* board = p.out.d_board + (int64_t)env * H * pitch + lane * pitch;
     for (int c0 = 0; c0 < pitch; c0 += 16) {
-      uint4 px = *reinterpret_cast<const uint4*>(backdrop + c0);
+      uint4 px = *reinterpret_cast<const uint4*>(e.backdrop + lane * pitch + c0);
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
         const unsigned m = sprite_bit(shown[i], lane, c0);

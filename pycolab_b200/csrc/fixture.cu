@@ -59,35 +59,28 @@ fixture_step(const StepParams p) {
   const int warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;   // index of static level data
   const int H = p.H, W = p.W, S = p.S, D = p.D, n = S + D;
+  const EnvAt e = env_at(p, env, S, D);
   const size_t board_bytes = board::board_bytes(H, p.pitch);
   uint8_t* my = smem_raw + warp * (sizeof(WarpState) + board_bytes);
   WarpState* st = reinterpret_cast<WarpState*>(my);
   Ctx c;
   c.p = &p; c.st = st; c.board = my + sizeof(WarpState);
-  c.backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  c.env = env; c.lane = lane; c.lvl = lvl; c.kept = 0;
+  c.backdrop = e.backdrop;
+  c.env = env; c.lane = lane; c.lvl = e.lvl; c.kept = 0;
 
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * D * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
   uint8_t* g_z = p.st.d_z_order + (int64_t)env * n;
   uint8_t* g_board = p.out.d_board + (int64_t)env * H * p.pitch;
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride
-                                 : g_sprites;
-  const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride
-                                 : g_drapes;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride
-                                 : g_plot;
-  const uint8_t* src_z = restart ? p.st.d_z_order_init + lvl * p.st.z_order_init_bstride
-                                 : g_z;
-  const PlotCarry carry = plot_carry(g_plot, restart);
-  board::stage_records(st, src_s, src_d, src_p, src_z, S, D, lane);
+  const PlotCarry carry = plot_carry(e.plot, restart);
+  board::stage_records(
+      st, e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites),
+      e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes),
+      e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot),
+      e.start(restart, p.st.d_z_order_init, p.st.z_order_init_bstride, g_z), S, D, lane);
   for (int i = lane; i < S * 4; i += 32) (&st->impassable[0][0])[i] = p.impassable[i >> 2][i & 3];
   for (int i = lane; i < (int)board_bytes; i += 32) c.board[i] = 0;
   __syncwarp();
@@ -98,7 +91,7 @@ fixture_step(const StepParams p) {
       ? p.st.d_groups + (int64_t)env * PCL_MAX_SCROLL_GROUPS * PCL_GROUP_WORDS : nullptr;
   if (lane < PCL_GROUP_WORDS) st->groups[0][lane] = st->plot[PCL_P_ORDER_R + lane];
   if (g_groups && n_sg > 1) {
-    const int32_t* src_g = restart ? p.st.d_groups_init + lvl * p.st.groups_init_bstride : g_groups;
+    const int32_t* src_g = e.start(restart, p.st.d_groups_init, p.st.groups_init_bstride, g_groups);
     if (lane >= PCL_GROUP_WORDS && lane < n_sg * PCL_GROUP_WORDS)
       (&st->groups[0][0])[lane] = src_g[lane];
   }
@@ -196,7 +189,7 @@ fixture_step(const StepParams p) {
     store_outputs(p.out, env, dir);
   }
   __syncwarp();
-  board::store_env(c, g_sprites, g_drapes, g_plot, g_z, g_board);
+  board::store_env(c, e.sprites, e.drapes, e.plot, g_z, g_board);
   if (g_groups && n_sg > 1 && lane >= PCL_GROUP_WORDS && lane < n_sg * PCL_GROUP_WORDS)
     g_groups[lane] = (&st->groups[0][0])[lane];
 }

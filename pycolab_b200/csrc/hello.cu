@@ -24,26 +24,22 @@ hello_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
   const int H = p.H, W = p.W, pitch = p.pitch, S = p.S, BW = p.BW;
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
-  int32_t* g_drape = p.st.d_drapes + (int64_t)env * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  const uint32_t* base = p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0];
+  const EnvAt e = env_at(p, env, S, 1);
+  const uint32_t* base = e.level(p.st.d_bits_init[0], p.st.bits_init_bstride[0]);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprites;
-  const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drape;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_d = e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
   // lane s < S owns sprite s; every lane knows the drape's roll counters
   Sprite sp = {};
   if (lane < S) sp = load_sprite(src_s + lane * PCL_SPRITE_WORDS);
   const int kset = sp.aux0;
   int roll_r = src_d[PCL_D_AUX0], roll_c = src_d[PCL_D_AUX1];
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   const Plot plot = step_plot(src_p, carry.error);
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   Directives dir = fresh_directives();
@@ -70,13 +66,13 @@ hello_step(const StepParams p) {
   __syncwarp();
   if (lane < S) {                                   // a plain Sprite: virtual = true position
     sp.vrow = sp.row; sp.vcol = sp.col;
-    store_sprite(g_sprites + lane * PCL_SPRITE_WORDS, sp, PCL_S_AUX1);
+    store_sprite(e.sprites + lane * PCL_SPRITE_WORDS, sp, PCL_S_AUX1);
   }
   if (lane == 0) {
-    g_drape[PCL_D_AUX0] = roll_r; g_drape[PCL_D_AUX1] = roll_c;
-    g_drape[PCL_D_LAST_FRAME] = src_d[PCL_D_LAST_FRAME];
-    store_carry(g_plot, carry);
-    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
+    e.drapes[PCL_D_AUX0] = roll_r; e.drapes[PCL_D_AUX1] = roll_c;
+    e.drapes[PCL_D_LAST_FRAME] = src_d[PCL_D_LAST_FRAME];
+    store_carry(e.plot, carry);
+    store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
 
@@ -95,7 +91,7 @@ hello_step(const StepParams p) {
     const int r = cell / pitch, c = cell - r * pitch;
     int code = 0;                                        // pitch padding stays 0
     if (c < W) {
-      code = backdrop[r * pitch + c];
+      code = e.backdrop[r * pitch + c];
       for (int k = 0; k < n; ++k) {
         const int ch = p.program_arg[k];                 // z-order, back to front
         if (ch == p.drape_char[0]) {

@@ -31,42 +31,38 @@ ordeal_step(const StepParams p) {
   const int warp = threadIdx.x >> 5;
   const int env = blockIdx.x * kWarpsPerBlock + warp;
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
   const int H = p.H, W = p.W, pitch = p.pitch, S = p.S, D = p.D, BW = p.BW;
+  const EnvAt e = env_at(p, env, S, 1);
   const int chapter = p.program_arg[0];
   const int tile = H * pitch;
   uint8_t* my = smem_raw + warp * (kRecWords * 4 + tile);
   int32_t* rec = reinterpret_cast<int32_t*>(my);
   uint8_t* s_bd = my + kRecWords * 4;
 
-  int32_t* g_sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
-  int32_t* g_drape = D ? p.st.d_drapes + (int64_t)env * PCL_DRAPE_WORDS : nullptr;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
   uint8_t* g_z = p.st.d_z_order ? p.st.d_z_order + (int64_t)env * (S + D) : nullptr;
   uint32_t* sword = D ? p.st.d_bits[0] + (int64_t)env * p.st.bits_bstride[0] : nullptr;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
-  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, backdrop + i * 16);
+  for (int i = lane; i < (tile >> 4); i += 32) cp_async16(s_bd + i * 16, e.backdrop + i * 16);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
   const bool restart = run == ENV_RESTART;
   if (restart) {                                   // a fresh Engine (engine.py:520-581)
-    const PlotCarry carry = plot_carry(g_plot, true);
-    if (lane < S * 8) rec[lane] = __ldg(p.st.d_sprites_init + lvl * p.st.sprites_init_bstride + lane);
+    const PlotCarry carry = plot_carry(e.plot, true);
+    if (lane < S * 8) rec[lane] = __ldg(e.level(p.st.d_sprites_init, p.st.sprites_init_bstride) + lane);
     if (D && lane >= 16 && lane < 24)
-      rec[lane] = __ldg(p.st.d_drapes_init + lvl * p.st.drapes_init_bstride + lane - 16);
-    if (lane < 16) rec[32 + lane] = __ldg(p.st.d_plot_init + lvl * p.st.plot_init_bstride + lane);
+      rec[lane] = __ldg(e.level(p.st.d_drapes_init, p.st.drapes_init_bstride) + lane - 16);
+    if (lane < 16) rec[32 + lane] = __ldg(e.level(p.st.d_plot_init, p.st.plot_init_bstride) + lane);
     if (D) {
-      const uint32_t* src = p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0];
+      const uint32_t* src = e.level(p.st.d_bits_init[0], p.st.bits_init_bstride[0]);
       for (int i = lane; i < H * BW; i += 32) sword[i] = __ldg(src + i);
     }
-    if (g_z && lane < S + D) g_z[lane] = p.st.d_z_order_init[lvl * p.st.z_order_init_bstride + lane];
+    if (g_z && lane < S + D) g_z[lane] = e.level(p.st.d_z_order_init, p.st.z_order_init_bstride)[lane];
     __syncwarp();
     if (lane == 0) store_carry(rec + 32, carry);
   } else {
-    if (lane < S * 8) rec[lane] = g_sprites[lane];
-    if (D && lane >= 16 && lane < 24) rec[lane] = g_drape[lane - 16];
-    if (lane < 16) rec[32 + lane] = g_plot[lane];
+    if (lane < S * 8) rec[lane] = e.sprites[lane];
+    if (D && lane >= 16 && lane < 24) rec[lane] = e.drapes[lane - 16];
+    if (lane < 16) rec[32 + lane] = e.plot[lane];
   }
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   cp_async_wait_all();
@@ -182,18 +178,13 @@ ordeal_step(const StepParams p) {
     if (g_z && z_changed) { g_z[0] = z0; g_z[1] = z1; }
   }
   __syncwarp();
-  if (lane < S * 8) g_sprites[lane] = rec[lane];
-  if (D && lane >= 16 && lane < 24) g_drape[lane - 16] = rec[lane];
-  if (lane < 16) g_plot[lane] = rec[32 + lane];
+  if (lane < S * 8) e.sprites[lane] = rec[lane];
+  if (D && lane >= 16 && lane < 24) e.drapes[lane - 16] = rec[lane];
+  if (lane < 16) e.plot[lane] = rec[32 + lane];
 
   // ---- final render in the (possibly new) z-order (engine.py:737-759)
-  uint8_t* board = p.out.d_board + (int64_t)env * tile;
-  const int segs_per_row = pitch >> 4;
-  const int total = H * segs_per_row;
-  for (int seg = lane; seg < total; seg += 32) {
-    const int r = seg / segs_per_row;
-    const int c0 = (seg - r * segs_per_row) << 4;
-    uint4 px = *reinterpret_cast<const uint4*>(s_bd + r * pitch + c0);
+  paint_segments(p.out.d_board + (int64_t)env * tile, s_bd, H, pitch, lane,
+                 [&](uint4& px, int r, int c0) {
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       const uint8_t ch = k == 0 ? z0 : z1;
@@ -205,8 +196,7 @@ ordeal_step(const StepParams p) {
         m = bits16(sword + (int64_t)r * BW, c0) & ((1u << min(16, W - c0)) - 1u);
       if (m) paint_bits(px, m, ch);
     }
-    *reinterpret_cast<uint4*>(board + r * pitch + c0) = px;
-  }
+  });
 }
 
 int check_spec(const pcl_spec& s) {

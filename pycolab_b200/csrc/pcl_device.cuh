@@ -336,6 +336,22 @@ __device__ __forceinline__ unsigned sprite_bit(const Sprite& s, int r, int c0) {
   const int dc = s.col - c0;
   return (visible(s) && s.row == r && (unsigned)dc < 16u) ? (1u << dc) : 0u;
 }
+// The final render of an H x pitch board, one lane per 16-byte segment: each segment
+// starts as the same segment of `base` (the backdrop or a staged tile), and
+// `paint(px, r, c0)` paints the segment `px` that starts at (r, c0).
+template <typename Paint>
+__device__ __forceinline__ void paint_segments(uint8_t* board, const uint8_t* base, int H,
+                                               int pitch, int lane, Paint paint) {
+  const int segs_per_row = pitch >> 4;
+  const int total = H * segs_per_row;
+  for (int seg = lane; seg < total; seg += 32) {
+    const int r = seg / segs_per_row;
+    const int c0 = (seg - r * segs_per_row) << 4;
+    uint4 px = *reinterpret_cast<const uint4*>(base + r * pitch + c0);
+    paint(px, r, c0);
+    *reinterpret_cast<uint4*>(board + r * pitch + c0) = px;
+  }
+}
 
 // ------------------------------------------------- TMA (1-D bulk) tile moves --
 // A board tile is a contiguous, 16-byte aligned run of H * pitch bytes, so it
@@ -411,6 +427,40 @@ __device__ __forceinline__ bool in_set(const uint32_t* set, int code) {
 
 enum { MODE_STEP = 0, MODE_RESET = 1 };
 enum EnvRun { ENV_SKIP, ENV_STEP, ENV_RESTART };
+
+// Where env `env` lives in the bound pcl_state (include/pcl.h): its live records are per
+// env; templates and the other static level data are per level, or one copy for every
+// level when their bstride is 0; without d_level, env e plays level e.
+struct EnvAt {
+  int64_t lvl;                   // the env's level
+  int32_t* sprites;              // the env's live records
+  int32_t* drapes;
+  int32_t* plot;
+  const uint8_t* backdrop;       // the level's backdrop
+
+  // The per-level array `base` (d_*_init, d_bits_init, d_pattern, ...) at the env's level.
+  template <typename T>
+  __device__ __forceinline__ T* level(T* base, int64_t bstride) const { return base + lvl * bstride; }
+  // The record a step starts from: the template at the env's level on a restart, else the
+  // live record.
+  template <typename T>
+  __device__ __forceinline__ const T* start(bool restart, const T* init, int64_t bstride,
+                                            const T* live) const {
+    return restart ? level(init, bstride) : live;
+  }
+};
+
+// S sprites and D drapes per env: constants where the program's check_spec fixes them.  A
+// program whose drape count may be 0 passes 1 and reads `drapes` only when it has one.
+__device__ __forceinline__ EnvAt env_at(const StepParams& p, int env, int S, int D) {
+  EnvAt e;
+  e.lvl = p.st.d_level ? p.st.d_level[env] : env;
+  e.sprites = p.st.d_sprites + (int64_t)env * S * PCL_SPRITE_WORDS;
+  e.drapes = p.st.d_drapes + (int64_t)env * D * PCL_DRAPE_WORDS;
+  e.plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
+  e.backdrop = e.level(p.st.d_backdrop, p.st.backdrop_bstride);
+  return e;
+}
 
 // What env `env` does in this launch, given its plot's game_over word.  A reset
 // restarts the envs the mask selects (all without a mask) and leaves the others

@@ -43,26 +43,22 @@ sequence_recall_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, 2);
   const int H = p.H, W = p.W, BW = p.BW, pitch = p.pitch;
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * 2 * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprite;
-  const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_d = e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
 
   Sprite pl = load_sprite(src_s);
   pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
   const int covered0 = src_d[PCL_D_AUX0];
   int covered = covered0;
   int cleared = src_d[PCL_DRAPE_WORDS + PCL_D_AUX0];
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   Plot plot = step_plot(src_p, carry.error);
   int pc = src_p[PCL_P_AUX0], fis = src_p[PCL_P_AUX1], timeout = src_p[PCL_P_AUX2];
   uint32_t seq = (uint32_t)src_p[PCL_P_AUX3];
@@ -105,7 +101,7 @@ sequence_recall_step(const StepParams p) {
     const int motion = action == 1 ? PCL_M_N : action == 2 ? PCL_M_S : action == 3 ? PCL_M_W
                                                                                   : PCL_M_E;
     walker_move(pl, 0, motion, plot, H, W, true, false, lane,
-                [&](int r, int c) { return backdrop[r * pitch + c] == '#'; });
+                [&](int r, int c) { return e.backdrop[r * pitch + c] == '#'; });
   }
   if (timeout <= 0) {
     terminate(dir);
@@ -116,7 +112,7 @@ sequence_recall_step(const StepParams p) {
 
   // ---- MaskDrape.update (:213-262)
   fis += 1;
-  const int above = backdrop[pl.row * pitch + pl.col];
+  const int above = e.backdrop[pl.row * pitch + pl.col];
   if (state == kQuit) {
     if (fis == 1) timeout = 1;
   } else if (state == kOff || state == kOn) {
@@ -140,13 +136,13 @@ sequence_recall_step(const StepParams p) {
 
   // ---- curtains: M's bit rows when its set changed, '%' at a restart and when it clears
   if (lane < H && (restart || covered != covered0 || clear_now)) {
-    const uint32_t* pct_init = p.st.d_bits_init[DPCT] + lvl * p.st.bits_init_bstride[DPCT] + lane * BW;
+    const uint32_t* pct_init = e.level(p.st.d_bits_init[DPCT], p.st.bits_init_bstride[DPCT]) + lane * BW;
     uint32_t* m_live = p.st.d_bits[DM] + (int64_t)env * p.st.bits_bstride[DM] + lane * BW;
     uint32_t* pct_live = p.st.d_bits[DPCT] + (int64_t)env * p.st.bits_bstride[DPCT] + lane * BW;
     for (int w = 0; w < BW; ++w) {
       uint32_t bits = 0;
       for (int c = 32 * w; c < min(32 * w + 32, W); ++c) {
-        const int ch = backdrop[lane * pitch + c] - '1';
+        const int ch = e.backdrop[lane * pitch + c] - '1';
         if (ch >= 0 && ch < 4 && ((covered >> ch) & 1)) bits |= 1u << (c & 31);
       }
       m_live[w] = bits;
@@ -155,26 +151,26 @@ sequence_recall_step(const StepParams p) {
   }
 
   if (lane == 0) {
-    store_sprite(g_sprite, pl);
-    const int32_t* init_d = p.st.d_drapes_init + lvl * p.st.drapes_init_bstride;
+    store_sprite(e.sprites, pl);
+    const int32_t* init_d = e.level(p.st.d_drapes_init, p.st.drapes_init_bstride);
 #pragma unroll
     for (int d = 0; d < 2; ++d) {
-      int32_t* r = g_drapes + d * PCL_DRAPE_WORDS;
+      int32_t* r = e.drapes + d * PCL_DRAPE_WORDS;
       const int32_t* r0 = init_d + d * PCL_DRAPE_WORDS;
       for (int w = 0; w < PCL_DRAPE_WORDS; ++w) r[w] = r0[w];
       r[PCL_D_AUX0] = d == DM ? covered : cleared;
     }
-    store_carry(g_plot, carry);
-    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
-    g_plot[PCL_P_AUX0] = pc; g_plot[PCL_P_AUX1] = fis;
-    g_plot[PCL_P_AUX2] = timeout; g_plot[PCL_P_AUX3] = (int)seq;
+    store_carry(e.plot, carry);
+    store_plot<ORDER_CLEAR>(e.plot, plot, dir);
+    e.plot[PCL_P_AUX0] = pc; e.plot[PCL_P_AUX1] = fis;
+    e.plot[PCL_P_AUX2] = timeout; e.plot[PCL_P_AUX3] = (int)seq;
     store_outputs(p.out, env, dir, dir.has_reward ? reward : 0.0);
   }
 
   // ---- render (engine.py:737-759): backdrop, M over the covered lights, P, '%'
   if (lane < H) {
-    const uint32_t* pct = p.st.d_bits_init[DPCT] + lvl * p.st.bits_init_bstride[DPCT] + lane * BW;
-    const uint8_t* brow = backdrop + lane * pitch;
+    const uint32_t* pct = e.level(p.st.d_bits_init[DPCT], p.st.bits_init_bstride[DPCT]) + lane * BW;
+    const uint8_t* brow = e.backdrop + lane * pitch;
     uint8_t* board = p.out.d_board + (int64_t)env * H * pitch + lane * pitch;
     for (int c0 = 0; c0 < pitch; c0 += 16) {
       uint4 px = *reinterpret_cast<const uint4*>(brow + c0);

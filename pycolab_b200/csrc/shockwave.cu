@@ -45,31 +45,27 @@ shockwave_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, 3);
   const int H = p.H, W = p.W, pitch = p.pitch, BW = p.BW;
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * 3 * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
   uint32_t* wave_bits = p.st.d_bits[0] + (int64_t)env * p.st.bits_bstride[0];
-  const uint32_t* danger_bits = p.st.d_bits_init[1] + lvl * p.st.bits_init_bstride[1];
-  const uint32_t* safe_bits = p.st.d_bits_init[2] + lvl * p.st.bits_init_bstride[2];
+  const uint32_t* danger_bits = e.level(p.st.d_bits_init[1], p.st.bits_init_bstride[1]);
+  const uint32_t* safe_bits = e.level(p.st.d_bits_init[2], p.st.bits_init_bstride[2]);
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprite;
-  const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_d = e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
   Sprite pl = load_sprite(src_s);
   pl.aux0 = pl.aux1 = pl.aux2 = 0;                                    // stored as zeros
   int impact = src_d[PCL_D_AUX0], steps = src_d[PCL_D_AUX1];
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   Plot plot = step_plot(src_p, carry.error);
   const int action = restart ? PCL_ACTION_NONE : env_action(p, env);
   Directives dir = fresh_directives();
   // Row `lane` of the curtain the LAST render showed (the art's '@' cells after a restart).
-  const uint32_t* old_base = restart ? p.st.d_bits_init[0] + lvl * p.st.bits_init_bstride[0] : wave_bits;
+  const uint32_t* old_base = e.start(restart, p.st.d_bits_init[0], p.st.bits_init_bstride[0], wave_bits);
   const u64 old_row = lane < H ? row_bits(old_base, lane, BW) : 0ull;
   const int old_row_p = pl.row, old_col_p = pl.col;
   const bool old_vis_p = visible(pl);
@@ -77,7 +73,7 @@ shockwave_step(const StepParams p) {
   // ---- PlayerSprite.update (:98-109)
   const int motion = action == 0 ? PCL_M_N : action == 1 ? PCL_M_W : action == 2 ? PCL_M_E
                    : action == 3 ? PCL_M_STAY : PCL_M_NONE;
-  auto wall = [&](int r, int c) { return in_set(p.impassable[0], backdrop[r * pitch + c]); };
+  auto wall = [&](int r, int c) { return in_set(p.impassable[0], e.backdrop[r * pitch + c]); };
   if (motion != PCL_M_NONE)
     walker_move(pl, 0, motion, plot, H, W, p.confined[0] != 0, false, lane, wall);
 
@@ -119,30 +115,24 @@ shockwave_step(const StepParams p) {
     if (BW > 1) row[1] = (uint32_t)(new_row >> 32);
   }
   if (lane == 0) {
-    store_sprite(g_sprite, pl);
-    g_drapes[PCL_D_AUX0] = impact; g_drapes[PCL_D_AUX1] = steps;
-    g_drapes[PCL_D_LAST_FRAME] = PCL_NEVER;
-    store_carry(g_plot, carry);
-    store_plot<ORDER_CLEAR>(g_plot, plot, dir);
+    store_sprite(e.sprites, pl);
+    e.drapes[PCL_D_AUX0] = impact; e.drapes[PCL_D_AUX1] = steps;
+    e.drapes[PCL_D_LAST_FRAME] = PCL_NEVER;
+    store_carry(e.plot, carry);
+    store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
 
   // ---- render (engine.py:737-759): backdrop, ' ', '^', '@', P
-  uint8_t* board = p.out.d_board + (int64_t)env * H * pitch;
-  const int segs_per_row = pitch >> 4;
-  const int total = H * segs_per_row;
-  for (int seg = lane; seg < total; seg += 32) {
-    const int r = seg / segs_per_row;
-    const int c0 = (seg - r * segs_per_row) << 4;
-    uint4 px = *reinterpret_cast<const uint4*>(backdrop + r * pitch + c0);
+  paint_segments(p.out.d_board + (int64_t)env * H * pitch, e.backdrop, H, pitch, lane,
+                 [&](uint4& px, int r, int c0) {
     const u64 wave_r = s_rows[threadIdx.x >> 5][r];
     paint_bits(px, (unsigned)((row_bits(danger_bits, r, BW) >> c0) & 0xffffull), p.drape_char[1]);
     paint_bits(px, (unsigned)((row_bits(safe_bits, r, BW) >> c0) & 0xffffull), p.drape_char[2]);
     paint_bits(px, (unsigned)((wave_r >> c0) & 0xffffull), p.drape_char[0]);
     const unsigned m = sprite_bit(pl, r, c0);
     if (m) paint_bits(px, m, p.sprite_char[0]);
-    *reinterpret_cast<uint4*>(board + r * pitch + c0) = px;
-  }
+  });
 }
 
 int check_spec(const pcl_spec& s) {

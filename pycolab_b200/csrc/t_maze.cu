@@ -126,25 +126,22 @@ t_maze_step(const StepParams p) {
   const int lane = threadIdx.x & 31;
   const int env = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (env >= p.B) return;
-  const int64_t lvl = p.st.d_level ? p.st.d_level[env] : env;
+  const EnvAt e = env_at(p, env, 1, ND);
   const int H = p.H, W = p.W, PH = p.PH, PW = p.PW, PWW = p.PWW, BW = p.BW;
-  int32_t* g_sprite = p.st.d_sprites + (int64_t)env * PCL_SPRITE_WORDS;
-  int32_t* g_drapes = p.st.d_drapes + (int64_t)env * ND * PCL_DRAPE_WORDS;
-  int32_t* g_plot = p.st.d_plot + (int64_t)env * PCL_PLOT_WORDS;
 
-  const EnvRun run = env_run(p, env, g_plot[PCL_P_GAME_OVER]);
+  const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
   const bool restart = run == ENV_RESTART;
-  const int32_t* src_s = restart ? p.st.d_sprites_init + lvl * p.st.sprites_init_bstride : g_sprite;
-  const int32_t* src_d = restart ? p.st.d_drapes_init + lvl * p.st.drapes_init_bstride : g_drapes;
-  const int32_t* src_p = restart ? p.st.d_plot_init + lvl * p.st.plot_init_bstride : g_plot;
+  const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
+  const int32_t* src_d = e.start(restart, p.st.d_drapes_init, p.st.drapes_init_bstride, e.drapes);
+  const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
 
   Sprite pl[1] = {load_sprite(src_s)};
   pl[0].aux2 = 0;                                                     // stored as zero
   Drape dr[ND];
 #pragma unroll
   for (int d = 0; d < ND; ++d) dr[d] = load_drape(src_d + d * PCL_DRAPE_WORDS);
-  const PlotCarry carry = plot_carry(g_plot, restart);
+  const PlotCarry carry = plot_carry(e.plot, restart);
   Plot plot = step_plot</*kOrder=*/true>(src_p, carry.error);
   int timeout = src_p[PCL_P_AUX0];                 // the_plot['timeout_frames']
   int tele_frame = src_p[PCL_P_AUX1];              // the_plot.get('teleportation_order_frame', -1)
@@ -153,7 +150,7 @@ t_maze_step(const StepParams p) {
   const uint32_t* pattern[ND];
 #pragma unroll
   for (int d = 1; d < ND; ++d)
-    pattern[d] = p.st.d_pattern[d] + (d == DDIRT ? (int64_t)env : lvl) * p.st.pattern_bstride[d];
+    pattern[d] = p.st.d_pattern[d] + (d == DDIRT ? (int64_t)env : e.lvl) * p.st.pattern_bstride[d];
   uint32_t* dirt = p.st.d_pattern[DDIRT] + (int64_t)env * p.st.pattern_bstride[DDIRT];
   uint32_t* q_bits = p.st.d_bits[DQ] + (int64_t)env * p.st.bits_bstride[DQ];
 
@@ -165,7 +162,7 @@ t_maze_step(const StepParams p) {
     if (draw) which_goal = mt_random53(g_mt, lane) < 0.5 ? 0 : 1;
     // 'left' blanks columns 6 and up, 'right' columns 0-5 (:263-266)
     const uint32_t keep = which_goal == 0 ? 0x3fu : ~0x3fu;
-    const uint32_t* q_init = p.st.d_bits_init[DQ] + lvl * p.st.bits_init_bstride[DQ];
+    const uint32_t* q_init = e.level(p.st.d_bits_init[DQ], p.st.bits_init_bstride[DQ]);
     for (int i = lane; i < H * BW; i += 32) q_bits[i] = (i % BW == 0) ? (q_init[i] & keep) : 0u;
     uint32_t* stream = scratch[threadIdx.x >> 5].stream;
     const int total = PH * PW;
@@ -178,7 +175,7 @@ t_maze_step(const StepParams p) {
       speckle_stream(mt, stream, total, lane);
       for (int i = lane; i < PCL_MT_WORDS; i += 32) g_mt[PCL_MT_WORDS + i] = mt[i];
     }
-    const uint32_t* dirt_init = p.st.d_pattern_init[DDIRT] + lvl * p.st.pattern_init_bstride[DDIRT];
+    const uint32_t* dirt_init = e.level(p.st.d_pattern_init[DDIRT], p.st.pattern_init_bstride[DDIRT]);
     for (int i = lane; i < PH * PWW; i += 32) {
       const int r = i / PWW, w = i - r * PWW;
       uint32_t v = dirt_init[i];
@@ -295,21 +292,20 @@ t_maze_step(const StepParams p) {
 
   __syncwarp();
   if (lane == 0) {
-    store_sprite(g_sprite, pl[0]);
+    store_sprite(e.sprites, pl[0]);
     dr[DQ].aux0 = which_goal; dr[DQ].aux1 = yo ? 1 : 0; dr[DQ].aux2 = in_limbo ? 1 : 0;
     dr[DTELE].aux1 = delay; dr[DTELE].aux2 = countdown;
 #pragma unroll
-    for (int d = 0; d < ND; ++d) store_drape(g_drapes + d * PCL_DRAPE_WORDS, dr[d]);
-    store_carry(g_plot, carry);
-    store_plot<ORDER_ALL>(g_plot, plot, dir);
-    g_plot[PCL_P_AUX0] = timeout; g_plot[PCL_P_AUX1] = tele_frame;
-    g_plot[PCL_P_AUX2] = tele_r; g_plot[PCL_P_AUX3] = tele_c;
+    for (int d = 0; d < ND; ++d) store_drape(e.drapes + d * PCL_DRAPE_WORDS, dr[d]);
+    store_carry(e.plot, carry);
+    store_plot<ORDER_ALL>(e.plot, plot, dir);
+    e.plot[PCL_P_AUX0] = timeout; e.plot[PCL_P_AUX1] = tele_frame;
+    e.plot[PCL_P_AUX2] = tele_r; e.plot[PCL_P_AUX3] = tele_c;
     store_outputs(p.out, env, dir, dir.has_reward ? reward : 0.0);
   }
 
   // ---- render (engine.py:737-759): backdrop, then * # l t r Q P; lane k paints four cells
   uint8_t* board = p.out.d_board + (int64_t)env * H * 16;
-  const uint8_t* backdrop = p.st.d_backdrop + lvl * p.st.backdrop_bstride;
   for (int k = lane; k < H * 4; k += 32) {
     const int r = k >> 2, c0 = (k & 3) << 2;
     uint32_t word = 0;
@@ -319,7 +315,7 @@ t_maze_step(const StepParams p) {
       const int c = c0 + j;
       uint32_t ch = 0;
       if (c < W) {
-        ch = backdrop[r * 16 + c];
+        ch = e.backdrop[r * 16 + c];
         if (visible(pl[0]) && pl[0].row == r && pl[0].col == c) ch = p.sprite_char[0];
         else if ((qrow >> c) & 1u) ch = p.drape_char[DQ];
         else {
