@@ -67,11 +67,13 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       its_showtime()), with the oracle worlds and their outputs keyed by env.
     raised: a dict, to compare the latched error words too.  Each env's word
       (engine.error_codes()) stays 0 while its oracle world raises nothing.  A world
-      whose play() raises IndexError (a NumPy look-up off the board) at step t must find
-      exactly ENV_ERR_INDEX latched after step t; lockstep then sets raised[env] = t and
-      compares that env no further, as the reference's Engine would play no further.
-      The same holds for a world whose its_showtime() raises, at the first launch (t = 0)
-      or at the launch that auto-resets the env."""
+      whose play() raises at step t must find exactly one error latched after step t:
+      ENV_ERR_INDEX for an IndexError (a NumPy look-up off the board),
+      ENV_ERR_EMPTY_CHOICE for a ValueError (np.random.choice of an empty list).
+      lockstep then sets raised[env] = t and compares that env no further, as the
+      reference's Engine would play no further.  The same holds for a world whose
+      its_showtime() raises, at the first launch (t = 0) or at the launch that
+      auto-resets the env."""
   import torch
   env_ids = [int(e) for e in env_ids]
   idx = torch.as_tensor(env_ids, dtype=torch.long, device=engine.device)
@@ -86,10 +88,15 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       return
     try:
       outs[e] = worlds[e].its_showtime()
-    except IndexError:
-      raised[e] = t
+    except (IndexError, ValueError) as exc:
+      latch(e, t, exc)
 
-  worlds, outs = {}, {}
+  def latch(e, t, exc):
+    from pycolab_b200 import _lib
+    raised[e] = t
+    latched[e] = _lib.ENV_ERR_INDEX if isinstance(exc, IndexError) else _lib.ENV_ERR_EMPTY_CHOICE
+
+  worlds, outs, latched = {}, {}, {}
   croppers = None
   if crop is not None:
     crop_spec, crop_state, make_cropper = crop
@@ -104,12 +111,11 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
 
   def check(t):
     if raised is not None:
-      from pycolab_b200 import _lib
       codes = pick(engine.error_codes())
       for k, e in enumerate(env_ids):
         if e in raised and raised[e] < t:
           continue
-        want = _lib.ENV_ERR_INDEX if e in raised else 0
+        want = latched.get(e, 0)
         if int(codes[k]) != want:
           raise Mismatch('error word at step %d env %d: device %#x oracle %#x' % (
               t, e, int(codes[k]), want))
@@ -156,8 +162,8 @@ def lockstep(engine, make_world, env_ids, actions, crop=None, curtains='', sprit
       else:
         try:
           outs[e] = worlds[e].play(int(actions[t, e]))
-        except IndexError:
-          raised[e] = t + 1
+        except (IndexError, ValueError) as exc:
+          latch(e, t + 1, exc)
     compared += check(t + 1)
   return compared
 

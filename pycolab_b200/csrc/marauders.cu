@@ -254,8 +254,8 @@ marauders_step(const StepParams p) {
       const u64 x = __shfl_sync(PCL_FULL, xrow, active ? r : 0);
       if (active) {
         uint4 px = tile4[seg];
-        paint_bits(px, (unsigned)(b >> (sg << 4)) & 0xffffu, 'B');
-        paint_bits(px, (unsigned)(x >> (sg << 4)) & 0xffffu, 'X');
+        paint_bits(px, (unsigned)shr_u64(b, sg << 4) & 0xffffu, 'B');   // 0 past column 64
+        paint_bits(px, (unsigned)shr_u64(x, sg << 4) & 0xffffu, 'X');
         tile4[seg] = px;
       }
       r += dr; sg += dsg;
@@ -273,6 +273,16 @@ marauders_step(const StepParams p) {
   for (int seg = lane; seg < total; seg += 32) dst[seg] = tile4[seg];
 }
 
+// Shared memory of one block (kWarpsPerBlock envs): the static records plus one staged
+// H x pitch tile per warp.
+size_t block_smem(int H, int pitch) {
+  return sizeof(int32_t) * kWarpsPerBlock * kRecWords + (size_t)H * pitch * kWarpsPerBlock;
+}
+
+// The most shared memory, static and dynamic, a block may opt in to on the H100 (227 KB).
+// check_spec accepts a spec only if its block fits, so an accepted spec always launches.
+constexpr size_t kMaxBlockSmem = 227 * 1024;
+
 int check_spec(const pcl_spec& s) {
   if (!chars_are(s.sprite_char, s.n_sprites, "Pabcdyz")) return PCL_ERR_UNSUPPORTED;
   if (!chars_are(s.drape_char, s.n_drapes, "BX")) return PCL_ERR_UNSUPPORTED;
@@ -281,6 +291,7 @@ int check_spec(const pcl_spec& s) {
   if (!groups_are(s, "PBXabcdyz", lens, 1)) return PCL_ERR_UNSUPPORTED;
   if (s.rows > 32 || s.rows < 11 || s.cols > 64 || s.bits_words < 2)
     return PCL_ERR_UNSUPPORTED;
+  if (block_smem(s.rows, s.pitch) > kMaxBlockSmem) return PCL_ERR_UNSUPPORTED;
   for (int i = 0; i < 7; ++i) {
     if (!set_is(s.impassable[i], "")) return PCL_ERR_UNSUPPORTED;
     if (s.sprite_confined[i] != (i == 0) || s.sprite_egocentric[i]) return PCL_ERR_UNSUPPORTED;
@@ -297,7 +308,8 @@ int check_state(const pcl_spec&, const pcl_state& st) {
 
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
   const size_t smem = (size_t)p.H * p.pitch * kWarpsPerBlock;   // one staged tile per warp
-  return launch_step(marauders_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);
+  return launch_step(marauders_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true,
+                     block_smem(p.H, p.pitch) - smem);
 }
 
 }  // namespace

@@ -321,6 +321,14 @@ __device__ __forceinline__ bool bit_at(const uint32_t* row, int c) {
 __device__ __forceinline__ uint32_t spread4(unsigned nib) {
   return ((nib * 0x00204081u) & 0x01010101u) * 0xffu;
 }
+// v >> n for any n, 0 from n = 64 on, so that a segment at or past column 64 of a
+// 64-bit curtain row reads no bits.  C++ leaves such a shift undefined; PTX's shr clamps
+// the shift amount, so this costs nothing over a plain shift.
+__device__ __forceinline__ unsigned long long shr_u64(unsigned long long v, unsigned n) {
+  unsigned long long r;
+  asm("shr.b64 %0, %1, %2;" : "=l"(r) : "l"(v), "r"(n));
+  return r;
+}
 // Paint `ch` into the 16-byte segment `seg` wherever `bits` is set.
 __device__ __forceinline__ void paint_bits(uint4& seg, unsigned bits, uint32_t ch) {
   const uint32_t c4 = ch * 0x01010101u;

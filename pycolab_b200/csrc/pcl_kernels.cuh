@@ -95,9 +95,12 @@ cudaError_t launch_pdl(void (*kern)(Params...), int grid, int block, size_t smem
 
 // A fused step kernel over p.B envs, one warp per env and `warps` envs per block,
 // with `smem` bytes of dynamic shared memory per block; `pdl`: launch_pdl.
+// static_smem: the kernel's static shared memory, which counts toward the same 48 KB a
+// block gets without opting in.
 inline cudaError_t launch_step(void (*kern)(StepParams), const StepParams& p, int warps,
-                               size_t smem, cudaStream_t s, bool pdl = false) {
-  if (smem > 48 * 1024) {   // opt in per launch: the attribute is per device, handles are not
+                               size_t smem, cudaStream_t s, bool pdl = false,
+                               size_t static_smem = 0) {
+  if (smem + static_smem > 48 * 1024) {   // opt in per launch: the attribute is per device, handles are not
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }

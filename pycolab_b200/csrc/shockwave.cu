@@ -126,10 +126,10 @@ shockwave_step(const StepParams p) {
   // ---- render (engine.py:737-759): backdrop, ' ', '^', '@', P
   paint_segments(p.out.d_board + (int64_t)env * H * pitch, e.backdrop, H, pitch, lane,
                  [&](uint4& px, int r, int c0) {
-    const u64 wave_r = s_rows[threadIdx.x >> 5][r];
-    paint_bits(px, (unsigned)((row_bits(danger_bits, r, BW) >> c0) & 0xffffull), p.drape_char[1]);
-    paint_bits(px, (unsigned)((row_bits(safe_bits, r, BW) >> c0) & 0xffffull), p.drape_char[2]);
-    paint_bits(px, (unsigned)((wave_r >> c0) & 0xffffull), p.drape_char[0]);
+    const u64 wave_r = s_rows[threadIdx.x >> 5][r];              // shr_u64: 0 past column 64
+    paint_bits(px, (unsigned)(shr_u64(row_bits(danger_bits, r, BW), c0) & 0xffffull), p.drape_char[1]);
+    paint_bits(px, (unsigned)(shr_u64(row_bits(safe_bits, r, BW), c0) & 0xffffull), p.drape_char[2]);
+    paint_bits(px, (unsigned)(shr_u64(wave_r, c0) & 0xffffull), p.drape_char[0]);
     const unsigned m = sprite_bit(pl, r, c0);
     if (m) paint_bits(px, m, p.sprite_char[0]);
   });

@@ -32,6 +32,10 @@ def lower(engine, roles):
   pl, wave = th[p_ch], th[w_ch]
   if set(pl.impassable) != {'='}:
     raise NotLoweredError("the wave's update() stops at '=': the player must do the same")
+  if '=' not in engine.backdrop.palette:
+    raise NotLoweredError("the wave's update() reads layers['='], which holds only characters "
+                          "of the backdrop: with no '=' in the art the reference raises "
+                          "KeyError at its_showtime()")
   if engine.rows > 32 or engine.cols > 64:
     raise NotLoweredError('shockwave program: boards up to 32 x 64')
   _set_sprites(game, [pl], [_sprite_record(pl)])

@@ -204,6 +204,18 @@ def ref_stock_marauders_art():
   return list(_import()['extraterrestrial_marauders'].GAME_ART)
 
 
+def ref_shockwave(art, width=2):
+  """examples/shockwave.py's make_game on `art`, with a ring `width` cells thick."""
+  _import()
+  from pycolab import ascii_art
+  from pycolab.examples import shockwave as m
+  return ascii_art.ascii_art_to_game(
+      art, what_lies_beneath='+', sprites={'P': m.PlayerSprite},
+      drapes={'@': ascii_art.Partial(m.ShockwaveDrape, width=width),
+              ' ': m.MinimalDrape, '^': m.MinimalDrape},
+      update_schedule=[' ', '^', 'P', '@'], z_order=[' ', '^', '@', 'P'])
+
+
 _NAMES = ('n', 'ne', 'e', 'se', 's', 'sw', 'w', 'nw', 'stay')
 
 

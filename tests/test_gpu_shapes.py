@@ -1,9 +1,9 @@
-"""Step kernels against the oracle at every board shape they branch on.
+"""scrolly_maze_step against the oracle at every board shape it branches on.
 
 scrolly_maze_step lays out shared memory by board shape (segments per row, W against 32
 and 64, H against 32 and 64, pitch against ceil16(W), where the window corner falls in
-a 64-bit word pair); marauders_step and shockwave_step hold one curtain row per lane in
-a 64-bit word, up to 32 x 64.  Each case steps a BatchedEngine with auto-reset beside B
+a 64-bit word pair).  The board shapes of marauders_step and shockwave_step are swept in
+test_gpu_marauders.py and test_gpu_shockwave.py.  Each case steps a BatchedEngine with auto-reset beside B
 oracle worlds and compares, every step, the whole [B, H, pitch] board (pad columns must
 stay 0), rewards, discounts, done flags, curtains, sprite registers and, at the end, the
 error codes.  Several levels and B not a multiple of 4 give a ragged last block whose
@@ -153,30 +153,3 @@ def test_scrolly_attached_cropper_board_shapes(name, pitch, rows, cols, pad):
   def make_crop():
     return em.ScrollingCrop(rows, cols, ['P'], pad_char=pad, scroll_margins=margins)
   _scrolly_case(name, B=7, T=100, pitch=pitch, crop=(spec, make_crop))
-
-
-@pytest.mark.parametrize('rows,cols', [(32, 64), (32, 39), (16, 64), (20, 63)])
-def test_marauders_board_shapes(rows, cols):
-  """One 64-bit curtain row per lane up to 32 x 64: the W == 64 mask, wraps by W - 1 and
-  the row roll over all 32 lanes."""
-  from pycolab_b200 import levels
-  from pycolab_b200.games import extraterrestrial_marauders as marauders
-  art = levels.marauders_level(rows, cols)
-  B = 10
-  actions = np.random.RandomState(rows + cols).randint(0, 4, size=(150, B))
-  rngs = [np.random.RandomState(900 + e) for e in range(B)]
-  _step_vs_oracle([marauders.make_game(art)], lambda e: ogames.make_marauders(art, rngs[e]),
-                  actions, 'BX', 'P', rng_seed=900)
-
-
-@pytest.mark.parametrize('rows,cols', [(32, 64), (31, 33), (32, 15)])
-def test_shockwave_board_shapes(rows, cols):
-  """Shockwave up to 32 x 64 (H * W = 2048, a power of two)."""
-  from pycolab_b200 import levels
-  from pycolab_b200.games import shockwave
-  art = levels.shockwave_level(rows + cols, rows, cols, 0.5)
-  B = 10
-  actions = np.random.RandomState(rows * cols).choice(5, size=(150, B), p=[.55, .15, .15, .1, .05])
-  rngs = [np.random.RandomState(700 + e) for e in range(B)]
-  _step_vs_oracle([shockwave.make_game(art)], lambda e: ogames.make_shockwave(art, rngs[e]),
-                  actions, '@', 'P', rng_seed=700)

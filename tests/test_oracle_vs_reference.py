@@ -410,47 +410,6 @@ def test_scrolly_maze_board_shapes(name):
               lambda: ss.oracle_world(maze, board, beneath, margins), actions)
 
 
-@pytest.mark.parametrize('rows,cols', [(32, 64), (32, 39), (16, 64), (20, 63)])
-def test_marauders_board_shapes(rows, cols):
-  """Marauders up to the 32 x 64 the kernel accepts (one 64-bit curtain row per lane)."""
-  art = levels.marauders_level(rows, cols)
-  rs = np.random.RandomState(rows * 100 + cols)
-  actions = rs.randint(0, 4, size=800).tolist()
-  np.random.seed(cols)
-  rng = np.random.RandomState(cols)
-  _lockstep(lambda: refdriver.ref_marauders(art), lambda: games.make_marauders(art, rng), actions)
-
-
-@pytest.mark.parametrize('rows,cols', [(32, 64), (31, 33), (32, 15)])
-def test_shockwave_board_shapes(rows, cols):
-  """Shockwave on generated levels up to 32 x 64 (H * W = 2048 is a power of two)."""
-  refdriver._import()
-  from pycolab.examples import shockwave as ref_shock
-  art = levels.shockwave_level(rows + cols, rows, cols, 0.5)
-  ref_shock.LEVELS.append(art)
-  steps = 0
-  try:
-    for seed in range(12):
-      np.random.seed(seed)
-      ref = ref_shock.make_game(len(ref_shock.LEVELS) - 1)
-      ora = games.make_shockwave(art, np.random.RandomState(seed))
-      r_out, o_out = ref.its_showtime(), ora.its_showtime()
-      rs = np.random.RandomState(200 + seed)
-      for _ in range(150):
-        np.testing.assert_array_equal(r_out[0].board, o_out[0])
-        np.testing.assert_array_equal(ref.things['@'].curtain, ora.things['@'].curtain)
-        assert r_out[1] == o_out[1] and type(r_out[1]) is type(o_out[1])
-        assert r_out[2] == o_out[2] and ref.game_over == ora.game_over
-        if ref.game_over:
-          break
-        a = int(rs.choice([0, 1, 2, 3, 4], p=[.55, .15, .15, .1, .05]))
-        r_out, o_out = ref.play(a), ora.play(a)
-        steps += 1
-  finally:
-    ref_shock.LEVELS.pop()
-  assert steps > 100
-
-
 # ----------------------------------------------- un-occluded layers, hand-built
 
 class _Thing(object):

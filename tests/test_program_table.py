@@ -13,12 +13,12 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden',
                       'boundary_statuses.json')
 
 
-def test_every_boundary_status_of_the_lowered_levels():
-  """The statuses of the golden file, case for case.  Among them, warehouse and
-  better_scrolly refuse a board whose block of four staged backdrop tiles (and, for
-  better_scrolly, coin bit rows) would exceed the 227 KB of shared memory a block can
-  opt in to (rows or pitch 32768, or better_scrolly's bits_words 32768): such a spec
-  could never launch."""
+def test_boundary_statuses_of_the_lowered_levels_and_their_refusals():
+  """The statuses of the golden file, case for case.  Among them, warehouse,
+  better_scrolly and marauders refuse a board whose block of four staged backdrop tiles
+  (and, for better_scrolly, coin bit rows; for marauders, its static records) would
+  exceed the 227 KB of shared memory a block can opt in to (rows or pitch 32768, or
+  better_scrolly's bits_words 32768): such a spec could never launch."""
   with open(GOLDEN) as f:
     encoded = json.load(f)
   got = boundary_sweep.sweep()
@@ -33,7 +33,7 @@ def test_every_boundary_status_of_the_lowered_levels():
     assert want[level + '/create'] == want[level + '/bind'] == _lib.OK, level
   for case in ('warehouse/spec.rows=32768', 'warehouse/spec.pitch=32768',
                'better_scrolly/spec.rows=32768', 'better_scrolly/spec.pitch=32768',
-               'better_scrolly/spec.bits_words=32768'):
+               'better_scrolly/spec.bits_words=32768', 'marauders/spec.pitch=32768'):
     assert want[case] == got[case] == _lib.ERR_UNSUPPORTED, case
   programs = set(spec.program for _, spec in boundary_sweep.lowered_specs())
   assert programs == set(range(1, 13))

@@ -2,8 +2,9 @@
 fire around `np.random.randint` impact points whose update() reads the STALE board.
 Goldens are the reference's own trajectories (tests/golden/shockwave_*: the stock level
 and generated ones, policy-driven so that some episodes are won), replayed in
-test_example_goldens.py and test_gpu_example_goldens.py; here a batched lock-step with
-per-env generators, and lowering."""
+test_example_goldens.py and test_gpu_example_goldens.py.  Here: lowering, and the oracle
+in lock-step with the live reference on the scripted rim cases (shockwave_cases.RIM) and
+on open levels at every width and board shape the GPU sweep steps."""
 
 import os
 
@@ -12,38 +13,16 @@ import pytest
 
 import golden_cases as gc
 import refdriver
+import shockwave_cases as sc
 from oracle import games as ogames
-from oracle import sampled_check
+from test_oracle_vs_reference import _lockstep
+
+needs_ref = pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
 
 
 @pytest.mark.parametrize('name', gc.names('shockwave_'))
 def test_goldens_hold_a_win(name):
   assert int((gc.load(name)['reward'] == 1).sum()) >= 1          # the safe-zone path
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('shape', [(12, 15), (32, 64), (9, 33)])
-def test_batched_shockwave_vs_oracle(shape):
-  """Auto-resetting batch over several generated levels, one NumPy generator per env
-  (RandomState(seed + e)), boards / curtains / rewards / discounts every step."""
-  from pycolab_b200 import batched, levels
-  from pycolab_b200.games import shockwave
-  arts = [levels.shockwave_level(30 + i, shape[0], shape[1], 0.45) for i in range(3)]
-  B, T, seed = 13, 220, 9
-  eng = batched.BatchedEngine([shockwave.make_game(a) for a in arts], batch=B, rng_seed=seed)
-  rngs = [np.random.RandomState(seed + e) for e in range(B)]
-  eng.its_showtime()
-  rs = np.random.RandomState(4)
-  actions = np.stack([rs.choice([0, 1, 2, 3, 4], size=B, p=[.6, .12, .12, .12, .04])
-                      for _ in range(T)]).astype(np.int32)
-  episodes = [0]
-
-  def count(t, eng, worlds, outs):
-    episodes[0] += sum(w.game_over for w in worlds.values()) if t < T else 0
-  sampled_check.lockstep(eng, lambda e: ogames.make_shockwave(arts[e % len(arts)], rngs[e]),
-                         range(B), actions, curtains='@', on_step=count)
-  assert episodes[0] > B
-  assert int(eng.error_codes().abs().max()) == 0
 
 
 def test_shockwave_lowers_and_validates_on_cpu():
@@ -83,3 +62,93 @@ def test_reference_shockwave_file_lowers_like_the_twin():
   finally:
     compat.uninstall()
     sys.modules.update(saved)
+
+
+def test_a_level_without_walls_is_not_lowered():
+  """The wave's update() reads layers['='], and layers holds only the characters on the
+  board: the reference raises KeyError at its_showtime() on a level with no '='.  Such a
+  level is refused, with the reason."""
+  from pycolab_b200 import errors, lowering
+  from pycolab_b200.games import shockwave
+  art = ['^^^^^', '     ', '  P  ']
+  with pytest.raises(errors.NotLoweredError, match="KeyError"):
+    lowering.lower(shockwave.make_game(art))
+  with pytest.raises(KeyError):
+    ogames.make_shockwave(art, np.random.RandomState(0)).its_showtime()
+  lowering.lower(shockwave.make_game(['^^^^^', '  =  ', '  P  ']))
+
+
+@needs_ref
+def test_reference_raises_on_a_level_without_walls():
+  with pytest.raises(KeyError):
+    refdriver.ref_shockwave(['^^^^^', '     ', '  P  ']).its_showtime()
+
+
+# ------------------------------------------------- the oracle against the reference
+
+def _wave(ref, ora, t):
+  """The ring's curtain and its step count."""
+  np.testing.assert_array_equal(ref.things['@'].curtain, ora.things['@'].curtain,
+                                err_msg='t=%d' % t)
+  assert ref.things['@']._steps_since_impact == ora.things['@'].aux['steps'], t
+
+
+def _pair(art, width, seed):
+  """A reference game and an oracle world drawing from one MT19937 stream: NumPy's global
+  generator and RandomState(seed), each seeded here once for all episodes."""
+  np.random.seed(seed)
+  rng = np.random.RandomState(seed)
+  return (lambda: refdriver.ref_shockwave(art, width)), (lambda: sc.make_world(art, rng, width))
+
+
+@needs_ref
+@pytest.mark.parametrize('name', sorted(sc.RIM))
+def test_rim_case_oracle_vs_reference(name):
+  """Boards, rewards, discounts, game over, P's position and the ring, at every step of
+  the scripted case and of 40 more steps of random play."""
+  art, width, seed, script, edges = sc.RIM[name]
+  actions = script + sc.random_actions(np.random.RandomState(len(name)), 40, 1)[:, 0].tolist()
+  _lockstep(*_pair(art, width, seed), actions, check=_wave)
+  seen, _ = sc.oracle_run(art, width, script, seed)
+  assert edges <= seen, (name, sorted(edges - seen))
+
+
+@needs_ref
+@pytest.mark.parametrize('shape', sc.SHAPES, ids=['%dx%d' % s for s in sc.SHAPES])
+def test_open_levels_oracle_vs_reference(shape):
+  """Open levels of every shape the GPU sweep steps, at every width, the first impact on
+  each corner and side of the board in turn."""
+  cells = sc.rim_cells(shape)
+  restarts = 0
+  for i, width in enumerate(sc.WIDTHS):
+    art = sc.sweep_level(shape, i)
+    seed = sc.impact_seed(shape, cells[i % len(cells)])
+    actions = sc.random_actions(np.random.RandomState(i), 80, 1)[:, 0].tolist()
+    restarts += _lockstep(*_pair(art, width, seed), actions, check=_wave)
+  assert restarts > 0 or shape[0] * shape[1] == 2     # P and a wall: no episode ends
+
+
+@needs_ref
+@pytest.mark.parametrize('rows,cols', [(32, 64), (31, 33), (32, 15)])
+def test_generated_level_board_shapes(rows, cols):
+  """Generated levels up to 32 x 64 (H * W = 2048 is a power of two)."""
+  from pycolab_b200 import levels
+  art = levels.shockwave_level(rows + cols, rows, cols, 0.5)
+  steps = 0
+  for seed in range(12):
+    np.random.seed(seed)
+    ref = refdriver.ref_shockwave(art)
+    ora = ogames.make_shockwave(art, np.random.RandomState(seed))
+    r_out, o_out = ref.its_showtime(), ora.its_showtime()
+    rs = np.random.RandomState(200 + seed)
+    for _ in range(150):
+      np.testing.assert_array_equal(r_out[0].board, o_out[0])
+      np.testing.assert_array_equal(ref.things['@'].curtain, ora.things['@'].curtain)
+      assert r_out[1] == o_out[1] and type(r_out[1]) is type(o_out[1])
+      assert r_out[2] == o_out[2] and ref.game_over == ora.game_over
+      if ref.game_over:
+        break
+      a = int(rs.choice([0, 1, 2, 3, 4], p=[.55, .15, .15, .1, .05]))
+      r_out, o_out = ref.play(a), ora.play(a)
+      steps += 1
+  assert steps > 100
