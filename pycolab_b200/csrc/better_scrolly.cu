@@ -200,11 +200,6 @@ size_t block_smem(int H, int pitch, int BW) {
   return (kRecWords * 4 + (size_t)H * pitch + bits_bytes) * kWarpsPerBlock;
 }
 
-// The most dynamic shared memory a block may ask for on the H100 (227 KB; the kernel
-// has no static shared memory).  check_spec accepts a spec only if its block fits,
-// so an accepted spec always launches.
-constexpr size_t kMaxBlockSmem = 227 * 1024;
-
 int check_spec(const pcl_spec& s) {
   if (!chars_are(s.sprite_char, s.n_sprites, "Pabc")) return PCL_ERR_UNSUPPORTED;
   if (!chars_are(s.drape_char, s.n_drapes, "@")) return PCL_ERR_UNSUPPORTED;

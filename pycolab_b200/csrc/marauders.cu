@@ -279,10 +279,6 @@ size_t block_smem(int H, int pitch) {
   return sizeof(int32_t) * kWarpsPerBlock * kRecWords + (size_t)H * pitch * kWarpsPerBlock;
 }
 
-// The most shared memory, static and dynamic, a block may opt in to on the H100 (227 KB).
-// check_spec accepts a spec only if its block fits, so an accepted spec always launches.
-constexpr size_t kMaxBlockSmem = 227 * 1024;
-
 int check_spec(const pcl_spec& s) {
   if (!chars_are(s.sprite_char, s.n_sprites, "Pabcdyz")) return PCL_ERR_UNSUPPORTED;
   if (!chars_are(s.drape_char, s.n_drapes, "BX")) return PCL_ERR_UNSUPPORTED;

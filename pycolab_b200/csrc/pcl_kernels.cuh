@@ -93,6 +93,11 @@ cudaError_t launch_pdl(void (*kern)(Params...), int grid, int block, size_t smem
   return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
+// The most shared memory, static and dynamic, one block may opt in to on the H100
+// (227 KB).  A program whose block grows with the board refuses, in check_spec, a spec
+// whose block would not fit, so an accepted spec always launches.
+constexpr size_t kMaxBlockSmem = 227 * 1024;
+
 // A fused step kernel over p.B envs, one warp per env and `warps` envs per block,
 // with `smem` bytes of dynamic shared memory per block; `pdl`: launch_pdl.
 // static_smem: the kernel's static shared memory, which counts toward the same 48 KB a

@@ -328,10 +328,10 @@ __device__ __forceinline__ void stamp(int k, uint32_t v) {
 #define PCL_STAMP_PATH(v) do {} while (0)
 #endif
 
-// The most dynamic shared memory a block may ask for on the H100: 227 KB per block less
-// the kernel's 2 KB of static selector tables.  check_spec accepts a spec only if its
-// block fits, so an accepted spec always launches.
-constexpr size_t kMaxBlockSmem = 227 * 1024 - 2048;
+// The most dynamic shared memory a block may ask for: the block budget less the kernel's
+// 2 KB of static selector tables.  check_spec accepts a spec only if its block fits, so
+// an accepted spec always launches.
+constexpr size_t kMaxDynamicSmem = kMaxBlockSmem - kWarpsPerBlock * sizeof(SelTable);
 
 // 8 blocks per SM (__launch_bounds__ below) on a 64x64 board: a block's dynamic shared
 // memory, its per-warp selector tables and the 1 KB the SM reserves per block fit 8 times
@@ -341,8 +341,8 @@ static_assert(8 * (kWarpsPerBlock * (warp_smem_bytes(64, 64, 64) + sizeof(SelTab
               "a 64x64 scrolly_maze block no longer fits 8 times per SM");
 static_assert(warp_smem_bytes(1, 1, 16) == kRecWords * 4 + kNbWords * 4,
               "delta rendering's scratch must fit a warp's region on the smallest board");
-static_assert(kMaxBlockSmem + kWarpsPerBlock * sizeof(SelTable) == 227 * 1024,
-              "kMaxBlockSmem must leave room for the static selector tables");
+static_assert(kMaxDynamicSmem == kMaxBlockSmem - 2048,
+              "kMaxDynamicSmem must leave room for the static selector tables");
 
 // 3x3 "blocked" mask (bit (dr+1)*3 + dc+1, sprites.py:495-507) around the virtual
 // position (vrow, vcol) of a walker whose 5x5 wall patch `field` is centred on
@@ -1092,7 +1092,7 @@ int check_spec(const pcl_spec& s) {
     if ((s.pattern_words & 1) || s.pattern_words < (((s.pattern_cols - s.cols) >> 5) & ~1) + nw ||
         s.pattern_words < (s.pattern_cols + 31) / 32 + 1) return PCL_ERR_INVALID;
     // one CTA (4 envs) stages tile + windows in shared memory: the launcher's own size
-    if (block_smem(s.rows, s.cols, s.pitch) > kMaxBlockSmem) return PCL_ERR_UNSUPPORTED;
+    if (block_smem(s.rows, s.cols, s.pitch) > kMaxDynamicSmem) return PCL_ERR_UNSUPPORTED;
   }
   for (int d = 0; d < 2; ++d)
     if (!margins_fit(s, d)) return PCL_ERR_INVALID;
@@ -1113,7 +1113,7 @@ CurtainAt curtain(const pcl_spec&, int d) {
 cudaError_t launch(const StepParams& p, cudaStream_t s) {
   if (p.PWW & 1) return cudaErrorInvalidValue;   // window rows are staged in 8-byte halves
   const size_t smem = block_smem(p.H, p.W, p.pitch);
-  if (smem > kMaxBlockSmem) return cudaErrorInvalidValue;   // board too large for one CTA
+  if (smem > kMaxDynamicSmem) return cudaErrorInvalidValue;   // board too large for one CTA
   // Programmatic dependent launch: this kernel may start (prologue only) before
   // the previous kernel of the stream has drained.
   return launch_step(scrolly_maze_step, p, kWarpsPerBlock, smem, s, /*pdl=*/true);

@@ -243,11 +243,6 @@ size_t block_smem(int H, int pitch) {
   return (kRecWords * 4 + (size_t)H * pitch) * kWarpsPerBlock;
 }
 
-// The most dynamic shared memory a block may ask for on the H100 (227 KB; the kernel
-// has no static shared memory).  check_spec accepts a spec only if its block fits,
-// so an accepted spec always launches.
-constexpr size_t kMaxBlockSmem = 227 * 1024;
-
 int check_spec(const pcl_spec& s) {
   const int nb = s.n_sprites - 1;
   if (nb < 1 || nb > 10) return PCL_ERR_UNSUPPORTED;

@@ -20,12 +20,9 @@ The levels here have floor up to the edge:
 import numpy as np
 
 from oracle import games as ogames
+from rim_sweep import MAX_BLOCK_SMEM, repitch
 
 PATROLLERS = 'abc'
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def open_level(seed, shape, n_coins, wall_density=0.08, fence=True):
@@ -62,12 +59,7 @@ def lowered(art, pitch=None):
   """The lowered facade game of `art`, its backdrop re-padded to `pitch` columns."""
   from pycolab_b200 import lowering
   from pycolab_b200.games import better_scrolly_maze
-  low = lowering.lower(better_scrolly_maze.make_game(art))
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
-  return low
+  return repitch(lowering.lower(better_scrolly_maze.make_game(art)), pitch)
 
 
 def make_world(art):
@@ -175,7 +167,7 @@ class Edges(object):
       self.seen.add('showtime_over')
     self._now(world, out)
 
-  def step(self, world, out):
+  def step(self, world, out, action):
     now = _snapshot(world)
     H, W = world.rows, world.cols
     prev = self.prev
@@ -221,40 +213,12 @@ class Edges(object):
       self.seen.add('shared_cell')
 
 
-def oracle_run(art, actions):
-  """Play `actions` on oracle worlds with auto-reset.  Returns (edges seen, restarts, the
-  step whose action raised IndexError or None; -1 if its_showtime raised)."""
-  edges = Edges()
-  world = make_world(art)
-  try:
-    out = world.its_showtime()
-  except IndexError:
-    edges.seen.add('raise')
-    return edges.seen, 0, -1
-  edges.start(world, out)
-  restarts = 0
-  for t, a in enumerate(actions):
-    if world.game_over:
-      restarts += 1
-      world = make_world(art)
-      edges.start(world, world.its_showtime())
-      continue
-    try:
-      out = world.play(int(a))
-    except IndexError:
-      edges.seen.add('raise')
-      return edges.seen, restarts, t
-    edges.step(world, out)
-  return edges.seen, restarts, None
-
-
 # ------------------------------------- the step kernel's shared-memory reads (render)
 
 # Mirrors better_scrolly.cu (block_smem, the per-warp layout and the render loop) and
 # the checks pcl_create applies to a better_scrolly spec.
 REC_WORDS = 64
 WARPS_PER_BLOCK = 4
-MAX_BLOCK_SMEM = 227 * 1024            # H100: the dynamic shared memory a block may opt in to
 
 
 def min_bits_words(W):

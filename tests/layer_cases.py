@@ -27,9 +27,7 @@ import collections
 import numpy as np
 
 import scrolly_shapes as ss
-
-SHARED, POOL, PER_ENV = 'shared', 'pool', 'per_env'
-BATCHES = (1, 5, 37)
+from rim_sweep import BATCHES, PER_ENV, POOL, SHARED, ceil16
 
 # build() -> Built.  games: lowered games (env e plays games[e % len(games)]);
 # make_world(e): a fresh oracle world for env e; draw(rs, T, B): int actions [T, B];
@@ -42,10 +40,6 @@ STEPS = 12
 def _batch(i, binding):
   B = BATCHES[i % len(BATCHES)]
   return max(B, 5) if binding == POOL else B
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def pitches(W):

@@ -20,15 +20,12 @@ rows 11-13 and P on the last row, so nothing there reaches the board's rim.  Her
 import numpy as np
 
 from oracle import games as ogames
+from rim_sweep import repitch
 
 UP = 'abcd'
 DOWN = 'yz'
 BOLTS = UP + DOWN
 SPRITES = 'P' + BOLTS
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def board(shape, cells):
@@ -90,12 +87,7 @@ def lowered(art, pitch=None):
   """The lowered facade game of `art`, its backdrop re-padded to `pitch` columns."""
   from pycolab_b200 import lowering
   from pycolab_b200.games import extraterrestrial_marauders as marauders
-  low = lowering.lower(marauders.make_game(art))
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
-  return low
+  return repitch(lowering.lower(marauders.make_game(art)), pitch)
 
 
 def make_world(art, rng):
@@ -296,42 +288,20 @@ class Edges(object):
     self.prev = now
     self._now(world, now)
 
+  def on_raise(self, world):
+    """play() raised ValueError: which way no column came to show an 'X'."""
+    self.seen.add('raise_hidden' if world.things['X'].curtain.any() else 'raise_last_hit')
+
   def _now(self, world, snap):
     X = snap['X']
     if world.cols > 1 and X[:, 0].any() and X[:, -1].any():
       self.seen.add('both_sides')
 
 
-def oracle_run(art, actions, seed=0):
-  """Play `actions` on oracle worlds with auto-reset, one generator RandomState(seed)
-  across the episodes.  Returns (edges seen, restarts, the step whose action raised
-  ValueError or None)."""
-  rng = np.random.RandomState(seed)
-  edges = Edges()
-  world = make_world(art, rng)
-  edges.start(world, world.its_showtime())
-  restarts = 0
-  for t, a in enumerate(actions):
-    if world.game_over:
-      restarts += 1
-      world = make_world(art, rng)
-      edges.start(world, world.its_showtime())
-      continue
-    try:
-      out = world.play(int(a))
-    except ValueError:
-      edges.seen.add('raise')
-      edges.seen.add('raise_hidden' if world.things['X'].curtain.any() else 'raise_last_hit')
-      return edges.seen, restarts, t
-    edges.step(world, out, int(a))
-  return edges.seen, restarts, None
-
-
 # ------------------------------------------------ the block's shared memory
 # Mirrors marauders.cu (s_rec, launch) and the bound pcl_create applies.
 WARPS_PER_BLOCK = 4
 STATIC_SMEM = WARPS_PER_BLOCK * 96 * 4      # s_rec: 96 record words per warp
-MAX_BLOCK_SMEM = 227 * 1024                 # H100: what a block may opt in to, static included
 
 
 def block_smem(H, pitch):

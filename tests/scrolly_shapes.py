@@ -11,6 +11,7 @@ scroll margins, and a Python model of the kernel's per-warp shared-memory layout
 import numpy as np
 
 from oracle import games as ogames
+from rim_sweep import MAX_BLOCK_SMEM, ceil16, repitch
 
 
 def open_level(seed, board_shape, world_shape, corner=None, wall_density=0.12,
@@ -107,11 +108,7 @@ def lowered(game, pitch=None, repack=False):
   """Lower a facade game; optionally widen its pitch (re-padding the backdrop) or re-pack
   its patterns at the smallest pattern_words pcl_create accepts."""
   from pycolab_b200 import lowering
-  low = lowering.lower(game)
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
+  low = repitch(lowering.lower(game), pitch)
   if repack:
     words = min_pattern_words(low.cols, low.pattern_cols)
     low.patterns = {d: lowering.pack_rows(lowering.unpack_rows(p, low.pattern_cols), words)
@@ -132,15 +129,10 @@ def oracle_world(maze, board, beneath, margins=DEFAULT_MARGINS):
 REC_WORDS = 64
 WARPS_PER_BLOCK = 4
 SEL_TABLE_BYTES = 512                  # one u16[256] selector table per warp (static)
-MAX_BLOCK_SMEM = 227 * 1024            # H100: shared memory one block may opt in to
 
 
 def window_words(W):
   return 4 if W < 2 else 2 * ((63 + W + 63) // 64)
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def warp_smem_bytes(H, W, pitch):

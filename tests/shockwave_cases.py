@@ -18,12 +18,9 @@ and walls on interior rows; here '^', ' ', '+' and '=' go anywhere:
 import numpy as np
 
 from oracle import games as ogames
+from rim_sweep import repitch
 
 ACTIONS = 5        # 0 north, 1 west, 2 east, 3 _stay(), 4 no call
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def open_level(seed, shape, walls=0.15, safe=0.2, bunkers=0.2, p_cell=None):
@@ -82,12 +79,7 @@ def make_game(art, width=2):
 def lowered(art, width=2, pitch=None):
   """The lowered facade game of `art`, its backdrop re-padded to `pitch` columns."""
   from pycolab_b200 import lowering
-  low = lowering.lower(make_game(art, width))
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
-  return low
+  return repitch(lowering.lower(make_game(art, width)), pitch)
 
 
 def make_world(art, rng, width=2):
@@ -254,21 +246,3 @@ class Edges(object):
     if all(sides.values()):
       self.seen.add('clip_all')
 
-
-def oracle_run(art, width, actions, seed):
-  """Play `actions` on oracle worlds with auto-reset, one generator RandomState(seed)
-  across the episodes.  Returns (edges seen, restarts)."""
-  rng = np.random.RandomState(seed)
-  edges = Edges()
-  world = make_world(art, rng, width)
-  edges.start(world, world.its_showtime())
-  restarts = 0
-  for a in actions:
-    if world.game_over:
-      restarts += 1
-      world = make_world(art, rng, width)
-      edges.start(world, world.its_showtime())
-      continue
-    out = world.play(int(a))
-    edges.step(world, out, int(a))
-  return edges.seen, restarts

@@ -7,13 +7,12 @@ last column, walkers meeting at (0, 0), coins collected from off the board, and 
 look-ups that raise IndexError; then random play on open levels.  Then the model of the
 step kernel's shared-memory reads, and pcl_create's bound on the block's shared memory."""
 
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import better_scrolly_cases as bc
 import refdriver
+import rim_sweep as rsw
 import trajectory as tj
 from oracle import sampled_check
 from pycolab_b200 import _lib
@@ -35,23 +34,18 @@ def _walkers(ref, ora, t):
       assert bool(ent._moving_east) == w.aux['moving_east'], (t, ch)
 
 
-def _script(name):
-  """The case's script, a quit, and the script again from a fresh episode."""
-  script = bc.RIM[name][1]
-  return script + [5] + script
-
-
 @needs_ref
 @pytest.mark.parametrize('name', STEADY)
 def test_rim_case_oracle_vs_reference(name):
   """Boards, rewards, discounts, game over, and every walker's position, visibility,
   virtual position and direction, at every step of the scripted case and of its replay
   after a quit."""
-  art, _, edges = bc.RIM[name]
-  actions = _script(name)
+  art, script, edges = bc.RIM[name]
+  actions = rsw.twice(script, 5)
   _lockstep(lambda: refdriver.ref_better_scrolly(art), lambda: bc.make_world(art), actions,
             check=_walkers)
-  seen, restarts, raised = bc.oracle_run(art, actions)
+  seen, restarts, raised = rsw.oracle_run(lambda: bc.make_world(art), bc.Edges(), actions,
+                                          IndexError)
   assert raised is None
   assert edges <= seen, (name, sorted(edges - seen))
   assert restarts >= 1
@@ -103,7 +97,8 @@ def test_open_levels_oracle_vs_reference(n_coins, fence):
   for seed in range(4):
     art = bc.open_level(seed, (6, 9), n_coins, fence=fence)
     actions = bc.random_actions(np.random.RandomState(seed), 300, 1)[:, 0].tolist()
-    seen, n, raised = bc.oracle_run(art, actions)
+    seen, n, raised = rsw.oracle_run(lambda: bc.make_world(art), bc.Edges(), actions,
+                                     IndexError)
     seen_any |= seen
     restarts += n
     assert raised != -1, art                  # no patroller starts in the last column
@@ -129,7 +124,7 @@ def _shapes():
   largest board pcl_create accepts at that pitch."""
   for W in range(1, 257):
     for extra in range(0, 161, 16):
-      pitch = bc.ceil16(W) + extra
+      pitch = rsw.ceil16(W) + extra
       for BW in (bc.min_bits_words(W), bc.min_bits_words(W) + 1):
         for H in sorted({1, 2, 3, bc.largest_rows(W, pitch, BW)} - {0}):
           if bc.accepted(H, W, pitch, BW):
@@ -165,21 +160,9 @@ def test_unbounded_coin_reads_leave_their_row_past_32_bw_columns():
 LARGEST = (226, 224)              # 4 * (256 + 226 * 224 + 226 * 8 * 4) = 227 KB exactly
 
 
-def _spec(H, W, pitch):
-  game = bc.lowered(bc.RIM['stacked'][0])
-  spec = game.make_spec(auto_reset=True)
-  spec.rows, spec.cols, spec.pitch = H, W, pitch
-  spec.bits_words = bc.min_bits_words(W)
-  return spec
-
-
-def _create(spec):
-  lib = _lib.load()
-  h = C.c_void_p()
-  status = lib.pcl_create(C.byref(spec), 4, -1, C.byref(h))   # device -1: no CUDA call
-  if status == _lib.OK:
-    lib.pcl_destroy(h)
-  return status
+def _status(H, W, pitch):
+  return rsw.create_status(bc.lowered(bc.RIM['stacked'][0]), 4, rows=H, cols=W, pitch=pitch,
+                           bits_words=bc.min_bits_words(W))
 
 
 @pytest.mark.parametrize('W', [4, 16, 30, 64, 89, 128, 224, 1000])
@@ -189,18 +172,10 @@ def test_largest_accepted_better_scrolly_board_is_launchable(W, extra):
   accepts, the block (4 warps, each staging 256 bytes of records, the H x pitch tile and
   H bit rows of BW words) fits the 227 KB a block can opt in to; one row more is
   refused."""
-  pitch = bc.ceil16(W) + extra
+  pitch = rsw.ceil16(W) + extra
   BW = bc.min_bits_words(W)
-  lo, hi = 1, 8192
-  assert _create(_spec(lo, W, pitch)) == _lib.OK
-  assert _create(_spec(hi, W, pitch)) == _lib.ERR_UNSUPPORTED
-  while hi - lo > 1:
-    mid = (lo + hi) // 2
-    if _create(_spec(mid, W, pitch)) == _lib.OK:
-      lo = mid
-    else:
-      hi = mid
-  assert bc.block_smem(lo, pitch, BW) <= bc.MAX_BLOCK_SMEM < bc.block_smem(lo + 1, pitch, BW)
+  lo = rsw.largest_accepted(lambda H: _status(H, W, pitch), 1, 8192)
+  assert bc.block_smem(lo, pitch, BW) <= rsw.MAX_BLOCK_SMEM < bc.block_smem(lo + 1, pitch, BW)
   assert bc.accepted(lo, W, pitch) and not bc.accepted(lo + 1, W, pitch)
 
 
@@ -209,8 +184,8 @@ def test_better_scrolly_bound_at_known_sizes():
   under 6 KB per block, and a block needs more than the 48 KB default only from about
   96 x 128 up."""
   H, W = LARGEST
-  assert bc.block_smem(H, W, bc.min_bits_words(W)) == bc.MAX_BLOCK_SMEM
-  assert _create(_spec(H, W, W)) == _lib.OK
-  assert _create(_spec(H + 1, W, W)) == _lib.ERR_UNSUPPORTED
+  assert bc.block_smem(H, W, bc.min_bits_words(W)) == rsw.MAX_BLOCK_SMEM
+  assert _status(H, W, W) == _lib.OK
+  assert _status(H + 1, W, W) == _lib.ERR_UNSUPPORTED
   assert bc.block_smem(29, 32, 2) < 48 * 1024 < bc.block_smem(96, 128, 5)
   assert bc.block_smem(64, 80, 4) < 48 * 1024

@@ -14,19 +14,18 @@ import numpy as np
 import pytest
 
 import better_scrolly_cases as bc
-from oracle import sampled_check
+import rim_sweep as rsw
 
 pytestmark = pytest.mark.gpu
 
 T = 60
-SHARED, POOL, PER_ENV = 'shared', 'pool', 'per_env'
-BINDINGS = (SHARED, POOL, PER_ENV)
-BATCHES = (1, 5, 37)
 COINS = (0, 1, 6, 40)
 # The largest board pcl_create accepts at its own pitch: 4 * (256 + H*pitch + H*BW*4)
 # is exactly 227 KB.  96 x 128 is past the 48 KB a block gets without opting in.
 LARGEST = (226, 224)
 SHAPES = [(2, 4), (1, 16), (5, 17), (29, 30), (33, 64), (45, 89), (64, 65), (96, 128), LARGEST]
+# What every run compares, and the edges it tracks.
+LOCKSTEP = dict(curtains='@', sprites='Pabc', make_edges=bc.Edges)
 
 
 def _cases():
@@ -34,58 +33,18 @@ def _cases():
   them so that each value of every axis meets several of the others.  The largest board
   runs at its own pitch only, with 5 envs."""
   out = []
-  for i, shape in enumerate(SHAPES):
-    extras = (0,) if shape == LARGEST else (0, 16, 64)
-    for j, extra in enumerate(extras):
-      k = 3 * i + j
-      coins = min(COINS[k % 4], shape[0] * shape[1] - 5)
-      binding = BINDINGS[(i + 2 * j) % 3]
-      B = 5 if shape == LARGEST else BATCHES[(k // 2) % 3]
-      out.append(('%dx%d_p%d_%s_%dc_B%d' % (shape + (bc.ceil16(shape[1]) + extra, binding,
-                                                      coins, B)),
-                  shape, extra, coins, binding, B))
+  for i, j, k, shape, pitch, binding, B in rsw.rotate(SHAPES):
+    if shape == LARGEST:
+      if j:
+        continue
+      B = 5
+    coins = min(COINS[k % 4], shape[0] * shape[1] - 5)
+    out.append(('%dx%d_p%d_%s_%dc_B%d' % (shape + (pitch, binding, coins, B)),
+                shape, pitch - rsw.ceil16(shape[1]), coins, binding, B))
   return out
 
 
 CASES = _cases()
-
-
-class _Track(object):
-  """on_step hook: the edges each sampled env's oracle world went through, and the
-  number of restarts."""
-
-  def __init__(self, raised):
-    self.raised = raised
-    self.edges, self.worlds, self.restarts = {}, {}, 0
-
-  def __call__(self, t, engine, worlds, outs):
-    for e, w in worlds.items():
-      if e in self.raised:
-        continue
-      if self.worlds.get(e) is not w:
-        self.edges.setdefault(e, bc.Edges()).start(w, outs[e])
-        self.restarts += t > 0
-      else:
-        self.edges[e].step(w, outs[e])
-      self.worlds[e] = w
-
-  def seen(self, e=None):
-    if e is not None:
-      return self.edges[e].seen if e in self.edges else set()
-    return set().union(*(x.seen for x in self.edges.values()))
-
-
-def _run(games, make_world, actions, share_levels=True):
-  from pycolab_b200 import batched
-  B = actions.shape[1]
-  eng = batched.BatchedEngine(games, batch=B, share_levels=share_levels)
-  eng.its_showtime()
-  raised = {}
-  track = _Track(raised)
-  compared = sampled_check.lockstep(eng, make_world, range(B), actions, curtains='@',
-                                    sprites='Pabc', pad_columns=True, on_step=track,
-                                    raised=raised)
-  return compared, raised, track
 
 
 @pytest.mark.parametrize('name,shape,extra,coins,binding,B', CASES, ids=[c[0] for c in CASES])
@@ -93,32 +52,20 @@ def test_better_scrolly_cases(name, shape, extra, coins, binding, B):
   """Random play with quits on fenced open levels (no patroller can reach the last
   column), env 0 quitting a third of the way in: P leaves the board and the episodes
   restart, and no env raises."""
-  n = 1 if binding == SHARED else 3 if binding == POOL else 2
-  if binding == POOL:
-    B = max(B, 5)
+  n, B = rsw.levels_and_batch(binding, B)
   seed = sum(shape) + extra + coins
   arts = [bc.open_level(seed + i, shape, coins) for i in range(n)]
-  pitch = bc.ceil16(shape[1]) + extra
+  pitch = rsw.ceil16(shape[1]) + extra
   games = [bc.lowered(a, pitch=pitch) for a in arts]
   actions = bc.random_actions(np.random.RandomState(seed), T, B)
   actions[T // 3, 0] = 5                     # env 0 restarts inside the run
-  compared, raised, track = _run(games, lambda e: bc.make_world(arts[e % n]), actions,
-                                 share_levels=binding != PER_ENV)
+  compared, raised, track = rsw.run(games, lambda e: bc.make_world(arts[e % n]), actions,
+                                    share_levels=binding != rsw.PER_ENV, **LOCKSTEP)
   assert not raised, (name, raised)
   assert track.restarts > 0, name
   assert compared >= T * B, (name, compared)
   if shape[0] * shape[1] <= 64:
     assert any(s.startswith('player_off') for s in track.seen()), (name, track.seen())
-
-
-def _rim_actions(name, B):
-  """Env 0 plays the script, quits, and plays it again; the others walk at random."""
-  script = bc.RIM[name][1]
-  actions = bc.random_actions(np.random.RandomState(len(name)), T, B)
-  first = script + [5] + script
-  actions[:, 0] = 4
-  actions[:len(first), 0] = first
-  return actions
 
 
 STEADY = sorted(name for name in bc.RIM if name not in bc.RAISES)
@@ -127,12 +74,13 @@ STEADY = sorted(name for name in bc.RIM if name not in bc.RAISES)
 @pytest.mark.parametrize('name', STEADY)
 @pytest.mark.parametrize('extra', [0, 64])
 def test_better_scrolly_rim(name, extra):
-  """The scripted rim cases, 6 envs of one level: env 0 must reach every edge the case
-  names, and restart; no env raises."""
-  art, _, edges = bc.RIM[name]
-  game = bc.lowered(art, pitch=bc.ceil16(len(art[0])) + extra)
-  actions = _rim_actions(name, 6)
-  _, raised, track = _run([game], lambda e: bc.make_world(art), actions)
+  """The scripted rim cases, 6 envs of one level: env 0 plays the script, quits, and
+  plays it again, and must reach every edge the case names, and restart; the others walk
+  at random.  No env raises."""
+  art, script, edges = bc.RIM[name]
+  game = bc.lowered(art, pitch=rsw.ceil16(len(art[0])) + extra)
+  actions = rsw.rim_actions(script, 5, 4, T, 6, bc.random_actions, len(name))
+  _, raised, track = rsw.run([game], lambda e: bc.make_world(art), actions, **LOCKSTEP)
   assert not raised, (name, raised)
   assert edges <= track.seen(0), (name, sorted(edges - track.seen(0)))
   assert track.restarts > 0
@@ -144,12 +92,13 @@ def test_better_scrolly_rim_raises(extra):
   last column and latches ENV_ERR_INDEX at the first launch, its_showtime; env 0 plays
   the raising script and latches it at the action that raises, as the even envs do
   where their oracle raises.  Every other env keeps a zero word."""
-  mid, show = bc.RIM['raise_mid_run'][0], bc.RIM['raise_at_showtime'][0]
+  (mid, script, _), show = bc.RIM['raise_mid_run'], bc.RIM['raise_at_showtime'][0]
   assert len(mid) == len(show) and len(mid[0]) == len(show[0])
-  pitch = bc.ceil16(len(mid[0])) + extra
+  pitch = rsw.ceil16(len(mid[0])) + extra
   games = [bc.lowered(mid, pitch=pitch), bc.lowered(show, pitch=pitch)]
-  actions = _rim_actions('raise_mid_run', 6)
-  _, raised, _ = _run(games, lambda e: bc.make_world((mid, show)[e % 2]), actions)
+  actions = rsw.rim_actions(script, 5, 4, T, 6, bc.random_actions, len('raise_mid_run'))
+  _, raised, _ = rsw.run(games, lambda e: bc.make_world((mid, show)[e % 2]), actions,
+                         **LOCKSTEP)
   assert raised.get(0) == bc.RAISES['raise_mid_run'] + 1, raised
   assert all(raised.get(e) == 0 for e in (1, 3, 5)), raised
   assert all(raised.get(e, 0) > 0 for e in (2, 4)), raised

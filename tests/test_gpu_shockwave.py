@@ -12,74 +12,29 @@ reached the edge it is there for."""
 import numpy as np
 import pytest
 
+import rim_sweep as rsw
 import shockwave_cases as sc
 from oracle import games as ogames
-from oracle import sampled_check
 
 pytestmark = pytest.mark.gpu
 
 T = 60
-SHARED, POOL, PER_ENV = 'shared', 'pool', 'per_env'
-BINDINGS = (SHARED, POOL, PER_ENV)
-BATCHES = (1, 5, 37)
 # A pitch of 4096 on the largest board: shockwave stages nothing in shared memory.
 WIDEST = ((32, 64), 4096)
+# What every run compares, and the edges it tracks.
+LOCKSTEP = dict(curtains='@', sprites='P', make_edges=sc.Edges)
 
 
 def _cases():
   """Every shape at pitch ceil16(W) + 0, 16 and 64, widths, bindings, batches and the
   first impact's cell rotated across them; the widest pitch with 5 envs."""
-  out = []
-  for i, shape in enumerate(sc.SHAPES):
-    for j, extra in enumerate((0, 16, 64)):
-      k = 3 * i + j
-      out.append((shape, sc.ceil16(shape[1]) + extra, sc.WIDTHS[k % len(sc.WIDTHS)],
-                  BINDINGS[(i + 2 * j) % 3], BATCHES[(k // 2) % 3], k))
-  out.append(WIDEST + (2, POOL, 5, 0))
+  out = [(shape, pitch, sc.WIDTHS[k % len(sc.WIDTHS)], binding, B, k)
+         for _, _, k, shape, pitch, binding, B in rsw.rotate(sc.SHAPES)]
+  out.append(WIDEST + (2, rsw.POOL, 5, 0))
   return [('%dx%d_p%d_w%d_%s_B%d' % (c[0] + c[1:5]),) + c for c in out]
 
 
 CASES = _cases()
-
-
-class _Track(object):
-  """on_step hook: the edges each sampled env's oracle world went through, and the
-  number of restarts."""
-
-  def __init__(self, actions):
-    self.actions = actions
-    self.edges, self.worlds, self.restarts = {}, {}, 0
-
-  def __call__(self, t, engine, worlds, outs):
-    for e, w in worlds.items():
-      if self.worlds.get(e) is not w:
-        self.edges.setdefault(e, sc.Edges()).start(w, outs[e])
-        self.restarts += t > 0
-      else:
-        self.edges[e].step(w, outs[e], int(self.actions[t - 1, e]))
-      self.worlds[e] = w
-
-  def seen(self, e=None):
-    if e is not None:
-      return self.edges[e].seen if e in self.edges else set()
-    return set().union(*(x.seen for x in self.edges.values()))
-
-
-def _run(games, make_world, actions, share_levels=True, rng_seed=0):
-  """Env e draws from RandomState(rng_seed + e) across its episodes, on the device and
-  in its oracle world make_world(e, rng)."""
-  from pycolab_b200 import batched
-  B = actions.shape[1]
-  eng = batched.BatchedEngine(games, batch=B, share_levels=share_levels, rng_seed=rng_seed)
-  eng.its_showtime()
-  rngs = [np.random.RandomState(rng_seed + e) for e in range(B)]
-  raised = {}
-  track = _Track(actions)
-  compared = sampled_check.lockstep(eng, lambda e: make_world(e, rngs[e]), range(B), actions,
-                                    curtains='@', sprites='P', pad_columns=True,
-                                    on_step=track, raised=raised)
-  assert not raised, raised
-  return compared, track
 
 
 @pytest.mark.parametrize('name,shape,pitch,width,binding,B,k', CASES,
@@ -87,16 +42,16 @@ def _run(games, make_world, actions, share_levels=True, rng_seed=0):
 def test_shockwave_cases(name, shape, pitch, width, binding, B, k):
   """Random play on open levels; env 0's first impact on a corner or side of the board,
   whose ring is clipped there.  A pool's levels differ in their '^' and ' ' cells."""
-  n = 1 if binding == SHARED else 3 if binding == POOL else 2
-  if binding == POOL:
-    B = max(B, 5)
+  n, B = rsw.levels_and_batch(binding, B)
   arts = [sc.sweep_level(shape, k + i) for i in range(n)]
   games = [sc.lowered(a, width, pitch=pitch) for a in arts]
   cells = sc.rim_cells(shape)
   seed = sc.impact_seed(shape, cells[k % len(cells)])
   actions = sc.random_actions(np.random.RandomState(k), T, B)
-  compared, track = _run(games, lambda e, rng: sc.make_world(arts[e % n], rng, width),
-                         actions, share_levels=binding != PER_ENV, rng_seed=seed)
+  compared, raised, track = rsw.run(
+      games, lambda e, rng: sc.make_world(arts[e % n], rng, width), actions,
+      share_levels=binding != rsw.PER_ENV, rng_seed=seed, **LOCKSTEP)
+  assert not raised, raised
   assert compared == (T + 1) * B
   first = track.edges[0]
   if width > 0 and shape[0] * shape[1] > 2:   # else P and a wall fill the board
@@ -112,11 +67,12 @@ def test_shockwave_rim(name, extra):
   it was found with and must reach every edge the case names; the others play at
   random."""
   art, width, seed, script, edges = sc.RIM[name]
-  game = sc.lowered(art, width, pitch=sc.ceil16(len(art[0])) + extra)
+  game = sc.lowered(art, width, pitch=rsw.ceil16(len(art[0])) + extra)
   actions = sc.random_actions(np.random.RandomState(len(name)), T, 6)
   actions[:len(script), 0] = script
-  _, track = _run([game], lambda e, rng: sc.make_world(art, rng, width), actions,
-                  rng_seed=seed)
+  _, raised, track = rsw.run([game], lambda e, rng: sc.make_world(art, rng, width), actions,
+                             rng_seed=seed, **LOCKSTEP)
+  assert not raised, raised
   assert edges <= track.seen(0), (name, sorted(edges - track.seen(0)))
 
 
@@ -129,8 +85,9 @@ def test_shockwave_generated_levels(shape):
   art = levels.shockwave_level(rows + cols, rows, cols, 0.5)
   actions = np.random.RandomState(rows * cols).choice(
       5, size=(150, 10), p=[.55, .15, .15, .1, .05]).astype(np.int32)
-  _, track = _run([sc.lowered(art)], lambda e, rng: ogames.make_shockwave(art, rng), actions,
-                  rng_seed=700)
+  _, raised, track = rsw.run([sc.lowered(art)], lambda e, rng: ogames.make_shockwave(art, rng),
+                             actions, rng_seed=700, **LOCKSTEP)
+  assert not raised, raised
   assert track.restarts > 0
 
 
@@ -144,6 +101,8 @@ def test_shockwave_generated_level_pools(shape):
   rs = np.random.RandomState(4)
   actions = np.stack([rs.choice([0, 1, 2, 3, 4], size=B, p=[.6, .12, .12, .12, .04])
                       for _ in range(T)]).astype(np.int32)
-  _, track = _run([sc.lowered(a) for a in arts],
-                  lambda e, rng: ogames.make_shockwave(arts[e % 3], rng), actions, rng_seed=9)
+  _, raised, track = rsw.run([sc.lowered(a) for a in arts],
+                             lambda e, rng: ogames.make_shockwave(arts[e % 3], rng), actions,
+                             rng_seed=9, **LOCKSTEP)
+  assert not raised, raised
   assert track.restarts > B

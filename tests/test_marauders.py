@@ -8,13 +8,14 @@ a marauder, P firing from row 0, and the np.random.choice of an empty column lis
 raises ValueError; then random play on open levels at every shape the GPU sweep steps.
 Then pcl_create's bound on the block's shared memory."""
 
-import ctypes as C
+import functools
 
 import numpy as np
 import pytest
 
 import marauders_cases as mc
 import refdriver
+import rim_sweep as rsw
 import trajectory as tj
 from oracle import games as ogames
 from oracle import sampled_check
@@ -38,18 +39,15 @@ def _drapes_and_bolts(ref, ora, t):
 
 
 def _pair(art, seed):
-  """Makers of a reference game and an oracle world that draw from the same MT19937
-  stream: NumPy's global generator and RandomState(seed), both seeded here and never
-  again, so that later episodes continue the stream on both sides."""
-  np.random.seed(seed)
-  rng = np.random.RandomState(seed)
-  return (lambda: refdriver.ref_marauders(art)), (lambda: mc.make_world(art, rng))
+  """A reference game and an oracle world on one MT19937 stream from `seed`."""
+  return rsw.seeded_pair(functools.partial(refdriver.ref_marauders, art),
+                         functools.partial(mc.make_world, art), seed)
 
 
-def _script(name):
-  """The case's script, a quit, and the script again from a fresh episode."""
-  script = mc.RIM[name][1]
-  return script + [4] + script
+def _oracle_run(art, actions, seed):
+  """The oracle with auto-reset, one generator RandomState(seed) across the episodes."""
+  return rsw.oracle_run(functools.partial(mc.make_world, art, np.random.RandomState(seed)),
+                        mc.Edges(), actions, ValueError)
 
 
 @needs_ref
@@ -58,10 +56,10 @@ def test_rim_case_oracle_vs_reference(name):
   """Boards, rewards, discounts, game over, both curtains, the marauders' direction and
   every sprite's position, visibility and virtual position, at every step of the scripted
   case and of its replay after a quit."""
-  art, _, edges = mc.RIM[name]
-  actions = _script(name)
+  art, script, edges = mc.RIM[name]
+  actions = rsw.twice(script, 4)
   _lockstep(*_pair(art, 0), actions, check=_drapes_and_bolts)
-  seen, restarts, raised = mc.oracle_run(art, actions, seed=0)
+  seen, restarts, raised = _oracle_run(art, actions, 0)
   assert raised is None
   assert edges <= seen, (name, sorted(edges - seen))
   assert restarts >= 1
@@ -78,7 +76,7 @@ def test_empty_column_choice_raises_at_the_same_step(name):
   got, t_ora = tj.run_until_raise(make_ora, script, ValueError)
   assert t_ref == t_ora == mc.RAISES[name]
   tj.assert_same_trajectory(want, got, name)
-  seen, _, raised = mc.oracle_run(art, script, seed=0)
+  seen, _, raised = _oracle_run(art, script, 0)
   assert raised == mc.RAISES[name] and edges <= seen, (raised, sorted(edges - seen))
 
 
@@ -103,7 +101,7 @@ def test_open_levels_oracle_vs_reference(shape):
   for seed in range(2):
     art = mc.sweep_level(shape, seed)
     actions = mc.random_actions(np.random.RandomState(seed), 200, 1)[:, 0].tolist()
-    seen, n, raised = mc.oracle_run(art, actions, seed=seed)
+    seen, n, raised = _oracle_run(art, actions, seed)
     seen_any |= seen
     restarts += n
     _lockstep(*_pair(art, seed), actions[:raised], check=_drapes_and_bolts)
@@ -130,31 +128,9 @@ def test_stock_layout_board_shapes(rows, cols):
 
 # ------------------------------------------------------------ pcl_create's bound
 
-def _spec(H, W, pitch):
-  game = mc.lowered(mc.RIM['one_column'][0])
-  spec = game.make_spec(auto_reset=True)
-  spec.rows, spec.cols, spec.pitch = H, W, pitch
-  spec.bits_words = (W + 31) // 32 + 1
-  return spec
-
-
-def _create(spec):
-  lib = _lib.load()
-  h = C.c_void_p()
-  status = lib.pcl_create(C.byref(spec), 4, -1, C.byref(h))   # device -1: no CUDA call
-  if status == _lib.OK:
-    lib.pcl_destroy(h)
-  return status
-
-
-def _widest_pitch(H, W):
-  lo, hi = mc.ceil16(W), 1 << 16
-  assert _create(_spec(H, W, lo)) == _lib.OK
-  assert _create(_spec(H, W, hi)) == _lib.ERR_UNSUPPORTED
-  while hi - lo > 16:
-    mid = (lo + hi) // 32 * 16
-    lo, hi = (mid, hi) if _create(_spec(H, W, mid)) == _lib.OK else (lo, mid)
-  return lo
+def _status(H, W, pitch):
+  return rsw.create_status(mc.lowered(mc.RIM['one_column'][0]), 4, rows=H, cols=W, pitch=pitch,
+                           bits_words=(W + 31) // 32 + 1)
 
 
 @pytest.mark.parametrize('H', [11, 12, 16, 31, 32])
@@ -163,17 +139,17 @@ def test_widest_accepted_marauders_pitch_is_launchable(H, W):
   """At the widest pitch pcl_create accepts, the block (the 1,536 bytes of static
   records and four staged H x pitch tiles) fits the 227 KB a block can opt in to; 16
   columns more do not."""
-  pitch = _widest_pitch(H, W)
-  assert mc.block_smem(H, pitch) <= mc.MAX_BLOCK_SMEM < mc.block_smem(H, pitch + 16)
+  pitch = rsw.largest_accepted(lambda p: _status(H, W, p), rsw.ceil16(W), 1 << 16, step=16)
+  assert mc.block_smem(H, pitch) <= rsw.MAX_BLOCK_SMEM < mc.block_smem(H, pitch + 16)
 
 
 def test_marauders_bound_at_known_sizes():
   """32 x 64 fits up to pitch 1792; 11 rows at pitch 5248 fill the 227 KB exactly; the
   stock 16 x 39 board at its own pitch needs 11.5 KB."""
-  assert _create(_spec(32, 64, 1792)) == _lib.OK
-  assert _create(_spec(32, 64, 1808)) == _lib.ERR_UNSUPPORTED
-  assert mc.block_smem(11, 5248) == 4 * 11 * 5248 + 1536 == mc.MAX_BLOCK_SMEM
-  assert _create(_spec(11, 64, 5248)) == _lib.OK
-  assert _create(_spec(11, 64, 5264)) == _lib.ERR_UNSUPPORTED
-  assert _create(_spec(16, 39, 32768)) == _lib.ERR_UNSUPPORTED
+  assert _status(32, 64, 1792) == _lib.OK
+  assert _status(32, 64, 1808) == _lib.ERR_UNSUPPORTED
+  assert mc.block_smem(11, 5248) == 4 * 11 * 5248 + 1536 == rsw.MAX_BLOCK_SMEM
+  assert _status(11, 64, 5248) == _lib.OK
+  assert _status(11, 64, 5264) == _lib.ERR_UNSUPPORTED
+  assert _status(16, 39, 32768) == _lib.ERR_UNSUPPORTED
   assert mc.block_smem(16, 48) == 4 * 16 * 48 + 1536

@@ -13,6 +13,7 @@ import pytest
 
 import golden_cases as gc
 import refdriver
+import rim_sweep as rsw
 import shockwave_cases as sc
 from oracle import games as ogames
 from test_oracle_vs_reference import _lockstep
@@ -94,11 +95,9 @@ def _wave(ref, ora, t):
 
 
 def _pair(art, width, seed):
-  """A reference game and an oracle world drawing from one MT19937 stream: NumPy's global
-  generator and RandomState(seed), each seeded here once for all episodes."""
-  np.random.seed(seed)
-  rng = np.random.RandomState(seed)
-  return (lambda: refdriver.ref_shockwave(art, width)), (lambda: sc.make_world(art, rng, width))
+  """A reference game and an oracle world on one MT19937 stream from `seed`."""
+  return rsw.seeded_pair(lambda: refdriver.ref_shockwave(art, width),
+                         lambda rng: sc.make_world(art, rng, width), seed)
 
 
 @needs_ref
@@ -109,7 +108,8 @@ def test_rim_case_oracle_vs_reference(name):
   art, width, seed, script, edges = sc.RIM[name]
   actions = script + sc.random_actions(np.random.RandomState(len(name)), 40, 1)[:, 0].tolist()
   _lockstep(*_pair(art, width, seed), actions, check=_wave)
-  seen, _ = sc.oracle_run(art, width, script, seed)
+  rng = np.random.RandomState(seed)
+  seen, _, _ = rsw.oracle_run(lambda: sc.make_world(art, rng, width), sc.Edges(), script)
   assert edges <= seen, (name, sorted(edges - seen))
 
 

@@ -6,18 +6,15 @@ board, onto it again from the last row or column, several at once, the player le
 and coming back, and the pushes that raise IndexError.  Then pcl_create's bound on the
 backdrop tile a warehouse_step block stages in shared memory."""
 
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import refdriver
+import rim_sweep as rsw
 import trajectory as tj
 import warehouse_cases as wc
 from oracle import sampled_check
 from pycolab_b200 import _lib
-from pycolab_b200 import lowering
-from pycolab_b200.games import warehouse_manager
 from test_oracle_vs_reference import _lockstep
 
 needs_ref = pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
@@ -32,22 +29,17 @@ def _virtual_positions(ref, ora, t):
       assert tuple(int(v) for v in ent.virtual_position) == (w.vrow, w.vcol), (t, ch)
 
 
-def _script(name):
-  """The case's script, a quit, and the script again from a fresh episode."""
-  script = wc.RIM[name][2]
-  return script + [5] + script
-
-
 @needs_ref
 @pytest.mark.parametrize('name', STEADY)
 def test_rim_case_oracle_vs_reference(name):
   """Boards, rewards, discounts, game over, and every sprite's position, visibility and
   virtual position, at every step of the scripted case and of its replay after a quit."""
-  art, beneath, _, edges = wc.RIM[name]
-  actions = _script(name)
+  art, beneath, script, edges = wc.RIM[name]
+  actions = rsw.twice(script, 5)
   _lockstep(lambda: refdriver.ref_warehouse(art, beneath), lambda: wc.make_world(art, beneath),
             actions, check=_virtual_positions)
-  seen, restarts, raised = wc.oracle_run(art, beneath, actions, wc.rim_boxes(name))
+  seen, restarts, raised = rsw.oracle_run(lambda: wc.make_world(art, beneath),
+                                          wc.Edges(wc.rim_boxes(name)), actions, IndexError)
   assert raised is None
   assert edges <= seen, (name, sorted(edges - seen))
   assert restarts >= 1
@@ -99,7 +91,8 @@ def test_open_levels_oracle_vs_reference(boxes):
   for seed in range(3):
     art = wc.open_level(seed, (8, 9), boxes)
     actions = wc.random_actions(np.random.RandomState(seed), 300, 1)[:, 0].tolist()
-    seen, n, raised = wc.oracle_run(art, ' ', actions, boxes)
+    seen, n, raised = rsw.oracle_run(lambda: wc.make_world(art, ' '), wc.Edges(boxes), actions,
+                                     IndexError)
     seen_any |= seen
     restarts += n
     _lockstep(lambda: refdriver.ref_warehouse(art, ' '), lambda: wc.make_world(art, ' '),
@@ -116,27 +109,15 @@ def test_open_levels_oracle_vs_reference(boxes):
 
 WARPS_PER_BLOCK = 4
 REC_BYTES = 512                   # 128 record words per warp
-MAX_BLOCK_SMEM = 227 * 1024       # H100: the dynamic shared memory a block may opt in to
 
 
 def block_smem(H, pitch):
   return WARPS_PER_BLOCK * (REC_BYTES + H * pitch)
 
 
-def _spec(H, W, pitch):
-  game = lowering.lower(warehouse_manager.make_game(wc.RIM['gapped_boxes'][0]))
-  spec = game.make_spec(auto_reset=True)
-  spec.rows, spec.cols, spec.pitch = H, W, pitch
-  return spec
-
-
-def _create(spec):
-  lib = _lib.load()
-  h = C.c_void_p()
-  status = lib.pcl_create(C.byref(spec), 5, -1, C.byref(h))   # device -1: no CUDA call
-  if status == _lib.OK:
-    lib.pcl_destroy(h)
-  return status
+def _status(H, W, pitch):
+  game = wc.lowered(wc.RIM['gapped_boxes'][0])
+  return rsw.create_status(game, 5, rows=H, cols=W, pitch=pitch)
 
 
 @pytest.mark.parametrize('W', [8, 64, 80, 128, 240, 256, 1000])
@@ -145,22 +126,14 @@ def test_largest_accepted_warehouse_board_is_launchable(W, extra):
   """pcl_create's shared-memory test and the launcher's agree: at the largest H it
   accepts, the block (4 warps, each staging 512 bytes of records and the H x pitch tile)
   fits the 227 KB a block can opt in to; one row more is refused."""
-  pitch = wc.ceil16(W) + extra
-  lo, hi = 1, 8192
-  assert _create(_spec(lo, W, pitch)) == _lib.OK
-  assert _create(_spec(hi, W, pitch)) == _lib.ERR_UNSUPPORTED
-  while hi - lo > 1:
-    mid = (lo + hi) // 2
-    if _create(_spec(mid, W, pitch)) == _lib.OK:
-      lo = mid
-    else:
-      hi = mid
-  assert block_smem(lo, pitch) <= MAX_BLOCK_SMEM < block_smem(lo + 1, pitch), (W, pitch, lo)
+  pitch = rsw.ceil16(W) + extra
+  lo = rsw.largest_accepted(lambda H: _status(H, W, pitch), 1, 8192)
+  assert block_smem(lo, pitch) <= rsw.MAX_BLOCK_SMEM < block_smem(lo + 1, pitch), (W, pitch, lo)
 
 
 def test_warehouse_bound_at_known_sizes():
   """240 x 240 fits, 256 x 256 does not; the 80 x 80 boards of the benchmark need 27.6 KB
   per block, above the 48 KB default only from 96 x 128 up."""
-  assert _create(_spec(240, 240, 240)) == _lib.OK
-  assert _create(_spec(256, 256, 256)) == _lib.ERR_UNSUPPORTED
+  assert _status(240, 240, 240) == _lib.OK
+  assert _status(256, 256, 256) == _lib.ERR_UNSUPPORTED
   assert block_smem(80, 80) < 48 * 1024 < block_smem(96, 128)

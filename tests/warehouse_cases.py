@@ -16,14 +16,11 @@ the edge:
 import numpy as np
 
 from oracle import games as ogames
+from rim_sweep import repitch
 
 BOX_ORDER = '1234567890'
 # Box characters by count, with gaps in the update order ('3', '7', '0').
 BOX_SETS = {1: '0', 2: '37', 3: '370', 7: '1345780', 10: '1234567890'}
-
-
-def ceil16(x):
-  return (x + 15) // 16 * 16
 
 
 def open_level(seed, shape, boxes, num_goals=None, wall_density=0.06):
@@ -50,12 +47,7 @@ def lowered(art, beneath=' ', pitch=None):
   """The lowered facade game of `art`, its backdrop re-padded to `pitch` columns."""
   from pycolab_b200 import lowering
   from pycolab_b200.games import warehouse_manager
-  low = lowering.lower(warehouse_manager.make_game(art, beneath))
-  if pitch is not None:
-    backdrop = np.zeros((low.rows, pitch), dtype=np.uint8)
-    backdrop[:, :low.cols] = low.backdrop[:, :low.cols]
-    low.backdrop, low.pitch = backdrop, pitch
-  return low
+  return repitch(lowering.lower(warehouse_manager.make_game(art, beneath)), pitch)
 
 
 def random_actions(rs, T, B, quit_p=0.02):
@@ -142,13 +134,13 @@ class Edges(object):
     self.boxes = boxes
     self.seen = set()
 
-  def start(self, world):
+  def start(self, world, out):
     self.prev = _snapshot(world)
     if world.game_over:
       self.seen.add('showtime_over')
     self._now(world)
 
-  def step(self, world, action):
+  def step(self, world, out, action):
     now = _snapshot(world)
     H, W = world.rows, world.cols
     moved = [b for b in self.boxes if now[b][3:] != self.prev[b][3:]]
@@ -176,27 +168,3 @@ class Edges(object):
     cells = [s[b][:2] for b in self.boxes if s[b][2]]
     if len(set(cells)) < len(cells):
       self.seen.add('shared_cell')
-
-
-def oracle_run(art, beneath, actions, boxes):
-  """Play `actions` on oracle worlds with auto-reset.  Returns (edges seen, restarts, the
-  step whose action raised IndexError or None)."""
-  edges = Edges(boxes)
-  world = make_world(art, beneath)
-  world.its_showtime()
-  edges.start(world)
-  restarts = 0
-  for t, a in enumerate(actions):
-    if world.game_over:
-      restarts += 1
-      world = make_world(art, beneath)
-      world.its_showtime()
-      edges.start(world)
-      continue
-    try:
-      world.play(int(a))
-    except IndexError:
-      edges.seen.add('raise')
-      return edges.seen, restarts, t
-    edges.step(world, int(a))
-  return edges.seen, restarts, None
