@@ -635,6 +635,30 @@ int pcl_observe(pcl_handle* h, const pcl_observe_spec* spec, const void* d_table
                 const uint8_t* d_valid, const uint8_t* d_board, void* d_out,
                 int32_t* d_unknown, void* stream);
 
+/* A cropper feeding a post-processor, in ONE launch from the board: pcl_crop_tracking
+ * (crop, d_board, d_crop_state, d_curtains: same checks, same corner state, NULL = the plot
+ * record's slot; the window moves exactly once per call whatever the depth) followed by
+ * pcl_observe over the crop_rows x crop_cols window, without the crop ever being stored:
+ *   out[b, d, jr, jc] = d_table[cell][d]
+ * where cell is the window's byte (the pad character off the board).  The strides of
+ * `spec` are in elements over (env, plane, window row, window column); any depth >= 1.
+ * A window cell, pad included, holding a byte >= 128 or one d_valid does not mark sets
+ * *d_unknown to 1 (upstream's RuntimeError for the cropped observation).
+ * Un-occluded layers (games with occlusion_in_layers=False): with d_planes set, d_board
+ * is not read; output plane d is source plane d_plane_of[d] (i32 [depth] on the device,
+ * -1 = a plane of zeros) cut at the same window, and the cell is that plane's bit: 1 where
+ * the plane's byte is non-zero, and off the board 1 exactly when d_plane_of[d] ==
+ * pad_plane (the source plane of the pad character, or -1).  Source plane k of env b
+ * starts at d_planes + b * plane_stride_b + k * plane_stride_d, rows plane_stride_r bytes
+ * apart, one byte per column (pcl_layers' output, or any u8 / bool planes).  The table is
+ * looked up at rows 0 and 1 then, and d_unknown is not set. */
+int pcl_crop_observe(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_board,
+                     int32_t* d_crop_state, const uint8_t* const* d_curtains,
+                     const pcl_observe_spec* spec, const void* d_table, const uint8_t* d_valid,
+                     const uint8_t* d_planes, const int32_t* d_plane_of, int32_t pad_plane,
+                     int64_t plane_stride_b, int64_t plane_stride_d, int64_t plane_stride_r,
+                     void* d_out, int32_t* d_unknown, void* stream);
+
 /* Multi-GPU hand-off record (SURVEY.md 8e): everything one env contributes to the
  * per-step all-gather, packed so that ONE collective moves it all.
  *   d_packed u8 [B, record_bytes]; one record = view_bytes of the env's observation

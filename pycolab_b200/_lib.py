@@ -225,6 +225,10 @@ SYMBOLS = {
                                    C.POINTER(Outputs), C.POINTER(HandoffState), C.c_void_p]),
     'pcl_observe': (C.c_int, [C.c_void_p, C.POINTER(ObserveSpec), C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'pcl_crop_observe': (C.c_int, [C.c_void_p, C.POINTER(CropSpec), C.c_void_p, C.c_void_p,
+                                   C.POINTER(C.c_void_p), C.POINTER(ObserveSpec), C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64,
+                                   C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     'pcl_error_codes': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     'pcl_launch_count': (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
 }

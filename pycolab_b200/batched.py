@@ -411,15 +411,22 @@ class BatchedEngine(object):
     every env: bool [B, len(chars), rows, cols], plane k = everywhere the owner of
     chars[k] places it, occluded or not.  Default chars: every character of the
     game, sorted (`self.chars`).  One kernel over the packed device state."""
-    torch = _torch()
     chars = self.chars if chars is None else ''.join(chars)
     if self.game.layers is not None:
       return self.game.layers(self, chars)
+    return self._layer_planes(chars)[:, :, :, :self.cols].bool()
+
+  def _layer_planes(self, chars):
+    """The un-occluded layers of `chars` as u8 planes [B, len(chars), rows, >= cols], one
+    byte per column: pcl_layers' [B, n, rows, pitch] output, or the game's layers hook."""
+    torch = _torch()
+    if self.game.layers is not None:
+      return self.game.layers(self, chars).contiguous().view(torch.uint8)
     out = torch.empty((self.batch, len(chars), self.rows, self.pitch), dtype=torch.uint8,
                       device=self.device)
     _lib.check(self._lib.pcl_layers(self._h, chars.encode('ascii'), len(chars), out.data_ptr(),
                                     self._stream()), 'pcl_layers', self._h)
-    return out[:, :, :, :self.cols].bool()
+    return out
 
   def error_codes(self):
     torch = _torch()
@@ -493,14 +500,8 @@ class BatchedEngine(object):
         self._crop_out[key] = torch.empty(shape, dtype=torch.uint8, device=self.device)
       out = self._crop_out[key]
     state_ptr = None if state is None else state.data_ptr()
-    if any(code < 0 for code in crop_spec.track):
-      # A tracked drape's position is the median of its curtain cells: hand the
-      # kernel the byte curtains (cropping.py:583-596).
-      curtains, ptrs = [], (C.c_void_p * _lib.MAX_TRACK)()
-      for i, code in enumerate(crop_spec.track):
-        if code < 0:
-          curtains.append(self._curtain_bytes(-code - 1))
-          ptrs[i] = curtains[-1].data_ptr()
+    curtains, ptrs = self._tracked_curtains(crop_spec)
+    if ptrs is not None:
       _check_crop(self._lib.pcl_crop_tracking(self._h, C.byref(crop_spec),
                                               self._board.data_ptr(), out.data_ptr(), state_ptr,
                                               ptrs, self._stream()),
@@ -510,6 +511,44 @@ class BatchedEngine(object):
                                      out.data_ptr(), state_ptr, self._stream()),
                   'pcl_crop', self._h, crop_spec)
     return out
+
+  def _tracked_curtains(self, crop_spec):
+    """(curtains, ptrs): a tracked drape's position is the median of its curtain cells, so
+    the cropper kernels take the byte curtains of the drapes `crop_spec.track` names
+    (cropping.py:583-596) as a MAX_TRACK array of device pointers; ptrs is None when the
+    list names no drape.  Keep `curtains` alive until the launch is enqueued."""
+    if not any(code < 0 for code in crop_spec.track):
+      return [], None
+    curtains, ptrs = [], (C.c_void_p * _lib.MAX_TRACK)()
+    for i, code in enumerate(crop_spec.track):
+      if code < 0:
+        curtains.append(self._curtain_bytes(-code - 1))
+        ptrs[i] = curtains[-1].data_ptr()
+    return curtains, ptrs
+
+  def _crop_observe(self, crop_spec, state, table, valid, is_3d, permute, unknown=None,
+                    layers=None):
+    """observers.crop_observe of this engine's boards through cropper `crop_spec` (its
+    corner in `state`, None = the plot record's slot).  `layers`: the layer characters of
+    a game built with occlusion_in_layers=False, whose un-occluded layers are cut instead
+    of the board."""
+    from pycolab_b200 import observers
+    if crop_spec.rows * crop_spec.cols > _lib.MAX_CROP_CELLS:
+      _check_crop(_lib.ERR_UNSUPPORTED, 'pcl_crop_observe', self._h, crop_spec)
+    curtains, ptrs = self._tracked_curtains(crop_spec)
+    planes, plane_of, pad_plane = None, None, -1
+    if layers is not None:
+      known = ''.join(sorted(set(ch for ch in layers if ch in self.chars)))
+      plane_of = [known.find(ch) for ch in layers]
+      if crop_spec.pad_char >= 0:
+        pad_plane = known.find(chr(crop_spec.pad_char))
+      # a source plane per character the game has (a zero plane for the others); one
+      # plane stands in when there is none, read by no output plane
+      planes = self._layer_planes(known or self.chars[:1])
+    return observers.crop_observe(
+        self._lib, self._h, crop_spec, self._board, state, ptrs, table, valid, is_3d, permute,
+        self._stream(), unknown=unknown, planes=planes, plane_of=plane_of,
+        pad_plane=pad_plane, check=lambda st, what: _check_crop(st, what, self._h, crop_spec))
 
   def pack_handoff(self, view, packed):
     """Pack `view` (u8 [B, ...], contiguous) with this step's reward / discount /
@@ -544,14 +583,29 @@ class BatchedEngine(object):
         C.byref(handoff_state), self._stream()), 'pcl_crop_handoff', self._h)
 
   # --- observation post-processors (rendering.py:304-661) over the whole batch
-  def to_feature_array(self, layers, permute=None):
+  def to_feature_array(self, layers, permute=None, crop_spec=None, state=None):
     """ObservationToFeatureArray: float32 one-hot planes, [B, C, rows, cols] (or
     the last three axes permuted).  A character the game lacks gives a zero plane.
     A game made with occlusion_in_layers=False copies its un-occluded layers
-    (`unoccluded_layers`), as upstream copies `observation.layers`."""
+    (`unoccluded_layers`), as upstream copies `observation.layers`.
+
+    With `crop_spec`, the planes of that cropper's window instead, [B, C, crop rows, crop
+    cols], in one launch from the board: the window moves as `crop(crop_spec, state)`
+    would move it, so call it once per step per cropper state, as `crop`.  Un-occluded
+    layers are cut at the same window, off-board cells set in the pad character's plane
+    (cropping.py `_do_crop`)."""
     from pycolab_b200 import observers
     torch = _torch()
     permute = observers.check_permute(permute, True, 'ObservationToFeatureArray')
+    if crop_spec is not None:
+      if self.game.occlusion_in_layers:
+        table, lay = observers.feature_table(layers, present=self.chars), None
+      else:
+        table = np.zeros((128, len(layers)), dtype=np.float32)
+        table[1] = 1.0                     # the cell is the layer's bit
+        lay = layers
+      out = self._crop_observe(crop_spec, state, table, None, True, permute, layers=lay)
+      return out.view(torch.float32)
     if self.game.occlusion_in_layers:
       out = observers.observe(self._lib, self._h, self._board, self.rows, self.cols,
                               observers.feature_table(layers, present=self.chars), None,
@@ -565,16 +619,21 @@ class BatchedEngine(object):
       out[:, known] = planes.float()
     return out if permute is None else out.permute([0] + [1 + i for i in permute])
 
-  def to_array(self, value_mapping, dtype=None, permute=None):
+  def to_array(self, value_mapping, dtype=None, permute=None, crop_spec=None, state=None):
     """ObservationToArray: map characters to scalars ([B, rows, cols]) or vectors
-    ([B, D, rows, cols]); raises RuntimeError on a character outside the mapping."""
+    ([B, D, rows, cols]); raises RuntimeError on a character outside the mapping.
+    With `crop_spec`, of that cropper's window (as `to_feature_array`); the pad
+    character of a window past the board must be in the mapping too."""
     from pycolab_b200 import observers
     torch = _torch()
     table, valid, is_3d = observers.value_table(value_mapping, dtype)
     permute = observers.check_permute(permute, is_3d, 'ObservationToArray')
     unknown = torch.zeros((1,), dtype=torch.int32, device=self.device)
-    out = observers.observe(self._lib, self._h, self._board, self.rows, self.cols, table,
-                            valid, is_3d, permute, self._stream(), unknown)
+    if crop_spec is not None:
+      out = self._crop_observe(crop_spec, state, table, valid, is_3d, permute, unknown)
+    else:
+      out = observers.observe(self._lib, self._h, self._board, self.rows, self.cols, table,
+                              valid, is_3d, permute, self._stream(), unknown)
     if int(unknown[0]):
       raise RuntimeError(
           'This ObservationToArray only knows array values for the characters {}, but it '
@@ -582,12 +641,15 @@ class BatchedEngine(object):
               ''.join(value_mapping.keys())))
     return out.view(observers.torch_dtype(table.dtype))
 
-  def repaint(self, character_mapping):
-    """ObservationCharacterRepainter over every board: u8 [B, rows, cols]."""
+  def repaint(self, character_mapping, crop_spec=None, state=None):
+    """ObservationCharacterRepainter over every board: u8 [B, rows, cols]; with
+    `crop_spec`, over that cropper's window (as `to_feature_array`)."""
     from pycolab_b200 import observers
+    table = observers.repaint_table(character_mapping)
+    if crop_spec is not None:
+      return self._crop_observe(crop_spec, state, table, None, False, None)
     return observers.observe(self._lib, self._h, self._board, self.rows, self.cols,
-                             observers.repaint_table(character_mapping), None, False, None,
-                             self._stream())
+                             table, None, False, None, self._stream())
 
   def sprite_state(self):
     """i32 [B, S, 8] device tensor of sprite records (PCL_S_* words)."""

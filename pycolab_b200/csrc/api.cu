@@ -843,6 +843,39 @@ int pcl_crop_tracking(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d
   return launched(h, pcl::launch_crop(p, (cudaStream_t)stream), "launch_crop");
 }
 
+int pcl_crop_observe(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_board,
+                     int32_t* d_crop_state, const uint8_t* const* d_curtains,
+                     const pcl_observe_spec* spec, const void* d_table, const uint8_t* d_valid,
+                     const uint8_t* d_planes, const int32_t* d_plane_of, int32_t pad_plane,
+                     int64_t plane_stride_b, int64_t plane_stride_d, int64_t plane_stride_r,
+                     void* d_out, int32_t* d_unknown, void* stream) {
+  Range nvtx_range("pcl_crop_observe");
+  if (!h || !crop || !spec || !d_table || !d_out) return PCL_ERR_INVALID;
+  if (d_planes ? !d_plane_of : !d_board) return PCL_ERR_INVALID;
+  if (spec->depth < 1 || spec->dtype < 0 || spec->dtype > 5) return PCL_ERR_INVALID;
+  if (!h->bound) return PCL_ERR_UNBOUND;
+  const int ok = crop_spec_ok(h, crop);
+  if (ok != PCL_OK) return ok;
+  pcl::CropObserveParams p;
+  memset(&p, 0, sizeof(p));
+  p.crop = crop_params(h, crop, d_board, nullptr, d_crop_state);
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
+    if (crop->track[i] > 0) continue;
+    if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
+    if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
+    p.crop.curtains[i] = d_curtains[i];
+  }
+  p.depth = spec->depth; p.dtype = spec->dtype;
+  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
+  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
+  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
+  p.table = d_table; p.valid = d_valid; p.out = d_out; p.unknown = d_unknown;
+  p.planes = d_planes; p.plane_of = d_plane_of; p.pad_plane = d_planes ? pad_plane : -1;
+  p.plane_stride_b = plane_stride_b; p.plane_stride_d = plane_stride_d;
+  p.plane_stride_r = plane_stride_r;
+  return launched(h, pcl::launch_crop_observe(p, (cudaStream_t)stream), "launch_crop_observe");
+}
+
 int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_board,
                      int32_t* d_crop_state, const pcl_outputs* out, const pcl_handoff* x,
                      void* stream) {

@@ -18,6 +18,7 @@
 #include <stdint.h>
 
 #include "../../include/pcl.h"
+#include "pcl_crop.cuh"
 #include "pcl_kernels.cuh"
 
 namespace pcl {
@@ -25,6 +26,16 @@ namespace pcl {
 namespace {
 
 constexpr int kThreads = 256;
+
+// Element d of a cell holding `byte`: its `words` words in row `byte` of a table staged
+// with `row_words` words per row, or zeros for a byte >= 128 (outside every mapping).
+template <typename T>
+__device__ __forceinline__ void put_element(T* dst, const T* table, int row_words, int words,
+                                            uint32_t byte, int d) {
+  const bool ascii = byte < 128;
+  const T* src = table + (byte & 0x7f) * row_words + d * words;
+  for (int w = 0; w < words; ++w) dst[w] = ascii ? src[w] : T(0);
+}
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
@@ -57,10 +68,8 @@ observe_kernel(const ObserveParams p) {
       const bool ascii = byte < 128;
       unknown |= !ascii || !valid[byte & 0x7f];
       T* dst = out + b * p.stride_b + (int64_t)r * p.stride_r + (int64_t)c * p.stride_c;
-      const T* src = table + (byte & 0x7f) * row_words;
       for (int d = 0; d < p.depth; ++d)
-        for (int w = 0; w < p.words; ++w)
-          dst[d * p.stride_d + w] = ascii ? src[d * p.words + w] : T(0);
+        put_element(dst + d * p.stride_d, table, row_words, p.words, byte, d);
     }
   }
   if (unknown && p.unknown) *p.unknown = 1;
@@ -78,6 +87,101 @@ cudaError_t launch_observe(const ObserveParams& p, cudaStream_t s) {
   if (bytes) observe_kernel<uint8_t><<<blocks, kThreads, smem, s>>>(p);
   else observe_kernel<uint32_t><<<blocks, kThreads, smem, s>>>(p);   // 4- / 8-byte bits
   return cudaGetLastError();
+}
+
+namespace {
+
+// ---- a cropper's window through a post-processor (pcl_crop_observe) ---------------
+// One warp per env, four envs per block, as crop_kernel (render.cu): the warp moves its
+// env's window corner once (crop_corner), then writes depth elements per window cell.
+// The table is staged in shared memory kCropChunk planes at a time, so any depth is one
+// launch and the corner advances exactly once per call.  The lanes walk the output in
+// the order of its strides, so that neighbouring lanes store neighbouring elements.
+constexpr int kCropChunk = 32;
+
+template <typename T>
+__global__ void __launch_bounds__(128) crop_observe_kernel(const CropObserveParams p) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  T* table = reinterpret_cast<T*>(smem_raw);               // [128, planes of this chunk]
+  __shared__ int s_hist[4][256];                           // drape medians (crop_corner)
+  __shared__ uint8_t valid[128];
+  __shared__ int plane_of[kCropChunk];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const CropParams& c = p.crop;
+  const int env = blockIdx.x * 4 + warp;
+  const bool active = env < c.B;                           // whole warps: every thread syncs
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");       // the step kernel's board and records
+  int wr = 0, wc = 0;
+  if (active) crop_corner(c, env, lane, s_hist[warp], &wr, &wc);
+  valid[threadIdx.x] = p.valid ? p.valid[threadIdx.x] : 1;
+
+  const int rows = c.crop.rows, cells = rows * c.crop.cols;
+  const int minor = p.col_major ? rows : c.crop.cols;
+  const uint32_t padv = c.crop.pad_char >= 0 ? (uint32_t)c.crop.pad_char : 0u;
+  const T* g_table = static_cast<const T*>(p.table);
+  T* out = static_cast<T*>(p.out) + (int64_t)env * p.stride_b;
+  const uint8_t* board = c.board + (int64_t)env * c.H * c.pitch;
+  const uint8_t* planes = p.planes + (int64_t)env * p.plane_stride_b;
+  bool unknown = false;
+  for (int k0 = 0; k0 < p.depth; k0 += kCropChunk) {
+    const int n = min(kCropChunk, p.depth - k0);
+    const int row_words = n * p.words;
+    __syncthreads();                                       // the last chunk's readers are done
+    for (int i = threadIdx.x; i < 128 * row_words; i += 128) {
+      const int row = i / row_words;
+      table[i] = g_table[((int64_t)row * p.depth + k0) * p.words + (i - row * row_words)];
+    }
+    if (p.planes && threadIdx.x < n) plane_of[threadIdx.x] = p.plane_of[k0 + threadIdx.x];
+    __syncthreads();
+    if (!active) continue;
+    // This lane's element as (fast, slow) = (plane, cell) or (cell, plane); each round
+    // the warp moves on by 32 elements.
+    const int nf = p.planes_fast ? n : cells, ns = p.planes_fast ? cells : n;
+    const int step_f = 32 % nf, step_s = 32 / nf;
+    int f = lane % nf, s = lane / nf;
+    while (s < ns) {
+      const int d = p.planes_fast ? f : s, i = p.planes_fast ? s : f;
+      const int major = minor == 1 ? i : (int)__umulhi((uint32_t)i, p.minor_recip);
+      const int jr = p.col_major ? i - major * minor : major;
+      const int jc = p.col_major ? major : i - major * minor;
+      uint32_t byte;
+      if (p.planes) {                                      // un-occluded: the layer's bit
+        const int k = plane_of[d];
+        byte = k >= 0 && crop_cell(c, planes + k * p.plane_stride_d, p.plane_stride_r, wr, wc,
+                                   jr, jc, k == p.pad_plane) != 0;
+      } else {
+        byte = crop_cell(c, board, c.pitch, wr, wc, jr, jc, padv);
+        unknown |= byte >= 128 || !valid[byte & 0x7f];
+      }
+      put_element(out + (k0 + d) * p.stride_d + jr * p.stride_r + jc * p.stride_c, table,
+                  row_words, p.words, byte, d);
+      f += step_f;
+      s += step_s;
+      if (f >= nf) { f -= nf; ++s; }
+    }
+  }
+  if (active && __any_sync(0xffffffffu, unknown) && lane == 0 && p.unknown) *p.unknown = 1;
+}
+
+}  // namespace
+
+cudaError_t launch_crop_observe(const CropObserveParams& p, cudaStream_t s) {
+  const pcl_crop_spec& c = p.crop.crop;
+  if (c.rows < 1 || c.cols < 1 || (int64_t)c.rows * c.cols > PCL_MAX_CROP_CELLS || p.depth < 1)
+    return cudaErrorInvalidValue;
+  CropObserveParams q = p;
+  const int64_t sd = llabs(p.stride_d), sr = llabs(p.stride_r), sc = llabs(p.stride_c);
+  q.planes_fast = p.depth > 1 && sd < sr && sd < sc;
+  q.col_major = sr < sc;
+  const int minor = q.col_major ? c.rows : c.cols;
+  // floor(2^32 / minor) + 1: __umulhi(i, recip) == i / minor for every i < 65536.
+  q.minor_recip = minor > 1 ? (uint32_t)(0x100000000ull / (uint32_t)minor) + 1u : 0u;
+  const bool bytes = p.dtype == 0 || p.dtype == 5;         // 1- and 2-byte elements
+  const size_t smem = 128 * (size_t)min(p.depth, kCropChunk) * p.words * (bytes ? 1 : 4);
+  const int grid = (p.crop.B + 3) / 4;
+  if (bytes) return launch_pdl(crop_observe_kernel<uint8_t>, grid, 128, smem, s, q);
+  return launch_pdl(crop_observe_kernel<uint32_t>, grid, 128, smem, s, q);
 }
 
 namespace {

@@ -120,6 +120,18 @@ __device__ __forceinline__ void crop_corner(const CropParams& p, int env, int la
   *out_wr = wr; *out_wc = wc;
 }
 
+// Cell (jr, jc) of the window at corner (wr, wc) of a plane with `pitch` bytes per row:
+// the plane's byte on the board, `padv` outside it (_do_crop :118-227).
+__device__ __forceinline__ uint32_t crop_cell(const CropParams& p, const uint8_t* plane,
+                                              int64_t pitch, int wr, int wc, int jr, int jc,
+                                              uint32_t padv) {
+  const int r = wr + jr, cc2 = wc + jc;
+  uint32_t b = padv;
+  if ((unsigned)r < (unsigned)p.H && (unsigned)cc2 < (unsigned)p.W)
+    b = plane[(int64_t)r * pitch + cc2];
+  return b;
+}
+
 // Four consecutive cells i .. i + 3 of the crop window (row-major over rows x cols)
 // as one little-endian word, pad character outside the board (_do_crop :118-227).
 // One division per word (by a runtime width, as a multiply-high with the reciprocal in
@@ -134,11 +146,7 @@ __device__ __forceinline__ uint32_t crop_word(const CropParams& p, const uint8_t
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (i + k >= cells) break;
-    const int r = wr + jr, cc2 = wc + jc;
-    uint32_t b = padv;
-    if ((unsigned)r < (unsigned)p.H && (unsigned)cc2 < (unsigned)p.W)
-      b = board[(int64_t)r * p.pitch + cc2];
-    v |= b << (8 * k);
+    v |= crop_cell(p, board, p.pitch, wr, wc, jr, jc, padv) << (8 * k);
     if (++jc == c.cols) { jc = 0; ++jr; }
   }
   return v;

@@ -234,6 +234,30 @@ struct ObserveParams {
 };
 cudaError_t launch_observe(const ObserveParams& p, cudaStream_t s);
 
+// A cropper's window run through an observation post-processor in one launch
+// (pcl_crop_observe): out[b, d, jr, jc] = table[cell][d], where the cell is the window's
+// board byte or, with `planes` set (un-occluded layers), the bit of plane plane_of[d].
+struct CropObserveParams {
+  CropParams crop;               // crop.out is unused
+  int depth, dtype;
+  int words;                     // words of T per element, as ObserveParams::words
+  int64_t stride_b, stride_d, stride_r, stride_c;   // in words of T
+  const void* table;             // [128, depth]
+  const uint8_t* valid;          // u8 [128] or NULL
+  void* out;
+  int32_t* unknown;              // i32 [1] or NULL
+  const uint8_t* planes;         // u8 source layer planes, or NULL for the board
+  const int32_t* plane_of;       // i32 [depth]: source plane of output plane d, or -1
+  int pad_plane;                 // source plane whose off-board cells are 1, or -1
+  int64_t plane_stride_b, plane_stride_d, plane_stride_r;   // in bytes
+  // Set by launch_crop_observe from the strides: the lanes of a warp walk the planes of a
+  // cell (planes_fast) or the cells of a plane, in row-major or column-major (col_major)
+  // order; minor_recip divides a cell index by the minor axis's length.
+  int planes_fast, col_major;
+  uint32_t minor_recip;
+};
+cudaError_t launch_crop_observe(const CropObserveParams& p, cudaStream_t s);
+
 cudaError_t launch_crop(const CropParams& p, cudaStream_t s);
 
 // Exchange state of the fused crop + hand-off kernel (pcl_crop_handoff).

@@ -95,6 +95,25 @@ def plane_chunks(depth):
   return [(k0, min(MAX_PLANES, depth - k0)) for k0 in range(0, depth, MAX_PLANES)]
 
 
+def _output(B, rows, cols, table, is_3d, permute, device):
+  """(out, strides, t_table): the output tensor [B] + permuted([depth,] rows, cols) in
+  the same-size unsigned container of `table.dtype`, the element strides of its
+  unpermuted axes ({0: plane, 1: row, 2: column} for a 3-D output, {0: row, 1: column}
+  otherwise) and the table on the device."""
+  import torch
+  depth = table.shape[1]
+  size = table.dtype.itemsize
+  base = [depth, rows, cols] if is_3d else [rows, cols]
+  perm = list(permute) if permute is not None else list(range(len(base)))
+  shape = [base[i] for i in perm]
+  container = getattr(torch, np.dtype(_CONTAINER[size]).name)
+  out = torch.empty([B] + shape, dtype=container, device=device)
+  strides = list(out.stride())[1:]
+  at = {base_dim: strides[perm.index(base_dim)] for base_dim in range(len(base))}
+  t_table = torch.from_numpy(np.ascontiguousarray(table).view(_CONTAINER[size])).to(device)
+  return out, at, t_table
+
+
 def observe(lib, handle, board, rows, cols, table, valid, is_3d, permute, stream,
             unknown=None):
   """Run pcl_observe over `board` (u8 [B, rows, pitch] CUDA tensor).  Returns a
@@ -102,18 +121,9 @@ def observe(lib, handle, board, rows, cols, table, valid, is_3d, permute, stream
   unsigned container of `table.dtype` (`torch_dtype` / `numpy_view` convert it).
   More than MAX_PLANES planes take one launch per MAX_PLANES."""
   import torch
-  B = board.shape[0]
   depth = table.shape[1]
   size = table.dtype.itemsize
-  base = [depth, rows, cols] if is_3d else [rows, cols]
-  perm = list(permute) if permute is not None else list(range(len(base)))
-  shape = [base[i] for i in perm]
-  container = getattr(torch, np.dtype(_CONTAINER[size]).name)
-  out = torch.empty([B] + shape, dtype=container, device=board.device)
-  strides = list(out.stride())[1:]
-  at = {base_dim: strides[perm.index(base_dim)] for base_dim in range(len(base))}
-  t_table = torch.from_numpy(np.ascontiguousarray(table).view(_CONTAINER[size])).to(
-      board.device)
+  out, at, t_table = _output(board.shape[0], rows, cols, table, is_3d, permute, board.device)
   t_valid = None if valid is None else torch.from_numpy(valid).to(board.device)
   for k0, planes in plane_chunks(depth):
     spec = _lib.ObserveSpec(planes, _CODE_OF_SIZE[size], out.stride()[0],
@@ -126,6 +136,43 @@ def observe(lib, handle, board, rows, cols, table, valid, is_3d, permute, stream
                                board.data_ptr(), d_out,
                                None if unknown is None else unknown.data_ptr(), stream),
                'pcl_observe')
+  return out
+
+
+def crop_observe(lib, handle, crop_spec, board, state, curtains, table, valid, is_3d, permute,
+                 stream, unknown=None, planes=None, plane_of=None, pad_plane=-1, check=None):
+  """Run pcl_crop_observe: crop_spec's window of `board` (u8 [B, rows, pitch] CUDA tensor),
+  moved once as `pcl_crop_tracking` moves it (`state`: the cropper's corner array, None =
+  the plot record's slot; `curtains`: the ctypes pointer array of tracked drapes' curtains,
+  or None), through the [128, depth] `table` in one launch.  Returns what `observe`
+  returns for a board of the window's shape.  With `planes` (u8 [B, n, rows, >= cols], one
+  byte per column) the output planes are the un-occluded layers plane_of[d] (-1: zeros)
+  of that window, off-board cells 1 in plane `pad_plane`.  `check(status, what)` judges
+  the call's status (default `_lib.check`)."""
+  import torch
+  depth = table.shape[1]
+  size = table.dtype.itemsize
+  device = (board if planes is None else planes).device
+  B = (board if planes is None else planes).shape[0]
+  out, at, t_table = _output(B, crop_spec.rows, crop_spec.cols, table, is_3d, permute, device)
+  t_valid = None if valid is None else torch.from_numpy(valid).to(device)
+  spec = _lib.ObserveSpec(depth, _CODE_OF_SIZE[size], out.stride()[0], at[0] if is_3d else 0,
+                          at[1] if is_3d else at[0], at[2] if is_3d else at[1])
+  plane_args = (None, None, -1, 0, 0, 0)
+  if planes is not None:
+    assert planes.dtype == torch.uint8 and planes.stride()[3] == 1
+    t_plane_of = torch.tensor(plane_of, dtype=torch.int32).to(device)
+    plane_args = (planes.data_ptr(), t_plane_of.data_ptr(), int(pad_plane)) + tuple(
+        planes.stride()[:3])
+  status = lib.pcl_crop_observe(
+      handle, C.byref(crop_spec), None if board is None else board.data_ptr(),
+      None if state is None else state.data_ptr(), curtains, C.byref(spec),
+      t_table.data_ptr(), None if t_valid is None else t_valid.data_ptr(), *plane_args,
+      out.data_ptr(), None if unknown is None else unknown.data_ptr(), stream)
+  if check is None:
+    _lib.check(status, 'pcl_crop_observe', handle)
+  else:
+    check(status, 'pcl_crop_observe')
   return out
 
 

@@ -60,6 +60,10 @@ def main():
   eng.curtain('#'), eng.curtain('@')
   eng.to_feature_array('P#@ ')
   eng.repaint({'#': '%'})
+  # the window through a post-processor in one launch: drape medians, and a depth past
+  # one staged chunk of the table (32 planes) in channels-last order
+  eng.to_feature_array('P#@ ' * 9, permute=(1, 2, 0), crop_spec=drapes,
+                       state=eng.new_crop_state())
   fused = pdist.FusedHandoff(eng, spec, eng.batch)
   fused.gather(); fused.gather()
   packed = torch.zeros((eng.batch, pdist.handoff_record_bytes(81)), dtype=torch.uint8, device='cuda')
