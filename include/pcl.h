@@ -492,6 +492,70 @@ int pcl_step(pcl_handle* h, const int32_t* d_actions, const pcl_outputs* out,
 int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps,
             const pcl_outputs* out, void* stream);
 
+/* A rollout (pcl_rollout): what each of T steps produced, kept in caller-owned [T, B, ...]
+ * buffers.  Every d_* field is a DEVICE pointer and NULL means "not kept"; the spec
+ * pointers are HOST pointers read during the call.  Slot t of a [T, B, ...] buffer starts
+ * t * B * (elements per env) elements from its base.
+ *   Per-step outputs, as pcl_outputs after step t: d_reward i32 [T, B] (int-reward
+ *   programs) or d_reward_f64 f64 [T, B] (float-reward programs; the other one is ignored),
+ *   d_has_reward u8 [T, B], d_discount f32 [T, B], d_done u8 [T, B].
+ *   d_attached: the attached cropper's view after every step, u8 [T, B, crop rows, crop
+ *   cols].  The attached cropper is the handle's own (pcl_attach_cropper, run inside the
+ *   step kernel) or, for programs without that epilogue, `crop` below.
+ *   crop, d_crop_state, d_crop: a cropper run after every step (pcl_crop(crop, board,
+ *   d_crop, d_crop_state)), for handles with no cropper attached; its view goes to
+ *   slot t of d_attached when that is kept, else to d_crop (u8 [B, crop rows, crop cols]).
+ *   observe, ...: one post-processor after every step, NULL = none.  With observe_crop
+ *   NULL it is pcl_observe over the board; with it, pcl_crop_observe over that window
+ *   (its corner in d_observe_state).  d_view is the base of slot 0, view_stride_t the
+ *   ELEMENTS between slots, and observe's strides address one slot.  Over the board a
+ *   depth past 32 is split into launches of at most 32 planes, and d_table then holds the
+ *   tables of those launches one after another, [128, n] each (for depth <= 32 that is
+ *   [128, depth]); over a window d_table is [128, depth].  d_unknown (i32 [1], may be
+ *   NULL) is set to 1 when any step's view met an unknown character. */
+struct pcl_crop_spec;
+struct pcl_observe_spec;
+typedef struct pcl_rollout_rec {
+  int32_t* d_reward;
+  double* d_reward_f64;
+  uint8_t* d_has_reward;
+  float* d_discount;
+  uint8_t* d_done;
+  uint8_t* d_attached;
+  const struct pcl_crop_spec* crop;
+  int32_t* d_crop_state;
+  uint8_t* d_crop;
+  const struct pcl_observe_spec* observe;
+  const struct pcl_crop_spec* observe_crop;
+  int32_t* d_observe_state;
+  const void* d_table;
+  const uint8_t* d_valid;
+  int32_t* d_unknown;
+  void* d_view;
+  int64_t view_stride_t;
+} pcl_rollout_rec;
+
+/* T = `steps` steps from one call: step t is pcl_step(h, d_actions + t * B *
+ * actions_per_env, out), then the attached cropper, then rec's observer: the launches
+ * pcl_step, pcl_crop and pcl_observe / pcl_crop_observe would make, in that order, with
+ * what they wrote sent to slot t of rec's buffers.  rec == NULL keeps nothing: that is
+ * pcl_run.  The board stays out->d_board at every step (boards are not kept: an identity
+ * repaint as the observer keeps them).  Afterwards `out` and the attached cropper's view
+ * hold step T-1's values, as after T pcl_step calls.
+ * Without auto_reset, an env frozen at step t (game over before it) writes nothing in that
+ * step; its slots of the kept outputs then hold done 1, has_reward 0, reward 0 and discount
+ * 0.0, and its view slots the view of its unchanged board.  (When the outputs are kept,
+ * `out` of an env frozen at step T-1 holds that record too.)
+ * Everything is checked once, with the statuses of the single entry points (a tracking list
+ * naming a drape is PCL_ERR_UNSUPPORTED: no curtains are exported between steps); then the
+ * launches are enqueued with no allocation and no host synchronisation, so the call can be
+ * captured into a CUDA graph.  Consecutive step launches are block-chained as pcl_run's
+ * are when no other kernel lies between them (no observer, no cropper after the step). */
+int pcl_rollout(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
+                const pcl_rollout_rec* rec, void* stream);
+/* sizeof(pcl_rollout_rec), for bindings to verify their layout at load time. */
+int pcl_rollout_rec_size(void);
+
 /* `steps` pcl_step()s issued from one C call over several handles in rotation:
  * step t advances handles[t % n_handles] with d_actions[t] (HOST array of `steps`
  * device pointers, each i32 [B, actions_per_env] of that handle) into
@@ -531,7 +595,6 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
  * (the curtains are not passed here: use pcl_crop_tracking), return their status
  * (PCL_ERR_UNSUPPORTED for the drape) with no env stepped. */
 #define PCL_HOST_SLOTS 8
-struct pcl_crop_spec;
 int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
                         const pcl_outputs* out, const struct pcl_crop_spec* crop,
                         uint8_t* d_crop, int32_t* d_crop_state, uint8_t* h_view,

@@ -183,6 +183,17 @@ class ObserveSpec(C.Structure):
               ('stride_d', C.c_int64), ('stride_r', C.c_int64), ('stride_c', C.c_int64)]
 
 
+class RolloutRec(C.Structure):
+  """include/pcl.h pcl_rollout_rec: [T, B, ...] destinations of a rollout (NULL = not kept)."""
+  _fields_ = [('d_reward', C.c_void_p), ('d_reward_f64', C.c_void_p),
+              ('d_has_reward', C.c_void_p), ('d_discount', C.c_void_p), ('d_done', C.c_void_p),
+              ('d_attached', C.c_void_p),
+              ('crop', C.POINTER(CropSpec)), ('d_crop_state', C.c_void_p), ('d_crop', C.c_void_p),
+              ('observe', C.POINTER(ObserveSpec)), ('observe_crop', C.POINTER(CropSpec)),
+              ('d_observe_state', C.c_void_p), ('d_table', C.c_void_p), ('d_valid', C.c_void_p),
+              ('d_unknown', C.c_void_p), ('d_view', C.c_void_p), ('view_stride_t', C.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol include/pcl.h declares.
 SYMBOLS = {
     'pcl_abi_version': (C.c_int, []),
@@ -196,6 +207,9 @@ SYMBOLS = {
     'pcl_reset': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_step': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Outputs), C.c_void_p]),
     'pcl_run': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs), C.c_void_p]),
+    'pcl_rollout': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs),
+                              C.POINTER(RolloutRec), C.c_void_p]),
+    'pcl_rollout_rec_size': (C.c_int, []),
     'pcl_step_host': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Outputs),
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),
@@ -267,6 +281,10 @@ def load():
     raise PclLibraryError('struct layout mismatch between include/pcl.h and _lib.py: library '
                           '%s, binding %s (pcl_spec, pcl_state, pcl_outputs, pcl_crop_spec)' % (
                               list(sizes), mine))
+  if lib.pcl_rollout_rec_size() != C.sizeof(RolloutRec):
+    raise PclLibraryError('struct layout mismatch between include/pcl.h and _lib.py: '
+                          'pcl_rollout_rec is %d bytes in the library, %d in the binding' % (
+                              lib.pcl_rollout_rec_size(), C.sizeof(RolloutRec)))
   _lib = lib
   return lib
 

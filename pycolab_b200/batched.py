@@ -62,6 +62,26 @@ class StepResult(object):
     return iter((self.board, self.reward, self.discount))
 
 
+class Trajectory(object):
+  """What `BatchedEngine.rollout` kept of T steps, each a [T, B, ...] device tensor.
+
+  reward: i32 [T, B] (f64 for games whose rewards are not integers, as `reward`);
+  has_reward, done: u8 [T, B]; discount: f32 [T, B].  Slot t holds what play() leaves in
+  the engine's outputs after step t; an env frozen at step t (auto_reset off) holds done 1,
+  has_reward 0, reward 0 and discount 0.0.  view: the observer's result of every step,
+  [T] + what to_feature_array / to_array / repaint return for one step, or None.
+  attached: u8 [T, B, rows, cols], the attached cropper's view of every step, or None.
+  unknown: i32 [1] for an ObservationToArray observer, 1 when a step met a character
+  outside its mapping; else None.
+  Pass the Trajectory as `out=` to a later rollout of the same shape to reuse its buffers.
+  """
+  __slots__ = ('reward', 'has_reward', 'discount', 'done', 'view', 'attached', 'unknown')
+
+  def __init__(self, reward, has_reward, discount, done, view, attached, unknown):
+    self.reward, self.has_reward, self.discount, self.done = reward, has_reward, discount, done
+    self.view, self.attached, self.unknown = view, attached, unknown
+
+
 class BatchedEngine(object):
 
   def __init__(self, games, batch=None, device=0, auto_reset=True, rng_seed=0,
@@ -211,6 +231,7 @@ class BatchedEngine(object):
     self._crop_dev = None
     self._crop_out = None
     self._attached = None       # attach_cropper: (spec, state, out, runs inside the step kernel)
+    self._tables = None         # rollout: id(observer), over a window -> its device tables
 
     self._spec = g0.make_spec(self.auto_reset)
     handle = C.c_void_p()
@@ -292,6 +313,156 @@ class BatchedEngine(object):
     _lib.check(self._lib.pcl_run(self._h, actions.data_ptr(), int(actions.shape[0]),
                                  C.byref(self._out), self._stream()), 'pcl_run', self._h)
     return self._result()
+
+  def rollout(self, actions, observer=None, crop_spec=None, state=None, keep_attached=False,
+              out=None):
+    """T steps from one C call (`pcl_rollout`), keeping every step's outputs.
+
+    actions: int32 [T, B] or [T, B, actions_per_env] on the device.  Each step is play(),
+    then the attached cropper, then `observer` (a `rendering.ObservationToFeatureArray`,
+    `ObservationToArray` or `ObservationCharacterRepainter`) over the board or, with
+    `crop_spec`, over that cropper's window (its corner in `state`), as
+    to_feature_array / to_array / repaint would run it.  Returns a `Trajectory`; with
+    keep_attached, it also holds the attached cropper's view of every step.  Afterwards
+    the engine's outputs and the attached view are step T-1's, as after T play()s.
+
+    An ObservationToArray raises RuntimeError, as to_array does, when any step met a
+    character outside its mapping; the flag is read once per call, and not at all while
+    the stream is being captured (read `Trajectory.unknown` then).  `out`: a Trajectory
+    of an earlier rollout of the same shape, whose buffers are reused, so that a captured
+    rollout replays into fixed memory."""
+    torch = _torch()
+    if not self._showtime:
+      raise RuntimeError('rollout() cannot be called until the Engine is placed in "play '
+                         'mode" via the its_showtime() method.')
+    if not (torch.is_tensor(actions) and actions.is_cuda and actions.dtype == torch.int32 and
+            actions.is_contiguous()):
+      raise TypeError('rollout actions are a contiguous int32 CUDA tensor [T, B(, words)]')
+    if actions.dim() < 2 or int(np.prod(actions.shape[1:])) != self.batch * self.actions_per_env:
+      raise ValueError('expected [T, %d] actions of %d words per env, got %s' % (
+          self.batch, self.actions_per_env, tuple(actions.shape)))
+    T, B = int(actions.shape[0]), self.batch
+    att = self._attached
+    if keep_attached and att is None:
+      raise ValueError('keep_attached needs a cropper attached with attach_cropper()')
+    obs = self._rollout_observer(observer, crop_spec)
+    crop = crop_spec if obs is not None else None
+    rows, cols = (crop.rows, crop.cols) if crop is not None else (self.rows, self.cols)
+    dev = self.device
+    want = dict(reward=((T, B), self.reward.dtype), has_reward=((T, B), torch.uint8),
+                discount=((T, B), torch.float32), done=((T, B), torch.uint8))
+    if keep_attached:
+      want['attached'] = ((T, B, att[0].rows, att[0].cols), torch.uint8)
+    if obs is not None:
+      base = [obs['depth'], rows, cols] if obs['is_3d'] else [rows, cols]
+      perm = obs['permute'] if obs['permute'] is not None else range(len(base))
+      want['view'] = (tuple([T, B] + [base[i] for i in perm]), obs['dtype'])
+      if obs['check']:
+        want['unknown'] = ((1,), torch.int32)
+    traj = out if out is not None else Trajectory(*[None] * 7)
+    for name in Trajectory.__slots__:
+      got = getattr(traj, name)
+      if name not in want:
+        if out is None:
+          continue
+        if got is not None:
+          raise ValueError('out= holds a %s this rollout does not produce' % name)
+      elif out is None:
+        setattr(traj, name, torch.empty(want[name][0], dtype=want[name][1], device=dev))
+      elif got is None or tuple(got.shape) != want[name][0] or got.dtype != want[name][1]:
+        raise ValueError('out=.%s is not %s %s' % (name, want[name][1], want[name][0]))
+    rec = _lib.RolloutRec()
+    if self.game.float_reward:
+      rec.d_reward_f64 = traj.reward.data_ptr()
+    else:
+      rec.d_reward = traj.reward.data_ptr()
+    rec.d_has_reward, rec.d_done = traj.has_reward.data_ptr(), traj.done.data_ptr()
+    rec.d_discount = traj.discount.data_ptr()
+    if keep_attached:
+      rec.d_attached = traj.attached.data_ptr()
+    if att is not None and not att[3]:          # the cropper that _after_step runs
+      rec.crop = C.pointer(att[0])
+      rec.d_crop_state, rec.d_crop = att[1].data_ptr(), att[2].data_ptr()
+    view = None
+    if obs is not None:
+      spec = obs['spec'](traj.view)
+      rec.observe = C.pointer(spec)
+      if crop is not None:
+        rec.observe_crop = C.pointer(crop)
+        rec.d_observe_state = None if state is None else state.data_ptr()
+      rec.d_table = obs['table'].data_ptr()
+      rec.d_valid = None if obs['valid'] is None else obs['valid'].data_ptr()
+      if obs['check']:
+        traj.unknown.zero_()
+        rec.d_unknown = traj.unknown.data_ptr()
+      rec.d_view = traj.view.data_ptr()
+      rec.view_stride_t = traj.view.stride()[0]
+    # an empty tensor has no address; a rollout of no step reads no action
+    d_actions = actions.data_ptr() if T else self._actions.data_ptr()
+    status = self._lib.pcl_rollout(self._h, d_actions, T, C.byref(self._out), C.byref(rec),
+                                   self._stream())
+    for spec in (crop, None if att is None else att[0]):
+      if spec is not None:
+        _check_crop(status, 'pcl_rollout', self._h, spec)
+    _lib.check(status, 'pcl_rollout', self._h)
+    if obs is not None and obs['check'] and not torch.cuda.is_current_stream_capturing():
+      if int(traj.unknown[0]):
+        raise RuntimeError(
+            'This ObservationToArray only knows array values for the characters {}, but it '
+            'received an observation with a character not in that set'.format(
+                ''.join(observer._value_mapping.keys())))
+    return traj
+
+  def _rollout_observer(self, observer, crop_spec):
+    """What `rollout` launches for `observer`: its table (on the device, cached per
+    observer object), valid mask, element type, depth, permute and whether it checks for
+    unknown characters; None without an observer."""
+    from pycolab_b200 import observers, rendering
+    if observer is None:
+      return None
+    torch = _torch()
+    if isinstance(observer, rendering.ObservationToFeatureArray):
+      if not self.game.occlusion_in_layers or self.game.layers is not None:
+        raise NotLoweredError(
+            'rollout() computes feature planes from the board, so it serves games whose '
+            'layers are the occluded board (occlusion_in_layers=True, no host-composed '
+            'layers); call to_feature_array() after each play() for this game')
+      table = observers.feature_table(observer._layers, present=self.chars)
+      valid, is_3d, permute, check = None, True, observer._permute, False
+    elif isinstance(observer, rendering.ObservationToArray):
+      table, valid, is_3d = observer._table, observer._valid, observer._is_3d
+      permute, check = observer._permute, True
+    elif isinstance(observer, rendering.ObservationCharacterRepainter):
+      table, valid, is_3d, permute, check = observer._table, None, False, None, False
+    else:
+      raise TypeError('a rollout observer is an ObservationToFeatureArray, ObservationToArray '
+                      'or ObservationCharacterRepainter, not %r' % type(observer).__name__)
+    depth, size = table.shape[1], table.dtype.itemsize
+    windowed = crop_spec is not None
+    if self._tables is None:
+      self._tables = {}
+    key = (id(observer), windowed)
+    if key not in self._tables:
+      # Over the board, pcl_rollout reads the table of each launch of <= 32 planes in turn.
+      chunks = [table] if windowed else [table[:, k0:k0 + n]
+                                         for k0, n in observers.plane_chunks(depth)]
+      flat = np.concatenate([np.ascontiguousarray(c).reshape(-1) for c in chunks])
+      t_table = torch.from_numpy(flat.view(observers._CONTAINER[size])).to(self.device)
+      t_valid = None if valid is None else torch.from_numpy(valid).to(self.device)
+      self._tables[key] = (observer, t_table, t_valid)    # the observer keeps its id unique
+    _, t_table, t_valid = self._tables[key]
+
+    def spec(view):
+      """The pcl_observe_spec of one slot of `view` [T, B, permuted axes]."""
+      base = [0, 1, 2] if is_3d else [0, 1]
+      perm = list(permute) if permute is not None else base
+      strides = list(view.stride())[2:]
+      at = {d: strides[perm.index(d)] for d in base}
+      return _lib.ObserveSpec(depth, observers._CODE_OF_SIZE[size], view.stride()[1],
+                              at[0] if is_3d else 0, at[1] if is_3d else at[0],
+                              at[2] if is_3d else at[1])
+    return dict(table=t_table, valid=t_valid, is_3d=is_3d, permute=permute, depth=depth,
+                dtype=observers.torch_dtype(table.dtype), check=check, spec=spec)
 
   def _host_buffers(self, slot, view_shape):
     """Pinned staging of one pipeline slot (allocated on first use)."""

@@ -513,25 +513,6 @@ int pcl_step(pcl_handle* h, const int32_t* d_actions, const pcl_outputs* out, vo
   return launch(h, p, (cudaStream_t)stream);
 }
 
-int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
-            void* stream) {
-  Range nvtx_range("pcl_run");
-  const int r = check_ready(h, out, (cudaStream_t)stream);
-  if (r != PCL_OK) return r;
-  if (!d_actions || steps < 0) return PCL_ERR_INVALID;
-  StepParams p = h->base;
-  p.mode = pcl::MODE_STEP;
-  p.out = *out;
-  Footprint run;
-  run.h = nullptr;
-  for (int t = 0; t < steps; ++t) {
-    p.actions = d_actions + (int64_t)t * h->batch * h->actions_per_env;
-    const int e = launch(h, p, (cudaStream_t)stream, &run);
-    if (e != PCL_OK) return e;
-  }
-  return PCL_OK;
-}
-
 int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const* d_actions,
                  const pcl_outputs* const* outs, int steps, void* stream) {
   Range nvtx_range("pcl_run_many");
@@ -800,6 +781,53 @@ pcl::CropParams crop_params(const pcl_handle* h, const pcl_crop_spec* crop,
   p.cols_recip = crop->cols > 1 ? (uint32_t)(0x100000000ull / (uint32_t)crop->cols) + 1u : 0u;
   return p;
 }
+
+int crop_launch(pcl_handle* h, const pcl::CropParams& p, cudaStream_t s) {
+  return launched(h, pcl::launch_crop(p, s), "launch_crop");
+}
+
+// What pcl_observe and pcl_crop_observe accept of a post-processor's spec; depth is
+// bounded by `max_depth` (0: any).
+bool observe_spec_ok(const pcl_observe_spec* spec, int max_depth) {
+  return spec->depth >= 1 && (max_depth == 0 || spec->depth <= max_depth) && spec->dtype >= 0 &&
+         spec->dtype <= 5;
+}
+
+// Bytes per element of a pcl_observe_spec dtype.
+int element_bytes(int dtype) { return dtype == 0 ? 1 : dtype == 5 ? 2 : dtype >= 3 ? 8 : 4; }
+
+pcl::ObserveParams observe_params(const pcl_handle* h, const pcl_observe_spec* spec,
+                                  const void* d_table, const uint8_t* d_valid,
+                                  const uint8_t* d_board, void* d_out, int32_t* d_unknown) {
+  pcl::ObserveParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
+  p.depth = spec->depth; p.dtype = spec->dtype;
+  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
+  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
+  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
+  p.table = d_table; p.valid = d_valid; p.board = d_board; p.out = d_out;
+  p.unknown = d_unknown;
+  return p;
+}
+
+// pcl_crop_observe's launch over the board (the caller adds curtains or layer planes).
+pcl::CropObserveParams crop_observe_params(const pcl_handle* h, const pcl_crop_spec* crop,
+                                           const uint8_t* d_board, int32_t* d_crop_state,
+                                           const pcl_observe_spec* spec, const void* d_table,
+                                           const uint8_t* d_valid, void* d_out,
+                                           int32_t* d_unknown) {
+  pcl::CropObserveParams p;
+  memset(&p, 0, sizeof(p));
+  p.crop = crop_params(h, crop, d_board, nullptr, d_crop_state);
+  p.depth = spec->depth; p.dtype = spec->dtype;
+  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
+  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
+  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
+  p.table = d_table; p.valid = d_valid; p.out = d_out; p.unknown = d_unknown;
+  p.pad_plane = -1;
+  return p;
+}
 }  // namespace
 
 int pcl_attach_cropper(pcl_handle* h, const pcl_crop_spec* crop, uint8_t* d_crop,
@@ -840,7 +868,7 @@ int pcl_crop_tracking(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d
     if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
     p.curtains[i] = d_curtains[i];
   }
-  return launched(h, pcl::launch_crop(p, (cudaStream_t)stream), "launch_crop");
+  return crop_launch(h, p, (cudaStream_t)stream);
 }
 
 int pcl_crop_observe(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_board,
@@ -852,24 +880,18 @@ int pcl_crop_observe(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   Range nvtx_range("pcl_crop_observe");
   if (!h || !crop || !spec || !d_table || !d_out) return PCL_ERR_INVALID;
   if (d_planes ? !d_plane_of : !d_board) return PCL_ERR_INVALID;
-  if (spec->depth < 1 || spec->dtype < 0 || spec->dtype > 5) return PCL_ERR_INVALID;
+  if (!observe_spec_ok(spec, 0)) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
   const int ok = crop_spec_ok(h, crop);
   if (ok != PCL_OK) return ok;
-  pcl::CropObserveParams p;
-  memset(&p, 0, sizeof(p));
-  p.crop = crop_params(h, crop, d_board, nullptr, d_crop_state);
+  pcl::CropObserveParams p = crop_observe_params(h, crop, d_board, d_crop_state, spec, d_table,
+                                                 d_valid, d_out, d_unknown);
   for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
     if (crop->track[i] > 0) continue;
     if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
     if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
     p.crop.curtains[i] = d_curtains[i];
   }
-  p.depth = spec->depth; p.dtype = spec->dtype;
-  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
-  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
-  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
-  p.table = d_table; p.valid = d_valid; p.out = d_out; p.unknown = d_unknown;
   p.planes = d_planes; p.plane_of = d_plane_of; p.pad_plane = d_planes ? pad_plane : -1;
   p.plane_stride_b = plane_stride_b; p.plane_stride_d = plane_stride_d;
   p.plane_stride_r = plane_stride_r;
@@ -952,19 +974,162 @@ int pcl_observe(pcl_handle* h, const pcl_observe_spec* spec, const void* d_table
                 int32_t* d_unknown, void* stream) {
   Range nvtx_range("pcl_observe");
   if (!h || !spec || !d_table || !d_board || !d_out) return PCL_ERR_INVALID;
-  if (spec->depth < 1 || spec->depth > 32 || spec->dtype < 0 || spec->dtype > 5)
-    return PCL_ERR_INVALID;
-  pcl::ObserveParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
-  p.depth = spec->depth; p.dtype = spec->dtype;
-  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
-  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
-  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
-  p.table = d_table; p.valid = d_valid; p.board = d_board; p.out = d_out;
-  p.unknown = d_unknown;
-  return launched(h, pcl::launch_observe(p, (cudaStream_t)stream), "launch_observe");
+  if (!observe_spec_ok(spec, 32)) return PCL_ERR_INVALID;
+  return launched(h, pcl::launch_observe(observe_params(h, spec, d_table, d_valid, d_board, d_out,
+                                                        d_unknown), (cudaStream_t)stream),
+                  "launch_observe");
 }
+
+}  // extern "C"
+
+namespace {
+
+// Slot t of a [T, B, per_env] buffer of T elements, or NULL when the buffer is not kept.
+template <typename T>
+T* slot(T* base, int t, int64_t per_env, int batch) {
+  return base ? base + (int64_t)t * batch * per_env : nullptr;
+}
+
+// Everything pcl_rollout checks, before anything is enqueued.
+int rollout_ok(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
+               const pcl_rollout_rec* rec, cudaStream_t s) {
+  const int r = check_ready(h, out, s);
+  if (r != PCL_OK) return r;
+  if (!d_actions || steps < 0) return PCL_ERR_INVALID;
+  if (!rec) return PCL_OK;
+  if (float_rewards(h) && rec->d_reward && !rec->d_reward_f64) return PCL_ERR_INVALID;
+  if (rec->crop) {                 // the cropper after each step: the handle has none attached
+    if (h->base.has_cropper || !rec->d_crop) return PCL_ERR_INVALID;
+    const int ok = crop_spec_ok(h, rec->crop);
+    if (ok != PCL_OK) return ok;
+    if (tracks_drape(rec->crop)) return PCL_ERR_UNSUPPORTED;   // no curtains between steps
+  }
+  if (rec->d_attached && !rec->crop && !h->base.has_cropper) return PCL_ERR_INVALID;
+  const pcl_observe_spec* spec = rec->observe;
+  if (!spec) return PCL_OK;
+  if (!rec->d_table || !observe_spec_ok(spec, 0)) return PCL_ERR_INVALID;
+  if (steps > 0 && !rec->d_view) return PCL_ERR_INVALID;     // no step, no view written
+  if ((uintptr_t)rec->d_view % element_bytes(spec->dtype)) return PCL_ERR_INVALID;
+  if (rec->observe_crop) {
+    const int ok = crop_spec_ok(h, rec->observe_crop);
+    if (ok != PCL_OK) return ok;
+    if (tracks_drape(rec->observe_crop)) return PCL_ERR_UNSUPPORTED;
+  }
+  return PCL_OK;
+}
+
+// pcl_rollout once checked (rollout_ok): the launches of every step, then step T-1's
+// outputs and attached view copied to where pcl_step and the cropper leave them.
+int rollout_enqueue(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
+                    const pcl_rollout_rec* rec, cudaStream_t s) {
+  static const pcl_rollout_rec kNothing = {};
+  const pcl_rollout_rec& x = rec ? *rec : kNothing;
+  const int64_t B = h->batch;
+  const bool f64 = float_rewards(h);
+  int32_t* keep_reward = f64 ? nullptr : x.d_reward;
+  double* keep_reward_f64 = f64 ? x.d_reward_f64 : nullptr;
+  // The attached cropper: inside the step kernel, or a crop launch after it.  The epilogue
+  // skips frozen envs, whose kept views must still be written: without auto_reset a kept
+  // view comes from a crop launch of the same cropper.
+  const bool in_step = h->base.has_cropper && !(x.d_attached && !h->spec.auto_reset);
+  const bool has_after = x.crop || (h->base.has_cropper && !in_step);
+  pcl::CropParams after = h->base.cropper;  // the crop launch after each step (has_after)
+  if (x.crop) after = crop_params(h, x.crop, out->d_board, x.d_crop, x.d_crop_state);
+  after.board = out->d_board;
+  uint8_t* view = after.out;       // where the attached cropper's view lives between calls
+  const int64_t view_cells = (int64_t)after.crop.rows * after.crop.cols;
+  // A frozen env writes nothing: its kept outputs hold the fixed record.
+  if (!h->spec.auto_reset && steps > 0) {
+    const size_t n = (size_t)steps * B;
+    if (keep_reward) PCL_CUDA(h, cudaMemsetAsync(keep_reward, 0, n * 4, s));
+    if (keep_reward_f64) PCL_CUDA(h, cudaMemsetAsync(keep_reward_f64, 0, n * 8, s));
+    if (x.d_has_reward) PCL_CUDA(h, cudaMemsetAsync(x.d_has_reward, 0, n, s));
+    if (x.d_discount) PCL_CUDA(h, cudaMemsetAsync(x.d_discount, 0, n * 4, s));
+    if (x.d_done) PCL_CUDA(h, cudaMemsetAsync(x.d_done, 1, n, s));
+  }
+  // Step launches chain only to a step launch right before them.
+  const bool chain = !x.observe && !has_after;
+  StepParams p = h->base;
+  p.mode = pcl::MODE_STEP;
+  p.out = *out;
+  p.has_cropper = in_step;
+  const pcl_observe_spec* spec = x.observe;
+  const int elem = spec ? element_bytes(spec->dtype) : 0;
+  Footprint run;
+  run.h = nullptr;
+  for (int t = 0; t < steps; ++t) {
+    p.actions = d_actions + (int64_t)t * B * h->actions_per_env;
+    if (keep_reward) p.out.d_reward = slot(keep_reward, t, 1, B);
+    if (keep_reward_f64) p.out.d_reward_f64 = slot(keep_reward_f64, t, 1, B);
+    if (x.d_has_reward) p.out.d_has_reward = slot(x.d_has_reward, t, 1, B);
+    if (x.d_discount) p.out.d_discount = slot(x.d_discount, t, 1, B);
+    if (x.d_done) p.out.d_done = slot(x.d_done, t, 1, B);
+    if (in_step && x.d_attached) p.cropper.out = slot(x.d_attached, t, view_cells, B);
+    if (!chain) run.h = nullptr;
+    int e = launch(h, p, s, &run);
+    if (e != PCL_OK) return e;
+    if (has_after) {
+      after.out = x.d_attached ? slot(x.d_attached, t, view_cells, B) : view;
+      e = crop_launch(h, after, s);
+      if (e != PCL_OK) return e;
+    }
+    if (!spec) continue;
+    uint8_t* base = (uint8_t*)x.d_view + t * x.view_stride_t * elem;
+    if (x.observe_crop) {
+      e = launched(h, pcl::launch_crop_observe(crop_observe_params(
+                          h, x.observe_crop, out->d_board, x.d_observe_state, spec, x.d_table,
+                          x.d_valid, base, x.d_unknown), s), "launch_crop_observe");
+      if (e != PCL_OK) return e;
+      continue;
+    }
+    // Over the board, at most 32 planes per launch, each with its own table.
+    const uint8_t* table = (const uint8_t*)x.d_table;
+    for (int k0 = 0; k0 < spec->depth; k0 += 32) {
+      pcl_observe_spec chunk = *spec;
+      chunk.depth = spec->depth - k0 < 32 ? spec->depth - k0 : 32;
+      e = launched(h, pcl::launch_observe(observe_params(h, &chunk, table, x.d_valid, out->d_board,
+                                                         base + k0 * spec->stride_d * elem,
+                                                         x.d_unknown), s), "launch_observe");
+      if (e != PCL_OK) return e;
+      table += 128 * chunk.depth * elem;
+    }
+  }
+  if (steps == 0) return PCL_OK;
+  // Step T-1's values where pcl_step and the cropper leave them.
+  auto last = [&](void* dst, const void* src, size_t bytes) -> int {
+    if (src && dst != src) PCL_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+    return PCL_OK;
+  };
+  int e = last(out->d_reward, slot(keep_reward, steps - 1, 1, B), B * 4);
+  if (e == PCL_OK) e = last(out->d_reward_f64, slot(keep_reward_f64, steps - 1, 1, B), B * 8);
+  if (e == PCL_OK) e = last(out->d_has_reward, slot(x.d_has_reward, steps - 1, 1, B), B);
+  if (e == PCL_OK) e = last(out->d_discount, slot(x.d_discount, steps - 1, 1, B), B * 4);
+  if (e == PCL_OK) e = last(out->d_done, slot(x.d_done, steps - 1, 1, B), B);
+  if (e == PCL_OK) e = last(view, slot(x.d_attached, steps - 1, view_cells, B), B * view_cells);
+  return e;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pcl_rollout(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
+                const pcl_rollout_rec* rec, void* stream) {
+  Range nvtx_range("pcl_rollout");
+  const int r = rollout_ok(h, d_actions, steps, out, rec, (cudaStream_t)stream);
+  if (r != PCL_OK) return r;
+  return rollout_enqueue(h, d_actions, steps, out, rec, (cudaStream_t)stream);
+}
+
+int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
+            void* stream) {
+  Range nvtx_range("pcl_run");
+  const int r = rollout_ok(h, d_actions, steps, out, nullptr, (cudaStream_t)stream);
+  if (r != PCL_OK) return r;
+  return rollout_enqueue(h, d_actions, steps, out, nullptr, (cudaStream_t)stream);
+}
+
+int pcl_rollout_rec_size(void) { return (int)sizeof(pcl_rollout_rec); }
 
 int pcl_error_codes(pcl_handle* h, int32_t* d_out, void* stream) {
   if (!h || !d_out) return PCL_ERR_INVALID;

@@ -70,6 +70,20 @@ def main():
   eng.pack_handoff(eng.crop(spec), packed)
   torch.cuda.synchronize()
   print('ok crop / layers / export / observe / handoff kernels')
+  # a rollout at B=7 with quits (action 5), so envs restart inside it: the attached cropper
+  # in the step kernel into its [T, B] slots, and 33 feature planes of a window per step
+  from pycolab_b200 import rendering
+  eng.attach_cropper(spec)
+  acts = rs.randint(0, 6, size=(20, eng.batch)).astype(np.int32)
+  traj = eng.rollout(torch.from_numpy(acts).cuda(), keep_attached=True,
+                     observer=rendering.ObservationToFeatureArray('P#@ ' * 8 + '+'),
+                     crop_spec=spec, state=eng.new_crop_state())
+  eng.rollout(torch.from_numpy(acts).cuda(), observer=rendering.ObservationToFeatureArray(
+      'P#@ ' * 9))                       # over the board: launches of 32 and 4 planes
+  eng.attach_cropper(None)
+  torch.cuda.synchronize()
+  assert int(traj.done.sum()) > 0
+  print('ok rollout')
   wide = levels.scrolly_maze_level(9, world_shape=(41, 161), board_shape=(12, 100))
   run('scrolly_maze_step W=100', [scrolly_maze.make_game(*wide)], 5, 5)
   # Board shapes the kernel's shared-memory layout branches on: 3 segments per row, a
