@@ -429,7 +429,8 @@ typedef struct pcl_outputs {
   uint8_t* d_has_reward;  /* u8 [B]; 0 = reference returned reward None */
   float*   d_discount;    /* f32 [B]; 1.0 running / 0.0 terminated unless a directive said otherwise
                              (plot.py:104,176-199,247-260) */
-  uint8_t* d_done;        /* u8 [B]; Engine.game_over after this step */
+  uint8_t* d_done;        /* u8 [B]; Engine.game_over after this step: 0 running, 1 ended by the
+                             game, PCL_DONE_TIME_LIMIT ended by the time limit (pcl_set_time_limit) */
   double*  d_reward_f64;  /* f64 [B]; the summed reward exactly as the reference's float sum produces
                              it, 0.0 if none.  Written only by programs whose rewards are not integers
                              (PCL_PROG_T_MAZE and PCL_PROG_SEQUENCE_RECALL always, PCL_PROG_COMPILED
@@ -565,6 +566,30 @@ int pcl_rollout_rec_size(void);
  * CUDA graph on `stream`. */
 int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const* d_actions,
                  const pcl_outputs* const* outs, int steps, void* stream);
+
+/* Episode time limit.  pcl_set_time_limit(h, L) with L >= 1: a step that leaves an env at
+ * frame L or later ends its episode, unless the game ended it in that same step.  An env's
+ * frame is 0 after its its_showtime() frame (pcl_reset, or a restart under auto_reset) and
+ * goes up by one per step, so with the limit set from the start the L-th step after a
+ * (re)start is the last one.  Such a step reports done = PCL_DONE_TIME_LIMIT, and its plot
+ * record's game-over word holds the same value; a game's own ending (terminate_episode,
+ * including a game's own step limit such as box_world's max_num_steps) stays done 1.  A
+ * truncated step's reward, has_reward, discount and board are what the step produced
+ * without a limit: the discount is the game's (1.0 unless a directive changed it), which is
+ * what value bootstrapping across a time limit wants.  The next step treats the env as after
+ * any ending: a restart under auto_reset (action ignored, templates restored, episode count
+ * + 1, random streams continued), else the env stays frozen and a rollout's slots hold the
+ * frozen record (done 1).  A masked pcl_reset starts an env's count afresh, which is how a
+ * host staggers its envs' episodes.
+ * L = 0 (the default) is no limit: every output, record and kernel behaves as without this
+ * call.  The limit is read when a step is launched: the next pcl_step, pcl_run, pcl_rollout,
+ * pcl_run_many and pcl_step_host* of the handle use it, and a CUDA graph captured earlier
+ * keeps the limit it was captured with.  PCL_ERR_INVALID for a NULL handle or L < 0.
+ * Cost (DESIGN.md section 5; H100 80GB HBM3, 700 W): with the limit off bench.py's C2 step is
+ * 6.33-6.39 us against the parent's 6.37; a wave of restarts the limit causes on C2 adds about
+ * 7.5 us once per L + 1 steps. */
+#define PCL_DONE_TIME_LIMIT 2
+int pcl_set_time_limit(pcl_handle* h, int32_t max_frames);
 
 /* The host-buffer and hand-off entry points below (pcl_step_host, pcl_step_host_async,
  * pcl_pack_handoff, pcl_pack_handoff_peers, pcl_crop_handoff) carry an int32 reward in their

@@ -28,6 +28,7 @@ DIR_NONE, DIR_ADD_REWARD, DIR_TERMINATE, DIR_DEFAULT_DISCOUNT, DIR_Z_ORDER = ran
 HOST_SLOTS = 8               # pcl_step_host_async completion slots
 NEVER = -(2 ** 31)           # INT32_MIN: "-inf"/None frame
 ACTION_NONE = -1
+DONE_TIME_LIMIT = 2          # done (and plot game-over word) of an episode the time limit ended
 
 OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_UNBOUND, ERR_NOMEM = 0, -1, -2, -3, -4, -5
 
@@ -215,6 +216,7 @@ SYMBOLS = {
                                 C.c_void_p, C.c_void_p]),
     'pcl_run_many': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p),
                                C.POINTER(C.c_void_p), C.c_int, C.c_void_p]),
+    'pcl_set_time_limit': (C.c_int, [C.c_void_p, C.c_int32]),
     'pcl_step_host_async': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Outputs),
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

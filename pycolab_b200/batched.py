@@ -9,6 +9,7 @@ C ABI (`pcl_step`); there is no CPU path.
 """
 
 import ctypes as C
+import numbers
 import random
 
 import numpy as np
@@ -34,6 +35,18 @@ def _check_crop(status, what, handle, crop_spec):
   _lib.check(status, what, handle)
 
 
+def _time_limit(n):
+  """The pcl_set_time_limit value of a `time_limit` argument: None or 0 is no limit."""
+  if n is None:
+    return 0
+  if isinstance(n, bool) or not isinstance(n, numbers.Integral):
+    raise TypeError('time_limit is None or an int number of steps, got %r' % (n,))
+  if not 0 <= n < 2 ** 31:
+    raise ValueError('time_limit is None, 0 (no limit) or a number of steps below 2**31, '
+                     'got %d' % n)
+  return int(n)
+
+
 def _mt_state(stream, seed):
   """u32 [625]: the MT19937 words (624 key words + position) of a generator seeded with
   `seed`: Python's random.Random ('python') or NumPy's RandomState ('numpy')."""
@@ -50,7 +63,9 @@ class StepResult(object):
   until the next step — copy to keep, as upstream rendering.py:55-63).
   reward: i32 [B] (f64 [B] for games whose rewards are not integers, e.g. t_maze) with
   has_reward u8 [B] == 0 where the reference returns None.
-  discount: f32 [B].  done: u8 [B] (Engine.game_over).
+  discount: f32 [B].  done: u8 [B] (Engine.game_over): 0 running, 1 ended by the game, 2
+  (_lib.DONE_TIME_LIMIT) ended by the engine's time limit, with the step's own reward and
+  discount.
   """
   __slots__ = ('board', 'reward', 'has_reward', 'discount', 'done')
 
@@ -67,9 +82,10 @@ class Trajectory(object):
 
   reward: i32 [T, B] (f64 for games whose rewards are not integers, as `reward`);
   has_reward, done: u8 [T, B]; discount: f32 [T, B].  Slot t holds what play() leaves in
-  the engine's outputs after step t; an env frozen at step t (auto_reset off) holds done 1,
-  has_reward 0, reward 0 and discount 0.0.  view: the observer's result of every step,
-  [T] + what to_feature_array / to_array / repaint return for one step, or None.
+  the engine's outputs after step t; done is 0 running, 1 ended by the game, 2 ended by the
+  time limit (a truncation: the discount is the game's).  An env frozen at step t (auto_reset
+  off) holds done 1, has_reward 0, reward 0 and discount 0.0.  view: the observer's result of
+  every step, [T] + what to_feature_array / to_array / repaint return for one step, or None.
   attached: u8 [T, B, rows, cols], the attached cropper's view of every step, or None.
   unknown: i32 [1] for an ObservationToArray observer, 1 when a step met a character
   outside its mapping; else None.
@@ -85,7 +101,7 @@ class Trajectory(object):
 class BatchedEngine(object):
 
   def __init__(self, games, batch=None, device=0, auto_reset=True, rng_seed=0,
-               env_offset=0, rng_states=None, share_levels=True):
+               env_offset=0, rng_states=None, share_levels=True, time_limit=None):
     """games: list of lowered games (`lowering.LoweredGame`) or set-up `Engine`s.
     Env e uses games[e % len(games)]; with a single game the static level data
     (backdrop, immutable patterns, reset templates) is shared by all envs.
@@ -95,7 +111,9 @@ class BatchedEngine(object):
     (False: bind no RNG, for programs that can take their draws from the templates)
     MT19937 states (624 key words + position) instead of seeds.
     share_levels=False stores the static level data once PER ENV instead of once
-    per level (the reference's layout: every Engine owns its backdrop)."""
+    per level (the reference's layout: every Engine owns its backdrop).
+    time_limit: see set_time_limit; None (the default) or 0 is no limit."""
+    limit = _time_limit(time_limit)
     torch = _torch()
     self._lib = _lib.load()
     if not torch.cuda.is_available():
@@ -247,7 +265,23 @@ class BatchedEngine(object):
       self.backdrop_live = per_env([g.backdrop for g in games], np.uint8)
       _lib.check(self._lib.pcl_bind_backdrop(self._h, self.backdrop_live.data_ptr()),
                  'pcl_bind_backdrop')
+    self.time_limit = 0
+    self.set_time_limit(limit)
     self._showtime = False
+
+  def set_time_limit(self, n):
+    """End every episode after n steps (pcl_set_time_limit); None or 0: no limit.
+
+    A step that leaves an env at frame n or later (n play()s after its its_showtime() or
+    restart frame) reports done 2 (_lib.DONE_TIME_LIMIT) unless the game ended the episode
+    in that step, which stays done 1.  Reward, discount and board are the step's own.  The
+    next step restarts the env under auto_reset and freezes it otherwise, as after any
+    ending; reset(mask) starts an env's count afresh.  Upstream pycolab has no time limit:
+    with none set the engine behaves exactly as without this call.  Applies from the next
+    step; a CUDA graph captured earlier keeps the limit it was captured with."""
+    limit = _time_limit(n)
+    _lib.check(self._lib.pcl_set_time_limit(self._h, limit), 'pcl_set_time_limit')
+    self.time_limit = limit
 
   # ---------------------------------------------------------------- running
   def _stream(self):

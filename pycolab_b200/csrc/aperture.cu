@@ -134,6 +134,7 @@ aperture_step(const StepParams p) {
   if (lane == 0) {
     store_sprite(rec, sp, PCL_S_AUX0);
     rec[8 + PCL_D_AUX0] = ap0; rec[8 + PCL_D_AUX1] = ap1;
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(rec + 16, plot, dir);
     store_outputs(p.out, env, dir);
     // final render, z-order X then A: patch the staged tile (engine.py:737-759)

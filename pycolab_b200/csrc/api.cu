@@ -44,6 +44,7 @@ struct pcl_handle {
   // StepParams::board_epoch: the board buffer of the last launch, and its epoch
   const uint8_t* last_board;
   uint32_t board_epoch;
+  int time_limit;                // pcl_set_time_limit; fill_params copies it into `base`
 };
 
 namespace {
@@ -154,6 +155,7 @@ void fill_params(const pcl_handle* h, StepParams* p) {
   p->st = h->st;
   p->code = h->code_dev;
   p->backdrop_live = h->backdrop_live;
+  p->time_limit = h->time_limit;
 }
 
 // Does the handle's Backdrop run compiled code on a live curtain (pcl_bind_backdrop)?
@@ -426,6 +428,7 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   h->derive_stale = 0;
   h->last_board = nullptr;
   h->board_epoch = 0;
+  h->time_limit = 0;
   *out = h;
   return PCL_OK;
 }
@@ -487,6 +490,13 @@ int pcl_bind_backdrop(pcl_handle* h, uint8_t* d_backdrop_live) {
   if (!h || !d_backdrop_live || !live_backdrop(h->spec)) return PCL_ERR_INVALID;
   h->backdrop_live = d_backdrop_live;
   h->base.backdrop_live = d_backdrop_live;   // pcl_bind_state's fill_params copies it too
+  return PCL_OK;
+}
+
+int pcl_set_time_limit(pcl_handle* h, int32_t max_frames) {
+  if (!h || max_frames < 0) return PCL_ERR_INVALID;
+  h->time_limit = max_frames;
+  h->base.time_limit = max_frames;   // pcl_bind_state's fill_params copies it too
   return PCL_OK;
 }
 

@@ -83,6 +83,7 @@ apprehend_step(const StepParams p) {
     store_sprite(e.sprites, pl);
     store_sprite(e.sprites + PCL_SPRITE_WORDS, ball);
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = __double2loint(acc); e.plot[PCL_P_AUX1] = __double2hiint(acc);
     store_outputs(p.out, env, dir);

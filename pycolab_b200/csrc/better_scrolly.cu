@@ -151,6 +151,7 @@ better_scrolly_step(const StepParams p) {
   if (lane == 0) {
 #pragma unroll
     for (int i = 0; i < kS; ++i) store_sprite(rec + i * PCL_SPRITE_WORDS, sp[i], PCL_S_AUX1);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(rec + 48, plot, dir);
     rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);

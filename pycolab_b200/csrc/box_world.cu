@@ -139,6 +139,7 @@ box_world_step(const StepParams p) {
     pl.aux0 = steps;
     store_sprite(e.sprites, pl);
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = over_ch; e.plot[PCL_P_AUX1] = over_at;
     store_outputs(p.out, env, dir);

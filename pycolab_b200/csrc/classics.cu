@@ -123,6 +123,7 @@ classics_step(const StepParams p) {
   __syncwarp();                 // every lane has read the staged records (racecheck: WAR)
   if (lane == 0) {
     store_sprite(rec, sp, PCL_S_AUX0);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(rec + 16, plot, dir);
     rec[16 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);

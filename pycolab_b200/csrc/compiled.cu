@@ -696,6 +696,7 @@ __device__ __forceinline__ void step(const StepParams& p) {
 
   __syncwarp();
   if (lane == 0) {
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_ALL>(st->plot, plot, dir);
     dir.reward = rw.has ? rw.sum_i : 0; dir.has_reward = rw.has;   // the code's own sums
     if (p.program_arg[0]) store_outputs(p.out, env, dir, rw.has ? rw.sum_f : 0.0);

@@ -295,6 +295,7 @@ cued_catch_step(const StepParams p) {
     }
     store_drape(e.drapes, {phase, tick1, choice, tick2, last_reset, trials, pairs, 0});
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = programmed; e.plot[PCL_P_AUX1] = which;
     e.plot[PCL_P_AUX2] = ball_reset; e.plot[PCL_P_AUX3] = noisy_pay ? 1 : 0;

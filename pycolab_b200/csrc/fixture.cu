@@ -185,6 +185,7 @@ fixture_step(const StepParams p) {
   __syncwarp();
   if (lane == 0) {
     group_in(plot, st, 0);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_ALL>(st->plot, plot, dir);
     store_outputs(p.out, env, dir);
   }

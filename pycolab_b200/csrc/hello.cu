@@ -72,6 +72,7 @@ hello_step(const StepParams p) {
     e.drapes[PCL_D_AUX0] = roll_r; e.drapes[PCL_D_AUX1] = roll_c;
     e.drapes[PCL_D_LAST_FRAME] = src_d[PCL_D_LAST_FRAME];
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
   }

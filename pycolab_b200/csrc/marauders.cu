@@ -224,6 +224,7 @@ marauders_step(const StepParams p) {
 #pragma unroll
     for (int i = 0; i < kS; ++i) store_sprite(rec + i * PCL_SPRITE_WORDS, sp[i], PCL_S_AUX0);
     rec[56 + PCL_DRAPE_WORDS + PCL_D_AUX0] = marauders.aux0;
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(rec + 72, plot, dir);
     rec[72 + PCL_P_AUX0] = plot.aux0; rec[72 + PCL_P_AUX1] = plot.aux1;
     store_outputs(p.out, env, dir);

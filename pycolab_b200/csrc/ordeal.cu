@@ -171,6 +171,7 @@ ordeal_step(const StepParams p) {
   if (lane == 0) {
     store_sprite(rec, pl, PCL_S_AUX0);
     if (S > 1) store_sprite(rec + 8, dd, PCL_S_AUX0);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(rec + 32, plot, dir);
     rec[32 + PCL_P_AUX0] = has_sword; rec[32 + PCL_P_AUX1] = last_pos;
     rec[32 + PCL_P_AUX2] = next_chapter;

@@ -536,6 +536,18 @@ __device__ __forceinline__ void store_plot(int32_t* rec, const Plot& q, const Di
   }
 }
 
+// The episode time limit (pcl_set_time_limit, include/pcl.h): a step that leaves the env at
+// frame p.time_limit or later ends the episode as PCL_DONE_TIME_LIMIT, unless the game ended
+// it in this step.  Only the game-over word changes; reward, discount and board stay the
+// step's own.  Called once per step with the step's final Plot, right before store_plot /
+// store_outputs: a truncation is an ending for the next step's env_run and for the host, but
+// nothing in the step itself may act on it as on a game's ending.
+__device__ __forceinline__ void apply_time_limit(const StepParams& p, const Plot& q,
+                                                 Directives& dir) {
+  if (p.time_limit > 0 && q.frame >= p.time_limit && !dir.game_over)
+    dir.game_over = PCL_DONE_TIME_LIMIT;
+}
+
 // The step's outputs for env `env` (one lane stores them).
 __device__ __forceinline__ void store_outputs(const pcl_outputs& out, int env, const Directives& dir) {
   out.d_reward[env] = dir.reward;

@@ -70,6 +70,9 @@ struct StepParams {
   uint32_t* block_sync;
   // Program::block_chaining: how this launch waits for the kernels before it (CHAIN_*).
   int chain;
+  // pcl_set_time_limit: a step that leaves an env at this frame or later ends its episode
+  // (apply_time_limit, pcl_device.cuh); 0: no limit.
+  int time_limit;
 };
 
 // StepParams::chain (launch, api.cu; scrolly_maze.cu, "Block chaining").  CHAIN_NONE: the

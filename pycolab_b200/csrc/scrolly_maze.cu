@@ -832,6 +832,7 @@ __device__ __forceinline__ void step_env(const StepParams& p) {
   if (lane == 0) {
     store_drape(rec + 32, walls, PCL_D_AUX0);
     store_drape(rec + 32 + PCL_DRAPE_WORDS, coins, PCL_D_AUX2);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_ALL>(rec + 48, plot, dir);
     rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);

@@ -161,6 +161,7 @@ sequence_recall_step(const StepParams p) {
       r[PCL_D_AUX0] = d == DM ? covered : cleared;
     }
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = pc; e.plot[PCL_P_AUX1] = fis;
     e.plot[PCL_P_AUX2] = timeout; e.plot[PCL_P_AUX3] = (int)seq;

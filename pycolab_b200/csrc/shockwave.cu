@@ -119,6 +119,7 @@ shockwave_step(const StepParams p) {
     e.drapes[PCL_D_AUX0] = impact; e.drapes[PCL_D_AUX1] = steps;
     e.drapes[PCL_D_LAST_FRAME] = PCL_NEVER;
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
   }

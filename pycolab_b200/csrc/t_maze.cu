@@ -298,6 +298,7 @@ t_maze_step(const StepParams p) {
 #pragma unroll
     for (int d = 0; d < ND; ++d) store_drape(e.drapes + d * PCL_DRAPE_WORDS, dr[d]);
     store_carry(e.plot, carry);
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_ALL>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = timeout; e.plot[PCL_P_AUX1] = tele_frame;
     e.plot[PCL_P_AUX2] = tele_r; e.plot[PCL_P_AUX3] = tele_c;

@@ -211,6 +211,7 @@ warehouse_step(const StepParams p) {
   if (lane == 0) {
     store_sprite(rec + NB * PCL_SPRITE_WORDS, player, PCL_S_AUX0);
     r_judge[PCL_D_AUX0] = on_goals;
+    apply_time_limit(p, plot, dir);
     store_plot<ORDER_KEEP>(r_plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
