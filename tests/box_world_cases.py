@@ -1,4 +1,4 @@
-"""Box-World test helpers: the reference module, a scripted player and an online driver.
+"""Box-World test helpers: the reference module, the golden cases and a scripted player.
 
 The scripted player reads the board (and the level's distractor cells) and walks, by
 breadth-first search over free cells, to the object its mode wants: 'solve' opens correct
@@ -17,6 +17,16 @@ from pycolab_b200 import levels
 
 KEYS, LOCKS = levels.BOX_WORLD_KEYS, levels.BOX_WORLD_LOCKS
 MODES = ('solve', 'distract', 'dither', 'random')
+ARGS = ((1, 2, 3, 4), (0, 1, 2, 3, 4), (0,), 1)     # make_game's arguments after grid_size
+# The goldens: (name, seed, grid_size, max_num_steps, modes, T)
+CASES = (
+    ('box_world_g12_s3_solve', 3, 12, 120, ('solve', 'distract', 'random'), 400),
+    ('box_world_g12_s10_mixed', 10, 12, 120, ('solve', 'dither', 'distract'), 500),
+    ('box_world_g12_s7_distract', 7, 12, 60, ('distract', 'solve', 'random'), 400),
+    ('box_world_g6_s1', 1, 6, 40, ('solve', 'random', 'distract'), 300),
+    ('box_world_g20_s2', 2, 20, 150, ('solve', 'dither'), 400),
+    ('box_world_g30_s5', 5, 30, 200, ('solve', 'distract'), 400),
+)
 _STEPS = ((-1, 0, 0), (1, 0, 1), (0, -1, 2), (0, 1, 3))     # (dr, dc, action)
 
 
@@ -117,36 +127,20 @@ def scripted_action(board, distractors, mode, rs, noise=0.05):
   return int(rs.randint(0, 4))
 
 
-def drive(make_env, distractors, modes, T, seed, on_frame=None):
-  """Play T actions of the scripted player on envs from make_env() (auto-reset rule of
-  tests/trajectory.py); episode k plays modes[k % len(modes)].  Returns the actions and, per
-  frame, board, float reward (NaN = None), discount and game over."""
+def drive(make_env, distractors, modes, T, seed):
+  """T actions of the scripted player on envs from make_env() under the auto-reset rule of
+  tests/trajectory.py (a restart step stores 0); episode k plays modes[k % len(modes)]."""
   rs = np.random.RandomState(seed)
   env = make_env()
-  out = env.its_showtime()
-  episode = 0
-  actions, boards, rewards, discounts, overs = [], [], [], [], []
-
-  def record(env, out):
-    boards.append(np.asarray(out[0].board if hasattr(out[0], 'board') else out[0],
-                             dtype=np.uint8).copy())
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-    discounts.append(float(out[2]))
-    overs.append(int(bool(env.game_over)))
-    if on_frame is not None:
-      on_frame(env, out)
-  record(env, out)
+  board = env.its_showtime()[0].board
+  episode, actions = 0, []
   for _ in range(T):
     if env.game_over:
       episode += 1
       actions.append(0)
       env = make_env()
-      out = env.its_showtime()
+      board = env.its_showtime()[0].board
     else:
-      a = scripted_action(boards[-1], distractors, modes[episode % len(modes)], rs)
-      actions.append(a)
-      out = env.play(a)
-    record(env, out)
-  return dict(actions=np.array(actions, dtype=np.int32), boards=np.stack(boards),
-              reward_f=np.array(rewards), discount=np.array(discounts),
-              game_over=np.array(overs, dtype=np.uint8))
+      actions.append(scripted_action(board, distractors, modes[episode % len(modes)], rs))
+      board = env.play(actions[-1])[0].board
+  return actions

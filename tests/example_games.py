@@ -1,14 +1,15 @@
-"""The example-game goldens of tests/golden/make_golden.py: one table keyed by family, the
-recorder of each side and the one replay.
+"""The example-game and research-game goldens of tests/golden/make_golden.py: one table keyed
+by family, the recorder of each side and the one replay.
 
 A golden `<family>_*` belongs to FAMILIES[family], which says:
-  keys       the arrays its goldens hold before the trajectory, in file order;
+  keys       the arrays its goldens hold, in file order; the trajectory's arrays
+             (trajectory.TRAJECTORY) follow them unless `keys` places them;
   inputs     those of `keys` a replay plays from; every other key is recorded per frame;
   sprites    the chars of its `sprites` rows (None: the golden's own `sprite_chars`);
   curtain    the drape whose curtain its `curtains` hold;
-  seed       (generator, key): the global generator, 'numpy' or 'python', that the
-             reference and the facade draw from, seeded from golden key `key`; the oracle
-             builds its own generator from the same key;
+  seed       (generator, key): the global generator, 'numpy', 'python' or 'both', that the
+             reference and the facade draw from, seeded from golden key `key` ('config':
+             the seed its config holds); the oracle builds its own generators from it;
   reference, oracle, facade
              build(name, g) -> (make_env, croppers) of each side: make_env() makes one env
              and sets the croppers' engine to it; `croppers` holds the croppers whose views
@@ -25,12 +26,18 @@ import random
 
 import numpy as np
 
+import box_world_cases as bwc
 import golden_cases as gc
+import lp_rnn_cases as lc
 import refdriver
 import story_cases
 import trajectory as tj
+from oracle import box_world as obw
+from oracle import cued_catch as occ
 from oracle import engine_model as em
 from oracle import games as ogames
+from oracle import sequence_recall as osr
+from oracle import t_maze as otm
 
 Family = collections.namedtuple(
     'Family', 'keys inputs reference oracle facade sprites curtain seed frames checks',
@@ -38,7 +45,7 @@ Family = collections.namedtuple(
 
 
 def family_of(name):
-  return FAMILIES[name.split('_')[0]]
+  return next(fam for key, fam in FAMILIES.items() if name.startswith(key + '_'))
 
 
 # ------------------------------------------------------------------ builders --
@@ -60,7 +67,7 @@ def _art(g):
 
 
 def _seed(g, key):
-  return int(g[key][0])
+  return gc.config_of(g)['seed'] if key == 'config' else int(g[key][0])
 
 
 class _FixedCrop(object):
@@ -215,6 +222,27 @@ def _int_rewards(env, out):
   assert out[1] is None or type(out[1]) is int
 
 
+def _float_rewards(env, out):
+  assert out[1] is None or isinstance(out[1], float)
+
+
+def _t_maze_windows(env, out):
+  """Float rewards, and each Scrolly's curtain the window of its rolled whole_pattern
+  (drapes.py:689-695)."""
+  _float_rewards(env, out)
+  for ch in '#*ltr':
+    d = env.things[ch]
+    r, c = d._northwest_corner
+    np.testing.assert_array_equal(d.curtain, d.whole_pattern[r:r + env.rows, c:c + env.cols], ch)
+
+
+def _box_world_plot(env, out):
+  """Float rewards, and the_plot['over_this'] holding a Position, as the reference's does."""
+  _float_rewards(env, out)
+  over = env.the_plot.get('over_this')
+  assert not over or type(over[1]).__name__ == 'Position'
+
+
 def _facade(module):
   return importlib.import_module('pycolab_b200.games.' + module).make_game
 
@@ -222,6 +250,52 @@ def _facade(module):
 def _oracle_maze(g):
   maze, board, beneath = gc.scrolly_art(g)
   return ogames.make_scrolly_maze(maze, board, '+', beneath)
+
+
+def _t_maze(g):
+  """t_maze's maze and cue art and make_game's arguments after them."""
+  cfg = gc.config_of(g)
+  return (tj.u8_to_art(g['maze_art']), tj.u8_to_art(g['cue_art']), cfg['level'],
+          cfg['cue_after_teleport'], cfg['timeout_frames'], cfg['teleport_delay'],
+          cfg['limbo_time'])
+
+
+def _reference_t_maze(name, g):
+  ref, args = lc.ref_module('t_maze'), _t_maze(g)[2:]    # on its own art, as `maze_art` holds
+  return _with(lambda: ref.make_game(*args))
+
+
+def _oracle_t_maze(name, g):
+  seed = _seed(g, 'config')
+  rng, np_rng = random.Random(seed), np.random.RandomState(seed)
+  return _with(lambda: otm.make_t_maze(*_t_maze(g), rng=rng, np_rng=np_rng))
+
+
+def _facade_t_maze(name, g):
+  maze, cue, *args = _t_maze(g)
+  return _with(lambda: _facade('t_maze')(*args, maze_art=maze, cue_art=cue))
+
+
+def _reference_lp_rnn(game, shim):
+  """The build of a Cued Catch or Sequence Recall golden's reference env: the reference's
+  module, shimmed, on the golden's art."""
+  def build(name, g):
+    ref, args = lc.ref_module(game), gc.config_of(g)['args']
+    return _with(lambda: shim(lc.with_art(ref, _art(g), lambda: ref.make_game(*args))))
+  return build
+
+
+def _box_level(g):
+  """(art, distractors, max_num_steps) of a box_world golden."""
+  return (_art(g), [tuple(int(v) for v in xy) for xy in g['distractors']],
+          gc.config_of(g)['max_num_steps'])
+
+
+def _reference_box_world(name, g):
+  ref, cfg = bwc.ref_module(), gc.config_of(g)
+  return _with(lambda: ref.make_game(cfg['grid_size'], *bwc.ARGS,
+                                     random_state=np.random.RandomState(cfg['seed']),
+                                     max_num_steps=cfg['max_num_steps']))
 
 
 FAMILIES = {
@@ -321,12 +395,47 @@ FAMILIES = {
         reference=lambda name, g: _with(lambda: _story(name, reference=True)),
         oracle=lambda name, g: _with(_oracle_list_story),
         facade=lambda name, g: _with(lambda: _story(name, reference=False))),
+    't_maze': Family(
+        ('maze_art', 'cue_art', 'actions', 'sprites', 'reward_f64', 'which_goal', 'config'),
+        ('maze_art', 'cue_art', 'actions', 'config'), sprites='P', seed=('both', 'config'),
+        checks={'facade': _t_maze_windows},
+        reference=_reference_t_maze, oracle=_oracle_t_maze, facade=_facade_t_maze),
+    'cued_catch': Family(
+        ('art', 'actions', 'sprites', 'reward_f64', 'reward_type', 'state', 'config'),
+        ('art', 'actions', 'config'), sprites='Pab', seed=('python', 'config'),
+        reference=_reference_lp_rnn('cued_catch', lc.shim_cued_catch),
+        oracle=lambda name, g: (lambda rng: _with(lambda: occ.make_cued_catch(
+            _art(g), *gc.config_of(g)['args'], rng=rng)))(random.Random(_seed(g, 'config'))),
+        facade=lambda name, g: _with(lambda: _facade('cued_catch')(
+            *gc.config_of(g)['args'], art=_art(g)))),
+    'sequence_recall': Family(
+        ('art', 'actions', 'sprites', 'reward_f64', 'state', 'config'),
+        ('art', 'actions', 'config'), sprites='P', seed=('python', 'config'),
+        checks={'facade': _float_rewards},
+        reference=_reference_lp_rnn('sequence_recall', lc.shim_sequence_recall),
+        oracle=lambda name, g: (lambda rng: _with(lambda: osr.make_sequence_recall(
+            _art(g), *gc.config_of(g)['args'], rng=rng)))(random.Random(_seed(g, 'config'))),
+        facade=lambda name, g: _with(lambda: _facade('sequence_recall')(
+            *gc.config_of(g)['args'], art=_art(g)))),
+    # Its files hold reward_f64 among the trajectory's arrays.
+    'box_world': Family(
+        ('art', 'distractors', 'config', 'actions', 'boards', 'reward', 'has_reward',
+         'reward_f64', 'discount', 'game_over', 'grid', 'over_this', 'steps'),
+        ('art', 'distractors', 'config', 'actions'),
+        checks={'oracle': _float_rewards, 'facade': _box_world_plot},
+        reference=_reference_box_world,
+        oracle=lambda name, g: _with(lambda: obw.make_box_world(*_box_level(g))),
+        facade=lambda name, g: _with(lambda: importlib.import_module(
+            'pycolab_b200.games.box_world').game_from_level(*_box_level(g)))),
 }
 
 # The goldens the parametrised replays cover: every one of FAMILIES but the Story goldens,
 # whose replays are the story tests' own (test_story, test_gpu_story).
 # story_classics_cropped crops on the device: the oracle has no replay of it.
 REPLAYS = [name for fam in FAMILIES if fam != 'story' for name in gc.names(fam + '_')]
+# test_cued_catch replays its goldens on the facade itself, then checks where the global
+# generator ends.
+FACADE_REPLAYS = [name for name in REPLAYS if not name.startswith('cued_catch_')]
 
 
 # ----------------------------------------------------------------- recorders --
@@ -337,12 +446,14 @@ class _Recorder(object):
   `check(env, out)`, if given, runs at every frame."""
 
   DTYPES = dict(sprites=np.int32, curtains=np.uint8, backdrops=np.uint8, reward_type=np.uint8,
-                corners=np.int32, has_sword=np.uint8, floats=np.float64)
+                corners=np.int32, has_sword=np.uint8, floats=np.float64, reward_f64=np.float64,
+                state=np.int64, which_goal=np.uint8, grid=np.uint8, over_this=np.int32,
+                steps=np.int32)
 
   def __init__(self, fam, g, croppers, check=None):
     self.chars = bytes(g['sprite_chars']).decode() if fam.sprites is None else fam.sprites
     self.curtain, self.croppers, self.check = fam.curtain, croppers, check
-    self.rows = {k: [] for k in fam.keys if k not in fam.inputs}
+    self.rows = {k: [] for k in fam.keys if k not in fam.inputs + tj.TRAJECTORY}
 
   def __call__(self, env, out):
     for key, rows in self.rows.items():   # in file order: a frame's corner after its crop
@@ -362,6 +473,12 @@ class _Recorder(object):
 
   def reward_type(self, env, out):
     return tj.reward_type(out[1])
+
+  def reward_f64(self, env, out):
+    return np.nan if out[1] is None else float(out[1])
+
+  def grid(self, env, out):
+    return bwc.object_grid(env.things, (env.rows, env.cols))
 
   def corners(self, env, out):
     return self.corner(self.croppers['crops'])
@@ -399,6 +516,21 @@ class EngineRecorder(_Recorder):
     state = getattr(cropper, '_state', None)     # the facade's window is device state
     return list(cropper._corner) if state is None else [int(v) for v in state[0, :2].cpu()]
 
+  def state(self, env, out):
+    """Sequence Recall's program state, or else Cued Catch's."""
+    if 'program' in env.the_plot:
+      return lc.sequence_recall_state(env)
+    return lc.cued_catch_state(env)
+
+  def which_goal(self, env, out):
+    return 0 if env.things['Q'].which_goal == 'left' else 1
+
+  def over_this(self, env, out):
+    return bwc.over_words(env.the_plot.get('over_this'))
+
+  def steps(self, env, out):
+    return env.things['.']._step_counter
+
 
 class WorldRecorder(_Recorder):
   """The recorder of oracle worlds (oracle/games.py, oracle/compiled.py) and of
@@ -423,6 +555,20 @@ class WorldRecorder(_Recorder):
   def corner(self, cropper):
     return list(cropper.corner)
 
+  def state(self, world, out):
+    if 'program' in world.plot.store:
+      return lc.sequence_recall_state(world)
+    return lc.oracle_cued_catch_state(world)
+
+  def which_goal(self, world, out):
+    return 0 if world.things['Q'].aux['which_goal'] == 'left' else 1
+
+  def over_this(self, world, out):
+    return bwc.over_words(obw.over_this(world))
+
+  def steps(self, world, out):
+    return world.things['.'].aux['steps']
+
 
 # -------------------------------------------------------------------- replay --
 
@@ -437,7 +583,10 @@ def play(side, name, g, frames=None, make_env=None, check=None):
     make_env, croppers = getattr(fam, side)(name, g)
   if fam.seed is not None and side != 'oracle':
     stream, key = fam.seed
-    (random if stream == 'python' else np.random).seed(_seed(g, key))
+    if stream != 'numpy':
+      random.seed(_seed(g, key))
+    if stream != 'python':
+      np.random.seed(_seed(g, key))
   rec = (WorldRecorder if side == 'oracle' else EngineRecorder)(fam, g, croppers, check)
   got = tj.run_trajectory(make_env, g['actions'].tolist()[:frames], on_frame=rec)
   got.update(rec.arrays())

@@ -1,4 +1,5 @@
-"""Generate the example-game and fixture goldens in this directory from the REAL reference.
+"""Generate the example-game, research-game and fixture goldens in this directory from the
+REAL reference.
 
 Run in the build container (where /root/reference exists):
 
@@ -15,6 +16,7 @@ and the oracle tests compare against these files.
 
 import json
 import os
+import random
 import sys
 
 import numpy as np
@@ -23,12 +25,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
+import box_world_cases as bwc
 import example_games as eg
+import lp_rnn_cases as lc
 import refdriver
 import trajectory as tj
 from pycolab_b200 import levels
-
-TRAJECTORY = ('boards', 'reward', 'has_reward', 'discount', 'game_over')
 
 
 def save(name, **arrays):
@@ -40,11 +42,16 @@ def save(name, **arrays):
 def record(name, **inputs):
   """Plays example golden `name` on the reference env its family builds from `inputs`
   (tests/example_games.py), then saves the inputs, the fields the family records and the
-  trajectory.  Returns what it saved."""
+  trajectory, in the family's order.  Returns what it saved."""
   got = dict(eg.play('reference', name, inputs), **inputs)
-  arrays = {k: got[k] for k in eg.family_of(name).keys + TRAJECTORY}
+  # a trajectory key the family's keys already place keeps its place
+  arrays = {k: got[k] for k in eg.family_of(name).keys + tj.TRAJECTORY}
   save(name, **arrays)
   return arrays
+
+
+def json_u8(obj):
+  return np.frombuffer(json.dumps(obj).encode(), np.uint8)
 
 
 # ------------------------------------------------------- example-game goldens --
@@ -141,8 +148,7 @@ def cropper(name, pad, margins, offset, saccade, T=300):
              offset=None if offset is None else list(offset), saccade=saccade)
   record(name, maze_art=tj.art_to_u8(maze), board_art=tj.art_to_u8(board),
          beneath=np.array([ord(beneath)], dtype=np.uint8),
-         config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
-         actions=actions.astype(np.int32))
+         config=json_u8(cfg), actions=actions.astype(np.int32))
 
 
 def croppers():
@@ -279,11 +285,85 @@ def stories():
   record('story_classics_cropped', actions=a2.astype(np.int32))
 
 
+# ----------------------------------------------------------- research goldens --
+
+def t_mazes():
+  """research/lp-rnn/t_maze.py on its own art: `random.seed` and `np.random.seed` fix the
+  streams the cue side and the speckle are drawn from at every make_game."""
+  ref = lc.ref_module('t_maze')
+  for name, level, cue_after, timeout, delay, limbo, seed, T in lc.T_MAZE_CASES:
+    actions = lc.t_maze_policy(900 + seed, limbo, T)
+    if name.endswith('_quit'):
+      actions = [6 if a == 5 and i % 3 == 0 else a for i, a in enumerate(actions)]
+    config = dict(level=level, cue_after_teleport=cue_after, timeout_frames=timeout,
+                  teleport_delay=delay, limbo_time=limbo, seed=900 + seed)
+    traj = record(name, maze_art=tj.art_to_u8(ref.MAZE_ART), cue_art=tj.art_to_u8(ref.CUE_ART),
+                  actions=np.array(actions, dtype=np.int32), config=json_u8(config))
+    r = traj['reward_f64']
+    print('  %s: %d episodes, +1 %d, -1 %d, quits/timeouts %d' % (
+        name, int(traj['game_over'].sum()), int((r > 0.5).sum()), int((r < -0.5).sum()),
+        int(traj['game_over'].sum()) - int((np.abs(r) > 0.5).sum())))
+
+
+def lp_rnn(name, art, args, seed, T, policy):
+  """A Cued Catch or Sequence Recall golden: `random.seed` fixes the stream the game draws
+  from.  Pass 1 lets policy(env) choose T actions on the reference env, pass 2 records them."""
+  g = dict(art=tj.art_to_u8(art), config=json_u8(dict(args=list(args), seed=900 + seed)))
+  random.seed(900 + seed)
+  actions = lc.closed_loop(eg.family_of(name).reference(name, g)[0], policy, T)
+  return record(name, actions=np.array(actions, dtype=np.int32), **g)
+
+
+def cued_catches():
+  """research/lp-rnn/cued_catch.py, shimmed (tests/lp_rnn_cases.py)."""
+  ref = lc.ref_module('cued_catch')
+  for name, art, args, seed, T, kw in lc.CUED_CATCH_CASES:
+    art = list(ref.GAME_ART) if art is None else lc.small_cued_catch_art()
+    traj = lp_rnn(name, art, args, seed, T,
+                  lc.cued_catch_policy(np.random.RandomState(seed), **kw))
+    print('  %s: %d episodes, reward sum %.3f, float frames %d' % (
+        name, int(traj['game_over'].sum()), float(np.nansum(traj['reward_f64'])),
+        int((traj['reward_type'] == 2).sum())))
+
+
+def sequence_recalls():
+  """research/lp-rnn/sequence_recall.py, shimmed (tests/lp_rnn_cases.py)."""
+  ref = lc.ref_module('sequence_recall')
+  for name, art, args, seed, T, kw in lc.SEQUENCE_RECALL_CASES:
+    art = list(ref.GAME_ART) if art == 'ref' else levels.sequence_recall_art(*art)
+    centre = tuple(int(x[0]) for x in np.where(tj.art_to_u8(art) == ord('P')))
+    traj = lp_rnn(name, art, args, seed, T,
+                  lc.sequence_recall_policy(np.random.RandomState(seed), centre, **kw))
+    r = traj['reward_f64']
+    print('  %s: %d episodes, +1 %d, wrong %d' % (
+        name, int(traj['game_over'].sum()), int((r > 0.9).sum()), int((r == -0.005).sum())))
+
+
+def box_worlds():
+  """research/box_world: the level the reference generates from RandomState(seed) at every
+  (re)start.  Pass 1 lets the scripted player of tests/box_world_cases.py choose the actions
+  on the reference env, pass 2 records them."""
+  for name, seed, grid_size, max_steps, modes, T in bwc.CASES:
+    g = dict(config=json_u8(dict(seed=seed, grid_size=grid_size, max_num_steps=max_steps,
+                                 modes=list(modes))))
+    make = eg.family_of(name).reference(name, g)[0]
+    first = make()
+    art = [bytes(r).decode() for r in first.its_showtime()[0].board]
+    distractors = list(first.things['.'].distractors)
+    traj = record(name, art=tj.art_to_u8(art),
+                  distractors=np.array(distractors, np.int32).reshape(-1, 2),
+                  actions=np.array(bwc.drive(make, distractors, modes, T, seed), np.int32), **g)
+    r = traj['reward_f64']
+    print('  %s: %d episodes, rewards %s' % (
+        name, int(traj['game_over'].sum()), sorted(set(float(v) for v in r[~np.isnan(r)]))))
+
+
 # The makers of each family of tests/example_games.py.
 MAKERS = dict(scrolly=scrollies, warehouse=warehouses, marauders=marauders,
               better=better_scrollies, crop=croppers, classic=classics, fluvial=fluvials,
               aperture=apertures, hello=hellos, apprehend=apprehends, shockwave=shockwaves,
-              ordeal=ordeals, story=stories)
+              ordeal=ordeals, story=stories, t_maze=t_mazes, cued_catch=cued_catches,
+              sequence_recall=sequence_recalls, box_world=box_worlds)
 
 
 # ------------------------------------------------------------ fixture goldens --
@@ -317,7 +397,7 @@ def fixture_walkers(name, seed, T=300):
       on_frame=lambda env, out: sprites.append(tj.sprite_rows(env, 'abc')))
   cfg = dict(walkers=walkers, scrollys={}, drapes='', schedule=schedule,
              z_order=z_order, what_lies_beneath=' ', action_chars='abc')
-  save(name, art=art, config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
+  save(name, art=art, config=json_u8(cfg),
        actions=motions, sprites=np.array(sprites, dtype=np.int32), **traj)
 
 
@@ -365,7 +445,7 @@ def fixture_scrolly(name, seed, margins, second_ego, T=400):
                 for ch in '#@'},
       drapes='', schedule=schedule, z_order='@#Pq', what_lies_beneath=' ',
       action_chars='')
-  save(name, art=art, config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
+  save(name, art=art, config=json_u8(cfg),
        pattern_hash=pattern.astype(np.uint8), pattern_at=pattern2.astype(np.uint8),
        actions=np.array(used, dtype=np.int32), boards=np.stack(boards),
        sprites=np.array(sprites, dtype=np.int32),
@@ -423,7 +503,7 @@ def fixture_groups(name, seed, margins, T=400):
                           margins=None if margins is None else list(margins))},
       drapes='', schedule=schedule, z_order='@#Pq', what_lies_beneath=' ',
       action_chars='', motion_of=dict([('#', 0), ('P', 0), ('@', 1), ('q', 1)]))
-  save(name, art=art, config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
+  save(name, art=art, config=json_u8(cfg),
        pattern_hash=pattern.astype(np.uint8), pattern_at=pattern2.astype(np.uint8),
        actions=np.array(used, dtype=np.int32).reshape(-1, 2), boards=np.stack(boards),
        sprites=np.array(sprites, dtype=np.int32),
@@ -467,7 +547,7 @@ def fixture_unoccluded(name, seed, T=120):
              scrollys={'#': dict(corner=list(corner), margins=[2, 3])},
              drapes='%', schedule=schedule, z_order=z_order, what_lies_beneath=' ',
              action_chars='', layer_chars=chars)
-  save(name, art=art, config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
+  save(name, art=art, config=json_u8(cfg),
        pattern_hash=pattern.astype(np.uint8), actions=motions.astype(np.int32),
        boards=np.stack(boards), layers=np.stack(layers).astype(np.uint8))
 
@@ -528,7 +608,7 @@ def fixture_directives(name, seed, T=250):
     z_orders.append(list(map(ord, engine.z_order)))
   cfg = dict(walkers=walkers, scrollys={}, drapes='%', schedule=schedule,
              z_order=z_order, what_lies_beneath=' ', action_chars=order)
-  save(name, art=art, config=np.frombuffer(json.dumps(cfg).encode(), np.uint8),
+  save(name, art=art, config=json_u8(cfg),
        actions=np.array(rows, dtype=np.int64), boards=np.stack(boards),
        reward=np.array(reward, dtype=np.int64),
        has_reward=np.array(has_reward, dtype=np.uint8),

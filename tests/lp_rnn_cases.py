@@ -1,7 +1,7 @@
-"""Shared pieces of the Cued Catch and Sequence Recall tests and golden fixtures: the
-reference's own modules (loaded by path), the two shims that let them run on Python 3 with
-NumPy 2 without touching their source, closed-loop policies, and the per-frame state the
-goldens record.
+"""Shared pieces of the lp-rnn tests and golden fixtures (t_maze, Cued Catch, Sequence
+Recall): the reference's own modules (loaded by path), the two shims that let Cued Catch and
+Sequence Recall run on Python 3 with NumPy 2 without touching their source, the golden cases
+and their policies, and the per-frame state the goldens record.
 
 The shims:
   * Cued Catch compares None with ints the Python 2 way (None below everything):
@@ -67,7 +67,53 @@ def with_art(module, art, make):
     module.GAME_ART = saved
 
 
+# -------------------------------------------------------------------------------- t_maze --
+
+# (name, level, cue_after_teleport, timeout_frames, teleport_delay, limbo_time, seed, T)
+T_MAZE_CASES = (
+    ('t_maze_L0_limbo4', 0, False, -1, 0, 4, 0, 700),
+    ('t_maze_L1_delay5_cue', 1, True, -1, 5, 0, 1, 700),
+    ('t_maze_L2_limbo10_timeout', 2, False, 90, 5, 10, 2, 700),
+    ('t_maze_L3_cue_limbo2', 3, True, -1, 0, 2, 3, 700),
+    ('t_maze_L4_delay5_limbo4', 4, False, 300, 5, 4, 4, 900),
+    ('t_maze_L5_quit', 5, True, -1, 0, 10, 5, 900),
+)
+
+
+def t_maze_policy(seed, limbo_time, T):
+  """Actions that reach the goals: north onto the teleporter, wait out limbo, then along the
+  hallway to one side (drawn per episode) and down the corridor; some noise, some quits."""
+  rs = np.random.RandomState(seed)
+  out = []
+  while len(out) < T:
+    side = int(rs.choice([3, 4]))
+    episode = [1, 1, 1] + [5] * (max(limbo_time, 0) + 3) + [side] * 100 + [2] * 8
+    episode = [int(rs.randint(1, 6)) if rs.random_sample() < 0.05 else a for a in episode]
+    out += episode
+  return out[:T]
+
+
 # ---------------------------------------------------------------------------- Cued Catch --
+
+# (name, art (None = the reference's), make_game args, seed, T, policy kwargs)
+CUED_CATCH_CASES = (
+    ('cued_catch_paper', None, (10, 10, 100, False, 0.0, 40), 0, 1500, {}),
+    ('cued_catch_free_trials', None, (3, 2, 12, False, 0.0, 3), 1, 400, {}),
+    ('cued_catch_sigma', None, (2, 3, 10, False, 0.5, 2), 2, 500, {}),
+    ('cued_catch_always', None, (2, 2, 8, True, 0.0, 0), 3, 300, {}),
+    ('cued_catch_quit0', None, (2, 3, 20, False, 0.0, 0), 4, 300, dict(quit_every=67, quit_action=0)),
+    ('cued_catch_quit4', None, (1, 1, 20, False, 1.5, 1), 5, 300, dict(quit_every=53, quit_action=4)),
+    ('cued_catch_small_board', 'small', (3, 2, 15, True, 0.25, 1), 6, 500, {}),
+)
+
+
+def small_cued_catch_art():
+  """5 x 14: a width that is no multiple of 4, 'Q' cells in row 0, balls in other columns,
+  and fewer than 7 rows, so the bands 3:5 and -2: overlap."""
+  from pycolab_b200 import levels
+  return levels.cued_catch_art(5, 14, player=(1, 2), balls=((1, 9), (2, 12)),
+                               cue_cells=((0, 0), (0, 5), (0, 13), (2, 7)))
+
 
 def cued_catch_policy(rs, quit_every=0, quit_action=4):
   """Mostly moves to the correct ball's row (read from the env), sometimes the other way or
@@ -115,6 +161,19 @@ def oracle_cued_catch_state(world):
 
 
 # ----------------------------------------------------------------------- Sequence Recall --
+
+# (name, art ('ref' or (rows, cols) for levels.sequence_recall_art), make_game args, seed, T,
+#  policy kwargs)
+SEQUENCE_RECALL_CASES = (
+    ('sequence_recall_paper', 'ref', (4, 60, 30, 1, 1000), 0, 1500, dict(wrong=0.15)),
+    ('sequence_recall_short', 'ref', (3, 2, 1, 0, -1), 1, 500, dict(wrong=0.3)),
+    ('sequence_recall_timeout', 'ref', (4, 3, 2, 2, 40), 2, 300, dict(idle_from=0)),
+    ('sequence_recall_quit', 'ref', (2, 2, 2, 1, -1), 3, 300, dict(quits=((20, 0), (75, 6), (140, 0)))),
+    ('sequence_recall_len1', 'ref', (1, 1, 1, 1, -1), 4, 200, dict(wrong=0.3)),
+    ('sequence_recall_len16', 'ref', (16, 1, 2, 0, -1), 5, 900, dict(wrong=0.1)),
+    ('sequence_recall_shape9x13', (9, 13), (5, 2, 1, 3, 120), 6, 600, dict(wrong=0.2)),
+)
+
 
 def _state_name(state):
   return state if isinstance(state, str) else state.name
@@ -170,38 +229,18 @@ def sequence_recall_state(env):
 
 # ----------------------------------------------------------------------------- running --
 
-def closed_loop(make_env, policy, T, on_frame=None):
-  """trajectory.run_trajectory, with each action chosen by policy(env) before the step.
-  Returns (traj, actions)."""
-  import trajectory as tj
+def closed_loop(make_env, policy, T):
+  """T actions, each chosen by policy(env) before the step, on envs from make_env() under the
+  auto-reset rule of tests/trajectory.py; a restart step stores 5."""
   env = make_env()
-  out = env.its_showtime()
-  boards, reward, has_reward, discount, over, actions = [], [], [], [], [], []
-
-  def record(env, out):
-    boards.append(tj.board_of(out[0]).copy())
-    reward.append(0 if out[1] is None else int(out[1]))
-    has_reward.append(0 if out[1] is None else 1)
-    discount.append(float(out[2]))
-    over.append(1 if env.game_over else 0)
-    if on_frame is not None:
-      on_frame(env, out)
-  record(env, out)
+  env.its_showtime()
+  actions = []
   for _ in range(T):
-    a = 5 if env.game_over else policy(env)
-    actions.append(a)
     if env.game_over:
+      actions.append(5)
       env = make_env()
-      out = env.its_showtime()
+      env.its_showtime()
     else:
-      out = env.play(a)
-    record(env, out)
-  return dict(boards=np.stack(boards), reward=np.array(reward, dtype=np.int64),
-              has_reward=np.array(has_reward, dtype=np.uint8),
-              discount=np.array(discount, dtype=np.float64),
-              game_over=np.array(over, dtype=np.uint8)), actions
-
-
-def reward_code(r):
-  """0 None, 1 a Python int, 2 a Python float."""
-  return 0 if r is None else 2 if isinstance(r, float) else 1
+      actions.append(policy(env))
+      env.play(actions[-1])
+  return actions

@@ -1,9 +1,10 @@
 """research/box_world: keys, locks and the gem as one per-env object grid (csrc/box_world.cu).
 
 CPU: the level generator against the reference's `make_game`, the oracle (oracle/box_world.py)
-in lock-step with the live reference and against goldens the reference made
-(tests/golden/box_world_*, by tests/golden/make_box_world_golden.py), lowering, the C
-boundary's statuses and the kernel's resources."""
+in lock-step with the live reference, lowering, the C boundary's statuses and the kernel's
+resources.  The goldens the reference made (tests/golden/box_world_*, by
+tests/golden/make_golden.py) replay on the oracle and the facade through
+tests/example_games.py."""
 
 import ctypes as C
 import os
@@ -19,7 +20,7 @@ import trajectory as tj
 from oracle import box_world as obw
 
 NAMES = gc.names('box_world_')
-ARGS = ((1, 2, 3, 4), (0, 1, 2, 3, 4), (0,), 1)
+ARGS = bwc.ARGS
 needs_ref = pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
 
 
@@ -166,28 +167,6 @@ def test_goldens_cover_every_outcome():
   assert timeouts >= 1
   assert any(((gc.load(n)['actions'] < 0) | (gc.load(n)['actions'] > 3)).any() for n in NAMES)
   assert {gc.config_of(gc.load(n))['grid_size'] for n in NAMES} >= {6, 12, 20, 30}
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_replays_reference_golden(name):
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  art, distractors = golden_level(g)
-  grids, overs, steps, rewards = [], [], [], []
-
-  def on_frame(env, out):
-    grids.append(oracle_grid(env))
-    overs.append(oracle_over(env))
-    steps.append(env.things['.'].aux['steps'])
-    rewards.append(np.nan if out[1] is None else out[1])
-    assert out[1] is None or isinstance(out[1], float)
-  got = tj.run_trajectory(lambda: obw.make_box_world(art, distractors, cfg['max_num_steps']),
-                          g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['reward_f64'], np.array(rewards, dtype=np.float64))
-  np.testing.assert_array_equal(g['grid'], np.stack(grids))
-  np.testing.assert_array_equal(g['over_this'], np.array(overs))
-  np.testing.assert_array_equal(g['steps'], np.array(steps))
 
 
 # ----------------------------------------------------------------------------- lowering --

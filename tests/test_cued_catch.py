@@ -1,9 +1,10 @@
 """research/lp-rnn/cued_catch.py: a trial cue per episode-drawn pairing, every frame paid, and
 reward noise from random.normalvariate.  Goldens are the shimmed reference's own trajectories
-(tests/golden/cued_catch_*, made by tests/golden/make_lp_rnn_golden.py); CPU: the oracle
-(oracle/cued_catch.py) in lock-step with the live reference and against the goldens,
-lowering, fingerprints and the C boundary's refusals; GPU: the goldens through the facade,
-batched auto-reset runs whose pairings, trials and noise are drawn ON THE DEVICE."""
+(tests/golden/cued_catch_*, made by tests/golden/make_golden.py; tests/example_games.py
+replays them on the oracle); CPU: the oracle (oracle/cued_catch.py) in lock-step with the
+live reference, lowering, fingerprints and the C boundary's refusals; GPU: the goldens
+through the facade, batched auto-reset runs whose pairings, trials and noise are drawn ON
+THE DEVICE."""
 
 import ctypes as C
 import os
@@ -13,25 +14,18 @@ import sys
 import numpy as np
 import pytest
 
+import example_games as eg
 import golden_cases as gc
 import lp_rnn_cases as lc
 import refdriver
 import trajectory as tj
 from oracle import cued_catch as occ
 from oracle import sampled_check
+from registered_games import global_generators  # noqa: F401  (a fixture)
 
 NAMES = gc.names('cued_catch_')
 REF = os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'research', 'lp-rnn',
                    'cued_catch.py')
-
-
-def _oracle_maker(art, args, rng):
-  return lambda: occ.make_cued_catch(art, *args, rng=rng)
-
-
-def _same_f64(want, got, label):
-  np.testing.assert_array_equal(np.asarray(want).view(np.int64), np.asarray(got).view(np.int64),
-                                err_msg=label)
 
 
 def test_goldens_cover_the_rules():
@@ -46,26 +40,6 @@ def test_goldens_cover_the_rules():
   assert (acts == 0).any() and (acts == 4).any()
   small = [g for g in gs if g['art'].shape[0] < 7]
   assert small and small[0]['art'].shape[1] % 4 and (small[0]['art'][0] == ord('Q')).any()
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_cued_catch_matches_reference_golden(name):
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  art = tj.u8_to_art(g['art'])
-  rng = random.Random(cfg['seed'])
-  rewards, types, states = [], [], []
-
-  def on_frame(world, out):
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-    types.append(lc.reward_code(out[1]))
-    states.append(lc.oracle_cued_catch_state(world))
-  got = tj.run_trajectory(_oracle_maker(art, cfg['args'], rng), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  _same_f64(g['reward_f64'], rewards, name)
-  np.testing.assert_array_equal(g['reward_type'], types)
-  np.testing.assert_array_equal(g['state'], states)
 
 
 @pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
@@ -88,7 +62,7 @@ def test_oracle_lockstep_with_reference(case):
   a, b = a_env.its_showtime(), b_env.its_showtime()
   for t in range(400):
     assert np.array_equal(a[0].board, b[0]), t
-    assert lc.reward_code(a[1]) == lc.reward_code(b[1]), t
+    assert tj.reward_type(a[1]) == tj.reward_type(b[1]), t
     assert np.float64(a[1]).view(np.int64) == np.float64(b[1]).view(np.int64), (t, a[1], b[1])
     assert a[2] == b[2] and a_env.game_over == b_env.game_over, t
     assert lc.cued_catch_state(a_env) == lc.oracle_cued_catch_state(b_env), t
@@ -240,31 +214,17 @@ def test_edited_cued_catch_copy_is_refused(tmp_path, edit):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('name', NAMES)
-def test_facade_cued_catch_golden(name):
+def test_facade_cued_catch_golden(global_generators, name):  # noqa: F811
   """B = 1 facade: the twin's CueDrape draws the pairings from the global `random`, the device
-  continues that stream in update() and hands it back after every step; boards, float64
-  reward bits, Python reward types and the mirrored state frame by frame, and the global
-  generator's state at the end."""
-  from pycolab_b200.games import cued_catch
+  continues that stream in update() and hands it back after every step; every array of the
+  golden frame by frame, and the global generator's state at the end."""
+  eg.assert_replays('facade', name)
+  # the oracle, drawing from its own Random(seed), ends where the global generator does
   g = gc.load(name)
   cfg = gc.config_of(g)
-  art = tj.u8_to_art(g['art'])
-  random.seed(cfg['seed'])
-  rewards, types, states = [], [], []
-
-  def on_frame(env, out):
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-    types.append(lc.reward_code(out[1]))
-    states.append(lc.cued_catch_state(env))
-  traj = tj.run_trajectory(lambda: cued_catch.make_game(*cfg['args'], art=art),
-                           g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, traj, name)
-  _same_f64(g['reward_f64'], rewards, name)
-  np.testing.assert_array_equal(g['reward_type'], types)
-  np.testing.assert_array_equal(g['state'], states)
-  # the oracle, drawing from its own Random(seed), ends where the global generator does
-  rng = random.Random(cfg['seed'])
-  tj.run_trajectory(_oracle_maker(art, cfg['args'], rng), g['actions'].tolist())
+  art, rng = tj.u8_to_art(g['art']), random.Random(cfg['seed'])
+  tj.run_trajectory(lambda: occ.make_cued_catch(art, *cfg['args'], rng=rng),
+                    g['actions'].tolist())
   assert random.getstate() == rng.getstate()
 
 

@@ -1,7 +1,7 @@
-"""The oracle (oracle/games.py, and the chained worlds of the Ordeal) replays every
-example-game golden of tests/example_games.py REPLAYS: every array the golden
-holds, frame by frame, boards, rewards, sprite registers, curtains, croppers' views and
-corners, chapters and float registers included.
+"""The oracle (oracle/games.py, the research games' oracles, and the chained worlds of the
+Ordeal) replays every golden of tests/example_games.py REPLAYS: every array the golden holds,
+frame by frame, boards, rewards, sprite registers, curtains, croppers' views and corners,
+chapters, float registers and the research games' private state included.
 """
 
 import pytest

@@ -1,12 +1,11 @@
 """research/box_world on the H100: the reference's goldens replayed on the device bit for bit
 (board, reward, has_reward, discount, done, every object curtain, occluded and un-occluded
-layers), the facade Engine with its Drapes and the_plot['over_this'], and pools of thousands
-of distinct generated levels in one handle, sampled against the oracle."""
+layers), and pools of thousands of distinct generated levels in one handle, sampled against
+the oracle.  The facade Engine's replays of the goldens are tests/example_games.py's."""
 
 import numpy as np
 import pytest
 
-import box_world_cases as bwc
 import golden_cases as gc
 import trajectory as tj
 from oracle import box_world as obw
@@ -60,37 +59,6 @@ def test_golden_replays_on_device(name):
       np.testing.assert_array_equal(unoccluded[k], want, '%s layer %s frame %d' % (name, ch, t))
   assert set(eng.object_chars) == set(np.unique(g['grid'][0])[1:].tobytes().decode())
   assert int(eng.error_codes().abs().max()) == 0
-
-
-def _facade_replay(make, g, name):
-  rewards, grids, overs, steps = [], [], [], []
-
-  def on_frame(env, out):
-    assert out[1] is None or isinstance(out[1], float)
-    rewards.append(np.nan if out[1] is None else out[1])
-    grids.append(bwc.object_grid(env.things, (env.rows, env.cols)))
-    over = env.the_plot.get('over_this')
-    overs.append(bwc.over_words(over))
-    if over:
-      assert type(over[1]).__name__ == 'Position'
-    steps.append(env.things['.']._step_counter)
-  got = tj.run_trajectory(make, g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  np.testing.assert_array_equal(g['reward_f64'], np.array(rewards, dtype=np.float64))
-  np.testing.assert_array_equal(g['grid'], np.stack(grids))
-  np.testing.assert_array_equal(g['over_this'], np.array(overs))
-  np.testing.assert_array_equal(g['steps'], np.array(steps))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES[:3])
-def test_facade_engine_reproduces_golden(name):
-  """One facade Engine per episode: Drape curtains, the player's step counter and
-  the_plot['over_this'] follow the device."""
-  from pycolab_b200.games import box_world
-  g, cfg, art, distractors = _golden(name)
-  _facade_replay(lambda: box_world.game_from_level(art, distractors, cfg['max_num_steps']),
-                 g, name)
 
 
 def _pool(n_levels, grid_size=12):

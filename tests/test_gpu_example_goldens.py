@@ -1,6 +1,6 @@
-"""The facade Engine on the H100 replays every example-game golden of
-tests/example_games.py REPLAYS: every array the golden holds, frame by frame, up to the family's
-frame limit, with the global generators seeded as the reference's were.
+"""The facade Engine on the H100 replays every golden of tests/example_games.py
+FACADE_REPLAYS: every array the golden holds, frame by frame, up to the family's frame limit,
+with the global generators seeded as the reference's were.
 """
 
 import pytest
@@ -11,6 +11,6 @@ from registered_games import global_generators  # noqa: F401  (a fixture)
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('name', eg.REPLAYS)
+@pytest.mark.parametrize('name', eg.FACADE_REPLAYS)
 def test_facade_replays(global_generators, name):  # noqa: F811
   eg.assert_replays('facade', name)

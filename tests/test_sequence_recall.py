@@ -1,10 +1,10 @@
 """research/lp-rnn/sequence_recall.py: a light sequence drawn per episode, a program counter
 over _make_program's states, and float64 rewards.  Goldens are the shimmed reference's own
-trajectories (tests/golden/sequence_recall_*, made by tests/golden/make_lp_rnn_golden.py);
-CPU: the oracle (oracle/sequence_recall.py) in lock-step with the live reference and against
-the goldens, lowering, fingerprints (the classes and _make_program) and refusals; GPU: the
-goldens through the facade, and batched auto-reset runs whose sequences are drawn ON THE
-DEVICE."""
+trajectories (tests/golden/sequence_recall_*, made by tests/golden/make_golden.py and
+replayed on the oracle and the facade by tests/example_games.py); CPU: the oracle
+(oracle/sequence_recall.py) in lock-step with the live reference, lowering, fingerprints (the
+classes and _make_program) and refusals; GPU: batched auto-reset runs whose sequences are
+drawn ON THE DEVICE."""
 
 import ctypes as C
 import os
@@ -17,18 +17,12 @@ import pytest
 import golden_cases as gc
 import lp_rnn_cases as lc
 import refdriver
-import trajectory as tj
 from oracle import sampled_check
 from oracle import sequence_recall as osr
 
 NAMES = gc.names('sequence_recall_')
 REF = os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'research', 'lp-rnn',
                    'sequence_recall.py')
-
-
-def _same_f64(want, got, label):
-  np.testing.assert_array_equal(np.asarray(want).view(np.int64), np.asarray(got).view(np.int64),
-                                err_msg=label)
 
 
 def test_goldens_cover_the_rules():
@@ -46,28 +40,6 @@ def test_goldens_cover_the_rules():
   # a SEEK on the wrong pad pays 0.0: the frame sums to -0.005 with the light turned on
   assert any(((g['state'][1:, 0] < g['state'][:-1, 0]) & (g['reward_f64'][1:] == -0.005)).any()
              for g in gs)
-
-
-def _oracle_maker(art, args, rng):
-  return lambda: osr.make_sequence_recall(art, *args, rng=rng)
-
-
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_sequence_recall_matches_reference_golden(name):
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  art = tj.u8_to_art(g['art'])
-  rng = random.Random(cfg['seed'])
-  rewards, states = [], []
-
-  def on_frame(world, out):
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-    states.append(lc.sequence_recall_state(world))
-  got = tj.run_trajectory(_oracle_maker(art, cfg['args'], rng), g['actions'].tolist(),
-                          on_frame=on_frame)
-  tj.assert_same_trajectory(g, got, name)
-  _same_f64(g['reward_f64'], rewards, name)
-  np.testing.assert_array_equal(g['state'], states)
 
 
 @pytest.mark.skipif(not refdriver.available(), reason='/root/reference not present')
@@ -237,29 +209,6 @@ def test_edited_sequence_recall_copy_is_refused(tmp_path, edit):
 
 
 # ------------------------------------------------------------------------------------ GPU --
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES)
-def test_facade_sequence_recall_golden(name):
-  """B = 1 facade: the twin's make_game draws the sequence from the global `random`; boards,
-  float64 reward bits and the mirrored program, frames_in_state and timeout, frame by frame."""
-  from pycolab_b200.games import sequence_recall
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  art = tj.u8_to_art(g['art'])
-  random.seed(cfg['seed'])
-  rewards, states = [], []
-
-  def on_frame(env, out):
-    assert out[1] is None or isinstance(out[1], float)
-    rewards.append(np.nan if out[1] is None else float(out[1]))
-    states.append(lc.sequence_recall_state(env))
-  traj = tj.run_trajectory(lambda: sequence_recall.make_game(*cfg['args'], art=art),
-                           g['actions'].tolist(), on_frame=on_frame)
-  tj.assert_same_trajectory(g, traj, name)
-  _same_f64(g['reward_f64'], rewards, name)
-  np.testing.assert_array_equal(g['state'], states)
-
 
 def _batched_vs_oracle(B, T, seed, args, arts, check_envs=None, policy_seed=3):
   from pycolab_b200 import batched

@@ -1,13 +1,12 @@
 """research/lp-rnn/t_maze.py: float64 rewards through the C ABI, five Scrollys that teleport
 by np.roll, and a cue side plus a 191 x 77 speckle field drawn from two generators at every
 (re)start.  Goldens are the reference's own trajectories on its own art
-(tests/golden/t_maze_*, made by tests/golden/make_t_maze_golden.py); CPU: the oracle
-(oracle/t_maze.py) in lock-step with the imported reference and against
-the goldens, lowering and the C boundary's refusals; GPU: the goldens through the facade, and
-batched auto-reset runs whose cue and speckle are drawn ON THE DEVICE from per-env streams."""
+(tests/golden/t_maze_*, made by tests/golden/make_golden.py and replayed on the oracle and
+the facade by tests/example_games.py); CPU: the oracle (oracle/t_maze.py) in lock-step with
+the imported reference, lowering and the C boundary's refusals; GPU: batched auto-reset runs
+whose cue and speckle are drawn ON THE DEVICE from per-env streams."""
 
 import ctypes as C
-import importlib.util
 import os
 import random
 import sys
@@ -16,44 +15,14 @@ import numpy as np
 import pytest
 
 import golden_cases as gc
+import lp_rnn_cases as lc
 import refdriver
-import trajectory as tj
 from oracle import engine_model as em
 from oracle import games as ogames
 from oracle import sampled_check
 from oracle import t_maze as otm
 
 NAMES = gc.names('t_maze_')
-
-
-def _ref_module():
-  refdriver._import()
-  path = os.path.join(refdriver.REFERENCE_ROOT, 'pycolab', 'examples', 'research', 'lp-rnn',
-                      't_maze.py')
-  spec = importlib.util.spec_from_file_location('ref_t_maze_test', path)
-  module = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(module)
-  return module
-
-
-def _oracle_maker(maze, cue, cfg, rng, np_rng):
-  return lambda: otm.make_t_maze(maze, cue, cfg['level'], cfg['cue_after_teleport'],
-                                    cfg['timeout_frames'], cfg['teleport_delay'],
-                                    cfg['limbo_time'], rng, np_rng)
-
-
-def _rewards(make_env, actions):
-  """run_trajectory plus the float rewards (NaN = None)."""
-  got = []
-  traj = tj.run_trajectory(make_env, actions, on_frame=lambda env, out: got.append(
-      np.nan if out[1] is None else float(out[1])))
-  traj['reward_f64'] = np.array(got, dtype=np.float64)
-  return traj
-
-
-def _same_f64(want, got, label):
-  np.testing.assert_array_equal(np.asarray(want).view(np.int64), np.asarray(got).view(np.int64),
-                                err_msg=label)
 
 
 def test_goldens_cover_the_rules():
@@ -68,18 +37,6 @@ def test_goldens_cover_the_rules():
   assert any(6 in gc.load(n)['actions'] for n in NAMES)
 
 
-@pytest.mark.parametrize('name', NAMES)
-def test_oracle_t_maze_matches_reference_golden(name):
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  maze, cue = tj.u8_to_art(g['maze_art']), tj.u8_to_art(g['cue_art'])
-  make = _oracle_maker(maze, cue, cfg, random.Random(cfg['seed']),
-                       np.random.RandomState(cfg['seed']))
-  got = _rewards(make, g['actions'].tolist())
-  tj.assert_same_trajectory(g, got, name)
-  _same_f64(g['reward_f64'], got['reward_f64'], name)
-
-
 # (level, cue_after_teleport, timeout_frames, teleport_delay, limbo_time)
 LOCKSTEP = [(0, False, -1, 0, 0), (1, True, 60, 5, 4), (2, False, -1, 5, 10), (3, True, -1, 0, 4),
             (4, False, 150, 0, 10), (5, True, -1, 5, 0), (2, True, -1, 0, 2), (1, False, -1, 5, 1)]
@@ -90,9 +47,7 @@ LOCKSTEP = [(0, False, -1, 0, 0), (1, True, 60, 5, 4), (2, False, -1, 5, 10), (3
 def test_oracle_lockstep_with_reference(case):
   """Every frame: board, float reward, discount, game over, the player and every plot entry
   the game keeps; the policy reaches both goals, quits and times out."""
-  sys.path.insert(0, os.path.join(os.path.dirname(__file__), 'golden'))
-  import make_t_maze_golden
-  ref = _ref_module()
+  ref = lc.ref_module('t_maze')
   level, cue_after, timeout, delay, limbo = case
   seed = 40 + level
   random.seed(seed)
@@ -101,7 +56,7 @@ def test_oracle_lockstep_with_reference(case):
   mk_ref = lambda: ref.make_game(level, cue_after, timeout, delay, limbo)
   mk_or = lambda: otm.make_t_maze(ref.MAZE_ART, ref.CUE_ART, level, cue_after, timeout, delay,
                                      limbo, rng, np_rng)
-  actions = make_t_maze_golden.t_maze_policy(seed, limbo, 900)
+  actions = lc.t_maze_policy(seed, limbo, 900)
   actions = [0 if i % 97 == 96 else a for i, a in enumerate(actions)]
   a_env, b_env = mk_ref(), mk_or()
   a, b = a_env.its_showtime(), b_env.its_showtime()
@@ -292,46 +247,6 @@ def test_edited_t_maze_copy_is_refused(tmp_path):
 
 
 # ------------------------------------------------------------------------------------ GPU --
-
-def _facade(maze, cue, cfg):
-  from pycolab_b200.games import t_maze
-  return lambda: t_maze.make_game(cfg['level'], cfg['cue_after_teleport'], cfg['timeout_frames'],
-                                  cfg['teleport_delay'], cfg['limbo_time'], maze_art=maze,
-                                  cue_art=cue)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', NAMES)
-def test_facade_t_maze_golden(name):
-  """B = 1 facade on the reference's art: the twin's drapes draw from the global `random` and
-  NumPy streams as upstream, one Engine per episode; rewards compared as float64 bits."""
-  g = gc.load(name)
-  cfg = gc.config_of(g)
-  maze, cue = tj.u8_to_art(g['maze_art']), tj.u8_to_art(g['cue_art'])
-  random.seed(cfg['seed'])
-  np.random.seed(cfg['seed'])
-  sprites, goals = [], []
-
-  def on_frame(env, out):
-    p = env.things['P']
-    sprites.append([[int(p.position[0]), int(p.position[1]), int(bool(p.visible)),
-                     int(p.virtual_position[0]), int(p.virtual_position[1])]])
-    goals.append(0 if env.things['Q'].which_goal == 'left' else 1)
-    assert out[1] is None or isinstance(out[1], float)
-    for ch in '#*ltr':           # the rolled whole_pattern, windowed as drapes.py:689-695
-      d = env.things[ch]
-      r, c = d._northwest_corner
-      np.testing.assert_array_equal(d.curtain, d.whole_pattern[r:r + env.rows, c:c + env.cols],
-                                    '%s frame %d' % (ch, len(goals)))
-  got = []
-  traj = tj.run_trajectory(_facade(maze, cue, cfg), g['actions'].tolist(),
-                           on_frame=lambda env, out: (on_frame(env, out), got.append(
-                               np.nan if out[1] is None else out[1])))
-  tj.assert_same_trajectory(g, traj, name)
-  _same_f64(g['reward_f64'], np.array(got, dtype=np.float64), name)
-  np.testing.assert_array_equal(g['sprites'], np.array(sprites))
-  np.testing.assert_array_equal(g['which_goal'], np.array(goals))
-
 
 def _batched_vs_oracle(B, T, seed, cfg, n_worlds, check_envs=None, policy_seed=3):
   """Auto-resetting batch over generated worlds (env e plays world e % n_worlds, one set of

@@ -9,6 +9,9 @@ at the NEXT step (that step's action is ignored) and returns its
 
 import numpy as np
 
+# The arrays of every trajectory, as run_trajectory returns them.
+TRAJECTORY = ('boards', 'reward', 'has_reward', 'discount', 'game_over')
+
 
 def board_of(obs):
   return np.asarray(obs.board if hasattr(obs, 'board') else obs, dtype=np.uint8)
@@ -121,7 +124,7 @@ def u8_to_art(arr):
 
 
 def assert_same_trajectory(want, got, label=''):
-  for key in ('boards', 'reward', 'has_reward', 'discount', 'game_over'):
+  for key in TRAJECTORY:
     w, g = np.asarray(want[key]), np.asarray(got[key])
     assert w.shape == g.shape, (label, key, w.shape, g.shape)
     if not np.array_equal(w, g):
