@@ -375,6 +375,18 @@ __global__ void gather_errors(const int32_t* plot, int32_t* out, int B) {
   if (i < B) out[i] = plot[(int64_t)i * PCL_PLOT_WORDS + PCL_P_ERROR];
 }
 
+// The output elements of a post-processor's launch (pcl_observe_spec), as ObserveParams
+// and CropObserveParams both hold them.
+template <typename Params>
+void fill_elements(Params* p, const pcl_observe_spec* spec, const void* d_table,
+                   const uint8_t* d_valid, void* d_out, int32_t* d_unknown) {
+  p->depth = spec->depth; p->dtype = spec->dtype;
+  p->words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
+  p->stride_b = spec->stride_b * p->words; p->stride_d = spec->stride_d * p->words;
+  p->stride_r = spec->stride_r * p->words; p->stride_c = spec->stride_c * p->words;
+  p->table = d_table; p->valid = d_valid; p->out = d_out; p->unknown = d_unknown;
+}
+
 }  // namespace
 
 extern "C" {
@@ -405,30 +417,14 @@ int pcl_create(const pcl_spec* spec, int batch, int device, pcl_handle** out) {
   const int v = validate(*spec);
   if (v != PCL_OK) return v;
   if (device >= 0 && cudaSetDevice(device) != cudaSuccess) return PCL_ERR_CUDA;
-  pcl_handle* h = new (std::nothrow) pcl_handle();
+  pcl_handle* h = new (std::nothrow) pcl_handle();   // value-initialised: every field zero
   if (!h) return PCL_ERR_NOMEM;
   h->spec = *spec;
   h->program = program_of(spec->program);
   h->batch = batch;
   h->device = device;
-  h->bound = 0;
   h->actions_per_env = h->program->actions_per_env ? h->program->actions_per_env(*spec) : 1;
-  h->launches = 0;
-  h->chained_launches = 0;
-  h->last_error[0] = 0;
-  h->host_ready = 0;
   h->pending_slot = -1;
-  h->code_host = nullptr;
-  h->code_words = 0;
-  h->code_dev = nullptr;
-  h->code_dev_words = 0;
-  h->code_stale = 0;
-  h->backdrop_live = nullptr;
-  h->derived_dev = nullptr;
-  h->derive_stale = 0;
-  h->last_board = nullptr;
-  h->board_epoch = 0;
-  h->time_limit = 0;
   *out = h;
   return PCL_OK;
 }
@@ -582,8 +578,7 @@ int host_pipeline_ready(pcl_handle* h) {
   return PCL_OK;
 }
 
-// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts, for every
-// cropper entry point.
+// cropping.py:362-391: what a ScrollingCropper / FixedCropper accepts (crop_accepted).
 int crop_spec_ok(const pcl_handle* h, const pcl_crop_spec* crop) {
   if (crop->rows <= 0 || crop->cols <= 0) return PCL_ERR_INVALID;
   // sprite_index names the tracked sprite only when no priority list is given (a
@@ -604,10 +599,41 @@ int crop_spec_ok(const pcl_handle* h, const pcl_crop_spec* crop) {
   return PCL_OK;
 }
 
-bool tracks_drape(const pcl_crop_spec* crop) {
-  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i)
-    if (crop->track[i] < 0) return true;
-  return false;
+// Does a cropper entry point accept `crop`, after its own argument checks?  One that
+// takes no curtains (Curtains::kNone) refuses drape tracking as unsupported; one that takes
+// the caller's d_curtains, one per tracking-list entry, needs each tracked drape's curtain
+// (pcl_crop passes none) on a board of at most 128 x 128 cells, and fills them into `p`
+// when given.
+enum class Curtains { kNone, kCaller };
+int crop_accepted(const pcl_handle* h, const pcl_crop_spec* crop, Curtains from,
+                  const uint8_t* const* d_curtains = nullptr, pcl::CropParams* p = nullptr) {
+  const int ok = crop_spec_ok(h, crop);
+  if (ok != PCL_OK) return ok;
+  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
+    if (crop->track[i] > 0) continue;
+    if (from == Curtains::kNone) return PCL_ERR_UNSUPPORTED;
+    if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
+    if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
+    if (p) p->curtains[i] = d_curtains[i];
+  }
+  return PCL_OK;
+}
+
+// A record with an int32 reward (the host steps' h_reward, the hand-off records) needs
+// every per-env output set, and a handle whose rewards are not float64.
+int int32_record_ok(const pcl_handle* h, const pcl_outputs& out) {
+  if (!outputs_set(out)) return PCL_ERR_INVALID;
+  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;
+  return PCL_OK;
+}
+
+// What pcl_step_host and pcl_step_host_async check before their own arguments.
+int step_host_ok(pcl_handle* h, const int32_t* h_actions, const int32_t* d_actions,
+                 const pcl_outputs* out, cudaStream_t s) {
+  int r = check_ready(h, out, s);
+  if (r == PCL_OK) r = int32_record_ok(h, *out);     // h_reward is int32
+  if (r == PCL_OK && (!h_actions || !d_actions)) r = PCL_ERR_INVALID;
+  return r;
 }
 
 }  // namespace
@@ -616,11 +642,9 @@ int pcl_step_host(pcl_handle* h, const int32_t* h_actions, int32_t* d_actions,
                   const pcl_outputs* out, uint8_t* h_board, int32_t* h_reward,
                   uint8_t* h_has_reward, float* h_discount, uint8_t* h_done, void* stream) {
   Range nvtx_range("pcl_step_host");
-  const int r = check_ready(h, out, (cudaStream_t)stream);
-  if (r != PCL_OK) return r;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
-  if (!h_actions || !d_actions) return PCL_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
+  const int r = step_host_ok(h, h_actions, d_actions, out, s);
+  if (r != PCL_OK) return r;
   const size_t plane = (size_t)h->spec.rows * h->spec.pitch;
   int e = step_host_enqueue(h, h_actions, d_actions, out, s);
   if (e != PCL_OK) return e;
@@ -637,19 +661,16 @@ int pcl_step_host_async(pcl_handle* h, const int32_t* h_actions, int32_t* d_acti
                         uint8_t* h_has_reward, float* h_discount, uint8_t* h_done, int slot,
                         void* stream) {
   Range nvtx_range("pcl_step_host_async");
-  const int r = check_ready(h, out, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int r = step_host_ok(h, h_actions, d_actions, out, s);
   if (r != PCL_OK) return r;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // h_reward is int32
-  if (!h_actions || !d_actions || slot < 0 || slot >= PCL_HOST_SLOTS) return PCL_ERR_INVALID;
-  if (crop && !d_crop) return PCL_ERR_INVALID;
+  if (slot < 0 || slot >= PCL_HOST_SLOTS || (crop && !d_crop)) return PCL_ERR_INVALID;
   if (crop) {                    // refuse the crop before the step, not after it
-    const int ok = crop_spec_ok(h, crop);
+    const int ok = crop_accepted(h, crop, Curtains::kNone);   // drape tracking: pcl_crop_tracking
     if (ok != PCL_OK) return ok;
-    if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;      // no curtains here: pcl_crop_tracking
   }
   int e = host_pipeline_ready(h);
   if (e != PCL_OK) return e;
-  cudaStream_t s = (cudaStream_t)stream;
   // This step overwrites the device outputs: the D2H of this handle's previous
   // async step must have read them.  Other handles sharing `s` are not held up.
   if (h->pending_slot >= 0) PCL_CUDA(h, cudaStreamWaitEvent(s, h->ev_done[h->pending_slot], 0));
@@ -812,12 +833,8 @@ pcl::ObserveParams observe_params(const pcl_handle* h, const pcl_observe_spec* s
   pcl::ObserveParams p;
   memset(&p, 0, sizeof(p));
   p.B = h->batch; p.H = h->spec.rows; p.W = h->spec.cols; p.pitch = h->spec.pitch;
-  p.depth = spec->depth; p.dtype = spec->dtype;
-  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
-  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
-  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
-  p.table = d_table; p.valid = d_valid; p.board = d_board; p.out = d_out;
-  p.unknown = d_unknown;
+  p.board = d_board;
+  fill_elements(&p, spec, d_table, d_valid, d_out, d_unknown);
   return p;
 }
 
@@ -830,12 +847,19 @@ pcl::CropObserveParams crop_observe_params(const pcl_handle* h, const pcl_crop_s
   pcl::CropObserveParams p;
   memset(&p, 0, sizeof(p));
   p.crop = crop_params(h, crop, d_board, nullptr, d_crop_state);
-  p.depth = spec->depth; p.dtype = spec->dtype;
-  p.words = spec->dtype >= 3 ? 2 : 1;     // 8-byte elements: two u32; 2-byte: two u8
-  p.stride_b = spec->stride_b * p.words; p.stride_d = spec->stride_d * p.words;
-  p.stride_r = spec->stride_r * p.words; p.stride_c = spec->stride_c * p.words;
-  p.table = d_table; p.valid = d_valid; p.out = d_out; p.unknown = d_unknown;
+  fill_elements(&p, spec, d_table, d_valid, d_out, d_unknown);
   p.pad_plane = -1;
+  return p;
+}
+
+// pcl_pack_handoff's launch: each env's view and outputs in one record.
+pcl::PackParams pack_params(const pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
+                            const pcl_outputs* out) {
+  pcl::PackParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = h->batch; p.view_bytes = view_bytes;
+  p.record_bytes = PCL_HANDOFF_RECORD_BYTES(view_bytes);
+  p.view = d_view; p.out = *out;
   return p;
 }
 }  // namespace
@@ -850,9 +874,8 @@ int pcl_attach_cropper(pcl_handle* h, const pcl_crop_spec* crop, uint8_t* d_crop
   }
   if (!d_crop) return PCL_ERR_INVALID;
   if (!h->program->crop_epilogue) return PCL_ERR_UNSUPPORTED;
-  const int ok = crop_spec_ok(h, crop);
+  const int ok = crop_accepted(h, crop, Curtains::kNone);   // drape medians need scratch memory
   if (ok != PCL_OK) return ok;
-  if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape medians need scratch memory
   h->base.cropper = crop_params(h, crop, nullptr, d_crop, d_crop_state);
   h->base.has_cropper = 1;
   return PCL_OK;
@@ -869,15 +892,9 @@ int pcl_crop_tracking(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d
   Range nvtx_range("pcl_crop (ScrollingCropper.crop)");
   if (!h || !crop || !d_board || !d_crop) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  const int ok = crop_spec_ok(h, crop);
-  if (ok != PCL_OK) return ok;
   pcl::CropParams p = crop_params(h, crop, d_board, d_crop, d_crop_state);
-  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
-    if (crop->track[i] > 0) continue;
-    if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
-    if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
-    p.curtains[i] = d_curtains[i];
-  }
+  const int ok = crop_accepted(h, crop, Curtains::kCaller, d_curtains, &p);
+  if (ok != PCL_OK) return ok;
   return crop_launch(h, p, (cudaStream_t)stream);
 }
 
@@ -892,16 +909,10 @@ int pcl_crop_observe(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   if (d_planes ? !d_plane_of : !d_board) return PCL_ERR_INVALID;
   if (!observe_spec_ok(spec, 0)) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  const int ok = crop_spec_ok(h, crop);
-  if (ok != PCL_OK) return ok;
   pcl::CropObserveParams p = crop_observe_params(h, crop, d_board, d_crop_state, spec, d_table,
                                                  d_valid, d_out, d_unknown);
-  for (int i = 0; i < PCL_MAX_TRACK && crop->track[i] != 0; ++i) {
-    if (crop->track[i] > 0) continue;
-    if (!d_curtains || !d_curtains[i]) return PCL_ERR_INVALID;
-    if (h->spec.rows > 128 || h->spec.cols > 128) return PCL_ERR_UNSUPPORTED;
-    p.crop.curtains[i] = d_curtains[i];
-  }
+  const int ok = crop_accepted(h, crop, Curtains::kCaller, d_curtains, &p.crop);
+  if (ok != PCL_OK) return ok;
   p.planes = d_planes; p.plane_of = d_plane_of; p.pad_plane = d_planes ? pad_plane : -1;
   p.plane_stride_b = plane_stride_b; p.plane_stride_d = plane_stride_d;
   p.plane_stride_r = plane_stride_r;
@@ -914,11 +925,9 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
   Range nvtx_range("pcl_crop_handoff");
   if (!h || !crop || !d_board || !out || !x) return PCL_ERR_INVALID;
   if (!h->bound) return PCL_ERR_UNBOUND;
-  if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
-  const int ok = crop_spec_ok(h, crop);
+  int ok = int32_record_ok(h, *out);                         // the record's reward is int32
+  if (ok == PCL_OK) ok = crop_accepted(h, crop, Curtains::kNone);
   if (ok != PCL_OK) return ok;
-  if (tracks_drape(crop)) return PCL_ERR_UNSUPPORTED;        // drape tracking: pcl_crop_tracking
   const int view = crop->rows * crop->cols;
   if (x->n_peers < 1 || x->n_peers > PCL_MAX_PEERS || x->rank < 0 || x->rank >= x->n_peers)
     return PCL_ERR_INVALID;
@@ -948,13 +957,10 @@ int pcl_crop_handoff(pcl_handle* h, const pcl_crop_spec* crop, const uint8_t* d_
 int pcl_pack_handoff(pcl_handle* h, const uint8_t* d_view, int32_t view_bytes,
                      const pcl_outputs* out, uint8_t* d_packed, void* stream) {
   if (!h || !d_view || !out || !d_packed || view_bytes <= 0) return PCL_ERR_INVALID;
-  if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
-  pcl::PackParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.view_bytes = view_bytes;
-  p.record_bytes = PCL_HANDOFF_RECORD_BYTES(view_bytes);
-  p.view = d_view; p.out = *out; p.packed = d_packed;
+  const int ok = int32_record_ok(h, *out);
+  if (ok != PCL_OK) return ok;
+  pcl::PackParams p = pack_params(h, d_view, view_bytes, out);
+  p.packed = d_packed;
   return launched(h, pcl::launch_pack_handoff(p, (cudaStream_t)stream), "launch_pack_handoff");
 }
 
@@ -964,13 +970,9 @@ int pcl_pack_handoff_peers(pcl_handle* h, const uint8_t* d_view, int32_t view_by
   if (!h || !d_view || !out || !d_peer_bases || view_bytes <= 0 || first_row < 0)
     return PCL_ERR_INVALID;
   if (n_peers < 1 || n_peers > PCL_MAX_PEERS) return PCL_ERR_INVALID;
-  if (!outputs_set(*out)) return PCL_ERR_INVALID;
-  if (float_rewards(h)) return PCL_ERR_UNSUPPORTED;     // the record's reward is int32
-  pcl::PackParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = h->batch; p.view_bytes = view_bytes;
-  p.record_bytes = PCL_HANDOFF_RECORD_BYTES(view_bytes);
-  p.view = d_view; p.out = *out;
+  const int ok = int32_record_ok(h, *out);
+  if (ok != PCL_OK) return ok;
+  pcl::PackParams p = pack_params(h, d_view, view_bytes, out);
   p.n_peers = n_peers; p.first_row = first_row;
   for (int i = 0; i < n_peers; ++i) {
     if (!d_peer_bases[i]) return PCL_ERR_INVALID;
@@ -1010,9 +1012,8 @@ int rollout_ok(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_out
   if (float_rewards(h) && rec->d_reward && !rec->d_reward_f64) return PCL_ERR_INVALID;
   if (rec->crop) {                 // the cropper after each step: the handle has none attached
     if (h->base.has_cropper || !rec->d_crop) return PCL_ERR_INVALID;
-    const int ok = crop_spec_ok(h, rec->crop);
+    const int ok = crop_accepted(h, rec->crop, Curtains::kNone);   // no curtains between steps
     if (ok != PCL_OK) return ok;
-    if (tracks_drape(rec->crop)) return PCL_ERR_UNSUPPORTED;   // no curtains between steps
   }
   if (rec->d_attached && !rec->crop && !h->base.has_cropper) return PCL_ERR_INVALID;
   const pcl_observe_spec* spec = rec->observe;
@@ -1020,12 +1021,7 @@ int rollout_ok(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_out
   if (!rec->d_table || !observe_spec_ok(spec, 0)) return PCL_ERR_INVALID;
   if (steps > 0 && !rec->d_view) return PCL_ERR_INVALID;     // no step, no view written
   if ((uintptr_t)rec->d_view % element_bytes(spec->dtype)) return PCL_ERR_INVALID;
-  if (rec->observe_crop) {
-    const int ok = crop_spec_ok(h, rec->observe_crop);
-    if (ok != PCL_OK) return ok;
-    if (tracks_drape(rec->observe_crop)) return PCL_ERR_UNSUPPORTED;
-  }
-  return PCL_OK;
+  return rec->observe_crop ? crop_accepted(h, rec->observe_crop, Curtains::kNone) : PCL_OK;
 }
 
 // pcl_rollout once checked (rollout_ok): the launches of every step, then step T-1's

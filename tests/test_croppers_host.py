@@ -10,9 +10,12 @@
   PCL_MAX_CROP_CELLS cells and for drape tracking past 128 rows or columns, on handles
   that reach no device (device -1, made-up addresses): each is refused before anything
   is enqueued, pcl_step_host_async included.
+- The same entry points over a grid of specs around every edge of the acceptance rule,
+  each refused spec against the rule restated in Python, status for status.
 """
 
 import ctypes as C
+import itertools
 
 import numpy as np
 import pytest
@@ -188,11 +191,15 @@ def _none_handle(H, W, S=2, D=2):
   return lib, h
 
 
-def _scrolly_handle():
+def _scrolly_spec():
   from pycolab_b200 import levels, lowering
   from pycolab_b200.games import scrolly_maze
   art = levels.scrolly_maze_level(3, world_shape=(33, 33), board_shape=(16, 16))
-  spec = lowering.lower(scrolly_maze.make_game(*art)).make_spec(True)
+  return lowering.lower(scrolly_maze.make_game(*art)).make_spec(True)
+
+
+def _scrolly_handle():
+  spec = _scrolly_spec()
   lib = _lib.load()
   h = C.c_void_p()
   assert lib.pcl_create(C.byref(spec), 4, -1, C.byref(h)) == _lib.OK
@@ -215,25 +222,71 @@ def _step_host_async(lib, h, spec):
                                  FAKE, FAKE, FAKE, FAKE, 0, None)
 
 
-def _calls(lib, h, spec):
+NO_CURTAINS = (0,) * _lib.MAX_TRACK                   # pcl_crop: d_curtains is NULL
+ALL_CURTAINS = (1,) * _lib.MAX_TRACK
+SOME_CURTAINS = (1, 0, 1, 0)
+
+
+def _curtains(present):
+  return (C.c_void_p * _lib.MAX_TRACK)(*[FAKE if p else None for p in present])
+
+
+def _entry_points(lib, h, scrolly):
+  """(name, on_scrolly, curtains, call(spec)) of every entry point that takes a crop spec,
+  with every other argument valid: each on the PROG_NONE handle `h` but pcl_attach_cropper,
+  which needs a program whose step kernel runs the cropper and gets `scrolly`, a
+  scrolly_maze handle.  `curtains` is None for an entry point that takes no curtains, else
+  which of the caller's are set.  pcl_rollout takes a spec in two slots; its calls have
+  steps = 0."""
+  out = _lib.Outputs(FAKE, FAKE, FAKE, FAKE, FAKE, FAKE)
+  x = _lib.HandoffState()
+  x.n_peers, x.rank, x.record_bytes, x.rows, x.first_row = 1, 0, 256, 4, 0
+  x.d_peer_base[0], x.d_peer_flags[0], x.d_local = FAKE, FAKE, FAKE
+  observe = _lib.ObserveSpec(1, 0, 35, 35, 7, 1)
+
+  def tracking(present):
+    return lambda spec: lib.pcl_crop_tracking(h, C.byref(spec), FAKE, FAKE, FAKE,
+                                              _curtains(present), None)
+
+  def crop_observe(spec):
+    return lib.pcl_crop_observe(h, C.byref(spec), FAKE, FAKE, _curtains(ALL_CURTAINS),
+                                C.byref(observe), FAKE, None, None, None, -1, 0, 0, 0, FAKE,
+                                None, None)
+
+  def rollout(slot):
+    def call(spec):
+      rec = _lib.RolloutRec()
+      if slot == 'crop':
+        rec.crop, rec.d_crop = C.pointer(spec), FAKE
+      else:
+        rec.observe, rec.observe_crop = C.pointer(observe), C.pointer(spec)
+        rec.d_table, rec.d_view = FAKE, FAKE
+      return lib.pcl_rollout(h, FAKE, 0, C.byref(out), C.byref(rec), None)
+    return call
+
+  return [
+      ('pcl_crop', False, NO_CURTAINS,
+       lambda spec: lib.pcl_crop(h, C.byref(spec), FAKE, FAKE, FAKE, None)),
+      ('pcl_crop_tracking', False, ALL_CURTAINS, tracking(ALL_CURTAINS)),
+      ('pcl_crop_tracking/some', False, SOME_CURTAINS, tracking(SOME_CURTAINS)),
+      ('pcl_crop_observe', False, ALL_CURTAINS, crop_observe),
+      ('pcl_crop_handoff', False, None,
+       lambda spec: lib.pcl_crop_handoff(h, C.byref(spec), FAKE, FAKE, C.byref(out), C.byref(x),
+                                         None)),
+      ('pcl_step_host_async', False, None, lambda spec: _step_host_async(lib, h, spec)),
+      ('pcl_rollout/crop', False, None, rollout('crop')),
+      ('pcl_rollout/observe_crop', False, None, rollout('observe_crop')),
+      ('pcl_attach_cropper', True, None,
+       lambda spec: lib.pcl_attach_cropper(scrolly, C.byref(spec), FAKE, FAKE)),
+  ]
+
+
+def _calls(lib, h, scrolly, spec):
   """{entry point: status} of every cropper entry point for `spec`, which every one of them
   must refuse: a spec one of them accepts would launch on the made-up addresses (device -1
   only means the handle selects no device; where a GPU is present the launch runs on the
   current one)."""
-  curtains = (C.c_void_p * _lib.MAX_TRACK)(*([FAKE] * _lib.MAX_TRACK))
-  out = _lib.Outputs(FAKE, FAKE, FAKE, FAKE, FAKE)
-  x = _lib.HandoffState()
-  x.n_peers, x.rank, x.record_bytes, x.rows, x.first_row = 1, 0, 256, 4, 0
-  x.d_peer_base[0], x.d_peer_flags[0], x.d_local = FAKE, FAKE, FAKE
-  got = {}
-  if not any(code < 0 for code in spec.track):
-    got['pcl_crop'] = lib.pcl_crop(h, C.byref(spec), FAKE, FAKE, FAKE, None)
-  got['pcl_crop_tracking'] = lib.pcl_crop_tracking(h, C.byref(spec), FAKE, FAKE, FAKE,
-                                                   curtains, None)
-  got['pcl_crop_handoff'] = lib.pcl_crop_handoff(h, C.byref(spec), FAKE, FAKE, C.byref(out),
-                                                 C.byref(x), None)
-  got['pcl_step_host_async'] = _step_host_async(lib, h, spec)
-  return got
+  return dict((name, call(spec)) for name, _, _, call in _entry_points(lib, h, scrolly))
 
 
 @pytest.mark.parametrize('window', [(256, 256), (257, 256), (65536, 1), (1, 65536),
@@ -243,15 +296,15 @@ def test_windows_past_the_cell_limit_are_unsupported_everywhere(window):
   before any launch (a launch would fail with a CUDA error instead)."""
   for track in (None, [1], [-1, 2]):
     lib, h = _none_handle(16, 16)
+    _, scrolly = _scrolly_handle()
     try:
-      got = _calls(lib, h, _spec(window[0], window[1], track))
+      got = _calls(lib, h, scrolly, _spec(window[0], window[1], track))
     finally:
       lib.pcl_destroy(h)
+      lib.pcl_destroy(scrolly)
     assert set(got.values()) == {_lib.ERR_UNSUPPORTED}, (track, got)
   lib, h = _scrolly_handle()
   try:
-    spec = _spec(window[0], window[1])
-    assert lib.pcl_attach_cropper(h, C.byref(spec), FAKE, FAKE) == _lib.ERR_UNSUPPORTED
     spec = _spec(255, 257)                          # 65 535 cells: the largest accepted
     assert lib.pcl_attach_cropper(h, C.byref(spec), FAKE, FAKE) == _lib.OK
   finally:
@@ -278,9 +331,93 @@ def test_step_host_async_refuses_drape_tracking_before_the_step(track):
   handle would fail to create its copy stream).  pcl_crop_tracking accepts the same spec,
   so it is not called here: it would launch on the made-up addresses."""
   lib, h = _none_handle(16, 16)
+  _, scrolly = _scrolly_handle()
   try:
     assert _step_host_async(lib, h, _spec(5, 7, track)) == _lib.ERR_UNSUPPORTED
-    bad = _spec(5, 7, [3])                                      # no sprite 2
-    assert set(_calls(lib, h, bad).values()) == {_lib.ERR_INVALID}
+    bad = _spec(5, 7, [5])                          # no sprite 4 on either handle
+    assert set(_calls(lib, h, scrolly, bad).values()) == {_lib.ERR_INVALID}
   finally:
     lib.pcl_destroy(h)
+    lib.pcl_destroy(scrolly)
+
+
+# ---- one acceptance rule, every entry point ----------------------------------------
+
+def _accepted(dims, spec, curtains):
+  """The C boundary's rule for a crop spec, restated: the status an entry point gives `spec`
+  on a handle of `dims` (rows, cols, n_sprites, n_drapes) once its other arguments pass.
+  `curtains` is None for an entry point that takes no curtains, else which are set."""
+  H, W, S, D = dims
+  track = []
+  for code in spec.track:
+    if code == 0:
+      break
+    track.append(code)
+  if spec.rows <= 0 or spec.cols <= 0:
+    return _lib.ERR_INVALID
+  if not track and spec.sprite_index >= S:
+    return _lib.ERR_INVALID
+  if spec.sprite_index >= 0 and (2 * spec.margin_rows >= spec.rows or
+                                 2 * spec.margin_cols >= spec.cols):
+    return _lib.ERR_INVALID
+  if spec.pad_char < 0 and (spec.rows > H or spec.cols > W):
+    return _lib.ERR_INVALID
+  if track and (spec.sprite_index < 0 or any(c > S or c < -D for c in track)):
+    return _lib.ERR_INVALID
+  if spec.rows * spec.cols > _lib.MAX_CROP_CELLS:
+    return _lib.ERR_UNSUPPORTED
+  for i, code in enumerate(track):
+    if code > 0:
+      continue
+    if curtains is None:
+      return _lib.ERR_UNSUPPORTED
+    if not curtains[i]:
+      return _lib.ERR_INVALID
+    if H > 128 or W > 128:
+      return _lib.ERR_UNSUPPORTED
+  return _lib.OK
+
+
+def _spec_grid(dims):
+  """Crop specs around every edge of the rule for a handle of `dims`."""
+  H, W, S, D = dims
+  windows = [(5, 7), (4, 6), (1, 1), (0, 5), (5, 0), (-1, 3), (H, W), (H + 1, W), (H, W + 1),
+             (255, 257), (256, 256), (65535, 1), (65536, 1)]
+  tracks = [[], [1], [S], [S + 1], [-1], [-D], [-D - 1], [1, -1], [-D, S], [S, -D - 1],
+            [-1, 1, -2, 2], [2, -1, 1, -2]]
+  for rows, cols in windows:
+    margins = set([(0, 0), ((rows - 1) // 2, (cols - 1) // 2), (rows // 2, 0), (0, cols // 2),
+                   ((rows + 1) // 2, 0), (0, (cols + 1) // 2)])
+    for (mr, mc), pad, sprite, track in itertools.product(
+        sorted(margins), (-1, ord('.')), (-1, 0, S - 1, S), tracks):
+      spec = _lib.CropSpec(rows, cols, sprite, pad, mr, mc, 0, 0, 1)
+      for i, code in enumerate(track):
+        spec.track[i] = code
+      yield spec
+
+
+@pytest.mark.parametrize('board', [(16, 16, 2, 2), (16, 16, 0, 1), (128, 128, 2, 2),
+                                   (129, 128, 2, 2), (128, 129, 2, 2)], ids=str)
+def test_every_entry_point_refuses_as_the_rule_does(board):
+  """Every entry point that takes a crop spec gives the rule's exact status for every spec
+  of the grid the rule refuses.  Only those are called: the handles' addresses are made up,
+  and an accepted spec would launch on them (the GPU tests cover accepted specs)."""
+  scrolly_spec = _scrolly_spec()
+  theirs = (scrolly_spec.rows, scrolly_spec.cols, scrolly_spec.n_sprites, scrolly_spec.n_drapes)
+  lib, h = _none_handle(*board)
+  _, scrolly = _scrolly_handle()
+  seen = {}
+  try:
+    for name, on_scrolly, curtains, call in _entry_points(lib, h, scrolly):
+      dims = theirs if on_scrolly else board
+      for spec in _spec_grid(dims):
+        want = _accepted(dims, spec, curtains)
+        seen.setdefault(name, set()).add(want)
+        if want != _lib.OK:
+          assert call(spec) == want, (name, [getattr(spec, f) for f, _ in spec._fields_[:9]],
+                                      list(spec.track))
+  finally:
+    lib.pcl_destroy(h)
+    lib.pcl_destroy(scrolly)
+  for name, statuses in seen.items():      # every entry point meets every verdict
+    assert statuses == {_lib.OK, _lib.ERR_INVALID, _lib.ERR_UNSUPPORTED}, name
