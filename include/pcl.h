@@ -551,7 +551,8 @@ typedef struct pcl_rollout_rec {
  * naming a drape is PCL_ERR_UNSUPPORTED: no curtains are exported between steps); then the
  * launches are enqueued with no allocation and no host synchronisation, so the call can be
  * captured into a CUDA graph.  Consecutive step launches are block-chained as pcl_run's
- * are when no other kernel lies between them (no observer, no cropper after the step). */
+ * are when no other kernel lies between them (no observer, no cropper after the step).
+ * pcl_rollout_episodes (below) also keeps each step's episode return and length. */
 int pcl_rollout(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
                 const pcl_rollout_rec* rec, void* stream);
 /* sizeof(pcl_rollout_rec), for bindings to verify their layout at load time. */
@@ -590,6 +591,51 @@ int pcl_run_many(pcl_handle* const* handles, int n_handles, const int32_t* const
  * 7.5 us once per L + 1 steps. */
 #define PCL_DONE_TIME_LIMIT 2
 int pcl_set_time_limit(pcl_handle* h, int32_t max_frames);
+
+/* Episode returns.  pcl_bind_episodes(h, d_return) binds a caller-owned f64 [B] device
+ * buffer of running returns; NULL turns tracking off (the default).  With it bound, every
+ * launch that steps or (re)starts an env updates that env's episode return R:
+ *   r = the step's reward as a double: (double)reward for int32-reward programs (exact),
+ *       the value stored to d_reward_f64 for float-reward programs, 0.0 when has_reward
+ *       is 0;
+ *   R = r when the step's frame is 0 (its_showtime: pcl_reset, or a restart under
+ *       auto_reset), else R = R + r, one IEEE double addition per step in step order.
+ * That is what `ret = r if frame == 0 else ret + r` computes in Python over the engine's
+ * own outputs and plot frames.  The episode length is the plot's frame after the step (the
+ * number of steps since the env's (re)start), so it is not stored again.  At a step with
+ * done != 0, R and the frame are the finished episode's return and length; a truncated
+ * episode's (PCL_DONE_TIME_LIMIT) return is the sum up to the cut.  An env a launch skips
+ * writes nothing: a frozen env without auto_reset, an env a masked pcl_reset leaves alone.
+ * R starts as whatever the buffer holds; the env's first (re)start after binding
+ * overwrites it.
+ * The binding is read when a step or reset is launched: pcl_step, pcl_reset, pcl_run,
+ * pcl_run_many, pcl_rollout* and pcl_step_host* of the handle use it, and a CUDA graph
+ * captured earlier keeps the binding it was captured with.  It survives pcl_bind_state.
+ * Every output, record and board is the same with and without it; the work per env-step is
+ * one 8-byte load and one 8-byte store, plus the kept slots in a rollout (DESIGN.md section 5
+ * has what was measured).  PCL_ERR_INVALID for a NULL handle or a d_return that is not 8-byte
+ * aligned. */
+int pcl_bind_episodes(pcl_handle* h, double* d_return);
+
+/* What pcl_rollout_episodes keeps of each step's episode, in caller-owned [T, B] DEVICE
+ * buffers; NULL = not kept.  d_return f64 [T, B]: R after step t.  d_length i32 [T, B]:
+ * the env's plot frame after step t. */
+typedef struct pcl_episode_rec {
+  double* d_return;
+  int32_t* d_length;
+} pcl_episode_rec;
+
+/* pcl_rollout that also keeps every step's episode return and length (pcl_episode_rec);
+ * ep == NULL is pcl_rollout.  A kept array needs a handle with bound returns
+ * (pcl_bind_episodes) and an aligned pointer, else PCL_ERR_INVALID.  Without auto_reset the
+ * kept slots of an env frozen at step t hold 0.0 and 0.  Afterwards the bound [B] buffer
+ * holds R after step T-1, as after T pcl_step calls.  Launch and chaining counts are
+ * pcl_rollout's. */
+int pcl_rollout_episodes(pcl_handle* h, const int32_t* d_actions, int steps,
+                         const pcl_outputs* out, const pcl_rollout_rec* rec,
+                         const pcl_episode_rec* ep, void* stream);
+/* sizeof(pcl_episode_rec), for bindings to verify their layout at load time. */
+int pcl_episode_rec_size(void);
 
 /* The host-buffer and hand-off entry points below (pcl_step_host, pcl_step_host_async,
  * pcl_pack_handoff, pcl_pack_handoff_peers, pcl_crop_handoff) carry an int32 reward in their

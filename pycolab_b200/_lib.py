@@ -195,6 +195,12 @@ class RolloutRec(C.Structure):
               ('d_unknown', C.c_void_p), ('d_view', C.c_void_p), ('view_stride_t', C.c_int64)]
 
 
+class EpisodeRec(C.Structure):
+  """include/pcl.h pcl_episode_rec: [T, B] episode returns and lengths a rollout keeps
+  (NULL = not kept)."""
+  _fields_ = [('d_return', C.c_void_p), ('d_length', C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/pcl.h declares.
 SYMBOLS = {
     'pcl_abi_version': (C.c_int, []),
@@ -211,6 +217,11 @@ SYMBOLS = {
     'pcl_rollout': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs),
                               C.POINTER(RolloutRec), C.c_void_p]),
     'pcl_rollout_rec_size': (C.c_int, []),
+    'pcl_bind_episodes': (C.c_int, [C.c_void_p, C.c_void_p]),
+    'pcl_rollout_episodes': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Outputs),
+                                       C.POINTER(RolloutRec), C.POINTER(EpisodeRec),
+                                       C.c_void_p]),
+    'pcl_episode_rec_size': (C.c_int, []),
     'pcl_step_host': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Outputs),
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),
@@ -287,6 +298,10 @@ def load():
     raise PclLibraryError('struct layout mismatch between include/pcl.h and _lib.py: '
                           'pcl_rollout_rec is %d bytes in the library, %d in the binding' % (
                               lib.pcl_rollout_rec_size(), C.sizeof(RolloutRec)))
+  if lib.pcl_episode_rec_size() != C.sizeof(EpisodeRec):
+    raise PclLibraryError('struct layout mismatch between include/pcl.h and _lib.py: '
+                          'pcl_episode_rec is %d bytes in the library, %d in the binding' % (
+                              lib.pcl_episode_rec_size(), C.sizeof(EpisodeRec)))
   _lib = lib
   return lib
 

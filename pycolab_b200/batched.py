@@ -98,10 +98,32 @@ class Trajectory(object):
     self.view, self.attached, self.unknown = view, attached, unknown
 
 
+class Episodes(object):
+  """The episode returns and lengths `BatchedEngine.rollout(..., episodes=)` kept of T
+  steps, each a [T, B] device tensor.
+
+  episode_return: f64 [T, B], the env's episode return after step t (the engine's
+  `episode_return` then).  episode_length: i32 [T, B], the env's frame after step t: the
+  number of play()s since its (re)start.  At a step whose done is nonzero they are the
+  finished episode's return and length, so with `traj` the rollout's Trajectory
+
+      finished_returns = ep.episode_return[traj.done > 0]
+      finished_lengths = ep.episode_length[traj.done > 0]
+
+  are what a training loop logs.  An env frozen at step t (auto_reset off) holds 0.0 and 0.
+  Make one with `BatchedEngine.new_episodes(T)`, and pass it again to reuse its buffers.
+  """
+  __slots__ = ('episode_return', 'episode_length')
+
+  def __init__(self, episode_return, episode_length):
+    self.episode_return, self.episode_length = episode_return, episode_length
+
+
 class BatchedEngine(object):
 
   def __init__(self, games, batch=None, device=0, auto_reset=True, rng_seed=0,
-               env_offset=0, rng_states=None, share_levels=True, time_limit=None):
+               env_offset=0, rng_states=None, share_levels=True, time_limit=None,
+               track_episodes=False):
     """games: list of lowered games (`lowering.LoweredGame`) or set-up `Engine`s.
     Env e uses games[e % len(games)]; with a single game the static level data
     (backdrop, immutable patterns, reset templates) is shared by all envs.
@@ -112,8 +134,11 @@ class BatchedEngine(object):
     MT19937 states (624 key words + position) instead of seeds.
     share_levels=False stores the static level data once PER ENV instead of once
     per level (the reference's layout: every Engine owns its backdrop).
-    time_limit: see set_time_limit; None (the default) or 0 is no limit."""
+    time_limit: see set_time_limit; None (the default) or 0 is no limit.
+    track_episodes: keep each env's episode return on the device (`episode_return`)."""
     limit = _time_limit(time_limit)
+    if not isinstance(track_episodes, bool):
+      raise TypeError('track_episodes is True or False, got %r' % (track_episodes,))
     torch = _torch()
     self._lib = _lib.load()
     if not torch.cuda.is_available():
@@ -267,6 +292,16 @@ class BatchedEngine(object):
                  'pcl_bind_backdrop')
     self.time_limit = 0
     self.set_time_limit(limit)
+    # f64 [B]: each env's episode return, updated on the device by every step and reset
+    # (pcl_bind_episodes): the sum of the rewards since the env's (re)start, its reset frame's
+    # included, added in step order as `ret = r if frame == 0 else ret + r` does over the
+    # engine's own reward and frame.  At a step with done != 0 it is the finished episode's
+    # return, and the env's plot frame its length.  None unless track_episodes.
+    self.episode_return = None
+    if track_episodes:
+      self.episode_return = torch.zeros((B,), dtype=torch.float64, device=dev)
+      _lib.check(self._lib.pcl_bind_episodes(self._h, self.episode_return.data_ptr()),
+                 'pcl_bind_episodes')
     self._showtime = False
 
   def set_time_limit(self, n):
@@ -348,8 +383,17 @@ class BatchedEngine(object):
                                  C.byref(self._out), self._stream()), 'pcl_run', self._h)
     return self._result()
 
+  def new_episodes(self, T):
+    """An `Episodes` of T steps for `rollout(..., episodes=)` on this engine."""
+    torch = _torch()
+    if self.episode_return is None:
+      raise ValueError('episodes need an engine made with track_episodes=True')
+    T = int(T)
+    return Episodes(torch.zeros((T, self.batch), dtype=torch.float64, device=self.device),
+                    torch.zeros((T, self.batch), dtype=torch.int32, device=self.device))
+
   def rollout(self, actions, observer=None, crop_spec=None, state=None, keep_attached=False,
-              out=None):
+              out=None, episodes=None):
     """T steps from one C call (`pcl_rollout`), keeping every step's outputs.
 
     actions: int32 [T, B] or [T, B, actions_per_env] on the device.  Each step is play(),
@@ -364,7 +408,12 @@ class BatchedEngine(object):
     character outside its mapping; the flag is read once per call, and not at all while
     the stream is being captured (read `Trajectory.unknown` then).  `out`: a Trajectory
     of an earlier rollout of the same shape, whose buffers are reused, so that a captured
-    rollout replays into fixed memory."""
+    rollout replays into fixed memory.
+
+    `episodes`: an `Episodes` (new_episodes(T)) that also keeps every step's episode return
+    and length, on an engine made with track_episodes=True; `ep.episode_return[traj.done >
+    0]` and `ep.episode_length[traj.done > 0]` are then the episodes that finished in the
+    rollout.  Afterwards `episode_return` is step T-1's, as after T play()s."""
     torch = _torch()
     if not self._showtime:
       raise RuntimeError('rollout() cannot be called until the Engine is placed in "play '
@@ -393,6 +442,21 @@ class BatchedEngine(object):
       want['view'] = (tuple([T, B] + [base[i] for i in perm]), obs['dtype'])
       if obs['check']:
         want['unknown'] = ((1,), torch.int32)
+    ep_rec = None
+    if episodes is not None:
+      if self.episode_return is None:
+        raise ValueError('episodes= needs an engine made with track_episodes=True')
+      if not isinstance(episodes, Episodes):
+        raise TypeError('episodes= is an Episodes (new_episodes(T)), not %r' % (
+            type(episodes).__name__,))
+      for name, dtype in (('episode_return', torch.float64), ('episode_length', torch.int32)):
+        got = getattr(episodes, name)
+        if (not torch.is_tensor(got) or tuple(got.shape) != (T, B) or got.dtype != dtype or
+            got.device != dev or not got.is_contiguous()):
+          raise ValueError('episodes.%s is not a contiguous %s %s on %s' % (
+              name, dtype, (T, B), dev))
+      ep_rec = _lib.EpisodeRec(episodes.episode_return.data_ptr() if T else None,
+                               episodes.episode_length.data_ptr() if T else None)
     traj = out if out is not None else Trajectory(*[None] * 7)
     for name in Trajectory.__slots__:
       got = getattr(traj, name)
@@ -433,12 +497,18 @@ class BatchedEngine(object):
       rec.view_stride_t = traj.view.stride()[0]
     # an empty tensor has no address; a rollout of no step reads no action
     d_actions = actions.data_ptr() if T else self._actions.data_ptr()
-    status = self._lib.pcl_rollout(self._h, d_actions, T, C.byref(self._out), C.byref(rec),
-                                   self._stream())
+    if ep_rec is None:
+      what = 'pcl_rollout'
+      status = self._lib.pcl_rollout(self._h, d_actions, T, C.byref(self._out), C.byref(rec),
+                                     self._stream())
+    else:
+      what = 'pcl_rollout_episodes'
+      status = self._lib.pcl_rollout_episodes(self._h, d_actions, T, C.byref(self._out),
+                                              C.byref(rec), C.byref(ep_rec), self._stream())
     for spec in (crop, None if att is None else att[0]):
       if spec is not None:
-        _check_crop(status, 'pcl_rollout', self._h, spec)
-    _lib.check(status, 'pcl_rollout', self._h)
+        _check_crop(status, what, self._h, spec)
+    _lib.check(status, what, self._h)
     if obs is not None and obs['check'] and not torch.cuda.is_current_stream_capturing():
       if int(traj.unknown[0]):
         raise RuntimeError(

@@ -47,6 +47,7 @@ aperture_step(const StepParams p) {
 
   const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
+  const double ep_so_far = load_episode(p, env);   // store_episode below
   const bool restart = run == ENV_RESTART;
   if (restart) {                                   // a fresh Engine (engine.py:520-581)
     const PlotCarry carry = plot_carry(e.plot, true);
@@ -135,6 +136,7 @@ aperture_step(const StepParams p) {
     store_sprite(rec, sp, PCL_S_AUX0);
     rec[8 + PCL_D_AUX0] = ap0; rec[8 + PCL_D_AUX1] = ap1;
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_KEEP>(rec + 16, plot, dir);
     store_outputs(p.out, env, dir);
     // final render, z-order X then A: patch the staged tile (engine.py:737-759)

@@ -45,6 +45,7 @@ struct pcl_handle {
   const uint8_t* last_board;
   uint32_t board_epoch;
   int time_limit;                // pcl_set_time_limit; fill_params copies it into `base`
+  double* ep_return;             // pcl_bind_episodes; fill_params copies it into `base`
 };
 
 namespace {
@@ -156,6 +157,7 @@ void fill_params(const pcl_handle* h, StepParams* p) {
   p->code = h->code_dev;
   p->backdrop_live = h->backdrop_live;
   p->time_limit = h->time_limit;
+  p->ep_return = h->ep_return;
 }
 
 // Does the handle's Backdrop run compiled code on a live curtain (pcl_bind_backdrop)?
@@ -177,12 +179,17 @@ bool live_backdrop(const pcl_spec& s) {
 // of a run) is CHAIN_NONE: the kernel as it ran before chaining, at no extra cost.
 
 // The per-env memory one step launch touches: [lo, hi) byte ranges, and which it writes.
+// footprint() lists at most kFootprintSpans of them: the three state records, a pattern per
+// drape, the board, five outputs, the cropper's view and state, the actions or the reset
+// mask, and the episode returns with a rollout's two kept slots.
+constexpr int kFootprintSpans = 3 + PCL_MAX_DRAPES + 1 + 5 + 2 + 1 + 3;
 struct Footprint {
   const pcl_handle* h;           // nullptr: no step launch to chain to
   bool counted;                  // the launch kept the per-block counters (HEAD, FOLLOWS)
   int n;
   struct { uintptr_t lo, hi; bool written; } span[16 + PCL_MAX_DRAPES];
 };
+static_assert(kFootprintSpans <= 16 + PCL_MAX_DRAPES, "footprint() outgrows Footprint::span");
 
 Footprint footprint(const pcl_handle* h, const StepParams& p) {
   Footprint f;
@@ -211,6 +218,11 @@ Footprint footprint(const pcl_handle* h, const StepParams& p) {
   }
   add(p.mode == pcl::MODE_STEP ? p.actions : nullptr, B * h->actions_per_env * 4, false);
   add(p.mode == pcl::MODE_RESET ? p.env_mask : nullptr, B, false);
+  if (p.ep_return) {                        // store_episode writes them only when bound
+    add(p.ep_return, B * 8, true);
+    add(p.ep_return_keep, B * 8, true);
+    add(p.ep_length_keep, B * 4, true);
+  }
   return f;
 }
 
@@ -493,6 +505,13 @@ int pcl_set_time_limit(pcl_handle* h, int32_t max_frames) {
   if (!h || max_frames < 0) return PCL_ERR_INVALID;
   h->time_limit = max_frames;
   h->base.time_limit = max_frames;   // pcl_bind_state's fill_params copies it too
+  return PCL_OK;
+}
+
+int pcl_bind_episodes(pcl_handle* h, double* d_return) {
+  if (!h || (uintptr_t)d_return % alignof(double)) return PCL_ERR_INVALID;
+  h->ep_return = d_return;
+  h->base.ep_return = d_return;      // pcl_bind_state's fill_params copies it too
   return PCL_OK;
 }
 
@@ -1002,12 +1021,17 @@ T* slot(T* base, int t, int64_t per_env, int batch) {
   return base ? base + (int64_t)t * batch * per_env : nullptr;
 }
 
-// Everything pcl_rollout checks, before anything is enqueued.
+// Everything pcl_rollout_episodes checks, before anything is enqueued.
 int rollout_ok(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
-               const pcl_rollout_rec* rec, cudaStream_t s) {
+               const pcl_rollout_rec* rec, const pcl_episode_rec* ep, cudaStream_t s) {
   const int r = check_ready(h, out, s);
   if (r != PCL_OK) return r;
   if (!d_actions || steps < 0) return PCL_ERR_INVALID;
+  if (ep && (ep->d_return || ep->d_length)) {   // kept from the bound returns
+    if (!h->ep_return) return PCL_ERR_INVALID;
+    if ((uintptr_t)ep->d_return % alignof(double) || (uintptr_t)ep->d_length % alignof(int32_t))
+      return PCL_ERR_INVALID;
+  }
   if (!rec) return PCL_OK;
   if (float_rewards(h) && rec->d_reward && !rec->d_reward_f64) return PCL_ERR_INVALID;
   if (rec->crop) {                 // the cropper after each step: the handle has none attached
@@ -1024,12 +1048,15 @@ int rollout_ok(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_out
   return rec->observe_crop ? crop_accepted(h, rec->observe_crop, Curtains::kNone) : PCL_OK;
 }
 
-// pcl_rollout once checked (rollout_ok): the launches of every step, then step T-1's
-// outputs and attached view copied to where pcl_step and the cropper leave them.
+// pcl_rollout_episodes once checked (rollout_ok): the launches of every step, then step
+// T-1's outputs and attached view copied to where pcl_step and the cropper leave them.  The
+// bound returns need no copy: every step updates them in place.
 int rollout_enqueue(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
-                    const pcl_rollout_rec* rec, cudaStream_t s) {
+                    const pcl_rollout_rec* rec, const pcl_episode_rec* ep, cudaStream_t s) {
   static const pcl_rollout_rec kNothing = {};
+  static const pcl_episode_rec kNoEpisodes = {};
   const pcl_rollout_rec& x = rec ? *rec : kNothing;
+  const pcl_episode_rec& y = ep ? *ep : kNoEpisodes;
   const int64_t B = h->batch;
   const bool f64 = float_rewards(h);
   int32_t* keep_reward = f64 ? nullptr : x.d_reward;
@@ -1052,6 +1079,8 @@ int rollout_enqueue(pcl_handle* h, const int32_t* d_actions, int steps, const pc
     if (x.d_has_reward) PCL_CUDA(h, cudaMemsetAsync(x.d_has_reward, 0, n, s));
     if (x.d_discount) PCL_CUDA(h, cudaMemsetAsync(x.d_discount, 0, n * 4, s));
     if (x.d_done) PCL_CUDA(h, cudaMemsetAsync(x.d_done, 1, n, s));
+    if (y.d_return) PCL_CUDA(h, cudaMemsetAsync(y.d_return, 0, n * 8, s));
+    if (y.d_length) PCL_CUDA(h, cudaMemsetAsync(y.d_length, 0, n * 4, s));
   }
   // Step launches chain only to a step launch right before them.
   const bool chain = !x.observe && !has_after;
@@ -1070,6 +1099,8 @@ int rollout_enqueue(pcl_handle* h, const int32_t* d_actions, int steps, const pc
     if (x.d_has_reward) p.out.d_has_reward = slot(x.d_has_reward, t, 1, B);
     if (x.d_discount) p.out.d_discount = slot(x.d_discount, t, 1, B);
     if (x.d_done) p.out.d_done = slot(x.d_done, t, 1, B);
+    p.ep_return_keep = slot(y.d_return, t, 1, B);
+    p.ep_length_keep = slot(y.d_length, t, 1, B);
     if (in_step && x.d_attached) p.cropper.out = slot(x.d_attached, t, view_cells, B);
     if (!chain) run.h = nullptr;
     int e = launch(h, p, s, &run);
@@ -1119,23 +1150,30 @@ int rollout_enqueue(pcl_handle* h, const int32_t* d_actions, int steps, const pc
 
 extern "C" {
 
+int pcl_rollout_episodes(pcl_handle* h, const int32_t* d_actions, int steps,
+                         const pcl_outputs* out, const pcl_rollout_rec* rec,
+                         const pcl_episode_rec* ep, void* stream) {
+  Range nvtx_range("pcl_rollout");
+  const int r = rollout_ok(h, d_actions, steps, out, rec, ep, (cudaStream_t)stream);
+  if (r != PCL_OK) return r;
+  return rollout_enqueue(h, d_actions, steps, out, rec, ep, (cudaStream_t)stream);
+}
+
 int pcl_rollout(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
                 const pcl_rollout_rec* rec, void* stream) {
-  Range nvtx_range("pcl_rollout");
-  const int r = rollout_ok(h, d_actions, steps, out, rec, (cudaStream_t)stream);
-  if (r != PCL_OK) return r;
-  return rollout_enqueue(h, d_actions, steps, out, rec, (cudaStream_t)stream);
+  return pcl_rollout_episodes(h, d_actions, steps, out, rec, nullptr, stream);
 }
 
 int pcl_run(pcl_handle* h, const int32_t* d_actions, int steps, const pcl_outputs* out,
             void* stream) {
   Range nvtx_range("pcl_run");
-  const int r = rollout_ok(h, d_actions, steps, out, nullptr, (cudaStream_t)stream);
+  const int r = rollout_ok(h, d_actions, steps, out, nullptr, nullptr, (cudaStream_t)stream);
   if (r != PCL_OK) return r;
-  return rollout_enqueue(h, d_actions, steps, out, nullptr, (cudaStream_t)stream);
+  return rollout_enqueue(h, d_actions, steps, out, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int pcl_rollout_rec_size(void) { return (int)sizeof(pcl_rollout_rec); }
+int pcl_episode_rec_size(void) { return (int)sizeof(pcl_episode_rec); }
 
 int pcl_error_codes(pcl_handle* h, int32_t* d_out, void* stream) {
   if (!h || !d_out) return PCL_ERR_INVALID;

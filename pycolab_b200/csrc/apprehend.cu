@@ -40,6 +40,7 @@ apprehend_step(const StepParams p) {
 
   const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
+  const double ep_so_far = load_episode(p, env);   // store_episode below
   const bool restart = run == ENV_RESTART;
   const int32_t* src_s = e.start(restart, p.st.d_sprites_init, p.st.sprites_init_bstride, e.sprites);
   const int32_t* src_p = e.start(restart, p.st.d_plot_init, p.st.plot_init_bstride, e.plot);
@@ -84,6 +85,7 @@ apprehend_step(const StepParams p) {
     store_sprite(e.sprites + PCL_SPRITE_WORDS, ball);
     store_carry(e.plot, carry);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = __double2loint(acc); e.plot[PCL_P_AUX1] = __double2hiint(acc);
     store_outputs(p.out, env, dir);

@@ -155,6 +155,7 @@ better_scrolly_step(const StepParams p) {
     store_plot<ORDER_KEEP>(rec + 48, plot, dir);
     rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);
+    store_episode(p, env, plot.frame, load_episode(p, env), (double)dir.reward);
   }
   __syncwarp();
   e.sprites[lane] = rec[lane];

@@ -143,6 +143,7 @@ box_world_step(const StepParams p) {
     store_plot<ORDER_KEEP>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = over_ch; e.plot[PCL_P_AUX1] = over_at;
     store_outputs(p.out, env, dir);
+    store_episode(p, env, plot.frame, load_episode(p, env), (double)dir.reward);
   }
   if (lane < H && (restart || (changed >= 0 && (lane == 0 || lane == changed))))
     for (int q = 0; q < segs; ++q)

@@ -122,8 +122,10 @@ classics_step(const StepParams p) {
   // ---- _apply_and_clear_plot (engine.py:761-847) + records back
   __syncwarp();                 // every lane has read the staged records (racecheck: WAR)
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     store_sprite(rec, sp, PCL_S_AUX0);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_KEEP>(rec + 16, plot, dir);
     rec[16 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);

@@ -696,7 +696,9 @@ __device__ __forceinline__ void step(const StepParams& p) {
 
   __syncwarp();
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, p.program_arg[0] ? (rw.has ? rw.sum_f : 0.0) : (double)(rw.has ? rw.sum_i : 0));
     store_plot<ORDER_ALL>(st->plot, plot, dir);
     dir.reward = rw.has ? rw.sum_i : 0; dir.has_reward = rw.has;   // the code's own sums
     if (p.program_arg[0]) store_outputs(p.out, env, dir, rw.has ? rw.sum_f : 0.0);

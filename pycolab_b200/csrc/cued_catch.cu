@@ -288,6 +288,7 @@ cued_catch_step(const StepParams p) {
   }
 
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       sp[i].aux0 = i == SP ? ttr : 0;
@@ -296,6 +297,7 @@ cued_catch_step(const StepParams p) {
     store_drape(e.drapes, {phase, tick1, choice, tick2, last_reset, trials, pairs, 0});
     store_carry(e.plot, carry);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, noisy && noisy_pay ? reward_f64 : (double)dir.reward);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = programmed; e.plot[PCL_P_AUX1] = which;
     e.plot[PCL_P_AUX2] = ball_reset; e.plot[PCL_P_AUX3] = noisy_pay ? 1 : 0;

@@ -74,6 +74,7 @@ fixture_step(const StepParams p) {
 
   const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) return;
+  const double ep_so_far = load_episode(p, env);   // store_episode below
   const bool restart = run == ENV_RESTART;
   const PlotCarry carry = plot_carry(e.plot, restart);
   board::stage_records(
@@ -186,6 +187,7 @@ fixture_step(const StepParams p) {
   if (lane == 0) {
     group_in(plot, st, 0);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_ALL>(st->plot, plot, dir);
     store_outputs(p.out, env, dir);
   }

@@ -75,6 +75,7 @@ hello_step(const StepParams p) {
     apply_time_limit(p, plot, dir);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
+    store_episode(p, env, plot.frame, load_episode(p, env), (double)dir.reward);
   }
 
   // ---- render (engine.py:737-759): backdrop, then the z-order back to front.

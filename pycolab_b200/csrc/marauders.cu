@@ -228,6 +228,7 @@ marauders_step(const StepParams p) {
     store_plot<ORDER_KEEP>(rec + 72, plot, dir);
     rec[72 + PCL_P_AUX0] = plot.aux0; rec[72 + PCL_P_AUX1] = plot.aux1;
     store_outputs(p.out, env, dir);
+    store_episode(p, env, plot.frame, load_episode(p, env), (double)dir.reward);
   }
   __syncwarp();
   g_sprites[lane] = rec[lane];

@@ -45,6 +45,7 @@ ordeal_step(const StepParams p) {
 
   const EnvRun run = env_run(p, env, e.plot[PCL_P_GAME_OVER]);
   if (run == ENV_SKIP) { cp_async_wait_all(); return; }
+  const double ep_so_far = load_episode(p, env);   // store_episode below
   const bool restart = run == ENV_RESTART;
   if (restart) {                                   // a fresh Engine (engine.py:520-581)
     const PlotCarry carry = plot_carry(e.plot, true);
@@ -172,6 +173,7 @@ ordeal_step(const StepParams p) {
     store_sprite(rec, pl, PCL_S_AUX0);
     if (S > 1) store_sprite(rec + 8, dd, PCL_S_AUX0);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_KEEP>(rec + 32, plot, dir);
     rec[32 + PCL_P_AUX0] = has_sword; rec[32 + PCL_P_AUX1] = last_pos;
     rec[32 + PCL_P_AUX2] = next_chapter;

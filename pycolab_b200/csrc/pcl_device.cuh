@@ -548,6 +548,27 @@ __device__ __forceinline__ void apply_time_limit(const StepParams& p, const Plot
     dir.game_over = PCL_DONE_TIME_LIMIT;
 }
 
+// Episode returns (pcl_bind_episodes, include/pcl.h).  load_episode reads the env's return
+// so far, 0.0 when nothing is bound; a kernel issues it with the step's first record loads,
+// after the env's launch wait, so that its round trip overlaps the step instead of adding to
+// its tail.  store_episode, once per step in the lane and right after apply_time_limit:
+// R = r on a (re)start (frame 0), else the return so far + r, and the kept slots of a
+// rollout.  `r` is the reward the step stores, as a double.  Nothing is written when
+// nothing is bound.
+__device__ __forceinline__ double load_episode(const StepParams& p, int env) {
+  return p.ep_return ? p.ep_return[env] : 0.0;
+}
+__device__ __forceinline__ void store_episode(const StepParams& p, int env, int frame,
+                                              double so_far, double r) {
+  if (!p.ep_return) return;
+  // __dadd_rn: never contracted into an fma with the multiply that made r, so the sum is
+  // the rounded r the step stores, added in IEEE double.
+  const double ret = frame == 0 ? r : __dadd_rn(so_far, r);
+  p.ep_return[env] = ret;
+  if (p.ep_return_keep) p.ep_return_keep[env] = ret;
+  if (p.ep_length_keep) p.ep_length_keep[env] = frame;
+}
+
 // The step's outputs for env `env` (one lane stores them).
 __device__ __forceinline__ void store_outputs(const pcl_outputs& out, int env, const Directives& dir) {
   out.d_reward[env] = dir.reward;

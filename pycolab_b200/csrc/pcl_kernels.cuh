@@ -73,6 +73,12 @@ struct StepParams {
   // pcl_set_time_limit: a step that leaves an env at this frame or later ends its episode
   // (apply_time_limit, pcl_device.cuh); 0: no limit.
   int time_limit;
+  // pcl_bind_episodes: f64 [B] running episode returns, or NULL (store_episode,
+  // pcl_device.cuh); and where this launch keeps each env's return and length
+  // (pcl_rollout_episodes slot t), each NULL = not kept.
+  double* ep_return;
+  double* ep_return_keep;
+  int32_t* ep_length_keep;
 };
 
 // StepParams::chain (launch, api.cu; scrolly_maze.cu, "Block chaining").  CHAIN_NONE: the

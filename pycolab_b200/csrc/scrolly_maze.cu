@@ -830,9 +830,13 @@ __device__ __forceinline__ void step_env(const StepParams& p) {
   PCL_STAMP(kStWait);
   __syncwarp();
   if (lane == 0) {
+    // The env's episode return so far (store_episode below), in this lane only and behind
+    // the pointer test, so that with nothing bound the step's path is the one without it.
+    const double ep_so_far = load_episode(p, env);
     store_drape(rec + 32, walls, PCL_D_AUX0);
     store_drape(rec + 32 + PCL_DRAPE_WORDS, coins, PCL_D_AUX2);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_ALL>(rec + 48, plot, dir);
     rec[48 + PCL_P_AUX0] = plot.aux0;
     store_outputs(p.out, env, dir);

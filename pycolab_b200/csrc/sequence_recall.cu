@@ -151,6 +151,7 @@ sequence_recall_step(const StepParams p) {
   }
 
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     store_sprite(e.sprites, pl);
     const int32_t* init_d = e.level(p.st.d_drapes_init, p.st.drapes_init_bstride);
 #pragma unroll
@@ -162,6 +163,7 @@ sequence_recall_step(const StepParams p) {
     }
     store_carry(e.plot, carry);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, dir.has_reward ? reward : 0.0);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = pc; e.plot[PCL_P_AUX1] = fis;
     e.plot[PCL_P_AUX2] = timeout; e.plot[PCL_P_AUX3] = (int)seq;

@@ -115,11 +115,13 @@ shockwave_step(const StepParams p) {
     if (BW > 1) row[1] = (uint32_t)(new_row >> 32);
   }
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     store_sprite(e.sprites, pl);
     e.drapes[PCL_D_AUX0] = impact; e.drapes[PCL_D_AUX1] = steps;
     e.drapes[PCL_D_LAST_FRAME] = PCL_NEVER;
     store_carry(e.plot, carry);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_CLEAR>(e.plot, plot, dir);
     store_outputs(p.out, env, dir);
   }

@@ -292,6 +292,7 @@ t_maze_step(const StepParams p) {
 
   __syncwarp();
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     store_sprite(e.sprites, pl[0]);
     dr[DQ].aux0 = which_goal; dr[DQ].aux1 = yo ? 1 : 0; dr[DQ].aux2 = in_limbo ? 1 : 0;
     dr[DTELE].aux1 = delay; dr[DTELE].aux2 = countdown;
@@ -299,6 +300,7 @@ t_maze_step(const StepParams p) {
     for (int d = 0; d < ND; ++d) store_drape(e.drapes + d * PCL_DRAPE_WORDS, dr[d]);
     store_carry(e.plot, carry);
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, dir.has_reward ? reward : 0.0);
     store_plot<ORDER_ALL>(e.plot, plot, dir);
     e.plot[PCL_P_AUX0] = timeout; e.plot[PCL_P_AUX1] = tele_frame;
     e.plot[PCL_P_AUX2] = tele_r; e.plot[PCL_P_AUX3] = tele_c;

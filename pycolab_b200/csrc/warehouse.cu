@@ -209,9 +209,11 @@ warehouse_step(const StepParams p) {
   // ---- _apply_and_clear_plot + records back
   __syncwarp();
   if (lane == 0) {
+    const double ep_so_far = load_episode(p, env);   // overlaps the stores below
     store_sprite(rec + NB * PCL_SPRITE_WORDS, player, PCL_S_AUX0);
     r_judge[PCL_D_AUX0] = on_goals;
     apply_time_limit(p, plot, dir);
+    store_episode(p, env, plot.frame, ep_so_far, (double)dir.reward);
     store_plot<ORDER_KEEP>(r_plot, plot, dir);
     store_outputs(p.out, env, dir);
   }
