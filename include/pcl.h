@@ -637,6 +637,36 @@ int pcl_rollout_episodes(pcl_handle* h, const int32_t* d_actions, int steps,
 /* sizeof(pcl_episode_rec), for bindings to verify their layout at load time. */
 int pcl_episode_rec_size(void);
 
+/* Seeded generators.  pcl_seed_rng writes, for every env whose d_env_mask byte is non-zero
+ * (NULL = all), each of its n_slots generator slots in pcl_state.d_rng (u32 [B, n_slots,
+ * PCL_MT_WORDS]) as a fresh generator seeded with d_seeds[env] (u32 [B], DEVICE) would hold
+ * them.  h_kinds (HOST, n_slots values, in d_rng slot order) names each slot's rule.  For a
+ * seed s in [0, 2^32):
+ *   PCL_SEED_NUMPY   the words of np.random.RandomState(s) (NumPy's legacy seeding): key
+ *                    word 0 is s, word i is 1812433253 * (w ^ (w >> 30)) + i of the word w
+ *                    before it, and the position is 624;
+ *   PCL_SEED_PYTHON  the words of random.Random(s).getstate()[1] (CPython's init_by_array
+ *                    over the one-word key [s]): the key words of init_genrand(19650218),
+ *                    the same for every seed, then its two mixing loops, then word 0 =
+ *                    0x80000000, and the position is 624.
+ * Either way the next draw twists first, as it does from any host-seeded words.  Unselected
+ * envs, and every array but d_rng, are left untouched.  The call allocates nothing and does
+ * not synchronise, so it can be captured into a CUDA graph.  The generators are all a restart
+ * draws from, so a pcl_reset of the same mask after this call runs each env's its_showtime()
+ * frame from its new words: that is Gymnasium's reset(seed=...), per env.  Draws made when
+ * the game was built (the reset templates) are not redrawn.
+ * Refusals, in order: PCL_ERR_INVALID for a NULL handle or NULL d_seeds; PCL_ERR_UNBOUND
+ * before pcl_bind_state; PCL_ERR_UNSUPPORTED for a program with no generator slots;
+ * PCL_ERR_INVALID when the bound d_rng is NULL, n_slots is not the program's slot count
+ * (1 for PCL_PROG_MARAUDERS, _SHOCKWAVE, _APPREHEND, _CUED_CATCH and _SEQUENCE_RECALL, 2 for
+ * PCL_PROG_T_MAZE, program_arg[1] for PCL_PROG_COMPILED), or h_kinds is NULL or holds a
+ * value that is not a PCL_SEED_*.
+ * Cost (DESIGN.md section 5; H100 80GB HBM3, 700 W): 54 us for 4096 envs of two slots, 420 us
+ * for 65 536. */
+enum { PCL_SEED_NUMPY = 0, PCL_SEED_PYTHON = 1 };
+int pcl_seed_rng(pcl_handle* h, const uint8_t* d_env_mask, const uint32_t* d_seeds,
+                 const int32_t* h_kinds, int n_slots, void* stream);
+
 /* The host-buffer and hand-off entry points below (pcl_step_host, pcl_step_host_async,
  * pcl_pack_handoff, pcl_pack_handoff_peers, pcl_crop_handoff) carry an int32 reward in their
  * host buffers and records: they return PCL_ERR_UNSUPPORTED for a program with float64

@@ -29,6 +29,7 @@ HOST_SLOTS = 8               # pcl_step_host_async completion slots
 NEVER = -(2 ** 31)           # INT32_MIN: "-inf"/None frame
 ACTION_NONE = -1
 DONE_TIME_LIMIT = 2          # done (and plot game-over word) of an episode the time limit ended
+SEED_NUMPY, SEED_PYTHON = 0, 1   # pcl_seed_rng kinds: RandomState(s) / random.Random(s) words
 
 OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_UNBOUND, ERR_NOMEM = 0, -1, -2, -3, -4, -5
 
@@ -222,6 +223,8 @@ SYMBOLS = {
                                        C.POINTER(RolloutRec), C.POINTER(EpisodeRec),
                                        C.c_void_p]),
     'pcl_episode_rec_size': (C.c_int, []),
+    'pcl_seed_rng': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int,
+                               C.c_void_p]),
     'pcl_step_host': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Outputs),
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),

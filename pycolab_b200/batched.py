@@ -10,6 +10,7 @@ C ABI (`pcl_step`); there is no CPU path.
 
 import ctypes as C
 import numbers
+import operator
 import random
 
 import numpy as np
@@ -54,6 +55,20 @@ def _mt_state(stream, seed):
     return np.array(random.Random(seed).getstate()[1], dtype=np.uint32)
   _, key, pos, _, _ = np.random.RandomState(seed).get_state()
   return np.append(key, pos).astype(np.uint32)
+
+
+SEED_LIMIT = 2 ** 32             # pcl_seed_rng takes seeds in [0, SEED_LIMIT)
+
+
+def _device_seeded(rng_seed, env_offset, batch):
+  """Does the constructor seed its generators on the device (pcl_seed_rng)?  Only when every
+  env's seed rng_seed + env_offset + e is an int in [0, 2**32), where the kernel writes the
+  words `_mt_state` would.  Other seeds keep the host words: a game that draws from Python's
+  `random` only takes any int there, and NumPy raises for them as it always has."""
+  if not (isinstance(rng_seed, numbers.Integral) and isinstance(env_offset, numbers.Integral)):
+    return False
+  first = int(rng_seed) + int(env_offset)
+  return 0 <= first and first + int(batch) <= SEED_LIMIT
 
 
 class StepResult(object):
@@ -129,7 +144,8 @@ class BatchedEngine(object):
     (backdrop, immutable patterns, reset templates) is shared by all envs.
     env_offset: global index of this shard's env 0 (per-env RNG streams are
     seeded rng_seed + global env index — NumPy RandomState(seed) or, for games that
-    draw from Python's `random`, random.Random(seed)); rng_states: explicit u32 [B, 625]
+    draw from Python's `random`, random.Random(seed); written on the device by pcl_seed_rng
+    when every such seed lies in [0, 2**32), else on the host); rng_states: explicit u32 [B, 625]
     (False: bind no RNG, for programs that can take their draws from the templates)
     MT19937 states (624 key words + position) instead of seeds.
     share_levels=False stores the static level data once PER ENV instead of once
@@ -242,16 +258,26 @@ class BatchedEngine(object):
       st.d_groups, st.d_groups_init = self.groups.data_ptr(), self._groups_init.data_ptr()
       st.groups_init_bstride = bstride(self._groups_init)
     self.actions_per_env = g0.actions_per_env
-    self.rng = None
+    self.env_offset = env_offset
+    self.rng = None             # u32 [B, slots * 625] as int32: each env's generator words
+    seed_on_device = False
     if draws:
+      slots = len(g0.rng_streams)
       if rng_states is not None:
         states = np.ascontiguousarray(rng_states, dtype=np.uint32).reshape(
-            B, len(g0.rng_streams) * _lib.MT_WORDS)
+            B, slots * _lib.MT_WORDS)
+        self.rng = torch.from_numpy(states.view(np.int32)).to(dev)
+      elif _device_seeded(rng_seed, env_offset, B):
+        seed_on_device = True     # written by pcl_seed_rng once the state is bound
+        self.rng = torch.empty((B, slots * _lib.MT_WORDS), dtype=torch.int32, device=dev)
       else:
         states = np.stack([np.concatenate([_mt_state(stream, rng_seed + env_offset + e)
                                            for stream in g0.rng_streams]) for e in range(B)])
-      self.rng = torch.from_numpy(states.view(np.int32)).to(dev)
+        self.rng = torch.from_numpy(states.view(np.int32)).to(dev)
       st.d_rng = self.rng.data_ptr()
+      self._seed_kinds = (C.c_int32 * slots)(*[
+          _lib.SEED_PYTHON if stream == 'python' else _lib.SEED_NUMPY
+          for stream in g0.rng_streams])
     self._state = st
 
     # Outputs.
@@ -282,6 +308,8 @@ class BatchedEngine(object):
                                     C.byref(handle)), 'pcl_create')
     self._h = handle
     _lib.check(self._lib.pcl_bind_state(self._h, C.byref(self._state)), 'pcl_bind_state')
+    if seed_on_device:
+      self._seed(None, self._seed_tensor(int(rng_seed)))
     if g0.code is not None:       # the compiled program's bytecode, shared by every level
       code = np.ascontiguousarray(g0.code, dtype=np.int32)
       _lib.check(self._lib.pcl_bind_code(self._h, code.ctypes.data, len(code)), 'pcl_bind_code')
@@ -341,17 +369,78 @@ class BatchedEngine(object):
     self._after_step()
     return self._result()
 
-  def reset(self, env_mask=None):
+  def reset(self, env_mask=None, seeds=None):
     """Rebuild the selected envs (u8/bool [B] device tensor; None = all) and run
-    their its_showtime() frame; other envs are untouched."""
+    their its_showtime() frame; other envs are untouched.
+
+    seeds: first seed each selected env's generators as a fresh generator with that seed
+    would be, Gymnasium's reset(seed=...) per env: an int s (env e gets s + env_offset + e,
+    the constructor's rng_seed rule, so shards agree) or ints [B] (a sequence or tensor),
+    each in [0, 2**32).  A Python-`random` slot gets random.Random(seed)'s words, a NumPy
+    slot RandomState(seed)'s, so the env's episode is the one an engine built with that
+    seed plays.  Two launches on the current stream (pcl_seed_rng, then pcl_reset), so a
+    CUDA graph may hold them; the range of a CUDA tensor's seeds is not checked while the
+    stream is being captured.  Draws the game made when it was built (the reset templates)
+    are not redrawn."""
+    d_seeds = None if seeds is None else self._seed_tensor(seeds)
     self._showtime = True
     mask = None
     if env_mask is not None:
       mask = env_mask.to(device=self.device, dtype=_torch().uint8).contiguous()
+    if d_seeds is not None:
+      self._seed(mask, d_seeds)
     _lib.check(self._lib.pcl_reset(self._h, None if mask is None else mask.data_ptr(),
                                    C.byref(self._out), self._stream()), 'pcl_reset', self._h)
     self._after_step()
     return self._result()
+
+  def _seed_tensor(self, seeds):
+    """The u32 [B] seeds of `reset(seeds=)` as an int32 device tensor of the same bits."""
+    torch = _torch()
+    if self.rng is None:
+      raise ValueError('seeds= needs an engine whose game draws from random generators on the '
+                       'device; this one has none (the game draws nothing, rng_states=False, '
+                       'or its levels are generated on the host)')
+    B = self.batch
+    if isinstance(seeds, numbers.Integral) and not isinstance(seeds, (bool, np.bool_)):
+      first = int(seeds) + int(self.env_offset)
+      if not (0 <= first and first + B <= SEED_LIMIT):
+        raise ValueError('seed %d gives env seeds %d .. %d (env_offset %d); each must lie in '
+                         '[0, 2**32)' % (int(seeds), first, first + B - 1, self.env_offset))
+      t = torch.arange(first, first + B, dtype=torch.int64, device=self.device)
+    else:
+      if torch.is_tensor(seeds):
+        t = seeds
+      else:
+        if isinstance(seeds, np.ndarray) and seeds.ndim != 1:
+          raise ValueError('expected %d seeds, one per env, got shape %s' % (B, seeds.shape))
+        try:
+          vals = [operator.index(s) for s in seeds]
+        except TypeError:
+          raise TypeError('seeds is an int or a [B] sequence or tensor of ints, got %r' % (
+              seeds,))
+        if len(vals) != B:
+          raise ValueError('expected %d seeds, one per env, got %d' % (B, len(vals)))
+        if vals and (min(vals) < 0 or max(vals) >= SEED_LIMIT):
+          raise ValueError('each seed must lie in [0, 2**32)')
+        t = torch.tensor(vals, dtype=torch.int64)
+      if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex:
+        raise TypeError('seeds is an int or a [B] sequence or tensor of ints, got %s' % t.dtype)
+      if tuple(t.shape) != (B,):
+        raise ValueError('expected %d seeds, one per env, got shape %s' % (B, tuple(t.shape)))
+      t = t.to(device=self.device, dtype=torch.int64)
+      if B and not (t.is_cuda and torch.cuda.is_current_stream_capturing()):
+        if bool(((t < 0) | (t >= SEED_LIMIT)).any()):
+          raise ValueError('each seed must lie in [0, 2**32)')
+    # the low 32 bits, as an int32 holds them
+    return torch.where(t >= 2 ** 31, t - SEED_LIMIT, t).to(torch.int32).contiguous()
+
+  def _seed(self, mask, d_seeds):
+    """pcl_seed_rng of the envs `mask` selects (None = all) on the current stream."""
+    _lib.check(self._lib.pcl_seed_rng(self._h, None if mask is None else mask.data_ptr(),
+                                      d_seeds.data_ptr(), self._seed_kinds,
+                                      len(self._seed_kinds), self._stream()),
+               'pcl_seed_rng', self._h)
 
   def play(self, actions):
     """Engine.play(actions) for every env (engine.py:583-639).

@@ -515,6 +515,28 @@ int pcl_bind_episodes(pcl_handle* h, double* d_return) {
   return PCL_OK;
 }
 
+int pcl_seed_rng(pcl_handle* h, const uint8_t* d_env_mask, const uint32_t* d_seeds,
+                 const int32_t* h_kinds, int n_slots, void* stream) {
+  Range nvtx_range("pcl_seed_rng (random.seed / np.random.seed per env)");
+  if (!h || !d_seeds) return PCL_ERR_INVALID;
+  if (!h->bound) return PCL_ERR_UNBOUND;
+  const int slots = h->program->rng_slots ? h->program->rng_slots(h->spec) : 0;
+  if (slots == 0) return PCL_ERR_UNSUPPORTED;
+  if (!h->st.d_rng || n_slots != slots || !h_kinds) return PCL_ERR_INVALID;
+  pcl::SeedParams p;
+  memset(&p, 0, sizeof(p));
+  for (int k = 0; k < slots; ++k) {
+    if (h_kinds[k] != PCL_SEED_NUMPY && h_kinds[k] != PCL_SEED_PYTHON) return PCL_ERR_INVALID;
+    if (h_kinds[k] == PCL_SEED_PYTHON) p.python_slots |= 1u << k;
+  }
+  p.rng = h->st.d_rng;
+  p.env_mask = d_env_mask;
+  p.seeds = d_seeds;
+  p.B = h->batch;
+  p.slots = slots;
+  return launched(h, pcl::launch_seed_rng(p, (cudaStream_t)stream), "launch_seed_rng");
+}
+
 int pcl_reset(pcl_handle* h, const uint8_t* d_env_mask, const pcl_outputs* out, void* stream) {
   Range nvtx_range("pcl_reset (Engine.its_showtime)");
   const int r = check_ready(h, out, (cudaStream_t)stream);

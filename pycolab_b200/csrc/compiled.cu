@@ -771,6 +771,8 @@ int check_state(const pcl_spec& s, const pcl_state& st) {
   return PCL_OK;
 }
 
+int rng_slots(const pcl_spec& s) { return s.program_arg[1]; }
+
 // Scrollys' curtains: kept in bits when their pattern is written, else their window.
 CurtainAt curtain(const pcl_spec& s, int d) {
   return s.drape_kind[d] && !((s.program_arg[2] >> d) & 1) ? CurtainAt::kPatternWindow
@@ -966,6 +968,7 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
 
 const Program kCompiled = {check_spec, check_state, curtain, launch, actions_per_env,
                            /*float_reward=*/false, /*crop_epilogue=*/false,
-                           /*scroll_groups=*/false, check_code, /*float_reward_arg0=*/true};
+                           /*scroll_groups=*/false, check_code, /*float_reward_arg0=*/true,
+                           /*derive=*/nullptr, /*block_chaining=*/false, rng_slots};
 
 }  // namespace pcl

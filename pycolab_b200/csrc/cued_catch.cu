@@ -362,6 +362,7 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
 
 const Program kCuedCatch = {check_spec, check_state, curtain_bits, launch, nullptr,
                             /*float_reward=*/false, /*crop_epilogue=*/false,
-                            /*scroll_groups=*/false, nullptr, /*float_reward_arg0=*/true};
+                            /*scroll_groups=*/false, nullptr, /*float_reward_arg0=*/true,
+                            /*derive=*/nullptr, /*block_chaining=*/false, one_rng_slot};
 
 }  // namespace pcl

@@ -154,6 +154,8 @@ struct Program {
   // derive() builds in StepParams::block_sync, and touches per env only the arrays
   // footprint() (api.cu) lists.
   bool block_chaining;
+  // Generator slots of pcl_state.d_rng per env, the slots pcl_seed_rng writes.  nullptr: 0.
+  int (*rng_slots)(const pcl_spec&);
 };
 extern const Program kScrollyMaze, kWarehouse, kMarauders, kFixture, kBetterScrolly, kClassics,
     kAperture, kOrdeal, kHello, kApprehend, kShockwave, kTMaze, kCompiled, kBoxWorld,
@@ -195,6 +197,9 @@ inline bool margins_fit(const pcl_spec& s, int d) {
 
 // Program::curtain of programs that keep every drape in d_bits.
 inline CurtainAt curtain_bits(const pcl_spec&, int) { return CurtainAt::kBits; }
+
+// Program::rng_slots of programs that draw from one generator per env.
+inline int one_rng_slot(const pcl_spec&) { return 1; }
 
 struct RenderParams {
   int B, H, W, pitch, S, D;
@@ -294,5 +299,15 @@ struct PackParams {
   uint8_t* peers[PCL_MAX_PEERS];
 };
 cudaError_t launch_pack_handoff(const PackParams& p, cudaStream_t s);
+
+// pcl_seed_rng (seed.cu).
+struct SeedParams {
+  uint32_t* rng;                 // u32 [B, slots, PCL_MT_WORDS]
+  const uint8_t* env_mask;       // u8 [B], or NULL = every env
+  const uint32_t* seeds;         // u32 [B]
+  int B, slots;
+  uint32_t python_slots;         // bit k set: slot k is PCL_SEED_PYTHON, else PCL_SEED_NUMPY
+};
+cudaError_t launch_seed_rng(const SeedParams& p, cudaStream_t s);
 
 }  // namespace pcl

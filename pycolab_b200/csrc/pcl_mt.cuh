@@ -3,6 +3,7 @@
 // key + position; state word 624 is the position).  Used by marauders.cu
 // (np.random.choice), shockwave.cu (np.random.randint), apprehend.cu
 // (random.uniform), t_maze.cu and compiled.cu (the draws of compiled update() code).
+// MtSeed, at the end, writes the words a fresh seed leaves (seed.cu, pcl_seed_rng).
 #pragma once
 
 #include <stdint.h>
@@ -100,5 +101,67 @@ __device__ __forceinline__ double mt_random53(uint32_t* mt, int lane) {
   return __dmul_rn(__dadd_rn(__dmul_rn((double)a, 67108864.0), (double)b),
                    1.0 / 9007199254740992.0);
 }
+
+// ---- Seeding (pcl.h PCL_SEED_*) -----------------------------------------------------------
+// The words of a generator freshly seeded with s, computed in registers one at a time so that
+// a caller can stage them: start(), then word(i) for i = 2 .. 623 in that order, then head()
+// for words 0 and 1.  Word 624, the position, is 624 under both rules.
+//   NumPy (RandomState(s)): w[0] = s, w[i] = init_step(w[i-1], i).
+//   Python (random.Random(s), init_by_array over the key [s]): g = the words of
+//   init_genrand(19650218), the NumPy recurrence from 19650218.  The first mixing loop runs
+//   i = 1 .. 623, then sets word 0 = word 623 and runs once more at i = 1:
+//     a[i] = mix1(g[i], a[i-1]) with a[0] = g[0], and a'[1] = mix1(a[1], a[623]).
+//   The second runs i = 2 .. 623, then sets word 0 = word 623 and runs once more at i = 1:
+//     b[i] = mix2(a[i], b[i-1], i) with b[1] = a'[1], and word 1 = mix2(a'[1], b[623], 1);
+//   then word 0 = 0x80000000.  start() runs the first loop once for a[623] and a'[1]; word(i)
+//   recomputes g[i] and a[i] beside b[i], so no word is ever read back.
+struct MtSeed {
+  uint32_t s;
+  bool python;
+  uint32_t w;        // the word before the next: NumPy w[i-1], Python b[i-1]
+  uint32_t g, a;     // Python: g[i-1], a[i-1]
+  uint32_t a1;       // Python: a'[1]
+
+  __host__ __device__ static uint32_t init_step(uint32_t prev, uint32_t i) {
+    return 1812433253u * (prev ^ (prev >> 30)) + i;
+  }
+  __host__ __device__ uint32_t mix1(uint32_t word, uint32_t prev) const {
+    return (word ^ ((prev ^ (prev >> 30)) * 1664525u)) + s;
+  }
+  __host__ __device__ static uint32_t mix2(uint32_t word, uint32_t prev, uint32_t i) {
+    return (word ^ ((prev ^ (prev >> 30)) * 1566083941u)) - i;
+  }
+
+  __host__ __device__ void start(uint32_t seed, bool python_rule) {
+    s = seed;
+    python = python_rule;
+    if (!python) {
+      w = init_step(s, 1);
+      return;
+    }
+    const uint32_t g0 = 19650218u;
+    g = init_step(g0, 1);
+    a = mix1(g, g0);                 // a[1]
+    uint32_t gi = g, ai = a;
+    for (uint32_t i = 2; i < 624; ++i) {
+      gi = init_step(gi, i);
+      ai = mix1(gi, ai);
+    }
+    a1 = mix1(a, ai);
+    w = a1;                          // b[1]
+  }
+
+  __host__ __device__ uint32_t word(uint32_t i) {
+    if (!python) return w = init_step(w, i);
+    g = init_step(g, i);
+    a = mix1(g, a);
+    return w = mix2(a, w, i);
+  }
+
+  __host__ __device__ void head(uint32_t* w0, uint32_t* w1) const {
+    *w0 = python ? 0x80000000u : s;
+    *w1 = python ? mix2(a1, w, 1) : init_step(s, 1);
+  }
+};
 
 }  // namespace pcl

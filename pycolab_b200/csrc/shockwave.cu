@@ -167,6 +167,8 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
 
 const Program kShockwave = {check_spec, check_state, curtain_bits, launch, nullptr,
                             /*float_reward=*/false, /*crop_epilogue=*/false,
-                            /*scroll_groups=*/false};
+                            /*scroll_groups=*/false, /*check_code=*/nullptr,
+                            /*float_reward_arg0=*/false, /*derive=*/nullptr, /*block_chaining=*/false,
+                            one_rng_slot};
 
 }  // namespace pcl

@@ -379,10 +379,15 @@ cudaError_t launch(const StepParams& p, cudaStream_t s) {
   return launch_step(t_maze_step, p, kWarpsPerBlock, 0, s);
 }
 
+// Slot 0 draws the cue (Python's random), slot 1 the speckle (NumPy's).
+int rng_slots(const pcl_spec&) { return 2; }
+
 }  // namespace
 
 const Program kTMaze = {check_spec, check_state, curtain, launch, nullptr,
                         /*float_reward=*/true, /*crop_epilogue=*/false,
-                        /*scroll_groups=*/false};
+                        /*scroll_groups=*/false, /*check_code=*/nullptr,
+                        /*float_reward_arg0=*/false, /*derive=*/nullptr, /*block_chaining=*/false,
+                        rng_slots};
 
 }  // namespace pcl
